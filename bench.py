@@ -152,7 +152,8 @@ def run_ours(args):
         def step_resident(self):
             # inputs already in HBM; mvs_fit runs the whole stage schedule (frames change stage on their own)
             self.x.copy_(self.x0_dev)
-            return self.ctx.fit(self.x, self.stages, self.opt)[1]
+            self.loss, st = self.ctx.fit(self.x, self.stages, self.opt)
+            return st
 
         def step_host(self):
             self.X_pin.copy_(torch.from_numpy(self.X0))
@@ -177,6 +178,8 @@ def run_ours(args):
         share_of = lambda n: [n // len(L) + (1 if i < n % len(L) else 0) for i in range(len(L))]
         stats = [[] for _ in L]
         err = []
+        for ln in L:
+            ln.timed_steps = 0
 
         def work(i, n, record):
             try:
@@ -187,6 +190,7 @@ def run_ours(args):
                         st = getattr(L[i], kind)()
                         if record:
                             stats[i].append(st)
+                            L[i].timed_steps += 1
                     L[i].stream.synchronize()
             except Exception as e:                                         # noqa: BLE001 -- re-raised below
                 err.append(e)
@@ -250,6 +254,8 @@ def run_ours(args):
     # headline: `inflight` batches in flight (throughput of a stream of 256-frame batches); then the same workload with ONE
     # batch at a time (latency of a batch; the dominant kernel's roofline is taken here, undisturbed by concurrent lanes)
     ms_res, stats_res, launches, _, wall = timed("step_resident", args.steps, args.warmup)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, lanes, rank)
     ms_e2e, stats_e2e, _, _, _ = timed("step_host", args.steps, max(1, min(args.warmup, n_lanes)))
     ms_one, stats_one, launches_one, prof, _ = timed("step_resident", args.steps, 1, dom_mask, use_lanes=1)
     ms_one_e2e, stats_one_e2e, _, _, _ = timed("step_host", args.steps, 1, use_lanes=1)
@@ -289,8 +295,8 @@ def run_ours(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json, sustained-copy figure)" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json, sustained-copy figure)" if peaks else "H100 SXM data sheet: 3350 GB/s HBM3"
         # ---- roofline of the dominant kernel: algorithmic bytes per launch (DESIGN.md section 5) / event time
         dom_ms, dom_n = prof.get(dom, (0.0, 0))
         # average active frames per launch of the dense-round kernels (compaction shrinks launches towards the tail):
@@ -300,20 +306,12 @@ def run_ours(args):
         na_avg = (dense_ev / dense_rd) if dense_rd else (sum(s_["frame_evals"] for s_ in stats_one) / max(sum(s_["rounds"] for s_ in stats_one), 1))
         alg = algorithmic_bytes(dom, na_avg, V, dense=bool(args.sdf))
         ach = (alg * dom_n) / (dom_ms * 1e-3) / 1e9 if dom_ms > 0 else None
-        # DRAM bytes per launch of that kernel from the committed `ncu --set full` capture (cold caches, 256 active
-        # frames): profiles/r01_traffic.json, written from the .ncu-rep files by the profiling scripts
-        traffic = None
-        try:
-            tf = "r02_traffic.json" if os.path.exists(os.path.join(ROOT, "profiles", "r02_traffic.json")) else "r01_traffic.json"
-            traffic = json.load(open(os.path.join(ROOT, "profiles", tf)))[dom]["traffic"]
-        except Exception:
-            pass
         roof = {"kernel": dom, "bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s",
-                "frac": (ach / hbm_peak) if ach else None, "traffic": traffic,
+                "frac": (ach / hbm_peak) if ach else None,
                 "algorithmic_bytes_per_launch": alg, "launches": dom_n, "avg_launch_us": (dom_ms * 1e3 / dom_n) if dom_n else None,
                 "avg_active_frames_per_launch": na_avg, "peak_source": peak_src,
                 "measured_in": "the one-batch-at-a-time timed leg (events around every launch of this kernel on its stream)",
-                "note": "the path is latency / L2 bound, not HBM bound: constants (20 MB) live in the 126 MB L2 and one "
+                "note": "the path is latency / L2 bound, not HBM bound: constants (20 MB) live in the 50 MB L2 and one "
                         "launch moves a few MB; see DESIGN.md section 5",
                 "kernel_time_share_of_step": {k: round(v[0] / max(sum(x_[0] for x_ in share.values()), 1e-9), 4)
                                               for k, v in share.items()},
@@ -322,11 +320,12 @@ def run_ours(args):
         # the tensor-core contraction, from the fully instrumented warm-up step (events around every launch)
         if "posedirs_gemm_tc" in share and share["posedirs_gemm_tc"][1] > 0:
             g_ms, g_n = share["posedirs_gemm_tc"]
-            tf32_peak = float(peaks.get("bf16_tflops_sustained", 1400.0)) / 2.0
+            tf32_peak = float(peaks.get("bf16_tflops_sustained", 989.0)) / 2.0
             g_ach = gemm_flops(na_avg) * g_n / (g_ms * 1e-3) / 1e12
             roof["posedirs_gemm"] = {"bound": "tensor", "achieved": g_ach, "peak": tf32_peak, "unit": "TFLOP/s",
                                      "frac": g_ach / tf32_peak, "avg_launch_us": g_ms * 1e3 / g_n,
-                                     "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained / 2 as the TF32 proxy",
+                                     "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained / 2 as the TF32 proxy" if peaks
+                                                    else "H100 SXM data sheet: 989 TFLOP/s dense BF16 / 2 (495 TF32)",
                                      "note": "M = frames in flight (skinny GEMM): bound by streaming posedirs once per "
                                              "128-frame tile, not by tensor throughput"}
         cpu = {"note": "measured at N = 1 only"} if world > 1 else \
@@ -365,6 +364,21 @@ def run_ours(args):
         ln.ctx.close()
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, lanes, rank):
+    """What the headline path (mvs_fit) hands its caller after the last timed step of every lane that ran one: the fitted
+    parameters [B][86] and final losses [B], float32.  A lane's inputs depend only on its seed (1000 + rank + 97 lane), so
+    two builds run with the same arguments can be compared output for output."""
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    for i, ln in enumerate(lanes):
+        if ln.timed_steps == 0:
+            continue
+        tag = "rank%d_lane%d" % (rank, i)
+        np.save(os.path.join(out_dir, "params_%s.npy" % tag), ln.x.detach().cpu().numpy().astype(np.float32))
+        np.save(os.path.join(out_dir, "loss_%s.npy" % tag), ln.loss.detach().cpu().numpy().astype(np.float32))
 
 
 def run_cfg5(args, model, gmm, cams, world, rank, local, dev):
@@ -565,9 +579,7 @@ def run_reference(args):
     env = dict(os.environ)
     cmd = [sys.executable, os.path.abspath(__file__), "--ref-worker", "--views", str(V), "--ref-device", args.ref_device,
            "--warmup", str(args.warmup)]
-    errlog = open(os.path.join(ROOT, "gpurun_out", "ref_workers.err"), "a") if os.path.isdir(os.path.join(ROOT, "gpurun_out")) \
-        else subprocess.DEVNULL
-    procs = [subprocess.Popen(cmd, stdin=subprocess.PIPE, stdout=subprocess.PIPE, stderr=errlog, env=env, text=True)
+    procs = [subprocess.Popen(cmd, stdin=subprocess.PIPE, stdout=subprocess.PIPE, env=env, text=True)
              for _ in range(cores)]
 
     def read_tagged(p, tag):
@@ -646,11 +658,13 @@ def main():
     ap.add_argument("--sweeps", type=int, default=6, help="cfg5: block-Jacobi sweeps")
     ap.add_argument("--seq-frames", type=int, default=128, help="cfg5: frames per rank (1024 / 8)")
     ap.add_argument("--cpu-seconds", type=float, default=30.0)
-    ap.add_argument("--ref-workers", type=int, default=32, help="host processes of the reference arm (capped at the physical cores; "
-                    "32 on the 64-core B200 hosts: more saturate the memory system, measured in round 1)")
+    ap.add_argument("--ref-workers", type=int, default=32, help="host processes of the reference arm (capped at half the logical "
+                    "cores)")
     ap.add_argument("--ref-seconds", type=float, default=200.0, help="target wall time of the --impl reference run (sizes the sample)")
     ap.add_argument("--ref-device", default="cpu", choices=["cpu", "cuda"], help="reference arm: host cores (default) or torch-CUDA")
     ap.add_argument("--ref-worker", action="store_true", help=argparse.SUPPRESS)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write each lane's final parameters and losses of its last timed step as DIR/*.npy")
     args = ap.parse_args()
     if args.ref_worker:
         run_ref_worker(args)

@@ -1,4 +1,4 @@
-/* mvsmpl.h -- C ABI of libmvsmpl.so, the B200-native (sm_100a) replacement of the
+/* mvsmpl.h -- C ABI of libmvsmpl.so, the H100-native (sm_90a) replacement of the
  * multi-view SMPL fitting hot path of boycehbz/MvSMPLfitting.
  *
  * Plain C, no torch / C++ types.  Every entry point returns 0 on success and a
@@ -34,7 +34,7 @@ typedef enum {
     MVS_OK = 0,
     MVS_ERR_INVALID = -1,      /* bad argument / call order */
     MVS_ERR_CUDA = -2,         /* CUDA runtime error */
-    MVS_ERR_NO_DEVICE = -3,    /* no usable sm_100 device: there is NO CPU fallback */
+    MVS_ERR_NO_DEVICE = -3,    /* no usable sm_90 device: there is NO CPU fallback */
     MVS_ERR_UNSUPPORTED = -4
 } mvs_status;
 

@@ -1,4 +1,4 @@
-"""Builds libmvsmpl.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libmvsmpl.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m mvsmplfitting_b200.build [--force]
 """
@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 OUT = os.path.join(_HERE, "libmvsmpl.so")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 

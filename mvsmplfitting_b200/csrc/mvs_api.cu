@@ -115,8 +115,8 @@ int mvs_create(int device, mvs_ctx** out) {
                          e != cudaSuccess ? cudaGetErrorString(e) : "device count is 0");
     if (device < 0 || device >= count) return set_error(nullptr, MVS_ERR_INVALID, "mvs_create: bad device %d", device);
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major < 10)
-        return set_error(nullptr, MVS_ERR_NO_DEVICE, "mvs_create: device %d is sm_%d%d; this library is built for sm_100a only",
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9 || prop.minor != 0)
+        return set_error(nullptr, MVS_ERR_NO_DEVICE, "mvs_create: device %d is sm_%d%d; this library is built for sm_90a only",
                          device, prop.major, prop.minor);
     if (cudaSetDevice(device) != cudaSuccess) return set_error(nullptr, MVS_ERR_CUDA, "cudaSetDevice failed");
     mvs_ctx* ctx = new mvs_ctx();

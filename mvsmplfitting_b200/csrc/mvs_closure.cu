@@ -840,7 +840,7 @@ int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st) {
 int launch_vertex_fwd_dense(mvs_ctx* ctx, cudaStream_t st, bool allow_tc, bool need_vposed) {
     DevModel& m = ctx->m;
     Workspace& w = ctx->ws;
-    if (allow_tc && tc_available(ctx)) return launch_vertex_fwd_tc(ctx, st, need_vposed);     // tcgen05 / TMA path (mvs_tc.cu)
+    if (allow_tc && tc_available(ctx)) return launch_vertex_fwd_tc(ctx, st, need_vposed);     // wgmma / TMA path (mvs_tc.cu)
     if (!ctx->attr_done) {
         MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertFwdSmem));
         MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertBwdSmem));

@@ -279,7 +279,7 @@ bool hybrid_available(const mvs_ctx* ctx);
 int launch_vertex_fwd_dense(mvs_ctx* ctx, cudaStream_t st, bool allow_tc = true, bool need_vposed = true);                                   // mvs_closure.cu
 int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);                      // mvs_closure.cu
 int launch_sdf_fused(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu
-// mvs_tc.cu: tcgen05 / TMA dense vertex forward
+// mvs_tc.cu: wgmma / TMA dense vertex forward
 int tc_upload_model(mvs_ctx* ctx, const float* Qk_host);
 bool tc_available(const mvs_ctx* ctx);
 int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed = true);

@@ -234,7 +234,7 @@ static int run_stage(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, con
     if (some_inactive)                                      // frames without a stage in this run leave the active list now
         MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
     if ((!step_mode || vp2) && hybrid_available(ctx)) {
-        // dense regime (SDF term on): four launches per round -- pose blend shapes of the active frames (tcgen05
+        // dense regime (SDF term on): four launches per round -- pose blend shapes of the active frames (wgmma
         // GEMM), skinning + box partials, the SDF term with the adjoint of its (short) vertex list, and the per-frame
         // closure adjoint + optimiser step + next pose forward.  Finished frames are compacted out once per chunk.
         const int chunk = 8;
@@ -263,7 +263,7 @@ static int run_stage(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, con
         w.na_bound = B;                                               // grids shrink with the (lagging) host view of the count
         while (rounds < max_rounds) {
             for (int r = 0; r < chunk; ++r) {
-                if ((rc = launch_vertex_fwd_dense(ctx, st, true, false))) return rc;   // tcgen05 GEMM + LBS + bbox partials
+                if ((rc = launch_vertex_fwd_dense(ctx, st, true, false))) return rc;   // wgmma GEMM + LBS + bbox partials
                 if ((rc = launch_sdf_fused(ctx, st))) return rc;   // samples + adjoint of the listed vertices
                 if ((rc = launch_frame_step(ctx, params_dev, &S, &cfg, nst, st))) return rc;
                 ++rounds;

@@ -387,6 +387,20 @@ __device__ __forceinline__ void lbfgs_advance_core(FrameScalars& s, const LbfgsP
         }
         case L_LS_FINISH: {                                    // lbfgs_ls.py:163-167, 399-434
             const float* bgl = s.low ? bg1 : bg0;
+            // A line search that ends on a non-finite point (a trial step far enough out that the closure overflows, or a
+            // NaN step length from the cubic interpolation of such values) would write NaN into the parameters, and the
+            // monitor's NaN guard (fitting.py:101-107) would then stop the frame with NaN parameters.  Instead the
+            // parameters, loss and gradient stay at the line search's start and the step ends: the next monitor check
+            // sees no progress and the stage finishes with the last finite iterate.  Deliberate departure from
+            // lbfgs_ls.py, which only differs where the reference itself would produce a non-finite result.
+            bool finite = isfinite(s.bt[s.low]) && isfinite(s.bf[s.low]);
+            VLOOP(i) if (!isfinite(bgl[i]) || !isfinite(fmaf(s.bt[s.low], d[i], x_init[i]))) finite = false;
+            if (!__all_sync(0xffffffffu, finite)) {
+                s.t = 0.f;
+                s.current_evals += s.ls_evals;
+                label = L_STEP_END;
+                break;
+            }
             s.t = s.bt[s.low];
             s.loss = s.bf[s.low];
             VLOOP(i) { g[i] = bgl[i]; x[i] = fmaf(s.t, d[i], x_init[i]); }

@@ -6,7 +6,7 @@
 // Why: the loss of the sparse regime depends on only 86 of the 6890 vertices (SURVEY H4), so one
 // closure is ~0.1 MFLOP + two passes over a 231 KB L2-resident slice of Qk.  Spread over five
 // kernels per evaluation and ~900 rounds per fit, the batched path is bound by launch + dependent
-// load latency (215 us per round measured, profiles/r01_ncu_summary.md).  Frames are independent
+// load latency.  Frames are independent
 // optimisation problems, so nothing forces them into lock-step rounds: here every frame advances
 // at its own pace, the optimiser state (7 vectors, 100-pair history = 69 KB) lives in shared
 // memory, and a 256-frame stage is ONE kernel launch.

@@ -1,4 +1,4 @@
-// Dense vertex forward on the 5th-generation tensor cores (sm_100a, tcgen05 + TMEM + TMA).
+// Dense vertex forward on the Hopper tensor cores (sm_90a: wgmma + TMA + mbarrier).
 //
 //   pose_offsets[b, 3n+c] = sum_k  pose_feature[b,k] * posedirs[k, 3n+c]        (lbs.py:192-195)
 //
@@ -8,22 +8,22 @@
 // pose features, 112 KB; only the live 8-row groups are fetched when few frames are active) RESIDENT in shared memory
 // for the CTA's whole life while posedirs tiles stream through a TMA ring:
 //
-//   warp 0   TMA producer   A once (7 boxes 128x32, or 8-row boxes), then B boxes 96x32 through a 6-stage mbarrier ring
-//   warp 1   MMA issuer     tcgen05.mma.cta_group::1.kind::tf32  M=128 N=96 K=8, fp32 accumulators in TMEM,
-//                           two accumulator buffers (2 x 96 columns) so tile i+1 runs under the epilogue of tile i
-//   warp 2   TMEM alloc / dealloc
-//   warps 4-7  epilogue     tcgen05.ld (lane = frame, 96 columns = 32 vertices x 3), pose offsets stored TRANSPOSED
-//                           (frame fastest) so that a warp's 32 frames form one 128-byte line per column
+//   warpgroup 0      TMA producer (one thread): A once (7 boxes 128x32, or 8-row boxes), then B boxes 96x32 through
+//                    a 2-stage mbarrier ring
+//   warpgroups 1, 2  wgmma.m64n96k8.f32.tf32 on 64 frames each, fp32 accumulators in registers; each warpgroup
+//                    releases a ring stage once its MMAs on it have retired, then stores its 64 x 96 tile of pose
+//                    offsets TRANSPOSED (frame fastest) through shared memory and the TMA store engine.  A warpgroup
+//                    whose 64 frames are all inactive exits at once.
 //
 // The rest of the vertex forward (template + shape blend shapes in fp32, linear blend skinning, box partials) is
-// skin_kernel / skin_small_kernel below: fused into this epilogue it ran in 128 threads and cost 10x the contraction.
+// skin_kernel / skin_small_kernel below.
 //
 // Precision: error-compensated "3xTF32".  Both operands are split into two TF32 numbers (x = hi + lo, lo = TF32(x - hi)) and
 // the tensor cores accumulate hi*hi + lo*hi + hi*lo in fp32 (the dropped lo*lo term is 2^-22 of a product), i.e. the pose
-// offsets come out with fp32-class accuracy.  Plain TF32 (round 1) left 1e-6 absolute on a vertex: harmless for the joints,
-// but the SDF samples are voxel-sized distances, so it was a 1e-5 .. 1e-4 relative error of the interpenetration term and
-// pushed its gradient past the 1e-4 parity bar (profiles/r02_sdf_pin_diag_before.json).  The tensor pipe was 1 % busy, so
-// the 3x MMA count is free; the price is operand traffic (B hi + B lo, and the A lo chunks stream through the ring).
+// offsets come out with fp32-class accuracy.  Plain TF32 leaves 1e-6 absolute on a vertex: harmless for the joints, but
+// the SDF samples are voxel-sized distances, so it is a 1e-5 .. 1e-4 relative error of the interpenetration term and
+// pushes its gradient past the 1e-4 parity bar.  The path is bound by operand streaming, so the 3x MMA count is free;
+// the price is operand traffic (B hi + B lo, and the A lo chunks stream through the ring).
 // The template and the shape blend shapes are NOT sent through the tensor cores.
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -51,14 +51,11 @@ posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     unsigned char* sA = base;                                        // A hi: 7 x [128 rows][128 B], 1024-aligned, resident
     unsigned char* sR = sA + (size_t)kTcKCh * kTcABytes;             // ring: kTcStages x (A lo chunk 16 KB | B hi chunk 12 KB | B lo chunk 12 KB)
-    float* sO = reinterpret_cast<float*>(sR + (size_t)kTcStages * kTcStageBytes);       // epilogue staging tile [32 columns][128 frames]
+    float* sO = reinterpret_cast<float*>(sR + (size_t)kTcStages * kTcStageBytes);       // epilogue staging: 2 x [32 columns][64 frames]
     uint64_t* bars = reinterpret_cast<uint64_t*>(sR + (size_t)kTcStages * kTcStageBytes + kTcEpiBytes);
     uint64_t* a_full = bars;                      // [1]
     uint64_t* b_full = bars + 1;                  // [stages]
     uint64_t* b_empty = b_full + kTcStages;       // [stages]
-    uint64_t* t_full = b_empty + kTcStages;       // [2]
-    uint64_t* t_empty = t_full + 2;               // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
 
     const int na = *na_ptr;
     const int m0 = blockIdx.y * kTcBM;
@@ -73,33 +70,26 @@ posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_
     const int tile_end = min(tile_begin + tiles_per_cta, ntiles);
     if (tile_begin >= tile_end) return;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int live_rows = min(kTcBM, na - m0);
+    const int live_wgs = (live_rows + kTcWgM - 1) / kTcWgM;          // consumer warpgroups with at least one active frame
     if (threadIdx.x == 0) TC_MARK(0);
 
     if (threadIdx.x == 0) {
         mbar_init(a_full, 1);
-        for (int s = 0; s < kTcStages; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&t_full[s], 1); mbar_init(&t_empty[s], 128); }
+        for (int s = 0; s < kTcStages; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], live_wgs); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(256));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     if (threadIdx.x == 0) TC_MARK(1);
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp < 4) {
+        if (warp == 0 && lane == 0) {
             // ---------------- TMA producer
-            // A operand.  Every CTA of the M tile reads it, so with 148 CTAs the 112 KB tile costs as much L2 traffic
-            // as posedirs itself; at the tail of a fit only a few of its 128 rows are live, and those are fetched as
-            // 8-row boxes (one swizzle atom each: same shared-memory image).  Rows that are not loaded hold whatever
-            // was there: their accumulator rows are never read.
+            // A operand.  Every CTA of the M tile reads it, so with one CTA per SM the 112 KB tile costs as much L2
+            // traffic as posedirs itself; at the tail of a fit only a few of its 128 rows are live, and those are fetched
+            // as 8-row boxes (one swizzle atom each: same shared-memory image).  Rows that are not loaded hold whatever
+            // was there: their accumulator rows are never stored.
             // lo parts: rows ldA.. of the A array, rows ncols.. of the posedirs array (same tensor maps, row offset)
-            const int live_rows = min(kTcBM, na - m0);
             const bool small = live_rows <= 32;
             const int groups = (live_rows + 7) / 8;
             if (small) {
@@ -131,82 +121,66 @@ posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ---------------- MMA issuer
-            constexpr uint32_t idesc = umma_idesc_tf32(kTcBM, kTcBN);
-            if (!mbar_wait(a_full, 0, err_flag)) return;
-            TC_MARK(2);
-            int stage = 0; uint32_t phase = 0;
-            int buf = 0; uint32_t tphase[2] = {0, 0};
-            for (int tile = tile_begin; tile < tile_end; ++tile) {
-                if (!mbar_wait(&t_empty[buf], tphase[buf] ^ 1, err_flag)) return;
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t d_tmem = tmem_base + (uint32_t)(buf * kTcBN);
-                for (int kc = 0; kc < kTcKCh; ++kc) {
-                    if (!mbar_wait(&b_full[stage], phase, err_flag)) return;
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t ah = smem_u32(sA + (size_t)kc * kTcABytes);
-                    const uint32_t al = smem_u32(sR + (size_t)stage * kTcStageBytes);
-                    const uint32_t bh = al + kTcABytes, bl = bh + kTcBBytes;
-#pragma unroll
-                    for (int k = 0; k < kTcBK / 8; ++k) {              // hi*hi, then the two correction products
-                        umma_tf32(d_tmem, umma_desc_k_sw128(ah + k * 32), umma_desc_k_sw128(bh + k * 32), idesc, (kc | k) ? 1u : 0u);
-                        umma_tf32(d_tmem, umma_desc_k_sw128(al + k * 32), umma_desc_k_sw128(bh + k * 32), idesc, 1u);
-                        umma_tf32(d_tmem, umma_desc_k_sw128(ah + k * 32), umma_desc_k_sw128(bl + k * 32), idesc, 1u);
-                    }
-                    umma_commit(&b_empty[stage]);                    // frees the B slot when these MMAs retire
-                    if (++stage == kTcStages) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&t_full[buf]);                           // accumulator of this tile complete
-                TC_MARK(3 + (tile - tile_begin));
-                tphase[buf] ^= 1;
-                buf ^= 1;
-            }
-        }
-    } else if (warp >= 4) {
-        // ---------------- epilogue: lane = frame row of the M tile; pose offsets go out TRANSPOSED
-        //                  poffT[column][slot] so that a warp's 32 frames form one 128-byte store
-        const int row = 32 * (warp & 3) + lane;
-        int buf = 0; uint32_t tphase[2] = {0, 0};
-        for (int tile = tile_begin; tile < tile_end; ++tile) {
-            if (!mbar_wait(&t_full[buf], tphase[buf], err_flag)) return;
-            if (threadIdx.x == 128) TC_MARK(8 + 2 * (tile - tile_begin));
-            tphase[buf] ^= 1;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t taddr = tmem_base + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)(buf * kTcBN);
-            uint32_t acc[kTcBN];
-            tmem_ld32(taddr, acc);
-            tmem_ld32(taddr + 32, acc + 32);
-            tmem_ld32(taddr + 64, acc + 64);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(&t_empty[buf]);                              // accumulator copied out: the MMA warp may reuse it
-            buf ^= 1;
-            // The tile leaves through shared memory and the TMA store engine, 32 columns ([column][frame] rows of 512 B) at a
-            // time: the four epilogue warps fill the staging tile (lane = frame: conflict-free), one thread issues the bulk
-            // tensor store, which clips the box at the array bounds (last vertex tile, frame padding).  Rows of slots that are
-            // not active hold whatever the accumulator held: nobody reads them.
-            const int c0 = tile * kTcBN;
-#pragma unroll
-            for (int ch = 0; ch < kTcBN / kTcEpiCols; ++ch) {          // unrolled: acc[] stays in registers
-                if (c0 + ch * kTcEpiCols >= ncols) break;
-                if (threadIdx.x == 128) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // staging tile free again
-                asm volatile("bar.sync 2, 128;" ::: "memory");
-#pragma unroll
-                for (int c = 0; c < kTcEpiCols; ++c) sO[c * kTcBM + row] = __uint_as_float(acc[ch * kTcEpiCols + c]);
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                asm volatile("bar.sync 2, 128;" ::: "memory");
-                if (threadIdx.x == 128) tma_store_2d(&map_o, sO, m0, c0 + ch * kTcEpiCols);
-            }
-            if (threadIdx.x == 128) TC_MARK(9 + 2 * (tile - tile_begin));
-        }
-        if (threadIdx.x == 128) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");         // all stores of this CTA have landed
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256));
-    if (threadIdx.x == 0) TC_MARK(20);
+
+    // ---------------- consumer warpgroup g: frames m0 + 64 g .. m0 + 64 g + 63
+    const int g = warp / 4 - 1;
+    if (g >= live_wgs) return;
+    const int wt = threadIdx.x - 128 * (g + 1);                       // thread of the warpgroup
+    const uint32_t a_row_off = (uint32_t)(g * kTcWgM * kTcBK * 4);    // 64 rows of 128 B = 8 swizzle atoms
+    float* sOw = sO + (size_t)g * kTcEpiCols * kTcWgM;
+    const int row = 16 * (wt >> 5) + ((wt & 31) >> 2);                // accumulator rows row, row + 8
+    const int colq = 2 * (wt & 3);                                    // accumulator columns 8 i + colq (+ 1)
+    float acc[kTcBN / 2];
+#pragma unroll
+    for (int i = 0; i < kTcBN / 2; ++i) acc[i] = 0.f;
+    if (!mbar_wait(a_full, 0, err_flag)) return;
+    if (wt == 0) TC_MARK(2);
+    int stage = 0; uint32_t phase = 0;
+    for (int tile = tile_begin; tile < tile_end; ++tile) {
+        for (int kc = 0; kc < kTcKCh; ++kc) {
+            if (!mbar_wait(&b_full[stage], phase, err_flag)) return;
+            const uint32_t ah = smem_u32(sA + (size_t)kc * kTcABytes) + a_row_off;
+            const uint32_t al = smem_u32(sR + (size_t)stage * kTcStageBytes) + a_row_off;
+            const uint32_t bh = smem_u32(sR + (size_t)stage * kTcStageBytes) + kTcABytes, bl = bh + kTcBBytes;
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kTcBK / 8; ++k) {                  // hi*hi, then the two correction products
+                wgmma_m64n96k8_tf32(acc, wgmma_desc_k_sw128(ah + k * 32), wgmma_desc_k_sw128(bh + k * 32), (kc | k) ? 1u : 0u);
+                wgmma_m64n96k8_tf32(acc, wgmma_desc_k_sw128(al + k * 32), wgmma_desc_k_sw128(bh + k * 32), 1u);
+                wgmma_m64n96k8_tf32(acc, wgmma_desc_k_sw128(ah + k * 32), wgmma_desc_k_sw128(bl + k * 32), 1u);
+            }
+            wgmma_commit();
+            wgmma_wait0();
+            if (wt == 0) mbar_arrive(&b_empty[stage]);              // this warpgroup's MMAs on the stage have retired
+            if (++stage == kTcStages) { stage = 0; phase ^= 1; }
+        }
+        if (wt == 0) TC_MARK(3 + (tile - tile_begin));
+        // The tile leaves through shared memory and the TMA store engine, 32 columns ([column][frame] rows of 256 B) at a
+        // time: the warpgroup fills its staging tile, one thread issues the bulk tensor store, which clips the box at the
+        // array bounds (last vertex tile, frame padding).  Rows of slots that are not active hold whatever the accumulator
+        // held: nobody reads them.
+        const int c0 = tile * kTcBN;
+#pragma unroll
+        for (int ch = 0; ch < kTcBN / kTcEpiCols; ++ch) {          // unrolled: acc[] stays in registers
+            if (c0 + ch * kTcEpiCols >= ncols) break;
+            if (wt == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // staging tile free again
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
+#pragma unroll
+            for (int i = 0; i < kTcEpiCols / 8; ++i)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int j = 0; j < 2; ++j)
+                        sOw[(8 * i + colq + j) * kTcWgM + row + 8 * h] = acc[4 * (ch * kTcEpiCols / 8 + i) + 2 * h + j];
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
+            if (wt == 0) tma_store_2d(&map_o, sOw, m0 + g * kTcWgM, c0 + ch * kTcEpiCols);
+        }
+    }
+    if (wt == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");         // all stores of this warpgroup have landed
+    if (threadIdx.x == 128) TC_MARK(20);
 }
 
 __global__ void __launch_bounds__(kSkinThreads)
@@ -262,7 +236,7 @@ static int encode_map(mvs_ctx* ctx, CUtensorMap* map, const float* ptr, uint64_t
     return MVS_OK;
 }
 
-// output of the contraction: poffT [ncols][ldA] fp32, frame fastest; box = 128 frames x kTcEpiCols columns, no swizzle
+// output of the contraction: poffT [ncols][ldA] fp32, frame fastest; box = 64 frames x kTcEpiCols columns, no swizzle
 static int encode_out_map(mvs_ctx* ctx, CUtensorMap* map, float* ptr, uint64_t ldA, uint64_t ncols) {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
@@ -271,7 +245,7 @@ static int encode_out_map(mvs_ctx* ctx, CUtensorMap* map, float* ptr, uint64_t l
     auto fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(p);
     cuuint64_t dims[2] = {(cuuint64_t)ldA, (cuuint64_t)ncols};
     cuuint64_t strides[1] = {(cuuint64_t)ldA * sizeof(float)};
-    cuuint32_t box[2] = {(cuuint32_t)kTcBM, (cuuint32_t)kTcEpiCols};
+    cuuint32_t box[2] = {(cuuint32_t)kTcWgM, (cuuint32_t)kTcEpiCols};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

@@ -1,23 +1,24 @@
-// Device-side building blocks of the tensor-core vertex forward (mvs_tc.cu) shared with the persistent dense-round
-// kernel (mvs_dense.cu): mbarrier / TMA / tcgen05 wrappers, tile constants, and the one vertex routine every skinning
-// variant calls (so that a frame gets the same bits whichever kernel evaluated it).
+// Device-side building blocks of the tensor-core vertex forward (mvs_tc.cu): mbarrier / TMA / wgmma wrappers, tile
+// constants, and the one vertex routine every skinning variant calls (so that a frame gets the same bits whichever
+// kernel evaluated it).
 #pragma once
 #include <cuda.h>
 #include "mvs_internal.cuh"
 
 namespace mvs {
 
-constexpr int kTcBM = 128;            // frames per CTA (UMMA M)
-constexpr int kTcBN = kTileC;         // 96 columns = 32 vertices (UMMA N)
+constexpr int kTcBM = 128;            // frames per CTA: two consumer warpgroups of 64 rows (wgmma M = 64)
+constexpr int kTcWgM = 64;            // frames per consumer warpgroup
+constexpr int kTcBN = kTileC;         // 96 columns = 32 vertices (wgmma N)
 constexpr int kTcBK = 32;             // floats per 128-byte swizzle row
 constexpr int kTcKCh = kFeatPad / kTcBK;   // 7 K chunks
 constexpr int kTcStages = 2;             // ring stages of (A lo chunk | B hi chunk | B lo chunk)
 constexpr int kTcABytes = kTcBM * kTcBK * 4;   // 16 KB
 constexpr int kTcBBytes = kTcBN * kTcBK * 4;   // 12 KB
-constexpr int kTcThreads = 256;
+constexpr int kTcThreads = 384;       // warpgroup 0: TMA producer; warpgroups 1, 2: wgmma + epilogue, 64 frames each
 constexpr int kTcStageBytes = kTcABytes + 2 * kTcBBytes;     // 40 KB
 constexpr int kTcEpiCols = 32;                                 // pose-offset columns per TMA store of the epilogue
-constexpr int kTcEpiBytes = kTcEpiCols * kTcBM * 4;            // 16 KB staging tile [column][frame]
+constexpr int kTcEpiBytes = kTcEpiCols * kTcBM * 4;            // 16 KB: one 8 KB staging tile [column][64 frames] per warpgroup
 constexpr size_t kTcSmem = 1024 /*align slack*/ + (size_t)kTcKCh * kTcABytes + (size_t)kTcStages * kTcStageBytes + kTcEpiBytes + 256;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -57,40 +58,37 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void*
                  ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
-// K-major, 128-byte swizzle, rows of 128 B packed 8 per 1024 B: LBO = 1 (ignored), SBO = 1024 B, version 1
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
+// wgmma shared-memory matrix descriptor: K-major, 128-byte swizzle, rows of 128 B packed 8 per 1024 B
+// (start >> 4, LBO = 1 (unused for swizzled K-major), SBO = 1024 B, layout type 1 = SWIZZLE_128B)
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;                   // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// kind::tf32, fp32 accumulate, A and B K-major, M = 128, N = 96
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 96] (+)= A[64 x 8] . B[96 x 8]^T, tf32 inputs (both K-major in shared memory), fp32 accumulators in registers:
+// with w = t / 32 and l = t % 32 for thread t of the warpgroup, d[4 i + 2 h + j] = D[16 w + l / 4 + 8 h][8 i + 2 (l % 4) + j]
+__device__ __forceinline__ void wgmma_m64n96k8_tf32(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "setp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-        "%24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+        "%48, %49, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
 }
 
 // One vertex of one frame: v_posed = template + shapedirs.betas + pose offset, then linear blend skinning

@@ -15,7 +15,7 @@ closure kernels evaluate (mvs_set_anchor), so frames stay independent inside a s
 ranks exchange ONE boundary frame with each neighbour (344 B halo) and all-reduce two scalars in ONE call (the global
 smoothness energy and the sum of the frames' own losses = the joint objective) -- the only collective on the path, as the
 north-star asks.  Block-Jacobi is a fixed-point iteration of the joint problem's stationarity conditions; its convergence on
-a 64-frame chain is recorded in profiles/r02_cfg5_convergence.json (scripts/cfg5_convergence.py).
+a 64-frame chain is measured by scripts/cfg5_convergence.py.
 """
 from __future__ import annotations
 

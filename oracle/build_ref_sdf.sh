@@ -11,7 +11,7 @@ SRC="$REF/sdf/sdf/csrc/sdf_cuda_kernel.cu"
 [ -f "$SRC" ] || { echo "reference SDF kernel not found at $SRC" >&2; exit 3; }
 mkdir -p "$HERE/_ref"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-"$NVCC" -gencode arch=compute_100a,code=sm_100a -std=c++17 -shared -Xcompiler -fPIC -I "$HERE/refshim" \
+"$NVCC" -gencode arch=compute_90a,code=sm_90a -std=c++17 -shared -Xcompiler -fPIC -I "$HERE/refshim" \
     -o "$HERE/_ref/libsdf_refcuda.so" "$SRC" "$HERE/ref_sdf_wrap.cu"
 sha256sum "$SRC" | cut -d' ' -f1 > "$HERE/_ref/sdf_cuda_kernel.sha256"
 echo "$HERE/_ref/libsdf_refcuda.so"

@@ -1,6 +1,6 @@
 """Convergence of the block-Jacobi sweeps of the jointly regularised sequence mode (cfg5) on a 64-frame chain: joint energy
 (sum of the frames' own losses + lambda * smoothness) after every sweep, against the value after many sweeps (the fixed point of
-the sweeps is a stationary point of the joint problem).  Writes profiles/r02_cfg5_convergence.json.  One GPU:
+the sweeps is a stationary point of the joint problem).  Prints the result as JSON.  One GPU:
     python scripts/cfg5_convergence.py"""
 import json
 import os
@@ -31,4 +31,4 @@ for lam in (5.0, 50.0, 500.0):
                              "sweeps_to_1e-3": need, "iterations": [r["frame_iterations"] for r in res]}
     print("lambda %g: E after sweeps 1..8 %s ... fixed point %.6g; sweeps to 1e-3: %s" % (lam, ["%.6g" % e for e in E[:8]], Einf, need))
     fitter.ctx.close()
-json.dump(out, open(os.path.join(ROOT, "gpurun_out", "r02_cfg5_convergence.json"), "w"), indent=1)
+print(json.dumps(out, indent=1))

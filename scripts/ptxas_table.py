@@ -20,7 +20,7 @@ for p in sorted(glob.glob(sys.argv[1] + "/*.log")):
             dem = re.sub(r"\(.*", "", dem).replace("mvs::", "")
             rows.append((p.split("/")[-1][:-4] + ".cu", dem, m.group(1), m.group(3) or "0", *st))
             name = None
-print("# ptxas resource table, sm_100a (`scripts/ptxas_table.sh`; static shared memory only — the resident,")
+print("# ptxas resource table, sm_90a (`scripts/ptxas_table.sh`; static shared memory only — the resident,")
 print("# frame_step, sdf_fused, skin and GEMM kernels take their shared memory dynamically, see DESIGN.md §4)\n")
 print("| file | kernel | registers | static smem B | stack B | spill st/ld B |")
 print("|---|---|---:|---:|---:|---:|")

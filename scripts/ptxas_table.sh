@@ -1,12 +1,12 @@
 #!/bin/bash
-# Static resource table (registers / stack / spills / static smem) of every kernel, cross-compiled for sm_100a.
-# No GPU needed.  Output: profiles/r01_ptxas.md
+# Static resource table (registers / stack / spills / static smem) of every kernel, cross-compiled for sm_90a.
+# No GPU needed.  Output: markdown on stdout
 set -e
 cd "$(dirname "$0")/.."
 T=$(mktemp -d)
 for f in mvsmplfitting_b200/csrc/*.cu; do
   b=$(basename "$f" .cu)
-  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Iinclude -Xptxas -v -c "$f" -o "$T/$b.o" 2> "$T/$b.log"
+  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Iinclude -Xptxas -v -c "$f" -o "$T/$b.o" 2> "$T/$b.log"
 done
-python scripts/ptxas_table.py "$T" > profiles/r01_ptxas.md
+python scripts/ptxas_table.py "$T"
 rm -rf "$T"

@@ -7,6 +7,7 @@ import os
 import numpy as np
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+DEMO = os.path.join(GOLD, "demo")          # the data the original project ships (data/keypoints, data/3DOH50K_Parameters.txt)
 
 
 def model_checksum(model):
@@ -34,3 +35,11 @@ def load_case(name):
 def relmax(a, b):
     """max-norm relative error of a against reference b"""
     return float(np.abs(np.asarray(a, dtype=np.float64) - b).max() / max(np.abs(b).max(), 1e-30))
+
+
+def snapshot_vposer_weights():
+    """decoder weights of the VPoser snapshot the original project ships (priors/snapshots/poser_epoch091.pkl), as read by its
+    own loader (oracle/make_golden_refruns.py); stored in two files so that each stays under 1 MB"""
+    a, b = np.load(os.path.join(GOLD, "vposer_snapshot_a.npz")), np.load(os.path.join(GOLD, "vposer_snapshot_b.npz"))
+    return dict(fc1_w=a["fc1_w"], fc1_b=a["fc1_b"], fc2_w=np.concatenate([a["fc2_w_top"], b["fc2_w_bottom"]]), fc2_b=a["fc2_b"],
+                out_w=b["out_w"], out_b=b["out_b"])

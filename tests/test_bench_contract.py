@@ -32,16 +32,6 @@ def test_algorithmic_bytes_cover_every_kernel_id():
     assert b.gemm_flops(128.0) == 2.0 * 128 * 207 * 20670
 
 
-def test_committed_traffic_file_matches_kernel_names():
-    import json
-    from mvsmplfitting_b200 import _lib
-    lib = _lib.load()
-    names = {lib.mvs_kernel_name(k).decode() for k in range(_lib.NUM_KERNEL_IDS)}
-    for f in ("r01_traffic.json", "r02_traffic.json"):
-        tr = json.load(open(os.path.join(ROOT, "profiles", f)))
-        assert set(tr) <= names and all(v["traffic"] > 0 for v in tr.values())
-
-
 def test_lanes_and_reference_worker_flags_parse():
     """--inflight (batches in flight) and the hidden --ref-worker mode are part of the command line the driver / the reference arm use"""
     import subprocess

@@ -1,43 +1,10 @@
-"""CPU: the drop-in layer reads model / camera / loss objects by duck typing.  Here the objects are the
-REFERENCE's own modules (authoring container only): what the layer extracts must be exactly what the
-reference modules hold, so the reference's init.py / non_linear_solver.py can hand them over unchanged."""
+"""CPU: the drop-in layer's mirror modules have the surface of the reference's modules, so that its init.py /
+non_linear_solver.py can hand them over unchanged."""
 import numpy as np
 import pytest
 import torch
 
 from mvsmplfitting_b200 import synthetic as S
-
-
-@pytest.mark.needs_reference
-def test_extraction_from_reference_objects(syn_model, syn_gmm):
-    from oracle import ref_harness as H
-    from mvsmplfitting_b200 import fitting as F
-    ns = H.import_reference()
-    rm = H.build_reference_model(syn_model)
-    d, mt, jmap, extra = F.extract_model(rm)
-    assert mt == "smpllsp"
-    assert np.array_equal(jmap, S.JOINT_MAP_LSP14) and np.array_equal(extra, S.FACE_VERTEX_IDS)
-    assert d["posedirs"].shape == (207, 3 * 6890)
-    assert np.array_equal(d["posedirs"], np.reshape(syn_model["posedirs"], [-1, 207]).T)
-    assert np.array_equal(d["lsp_regressor"], syn_model["lsp_regressor"])
-    assert d["parents"][0] == -1 and np.array_equal(d["parents"][1:], S.SMPL_PARENTS[1:])
-    cams = S.make_cameras(3)
-    rc = H.build_reference_cameras(cams)
-    R, t, f, c = F._camera_params(rc[1])
-    assert np.array_equal(R, cams["R"][1]) and np.array_equal(t, cams["t"][1]) and np.allclose(f, cams["f"][1])
-    gp = H.build_reference_gmm(syn_gmm)
-    loss = ns.fitting.create_loss("smplify", rho=100.0, use_joints_conf=True, dtype=torch.float32, body_pose_prior=gp,
-                                  shape_prior=ns.prior.create_prior("l2"), angle_prior=ns.prior.create_prior("angle"),
-                                  interpenetration=False, fix_shape=False)
-    loss.reset_loss_weights(dict(data_weight=0.3, body_pose_weight=4.78, shape_weight=5.0, bending_prior_weight=15.0))
-    rg = dict(betas=True, global_orient=True, body_pose=True, transl=True, scale=False)
-    cfg, kind = F.loss_config_from(loss, rg, use_vposer=False)
-    assert kind == "gmm" and cfg.body_prior == 1 and cfg.frozen_mask == 1 << 4
-    assert abs(cfg.body_pose_weight - 4.78) < 1e-6 and abs(cfg.data_weight - 0.3) < 1e-6 and cfg.rho == 100.0
-    loss2 = ns.fitting.create_loss("smplify", rho=100.0, body_pose_prior=ns.prior.create_prior("l2"),
-                                   shape_prior=ns.prior.create_prior("l2"), angle_prior=ns.prior.create_prior("angle"),
-                                   interpenetration=False)
-    assert F.loss_config_from(loss2, rg, use_vposer=False)[1] == "l2"
 
 
 def test_mirror_modules_have_the_reference_surface(tmp_path, syn_model, syn_gmm):

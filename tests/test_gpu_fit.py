@@ -167,3 +167,24 @@ def test_fit_seq_guards(syn_model, syn_gmm):
     final, st = ctx.fit(x, _stages(ctx), ctx.make_lbfgs_config(max_outer=1), warm=[False, False])      # no warm frame: plain mvs_fit
     assert st["frames_nan"] == 0 and torch.isfinite(final).all()
     ctx.close()
+
+
+def test_fit_keeps_parameters_finite_when_a_line_search_ends_on_a_non_finite_point(syn_model, syn_gmm):
+    """Frame 91 of the benchmark's first batch (8 views, seed 1000, SDF term on a 128 grid in stages 2-3) ends stage 2 on
+    the jump of the as-written SDF term, and a stage-3 line search from there reaches only non-finite trial points.  The
+    optimiser keeps the line search's start instead of writing NaN into the parameters, so the fit ends finite."""
+    cams = S.make_cameras(8)
+    fr = S.make_frames(syn_model, cams, 256, seed=1000)
+    sl = slice(91, 92)
+    ctx = _ctx(syn_model, cams, syn_gmm, 1)
+    ctx.set_keypoints(np.ascontiguousarray(fr["gt_uv"][:, sl]), np.ascontiguousarray(fr["conf"][:, sl]), fr["joint_weights"])
+    sw = S.STAGE_WEIGHTS
+    stages = [ctx.make_loss_config(body_prior="gmm", interpenetration=True, sdf_grid=128, data_weight=500.0 / 1536,
+                                   body_pose_weight=sw["body_pose_prior_weights"][i], shape_weight=sw["shape_weights"][i],
+                                   bending_prior_weight=3.17 * sw["body_pose_prior_weights"][i],
+                                   coll_loss_weight=sw["coll_loss_weights"][i]) for i in range(4)]
+    x = torch.tensor(S.pack_params(fr["init"])[sl], device="cuda")
+    final, st = ctx.fit(x, stages)
+    torch.cuda.synchronize()
+    assert st["frames_nan"] == 0 and torch.isfinite(final).all() and torch.isfinite(x).all(), (final, st)
+    ctx.close()

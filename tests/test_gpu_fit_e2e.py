@@ -2,7 +2,8 @@
 
 * SDF off: tests/golden/fit_e2e_ref.npz (oracle/make_golden_fit.py: the reference's own non_linear_solver on 16 frames,
   torch CPU).  The benchmark metric counts L-BFGS iterations, so the counts themselves are pinned here.
-* SDF on: the reference runs live on torch-CUDA with its own SDF kernel (oracle/_ref), the only place it can.
+* SDF on: tests/golden/fit_e2e_sdf_ref.npz (oracle/make_golden_refruns.py: the same solver on torch-CUDA with the
+  reference's own SDF kernel, the only place it can run, on 16 frames).
 
 L-BFGS with ftol = 1e-9 on an fp32 loss is chaotic in the last bits: closures that agree to 1e-7 stop after different
 iteration counts (the reference against its own fp64 run does too).  So single trajectories are not comparable; what is
@@ -77,16 +78,14 @@ def test_four_stage_fit_matches_reference_fixture(syn_model, syn_gmm):
 
 
 def test_four_stage_fit_with_sdf_matches_live_reference_run(syn_model, syn_gmm):
-    from oracle import ref_harness as RH, ref_sdf
-    if not (RH.available() and ref_sdf.available()):
-        pytest.skip("reference tree / SDF kernel not staged (python -m oracle.stage_reference)")
-    from oracle import ref_fit as RF
-    B, V = 16, 8
+    z = np.load(os.path.join(G.GOLD, "fit_e2e_sdf_ref.npz"))
+    B, V = int(z["B"]), int(z["V"])
     cams = S.make_cameras(V)
-    fr = S.make_frames(syn_model, cams, B, seed=4200)
+    fr = S.make_frames(syn_model, cams, B, seed=int(z["seed"]))
     X0 = S.pack_params(fr["init"])
-    sc = RF.build_scene(syn_model, syn_gmm, cams, device="cuda")
-    runs = [RF.fit_frame(sc, fr, b, S.STAGE_WEIGHTS, interpenetration=True) for b in range(B)]
+    assert np.array_equal(X0, z["X0"]), "synthetic frame generator changed: regenerate the fixture"
+    runs = [dict(iterations=int(z["iterations"][b]), evals=int(z["evals"][b]), final_loss=float(z["final_loss"][b]),
+                 params=z["params"][b], per_stage=z["per_stage"][b].tolist()) for b in range(B)]
     ref_it = np.mean([r["iterations"] for r in runs]); ref_ev = np.mean([r["evals"] for r in runs])
     ref_final = np.array([r["final_loss"] for r in runs])
     final, x, st = device_fit(syn_model, syn_gmm, cams, fr, X0, sdf=True)

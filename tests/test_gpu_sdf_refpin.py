@@ -1,24 +1,28 @@
 """GPU: the SDF interpenetration term pinned to the REFERENCE'S OWN CUDA kernel.
 
-oracle/_ref/libsdf_refcuda.so is sdf/sdf/csrc/sdf_cuda_kernel.cu of the reference compiled unchanged (oracle/build_ref_sdf.sh:
-only an <ATen/ATen.h> stand-in and a C entry point are added).  Checked against it, voxel for voxel:
+The reference's sdf/sdf/csrc/sdf_cuda_kernel.cu, compiled unchanged (oracle/build_ref_sdf.sh: only an <ATen/ATen.h>
+stand-in and a C entry point are added), was run by oracle/make_golden_refruns.py; its grids (whole, or every inside voxel
+and a seeded sample of the others for the large ones) are stored in tests/golden/refpin_grids.npz.  Checked against
+them, voxel for voxel:
   * mvs_sdf_grid (the product's replacement of the op sdf.csrc.sdf),
   * oracle/sdf_ref.c (the plain-C restatement every other SDF test uses as its checker),
-and, through the UNMODIFIED reference closure (code/utils/fitting.py:162-203,352-393 on torch-CUDA, staged under
-oracle/_ref/reference by oracle/stage_reference.py) with that kernel as its `sdf.csrc`:
+and, against the UNMODIFIED reference closure (code/utils/fitting.py:162-203,352-393 on torch-CUDA) with that kernel as its
+`sdf.csrc` (tests/golden/refpin_closure.npz):
   * mvs_closure with interpenetration on -- the batched chain and (exec mode 3) the dense-regime kernels the optimiser
     runs in SDF stages -- loss and every gradient segment within the 1e-4 parity bar.
 """
+import os
+
 import numpy as np
 import pytest
 import torch
 
 from mvsmplfitting_b200 import synthetic as S
-from oracle import ref_sdf, sdf_oracle
+from oracle import sdf_oracle
 from oracle.lbfgs_oracle import PARAM_SEGMENTS
 from tests import golden_util as G
 
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not ref_sdf.available(), reason="oracle/_ref/libsdf_refcuda.so not built")]
+pytestmark = pytest.mark.gpu
 
 SEG_NAMES = ("betas", "global_orient", "body_pose", "transl", "scale")
 
@@ -51,21 +55,29 @@ def _compare(name, phi, ref):
     return int(flips.sum()), md
 
 
+def _ref_grid(grid, as_written, B, nf_used):
+    """(flat voxel indices, reference kernel's phi there, its inside-voxel count over the whole grid)"""
+    z = np.load(os.path.join(G.GOLD, "refpin_grids.npz"))
+    k = "g%d_%s_b%d_f%s" % (grid, "aw" if as_written else "all", B, "all" if nf_used is None else nf_used)
+    return z[k + "_idx"], z[k + "_phi"], int(z[k + "_inside_total"])
+
+
 @pytest.mark.parametrize("grid,as_written,B,nf_used", [(128, True, 2, None), (32, False, 1, None), (64, True, 3, None), (48, False, 1, 900)])
 def test_grid_op_and_c_restatement_match_the_reference_kernel(grid, as_written, B, nf_used, syn_model, syn_gmm):
     vn = normalised_verts(syn_model, B, 3)
     faces = syn_model["f"] if nf_used is None else syn_model["f"][:nf_used]
     f_dev = torch.tensor(faces.astype(np.int32), device="cuda")
     v_dev = torch.tensor(vn, device="cuda")
-    ref = ref_sdf.grid(f_dev, v_dev, grid, as_written=as_written).cpu().numpy()
+    idx, ref, inside_total = _ref_grid(grid, as_written, B, nf_used)
     if as_written:
-        assert (ref > 0).any(), "triangle 0 must shadow some voxels"
+        assert inside_total > 0, "triangle 0 must shadow some voxels"
     ctx = make_ctx(syn_model, S.make_cameras(2), 1, syn_gmm)
     ours = ctx.sdf_grid(f_dev, v_dev, grid, num_faces=(1 if as_written else faces.shape[0])).cpu().numpy()
     c_port = sdf_oracle.sdf_grid(faces, vn, grid, all_faces=not as_written)
     # the reference launches (B G^3) / 512 blocks, integer division (sdf_cuda_kernel.cu:316-317): a tail of < 512 voxels
     # keeps phi's initial zeros -- reproduced by both
-    assert ours.shape == ref.shape == c_port.shape
+    assert ours.shape == c_port.shape == (B, grid, grid, grid)
+    ours, c_port = ours.reshape(-1)[idx], c_port.reshape(-1)[idx]
     fl_o, md_o = _compare("mvs_sdf_grid vs reference kernel", ours, ref)
     fl_c, md_c = _compare("oracle/sdf_ref.c vs reference kernel", c_port, ref)
     # same arithmetic, same compiler: no inside / outside decision may differ, distances within 2 ulp of the largest
@@ -73,42 +85,8 @@ def test_grid_op_and_c_restatement_match_the_reference_kernel(grid, as_written, 
     # compiler's choice of which product of  a*b - c*d  joins the FMA may differ (measured: 1 ulp on a few voxels)
     assert fl_o == 0 and md_o <= 4.8e-7
     # the C restatement is built without FMA contraction: a voxel whose ray grazes an edge may flip (counted, <= 1e-4 of
-    # the grid), everything else within a few ulp
+    # the compared voxels), everything else within a few ulp
     assert fl_c <= max(1, int(1e-4 * ref.size)) and md_c < 2e-6
-
-
-def _reference_runs(model, gmm, cams, fr, w, cw, B):
-    from oracle import ref_harness as RH
-    ref_model = RH.build_reference_model(model)
-    ref_cams = RH.build_reference_cameras(cams)
-    prior = RH.build_reference_gmm(gmm)
-    outs = [RH.reference_closure_eval(ref_model, ref_cams, fr, b, w, prior, device="cuda", interpenetration=True,
-                                      coll_loss_weight=cw) for b in range(B)]
-    outs0 = [RH.reference_closure_eval(ref_model, ref_cams, fr, b, w, prior, device="cuda", interpenetration=False)
-             for b in range(B)]
-    loss = np.array([o["loss"] for o in outs])
-    loss0 = np.array([o["loss"] for o in outs0])
-    grad = np.stack([np.concatenate([o["grads"][k] for k in SEG_NAMES]) for o in outs])
-    return loss, grad, loss0
-
-
-def _fp64_arbiter(model, gmm, cams, fr, w, cw, grid, X):
-    """the reference's formulas in float64 (oracle glue) on a grid from the REFERENCE kernel: what the reference's fp32 run and
-    the product both approximate; the distance between the reference's own fp32 run and this is its noise floor"""
-    from oracle import closure_oracle as O
-
-    def ref_grid(faces, vn, G_, all_faces=False):
-        return ref_sdf.grid(torch.tensor(np.asarray(faces, dtype=np.int32), device="cuda"),
-                            torch.tensor(np.asarray(vn, dtype=np.float32), device="cuda"), G_, as_written=not all_faces).cpu().numpy()
-    old = sdf_oracle.GRID_FN
-    sdf_oracle.GRID_FN = ref_grid
-    try:
-        om = O.OracleModel.from_numpy(model, dtype=torch.float64)
-        pri = O.OraclePriors.gmm_from_dict(gmm, torch.float64)
-        cfg = O.LossConfig(interpenetration=True, coll_loss_weight=cw, sdf_grid=grid, **w)
-        return O.closure_eval_batch(om, cfg, pri, O.cams_to_torch(cams, torch.float64), X, fr["gt_uv"], fr["conf"], fr["joint_weights"])
-    finally:
-        sdf_oracle.GRID_FN = old
 
 
 @pytest.mark.parametrize("exec_mode", [0, 3])
@@ -119,18 +97,19 @@ def test_closure_with_interpenetration_matches_reference_run(exec_mode, syn_mode
     body is scaled) and is computed as a sum of cancelling terms of magnitude 1e6, so the reference's OWN fp32 run sits
     6e-5 from the float64 evaluation of its formulas (and a faithful fp32 restatement on the CPU 1.0e-4): for that one
     scalar the bar is 5e-4 against the closer of the reference run and the float64 evaluation."""
-    from oracle import ref_harness as RH
-    if not RH.available():
-        pytest.skip("reference tree not staged (python -m oracle.stage_reference)")
     B, grid, cw = 6, 128, 1000.0
     cams = S.make_cameras(4)
     fr = S.make_frames(syn_model, cams, B, seed=2)
     w = dict(data_weight=500.0 / 1536, body_pose_weight=57.4, shape_weight=10.0, bending_prior_weight=3.17 * 57.4)
-    ref_loss, ref_grad, ref_loss0 = _reference_runs(syn_model, syn_gmm, cams, fr, w, cw, B)
+    z = np.load(os.path.join(G.GOLD, "refpin_closure.npz"))
+    ref_loss, ref_grad, ref_loss0 = z["ref_loss"], z["ref_grad"], z["ref_loss0"]
     pen = ref_loss - ref_loss0
     assert (pen > 0).sum() >= 2, "test frames must exercise the term"
     X = S.pack_params(fr["init"])
-    arb = _fp64_arbiter(syn_model, syn_gmm, cams, fr, w, cw, grid, X)
+    assert np.array_equal(X, z["X"]), "synthetic frame generator changed: regenerate the fixture"
+    # the reference's formulas in float64 (oracle glue) on a grid from the REFERENCE kernel: what the reference's fp32 run and
+    # the product both approximate; the distance between the reference's own fp32 run and this is its noise floor
+    arb = dict(loss=z["arb_loss"], grad=z["arb_grad"])
     ctx = make_ctx(syn_model, cams, B, syn_gmm)
     ctx.set_keypoints(fr["gt_uv"], fr["conf"], fr["joint_weights"])
     ctx.set_exec_mode(exec_mode)
@@ -162,27 +141,15 @@ def test_closure_with_interpenetration_matches_reference_run(exec_mode, syn_mode
 
 def test_all_faces_closure_matches_oracle_on_reference_kernel_grid(syn_model, syn_gmm):
     """intended semantics (every face): the reference's Python call cannot produce it, so the checker is the oracle glue
-    (oracle/sdf_oracle.py, fitting.py:352-393 restated) sampling a grid computed by the REFERENCE kernel with faces.size(0) = F"""
-    from oracle import closure_oracle as O
+    (oracle/sdf_oracle.py, fitting.py:352-393 restated) sampling a grid computed by the REFERENCE kernel with faces.size(0) = F
+    (tests/golden/refpin_closure.npz)"""
     B, grid, cw = 2, 16, 0.05
     cams = S.make_cameras(4)
     fr = S.make_frames(syn_model, cams, B, seed=2)
     w = dict(data_weight=500.0 / 1536, body_pose_weight=57.4, shape_weight=10.0, bending_prior_weight=3.17 * 57.4)
     X = S.pack_params(fr["init"])
-
-    def ref_grid(faces, vn, G_, all_faces=False):
-        return ref_sdf.grid(torch.tensor(np.asarray(faces, dtype=np.int32), device="cuda"),
-                            torch.tensor(np.asarray(vn, dtype=np.float32), device="cuda"), G_, as_written=not all_faces).cpu().numpy()
-
-    old = sdf_oracle.GRID_FN
-    sdf_oracle.GRID_FN = ref_grid
-    try:
-        om = O.OracleModel.from_numpy(syn_model, dtype=torch.float32)
-        pri = O.OraclePriors.gmm_from_dict(syn_gmm, torch.float32)
-        cfg = O.LossConfig(interpenetration=True, coll_loss_weight=cw, sdf_grid=grid, sdf_all_faces=True, **w)
-        ref = O.closure_eval_batch(om, cfg, pri, O.cams_to_torch(cams, torch.float32), X, fr["gt_uv"], fr["conf"], fr["joint_weights"])
-    finally:
-        sdf_oracle.GRID_FN = old
+    z = np.load(os.path.join(G.GOLD, "refpin_closure.npz"))
+    ref = dict(loss=z["allfaces_loss"], grad=z["allfaces_grad"])
     for mode in (0, 3):
         ctx = make_ctx(syn_model, cams, B, syn_gmm)
         ctx.set_keypoints(fr["gt_uv"], fr["conf"], fr["joint_weights"])

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 / TMA dense vertex forward (mvs_tc.cu) against the fp32 SIMT kernel and the oracle."""
+"""GPU: the wgmma / TMA dense vertex forward (mvs_tc.cu) against the fp32 SIMT kernel and the oracle."""
 import numpy as np
 import pytest
 import torch

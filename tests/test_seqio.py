@@ -2,14 +2,13 @@
 import json
 import os
 import pickle
-import sys
 
 import numpy as np
 import pytest
 
 from mvsmplfitting_b200 import seqio
 
-REF = "/root/reference"
+DEMO = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "demo")       # data the original project ships
 
 
 def write_demo(tmp, V=3, B=4, missing=((1, 2),), seed=0):
@@ -184,21 +183,15 @@ def test_fit_sequences_lockstep_warm_start(tmp_path):
     assert sorted(os.listdir(tmp_path / "res" / "0007")) == a["frames"]
 
 
-@pytest.mark.needs_reference
 def test_readers_equal_the_reference_on_its_demo_data():
-    """the reference's own load_camera_para / read_keypoints on the data it ships (authoring container only)"""
-    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    from oracle import ref_harness as H
-    H.import_reference()
-    with H.in_reference_dir():
-        from utils.utils import load_camera_para
-        from utils.data_parser import read_keypoints
-    e_ref, i_ref = load_camera_para(os.path.join(REF, "data", "3DOH50K_Parameters.txt"))
-    e, i = seqio.load_camera_para(os.path.join(REF, "data", "3DOH50K_Parameters.txt"))
-    assert e.shape == (6, 4, 4) and np.array_equal(e, e_ref) and np.array_equal(i, i_ref)
-    seq = seqio.load_sequence(os.path.join(REF, "data", "keypoints"), "0000")
+    """against what the original project's own load_camera_para / read_keypoints return for the data it ships
+    (tests/golden/demo_readers_ref.npz, oracle/make_golden_refruns.py)"""
+    ref = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "demo_readers_ref.npz"))
+    e, i = seqio.load_camera_para(os.path.join(DEMO, "3DOH50K_Parameters.txt"))
+    assert e.shape == (6, 4, 4) and np.array_equal(e, ref["extrinsics"]) and np.array_equal(i, ref["intrinsics"])
+    seq = seqio.load_sequence(os.path.join(DEMO, "keypoints"), "0000")
     assert len(seq["cameras"]) == 6 and seq["frames"] == ["00001"] and seq["present"].all()
-    for v, cam in enumerate(seq["cameras"]):
-        ref = read_keypoints(os.path.join(REF, "data", "keypoints", "0000", cam, "00001_keypoints.json"),
-                             use_hands=False, use_face=False).keypoints[0]
-        assert np.array_equal(seq["gt_uv"][v, 0], ref[:, :2]) and np.array_equal(seq["conf"][v, 0], ref[:, 2])
+    assert list(seq["cameras"]) == ref["cameras"].tolist()
+    for v in range(len(seq["cameras"])):
+        kp = ref["keypoints"][v]
+        assert np.array_equal(seq["gt_uv"][v, 0], kp[:, :2]) and np.array_equal(seq["conf"][v, 0], kp[:, 2])

@@ -96,13 +96,8 @@ REAL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "vpose
 
 
 def _real_weights():
-    """decoder weights of the snapshot the reference ships (priors/snapshots/poser_epoch091.pkl), read through the reference's
-    own loader from /root/reference or the staged copy under oracle/_ref/reference; the fixture itself holds no weights"""
-    import pytest
-    from oracle import ref_harness as RH
-    if not RH.available() or not os.path.exists(os.path.join(RH.REF_ROOT, "priors", "snapshots", "poser_epoch091.pkl")):
-        pytest.skip("reference snapshot not present (python -m oracle.stage_reference)")
-    return RH.vposer_weights_numpy(RH.load_reference_vposer())
+    """decoder weights of the snapshot the original project ships (priors/snapshots/poser_epoch091.pkl)"""
+    return G.snapshot_vposer_weights()
 
 
 def test_shipped_snapshot_known_answer_and_restatement(syn_model):
