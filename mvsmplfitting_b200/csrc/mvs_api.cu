@@ -204,7 +204,7 @@ int mvs_set_model(mvs_ctx* ctx, const mvs_model_desc* d) {
         }
         int rc = dev_upload(ctx, &m.Qk, Q.data(), Q.size());
         if (rc) return rc;
-        if ((rc = tc_upload_model(ctx, Q.data()))) return rc;
+        if ((rc = tc_upload_model(ctx))) return rc;
         std::vector<float> stv((size_t)N * 33);
         for (int n = 0; n < N; ++n)
             for (int c = 0; c < 3; ++c) {

@@ -280,7 +280,7 @@ int launch_vertex_fwd_dense(mvs_ctx* ctx, cudaStream_t st, bool allow_tc = true,
 int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);                      // mvs_closure.cu
 int launch_sdf_fused(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu
 // mvs_tc.cu: wgmma / TMA dense vertex forward
-int tc_upload_model(mvs_ctx* ctx, const float* Qk_host);
+int tc_upload_model(mvs_ctx* ctx);                 // after m.Qk is on the device
 bool tc_available(const mvs_ctx* ctx);
 int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed = true);
 int tc_check_error(mvs_ctx* ctx);

@@ -2,18 +2,22 @@
 //
 //   pose_offsets[b, 3n+c] = sum_k  pose_feature[b,k] * posedirs[k, 3n+c]        (lbs.py:192-195)
 //
-// is the one dense contraction of the path: M = frames in flight, N = 20670, K = 207.  It is skinny in M
-// (<= a few hundred frames), so it is bound by streaming the 17 MB of posedirs from L2/HBM once per 128-frame
-// tile, not by tensor throughput; the kernel is therefore organised around keeping the A operand (the frames'
-// pose features, 112 KB; only the live 8-row groups are fetched when few frames are active) RESIDENT in shared memory
-// for the CTA's whole life while posedirs tiles stream through a TMA ring:
+// is the one dense contraction of the path: 20670 posedirs rows x K = 207 against the frames in flight (a few hundred at
+// most, usually a few dozen, one to three at the tail of a stage).  It is bound by streaming the 18.5 MB of fp32 posedirs,
+// not by tensor throughput, so the kernel is organised to read posedirs exactly once per launch at any active count up to
+// one column tile, and to keep enough of it in flight to approach HBM bandwidth:
 //
-//   warpgroup 0      TMA producer (one thread): A once (7 boxes 128x32, or 8-row boxes), then B boxes 96x32 through
-//                    a 2-stage mbarrier ring
-//   warpgroups 1, 2  wgmma.m64n96k8.f32.tf32 on 64 frames each, fp32 accumulators in registers; each warpgroup
-//                    releases a ring stage once its MMAs on it have retired, then stores its 64 x 96 tile of pose
-//                    offsets TRANSPOSED (frame fastest) through shared memory and the TMA store engine.  A warpgroup
-//                    whose 64 frames are all inactive exits at once.
+//   transposed product   poffT[3N][frames] = Qk[:, :207] . Phi^T: posedirs rows are the wgmma M side (64 per warpgroup),
+//                        the active frames the N side (8 .. 128, the instance is chosen from the host's bound of the
+//                        active count; batches above 128 run column tiles of 128 frames as a second grid dimension).  The
+//                        accumulator fragment is [coordinate][frame], the layout of poffT, and is stored straight from
+//                        registers.
+//   warp 8               TMA producer (one thread): per (row tile, k chunk) the fp32 posedirs box 128 x 32 (straight from
+//                        the model's Qk rows) and the frames' feature hi and lo boxes, through a 4-stage mbarrier ring.
+//   warpgroups 0, 1      64 posedirs rows each: load the fp32 A fragment from shared memory, split it into TF32 hi and lo
+//                        in registers, issue wgmma.m64nNk8 with A from registers and B (features) from shared memory; one
+//                        wgmma group stays in flight while the next chunk is split, and a ring stage is released once the
+//                        group that read it has retired.  CTAs are persistent over a contiguous range of row tiles.
 //
 // The rest of the vertex forward (template + shape blend shapes in fp32, linear blend skinning, box partials) is
 // skin_kernel / skin_small_kernel below.
@@ -22,8 +26,9 @@
 // the tensor cores accumulate hi*hi + lo*hi + hi*lo in fp32 (the dropped lo*lo term is 2^-22 of a product), i.e. the pose
 // offsets come out with fp32-class accuracy.  Plain TF32 leaves 1e-6 absolute on a vertex: harmless for the joints, but
 // the SDF samples are voxel-sized distances, so it is a 1e-5 .. 1e-4 relative error of the interpenetration term and
-// pushes its gradient past the 1e-4 parity bar.  The path is bound by operand streaming, so the 3x MMA count is free;
-// the price is operand traffic (B hi + B lo, and the A lo chunks stream through the ring).
+// pushes its gradient past the 1e-4 parity bar.  The features are split by the kernels that compute them (PhiTc); posedirs
+// is split on chip, so only one fp32 copy of it exists and streams.  Per k8 step the products are issued in the order
+// F_hi.P_hi, F_lo.P_hi, F_hi.P_lo, each an exact product of two TF32 numbers accumulated in fp32.
 // The template and the shape blend shapes are NOT sent through the tensor cores.
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -41,82 +46,55 @@ __device__ long long g_tc_clk[32];      // clock64 stamps of CTA (0,0): see scri
 #define TC_MARK(i) do {} while (0)
 #endif
 
+template <int NF>
 __global__ void __launch_bounds__(kTcThreads, 1)
-posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_a8,
-                        const __grid_constant__ CUtensorMap map_b, const __grid_constant__ CUtensorMap map_o, int ldA, int ncols,
+posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constant__ CUtensorMap map_f, int ldA, int nrows,
                         const int* __restrict__ na_ptr, int cta_slots, int ntiles, float* __restrict__ poffT,
                         int* __restrict__ err_flag) {
+    constexpr uint32_t kFBytes = tc_fbytes(NF), kStageBytes = tc_stage_bytes(NF);
     pdl_wait();
     extern __shared__ unsigned char smem_raw[];
-    unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    unsigned char* sA = base;                                        // A hi: 7 x [128 rows][128 B], 1024-aligned, resident
-    unsigned char* sR = sA + (size_t)kTcKCh * kTcABytes;             // ring: kTcStages x (A lo chunk 16 KB | B hi chunk 12 KB | B lo chunk 12 KB)
-    float* sO = reinterpret_cast<float*>(sR + (size_t)kTcStages * kTcStageBytes);       // epilogue staging: 2 x [32 columns][64 frames]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sR + (size_t)kTcStages * kTcStageBytes + kTcEpiBytes);
-    uint64_t* a_full = bars;                      // [1]
-    uint64_t* b_full = bars + 1;                  // [stages]
-    uint64_t* b_empty = b_full + kTcStages;       // [stages]
+    unsigned char* sR = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    // ring: kTcStages x (posedirs fp32 [128 rows][128 B] | features hi [NF rows][128 B] | features lo), all 1024-aligned
+    uint64_t* full = reinterpret_cast<uint64_t*>(sR + (size_t)kTcStages * kStageBytes);      // [stages]
+    uint64_t* empty = full + kTcStages;                                                      // [stages]
 
     const int na = *na_ptr;
-    const int m0 = blockIdx.y * kTcBM;
-    if (m0 >= na) return;
-    // the launch provides cta_slots CTAs per M tile of the FULL batch; with fewer active M tiles the survivors
-    // spread the vertex tiles over all of them (the tail of a stage runs one M tile on every SM)
-    const int active_m = (na + kTcBM - 1) / kTcBM;
-    const int ctas_n = max(1, min((int)gridDim.x, cta_slots / active_m));
-    if ((int)blockIdx.x >= ctas_n) return;
-    const int tiles_per_cta = (ntiles + ctas_n - 1) / ctas_n;
+    const int f0 = blockIdx.y * kTcCols;                              // this CTA's column tile of frames
+    if (f0 >= na) return;
+    // the launch provides cta_slots CTAs per column tile of the bound; with fewer active column tiles the survivors
+    // spread the row tiles over all of them
+    const int active_c = (na + kTcCols - 1) / kTcCols;
+    const int ctas = max(1, min((int)gridDim.x, cta_slots / active_c));
+    if ((int)blockIdx.x >= ctas) return;
+    const int tiles_per_cta = (ntiles + ctas - 1) / ctas;
     const int tile_begin = blockIdx.x * tiles_per_cta;
     const int tile_end = min(tile_begin + tiles_per_cta, ntiles);
     if (tile_begin >= tile_end) return;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int live_rows = min(kTcBM, na - m0);
-    const int live_wgs = (live_rows + kTcWgM - 1) / kTcWgM;          // consumer warpgroups with at least one active frame
     if (threadIdx.x == 0) TC_MARK(0);
 
     if (threadIdx.x == 0) {
-        mbar_init(a_full, 1);
-        for (int s = 0; s < kTcStages; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], live_wgs); }
+        for (int s = 0; s < kTcStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
     if (threadIdx.x == 0) TC_MARK(1);
 
-    if (warp < 4) {
-        if (warp == 0 && lane == 0) {
-            // ---------------- TMA producer
-            // A operand.  Every CTA of the M tile reads it, so with one CTA per SM the 112 KB tile costs as much L2
-            // traffic as posedirs itself; at the tail of a fit only a few of its 128 rows are live, and those are fetched
-            // as 8-row boxes (one swizzle atom each: same shared-memory image).  Rows that are not loaded hold whatever
-            // was there: their accumulator rows are never stored.
-            // lo parts: rows ldA.. of the A array, rows ncols.. of the posedirs array (same tensor maps, row offset)
-            const bool small = live_rows <= 32;
-            const int groups = (live_rows + 7) / 8;
-            if (small) {
-                mbar_expect_tx(a_full, kTcKCh * groups * 8 * kTcBK * 4);
-                for (int kc = 0; kc < kTcKCh; ++kc)
-                    for (int gq = 0; gq < groups; ++gq)
-                        tma_load_2d(sA + (size_t)kc * kTcABytes + (size_t)gq * 1024, &map_a8, kc * kTcBK, m0 + 8 * gq, a_full);
-            } else {
-                mbar_expect_tx(a_full, kTcKCh * kTcABytes);
-                for (int kc = 0; kc < kTcKCh; ++kc) tma_load_2d(sA + (size_t)kc * kTcABytes, &map_a, kc * kTcBK, m0, a_full);
-            }
-            const uint32_t stage_bytes = (small ? groups * 8 * kTcBK * 4 : kTcABytes) + 2 * kTcBBytes;
+    if (warp == 8) {
+        if (lane == 0) {
+            // ---------------- TMA producer.  Rows past 3N (last row tile) are zero-filled by the tensor map; feature rows
+            // past the active frames hold stale slots, which only feed accumulator columns that are never stored.
+            // lo parts of the features: rows ldA.. of PhiTc (same tensor map, row offset)
             int stage = 0; uint32_t phase = 0;
             for (int tile = tile_begin; tile < tile_end; ++tile) {
                 for (int kc = 0; kc < kTcKCh; ++kc) {
-                    if (!mbar_wait(&b_empty[stage], phase ^ 1, err_flag)) return;
-                    unsigned char* sAl = sR + (size_t)stage * kTcStageBytes;
-                    unsigned char* sBh = sAl + kTcABytes;
-                    unsigned char* sBl = sBh + kTcBBytes;
-                    mbar_expect_tx(&b_full[stage], stage_bytes);
-                    if (small) {
-                        for (int gq = 0; gq < groups; ++gq) tma_load_2d(sAl + (size_t)gq * 1024, &map_a8, kc * kTcBK, ldA + m0 + 8 * gq, &b_full[stage]);
-                    } else {
-                        tma_load_2d(sAl, &map_a, kc * kTcBK, ldA + m0, &b_full[stage]);
-                    }
-                    tma_load_2d(sBh, &map_b, kc * kTcBK, tile * kTcBN, &b_full[stage]);
-                    tma_load_2d(sBl, &map_b, kc * kTcBK, ncols + tile * kTcBN, &b_full[stage]);
+                    if (!mbar_wait(&empty[stage], phase ^ 1, err_flag)) return;
+                    unsigned char* sP = sR + (size_t)stage * kStageBytes;
+                    mbar_expect_tx(&full[stage], kStageBytes);
+                    tma_load_2d(sP, &map_p, kc * kTcBK, tile * kTcRows, &full[stage]);
+                    tma_load_2d(sP + kTcPBytes, &map_f, kc * kTcBK, f0, &full[stage]);
+                    tma_load_2d(sP + kTcPBytes + kFBytes, &map_f, kc * kTcBK, ldA + f0, &full[stage]);
                     if (++stage == kTcStages) { stage = 0; phase ^= 1; }
                 }
             }
@@ -124,63 +102,71 @@ posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_
         return;
     }
 
-    // ---------------- consumer warpgroup g: frames m0 + 64 g .. m0 + 64 g + 63
-    const int g = warp / 4 - 1;
-    if (g >= live_wgs) return;
-    const int wt = threadIdx.x - 128 * (g + 1);                       // thread of the warpgroup
-    const uint32_t a_row_off = (uint32_t)(g * kTcWgM * kTcBK * 4);    // 64 rows of 128 B = 8 swizzle atoms
-    float* sOw = sO + (size_t)g * kTcEpiCols * kTcWgM;
-    const int row = 16 * (wt >> 5) + ((wt & 31) >> 2);                // accumulator rows row, row + 8
-    const int colq = 2 * (wt & 3);                                    // accumulator columns 8 i + colq (+ 1)
-    float acc[kTcBN / 2];
+    // ---------------- consumer warpgroup g: posedirs rows 64 g .. 64 g + 63 of each row tile
+    const int g = warp >> 2;
+    const int wt = threadIdx.x & 127;                                  // thread of the warpgroup
+    const int q = lane & 3;
+    const int frow = kTcWgRows * g + 16 * (wt >> 5) + (lane >> 2);    // A fragment / accumulator rows frow, frow + 8
+    const int xr = (lane >> 2) & 7;                                   // 128-byte swizzle phase of those rows
+    float acc[NF / 2];
 #pragma unroll
-    for (int i = 0; i < kTcBN / 2; ++i) acc[i] = 0.f;
-    if (!mbar_wait(a_full, 0, err_flag)) return;
-    if (wt == 0) TC_MARK(2);
+    for (int i = 0; i < NF / 2; ++i) acc[i] = 0.f;
     int stage = 0; uint32_t phase = 0;
     for (int tile = tile_begin; tile < tile_end; ++tile) {
-        for (int kc = 0; kc < kTcKCh; ++kc) {
-            if (!mbar_wait(&b_full[stage], phase, err_flag)) return;
-            const uint32_t ah = smem_u32(sA + (size_t)kc * kTcABytes) + a_row_off;
-            const uint32_t al = smem_u32(sR + (size_t)stage * kTcStageBytes) + a_row_off;
-            const uint32_t bh = smem_u32(sR + (size_t)stage * kTcStageBytes) + kTcABytes, bl = bh + kTcBBytes;
-            wgmma_fence();
+        int held = 0;                                                 // ring stage read by the wgmma group in flight
 #pragma unroll
-            for (int k = 0; k < kTcBK / 8; ++k) {                  // hi*hi, then the two correction products
-                wgmma_m64n96k8_tf32(acc, wgmma_desc_k_sw128(ah + k * 32), wgmma_desc_k_sw128(bh + k * 32), (kc | k) ? 1u : 0u);
-                wgmma_m64n96k8_tf32(acc, wgmma_desc_k_sw128(al + k * 32), wgmma_desc_k_sw128(bh + k * 32), 1u);
-                wgmma_m64n96k8_tf32(acc, wgmma_desc_k_sw128(ah + k * 32), wgmma_desc_k_sw128(bl + k * 32), 1u);
+        for (int kc = 0; kc < kTcKCh; ++kc) {
+            // a timeout raises the error flag (the host reports it) and the warpgroup carries on: leaving the loop here
+            // would be a divergent exit with a wgmma group in flight, which makes ptxas serialise every group
+            mbar_wait(&full[stage], phase, err_flag);
+            if (kc == 0 && tile == tile_begin && wt == 0) TC_MARK(2);
+            const unsigned char* sP = sR + (size_t)stage * kStageBytes;
+            const uint32_t bh = smem_u32(sP + kTcPBytes), bl = bh + kFBytes;
+#pragma unroll
+            for (int k = 0; k < kTcBK / 8; ++k) {
+                // A fragment of the k8 step, split x = hi + lo (tf32_split: round to nearest, ties away, as the host-side
+                // split of the earlier pre-split copy did); columns k >= 207 hold shape blend shapes and the template in
+                // Qk and enter as zero
+                uint32_t ahi[4], alo[4];
+#pragma unroll
+                for (int v = 0; v < 4; ++v) {
+                    const int r = frow + 8 * (v & 1), c16 = 2 * k + (v >> 1);        // row, logical 16-byte column group
+                    float x = *reinterpret_cast<const float*>(sP + r * 128 + ((c16 ^ xr) << 4) + 4 * q);
+                    if (kc * kTcBK + 4 * c16 + q >= kPoseBasis) x = 0.f;
+                    float hi, lo;
+                    tf32_split(x, hi, lo);
+                    ahi[v] = __float_as_uint(hi);
+                    alo[v] = __float_as_uint(lo);
+                }
+                wgmma_fence();                                            // hi*hi, then the two correction products
+                WgmmaTf32Rs<NF>::mma(acc, ahi, wgmma_desc_k_sw128(bh + k * 32), (kc | k) ? 1u : 0u);
+                WgmmaTf32Rs<NF>::mma(acc, ahi, wgmma_desc_k_sw128(bl + k * 32), 1u);
+                WgmmaTf32Rs<NF>::mma(acc, alo, wgmma_desc_k_sw128(bh + k * 32), 1u);
+                wgmma_commit();
+                // one group in flight while the next fragment is split; once the first group of this chunk is issued,
+                // every group of the previous chunk has retired and its ring stage goes back to the producer
+                wgmma_wait1();
+                if (k == 0 && kc > 0) mbar_arrive_if(&empty[held], wt == 0);
             }
-            wgmma_commit();
-            wgmma_wait0();
-            if (wt == 0) mbar_arrive(&b_empty[stage]);              // this warpgroup's MMAs on the stage have retired
+            held = stage;
             if (++stage == kTcStages) { stage = 0; phase ^= 1; }
         }
+        wgmma_wait0();
+        mbar_arrive_if(&empty[held], wt == 0);
         if (wt == 0) TC_MARK(3 + (tile - tile_begin));
-        // The tile leaves through shared memory and the TMA store engine, 32 columns ([column][frame] rows of 256 B) at a
-        // time: the warpgroup fills its staging tile, one thread issues the bulk tensor store, which clips the box at the
-        // array bounds (last vertex tile, frame padding).  Rows of slots that are not active hold whatever the accumulator
-        // held: nobody reads them.
-        const int c0 = tile * kTcBN;
+        // d[4 i + 2 h + j] = poffT[row tile + frow + 8 h][f0 + 8 i + 2 q + j]: 32-byte row segments per quad.  Slots past
+        // the active count are not stored (ldA is a multiple of 64, so a pair that starts below na stays inside the row).
 #pragma unroll
-        for (int ch = 0; ch < kTcBN / kTcEpiCols; ++ch) {          // unrolled: acc[] stays in registers
-            if (c0 + ch * kTcEpiCols >= ncols) break;
-            if (wt == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // staging tile free again
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
+        for (int h = 0; h < 2; ++h) {
+            const int row = tile * kTcRows + frow + 8 * h;
+            if (row >= nrows) continue;
+            float* dst = poffT + (size_t)row * ldA + f0 + 2 * q;
 #pragma unroll
-            for (int i = 0; i < kTcEpiCols / 8; ++i)
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-#pragma unroll
-                    for (int j = 0; j < 2; ++j)
-                        sOw[(8 * i + colq + j) * kTcWgM + row + 8 * h] = acc[4 * (ch * kTcEpiCols / 8 + i) + 2 * h + j];
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
-            if (wt == 0) tma_store_2d(&map_o, sOw, m0 + g * kTcWgM, c0 + ch * kTcEpiCols);
+            for (int i = 0; i < NF / 8; ++i)
+                if (f0 + 8 * i + 2 * q < na) *reinterpret_cast<float2*>(dst + 8 * i) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
         }
     }
-    if (wt == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");         // all stores of this warpgroup have landed
-    if (threadIdx.x == 128) TC_MARK(20);
+    if (threadIdx.x == 0) TC_MARK(20);
 }
 
 __global__ void __launch_bounds__(kSkinThreads)
@@ -198,23 +184,16 @@ skin_small_kernel(SkinArgs ar, const int* __restrict__ na_ptr) {
 }
 
 // ------------------------------------------------------------------------------------------------ host side
+constexpr int kTcInstances[] = {8, 16, 32, 64, 128};       // wgmma N instances of posedirs_gemm_tc_kernel
+constexpr int kTcNumInst = 5;
+
 struct TcState {
-    CUtensorMap map_a, map_a8, map_b, map_o;
-    float* Qtc = nullptr;       // [2][3N][224] posedirs rows split into TF32 hi | lo parts (columns >= 207 zero)
-    float* poffT = nullptr;     // [3N][ldA] pose offsets, frame fastest (output of the tensor-core contraction)
+    CUtensorMap map_p;              // fp32 posedirs: the model's Qk rows [3N][224], box 128 rows x 32
+    CUtensorMap map_f[kTcNumInst];  // PhiTc [2][ldA][224] (hi rows, then lo rows), box kTcInstances[i] rows x 32
+    float* poffT = nullptr;         // [3N][ldA] pose offsets, frame fastest (output of the tensor-core contraction)
     int* err = nullptr;
     bool ready = false;
 };
-
-static float round_tf32(float x) {                      // cvt.rna.tf32.f32: nearest, ties away from zero
-    uint32_t u;
-    memcpy(&u, &x, 4);
-    if ((u & 0x7F800000u) == 0x7F800000u) return x;
-    u = (u + 0x1000u) & 0xFFFFE000u;
-    float r;
-    memcpy(&r, &u, 4);
-    return r;
-}
 
 static int encode_map(mvs_ctx* ctx, CUtensorMap* map, const float* ptr, uint64_t rows, uint32_t box_rows) {
     static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
@@ -236,37 +215,11 @@ static int encode_map(mvs_ctx* ctx, CUtensorMap* map, const float* ptr, uint64_t
     return MVS_OK;
 }
 
-// output of the contraction: poffT [ncols][ldA] fp32, frame fastest; box = 64 frames x kTcEpiCols columns, no swizzle
-static int encode_out_map(mvs_ctx* ctx, CUtensorMap* map, float* ptr, uint64_t ldA, uint64_t ncols) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || !p)
-        return set_error(ctx, MVS_ERR_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
-    auto fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(p);
-    cuuint64_t dims[2] = {(cuuint64_t)ldA, (cuuint64_t)ncols};
-    cuuint64_t strides[1] = {(cuuint64_t)ldA * sizeof(float)};
-    cuuint32_t box[2] = {(cuuint32_t)kTcWgM, (cuuint32_t)kTcEpiCols};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(ctx, MVS_ERR_CUDA, "cuTensorMapEncodeTiled (output) failed (%d)", (int)r);
-    return MVS_OK;
-}
-
-// posedirs copy for the tensor path (called from mvs_set_model with the host Qk rows)
-int tc_upload_model(mvs_ctx* ctx, const float* Qk_host) {
+// state of the tensor path (called from mvs_set_model once the Qk rows are on the device: the kernel reads them directly)
+int tc_upload_model(mvs_ctx* ctx) {
     TcState* T = new TcState();
     ctx->tc = T;
-    const size_t n = (size_t)3 * ctx->m.N * kFeatPad;
-    std::vector<float> q(2 * n);                 // hi rows, then lo rows: posedirs = hi + lo, both TF32 (hi - x is exact in fp32)
-    for (size_t i = 0; i < n; ++i) {
-        const bool pose = (i % kFeatPad) < (size_t)kPoseBasis;
-        const float hi = pose ? round_tf32(Qk_host[i]) : 0.f;
-        q[i] = hi;
-        q[n + i] = pose ? round_tf32(Qk_host[i] - hi) : 0.f;
-    }
-    int rc = dev_upload(ctx, &T->Qtc, q.data(), 2 * n);
-    if (rc) return rc;
+    int rc;
     if ((rc = dev_alloc(ctx, &T->err, 1))) return rc;
     MVS_CUDA_OK(ctx, cudaMemset(T->err, 0, sizeof(int)));
     return MVS_OK;
@@ -276,6 +229,12 @@ bool tc_available(const mvs_ctx* ctx) {
     return ctx->exec_mode != 1 && ctx->tc != nullptr && ctx->ws.PhiTc != nullptr;
 }
 
+template <int NF>
+static int tc_set_smem(mvs_ctx* ctx) {
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<NF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(NF)));
+    return MVS_OK;
+}
+
 int tc_prepare(mvs_ctx* ctx) {
     TcState* T = static_cast<TcState*>(ctx->tc);
     Workspace& w = ctx->ws;
@@ -283,12 +242,13 @@ int tc_prepare(mvs_ctx* ctx) {
     if (!T) return set_error(ctx, MVS_ERR_INVALID, "tensor-core path not initialised (mvs_set_model)");
     if (!T->ready) {
         int rc;
-        if ((rc = encode_map(ctx, &T->map_a, w.PhiTc, (uint64_t)2 * w.ldA, kTcBM))) return rc;       // hi rows, then lo rows
-        if ((rc = encode_map(ctx, &T->map_a8, w.PhiTc, (uint64_t)2 * w.ldA, 8))) return rc;
-        if ((rc = encode_map(ctx, &T->map_b, T->Qtc, (uint64_t)2 * 3 * m.N, kTcBN))) return rc;
+        if ((rc = encode_map(ctx, &T->map_p, m.Qk, (uint64_t)3 * m.N, kTcRows))) return rc;
+        for (int i = 0; i < kTcNumInst; ++i)                                                       // hi rows, then lo rows
+            if ((rc = encode_map(ctx, &T->map_f[i], w.PhiTc, (uint64_t)2 * w.ldA, kTcInstances[i]))) return rc;
         if ((rc = dev_alloc(ctx, &T->poffT, (size_t)3 * m.N * w.ldA))) return rc;
-        if ((rc = encode_out_map(ctx, &T->map_o, T->poffT, (uint64_t)w.ldA, (uint64_t)3 * m.N))) return rc;
-        MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem));
+        if ((rc = tc_set_smem<8>(ctx)) || (rc = tc_set_smem<16>(ctx)) || (rc = tc_set_smem<32>(ctx)) || (rc = tc_set_smem<64>(ctx)) ||
+            (rc = tc_set_smem<128>(ctx)))
+            return rc;
         MVS_CUDA_OK(ctx, cudaFuncSetAttribute(skin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSkinSmem));
         T->ready = true;
     }
@@ -301,25 +261,30 @@ float* tc_poffT(mvs_ctx* ctx) {
     return T->poffT;
 }
 
-const void* tc_maps(mvs_ctx* ctx) {            // [map_a, map_a8, map_b] (CUtensorMap x 3) for the persistent dense-round kernel
-    TcState* T = static_cast<TcState*>(ctx->tc);
-    if (!T || tc_prepare(ctx) != MVS_OK) return nullptr;
-    return &T->map_a;
-}
 int* tc_err_flag(mvs_ctx* ctx) { TcState* T = static_cast<TcState*>(ctx->tc); return T ? T->err : nullptr; }
+
+template <int NF>
+static cudaError_t launch_gemm(mvs_ctx* ctx, const TcState* T, int inst, dim3 grid, cudaStream_t st, int ntiles) {
+    const Workspace& w = ctx->ws;
+    return launch_pdl(posedirs_gemm_tc_kernel<NF>, grid, dim3(kTcThreads), tc_smem(NF), st, T->map_p, T->map_f[inst], w.ldA,
+                      3 * ctx->m.N, (const int*)w.na, ctx->sm_count, ntiles, T->poffT, T->err);
+}
 
 int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed) {
     TcState* T = static_cast<TcState*>(ctx->tc);
     Workspace& w = ctx->ws;
     const DevModel& m = ctx->m;
     { const int rc = tc_prepare(ctx); if (rc) return rc; }
-    const int ntiles = (m.N + kTileV - 1) / kTileV;
     const int nb = w.na_bound > 0 ? w.na_bound : w.B;             // upper bound of the active-frame count
-    const int mtiles = (nb + kTcBM - 1) / kTcBM;
-    dim3 grid(std::min(ctx->sm_count, ntiles), mtiles);          // surplus CTAs exit: the kernel splits the tiles from *na
+    const int ntiles = (3 * m.N + kTcRows - 1) / kTcRows;
+    const int nf = tc_cols_for(nb);
+    dim3 grid(std::min(ctx->sm_count, ntiles), (nb + kTcCols - 1) / kTcCols);   // surplus CTAs exit: the kernel splits the tiles from *na
     MVS_LAUNCH(ctx, KID_VERTEX_FWD_TC, st,
-               MVS_CUDA_OK(ctx, launch_pdl(posedirs_gemm_tc_kernel, grid, dim3(kTcThreads), kTcSmem, st, T->map_a, T->map_a8, T->map_b, T->map_o, w.ldA,
-                                           3 * m.N, (const int*)w.na, ctx->sm_count, ntiles, T->poffT, T->err)));
+               MVS_CUDA_OK(ctx, nf == 8    ? launch_gemm<8>(ctx, T, 0, grid, st, ntiles)
+                                : nf == 16 ? launch_gemm<16>(ctx, T, 1, grid, st, ntiles)
+                                : nf == 32 ? launch_gemm<32>(ctx, T, 2, grid, st, ntiles)
+                                : nf == 64 ? launch_gemm<64>(ctx, T, 3, grid, st, ntiles)
+                                           : launch_gemm<128>(ctx, T, 4, grid, st, ntiles)));
     const int nchunks = (m.N + kSkinV - 1) / kSkinV, fgroups = (nb + 31) / 32;
     const SkinArgs sa{T->poffT, m.ST, w.Phi, w.At, w.ldA, m.ell_j, m.ell_w, m.KW, m.N, need_vposed ? w.vposed : nullptr, w.verts, w.bboxp};
     if (nb <= kSkinSmallMax) {                          // straggler tail: lane = vertex, one chunk per CTA

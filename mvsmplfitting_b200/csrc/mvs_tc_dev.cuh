@@ -7,19 +7,22 @@
 
 namespace mvs {
 
-constexpr int kTcBM = 128;            // frames per CTA: two consumer warpgroups of 64 rows (wgmma M = 64)
-constexpr int kTcWgM = 64;            // frames per consumer warpgroup
-constexpr int kTcBN = kTileC;         // 96 columns = 32 vertices (wgmma N)
+// Tiles of posedirs_gemm_tc_kernel.  The contraction runs transposed, poffT = Qk[:, :207] . Phi^T: the 3N posedirs rows
+// are the wgmma M side (64 rows per consumer warpgroup, 128 per CTA tile) and the active frames the N side, so the
+// accumulator fragment is already [coordinate][frame], the layout of poffT.
+constexpr int kTcRows = 128;          // posedirs rows per CTA tile: two consumer warpgroups of 64 rows (wgmma M = 64)
+constexpr int kTcWgRows = 64;         // posedirs rows per consumer warpgroup
+constexpr int kTcCols = 128;          // frames per column tile (largest wgmma N instance used); larger batches run several
 constexpr int kTcBK = 32;             // floats per 128-byte swizzle row
 constexpr int kTcKCh = kFeatPad / kTcBK;   // 7 K chunks
-constexpr int kTcStages = 2;             // ring stages of (A lo chunk | B hi chunk | B lo chunk)
-constexpr int kTcABytes = kTcBM * kTcBK * 4;   // 16 KB
-constexpr int kTcBBytes = kTcBN * kTcBK * 4;   // 12 KB
-constexpr int kTcThreads = 384;       // warpgroup 0: TMA producer; warpgroups 1, 2: wgmma + epilogue, 64 frames each
-constexpr int kTcStageBytes = kTcABytes + 2 * kTcBBytes;     // 40 KB
-constexpr int kTcEpiCols = 32;                                 // pose-offset columns per TMA store of the epilogue
-constexpr int kTcEpiBytes = kTcEpiCols * kTcBM * 4;            // 16 KB: one 8 KB staging tile [column][64 frames] per warpgroup
-constexpr size_t kTcSmem = 1024 /*align slack*/ + (size_t)kTcKCh * kTcABytes + (size_t)kTcStages * kTcStageBytes + kTcEpiBytes + 256;
+constexpr int kTcStages = 4;          // ring stages of (posedirs chunk | feature hi chunk | feature lo chunk)
+constexpr int kTcPBytes = kTcRows * kTcBK * 4;     // 16 KB fp32 posedirs per stage (split into TF32 hi | lo on chip)
+constexpr int kTcThreads = 288;       // warpgroups 0, 1: convert + wgmma + store, 64 rows each; warp 8: TMA producer
+// frame columns of one launch (wgmma N): the active-frame bound rounded up to 8, 16, 32, 64 or 128
+__host__ __device__ constexpr int tc_cols_for(int nb) { return nb <= 8 ? 8 : nb <= 16 ? 16 : nb <= 32 ? 32 : nb <= 64 ? 64 : 128; }
+__host__ __device__ constexpr int tc_fbytes(int nf) { return nf * kTcBK * 4; }            // one feature chunk (hi or lo): nf rows of 128 B
+__host__ __device__ constexpr int tc_stage_bytes(int nf) { return kTcPBytes + 2 * tc_fbytes(nf); }
+__host__ __device__ constexpr size_t tc_smem(int nf) { return 1024 /*align slack*/ + (size_t)kTcStages * tc_stage_bytes(nf) + 256 /*barriers*/; }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -31,6 +34,11 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// arrive if `pred`, as a predicated instruction rather than a branch (no divergent path between in-flight wgmma groups)
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
+                 ::"r"(smem_u32(bar)), "r"((uint32_t)pred) : "memory");
 }
 // bounded spin: a protocol bug must not hang the GPU -- after ~2 s the kernel raises the error flag and carries on
 __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, int* err_flag) {
@@ -71,25 +79,93 @@ __device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// D[64 x 96] (+)= A[64 x 8] . B[96 x 8]^T, tf32 inputs (both K-major in shared memory), fp32 accumulators in registers:
-// with w = t / 32 and l = t % 32 for thread t of the warpgroup, d[4 i + 2 h + j] = D[16 w + l / 4 + 8 h][8 i + 2 (l % 4) + j]
-__device__ __forceinline__ void wgmma_m64n96k8_tf32(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %50, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
-        "%48, %49, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
-          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
-          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
-          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
-          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-        : "l"(adesc), "l"(bdesc), "r"(accumulate)
-        : "memory");
-}
+__device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// D[64 x N] (+)= A[64 x 8] . B[N x 8]^T, tf32: A from registers, B K-major in shared memory, fp32 accumulators in registers.
+// For thread t of the warpgroup with w = t / 32, l = t % 32, g = l / 4, q = l % 4:
+//   a[0] = A[16 w + g][q], a[1] = A[16 w + g + 8][q], a[2] = A[16 w + g][q + 4], a[3] = A[16 w + g + 8][q + 4]
+//   d[4 i + 2 h + j] = D[16 w + g + 8 h][8 i + 2 q + j]
+template <int N> struct WgmmaTf32Rs;
+template <> struct WgmmaTf32Rs<8> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %9, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n8k8.f32.tf32.tf32 "
+            "{%0, %1, %2, %3}, "
+            "{%4, %5, %6, %7}, %8, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate)
+            : "memory");
+    }
+};
+template <> struct WgmmaTf32Rs<16> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %13, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+            "{%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate)
+            : "memory");
+    }
+};
+template <> struct WgmmaTf32Rs<32> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %21, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+            "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate)
+            : "memory");
+    }
+};
+template <> struct WgmmaTf32Rs<64> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %37, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+            "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate)
+            : "memory");
+    }
+};
+template <> struct WgmmaTf32Rs<128> {
+    static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %69, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+            "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+            "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+            "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate)
+            : "memory");
+    }
+};
+
 
 // One vertex of one frame: v_posed = template + shapedirs.betas + pose offset, then linear blend skinning
 // (lbs.py:179,203,207-220).  skin_kernel (lane = frame) and skin_small_kernel (lane = vertex) both call this with every

@@ -47,7 +47,7 @@ print("longest two-loop recursion: %.2f us with %d history pairs" % (buf[40] / g
 tb = (ctypes.c_longlong * 32)()
 if hasattr(lib, "mvs_debug_tc_clocks") and lib.mvs_debug_tc_clocks(tb, 32) == 0 and tb[0]:
     def us(i): return (tb[i] - tb[0]) / ghz / 1e3
-    print("posedirs_gemm_tc CTA(0,0), us from kernel entry: setup done %.2f | A operand landed %.2f | MMA tile commits %s | "
+    print("posedirs_gemm_tc CTA(0,0), us from kernel entry: setup done %.2f | first ring stage landed %.2f | row tiles done %s | "
           "epilogue (tile ready, stored) %s | exit %.2f" % (
               us(1), us(2), ["%.2f" % us(3 + i) for i in range(4) if tb[3 + i] > tb[0]],
               ["%.2f/%.2f" % (us(8 + 2 * i), us(9 + 2 * i)) for i in range(4) if tb[8 + 2 * i] > tb[0]], us(20)))
