@@ -197,8 +197,10 @@ frame_fwd_resident_kernel(ResidentModel m, const LossParams* __restrict__ lp_tab
 // One round of the dense regime for one frame (multi-kernel path): see frame_step_body.
 __global__ void __launch_bounds__(kResThreads, 2)
 frame_step_kernel(FrameStepArgs a, const int* __restrict__ fidx, const int* __restrict__ na_ptr) {
-    pdl_wait();
     extern __shared__ __align__(16) unsigned char smem_raw[];
+    // the model tables are constants of the run: staged while the previous kernel of the round drains
+    resident_setup(*reinterpret_cast<ResidentSmem*>(smem_raw), a.m);
+    pdl_wait();
     const int slot = blockIdx.x;
     if (slot >= *na_ptr) return;
     frame_step_body(smem_raw, a, slot, fidx[slot]);
@@ -216,6 +218,7 @@ static ResidentModel make_resident_model(const mvs_ctx* ctx) {
     ResidentModel r;
     r.Qk = m.Qk; r.Jt = m.Jt; r.JS = m.JS; r.ell_j = m.ell_j; r.ell_w = m.ell_w; r.KW = m.KW;
     r.K = m.K; r.nsup = m.nsup; r.kp_ptr = m.kp_ptr; r.kp_spos = m.kp_spos; r.kp_w = m.kp_w; r.kp_chain = m.kp_chain;
+    r.nkpe = m.n_kp_entries;
     r.sup = m.sup; r.sup_ptr = m.sup_ptr; r.sup_k = m.sup_k; r.sup_w = m.sup_w;
     r.supj_ptr = m.supj_ptr; r.supj_i = m.supj_i; r.supj_w = m.supj_w;
     r.M = m.M; r.gmm_means = m.gmm_means; r.gmm_prec = m.gmm_prec; r.gmm_lognllw = m.gmm_lognllw;

@@ -18,6 +18,49 @@ constexpr int kResMaxSup = 96;            // support vertices (SMPL: 86)
 constexpr int kResMaxSupJ = 512;          // (support vertex, joint) pairs with a non-zero skinning weight (SMPL: <= 344)
 constexpr int kResMaxVK = 272;            // views x keypoints (16 x 17)
 constexpr int kResMaxM = 8;               // GMM components
+constexpr int kResMaxKpE = 256;           // (keypoint, support vertex) entries staged in shared memory
+// resident_closure splits the CTA from P4 to P10: warps 0-5 run the data term and its adjoint, warps 6-7 the part of the
+// priors that only needs the pose (GMM mat-vec and log-likelihoods, |theta|^2).  Each group syncs on its own named barrier;
+// warp 6 then joins the data warps for P8.
+constexpr int kDataThreads = 192;
+constexpr int kPriorThreads = kResThreads - kDataThreads;
+
+__device__ __forceinline__ void bar_sync_n(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void data_sync() { bar_sync_n(1, kDataThreads); }
+__device__ __forceinline__ void prior_sync() { bar_sync_n(2, kPriorThreads); }
+// P8 (dPhi, kFeatPad columns) runs on the data warps and warp 6
+constexpr int kP8Threads = kDataThreads + 32;
+static_assert(kFeatPad == kP8Threads, "one P8 column per thread");
+__device__ __forceinline__ void p8_sync() { bar_sync_n(3, kP8Threads); }
+
+__device__ __forceinline__ void cp_async4(float* dst, const float* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async8(float* dst, const float* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async16(float* dst, const float* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait_group() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// sum_{q < n} v(q) in ascending q -- the order of `for (q) a += v(q)` -- with eight loads in flight instead of one
+template <class F>
+__device__ __forceinline__ float serial_sum8(int n, F v) {
+    float a = 0.f;
+    for (int q0 = 0; q0 < n; q0 += 8) {
+        float r[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) r[u] = q0 + u < n ? v(q0 + u) : 0.f;
+#pragma unroll
+        for (int u = 0; u < 8; ++u)
+            if (q0 + u < n) a += r[u];
+    }
+    return a;
+}
 
 // Depth-level schedule of the kinematic tree: joints of one level only depend on the level above (forward) / below
 // (adjoint), so a level is processed by parallel lane groups and the 23-step serial chain becomes <= 9 level steps
@@ -33,7 +76,7 @@ struct ResidentModel {                    // device pointers + sizes, by value
     const float* Qk; const float* Jt; const float* JS;
     const int* ell_j; const float* ell_w; int KW;
     int K, nsup;
-    const int* kp_ptr; const int* kp_spos; const float* kp_w; const int* kp_chain;
+    const int* kp_ptr; const int* kp_spos; const float* kp_w; const int* kp_chain; int nkpe;
     const int* sup; const int* sup_ptr; const int* sup_k; const float* sup_w;
     const int* supj_ptr; const int* supj_i; const float* supj_w;      // per joint: (support index, weight)
     int M; const float* gmm_means; const float* gmm_prec; const float* gmm_lognllw;
@@ -68,6 +111,11 @@ struct ResidentSmem {
     // per joint: the support vertices it skins (copy of supj_*: the dA loop of P7 is a chain of dependent list reads)
     int sj_ptr[kJoints + 1], sj_i[kResMaxSupJ], sj_on;
     float sj_w[kResMaxSupJ];
+    // keypoint regressor over the support vertices and its transpose (copies of kp_* / sup_*: P6 would otherwise walk
+    // chains of dependent list reads from L2); the entry lists only when they fit (kp_on)
+    int sup[kResMaxSup], kp_ptr[kMaxKeypoints + 1], kp_chain[kMaxKeypoints], sup_ptr[kResMaxSup + 1], kp_on;
+    int kp_spos[kResMaxKpE], sup_k[kResMaxKpE];
+    float kp_w[kResMaxKpE], sup_w[kResMaxKpE];
     // dense regime: frame scalars of the SDF term and its box-extreme vertex list (frame_step_kernel)
     int ext_n[8];
     float ext_d[24];
@@ -140,6 +188,7 @@ __device__ __forceinline__ void chain_fwd_levels(ResidentSmem& S) {
 //   role C (threads 128..157)  drel_j = Gam_p^T dg_j;  dJ_j += drel_j, dJ_p -= sum_j drel_j     3 lanes per parent
 //   role D (threads 160..189)  dg_p += sum_j dg_j                                3 lanes per parent
 // Children are gathered in descending index order = the summation order of the plain j = 23..1 sweep.
+// The kDataThreads data-term threads call; ends with their barrier.
 __device__ __forceinline__ void chain_bwd_levels(ResidentSmem& S) {
     const int t = threadIdx.x;
     for (int L = S.nlev - 2; L >= 0; --L) {
@@ -197,7 +246,7 @@ __device__ __forceinline__ void chain_bwd_levels(ResidentSmem& S) {
                 S.dg[3 * p + r] = acc;
             }
         }
-        __syncthreads();
+        data_sync();
     }
 }
 
@@ -303,6 +352,34 @@ static __device__ void vposer_decode_bwd(const ResidentModel& m, VposerSmem& W) 
     __syncthreads();
 }
 
+// P8 of the closure for feature column k: dPhi[k] = sum_col dvp[col] Qk[row(col)][k] in ascending col, then the
+// penetration partials.  32 independent L2 loads in flight: the phase is as long as its round trips to L2 (258 rows: 8
+// instead of 21).
+__device__ __forceinline__ void dphi_col(ResidentSmem& S, const ResidentModel& m, const DenseIn& din, int ncol_all, int k) {
+    float a = 0.f;
+    int col = 0;
+    for (; col + 32 <= ncol_all; col += 32) {
+        float qv[32];
+#pragma unroll
+        for (int u = 0; u < 32; ++u) qv[u] = __ldg(m.Qk + (size_t)S.rowbase[col + u] * kFeatPad + k);
+#pragma unroll
+        for (int u = 0; u < 32; ++u) a = fmaf(S.dvp[col + u], qv[u], a);
+    }
+    for (; col + 8 <= ncol_all; col += 8) {
+        float qv[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) qv[u] = __ldg(m.Qk + (size_t)S.rowbase[col + u] * kFeatPad + k);
+#pragma unroll
+        for (int u = 0; u < 8; ++u) a = fmaf(S.dvp[col + u], qv[u], a);
+    }
+    for (; col < ncol_all; ++col) a = fmaf(S.dvp[col], __ldg(m.Qk + (size_t)S.rowbase[col] * kFeatPad + k), a);
+    if (din.part) {
+        const float pa = serial_sum8(din.nfl, [&](int q) { return din.part[(size_t)din.fl[q] * kPartFloats + kSkinFloats + k]; });
+        a = fmaf(pa, din.factor, a);
+    }
+    S.dPhi[k] = a;
+}
+
 // ------------------------------------------------------------------------------------------------
 // One closure evaluation at S.x (already loaded).  Writes S.sc[2] = total loss and S.lg_new = gradient
 // (frozen segments zeroed).  All kResThreads threads must call it.
@@ -317,6 +394,11 @@ static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m,
     const bool vp2 = (lp.use_vposer == 2) && W != nullptr;
     if (vp2) vposer_decode(S, m, *W);
     const float* theta = vp2 ? W->th : &S.x[kOffPose];          // the 69 body-pose entries the model sees
+    const bool kp_sm = S.kp_on != 0;
+    const int* kp_spos = kp_sm ? S.kp_spos : m.kp_spos;
+    const float* kp_w = kp_sm ? S.kp_w : m.kp_w;
+    const int* sup_k = kp_sm ? S.sup_k : m.sup_k;
+    const float* sup_w = kp_sm ? S.sup_w : m.sup_w;
 
     // ---- P1 Rodrigues, rest joints (skipped when the caller restored them: the previous frame_step computed the pose
     //      forward of exactly this trial point for the dense kernels and parked it in the per-frame pose cache)
@@ -352,304 +434,291 @@ static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m,
         __syncthreads();
     }
     PHASE_MARK(4);
-    // ---- P4 v_posed for the support columns: warp per Qk row, 2 x LDG.128 per lane
-    if (din.verts) {                  // dense regime: the vertex kernels already have them (v_posed: bit for bit skin_vertex's)
-        for (int col = t; col < ncol; col += kResThreads) {
-            const int n = m.sup[col / 3], c = col % 3;
-            S.vp[col] = vposed_of(din.ST + (size_t)n * 33 + 11 * c, &S.x[kOffBetas], din.poffT[(size_t)(3 * n + c) * din.ldA + din.slot]);
-            S.v[col] = din.verts[3 * n + c];
+    if (t >= kDataThreads) {
+        const int M = m.M;
+        const bool gmm = !lp.use_vposer && lp.body_prior == MVS_PRIOR_GMM;
+        // ---- P11a priors (fitting.py:327-350) that need only the pose: GMM components and |theta|^2, on warps 6-7 while
+        //      warps 0-5 run P4-P10.  Same expressions and orders as one phase per barrier on all warps.
+        const int pt = t - kDataThreads;
+        if (gmm)
+            for (int e = pt; e < M * 69; e += kPriorThreads) S.gm_diff[e] = theta[e % 69] - m.gmm_means[e];
+        for (int i = pt; i < 69; i += kPriorThreads)
+            S.red[i] = vp2 ? ((i < kVpZ) ? S.x[kOffPose + i] * S.x[kOffPose + i] : 0.f) : theta[i] * theta[i];  // |z|^2 (fitting.py:327-329)
+        prior_sync();
+        if (gmm) {
+            for (int e = pt; e < M * 69; e += kPriorThreads) {
+                const int mm = e / 69, i = e % 69;
+                const float* P = m.gmm_prec + (size_t)mm * 69 * 69 + i;
+                const float* df = &S.gm_diff[mm * 69];
+                float y = 0.f;
+#pragma unroll
+                for (int j = 0; j < 69; ++j) y = fmaf(__ldg(P + j * 69), df[j], y);       // all 69 loads of the row in flight
+                S.gm_y[e] = y;
+            }
         }
-        // the box-extreme vertices of the penetration term ride along as support entries nsup .. nsup + n_extra - 1
-        if (t < 3 * din.n_extra) {
-            const int n = din.extra_n[t / 3], c = t % 3;
-            S.vp[ncol + t] = vposed_of(din.ST + (size_t)n * 33 + 11 * c, &S.x[kOffBetas], din.poffT[(size_t)(3 * n + c) * din.ldA + din.slot]);
-            S.dv[ncol + t] = din.extra_d[t];
-            S.rowbase[ncol + t] = 3 * n + c;
+        if (pt == 0) { float a = 0.f; for (int i = 0; i < 69; ++i) a += S.red[i]; S.sc[1] = a; }
+        prior_sync();
+        if (gmm) {
+            for (int mm = warp - kDataThreads / 32; mm < M; mm += kPriorThreads / 32) {
+                float p = 0.f;
+                for (int i = lane; i < 69; i += 32) p = fmaf(S.gm_y[mm * 69 + i], S.gm_diff[mm * 69 + i], p);
+                p = warp_sum(p);
+                if (lane == 0) S.gm_ll[mm] = 0.5f * p - m.gmm_lognllw[mm];
+            }
+        }
+        if (have_grad && warp == kDataThreads / 32) {    // P8 for the feature columns 192 .. 223, between the data warps' barriers
+            p8_sync();
+            dphi_col(S, m, din, ncol + 3 * din.n_extra, kDataThreads + lane);
+            p8_sync();
         }
     } else {
-        // warp per Qk row (896 B = 2 x LDG.128 per lane), FOUR rows in flight per warp: the 231 KB slice comes from L2
-        // and the phase is pure latency, so the depth of the load queue is what sets its length
-        const float4 ph0 = *reinterpret_cast<const float4*>(&S.Phi[4 * lane]);
-        const float4 ph1 = lane < 24 ? *reinterpret_cast<const float4*>(&S.Phi[128 + 4 * lane]) : make_float4(0.f, 0.f, 0.f, 0.f);
-        constexpr int kW = kResThreads / 32;
-        for (int col0 = warp; col0 < ncol; col0 += 4 * kW) {
-            float4 a[4], bq[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const int col = col0 + u * kW;
-                const float* r = m.Qk + (size_t)S.rowbase[col < ncol ? col : col0] * kFeatPad;
-                a[u] = __ldg(reinterpret_cast<const float4*>(r + 4 * lane));
-                bq[u] = lane < 24 ? __ldg(reinterpret_cast<const float4*>(r + 128 + 4 * lane)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        // ---- P4 v_posed for the support columns
+        if (din.verts) {                  // dense regime: the vertex kernels already have them (v_posed: bit for bit skin_vertex's)
+            for (int col = t; col < ncol; col += kDataThreads) {
+                const int n = S.sup[col / 3], c = col % 3;
+                S.vp[col] = vposed_of(din.ST + (size_t)n * 33 + 11 * c, &S.x[kOffBetas], din.poffT[(size_t)(3 * n + c) * din.ldA + din.slot]);
+                S.v[col] = din.verts[3 * n + c];
             }
+            // the box-extreme vertices of the penetration term ride along as support entries nsup .. nsup + n_extra - 1
+            if (t < 3 * din.n_extra) {
+                const int n = din.extra_n[t / 3], c = t % 3;
+                S.vp[ncol + t] = vposed_of(din.ST + (size_t)n * 33 + 11 * c, &S.x[kOffBetas], din.poffT[(size_t)(3 * n + c) * din.ldA + din.slot]);
+                S.dv[ncol + t] = din.extra_d[t];
+                S.rowbase[ncol + t] = 3 * n + c;
+            }
+        } else {
+            // warp per Qk row (896 B = 2 x LDG.128 per lane), FOUR rows in flight per warp: the 231 KB slice comes from L2
+            // and the phase is pure latency, so the depth of the load queue is what sets its length
+            const float4 ph0 = *reinterpret_cast<const float4*>(&S.Phi[4 * lane]);
+            const float4 ph1 = lane < 24 ? *reinterpret_cast<const float4*>(&S.Phi[128 + 4 * lane]) : make_float4(0.f, 0.f, 0.f, 0.f);
+            constexpr int kW = kDataThreads / 32;
+            for (int col0 = warp; col0 < ncol; col0 += 4 * kW) {
+                float4 a[4], bq[4];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                float p = a[u].x * ph0.x;
-                p = fmaf(a[u].y, ph0.y, p); p = fmaf(a[u].z, ph0.z, p); p = fmaf(a[u].w, ph0.w, p);
-                p = fmaf(bq[u].x, ph1.x, p); p = fmaf(bq[u].y, ph1.y, p); p = fmaf(bq[u].z, ph1.z, p); p = fmaf(bq[u].w, ph1.w, p);
-                p = warp_sum(p);
-                const int col = col0 + u * kW;
-                if (lane == 0 && col < ncol) S.vp[col] = p;
+                for (int u = 0; u < 4; ++u) {
+                    const int col = col0 + u * kW;
+                    const float* r = m.Qk + (size_t)S.rowbase[col < ncol ? col : col0] * kFeatPad;
+                    a[u] = __ldg(reinterpret_cast<const float4*>(r + 4 * lane));
+                    bq[u] = lane < 24 ? __ldg(reinterpret_cast<const float4*>(r + 128 + 4 * lane)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                }
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    float p = a[u].x * ph0.x;
+                    p = fmaf(a[u].y, ph0.y, p); p = fmaf(a[u].z, ph0.z, p); p = fmaf(a[u].w, ph0.w, p);
+                    p = fmaf(bq[u].x, ph1.x, p); p = fmaf(bq[u].y, ph1.y, p); p = fmaf(bq[u].z, ph1.z, p); p = fmaf(bq[u].w, ph1.w, p);
+                    p = warp_sum(p);
+                    const int col = col0 + u * kW;
+                    if (lane == 0 && col < ncol) S.vp[col] = p;
+                }
             }
         }
-    }
-    __syncthreads();
-    PHASE_MARK(5);
-    // ---- P5 linear blend skinning of the support vertices
-    if (!din.verts && t < nsup) {
-        const int n = m.sup[t];
-        float T[12];
+        data_sync();
+        PHASE_MARK(5);
+        // ---- P5 linear blend skinning of the support vertices
+        if (!din.verts && t < nsup) {
+            const int n = S.sup[t];
+            float T[12];
 #pragma unroll
-        for (int c = 0; c < 12; ++c) T[c] = 0.f;
-        for (int e = 0; e < m.KW; ++e) {
-            const float w = m.ell_w[(size_t)n * m.KW + e];
-            if (w != 0.f) {
-                const float* Aj = &S.A[12 * m.ell_j[(size_t)n * m.KW + e]];
-#pragma unroll
-                for (int c = 0; c < 12; ++c) T[c] = fmaf(w, Aj[c], T[c]);
-            }
-        }
-        const float p0 = S.vp[3 * t], p1 = S.vp[3 * t + 1], p2 = S.vp[3 * t + 2];
-#pragma unroll
-        for (int r = 0; r < 3; ++r) S.v[3 * t + r] = T[4 * r] * p0 + T[4 * r + 1] * p1 + T[4 * r + 2] * p2 + T[4 * r + 3];
-    }
-    __syncthreads();
-    PHASE_MARK(6);
-    // ---- P6 keypoints, projection, GMoF data term and its adjoint down to the support vertices
-    if (t < K) {
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-        for (int e = m.kp_ptr[t]; e < m.kp_ptr[t + 1]; ++e) {
-            const int pos = m.kp_spos[e];
-            const float w = m.kp_w[e];
-            a0 = fmaf(w, S.v[3 * pos], a0); a1 = fmaf(w, S.v[3 * pos + 1], a1); a2 = fmaf(w, S.v[3 * pos + 2], a2);
-        }
-        const int cj = m.kp_chain[t];
-        if (cj >= 0) { a0 += S.g[3 * cj]; a1 += S.g[3 * cj + 1]; a2 += S.g[3 * cj + 2]; }
-        S.q[3 * t] = a0 + S.x[kOffTransl]; S.q[3 * t + 1] = a1 + S.x[kOffTransl + 1]; S.q[3 * t + 2] = a2 + S.x[kOffTransl + 2];
-        if (joints_out) {
-            joints_out[((size_t)b * K + t) * 3] = S.q[3 * t]; joints_out[((size_t)b * K + t) * 3 + 1] = S.q[3 * t + 1];
-            joints_out[((size_t)b * K + t) * 3 + 2] = S.q[3 * t + 2];
-        }
-    }
-    __syncthreads();
-    PHASE_MARK(7);
-    {
-        const float rho2 = lp.rho * lp.rho, dw2 = lp.data_weight * lp.data_weight;
-        for (int idx = t; idx < V * K; idx += kResThreads) {
-            const int v = idx / K, k = idx % K;
-            float xc[3], uv[2];
-            project_fwd(cams.cam[v], &S.q[3 * k], xc, uv);
-            const size_t o = ((size_t)v * B + b) * K + k;
-            if (proj_out) { proj_out[2 * o] = uv[0]; proj_out[2 * o + 1] = uv[1]; }
-            float w = joint_w[k];
-            if (lp.use_joints_conf) w *= conf[o];
-            const float w2 = w * w;
-            float d0, d1;
-            const float g0 = gmof(gt_uv[2 * o] - uv[0], rho2, &d0);
-            const float g1 = gmof(gt_uv[2 * o + 1] - uv[1], rho2, &d1);
-            S.lterm[idx] = w2 * g0 + w2 * g1;
-            const float duv[2] = {-(w2 * d0) * dw2, -(w2 * d1) * dw2};
-            float dqv[3] = {0.f, 0.f, 0.f};
-            project_bwd(cams.cam[v], xc, duv, dqv);
-            S.contrib[3 * idx] = dqv[0]; S.contrib[3 * idx + 1] = dqv[1]; S.contrib[3 * idx + 2] = dqv[2];
-        }
-        __syncthreads();
-        PHASE_MARK(8);
-        if (t < K) {
-            float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-            for (int v = 0; v < V; ++v) {
-                a0 += S.contrib[3 * (v * K + t)]; a1 += S.contrib[3 * (v * K + t) + 1]; a2 += S.contrib[3 * (v * K + t) + 2];
-            }
-            S.dq[3 * t] = a0; S.dq[3 * t + 1] = a1; S.dq[3 * t + 2] = a2;
-        } else if (t >= 32 && t < 32 + V) {
-            const int v = t - 32;
-            float a = 0.f;
-            for (int k = 0; k < K; ++k) a += S.lterm[v * K + k];
-            S.vsum[v] = a * dw2;
-        }
-        __syncthreads();
-        PHASE_MARK(9);
-        if (t == 0) {
-            float a = 0.f;
-            for (int v = 0; v < V; ++v) a += S.vsum[v];
-            S.sc[0] = a;
-        }
-        if (t >= 32 && t < 35) {
-            float a = 0.f;
-            for (int k = 0; k < K; ++k) a += S.dq[3 * k + t - 32];
-            S.grad[kOffTransl + t - 32] = a;
-        }
-        if (t >= 64 && t < 64 + kJoints) {
-            const int j = t - 64;
-            float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-            for (int k = 0; k < K; ++k)
-                if (m.kp_chain[k] == j) { a0 += S.dq[3 * k]; a1 += S.dq[3 * k + 1]; a2 += S.dq[3 * k + 2]; }
-            S.dg[3 * j] = a0; S.dg[3 * j + 1] = a1; S.dg[3 * j + 2] = a2;
-        }
-        if (t >= 96 && t < 96 + nsup) {
-            const int i = t - 96;
-            float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-            for (int e = m.sup_ptr[i]; e < m.sup_ptr[i + 1]; ++e) {
-                const int k = m.sup_k[e];
-                const float w = m.sup_w[e];
-                a0 = fmaf(w, S.dq[3 * k], a0); a1 = fmaf(w, S.dq[3 * k + 1], a1); a2 = fmaf(w, S.dq[3 * k + 2], a2);
-            }
-            S.dv[3 * i] = a0; S.dv[3 * i + 1] = a1; S.dv[3 * i + 2] = a2;
-        }
-    }
-    __syncthreads();
-    PHASE_MARK(10);
-    if (have_grad) {
-        // ---- P7 adjoint of skinning: dvp = T3x3^T dv ; dA_j = sum_i W[i,j] [dv (x) vp | dv]
-        const int nx = din.n_extra, ncol_all = ncol + 3 * nx;
-        if (t < nsup + nx) {
-            const int n = t < nsup ? m.sup[t] : din.extra_n[t - nsup];
-            float G[9];
-#pragma unroll
-            for (int c = 0; c < 9; ++c) G[c] = 0.f;
+            for (int c = 0; c < 12; ++c) T[c] = 0.f;
             for (int e = 0; e < m.KW; ++e) {
                 const float w = m.ell_w[(size_t)n * m.KW + e];
                 if (w != 0.f) {
                     const float* Aj = &S.A[12 * m.ell_j[(size_t)n * m.KW + e]];
 #pragma unroll
-                    for (int r = 0; r < 3; ++r)
-#pragma unroll
-                        for (int c = 0; c < 3; ++c) G[3 * r + c] = fmaf(w, Aj[4 * r + c], G[3 * r + c]);
+                    for (int c = 0; c < 12; ++c) T[c] = fmaf(w, Aj[c], T[c]);
                 }
             }
-            const float d0 = S.dv[3 * t], d1 = S.dv[3 * t + 1], d2 = S.dv[3 * t + 2];
-            S.dvp[3 * t] = G[0] * d0 + G[3] * d1 + G[6] * d2;
-            S.dvp[3 * t + 1] = G[1] * d0 + G[4] * d1 + G[7] * d2;
-            S.dvp[3 * t + 2] = G[2] * d0 + G[5] * d1 + G[8] * d2;
+            const float p0 = S.vp[3 * t], p1 = S.vp[3 * t + 1], p2 = S.vp[3 * t + 2];
+#pragma unroll
+            for (int r = 0; r < 3; ++r) S.v[3 * t + r] = T[4 * r] * p0 + T[4 * r + 1] * p1 + T[4 * r + 2] * p2 + T[4 * r + 3];
         }
-        for (int e = t; e < kSkinFloats; e += kResThreads) {
-            const int j = e / 12, r = (e % 12) / 4, c = e % 4;
-            float a = 0.f;
-            if (S.sj_on) {
+        data_sync();
+        PHASE_MARK(6);
+        // ---- P6 keypoints, projection, GMoF data term and its adjoint down to the support vertices
+        if (t < K) {
+            float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+            for (int e = S.kp_ptr[t]; e < S.kp_ptr[t + 1]; ++e) {
+                const int pos = kp_spos[e];
+                const float w = kp_w[e];
+                a0 = fmaf(w, S.v[3 * pos], a0); a1 = fmaf(w, S.v[3 * pos + 1], a1); a2 = fmaf(w, S.v[3 * pos + 2], a2);
+            }
+            const int cj = S.kp_chain[t];
+            if (cj >= 0) { a0 += S.g[3 * cj]; a1 += S.g[3 * cj + 1]; a2 += S.g[3 * cj + 2]; }
+            S.q[3 * t] = a0 + S.x[kOffTransl]; S.q[3 * t + 1] = a1 + S.x[kOffTransl + 1]; S.q[3 * t + 2] = a2 + S.x[kOffTransl + 2];
+            if (joints_out) {
+                joints_out[((size_t)b * K + t) * 3] = S.q[3 * t]; joints_out[((size_t)b * K + t) * 3 + 1] = S.q[3 * t + 1];
+                joints_out[((size_t)b * K + t) * 3 + 2] = S.q[3 * t + 2];
+            }
+        }
+        data_sync();
+        PHASE_MARK(7);
+        {
+            const float rho2 = lp.rho * lp.rho, dw2 = lp.data_weight * lp.data_weight;
+            for (int idx = t; idx < V * K; idx += kDataThreads) {
+                const int v = idx / K, k = idx % K;
+                float xc[3], uv[2];
+                project_fwd(cams.cam[v], &S.q[3 * k], xc, uv);
+                const size_t o = ((size_t)v * B + b) * K + k;
+                if (proj_out) { proj_out[2 * o] = uv[0]; proj_out[2 * o + 1] = uv[1]; }
+                float w = joint_w[k];
+                if (lp.use_joints_conf) w *= conf[o];
+                const float w2 = w * w;
+                float d0, d1;
+                const float g0 = gmof(gt_uv[2 * o] - uv[0], rho2, &d0);
+                const float g1 = gmof(gt_uv[2 * o + 1] - uv[1], rho2, &d1);
+                S.lterm[idx] = w2 * g0 + w2 * g1;
+                const float duv[2] = {-(w2 * d0) * dw2, -(w2 * d1) * dw2};
+                float dqv[3] = {0.f, 0.f, 0.f};
+                project_bwd(cams.cam[v], xc, duv, dqv);
+                S.contrib[3 * idx] = dqv[0]; S.contrib[3 * idx + 1] = dqv[1]; S.contrib[3 * idx + 2] = dqv[2];
+            }
+            data_sync();
+            PHASE_MARK(8);
+            if (t < K) {
+                float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+                for (int v = 0; v < V; ++v) {
+                    a0 += S.contrib[3 * (v * K + t)]; a1 += S.contrib[3 * (v * K + t) + 1]; a2 += S.contrib[3 * (v * K + t) + 2];
+                }
+                S.dq[3 * t] = a0; S.dq[3 * t + 1] = a1; S.dq[3 * t + 2] = a2;
+            } else if (t >= 32 && t < 32 + V) {
+                const int v = t - 32;
+                float a = 0.f;
+                for (int k = 0; k < K; ++k) a += S.lterm[v * K + k];
+                S.vsum[v] = a * dw2;
+            }
+            data_sync();
+            PHASE_MARK(9);
+            if (t == 0) {
+                float a = 0.f;
+                for (int v = 0; v < V; ++v) a += S.vsum[v];
+                S.sc[0] = a;
+            }
+            if (t >= 32 && t < 35) {
+                float a = 0.f;
+                for (int k = 0; k < K; ++k) a += S.dq[3 * k + t - 32];
+                S.grad[kOffTransl + t - 32] = a;
+            }
+            if (t >= 64 && t < 64 + kJoints) {
+                const int j = t - 64;
+                float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+                for (int k = 0; k < K; ++k)
+                    if (S.kp_chain[k] == j) { a0 += S.dq[3 * k]; a1 += S.dq[3 * k + 1]; a2 += S.dq[3 * k + 2]; }
+                S.dg[3 * j] = a0; S.dg[3 * j + 1] = a1; S.dg[3 * j + 2] = a2;
+            }
+            if (t >= 96 && t < 96 + nsup) {
+                const int i = t - 96;
+                float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+                for (int e = S.sup_ptr[i]; e < S.sup_ptr[i + 1]; ++e) {
+                    const int k = sup_k[e];
+                    const float w = sup_w[e];
+                    a0 = fmaf(w, S.dq[3 * k], a0); a1 = fmaf(w, S.dq[3 * k + 1], a1); a2 = fmaf(w, S.dq[3 * k + 2], a2);
+                }
+                S.dv[3 * i] = a0; S.dv[3 * i + 1] = a1; S.dv[3 * i + 2] = a2;
+            }
+        }
+        data_sync();
+        PHASE_MARK(10);
+        if (have_grad) {
+            // ---- P7 adjoint of skinning: dvp = T3x3^T dv ; dA_j = sum_i W[i,j] [dv (x) vp | dv]
+            const int nx = din.n_extra, ncol_all = ncol + 3 * nx;
+            if (t < nsup + nx) {
+                const int n = t < nsup ? S.sup[t] : din.extra_n[t - nsup];
+                float G[9];
+#pragma unroll
+                for (int c = 0; c < 9; ++c) G[c] = 0.f;
+                for (int e = 0; e < m.KW; ++e) {
+                    const float w = m.ell_w[(size_t)n * m.KW + e];
+                    if (w != 0.f) {
+                        const float* Aj = &S.A[12 * m.ell_j[(size_t)n * m.KW + e]];
+#pragma unroll
+                        for (int r = 0; r < 3; ++r)
+#pragma unroll
+                            for (int c = 0; c < 3; ++c) G[3 * r + c] = fmaf(w, Aj[4 * r + c], G[3 * r + c]);
+                    }
+                }
+                const float d0 = S.dv[3 * t], d1 = S.dv[3 * t + 1], d2 = S.dv[3 * t + 2];
+                S.dvp[3 * t] = G[0] * d0 + G[3] * d1 + G[6] * d2;
+                S.dvp[3 * t + 1] = G[1] * d0 + G[4] * d1 + G[7] * d2;
+                S.dvp[3 * t + 2] = G[2] * d0 + G[5] * d1 + G[8] * d2;
+            }
+            for (int e = t; e < kSkinFloats; e += kDataThreads) {
+                const int j = e / 12, r = (e % 12) / 4, c = e % 4;
+                float a = 0.f;
+                if (S.sj_on) {
 #pragma unroll 4
-                for (int q2 = S.sj_ptr[j]; q2 < S.sj_ptr[j + 1]; ++q2) {
-                    const int i = S.sj_i[q2];
-                    const float wd = S.sj_w[q2] * S.dv[3 * i + r];
-                    a = (c < 3) ? fmaf(wd, S.vp[3 * i + c], a) : a + wd;
-                }
-            } else {
+                    for (int q2 = S.sj_ptr[j]; q2 < S.sj_ptr[j + 1]; ++q2) {
+                        const int i = S.sj_i[q2];
+                        const float wd = S.sj_w[q2] * S.dv[3 * i + r];
+                        a = (c < 3) ? fmaf(wd, S.vp[3 * i + c], a) : a + wd;
+                    }
+                } else {
 #pragma unroll 4
-                for (int q2 = m.supj_ptr[j]; q2 < m.supj_ptr[j + 1]; ++q2) {
-                    const int i = m.supj_i[q2];
-                    const float wd = m.supj_w[q2] * S.dv[3 * i + r];
-                    a = (c < 3) ? fmaf(wd, S.vp[3 * i + c], a) : a + wd;
+                    for (int q2 = m.supj_ptr[j]; q2 < m.supj_ptr[j + 1]; ++q2) {
+                        const int i = m.supj_i[q2];
+                        const float wd = m.supj_w[q2] * S.dv[3 * i + r];
+                        a = (c < 3) ? fmaf(wd, S.vp[3 * i + c], a) : a + wd;
+                    }
                 }
-            }
-            for (int k = 0; k < nx; ++k) {                     // box-extreme vertices: generic (dense-W) joint ownership
-                const float w = __ldg(din.Wd + (size_t)din.extra_n[k] * kJoints + j);
-                if (w != 0.f) {
-                    const float wd = w * S.dv[3 * (nsup + k) + r];
-                    a = (c < 3) ? fmaf(wd, S.vp[3 * (nsup + k) + c], a) : a + wd;
+                for (int k = 0; k < nx; ++k) {                     // box-extreme vertices: generic (dense-W) joint ownership
+                    const float w = __ldg(din.Wd + (size_t)din.extra_n[k] * kJoints + j);
+                    if (w != 0.f) {
+                        const float wd = w * S.dv[3 * (nsup + k) + r];
+                        a = (c < 3) ? fmaf(wd, S.vp[3 * (nsup + k) + c], a) : a + wd;
+                    }
                 }
+                if (din.part) {                                    // penetration gradient: unit-factor block partials
+                    const float pa = serial_sum8(din.nfl, [&](int q) { return din.part[(size_t)din.fl[q] * kPartFloats + e]; });
+                    a = fmaf(pa, din.factor, a);
+                }
+                S.dA[e] = a;
             }
-            if (din.part) {                                    // penetration gradient: unit-factor block partials
-                float pa = 0.f;                                // fixed summation order (ascending block index)
-                for (int q = 0; q < din.nfl; ++q) pa += din.part[(size_t)din.fl[q] * kPartFloats + e];
-                a = fmaf(pa, din.factor, a);
-            }
-            S.dA[e] = a;
-        }
-        __syncthreads();
-        PHASE_MARK(11);
-        // ---- P8 dPhi[k] = sum_col dvp[col] Qk[row(col)][k]   (thread per k, coalesced rows)
-        if (t < kFeatPad) {
-            float a = 0.f;
-            int col = 0;
-            for (; col + 32 <= ncol_all; col += 32) {          // 32 independent L2 loads in flight per thread: the phase is as long
-                float qv[32];                                  // as its round trips to L2 (258 rows: 8 instead of 21)
+            p8_sync();                                         // dvp ready for P8 (warp 6 included)
+            PHASE_MARK(11);
+            // ---- P8 dPhi[k] = sum_col dvp[col] Qk[row(col)][k]   (thread per k, coalesced rows; warp 6 takes k >= 192)
+            dphi_col(S, m, din, ncol_all, t);
+            p8_sync();
+            PHASE_MARK(12);
+            // ---- P9 adjoint of the skinning transforms
+            if (t < kJoints)
+                skin_transform_bwd(&S.dA[12 * t], &S.Gam[9 * t], &S.J[3 * t], &S.dGam[9 * t], &S.dg[3 * t], &S.dJ[3 * t]);
+            data_sync();
+            PHASE_MARK(14);
+            // reverse sweep over the tree, level-parallel
+            chain_bwd_levels(S);
+            if (warp == 0) {
+                const float sc = S.x[kOffScale];
+                if (lane < 9) S.dR[lane] = sc * S.dGam[lane];
+                if (lane == 0) {
+                    float ds = 0.f;
 #pragma unroll
-                for (int u = 0; u < 32; ++u) qv[u] = __ldg(m.Qk + (size_t)S.rowbase[col + u] * kFeatPad + t);
-#pragma unroll
-                for (int u = 0; u < 32; ++u) a = fmaf(S.dvp[col + u], qv[u], a);
+                    for (int i = 0; i < 9; ++i) ds = fmaf(S.dGam[i], S.R[i], ds);
+                    S.grad[kOffScale] = ds;
+                }
+                if (lane < 3) S.dJ[lane] += S.dg[lane];
             }
-            for (; col + 8 <= ncol_all; col += 8) {
-                float qv[8];
-#pragma unroll
-                for (int u = 0; u < 8; ++u) qv[u] = __ldg(m.Qk + (size_t)S.rowbase[col + u] * kFeatPad + t);
-#pragma unroll
-                for (int u = 0; u < 8; ++u) a = fmaf(S.dvp[col + u], qv[u], a);
+            data_sync();
+            PHASE_MARK(15);
+            // ---- P10 pose-feature adjoint, Rodrigues adjoint, shape gradient
+            for (int k = t; k < kPoseBasis; k += kDataThreads) S.dR[9 + k] += S.dPhi[k];
+            data_sync();
+            PHASE_MARK(16);
+            if (t < kJoints) {
+                float dr[3] = {0.f, 0.f, 0.f};
+                rodrigues_bwd(t == 0 ? &S.x[kOffOrient] : &theta[3 * (t - 1)], &S.dR[9 * t], dr);
+                float* go = (vp2 && t > 0) ? &W->dth[3 * (t - 1)] : &S.grad[kOffOrient + 3 * t];     // decoded pose: adjoint goes on
+                go[0] = dr[0]; go[1] = dr[1]; go[2] = dr[2];
+            } else if (t >= 32 && t < 32 + kBetas) {
+                const int l = t - 32;
+                float a = S.dPhi[kPoseBasis + l];
+                for (int jc = 0; jc < kJoints * 3; ++jc) a = fmaf(m.JS[jc * kBetas + l], S.dJ[jc], a);
+                S.grad[kOffBetas + l] = a;
             }
-            for (; col < ncol_all; ++col) a = fmaf(S.dvp[col], __ldg(m.Qk + (size_t)S.rowbase[col] * kFeatPad + t), a);
-            if (din.part) {
-                float pa = 0.f;
-                for (int q = 0; q < din.nfl; ++q) pa += din.part[(size_t)din.fl[q] * kPartFloats + kSkinFloats + t];
-                a = fmaf(pa, din.factor, a);
-            }
-            S.dPhi[t] = a;
-        }
-        __syncthreads();
-        PHASE_MARK(12);
-        // ---- P9 adjoint of the skinning transforms
-        if (t < kJoints)
-            skin_transform_bwd(&S.dA[12 * t], &S.Gam[9 * t], &S.J[3 * t], &S.dGam[9 * t], &S.dg[3 * t], &S.dJ[3 * t]);
-        __syncthreads();
-        PHASE_MARK(14);
-        // reverse sweep over the tree, level-parallel
-        chain_bwd_levels(S);
-        if (warp == 0) {
-            const float sc = S.x[kOffScale];
-            if (lane < 9) S.dR[lane] = sc * S.dGam[lane];
-            if (lane == 0) {
-                float ds = 0.f;
-#pragma unroll
-                for (int i = 0; i < 9; ++i) ds = fmaf(S.dGam[i], S.R[i], ds);
-                S.grad[kOffScale] = ds;
-            }
-            if (lane < 3) S.dJ[lane] += S.dg[lane];
-        }
-        __syncthreads();
-        PHASE_MARK(15);
-        // ---- P10 pose-feature adjoint, Rodrigues adjoint, shape gradient
-        if (t < kPoseBasis) S.dR[9 + t] += S.dPhi[t];
-        __syncthreads();
-        PHASE_MARK(16);
-        if (t < kJoints) {
-            float dr[3] = {0.f, 0.f, 0.f};
-            rodrigues_bwd(t == 0 ? &S.x[kOffOrient] : &theta[3 * (t - 1)], &S.dR[9 * t], dr);
-            float* go = (vp2 && t > 0) ? &W->dth[3 * (t - 1)] : &S.grad[kOffOrient + 3 * t];     // decoded pose: adjoint goes on
-            go[0] = dr[0]; go[1] = dr[1]; go[2] = dr[2];
-        } else if (t >= 32 && t < 32 + kBetas) {
-            const int l = t - 32;
-            float a = S.dPhi[kPoseBasis + l];
-            for (int jc = 0; jc < kJoints * 3; ++jc) a = fmaf(m.JS[jc * kBetas + l], S.dJ[jc], a);
-            S.grad[kOffBetas + l] = a;
         }
     }
-    // ---- P11 priors (fitting.py:327-350), all GMM components in parallel
+    __syncthreads();                      // the two groups join: P11b applies the priors after the data-term gradient
+    PHASE_MARK(17);
     const float bpw = lp.body_pose_weight, bpw2 = bpw * bpw;
     const int M = m.M;
-    if (!lp.use_vposer && lp.body_prior == MVS_PRIOR_GMM)
-        for (int e = t; e < M * 69; e += kResThreads) S.gm_diff[e] = theta[e % 69] - m.gmm_means[e];
-    if (vp2) S.red[t] = (t < kVpZ) ? S.x[kOffPose + t] * S.x[kOffPose + t] : 0.f;      // |z|^2 (fitting.py:327-329)
-    else S.red[t] = (t < 69) ? theta[t] * theta[t] : 0.f;
-    __syncthreads();
-    PHASE_MARK(17);
-    if (!lp.use_vposer && lp.body_prior == MVS_PRIOR_GMM) {
-        for (int e = t; e < M * 69; e += kResThreads) {
-            const int mm = e / 69, i = e % 69;
-            const float* P = m.gmm_prec + (size_t)mm * 69 * 69 + i;
-            const float* df = &S.gm_diff[mm * 69];
-            float y = 0.f;
-#pragma unroll
-            for (int j = 0; j < 69; ++j) y = fmaf(__ldg(P + j * 69), df[j], y);       // all 69 loads of the row in flight
-            S.gm_y[e] = y;
-        }
-    }
-    if (t == 0) { float a = 0.f; for (int i = 0; i < 69; ++i) a += S.red[i]; S.sc[1] = a; }
-    __syncthreads();
-    PHASE_MARK(18);
-    if (!lp.use_vposer && lp.body_prior == MVS_PRIOR_GMM && warp < M) {
-        float p = 0.f;
-        for (int i = lane; i < 69; i += 32) p = fmaf(S.gm_y[warp * 69 + i], S.gm_diff[warp * 69 + i], p);
-        p = warp_sum(p);
-        if (lane == 0) S.gm_ll[warp] = 0.5f * p - m.gmm_lognllw[warp];
-    }
-    __syncthreads();
-    PHASE_MARK(19);
     float pprior = 0.f, l2extra = 0.f;
     if (vp2) pprior = S.sc[1] * bpw2;
     if (!lp.use_vposer) {
@@ -680,8 +749,6 @@ static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m,
         shape_loss = a * sw2;
         if (have_grad && t >= 96 && t < 96 + kBetas) S.grad[kOffBetas + t - 96] += 2.f * S.x[t - 96] * sw2;
     }
-    __syncthreads();
-    PHASE_MARK(20);
     float angle = 0.f;
     {
         const int idx[4] = {52, 55, 9, 12};
@@ -692,10 +759,11 @@ static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m,
         angle *= lp.bending_prior_weight;
         float gs = lp.bending_prior_weight;
         if (angle > 1e4f && !lp.use_vposer) { angle = 0.f; gs = 0.f; }
-        if (have_grad && t == 0) {
+        if (have_grad) {                  // by the thread that added the pose prior to the same entry above: no barrier between
             float* gth = vp2 ? W->dth : &S.grad[kOffPose];
 #pragma unroll
-            for (int i = 0; i < 4; ++i) gth[idx[i]] += 2.f * sg[i] * ev[i] * gs;
+            for (int i = 0; i < 4; ++i)
+                if (t == idx[i]) gth[idx[i]] += 2.f * sg[i] * ev[i] * gs;
         }
     }
     __syncthreads();
@@ -748,6 +816,15 @@ __device__ __forceinline__ void resident_setup(ResidentSmem& S, const ResidentMo
         if (t >= 96 && t < 96 + kJoints + 1) S.sj_ptr[t - 96] = m.supj_ptr[t - 96];
         for (int q = t; q < nsj; q += kResThreads) { S.sj_i[q] = m.supj_i[q]; S.sj_w[q] = m.supj_w[q]; }
     }
+    if (t < m.nsup) S.sup[t] = m.sup[t];
+    if (t <= m.nsup) S.sup_ptr[t] = m.sup_ptr[t];
+    if (t < m.K) S.kp_chain[t] = m.kp_chain[t];
+    if (t <= m.K) S.kp_ptr[t] = m.kp_ptr[t];
+    if (t == 66) S.kp_on = m.nkpe <= kResMaxKpE ? 1 : 0;
+    if (m.nkpe <= kResMaxKpE)
+        for (int q = t; q < m.nkpe; q += kResThreads) {
+            S.kp_spos[q] = m.kp_spos[q]; S.kp_w[q] = m.kp_w[q]; S.sup_k[q] = m.sup_k[q]; S.sup_w[q] = m.sup_w[q];
+        }
 }
 
 // A frame that finished stage k of a multi-stage run starts stage k + 1 at once, with a fresh optimiser (the reference
@@ -829,9 +906,9 @@ struct FrameStepArgs {
 // frame's trial point, finishes the closure (keypoint term, adjoint, priors), advances the frame's L-BFGS state
 // machine and -- if the frame needs another evaluation -- runs the pose forward of the NEXT trial point and
 // writes its feature row / skinning transforms for the next dense vertex launch.
-// `smem_raw`: sizeof(ResidentSmem) + 2 H 86 floats (+ VposerSmem).  All kResThreads threads call; no trailing barrier.
-__device__ __forceinline__ void frame_step_body(unsigned char* smem_raw, const FrameStepArgs& a, const int slot, const int b,
-                                                int* na_next = nullptr, int* fidx_next = nullptr) {
+// `smem_raw`: sizeof(ResidentSmem) + 2 H 86 floats (+ VposerSmem).  All kResThreads threads call; no trailing barrier
+// The caller stages the model tables (resident_setup) first: they are constants of the run.
+__device__ __forceinline__ void frame_step_body(unsigned char* smem_raw, const FrameStepArgs& a, const int slot, const int b) {
     ResidentSmem& S = *reinterpret_cast<ResidentSmem*>(smem_raw);
     const ResidentModel& m = a.m; const CamSet& cams = a.cams; const LossParams* lp_tab = a.lp_tab; const int nstages = a.nstages;
     const LbfgsCfg& cfg = a.cfg; const LbfgsState& L = a.L; float* params = a.params;
@@ -841,80 +918,74 @@ __device__ __forceinline__ void frame_step_body(unsigned char* smem_raw, const F
     const FrameBox* box = a.box; const float* __restrict__ Wd = a.Wd;
     float* Phi = a.Phi; float* PhiTc = a.PhiTc; float* At = a.At; float* slot_tr = a.slot_tr; float* pose_cache = a.pose_cache;
     int* pose_valid = a.pose_valid;
-    const FrameScalars fs0 = L.sc[b];
-    if (fs0.phase == PH_DONE) return;
-    PHASE_MARK(0);
-    const int nparts = (N + 255) / 256;                         // sdf_fused_kernel emits per 256-vertex block
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    resident_setup(S, m);
-    if (t < (int)(sizeof(LossParams) / 4))          // the loss parameters of the stage THIS frame is in
-        reinterpret_cast<int*>(&S.lp)[t] = reinterpret_cast<const int*>(&lp_tab[fs0.stage])[t];
+    const int nparts = (N + 255) / 256;                         // sdf_fused_kernel emits per 256-vertex block
     float* x_eval = L.x_eval + (size_t)b * kParams;
-    for (int i = t; i < kParams; i += kResThreads) S.x[i] = x_eval[i];
-    // Stage this frame's curvature history (<= 2 x 100 x 86 floats) into shared memory with cp.async while the
-    // closure runs: the two-loop recursion is ~200 DEPENDENT dot products, at L2 latency it costs ~80 us, from
-    // shared memory ~5 us.
     float* hy = reinterpret_cast<float*>(smem_raw + sizeof(ResidentSmem));
     float* hs = hy + (size_t)L.H * kParams;
     VposerSmem* W = with_vposer ? reinterpret_cast<VposerSmem*>(hs + (size_t)L.H * kParams) : nullptr;
+    const int phase0 = L.sc[b].phase, stage0 = L.sc[b].stage, hl = L.sc[b].hist_len;
+    // Everything that needs only the frame index is requested at once, ahead of the branch on the frame's phase
+    // (cp.async group 0): the frame's scalars (for the optimiser step; not kept in registers through the closure); the trial point; the optimiser's eight 86-vectors (one read now, one write-back after the step:
+    // every dot product / axpy of the state machine then runs out of shared memory); and the pose forward of this trial
+    // point, computed by the previous round's frame_step for the dense kernels (loaded next to its validity flag instead of
+    // behind it: an invalid cache is simply overwritten by P1-P3 of the closure).
+    if (t < kParams) {
+        const size_t o = (size_t)b * kParams + t, o2 = (size_t)b * 2 * kParams + t;
+        cp_async4(&S.x[t], x_eval + t);
+        cp_async4(&S.lx[t], params + o);
+        cp_async4(&S.lg[t], L.g + o);
+        cp_async4(&S.ld[t], L.d + o);
+        cp_async4(&S.lprev_g[t], L.prev_g + o);
+        cp_async4(&S.lx_init[t], L.x_init + o);
+        cp_async4(&S.lg_prev[t], L.g_prev + o);
+        cp_async4(&S.lbg0[t], L.bg + o2);
+        cp_async4(&S.lbg1[t], L.bg + o2 + kParams);
+    }
+    if (t >= 128 && t < 128 + (int)(sizeof(FrameScalars) / 4))
+        cp_async4(reinterpret_cast<float*>(&S.fs) + (t - 128), reinterpret_cast<const float*>(&L.sc[b]) + (t - 128));
     {
-        const int hl = fs0.hist_len;
+        const float* src = pose_cache + (size_t)b * kPoseCacheFloats;      // R | J | Gam | g | A are contiguous (864 floats)
+        for (int i = t; i < kPoseCacheFloats / 4; i += kResThreads) cp_async16(&S.R[4 * i], src + 4 * i);
+    }
+    cp_async_commit();
+    const bool pose_ready = pose_valid[b] != 0;
+    if (phase0 == PH_DONE) { cp_async_wait_all(); return; }
+    PHASE_MARK(0);
+    if (t < (int)(sizeof(LossParams) / 4))          // the loss parameters of the stage THIS frame is in
+        reinterpret_cast<int*>(&S.lp)[t] = reinterpret_cast<const int*>(&lp_tab[stage0])[t];
+    // Stage this frame's curvature history (<= 2 x 100 x 86 floats) into shared memory while the closure runs (cp.async
+    // group 1): the two-loop recursion is ~200 DEPENDENT dot products, at L2 latency it costs ~80 us, from shared memory ~5 us.
+    {
         const float* gy = L.hist_y + (size_t)b * L.H * kParams;
         const float* gs = L.hist_s + (size_t)b * L.H * kParams;
         // ring buffer: with hl < H the live rows are [0, hl); when full all rows are live.  8-byte packets
         // (rows are 344 B: 8-byte aligned)
         const int total = hl * kParams / 2;
         for (int i = t; i < total; i += kResThreads) {
-            const unsigned sy = (unsigned)__cvta_generic_to_shared(hy + 2 * i);
-            const unsigned ss = (unsigned)__cvta_generic_to_shared(hs + 2 * i);
-            asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(sy), "l"(gy + 2 * i));
-            asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(ss), "l"(gs + 2 * i));
+            cp_async8(hy + 2 * i, gy + 2 * i);
+            cp_async8(hs + 2 * i, gs + 2 * i);
         }
-        for (int i = t; i < hl; i += kResThreads) S.ro[i] = L.ro[(size_t)b * L.H + i];
+        for (int i = t; i < hl; i += kResThreads) cp_async4(&S.ro[i], L.ro + (size_t)b * L.H + i);
         {   // block Gram of the live part of the ring
             const float* gg = L.gram + (size_t)b * kGramFloats;
             const int nfl4 = ((hl == L.H ? L.H : hl) + 7) / 8 * 16;      // float4 packets
-            for (int i = t; i < nfl4; i += kResThreads) {
-                const unsigned sg = (unsigned)__cvta_generic_to_shared(S.gram + 4 * i);
-                asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(sg), "l"(gg + 4 * i));
-            }
+            for (int i = t; i < nfl4; i += kResThreads) cp_async16(S.gram + 4 * i, gg + 4 * i);
         }
-        asm volatile("cp.async.commit_group;");
-        // the optimiser's seven 86-vectors: one coalesced read now, one write-back after the step (every dot
-        // product / axpy of the state machine then runs out of shared memory instead of ~30 dependent L2 round trips)
-        for (int i = t; i < kParams; i += kResThreads) {
-            S.lx[i] = params[(size_t)b * kParams + i];
-            S.lg[i] = L.g[(size_t)b * kParams + i];
-            S.ld[i] = L.d[(size_t)b * kParams + i];
-            S.lprev_g[i] = L.prev_g[(size_t)b * kParams + i];
-            S.lx_init[i] = L.x_init[(size_t)b * kParams + i];
-            S.lg_prev[i] = L.g_prev[(size_t)b * kParams + i];
-            S.lbg0[i] = L.bg[(size_t)b * 2 * kParams + i];
-            S.lbg1[i] = L.bg[(size_t)b * 2 * kParams + kParams + i];
-        }
-    }
-    // pose forward of THIS trial point: computed by the previous round's frame_step (for the dense kernels), restored here
-    // (loaded unconditionally, next to the validity flag instead of behind it: an invalid cache is simply overwritten
-    // by P1-P3 of the closure)
-    const bool pose_ready = pose_valid[b] != 0;
-    {
-        float* dst = &S.R[0];                         // R | J | Gam | g | A are contiguous (864 floats)
-        const float* src = pose_cache + (size_t)b * kPoseCacheFloats;
-        for (int i = t; i < kPoseCacheFloats; i += kResThreads) dst[i] = src[i];
+        cp_async_commit();
     }
     if (warp == 7) {
         // frame scalars of the penetration term (fitting.py:386-392): total of the sampled values -> loss, the
         // factor of the listed vertices' adjoint, and the <= 6 box-extreme vertices that carry the gradient through
         // the box centre (mean of min / max vertex) and scale (0.6 x the largest extent)
         float a = 0.f;
-        if (lane < 5)
-            for (int p = 0; p < nparts; ++p) a += parts5[((size_t)slot * nparts + p) * 5 + lane];
+        if (lane < 5) a = serial_sum8(nparts, [&](int p) { return parts5[((size_t)slot * nparts + p) * 5 + lane]; });
         float tot[5];
 #pragma unroll
         for (int q = 0; q < 5; ++q) tot[q] = __shfl_sync(0xffffffffu, a, q);
         if (lane == 0) {
             const FrameBox fb = box[slot];
-            const float coll_w = lp_tab[fs0.stage].coll_loss_weight;
+            const float coll_w = lp_tab[stage0].coll_loss_weight;
             const float wsum = coll_w * tot[0];                 // coll_loss_weight * cur_loss.sum() / 1
             const float cg = 2.f * wsum * coll_w;               // d pen / d (sum of samples)
             const float inv_s = 1.f / fb.scale;
@@ -944,6 +1015,7 @@ __device__ __forceinline__ void frame_step_body(unsigned char* smem_raw, const F
         }
         if (lane == 0) S.nfl = nfl < 64 ? nfl : 64;
     }
+    cp_async_wait_group<1>();                          // group 0: the frame state the closure starts from
     __syncthreads();
     PHASE_MARK(1);
     DenseIn din;
@@ -961,7 +1033,7 @@ __device__ __forceinline__ void frame_step_body(unsigned char* smem_raw, const F
     din.pose_ready = pose_ready;
     resident_closure(S, m, cams, S.lp, gt_uv, conf, joint_w, B, b, true, nullptr, nullptr, din, W);
     for (int i = t; i < kParams; i += kResThreads) L.g_eval[(size_t)b * kParams + i] = S.lg_new[i];
-    asm volatile("cp.async.wait_all;");
+    cp_async_wait_all();                               // group 1: history, curvature scalars, block Gram
     __syncthreads();
     PHASE_MARK(23);
     if (cfg.step_mode == 2) {                          // closure only (mvs_closure in exec mode 3): no optimiser step
@@ -969,7 +1041,7 @@ __device__ __forceinline__ void frame_step_body(unsigned char* smem_raw, const F
         return;
     }
     if (warp == 0) {
-        FrameScalars s = fs0;
+        FrameScalars s = S.fs;
         LbfgsPtrs P{S.lx, S.lg, S.ld, S.lprev_g, S.lx_init, S.lg_prev, S.lbg0, S.lbg1, hy, hs, S.ro, S.al, S.lx_eval,
                     S.lg_new, L.H, S.gram, S.tl_scratch};
         lbfgs_advance_core(s, P, S.sc[2], cfg, lane, S.lp.use_vposer == 2 ? 32 : kOffTransl - kOffPose);
@@ -979,7 +1051,15 @@ __device__ __forceinline__ void frame_step_body(unsigned char* smem_raw, const F
             VLOOP(i) S.lx_eval[i] = S.lx[i];
             __syncwarp();
         }
-        VLOOP(i) {
+        VLOOP(i) S.x[i] = S.lx_eval[i];                // the next trial point: input of next_pose_forward
+        if (lane == 0) { L.sc[b] = s; S.fs = s; }
+    }
+    __syncthreads();
+    PHASE_MARK(24);
+    // global write-back of the optimiser state, on warps 4-7: the first two phases of next_pose_forward run on warps 0-3
+    if (warp >= 4) {
+        const int u = t - 128;
+        for (int i = u; i < kParams; i += kResThreads - 128) {
             params[(size_t)b * kParams + i] = S.lx[i];
             L.g[(size_t)b * kParams + i] = S.lg[i];
             L.d[(size_t)b * kParams + i] = S.ld[i];
@@ -990,35 +1070,24 @@ __device__ __forceinline__ void frame_step_body(unsigned char* smem_raw, const F
             L.bg[(size_t)b * 2 * kParams + kParams + i] = S.lbg1[i];
             x_eval[i] = S.lx_eval[i];
         }
-        if (s.pushed_slot >= 0) {                       // write the new curvature pair through to global memory
-            const int wslot = s.pushed_slot;
-            VLOOP(i) {
+        const int wslot = S.fs.pushed_slot;
+        if (wslot >= 0) {                               // write the new curvature pair through to global memory
+            for (int i = u; i < kParams; i += kResThreads - 128) {
                 L.hist_y[((size_t)b * L.H + wslot) * kParams + i] = hy[(size_t)wslot * kParams + i];
                 L.hist_s[((size_t)b * L.H + wslot) * kParams + i] = hs[(size_t)wslot * kParams + i];
             }
-            if (lane == 0) L.ro[(size_t)b * L.H + wslot] = S.ro[wslot];
-            float* gg = L.gram + (size_t)b * kGramFloats + (wslot >> 3) * 64;
-            gg[lane] = S.gram[(wslot >> 3) * 64 + lane]; gg[lane + 32] = S.gram[(wslot >> 3) * 64 + lane + 32];
+            if (u == 0) L.ro[(size_t)b * L.H + wslot] = S.ro[wslot];
+            if (u < 64) L.gram[(size_t)b * kGramFloats + (wslot >> 3) * 64 + u] = S.gram[(wslot >> 3) * 64 + u];
         }
-        if (lane == 0) { L.sc[b] = s; S.fs = s; }
     }
-    __syncthreads();
-    PHASE_MARK(24);
     if (S.fs.phase == PH_DONE) return;
-    // pose forward of the next trial point -> Phi row and skinning transforms for the next vertex launch.  The persistent
-    // dense-round kernel hands out next round's slots here (atomic counter = compaction every round; a frame's arithmetic
-    // does not depend on the slot it lands in), the multi-kernel path keeps the slot until its next compaction.
-    if (na_next) {
-        if (t == 0) { const int ns = atomicAdd(na_next, 1); fidx_next[ns] = b; S.nfl = ns; }
-        __syncthreads();
-    }
-    const int slot_next = na_next ? S.nfl : slot;
-    for (int i = t; i < kParams; i += kResThreads) S.x[i] = S.lx_eval[i];
-    __syncthreads();
-    PHASE_MARK(25);
+    // pose forward of the next trial point -> Phi row and skinning transforms for the next vertex launch (the frame keeps
+    // its slot until the next compaction).  vp2n: the stage the NEXT evaluation belongs to (S.lp unless the frame just
+    // changed stage).
     {
-        const bool vp2n = W != nullptr && lp_tab[S.fs.stage].use_vposer == 2;     // the stage the NEXT evaluation belongs to
-        next_pose_forward(S, m, W, vp2n, slot_next, b, Phi, PhiTc, At, ldA, slot_tr, pose_cache, pose_valid);
+        const int nst = S.fs.stage;
+        const bool vp2n = W != nullptr && (nst == stage0 ? S.lp.use_vposer : lp_tab[nst].use_vposer) == 2;
+        next_pose_forward(S, m, W, vp2n, slot, b, Phi, PhiTc, At, ldA, slot_tr, pose_cache, pose_valid);
     }
     PHASE_MARK(28);
 }

@@ -5,12 +5,12 @@ import torch
 from mvsmplfitting_b200 import _lib, synthetic as S
 _lib.LIB_PATH = os.path.join(os.path.dirname(_lib.LIB_PATH), "libmvsmpl_dbg.so")
 from mvsmplfitting_b200.context import FittingContext
-NAMES = {0: "start", 1: "prologue (state loads, history cp.async issue, SDF scalars)", 2: "P1 rodrigues/J", 3: "P2 chain",
+NAMES = {0: "start", 1: "prologue (frame state cp.async, history cp.async issue, SDF scalars)", 2: "P1 rodrigues/J", 3: "P2 chain",
          4: "P3 A/Phi", 5: "P4 vposed gather", 6: "P5", 7: "P6 keypoints", 8: "P6 projection", 9: "P6 reduce", 10: "P6 scatter",
-         11: "P7 dvp/dA", 12: "P8 dPhi", 13: "SDF parts", 14: "P9 skin_transform_bwd", 15: "reverse sweep", 16: "P10a",
-         17: "P10 rodrigues_bwd/betas + gm_diff", 18: "GMM matvec", 19: "GMM ll", 20: "priors", 21: "angle", 22: "total/grad",
-         23: "g_eval store + cp.async wait", 24: "L-BFGS advance + write-back", 25: "x copy", 26: "rodrigues (next)", 27: "chain (next)",
-         28: "A/Phi store (next)"}
+         11: "P7 dvp/dA", 12: "P8 dPhi", 14: "P9 skin_transform_bwd", 15: "reverse sweep", 16: "P10a",
+         17: "P10 rodrigues_bwd/betas, join with warps 6-7 (GMM, |theta|^2)", 21: "priors + angle", 22: "total/grad",
+         23: "g_eval store + cp.async wait", 24: "L-BFGS advance", 26: "rodrigues (next) + write-back (warps 4-7)",
+         27: "chain (next)", 28: "A/Phi store (next)"}
 model = S.make_model(0); gmm = S.make_gmm(7); cams = S.make_cameras(8)
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 256
 fr = S.make_frames(model, cams, B, seed=1000)
@@ -31,7 +31,7 @@ clk = torch.cuda.get_device_properties(0).clock_rate if hasattr(torch.cuda.get_d
 ghz = 1.965
 prev = buf[0]
 print("phase                                                        cycles      us (at %.3f GHz)" % ghz)
-for i in range(1, 29):
+for i in sorted(NAMES)[1:]:
     if buf[i] == 0 or buf[i] < prev:
         print("%2d %-56s (not reached in the last launch)" % (i, NAMES.get(i, "")))
         continue
@@ -39,7 +39,7 @@ for i in range(1, 29):
     print("%2d %-56s %8d %8.2f" % (i, NAMES.get(i, ""), d, d / ghz / 1e3))
     prev = buf[i]
 print("total %.2f us" % ((prev - buf[0]) / ghz / 1e3))
-print("max over all CTAs and launches (us): closure %.2f | history wait %.2f | advance+write-back %.2f | next pose %.2f | "
+print("max over all CTAs and launches (us): closure %.2f | history wait %.2f | advance (+ write-back) %.2f | next pose %.2f | "
       "start->advanced %.2f | start->end %.2f" % tuple(buf[32 + k] / ghz / 1e3 for k in range(6)))
 
 print("longest two-loop recursion: %.2f us with %d history pairs" % (buf[40] / ghz / 1e3, buf[41]))
