@@ -837,10 +837,10 @@ int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st) {
 
 // need_vposed = false: the caller's consumers recompute v_posed where they need it (the dense rounds: sdf_fused / frame_step read
 // ST . [beta; 1] + pose offsets for their few vertices), so the skinning kernel does not write the [B][N][3] array at all
-int launch_vertex_fwd_dense(mvs_ctx* ctx, cudaStream_t st, bool allow_tc, bool need_vposed) {
+int launch_vertex_fwd_dense(mvs_ctx* ctx, cudaStream_t st, bool allow_tc, bool need_vposed, bool sdf_setup) {
     DevModel& m = ctx->m;
     Workspace& w = ctx->ws;
-    if (allow_tc && tc_available(ctx)) return launch_vertex_fwd_tc(ctx, st, need_vposed);     // wgmma / TMA path (mvs_tc.cu)
+    if (allow_tc && tc_available(ctx)) return launch_vertex_fwd_tc(ctx, st, need_vposed, sdf_setup);     // wgmma / TMA path (mvs_tc.cu)
     if (!ctx->attr_done) {
         MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertFwdSmem));
         MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertBwdSmem));

@@ -123,6 +123,8 @@ struct Workspace {
     float* sdf_part = nullptr;        // [B][P][512] unit-factor partial adjoints (288 skin | 224 feature)
     int* sdf_pflag = nullptr;         // [B][P] 1 iff the block has vertices with a non-zero sample gradient
     unsigned char* sdf_box = nullptr; // [B] FrameBox
+    unsigned char* sdf_setup = nullptr;   // [B] SdfFrameSetup, written by the skinning kernel's last CTA of each frame
+    int* sdf_arrive = nullptr;        // [B] chunk boxes of the frame written so far this round (0 between rounds)
     // accelerated all-faces SDF (mvs_sdf_bins.cuh): per slot triangle corners, cell lists, ray-bin lists, meta (s_lo, s_scale, overflow)
     float* bins_tri = nullptr; int* bins_cell_ptr = nullptr; unsigned short* bins_cell_idx = nullptr;
     int* bins_ray_ptr = nullptr; unsigned short* bins_ray_idx = nullptr; float* bins_meta = nullptr;
@@ -136,10 +138,35 @@ struct FrameBox {                     // bounding box of one frame's mesh (fitti
     float pad;
 };
 
+// What sdf_fused needs of a frame before it touches a vertex: the frame box, triangle 0 in box coordinates, the cone it
+// spans from the corner (-1,-1,-1) and the triangle's plane with their margins, the vertex-level pads, and the chunk-cull
+// verdict of every 64-vertex chunk.  Computed once per frame and round by the skinning kernel (sdf_frame_setup in
+// mvs_tc_dev.cuh) instead of by every sdf_fused CTA.
+constexpr int kSdfSkipWords = 8;      // chunk-cull bits for up to 256 chunks (16384 vertices); larger meshes are not culled
+struct __align__(16) SdfFrameSetup {
+    FrameBox fb;
+    float tri[9];
+    float cn[3][3], cm[3];
+    float pn[3], pd, pm;
+    float vpad[3], vpadp;
+    float unused[2];
+    unsigned skip[kSdfSkipWords];     // bit (c & 31) of word c / 32: no vertex of chunk c can see phi != 0
+};
+static_assert(sizeof(SdfFrameSetup) == 208, "SdfFrameSetup layout");
+
+// Per-launch arguments of the set-up; rec == nullptr: the skinning kernel does not compute it (SDF term off)
+struct SdfSetupArgs {
+    SdfFrameSetup* rec; FrameBox* boxout; int* arrive; const float* slot_tr;
+    int f0, f1, f2, G, cull;          // triangle 0, grid size, cone/plane culls on (as-written semantics: one face)
+};
+
 // sdf_fused_kernel gives a CTA 1 or 2 blocks of 256 vertices (results are emitted per block and do not depend on it).
 // Measured on the benchmark (us per launch, ~150 active frames): 1 block 40.0, 2 blocks 37.7, 3: 40.7, 4: 42, 8: 54,
 // 16: 76 -- the few expensive blocks near the cone must not pile up in one CTA, and small CTAs balance better than the
-// shorter prologue of large ones saves.
+// shorter prologue of large ones saves.  Re-measured once the prologue became a single load of the skinning kernel's set-up
+// record (H100, one dense round, us per launch at 256 / 64 / 8 / 1 active frames): 1 block 65.5 / 28.8 / 15.8 / 17.0,
+// 2: 54.2 / 30.1 / 19.6 / 20.2, 4: 54.8 / 29.8 / 22.6 / 21.9, 8: 52.7 / 28.9 / 25.4 / 24.5.  No setting beats this rule by
+// more than the spread of a single sample (~3 %), so it stays.
 constexpr int kSdfMaxPasses = 8;
 __host__ __device__ inline int sdf_passes_for(int na, int nblocks, int cta_slots) {
     return (long long)na * nblocks > 2LL * cta_slots ? 2 : 1;
@@ -276,13 +303,15 @@ int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const void* lbfgs_cfg
                           const void* stage_rng_dev = nullptr);
 // dense regime (SDF term): per round  posedirs_gemm_tc -> skin -> sdf_fused -> frame_step
 bool hybrid_available(const mvs_ctx* ctx);
-int launch_vertex_fwd_dense(mvs_ctx* ctx, cudaStream_t st, bool allow_tc = true, bool need_vposed = true);                                   // mvs_closure.cu
+int launch_vertex_fwd_dense(mvs_ctx* ctx, cudaStream_t st, bool allow_tc = true, bool need_vposed = true, bool sdf_setup = false);                                   // mvs_closure.cu
 int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);                      // mvs_closure.cu
 int launch_sdf_fused(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu
+int ensure_sdf_setup_ws(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu: set-up records, arrival counters (zeroed on st), boxes
+SdfSetupArgs make_sdf_setup_args(mvs_ctx* ctx);          // mvs_sdf.cu
 // mvs_tc.cu: wgmma / TMA dense vertex forward
 int tc_upload_model(mvs_ctx* ctx);                 // after m.Qk is on the device
 bool tc_available(const mvs_ctx* ctx);
-int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed = true);
+int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed = true, bool sdf_setup = false);
 int tc_check_error(mvs_ctx* ctx);
 float* tc_poffT(mvs_ctx* ctx);                 // [3N][ldA] pose offsets of the tensor-core contraction (allocated on first use)
 int tc_prepare(mvs_ctx* ctx);                  // tensor maps + pose-offset buffer (idempotent)

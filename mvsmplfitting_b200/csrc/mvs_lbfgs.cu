@@ -263,7 +263,7 @@ static int run_stage(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, con
         w.na_bound = B;                                               // grids shrink with the (lagging) host view of the count
         while (rounds < max_rounds) {
             for (int r = 0; r < chunk; ++r) {
-                if ((rc = launch_vertex_fwd_dense(ctx, st, true, false))) return rc;   // wgmma GEMM + LBS + bbox partials
+                if ((rc = launch_vertex_fwd_dense(ctx, st, true, false, true))) return rc;   // wgmma GEMM + LBS + SDF set-up
                 if ((rc = launch_sdf_fused(ctx, st))) return rc;   // samples + adjoint of the listed vertices
                 if ((rc = launch_frame_step(ctx, params_dev, &S, &cfg, nst, st))) return rc;
                 ++rounds;
@@ -364,7 +364,7 @@ int dense_regime_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, floa
     w.na_bound = B;
     if ((rc = launch_frame_fwd_dense(ctx, S.x_eval, &S, 1, st))) return rc;
     if ((rc = frame_step_begin_run(ctx, st))) return rc;
-    if ((rc = launch_vertex_fwd_dense(ctx, st, true, false))) return rc;
+    if ((rc = launch_vertex_fwd_dense(ctx, st, true, false, true))) return rc;
     if ((rc = launch_sdf_fused(ctx, st))) return rc;
     if ((rc = launch_frame_step(ctx, const_cast<float*>(x_dev) /* read only in this mode */, &S, &cfg, 1, st))) return rc;
     if (loss_dev) MVS_CUDA_OK(ctx, cudaMemcpyAsync(loss_dev, S.loss_eval, (size_t)B * sizeof(float), cudaMemcpyDeviceToDevice, st));

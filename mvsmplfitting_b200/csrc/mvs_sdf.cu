@@ -20,6 +20,37 @@
 #include <cstdlib>
 #include "mvs_internal.cuh"
 #include "mvs_lbfgs_core.cuh"
+// -DMVS_PHASE_DBG (scripts/sdf_phase_times.py): thread 0 of every sdf_fused CTA that runs to the end stamps clock64() at
+// entry (0), after pdl_wait (1), after the box fold and its barrier (2), once the cone/plane set-up and the chunk-cull
+// verdicts are ready (3), after sampling and its barrier (4) and after the block reduction and adjoint (5).  The intervals
+// 1..5 are summed over CTAs into g_sdf_clk[1..5] and maxed into [9..13]; [16] counts the CTAs, [17] sums the CTAs'
+// entry->end globaltimer nanoseconds (the cycles/ns ratio gives the SM clock of the run).
+#ifdef MVS_PHASE_DBG
+namespace mvs {
+__device__ unsigned long long g_sdf_clk[32];
+__device__ __forceinline__ void sdf_mark(int i) {
+    if (threadIdx.x != 0) return;
+    __shared__ long long s_clk[6];
+    __shared__ unsigned long long s_ns0;
+    const long long c = clock64();
+    s_clk[i] = c;
+    if (i == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(s_ns0));
+    if (i == 5) {
+        unsigned long long ns;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
+        for (int k = 1; k <= 5; ++k) {
+            const unsigned long long d = (unsigned long long)(s_clk[k] - s_clk[k - 1]);
+            atomicAdd(&g_sdf_clk[k], d);
+            atomicMax(&g_sdf_clk[8 + k], d);
+        }
+        atomicAdd(&g_sdf_clk[16], 1ull);
+        atomicAdd(&g_sdf_clk[17], ns - s_ns0);
+        atomicAdd(&g_sdf_clk[18], (unsigned long long)(s_clk[5] - s_clk[0]));
+    }
+}
+}  // namespace mvs
+#define SDF_MARK(i) mvs::sdf_mark(i)
+#endif
 #include "mvs_sdf_dev.cuh"
 
 namespace mvs {
@@ -274,7 +305,7 @@ constexpr int kBinsThreads = 1024;
 constexpr size_t kBinsSmem = (size_t)kBinCells * sizeof(int) + 64 * sizeof(float);
 
 struct SdfBinsArgs {
-    const float* verts; const float* slot_tr; const float* bboxp; const int* faces; int N, F, nbox;
+    const float* verts; const float* slot_tr; const SdfFrameSetup* setup; const int* faces; int N, F;
     float* tri; int* cell_ptr; unsigned short* cell_idx; int* ray_ptr; unsigned short* ray_idx; float* meta;
 };
 
@@ -321,41 +352,10 @@ sdf_bins_kernel(SdfBinsArgs a, const int* __restrict__ na_ptr) {
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     const float* vf = a.verts + (size_t)slot * a.N * 3;
     const float tr[3] = {a.slot_tr[4 * slot], a.slot_tr[4 * slot + 1], a.slot_tr[4 * slot + 2]};
-    // ---- frame box: min / max of the skinning kernel's chunk boxes (exact operations: any order gives sdf_fused's values)
-    float lo[3] = {3e38f, 3e38f, 3e38f}, hi[3] = {-3e38f, -3e38f, -3e38f};
-    for (int tl = t; tl < a.nbox; tl += kBinsThreads) {
-        const float* bp = a.bboxp + ((size_t)slot * a.nbox + tl) * 12;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) { lo[c] = fminf(lo[c], bp[c]); hi[c] = fmaxf(hi[c], bp[3 + c]); }
-    }
-#pragma unroll
-    for (int c = 0; c < 3; ++c)
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            lo[c] = fminf(lo[c], __shfl_xor_sync(0xffffffffu, lo[c], o));
-            hi[c] = fmaxf(hi[c], __shfl_xor_sync(0xffffffffu, hi[c], o));
-        }
-    float* wb = reinterpret_cast<float*>(hist);                // [32][6] during the prologue
-    if (lane == 0) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) { wb[warp * 6 + c] = lo[c]; wb[warp * 6 + 3 + c] = hi[c]; }
-    }
-    __syncthreads();
-    float centre[3], scale;
-    {
-        float ext = -1.f;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            float l = wb[c], h2 = wb[3 + c];
-            for (int w = 1; w < kBinsThreads / 32; ++w) { l = fminf(l, wb[w * 6 + c]); h2 = fmaxf(h2, wb[w * 6 + 3 + c]); }
-            const float lc = l + tr[c], hc = h2 + tr[c];       // as sdf_fused_body (body_models_scale.py:403, fitting.py:352-359)
-            centre[c] = (lc + hc) / 2.f;
-            const float e = hc - lc;
-            if (e > ext) ext = e;
-        }
-        scale = 0.6f * ext;
-    }
-    __syncthreads();
+    // ---- frame box: the set-up the skinning kernel computed for this frame (the box sdf_fused uses)
+    const FrameBox& fbx = a.setup[slot].fb;
+    const float centre[3] = {fbx.centre[0], fbx.centre[1], fbx.centre[2]}, scale = fbx.scale;
+    float* wb = reinterpret_cast<float*>(hist);                // [32][4] scratch of the projected-box fold
     // ---- triangle corners in box coordinates (the brute force's operands, same expression) + bounding box of the projected mesh
     float* tri = a.tri + (size_t)slot * a.F * 9;
     float smn[2] = {3e38f, 3e38f}, smx[2] = {-3e38f, -3e38f};
@@ -471,7 +471,9 @@ static int ensure_sdf_bins_ws(mvs_ctx* ctx) {
 template <bool kAll>
 __global__ void __launch_bounds__(kSdfFThreads, 3)
 sdf_fused_kernel(SdfFusedArgs ar, const int* __restrict__ na_ptr, int passes) {
+    SDF_MARK(0);
     pdl_wait();
+    SDF_MARK(1);
     __shared__ SdfFusedSmem sm;
     sdf_fused_body<kAll>(sm, ar, *na_ptr, (int)blockIdx.y, (int)blockIdx.x, passes);
 }
@@ -495,16 +497,39 @@ int ensure_sdf_fused_ws(mvs_ctx* ctx) {
     return MVS_OK;
 }
 
+int ensure_sdf_setup_ws(mvs_ctx* ctx, cudaStream_t st) {
+    Workspace& w = ctx->ws;
+    int rc;
+    if ((rc = ensure_sdf_fused_ws(ctx))) return rc;
+    if (!w.sdf_setup) {
+        if ((rc = dev_alloc(ctx, &w.sdf_setup, (size_t)w.B * sizeof(SdfFrameSetup)))) return rc;
+        if ((rc = dev_alloc(ctx, &w.sdf_arrive, (size_t)w.B))) return rc;
+        MVS_CUDA_OK(ctx, cudaMemsetAsync(w.sdf_arrive, 0, (size_t)w.B * sizeof(int), st));
+    }
+    return MVS_OK;
+}
+
+SdfSetupArgs make_sdf_setup_args(mvs_ctx* ctx) {
+    Workspace& w = ctx->ws;
+    const DevModel& m = ctx->m;
+    SdfSetupArgs a;
+    a.rec = reinterpret_cast<SdfFrameSetup*>(w.sdf_setup); a.boxout = reinterpret_cast<FrameBox*>(w.sdf_box);
+    a.arrive = w.sdf_arrive; a.slot_tr = w.slot_tr;
+    a.f0 = m.tri0[0]; a.f1 = m.tri0[1]; a.f2 = m.tri0[2]; a.G = ctx->loss.sdf_grid;
+    a.cull = ctx->loss.sdf_all_faces ? (m.F == 1) : 1;        // the cone/plane tests hold for a single face (num_faces == 1)
+    return a;
+}
+
 SdfFusedArgs make_sdf_fused_args(mvs_ctx* ctx) {
     Workspace& w = ctx->ws;
     const DevModel& m = ctx->m;
     const LossParams& lp = ctx->loss;
     SdfFusedArgs a;
     a.verts = w.verts; a.poffT = tc_poffT(ctx); a.Phi = w.Phi; a.ST = m.ST; a.slot_tr = w.slot_tr;
-    a.N = m.N; a.nbox = (m.N + 63) / 64; a.bboxp = w.bboxp; a.faces = m.faces; a.num_faces = lp.sdf_all_faces ? m.F : 1;
-    a.f0 = m.tri0[0]; a.f1 = m.tri0[1]; a.f2 = m.tri0[2]; a.G = lp.sdf_grid;
+    a.N = m.N; a.nbox = (m.N + 63) / 64; a.setup = reinterpret_cast<const SdfFrameSetup*>(w.sdf_setup); a.faces = m.faces;
+    a.num_faces = lp.sdf_all_faces ? m.F : 1; a.G = lp.sdf_grid;
     a.At = w.At; a.ldA = w.ldA; a.ell_j = m.ell_j; a.ell_w = m.ell_w; a.KW = m.KW; a.Wd = m.Wd; a.Qk = m.Qk;
-    a.parts5 = w.sdf_parts5; a.part = w.sdf_part; a.pflag = w.sdf_pflag; a.boxout = reinterpret_cast<FrameBox*>(w.sdf_box);
+    a.parts5 = w.sdf_parts5; a.part = w.sdf_part; a.pflag = w.sdf_pflag;
     a.gcoord = w.sdf_gcoord;
     // sdf_all_faces: 0 as written (triangle 0), 1 all faces over candidate lists (accelerated), 2 all faces by brute force
     const bool binned = lp.sdf_all_faces == 1 && w.bins_tri != nullptr;
@@ -532,7 +557,8 @@ int launch_sdf_fused(mvs_ctx* ctx, cudaStream_t st) {
     if (ctx->loss.sdf_all_faces == 1) {                  // accelerated all-faces mode: this round's candidate lists first
         if ((rc = ensure_sdf_bins_ws(ctx))) return rc;
         SdfBinsArgs ba;
-        ba.verts = w.verts; ba.slot_tr = w.slot_tr; ba.bboxp = w.bboxp; ba.faces = m.faces; ba.N = N; ba.F = m.F; ba.nbox = (N + 63) / 64;
+        ba.verts = w.verts; ba.slot_tr = w.slot_tr; ba.setup = reinterpret_cast<const SdfFrameSetup*>(w.sdf_setup); ba.faces = m.faces;
+        ba.N = N; ba.F = m.F;
         ba.tri = w.bins_tri; ba.cell_ptr = w.bins_cell_ptr; ba.cell_idx = w.bins_cell_idx; ba.ray_ptr = w.bins_ray_ptr;
         ba.ray_idx = w.bins_ray_idx; ba.meta = w.bins_meta;
         MVS_LAUNCH(ctx, KID_SDF_BBOX, st,
@@ -578,3 +604,34 @@ int launch_sdf_terms(mvs_ctx* ctx, const float* x_dev, cudaStream_t st) {
 }
 
 }  // namespace mvs
+
+// Testing aid, not part of the ABI (tests/test_gpu_sdf_setup.py): copies the dense-regime SDF state of the last round to host
+// buffers (null pointers are skipped): the chunk boxes [B][nbox][12], the slot translations [B][4], the FrameBox of every
+// slot as frame_step reads it [B][12 words], the per-block sums [B][nblocks][5] and flags [B][nblocks], and the arrival
+// counters [B].  Synchronises the device first.
+extern "C" int mvs_debug_sdf_state(mvs_ctx* ctx, float* bboxp, float* slot_tr, void* box, float* parts5, int* pflag, int* arrive) {
+    const mvs::Workspace& w = ctx->ws;
+    const size_t B = (size_t)w.B, N = (size_t)ctx->m.N, nbox = (N + 63) / 64, nblocks = (N + mvs::kSdfFThreads - 1) / mvs::kSdfFThreads;
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+    if (!w.sdf_setup || !w.sdf_box || !w.sdf_parts5) return -2;
+    struct { void* dst; const void* src; size_t bytes; } cp[] = {
+        {bboxp, w.bboxp, B * nbox * 12 * sizeof(float)}, {slot_tr, w.slot_tr, B * 4 * sizeof(float)},
+        {box, w.sdf_box, B * sizeof(mvs::FrameBox)}, {parts5, w.sdf_parts5, B * nblocks * 5 * sizeof(float)},
+        {pflag, w.sdf_pflag, B * nblocks * sizeof(int)}, {arrive, w.sdf_arrive, B * sizeof(int)}};
+    for (auto& c : cp)
+        if (c.dst && cudaMemcpy(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+    return 0;
+}
+
+#ifdef MVS_PHASE_DBG
+extern "C" int mvs_debug_sdf_clocks(unsigned long long* out, int n, int reset) {   // debug builds only; not part of the ABI
+    unsigned long long h[32];
+    if (cudaMemcpyFromSymbol(h, mvs::g_sdf_clk, sizeof(h)) != cudaSuccess) return -1;
+    for (int i = 0; i < n && i < 32; ++i) out[i] = h[i];
+    if (reset) {
+        for (int i = 0; i < 32; ++i) h[i] = 0;
+        if (cudaMemcpyToSymbol(mvs::g_sdf_clk, h, sizeof(h)) != cudaSuccess) return -1;
+    }
+    return 0;
+}
+#endif

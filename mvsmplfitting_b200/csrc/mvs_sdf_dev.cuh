@@ -6,11 +6,17 @@
 #include "mvs_sdf_geom.cuh"
 #include "mvs_sdf_bins.cuh"
 
+// A translation unit may define SDF_MARK(i) before including this file (clock instrumentation of sdf_fused_body, see
+// scripts/sdf_phase_times.py); default: nothing.
+#ifndef SDF_MARK
+#define SDF_MARK(i) do {} while (0)
+#endif
+
 namespace mvs {
 
 // ---------------------------------------------------------------------------------- dense regime, v4: fused adjoint
-// sdf_fused_kernel: P CTAs per frame, 1, 2 or 4 blocks of 256 vertices each.  Per CTA: fold the skinning kernel's box partials (all
-// threads), sample phi at the <= 8 voxels around each vertex, compact the vertices with a non-zero sample gradient
+// sdf_fused_kernel: P CTAs per frame, 1 to kSdfMaxPasses blocks of 256 vertices each.  Per CTA: load the frame's set-up record
+// (box, triangle 0, cone / plane, chunk-cull verdicts; written once per frame by the skinning kernel), sample phi at the <= 8 voxels around each vertex, compact the vertices with a non-zero sample gradient
 // (deterministic order: warp, pass, lane) and -- because with the as-written semantics that list holds a handful of
 // vertices -- run the adjoint of the vertex stage for exactly those vertices right here:
 //     d v_posed = T_3x3^T g,   dA_j += W[n,j] [g (x) v_posed | g],   dPhi += d v_posed . Qk[rows of n]
@@ -57,8 +63,6 @@ struct SdfBinsDev {
 // Shared-memory working set of sdf_fused_body (static in sdf_fused_kernel, a slice of the dynamic buffer in the persistent
 // dense-round kernel)
 struct SdfFusedSmem {
-    float s_wb[8][6];
-    int s_wi[8][6];
     float ctab[256];
     float s_red[kSdfMaxPasses][8][5];
     int s_wcnt[kSdfMaxPasses][8], s_woff[kSdfMaxPasses][9];
@@ -70,16 +74,15 @@ struct SdfFusedSmem {
     int c_n[kSdfFChunk];
     float c_dv[kSdfFChunk * 3], c_vp[kSdfFChunk * 3], c_dvp[kSdfFChunk * 3];
     float s_dphi[8][kFeatPad];
-    float s_ch[256][6];                    // the skinning kernel's per-64-vertex boxes (pre-transl lo | hi)
 };
 
-// verts / poffT / Phi / slot_tr / bboxp / At are rewritten every round by other CTAs of the persistent kernel: plain
-// pointers.  v_posed of the (few) listed vertices is recomputed from the pose offsets (vposed_of).
+// verts / poffT / Phi / slot_tr / setup / At are rewritten every round by the preceding kernels: plain pointers.  v_posed
+// of the (few) listed vertices is recomputed from the pose offsets (vposed_of).
 struct SdfFusedArgs {
     const float* verts; const float* poffT; const float* Phi; const float* ST; const float* slot_tr;
-    int N, nbox; const float* bboxp; const int* faces; int num_faces, f0, f1, f2, G;
+    int N, nbox; const SdfFrameSetup* setup; const int* faces; int num_faces, G;
     const float* At; int ldA; const int* ell_j; const float* ell_w; int KW; const float* Wd; const float* Qk;
-    float* parts5; float* part; int* pflag; FrameBox* boxout; float* gcoord;
+    float* parts5; float* part; int* pflag; float* gcoord;
     SdfBinsDev bins;
 };
 
@@ -87,108 +90,52 @@ struct SdfFusedArgs {
 template <bool kAll>
 __device__ __forceinline__ void sdf_fused_body(SdfFusedSmem& sm, const SdfFusedArgs& ar, const int na, const int slot, const int pidx,
                                                const int passes) {
-    const float* verts = ar.verts; const float* slot_tr = ar.slot_tr; const float* bboxp = ar.bboxp;
-    const int N = ar.N, nbox = ar.nbox, num_faces = ar.num_faces, f0 = ar.f0, f1 = ar.f1, f2 = ar.f2, G = ar.G, ldA = ar.ldA, KW = ar.KW;
+    const float* verts = ar.verts; const float* slot_tr = ar.slot_tr;
+    const int N = ar.N, nbox = ar.nbox, num_faces = ar.num_faces, G = ar.G, ldA = ar.ldA, KW = ar.KW;
     const int* __restrict__ faces = ar.faces; const float* At = ar.At;
     const int* __restrict__ ell_j = ar.ell_j; const float* __restrict__ ell_w = ar.ell_w;
     const float* __restrict__ Wd = ar.Wd; const float* __restrict__ Qk = ar.Qk;
-    float* parts5 = ar.parts5; float* part = ar.part; int* pflag = ar.pflag; FrameBox* boxout = ar.boxout; float* gcoord = ar.gcoord;
-    auto& s_wb = sm.s_wb; auto& s_wi = sm.s_wi; auto& ctab = sm.ctab; auto& s_red = sm.s_red; auto& s_wcnt = sm.s_wcnt;
+    float* parts5 = ar.parts5; float* part = ar.part; int* pflag = ar.pflag; float* gcoord = ar.gcoord;
+    auto& ctab = sm.ctab; auto& s_red = sm.s_red; auto& s_wcnt = sm.s_wcnt;
     auto& s_woff = sm.s_woff; auto& s_mask = sm.s_mask; auto& seg_n = sm.seg_n; auto& seg_g = sm.seg_g; auto& sA = sm.sA;
-    auto& c_n = sm.c_n; auto& c_dv = sm.c_dv; auto& c_vp = sm.c_vp; auto& c_dvp = sm.c_dvp; auto& s_dphi = sm.s_dphi; auto& s_ch = sm.s_ch;
+    auto& c_n = sm.c_n; auto& c_dv = sm.c_dv; auto& c_vp = sm.c_vp; auto& c_dvp = sm.c_dvp; auto& s_dphi = sm.s_dphi;
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    // every load of the prologue is addressed by the slot alone (no slot -> frame -> state chain): one round trip
-    const float* vf = verts + (size_t)slot * N * 3;
-    const float4 tr4 = *reinterpret_cast<const float4*>(slot_tr + 4 * slot);
-    float traw[9];
-    {
-        const int fid[3] = {f0, f1, f2};
-#pragma unroll
-        for (int q = 0; q < 9; ++q) traw[q] = vf[3 * fid[q / 3] + q % 3];
-    }
     if (slot >= na) return;
     if (pidx * passes * kSdfFThreads >= N) return;
-    const float tr[3] = {tr4.x, tr4.y, tr4.z};
-    // ---- bounding box: every thread takes one partial, warps fold with shuffles (ties -> lowest vertex index)
-    {
-        float lo[3] = {3e38f, 3e38f, 3e38f}, hi[3] = {-3e38f, -3e38f, -3e38f};
-        int ilo[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff}, ihi[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff};
-        for (int tl = t; tl < nbox; tl += kSdfFThreads) {
-            const float* bp = bboxp + ((size_t)slot * nbox + tl) * 12;
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const float l2 = bp[c], h2 = bp[3 + c];
-                const int il2 = __float_as_int(bp[6 + c]), ih2 = __float_as_int(bp[9 + c]);
-                if (l2 < lo[c] || (l2 == lo[c] && il2 < ilo[c])) { lo[c] = l2; ilo[c] = il2; }
-                if (h2 > hi[c] || (h2 == hi[c] && ih2 < ihi[c])) { hi[c] = h2; ihi[c] = ih2; }
-                if (tl < 256) { s_ch[tl][c] = l2; s_ch[tl][3 + c] = h2; }
-            }
-        }
-#pragma unroll
-        for (int c = 0; c < 3; ++c) { warp_argmin(lo[c], ilo[c]); warp_argmax(hi[c], ihi[c]); }
-        if (lane == 0) {
-#pragma unroll
-            for (int c = 0; c < 3; ++c) { s_wb[warp][c] = lo[c]; s_wb[warp][3 + c] = hi[c]; s_wi[warp][c] = ilo[c]; s_wi[warp][3 + c] = ihi[c]; }
-        }
-        if (t < G && t < 256) ctab[t] = (float)(-1 + (t + 0.5) * (double)(float)(2. / (G - 1)));   // voxel_centre, tabulated
-    }
-    __syncthreads();
-    // every warp folds the eight warp boxes itself (each lane holds one of them): no second barrier
-    FrameBox fb;
-    {
-        const int wsrc = lane & 7;
-        float lo[3], hi[3];
-        int ilo[3], ihi[3];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) { lo[c] = s_wb[wsrc][c]; hi[c] = s_wb[wsrc][3 + c]; ilo[c] = s_wi[wsrc][c]; ihi[c] = s_wi[wsrc][3 + c]; }
-#pragma unroll
-        for (int c = 0; c < 3; ++c) { warp_argmin(lo[c], ilo[c]); warp_argmax(hi[c], ihi[c]); }
-        float ext = -1.f;
-        fb.cmax = 0;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            // the partials are on pre-transl vertices; fl(v + tr) is monotone in v, so min/max and their
-            // arg-indices commute with the translation (body_models_scale.py:403)
-            const float lc = lo[c] + tr[c], hc = hi[c] + tr[c];
-            fb.centre[c] = (lc + hc) / 2.f;
-            fb.ilo[c] = ilo[c]; fb.ihi[c] = ihi[c];
-            const float e = hc - lc;
-            if (e > ext) { ext = e; fb.cmax = c; }
-        }
-        fb.scale = 0.6f * ext;
-        fb.pad = 0.f;
-        if (pidx == 0 && t == 0) boxout[slot] = fb;
-    }
-    // triangle 0 in box coordinates (fitting.py:362-363) and the cone it spans from the corner (-1,-1,-1): per thread,
-    // in registers (identical values in every thread)
-    float tri[9], cn[3][3], cm[3];
-#pragma unroll
-    for (int q = 0; q < 9; ++q) tri[q] = ((traw[q] + tr[q % 3]) - fb.centre[q % 3]) / fb.scale;
+    // ---- prologue: the frame's set-up (box, triangle 0, cone / plane, chunk-cull verdicts; computed once per frame by the
+    //      skinning kernel, sdf_frame_setup), its translation and this CTA's first vertices, all addressed by the slot alone:
+    //      one round trip
+    const SdfFrameSetup* rec = ar.setup + slot;
+    const float* vf = verts + (size_t)slot * N * 3;
+    const float4 tr4 = *reinterpret_cast<const float4*>(slot_tr + 4 * slot);
+    const FrameBox fb = rec->fb;
+    float cn[3][3], cm[3], pn[3], vpad[3];
 #pragma unroll
     for (int q = 0; q < 3; ++q) {
-        const float* a = &tri[3 * q];
-        const float* bb = &tri[3 * ((q + 1) % 3)];
-        const float ea[3] = {a[0] + 1.f, a[1] + 1.f, a[2] + 1.f}, eb[3] = {bb[0] + 1.f, bb[1] + 1.f, bb[2] + 1.f};
-        cn[q][0] = ea[1] * eb[2] - ea[2] * eb[1]; cn[q][1] = ea[2] * eb[0] - ea[0] * eb[2]; cn[q][2] = ea[0] * eb[1] - ea[1] * eb[0];
-        cm[q] = 3.5e-4f * sqrtf(cn[q][0] * cn[q][0] + cn[q][1] * cn[q][1] + cn[q][2] * cn[q][2]);
+        cn[q][0] = rec->cn[q][0]; cn[q][1] = rec->cn[q][1]; cn[q][2] = rec->cn[q][2];
+        cm[q] = rec->cm[q]; pn[q] = rec->pn[q]; vpad[q] = rec->vpad[q];
     }
-    // plane of triangle 0 in the same shifted coordinates (w = centre + 1, the corner is the origin): the ray from a
-    // voxel centre to the corner can only cross the triangle if the two lie on opposite sides of this plane, i.e.
-    // <pn, w> - pd has the sign of pd.  Voxels between the corner and the triangle pass the cone test but fail this one.
-    float pn[3], pd, pm;
+    const float pd = rec->pd, pm = rec->pm, vpadp = rec->vpadp;
+    const float* tri = rec->tri;                       // triangle 0 in box coordinates: read only by the (rare) exact voxel tests
+    // Chunk-level cull (sdf_frame_setup): lane p of a warp reads the verdict of the warp's 64-vertex chunk in pass p; the
+    // pass loop takes it with a shuffle.  A culled chunk's value and gradient are exactly zero: its warps skip loads,
+    // divisions, corners.
+    bool my_skip = false;
+    if (lane < passes) {
+        const int chunk = ((pidx * passes + lane) * kSdfFThreads + warp * 32) / 64;
+        if (chunk < nbox && chunk < 32 * kSdfSkipWords) my_skip = (rec->skip[chunk >> 5] >> (chunk & 31)) & 1u;
+    }
+    float vcur[3] = {0.f, 0.f, 0.f};                   // this pass' vertex; the next one is fetched a pass ahead
     {
-        const float e1[3] = {tri[3] - tri[0], tri[4] - tri[1], tri[5] - tri[2]}, e2[3] = {tri[6] - tri[0], tri[7] - tri[1], tri[8] - tri[2]};
-        pn[0] = e1[1] * e2[2] - e1[2] * e2[1]; pn[1] = e1[2] * e2[0] - e1[0] * e2[2]; pn[2] = e1[0] * e2[1] - e1[1] * e2[0];
-        pd = pn[0] * (tri[0] + 1.f) + pn[1] * (tri[1] + 1.f) + pn[2] * (tri[2] + 1.f);
-        pm = 2e-3f * sqrtf(pn[0] * pn[0] + pn[1] * pn[1] + pn[2] * pn[2]);      // conservative: |w| <= 2 sqrt 3, fp32 rounding
+        const int n0 = pidx * passes * kSdfFThreads + t;
+        if (n0 < N) { vcur[0] = vf[3 * n0]; vcur[1] = vf[3 * n0 + 1]; vcur[2] = vf[3 * n0 + 2]; }
     }
-    // vertex-level early-out: the 8 voxel centres a vertex at `loc` can touch lie within +-vhalf of (loc + 1) G/(G-1) on
-    // every axis, so each plane function varies by at most vhalf * |n|_1 over them
-    const float vgs = (float)G / (float)(G - 1), vhalf = 2.02f / (float)(G - 1) + 1e-5f;
-    float vpad[3];
-#pragma unroll
-    for (int q = 0; q < 3; ++q) vpad[q] = vhalf * (fabsf(cn[q][0]) + fabsf(cn[q][1]) + fabsf(cn[q][2]));
-    const float vpadp = vhalf * (fabsf(pn[0]) + fabsf(pn[1]) + fabsf(pn[2]));
+    if (t < G && t < 256) ctab[t] = (float)(-1 + (t + 0.5) * (double)(float)(2. / (G - 1)));   // voxel_centre, tabulated
+    const float tr[3] = {tr4.x, tr4.y, tr4.z};
+    const float vgs = (float)G / (float)(G - 1);
+    __syncthreads();
+    SDF_MARK(2);
+    SDF_MARK(3);
     // ---- sampling: block (pidx * passes + pass) of 256 vertices per pass, one vertex per thread and pass.  Sums,
     //      vertex lists and adjoint partials are emitted PER BLOCK, so the arithmetic of a frame does not depend on
     //      how many blocks this launch gave to one CTA (i.e. not on how many other frames are still active): frames
@@ -211,43 +158,6 @@ __device__ __forceinline__ void sdf_fused_body(SdfFusedSmem& sm, const SdfFusedA
     const bool cull = (num_faces == 1);
     const bool tab = (G <= 256);
     const int nblocks = (N + kSdfFThreads - 1) / kSdfFThreads;
-    // Chunk-level cull: the skinning kernel left the box of every 64 consecutive vertices.  The voxel centres a vertex
-    // at `loc` can touch lie within (loc + 1) G/(G-1) +- 2/(G-1) (+1 shifted); if that whole box is on the negative
-    // side of one cone plane and on the positive side of another, no vertex of the chunk can see a voxel with
-    // phi != 0: value and gradient are exactly zero and its two warps skip loads, divisions, corners.  Lane p of a
-    // warp tests the warp's chunk of pass p once; the pass loop reads the verdict with a shuffle.
-    bool my_skip = false;
-    if (lane < passes) {
-        const int chunk = ((pidx * passes + lane) * kSdfFThreads + warp * 32) / 64;
-        if (cull && nbox <= 256 && chunk < nbox) {
-            const float gs = (float)G / (float)(G - 1), pad = 2.02f / (float)(G - 1) + 1e-5f;
-            float wlo[3], whi[3];
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const float l_lo = ((s_ch[chunk][c] + tr[c]) - fb.centre[c]) / fb.scale;
-                const float l_hi = ((s_ch[chunk][3 + c] + tr[c]) - fb.centre[c]) / fb.scale;
-                wlo[c] = (l_lo + 1.f) * gs - pad; whi[c] = (l_hi + 1.f) * gs + pad;
-            }
-            bool all_neg = false, all_pos = false;
-#pragma unroll
-            for (int q = 0; q < 3; ++q) {
-                float smin = 0.f, smax = 0.f;
-#pragma unroll
-                for (int c = 0; c < 3; ++c) {
-                    const float a = cn[q][c] * wlo[c], b2 = cn[q][c] * whi[c];
-                    smin += fminf(a, b2); smax += fmaxf(a, b2);
-                }
-                all_neg = all_neg || (smax < -cm[q]);
-                all_pos = all_pos || (smin > cm[q]);
-            }
-            my_skip = all_neg && all_pos;
-        }
-    }
-    float vcur[3] = {0.f, 0.f, 0.f};                   // this pass' vertex; the next one is fetched a pass ahead
-    {
-        const int n0 = pidx * passes * kSdfFThreads + t;
-        if (n0 < N) { vcur[0] = vf[3 * n0]; vcur[1] = vf[3 * n0 + 1]; vcur[2] = vf[3 * n0 + 2]; }
-    }
 #pragma unroll 1
     for (int pass = 0; pass < passes; ++pass) {
         const int blk = pidx * passes + pass;
@@ -427,6 +337,7 @@ __device__ __forceinline__ void sdf_fused_body(SdfFusedSmem& sm, const SdfFusedA
         if (lane == 0) { s_wcnt[pass][warp] = __popc(nzm); s_mask[pass][warp] = nzm; }
     }
     __syncthreads();
+    SDF_MARK(4);
     if (t < 5 * passes) {
         const int pass = t / 5, q = t % 5, blk = pidx * passes + pass;
         if (blk < nblocks) {
@@ -544,6 +455,7 @@ __device__ __forceinline__ void sdf_fused_body(SdfFusedSmem& sm, const SdfFusedA
         }
     }
     __syncthreads();
+    SDF_MARK(5);
 }
 
 int ensure_sdf_fused_ws(mvs_ctx* ctx);                 // mvs_sdf.cu: allocates the dense-regime SDF scratch

@@ -270,11 +270,17 @@ static cudaError_t launch_gemm(mvs_ctx* ctx, const TcState* T, int inst, dim3 gr
                       3 * ctx->m.N, (const int*)w.na, ctx->sm_count, ntiles, T->poffT, T->err);
 }
 
-int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed) {
+int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool sdf_setup) {
     TcState* T = static_cast<TcState*>(ctx->tc);
     Workspace& w = ctx->ws;
     const DevModel& m = ctx->m;
     { const int rc = tc_prepare(ctx); if (rc) return rc; }
+    SdfSetupArgs sd{};
+    if (sdf_setup) {                                    // the skinning kernel also computes each frame's SDF set-up
+        const int rc = ensure_sdf_setup_ws(ctx, st);
+        if (rc) return rc;
+        sd = make_sdf_setup_args(ctx);
+    }
     const int nb = w.na_bound > 0 ? w.na_bound : w.B;             // upper bound of the active-frame count
     const int ntiles = (3 * m.N + kTcRows - 1) / kTcRows;
     const int nf = tc_cols_for(nb);
@@ -286,7 +292,7 @@ int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed) {
                                 : nf == 64 ? launch_gemm<64>(ctx, T, 3, grid, st, ntiles)
                                            : launch_gemm<128>(ctx, T, 4, grid, st, ntiles)));
     const int nchunks = (m.N + kSkinV - 1) / kSkinV, fgroups = (nb + 31) / 32;
-    const SkinArgs sa{T->poffT, m.ST, w.Phi, w.At, w.ldA, m.ell_j, m.ell_w, m.KW, m.N, need_vposed ? w.vposed : nullptr, w.verts, w.bboxp};
+    const SkinArgs sa{T->poffT, m.ST, w.Phi, w.At, w.ldA, m.ell_j, m.ell_w, m.KW, m.N, need_vposed ? w.vposed : nullptr, w.verts, w.bboxp, sd};
     if (nb <= kSkinSmallMax) {                          // straggler tail: lane = vertex, one chunk per CTA
         MVS_LAUNCH(ctx, KID_SKIN, st,
                    MVS_CUDA_OK(ctx, launch_pdl(skin_small_kernel, dim3(nchunks), dim3(kSkinSmallThreads), 0, st, sa, (const int*)w.na)));

@@ -231,7 +231,188 @@ struct SkinArgs {
     const float* poffT; const float* ST; const float* Phi; const float* At; int ldA;
     const int* ell_j; const float* ell_w; int KW; int N;
     float* vposed; float* verts; float* bboxp;
+    SdfSetupArgs sdf;
 };
+
+// ------------------------------------------------------------------------------------------------ per-frame SDF set-up
+// One warp computes frame `slot`'s SdfFrameSetup from the frame's nbox chunk boxes and skinned vertices, with the
+// expressions sdf_fused used to evaluate in every CTA: the box (ties -> lowest vertex index), triangle 0 in box coordinates
+// (fitting.py:362-363), the cone of planes it spans from the corner (-1,-1,-1), the plane of the triangle, the vertex-level
+// pads and the chunk-cull verdicts.  The chunk boxes and vertices were written by other CTAs of the same launch, so they are
+// read through L2 (__ldcg).  Resets the frame's arrival counter for the next round.
+static __device__ __noinline__ void sdf_frame_setup(const SdfSetupArgs sa, const float* bboxp, const float* verts, const int N,
+                                             const int nbox, const int slot, const int lane) {
+    const float tr[3] = {sa.slot_tr[4 * slot], sa.slot_tr[4 * slot + 1], sa.slot_tr[4 * slot + 2]};
+    const float* vf = verts + (size_t)slot * N * 3;
+    float traw[9];
+    {
+        const int fid[3] = {sa.f0, sa.f1, sa.f2};
+#pragma unroll
+        for (int q = 0; q < 9; ++q) traw[q] = __ldcg(vf + 3 * fid[q / 3] + q % 3);
+    }
+    // ---- bounding box: each lane folds its chunks in ascending order, the warp folds the lanes.  Chunks are loaded
+    //      kSetupCh per lane at a time, all loads in flight; the first group's boxes stay in registers for the verdicts.
+    constexpr int kSetupCh = 4;
+    float lo[3] = {3e38f, 3e38f, 3e38f}, hi[3] = {-3e38f, -3e38f, -3e38f};
+    int ilo[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff}, ihi[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff};
+    float cb[kSetupCh][6];                             // pre-transl lo | hi of chunks lane + 32 i
+#pragma unroll 1
+    for (int g0 = 0; g0 < nbox; g0 += 32 * kSetupCh) {
+        float bv[kSetupCh][12];
+#pragma unroll
+        for (int i = 0; i < kSetupCh; ++i) {
+            const int tl = g0 + 32 * i + lane;
+            const float* bp = bboxp + ((size_t)slot * nbox + min(tl, nbox - 1)) * 12;
+#pragma unroll
+            for (int e = 0; e < 12; ++e) bv[i][e] = __ldcg(bp + e);
+        }
+#pragma unroll
+        for (int i = 0; i < kSetupCh; ++i) {
+            if (g0 + 32 * i + lane >= nbox) break;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float l2 = bv[i][c], h2 = bv[i][3 + c];
+                const int il2 = __float_as_int(bv[i][6 + c]), ih2 = __float_as_int(bv[i][9 + c]);
+                if (l2 < lo[c] || (l2 == lo[c] && il2 < ilo[c])) { lo[c] = l2; ilo[c] = il2; }
+                if (h2 > hi[c] || (h2 == hi[c] && ih2 < ihi[c])) { hi[c] = h2; ihi[c] = ih2; }
+            }
+        }
+        if (g0 == 0) {
+#pragma unroll
+            for (int i = 0; i < kSetupCh; ++i)
+#pragma unroll
+                for (int e = 0; e < 6; ++e) cb[i][e] = bv[i][e];
+        }
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { warp_argmin(lo[c], ilo[c]); warp_argmax(hi[c], ihi[c]); }
+    FrameBox fb;
+    {
+        float ext = -1.f;
+        fb.cmax = 0;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            // the partials are on pre-transl vertices; fl(v + tr) is monotone in v, so min/max and their
+            // arg-indices commute with the translation (body_models_scale.py:403)
+            const float lc = lo[c] + tr[c], hc = hi[c] + tr[c];
+            fb.centre[c] = (lc + hc) / 2.f;
+            fb.ilo[c] = ilo[c]; fb.ihi[c] = ihi[c];
+            const float e = hc - lc;
+            if (e > ext) { ext = e; fb.cmax = c; }
+        }
+        fb.scale = 0.6f * ext;
+        fb.pad = 0.f;
+    }
+    // triangle 0 in box coordinates and the cone it spans from the corner (-1,-1,-1)
+    float tri[9], cn[3][3], cm[3];
+#pragma unroll
+    for (int q = 0; q < 9; ++q) tri[q] = ((traw[q] + tr[q % 3]) - fb.centre[q % 3]) / fb.scale;
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+        const float* a = &tri[3 * q];
+        const float* bb = &tri[3 * ((q + 1) % 3)];
+        const float ea[3] = {a[0] + 1.f, a[1] + 1.f, a[2] + 1.f}, eb[3] = {bb[0] + 1.f, bb[1] + 1.f, bb[2] + 1.f};
+        cn[q][0] = ea[1] * eb[2] - ea[2] * eb[1]; cn[q][1] = ea[2] * eb[0] - ea[0] * eb[2]; cn[q][2] = ea[0] * eb[1] - ea[1] * eb[0];
+        cm[q] = 3.5e-4f * sqrtf(cn[q][0] * cn[q][0] + cn[q][1] * cn[q][1] + cn[q][2] * cn[q][2]);
+    }
+    // plane of triangle 0 in the same shifted coordinates (w = centre + 1, the corner is the origin): the ray from a
+    // voxel centre to the corner can only cross the triangle if the two lie on opposite sides of this plane, i.e.
+    // <pn, w> - pd has the sign of pd.  Voxels between the corner and the triangle pass the cone test but fail this one.
+    float pn[3], pd, pm;
+    {
+        const float e1[3] = {tri[3] - tri[0], tri[4] - tri[1], tri[5] - tri[2]}, e2[3] = {tri[6] - tri[0], tri[7] - tri[1], tri[8] - tri[2]};
+        pn[0] = e1[1] * e2[2] - e1[2] * e2[1]; pn[1] = e1[2] * e2[0] - e1[0] * e2[2]; pn[2] = e1[0] * e2[1] - e1[1] * e2[0];
+        pd = pn[0] * (tri[0] + 1.f) + pn[1] * (tri[1] + 1.f) + pn[2] * (tri[2] + 1.f);
+        pm = 2e-3f * sqrtf(pn[0] * pn[0] + pn[1] * pn[1] + pn[2] * pn[2]);      // conservative: |w| <= 2 sqrt 3, fp32 rounding
+    }
+    // vertex-level early-out: the 8 voxel centres a vertex at `loc` can touch lie within +-vhalf of (loc + 1) G/(G-1) on
+    // every axis, so each plane function varies by at most vhalf * |n|_1 over them
+    const int G = sa.G;
+    const float vhalf = 2.02f / (float)(G - 1) + 1e-5f;
+    float vpad[3];
+#pragma unroll
+    for (int q = 0; q < 3; ++q) vpad[q] = vhalf * (fabsf(cn[q][0]) + fabsf(cn[q][1]) + fabsf(cn[q][2]));
+    const float vpadp = vhalf * (fabsf(pn[0]) + fabsf(pn[1]) + fabsf(pn[2]));
+    SdfFrameSetup* rec = sa.rec + slot;
+    // Chunk-level cull: the voxel centres a vertex at `loc` can touch lie within (loc + 1) G/(G-1) +- 2/(G-1) (+1
+    // shifted); if the whole box of a 64-vertex chunk is on the negative side of one cone plane and on the positive side
+    // of another, no vertex of the chunk can see a voxel with phi != 0: value and gradient are exactly zero.
+    const bool cull = sa.cull && nbox <= 32 * kSdfSkipWords;
+#pragma unroll 1
+    for (int k = 0; k < kSdfSkipWords; ++k) {
+        const int chunk = 32 * k + lane;
+        bool skip = false;
+        if (cull && chunk < nbox) {
+            float bx[6];
+            if (k < kSetupCh) {
+#pragma unroll
+                for (int e = 0; e < 6; ++e) bx[e] = cb[0][e];
+#pragma unroll
+                for (int i = 1; i < kSetupCh; ++i)
+                    if (k == i)
+#pragma unroll
+                        for (int e = 0; e < 6; ++e) bx[e] = cb[i][e];
+            } else {
+                const float* bp = bboxp + ((size_t)slot * nbox + chunk) * 12;
+#pragma unroll
+                for (int e = 0; e < 6; ++e) bx[e] = __ldcg(bp + e);
+            }
+            const float gs = (float)G / (float)(G - 1), pad = 2.02f / (float)(G - 1) + 1e-5f;
+            float wlo[3], whi[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float l_lo = ((bx[c] + tr[c]) - fb.centre[c]) / fb.scale;
+                const float l_hi = ((bx[3 + c] + tr[c]) - fb.centre[c]) / fb.scale;
+                wlo[c] = (l_lo + 1.f) * gs - pad; whi[c] = (l_hi + 1.f) * gs + pad;
+            }
+            bool all_neg = false, all_pos = false;
+#pragma unroll
+            for (int q = 0; q < 3; ++q) {
+                float smin = 0.f, smax = 0.f;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    const float a = cn[q][c] * wlo[c], b2 = cn[q][c] * whi[c];
+                    smin += fminf(a, b2); smax += fmaxf(a, b2);
+                }
+                all_neg = all_neg || (smax < -cm[q]);
+                all_pos = all_pos || (smin > cm[q]);
+            }
+            skip = all_neg && all_pos;
+        }
+        const unsigned bits = __ballot_sync(0xffffffffu, skip);
+        if (lane == 0) rec->skip[k] = bits;
+    }
+    if (lane == 0) {
+        rec->fb = fb;
+#pragma unroll
+        for (int q = 0; q < 9; ++q) rec->tri[q] = tri[q];
+#pragma unroll
+        for (int q = 0; q < 3; ++q) {
+            rec->cn[q][0] = cn[q][0]; rec->cn[q][1] = cn[q][1]; rec->cn[q][2] = cn[q][2];
+            rec->cm[q] = cm[q]; rec->pn[q] = pn[q]; rec->vpad[q] = vpad[q];
+        }
+        rec->pd = pd; rec->pm = pm; rec->vpadp = vpadp;
+        rec->unused[0] = 0.f; rec->unused[1] = 0.f;
+        sa.boxout[slot] = fb;
+        sa.arrive[slot] = 0;
+    }
+}
+
+// Arrival protocol of the skinning kernels (SDF term on).  Every CTA has written its chunk boxes and vertices; each thread
+// fences its own writes (__threadfence: visible device-wide before anything it does later), the CTA barrier orders all of
+// them before the one atomicAdd per frame that adds the CTA's chunk count to the frame's counter.  Exactly one CTA sees its
+// add complete the frame's nbox: every other CTA's fence-then-add precedes it in the counter's modification order, so
+// after its own fence that CTA reads every chunk box and vertex of the frame (through L2).  It computes the set-up and
+// puts the counter back to 0; nothing else touches the counter before the next round's skinning launch.
+// `mine`: frames whose set-up this CTA computes (bit i = frame base + i), from the caller's adds; `nwarps` warps share them.
+__device__ __forceinline__ void sdf_setup_frames(const SdfSetupArgs& sa, const float* bboxp, const float* verts, const int N,
+                                                 const int nbox, const int base, unsigned mine, const int warp, const int lane,
+                                                 const int nwarps) {
+    if (!mine) return;
+    __threadfence();
+    for (int k = 0; mine; mine &= mine - 1, ++k)
+        if (k % nwarps == warp) sdf_frame_setup(sa, bboxp, verts, N, nbox, base + __ffs(mine) - 1, lane);
+}
 
 // skin_kernel's CTA (vbx, vby) of a virtual grid (nchunks, frame groups); `sk` = kSkinSmem bytes of shared memory.
 // All kSkinThreads threads must call.
@@ -354,6 +535,22 @@ __device__ __forceinline__ void skin_body(float* sk, const SkinArgs& ar, const i
             for (int r = 0; r < 3; ++r) { bp[r] = lo[r]; bp[3 + r] = hi[r]; bp[6 + r] = __int_as_float(ilo[r]); bp[9 + r] = __int_as_float(ihi[r]); }
         }
     }
+    if (ar.sdf.rec != nullptr) {                          // per-frame SDF set-up by the last CTA of each frame (sdf_setup_frames)
+        __threadfence();
+        __syncthreads();
+        unsigned* s_mine = reinterpret_cast<unsigned*>(Bb);   // staging buffers are free once every thread is here
+        if (warp == 0) {
+            bool last = false;
+            if (f0 + lane < na) {
+                const int cnt = (nchunks - vbx + nx - 1) / nx;                    // chunks this CTA skinned for each frame
+                last = atomicAdd(ar.sdf.arrive + f0 + lane, cnt) + cnt == nchunks;
+            }
+            const unsigned m = __ballot_sync(0xffffffffu, last);
+            if (lane == 0) *s_mine = m;
+        }
+        __syncthreads();
+        sdf_setup_frames(ar.sdf, bboxp, verts, N, nchunks, f0, *s_mine, warp, lane, kSkinThreads / 32);
+    }
     __syncthreads();
 }
 
@@ -369,6 +566,7 @@ struct SkinSmallSmem {
     float Bs[kSkinSmallMax][kBetas];
     float s_b[kSkinSmallMax][6];
     int s_i[kSkinSmallMax][6];
+    unsigned mine;                         // frames whose SDF set-up this CTA computes
 };
 
 // skin_small_kernel's CTA for one 64-vertex chunk, executed by the kSkinSmallThreads threads t = 0..63 of a thread group
@@ -432,6 +630,17 @@ __device__ __forceinline__ void skin_small_body(SkinSmallSmem& sm, const SkinArg
                 }
             }
         }
+    }
+    if (ar.sdf.rec != nullptr) {                          // per-frame SDF set-up by the last CTA of each frame (sdf_setup_frames)
+        __threadfence();
+        asm volatile("bar.sync %0, %1;" ::"r"(bar), "r"(kSkinSmallThreads) : "memory");
+        if (warp == 0) {
+            const bool last = lane < na && atomicAdd(ar.sdf.arrive + lane, 1) + 1 == nchunks;   // one chunk per CTA
+            const unsigned m = __ballot_sync(0xffffffffu, last);
+            if (lane == 0) sm.mine = m;
+        }
+        asm volatile("bar.sync %0, %1;" ::"r"(bar), "r"(kSkinSmallThreads) : "memory");
+        sdf_setup_frames(ar.sdf, bboxp, verts, N, nchunks, 0, sm.mine, warp, lane, kSkinSmallThreads / 32);
     }
 }
 
