@@ -42,6 +42,9 @@ template int dev_alloc<float>(mvs_ctx*, float**, size_t);
 template int dev_alloc<int>(mvs_ctx*, int**, size_t);
 template int dev_alloc<double>(mvs_ctx*, double**, size_t);
 template int dev_alloc<unsigned char>(mvs_ctx*, unsigned char**, size_t);
+template int dev_alloc<int2>(mvs_ctx*, int2**, size_t);
+template int dev_alloc<FrameBox>(mvs_ctx*, FrameBox**, size_t);
+template int dev_alloc<SdfFrameSetup>(mvs_ctx*, SdfFrameSetup**, size_t);
 template int dev_upload<float>(mvs_ctx*, float**, const float*, size_t);
 template int dev_upload<int>(mvs_ctx*, int**, const int*, size_t);
 

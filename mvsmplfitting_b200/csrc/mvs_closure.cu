@@ -337,7 +337,7 @@ vertex_bwd_kernel(const float* __restrict__ Qk, const float* __restrict__ At, in
                   const int* __restrict__ ell_j, const float* __restrict__ ell_w, int KW,
                   const float* __restrict__ Wd, const int* __restrict__ blist_n, const int* __restrict__ blist_pos,
                   int nvb, int nv_fwd, const float* __restrict__ vposed, const float* __restrict__ dv,
-                  const int* __restrict__ na_ptr, int tiles_per_strip, int ntiles, float* __restrict__ part) {
+                  const int* __restrict__ na_ptr, int ntiles, float* __restrict__ part) {
     extern __shared__ __align__(16) float smem[];
     float* DV = smem;                          // [96][65]   upstream d loss / d vertex, column-major
     float* VP = DV + kTileC * kDvLd;           // [96][65]   v_posed
@@ -368,7 +368,6 @@ vertex_bwd_kernel(const float* __restrict__ Qk, const float* __restrict__ At, in
     // strided tile -> strip map: neighbouring tiles (e.g. the three keypoint-support tiles that always carry
     // gradient) land in different CTAs instead of serialising inside one
     const int nstrips_g = gridDim.x;
-    (void)tiles_per_strip;
     for (int tile = strip; tile < ntiles; tile += nstrips_g) {
         const int v0 = tile * kTileV;
         __syncthreads();
@@ -760,11 +759,11 @@ int launch_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* gra
     MVS_LAUNCH(ctx, KID_FRAME_FWD, st,
                frame_fwd_kernel<<<B, kFrameThreads, 0, st>>>(x_dev, w.fidx, w.na, par, m.Jt, m.JS, w.Phi, w.PhiTc, w.At, w.ldA,
                                                              w.gchain, w.slot_tr));
-    if (dense) {
-        // with the SDF term this chain is the plain-fp32 cross-check of the dense-regime kernels: the sampled distances are
-        // voxel-sized numbers, TF32 pose offsets would cost them 1e-5 .. 1e-4 relative (the dense-regime kernels re-evaluate
-        // the vertices that matter in fp32 instead, mvs_sdf_dev.cuh)
-        int rc = launch_vertex_fwd_dense(ctx, st, !sdf_on);
+    // with the SDF term this chain is the plain-fp32 cross-check of the dense-regime kernels: the sampled distances are
+    // voxel-sized numbers, TF32 pose offsets would cost them 1e-5 .. 1e-4 relative (the dense-regime kernels re-evaluate
+    // the vertices that matter in fp32 instead, mvs_sdf_dev.cuh)
+    if (dense && !sdf_on && tc_available(ctx)) {
+        int rc = launch_vertex_fwd_tc(ctx, st, true, false);       // wgmma / TMA path (mvs_tc.cu)
         if (rc) return rc;
     } else {
         dim3 g2((nv + kTileV - 1) / kTileV, ftiles);
@@ -809,7 +808,7 @@ int launch_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* gra
         MVS_LAUNCH(ctx, KID_VERTEX_BWD, st,
                    vertex_bwd_kernel<<<g4, kVertThreads, kVertBwdSmem, st>>>(m.Qk, w.At, w.ldA, m.ell_j, m.ell_w, m.KW, m.Wd,
                                                                              blist_n, blist_pos, nvb, nv, w.vposed, w.dv,
-                                                                             w.na, tps, ntiles, w.part));
+                                                                             w.na, ntiles, w.part));
     }
     PriorModel pm{m.M, m.gmm_means, m.gmm_prec, m.gmm_lognllw};
     MVS_LAUNCH(ctx, KID_FRAME_BWD, st,
@@ -831,25 +830,6 @@ int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st) {
     MVS_LAUNCH(ctx, KID_FRAME_FWD, st,
                frame_fwd_kernel<<<w.na_bound > 0 ? w.na_bound : w.B, kFrameThreads, 0, st>>>(x_dev, w.fidx, w.na, ctx->parents, m.Jt,
                                                               m.JS, w.Phi, w.PhiTc, w.At, w.ldA, w.gchain, w.slot_tr));
-    MVS_CUDA_OK(ctx, cudaGetLastError());
-    return MVS_OK;
-}
-
-// need_vposed = false: the caller's consumers recompute v_posed where they need it (the dense rounds: sdf_fused / frame_step read
-// ST . [beta; 1] + pose offsets for their few vertices), so the skinning kernel does not write the [B][N][3] array at all
-int launch_vertex_fwd_dense(mvs_ctx* ctx, cudaStream_t st, bool allow_tc, bool need_vposed, bool sdf_setup) {
-    DevModel& m = ctx->m;
-    Workspace& w = ctx->ws;
-    if (allow_tc && tc_available(ctx)) return launch_vertex_fwd_tc(ctx, st, need_vposed, sdf_setup);     // wgmma / TMA path (mvs_tc.cu)
-    if (!ctx->attr_done) {
-        MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertFwdSmem));
-        MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertBwdSmem));
-        ctx->attr_done = true;
-    }
-    dim3 g2((m.N + kTileV - 1) / kTileV, (w.B + kTileF - 1) / kTileF);
-    MVS_LAUNCH(ctx, KID_VERTEX_FWD, st,
-               vertex_fwd_kernel<<<g2, kVertThreads, kVertFwdSmem, st>>>(m.Qk, w.Phi, w.At, w.ldA, m.ell_j, m.ell_w, m.KW,
-                                                                         nullptr, m.N, w.na, w.vposed, w.verts));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }

@@ -82,6 +82,14 @@ struct DevModel {
     float *vp_b1 = nullptr, *vp_b2 = nullptr, *vp_b3 = nullptr;
 };
 
+struct FrameBox;
+struct SdfFrameSetup;
+// optimiser state and configuration (mvs_lbfgs_core.cuh), tensor-core path state (mvs_tc.cu)
+struct LbfgsState;
+struct LbfgsCfg;
+struct FrameScalars;
+struct TcState;
+
 // Per-batch workspace (slot-indexed: slot = position in the active-frame list)
 struct Workspace {
     int B = 0, ldA = 0;               // ldA = B rounded up to kTileF
@@ -113,8 +121,7 @@ struct Workspace {
     float* anchor = nullptr;          // [B][86] quadratic anchor (sequence mode)
     float* anchor_w = nullptr;        // [B][86]
     // SDF scratch
-    float* bbox_part = nullptr;       // [B][nbt][6]
-    float* sdf_frame = nullptr;       // [B][16]  centre(3) scale(1) argmin/argmax ids etc.
+    FrameBox* sdf_frame = nullptr;    // [B] frame boxes of the batched chain's SDF term (launch_sdf_terms)
     float* sdf_gcoord = nullptr;      // [B][N][3]
     float* sdf_valpart = nullptr;     // [B][nbt]
     float* bboxp = nullptr;           // [B][nchunks][12] per-chunk bbox partials written by the skinning kernel
@@ -122,8 +129,8 @@ struct Workspace {
     float* sdf_parts5 = nullptr;      // [B][P][5] per 256-vertex block: value, d value/d local (3), <d value/d local, local>
     float* sdf_part = nullptr;        // [B][P][512] unit-factor partial adjoints (288 skin | 224 feature)
     int* sdf_pflag = nullptr;         // [B][P] 1 iff the block has vertices with a non-zero sample gradient
-    unsigned char* sdf_box = nullptr; // [B] FrameBox
-    unsigned char* sdf_setup = nullptr;   // [B] SdfFrameSetup, written by the skinning kernel's last CTA of each frame
+    FrameBox* sdf_box = nullptr;      // [B] frame boxes of the dense rounds, written with the set-up, read by frame_step
+    SdfFrameSetup* sdf_setup = nullptr;   // [B] written by the skinning kernel's last CTA of each frame
     int* sdf_arrive = nullptr;        // [B] chunk boxes of the frame written so far this round (0 between rounds)
     // accelerated all-faces SDF (mvs_sdf_bins.cuh): per slot triangle corners, cell lists, ray-bin lists, meta (s_lo, s_scale, overflow)
     float* bins_tri = nullptr; int* bins_cell_ptr = nullptr; unsigned short* bins_cell_idx = nullptr;
@@ -203,12 +210,12 @@ struct mvs_ctx {
     int exec_mode = 0;               // 0 auto (frame-resident kernels where they apply), 1 batched kernels only
     bool have_model = false, have_cams = false, have_kp = false, have_loss = false;
     std::vector<void*> allocs;       // everything cudaMalloc'ed, freed in mvs_destroy
-    void* lbfgs = nullptr;           // optimiser state (mvs_lbfgs.cu)
+    mvs::LbfgsState* lbfgs = nullptr;    // optimiser state (mvs_lbfgs.cu)
     mvs::Profiler prof;
-    void* tc = nullptr;              // tensor-core path state (mvs_tc.cu)
+    mvs::TcState* tc = nullptr;          // tensor-core path state (mvs_tc.cu)
     float* rest_joints = nullptr;    // [K,3] keypoints of the rest pose at scale rest_scale (mvs_init.cu), computed once
     float rest_scale = -1.f;
-    int* stage_rng = nullptr;        // [B][2] per-frame slice of the stage table (mvs_fit_seq), device
+    int2* stage_rng = nullptr;       // [B] per-frame slice of the stage table (mvs_fit_seq), device
 };
 
 namespace mvs {
@@ -298,12 +305,11 @@ int launch_vposer_decode(mvs_ctx* ctx, const float* x_dev, float* body_pose_dev,
 int launch_closure_resident(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev,
                             float* proj_dev, cudaStream_t st);
 bool resident_lbfgs_available(const mvs_ctx* ctx, int history);
-int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const void* lbfgs_cfg, int history, const void* lp_tab_dev,
-                          const void* lp_tab_host, int nstages, void* frame_scalars_out, float* last_grad_dev, cudaStream_t st,
-                          const void* stage_rng_dev = nullptr);
+int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
+                          const LossParams* lp_tab_host, int nstages, FrameScalars* frame_scalars_out, float* last_grad_dev,
+                          cudaStream_t st, const int2* stage_rng_dev);
 // dense regime (SDF term): per round  posedirs_gemm_tc -> skin -> sdf_fused -> frame_step
 bool hybrid_available(const mvs_ctx* ctx);
-int launch_vertex_fwd_dense(mvs_ctx* ctx, cudaStream_t st, bool allow_tc = true, bool need_vposed = true, bool sdf_setup = false);                                   // mvs_closure.cu
 int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);                      // mvs_closure.cu
 int launch_sdf_fused(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu
 int ensure_sdf_setup_ws(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu: set-up records, arrival counters (zeroed on st), boxes
@@ -311,14 +317,13 @@ SdfSetupArgs make_sdf_setup_args(mvs_ctx* ctx);          // mvs_sdf.cu
 // mvs_tc.cu: wgmma / TMA dense vertex forward
 int tc_upload_model(mvs_ctx* ctx);                 // after m.Qk is on the device
 bool tc_available(const mvs_ctx* ctx);
-int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed = true, bool sdf_setup = false);
+int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool sdf_setup);
 int tc_check_error(mvs_ctx* ctx);
 float* tc_poffT(mvs_ctx* ctx);                 // [3N][ldA] pose offsets of the tensor-core contraction (allocated on first use)
 int tc_prepare(mvs_ctx* ctx);                  // tensor maps + pose-offset buffer (idempotent)
-int launch_frame_step(mvs_ctx* ctx, float* params_dev, const void* lbfgs_state, const void* lbfgs_cfg, int nstages,
-                      cudaStream_t st);
+int launch_frame_step(mvs_ctx* ctx, float* params_dev, const LbfgsState& L, const LbfgsCfg& cfg, int nstages, cudaStream_t st);
 int frame_step_begin_run(mvs_ctx* ctx, cudaStream_t st);                 // mvs_resident.cu
-int launch_frame_fwd_dense(mvs_ctx* ctx, const float* x_dev, const void* lbfgs_state, int nstages, cudaStream_t st);   // mvs_resident.cu
+int launch_frame_fwd_dense(mvs_ctx* ctx, const float* x_dev, const LbfgsState& L, int nstages, cudaStream_t st);   // mvs_resident.cu
 bool resident_lbfgs_available_for(const mvs_ctx* ctx, const LossParams& lp, int history);
 bool hybrid_available_for(const mvs_ctx* ctx, const LossParams& lp);
 int dense_regime_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, cudaStream_t st);   // mvs_lbfgs.cu

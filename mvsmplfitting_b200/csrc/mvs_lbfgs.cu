@@ -137,7 +137,7 @@ __global__ void iota2_kernel(int* p, int n, int* na) {
 }
 
 static int ensure_state(mvs_ctx* ctx, int H) {
-    LbfgsState* S = static_cast<LbfgsState*>(ctx->lbfgs);
+    LbfgsState* S = ctx->lbfgs;
     const int B = ctx->ws.B;
     if (S && S->B == B && S->H == H) return MVS_OK;
     if (S) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_run: history_size changed between calls (%d -> %d)", S->H, H);
@@ -175,51 +175,191 @@ static int ensure_state(mvs_ctx* ctx, int H) {
     return MVS_OK;
 }
 
-// Runs the stages lps[0 .. nst) (nst == 1: ctx->loss).  nst > 1 requires that all of them run in the same regime
-// (frame-resident or dense rounds, see run_fit): every frame then walks through the stages at its own pace.
-static int run_stage(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, const mvs_lbfgs_config* c,
-                     mvs_lbfgs_stats* stats, cudaStream_t st, int step_mode = 0, int reset = 1,
-                     float* last_grad_dev = nullptr, const LossParams* lps = nullptr, int nst = 1,
-                     const int2* stage_rng = nullptr, bool some_inactive = false) {
-    const int B = ctx->ws.B;
+// What a run does beyond its optimiser configuration.  The defaults are one mvs_lbfgs_run: a fresh optimiser for the stage
+// in ctx->loss, every frame active.
+struct RunOpts {
+    bool step = false;                // one LBFGS.step() per call, state kept in the context (mvs_lbfgs_step)
+    bool reset = true;                // false: the next step() of the same optimiser (lbfgs_init_kernel)
+    float* last_grad = nullptr;       // [B][86] gradient at the last evaluated point
+    const LossParams* lps = nullptr;  // stage table lps[0 .. nst); nullptr: ctx->loss alone
+    int nst = 1;
+    const int2* stage_rng = nullptr;  // [B] per-frame slice of the stage table (mvs_fit_seq); nullptr: all of it
+    bool some_inactive = false;       // some frame has no stage in this run
+};
+
+enum Regime { kResident, kDense, kBatched };
+
+// Shared set-up of a run: optimiser configuration, state for history size H, zeroed totals, stage table on the device
+static int begin_run(mvs_ctx* ctx, const mvs_lbfgs_config* c, bool step, const LossParams* lps, int nst, LbfgsCfg* cfg,
+                     cudaStream_t st) {
     const int H = c->history_size > 0 ? c->history_size : 100;
     if (H > 128) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_run: history_size must be <= 128");
     int rc = ensure_state(ctx, H);
     if (rc) return rc;
-    LbfgsState& S = *static_cast<LbfgsState*>(ctx->lbfgs);
-    LbfgsCfg cfg;
-    cfg.max_outer = c->max_outer > 0 ? c->max_outer : 30;
-    cfg.max_iter = c->max_iter > 0 ? c->max_iter : 30;
-    cfg.max_eval = c->max_eval > 0 ? c->max_eval : cfg.max_iter * 5 / 4;
-    cfg.history = H;
-    cfg.max_ls = 25;                                            // _strong_Wolfe default (lbfgs_ls.py:41)
-    cfg.step_mode = step_mode;
-    cfg.lr = c->lr > 0.f ? c->lr : 1.f;
-    cfg.tol_grad = c->tolerance_grad; cfg.tol_change = c->tolerance_change;
-    cfg.ftol = (double)c->ftol; cfg.gtol = (double)c->gtol;
-
-    Workspace& w = ctx->ws;
+    LbfgsState& S = *ctx->lbfgs;
+    cfg->max_outer = c->max_outer > 0 ? c->max_outer : 30;
+    cfg->max_iter = c->max_iter > 0 ? c->max_iter : 30;
+    cfg->max_eval = c->max_eval > 0 ? c->max_eval : cfg->max_iter * 5 / 4;
+    cfg->history = H;
+    cfg->max_ls = 25;                                           // _strong_Wolfe default (lbfgs_ls.py:41)
+    cfg->step_mode = step ? 1 : 0;
+    cfg->lr = c->lr > 0.f ? c->lr : 1.f;
+    cfg->tol_grad = c->tolerance_grad; cfg->tol_change = c->tolerance_change;
+    cfg->ftol = (double)c->ftol; cfg->gtol = (double)c->gtol;
     MVS_CUDA_OK(ctx, cudaMemsetAsync(S.totals, 0, 4 * sizeof(long long), st));
-    if (!lps) { lps = &ctx->loss; nst = 1; }
     if (nst > kMaxStages) return set_error(ctx, MVS_ERR_INVALID, "at most %d stages per run", kMaxStages);
     // stage table for the multi-stage kernels (the previous run ended with a stream synchronisation, so the pinned
     // staging copy is free)
     for (int i = 0; i < nst; ++i) S.lp_tab_host[i] = lps[i];
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(S.lp_tab, S.lp_tab_host, (size_t)nst * sizeof(LossParams), cudaMemcpyHostToDevice, st));
-    if (!step_mode && resident_lbfgs_available(ctx, H)) {
-        // sparse regime: every frame runs its whole stage inside one CTA (mvs_resident.cu): one launch, no rounds
-        rc = launch_lbfgs_resident(ctx, params_dev, &cfg, H, S.lp_tab, lps, nst, S.sc, last_grad_dev, st, stage_rng);
-        if (rc) return rc;
-        MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_finalize_kernel<<<(B + 255) / 256, 256, 0, st>>>(S, B, final_loss_dev, S.totals, 1));
-        long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
-        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-        if (stats) {
-            stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
-            stats->rounds += (int)th[3];          // critical path: the largest per-frame evaluation count
+    return MVS_OK;
+}
+
+// Start of a dense run: pose forward of every active slot, frame_step's pose cache invalidated
+static int dense_begin(mvs_ctx* ctx, const LbfgsState& S, int nst, cudaStream_t st) {
+    const int rc = launch_frame_fwd_dense(ctx, S.x_eval, S, nst, st);
+    return rc ? rc : frame_step_begin_run(ctx, st);
+}
+
+// One dense round: pose blend shapes of the active frames (wgmma GEMM), skinning + box partials + each frame's SDF set-up,
+// the SDF term with the adjoint of its (short) vertex list, and the per-frame closure adjoint + optimiser step + next pose
+// forward
+static int dense_round(mvs_ctx* ctx, float* params_dev, const LbfgsState& S, const LbfgsCfg& cfg, int nst, cudaStream_t st) {
+    int rc;
+    if ((rc = launch_vertex_fwd_tc(ctx, st, false, true))) return rc;
+    if ((rc = launch_sdf_fused(ctx, st))) return rc;
+    return launch_frame_step(ctx, params_dev, S, cfg, nst, st);
+}
+
+// Dense regime (SDF term on): rounds of dense_round until no frame is active.  Finished frames are compacted out once per
+// chunk of rounds.
+static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int nst, cudaStream_t st) {
+    LbfgsState& S = *ctx->lbfgs;
+    Workspace& w = ctx->ws;
+    const int B = w.B;
+    const int chunk = 8;
+    const long long max_rounds = ((long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8) * nst;
+    long long rounds = 0;
+    int na_host = B;
+    static const bool trace_na = getenv("MVS_TRACE_NA") != nullptr;       // debugging aid: active-list size per chunk
+    // debugging aid: how long the host thread waited for the GPU inside the round loop (close to 0 = the GPU waits for the host)
+    static const bool trace_host = getenv("MVS_TRACE_HOST") != nullptr;
+    double blocked_us = 0.0;
+    const auto loop_t0 = std::chrono::steady_clock::now();
+    int rc = dense_begin(ctx, S, nst, st);
+    if (rc) return rc;
+    // The host only needs the active count to know when to stop, so chunk k+1 is enqueued BEFORE the count of
+    // chunk k is awaited (kernels exit at once when the list is empty): the GPU never idles on the host round trip.
+    if (!S.na_event[0]) {
+        // blocking sync: the host thread sleeps while it waits for a chunk (several contexts are driven by as many host
+        // threads; spinning ones would compete with the threads that have launches to enqueue)
+        MVS_CUDA_OK(ctx, cudaEventCreateWithFlags(&S.na_event[0], cudaEventDisableTiming | cudaEventBlockingSync));
+        MVS_CUDA_OK(ctx, cudaEventCreateWithFlags(&S.na_event[1], cudaEventDisableTiming | cudaEventBlockingSync));
+    }
+    int* na_slots = reinterpret_cast<int*>(S.na_host);           // [0], [1]: two chunks in flight
+    int pending = -1;                                             // chunk whose count has not been read yet
+    long long chunk_idx = 0;
+    w.na_bound = B;                                               // grids shrink with the (lagging) host view of the count
+    while (rounds < max_rounds) {
+        for (int r = 0; r < chunk; ++r) {
+            if ((rc = dense_round(ctx, params_dev, S, cfg, nst, st))) return rc;
+            ++rounds;
         }
-        MVS_CUDA_OK(ctx, cudaGetLastError());
-        return MVS_OK;
+        // compaction changes slot -> frame, so the surviving frames' Phi / transforms are rebuilt for their new slots
+        MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
+        if ((rc = launch_frame_fwd_dense(ctx, S.x_eval, S, nst, st))) return rc;
+        const int cur = (int)(chunk_idx & 1);
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(&na_slots[cur], w.na, sizeof(int), cudaMemcpyDeviceToHost, st));
+        MVS_CUDA_OK(ctx, cudaEventRecord(S.na_event[cur], st));
+        if (pending >= 0) {
+            const auto tb0 = std::chrono::steady_clock::now();
+            MVS_CUDA_OK(ctx, cudaEventSynchronize(S.na_event[pending]));
+            if (trace_host) blocked_us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - tb0).count();
+            na_host = na_slots[pending];
+            if (trace_na) fprintf(stderr, "[mvs] dense regime: chunk %lld, active frames %d\n", chunk_idx - 1, na_host);
+            if (na_host <= 0) break;
+            w.na_bound = na_host;                                 // the list only shrinks: still an upper bound
+        }
+        pending = cur;
+        ++chunk_idx;
+    }
+    w.na_bound = B;
+    if (trace_host) {
+        const double enq = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - loop_t0).count();
+        const auto td0 = std::chrono::steady_clock::now();
+        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+        const double drain = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - td0).count();
+        fprintf(stderr, "[mvs] dense regime host loop: %lld rounds, %.0f us in the loop (%.0f us of it blocked on the GPU), %.0f us "
+                        "draining afterwards\n", rounds, enq, blocked_us, drain);
+    }
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    return tc_check_error(ctx);
+}
+
+// Batched chain: launch_closure + lbfgs_advance_kernel + lbfgs_compact_kernel per round, the host reads the active count
+// after every chunk of rounds
+static int run_batched(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, bool vp2, cudaStream_t st) {
+    LbfgsState& S = *ctx->lbfgs;
+    Workspace& w = ctx->ws;
+    const int B = w.B;
+    const int chunk = 8;
+    const long long max_rounds = (long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8;
+    long long rounds = 0;
+    int na_host = B;
+    while (na_host > 0 && rounds < max_rounds) {
+        for (int r = 0; r < chunk; ++r) {
+            const int rc = launch_closure(ctx, S.x_eval, S.loss_eval, S.g_eval, nullptr, nullptr, nullptr, st);
+            if (rc) return rc;
+            MVS_LAUNCH(ctx, KID_LBFGS_ADVANCE, st, lbfgs_advance_kernel<<<B, 32, 0, st>>>(S, cfg, params_dev, w.fidx, w.na, vp2 ? 32 : kOffTransl - kOffPose));
+            MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
+            ++rounds;
+        }
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(S.na_host, w.na, sizeof(int), cudaMemcpyDeviceToHost, st));
+        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+        na_host = *S.na_host;
+    }
+    return MVS_OK;
+}
+
+// End of a run: final losses and totals.  The frame-resident kernel wrote the last gradient itself and leaves the active
+// list alone; the round-based regimes copy the gradient and leave the context usable for plain closures (full active list).
+// The dense and frame-resident regimes report the largest per-frame evaluation count (the critical path) as rounds.
+static int end_run(mvs_ctx* ctx, Regime rg, float* final_loss_dev, float* last_grad_dev, mvs_lbfgs_stats* stats, cudaStream_t st) {
+    LbfgsState& S = *ctx->lbfgs;
+    Workspace& w = ctx->ws;
+    const int B = w.B;
+    MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_finalize_kernel<<<(B + 255) / 256, 256, 0, st>>>(S, B, final_loss_dev, S.totals, rg != kBatched));
+    if (rg != kResident && last_grad_dev)
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(last_grad_dev, S.g_eval, (size_t)B * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    if (rg != kResident) MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    if (stats) {
+        stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
+        stats->rounds += (int)th[3];
+        if (rg == kDense) { stats->dense_frame_evals += th[1]; stats->dense_rounds += (int)th[3]; }
+    }
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    return MVS_OK;
+}
+
+// Runs the stages o.lps[0 .. o.nst) (default: ctx->loss).  nst > 1 requires that all of them run in the same regime
+// (frame-resident or dense rounds, see run_fit): every frame then walks through the stages at its own pace.
+static int run_stage(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats,
+                     cudaStream_t st, const RunOpts& o) {
+    const LossParams* lps = o.lps ? o.lps : &ctx->loss;
+    const int nst = o.lps ? o.nst : 1;
+    LbfgsCfg cfg;
+    int rc = begin_run(ctx, c, o.step, lps, nst, &cfg, st);
+    if (rc) return rc;
+    LbfgsState& S = *ctx->lbfgs;
+    Workspace& w = ctx->ws;
+    const int B = w.B;
+    if (!o.step && resident_lbfgs_available(ctx, cfg.history)) {
+        // sparse regime: every frame runs its whole stage inside one CTA (mvs_resident.cu): one launch, no rounds
+        rc = launch_lbfgs_resident(ctx, params_dev, cfg, cfg.history, S.lp_tab, lps, nst, S.sc, o.last_grad, st, o.stage_rng);
+        return rc ? rc : end_run(ctx, kResident, final_loss_dev, nullptr, stats, st);
     }
     // use_vposer = 2 (VPoser decode on the device) exists in the frame-resident closure and in the dense-regime kernels, not in
     // the SIMT reference chain.  mvs_lbfgs_step therefore runs its one step() per call through the dense rounds when the SDF
@@ -230,120 +370,12 @@ static int run_stage(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, con
         return set_error(ctx, MVS_ERR_INVALID, "use_vposer = 2 (VPoser decode on the device) is not implemented in the batched "
                                                "reference chain (exec mode 1): use use_vposer = 1 there");
     MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-    MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_init_kernel<<<B, 32, 0, st>>>(S, params_dev, B, reset, nst, stage_rng));
-    if (some_inactive)                                      // frames without a stage in this run leave the active list now
+    MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_init_kernel<<<B, 32, 0, st>>>(S, params_dev, B, o.reset ? 1 : 0, nst, o.stage_rng));
+    if (o.some_inactive)                                    // frames without a stage in this run leave the active list now
         MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
-    if ((!step_mode || vp2) && hybrid_available(ctx)) {
-        // dense regime (SDF term on): four launches per round -- pose blend shapes of the active frames (wgmma
-        // GEMM), skinning + box partials, the SDF term with the adjoint of its (short) vertex list, and the per-frame
-        // closure adjoint + optimiser step + next pose forward.  Finished frames are compacted out once per chunk.
-        const int chunk = 8;
-        const long long max_rounds = ((long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8) * nst;
-        long long rounds = 0;
-        int na_host = B;
-        static const bool trace_na = getenv("MVS_TRACE_NA") != nullptr;       // debugging aid: active-list size per chunk
-        // debugging aid: how long the host thread waited for the GPU inside the round loop (close to 0 = the GPU waits for the host)
-        static const bool trace_host = getenv("MVS_TRACE_HOST") != nullptr;
-        double blocked_us = 0.0;
-        const auto loop_t0 = std::chrono::steady_clock::now();
-        rc = launch_frame_fwd_dense(ctx, S.x_eval, &S, nst, st);
-        if (rc) return rc;
-        if ((rc = frame_step_begin_run(ctx, st))) return rc;
-        // The host only needs the active count to know when to stop, so chunk k+1 is enqueued BEFORE the count of
-        // chunk k is awaited (kernels exit at once when the list is empty): the GPU never idles on the host round trip.
-        if (!S.na_event[0]) {
-            // blocking sync: the host thread sleeps while it waits for a chunk (several contexts are driven by as many host
-            // threads; spinning ones would compete with the threads that have launches to enqueue)
-            MVS_CUDA_OK(ctx, cudaEventCreateWithFlags(&S.na_event[0], cudaEventDisableTiming | cudaEventBlockingSync));
-            MVS_CUDA_OK(ctx, cudaEventCreateWithFlags(&S.na_event[1], cudaEventDisableTiming | cudaEventBlockingSync));
-        }
-        int* na_slots = reinterpret_cast<int*>(S.na_host);           // [0], [1]: two chunks in flight
-        int pending = -1;                                             // chunk whose count has not been read yet
-        long long chunk_idx = 0;
-        w.na_bound = B;                                               // grids shrink with the (lagging) host view of the count
-        while (rounds < max_rounds) {
-            for (int r = 0; r < chunk; ++r) {
-                if ((rc = launch_vertex_fwd_dense(ctx, st, true, false, true))) return rc;   // wgmma GEMM + LBS + SDF set-up
-                if ((rc = launch_sdf_fused(ctx, st))) return rc;   // samples + adjoint of the listed vertices
-                if ((rc = launch_frame_step(ctx, params_dev, &S, &cfg, nst, st))) return rc;
-                ++rounds;
-            }
-            // compaction changes slot -> frame, so the surviving frames' Phi / transforms are rebuilt for their new slots
-            MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
-            if ((rc = launch_frame_fwd_dense(ctx, S.x_eval, &S, nst, st))) return rc;
-            const int cur = (int)(chunk_idx & 1);
-            MVS_CUDA_OK(ctx, cudaMemcpyAsync(&na_slots[cur], w.na, sizeof(int), cudaMemcpyDeviceToHost, st));
-            MVS_CUDA_OK(ctx, cudaEventRecord(S.na_event[cur], st));
-            if (pending >= 0) {
-                const auto tb0 = std::chrono::steady_clock::now();
-                MVS_CUDA_OK(ctx, cudaEventSynchronize(S.na_event[pending]));
-                if (trace_host) blocked_us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - tb0).count();
-                na_host = na_slots[pending];
-                if (trace_na) fprintf(stderr, "[mvs] dense regime: chunk %lld, active frames %d\n", chunk_idx - 1, na_host);
-                if (na_host <= 0) break;
-                w.na_bound = na_host;                                 // the list only shrinks: still an upper bound
-            }
-            pending = cur;
-            ++chunk_idx;
-        }
-        w.na_bound = B;
-        if (trace_host) {
-            const double enq = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - loop_t0).count();
-            const auto td0 = std::chrono::steady_clock::now();
-            MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-            const double drain = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - td0).count();
-            fprintf(stderr, "[mvs] dense regime host loop: %lld rounds, %.0f us in the loop (%.0f us of it blocked on the GPU), %.0f us "
-                            "draining afterwards\n", rounds, enq, blocked_us, drain);
-        }
-        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-        if ((rc = tc_check_error(ctx))) return rc;
-        MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_finalize_kernel<<<(B + 255) / 256, 256, 0, st>>>(S, B, final_loss_dev, S.totals, 1));
-        if (last_grad_dev)
-            MVS_CUDA_OK(ctx, cudaMemcpyAsync(last_grad_dev, S.g_eval, (size_t)B * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
-        MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-        if (stats) {
-            stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
-            stats->rounds += (int)th[3];
-            stats->dense_frame_evals += th[1]; stats->dense_rounds += (int)th[3];
-        }
-        MVS_CUDA_OK(ctx, cudaGetLastError());
-        return MVS_OK;
-    }
-    const int chunk = 8;
-    const long long max_rounds = (long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8;
-    long long rounds = 0;
-    int na_host = B;
-    while (na_host > 0 && rounds < max_rounds) {
-        for (int r = 0; r < chunk; ++r) {
-            rc = launch_closure(ctx, S.x_eval, S.loss_eval, S.g_eval, nullptr, nullptr, nullptr, st);
-            if (rc) return rc;
-            MVS_LAUNCH(ctx, KID_LBFGS_ADVANCE, st, lbfgs_advance_kernel<<<B, 32, 0, st>>>(S, cfg, params_dev, w.fidx, w.na, vp2 ? 32 : kOffTransl - kOffPose));
-            MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
-            ++rounds;
-        }
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(S.na_host, w.na, sizeof(int), cudaMemcpyDeviceToHost, st));
-        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-        na_host = *S.na_host;
-    }
-    MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_finalize_kernel<<<(B + 255) / 256, 256, 0, st>>>(S, B, final_loss_dev, S.totals, 0));
-    if (last_grad_dev)
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(last_grad_dev, S.g_eval, (size_t)B * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    long long* tot_host = reinterpret_cast<long long*>(S.na_host) + 1;
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(tot_host, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
-    // leave the context usable for plain closures: full active list again
-    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    if (stats) {
-        stats->frame_iterations += tot_host[0];
-        stats->frame_evals += tot_host[1];
-        stats->frames_nan += (int)tot_host[2];
-        stats->rounds += (int)tot_host[3];
-    }
-    MVS_CUDA_OK(ctx, cudaGetLastError());
-    return MVS_OK;
+    const Regime rg = (!o.step || vp2) && hybrid_available(ctx) ? kDense : kBatched;
+    rc = rg == kDense ? run_dense(ctx, params_dev, cfg, nst, st) : run_batched(ctx, params_dev, cfg, vp2, st);
+    return rc ? rc : end_run(ctx, rg, final_loss_dev, o.last_grad, stats, st);
 }
 
 // One closure evaluation through the dense-regime kernels (posedirs_gemm_tc -> skin -> sdf_fused -> frame_step with the
@@ -351,9 +383,9 @@ static int run_stage(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, con
 // gradient segment of the kernels the optimiser actually runs with the SDF term on (DESIGN.md section 2).
 int dense_regime_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, cudaStream_t st) {
     const int B = ctx->ws.B;
-    int rc = ensure_state(ctx, static_cast<LbfgsState*>(ctx->lbfgs) ? static_cast<LbfgsState*>(ctx->lbfgs)->H : 100);
+    int rc = ensure_state(ctx, ctx->lbfgs ? ctx->lbfgs->H : 100);
     if (rc) return rc;
-    LbfgsState& S = *static_cast<LbfgsState*>(ctx->lbfgs);
+    LbfgsState& S = *ctx->lbfgs;
     Workspace& w = ctx->ws;
     LbfgsCfg cfg{};
     cfg.max_outer = 1; cfg.max_iter = 1; cfg.max_eval = 1; cfg.history = S.H; cfg.max_ls = 25; cfg.step_mode = 2; cfg.lr = 1.f;
@@ -362,11 +394,8 @@ int dense_regime_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, floa
     MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
     MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_init_kernel<<<B, 32, 0, st>>>(S, x_dev, B, 1, 1, nullptr));
     w.na_bound = B;
-    if ((rc = launch_frame_fwd_dense(ctx, S.x_eval, &S, 1, st))) return rc;
-    if ((rc = frame_step_begin_run(ctx, st))) return rc;
-    if ((rc = launch_vertex_fwd_dense(ctx, st, true, false, true))) return rc;
-    if ((rc = launch_sdf_fused(ctx, st))) return rc;
-    if ((rc = launch_frame_step(ctx, const_cast<float*>(x_dev) /* read only in this mode */, &S, &cfg, 1, st))) return rc;
+    if ((rc = dense_begin(ctx, S, 1, st))) return rc;
+    if ((rc = dense_round(ctx, const_cast<float*>(x_dev) /* read only in this mode */, S, cfg, 1, st))) return rc;
     if (loss_dev) MVS_CUDA_OK(ctx, cudaMemcpyAsync(loss_dev, S.loss_eval, (size_t)B * sizeof(float), cudaMemcpyDeviceToDevice, st));
     if (grad_dev) MVS_CUDA_OK(ctx, cudaMemcpyAsync(grad_dev, S.g_eval, (size_t)B * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
     MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));         // the pinned stage table is reused by the next call
@@ -403,7 +432,7 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
         const int rc = make_loss_params(ctx, &wc[kWarmSkip], &wlps[kWarmSkip]);
         if (rc) return rc;
         if (!ctx->stage_rng) {
-            const int rc2 = dev_alloc(ctx, &ctx->stage_rng, (size_t)B * 2);
+            const int rc2 = dev_alloc(ctx, &ctx->stage_rng, (size_t)B);
             if (rc2) return rc2;
         }
     }
@@ -415,6 +444,7 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
     };
     const int max_run = any_warm ? kMaxStages / 2 : kMaxStages;       // the table holds the cold and the warm slice of a run
     std::vector<int> rng;
+    std::vector<LossParams> tab;                                      // stage table of a warm run (read by run_stage)
     int i = 0;
     while (i < n_stages) {
         const int rg = regime(lps[i]);
@@ -424,32 +454,34 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
             ++j;
         ctx->loss = lps[i];
         ctx->have_loss = true;
-        int rc;
+        RunOpts o;
         if (!any_warm) {
-            rc = run_stage(ctx, x_dev, final_loss_dev, opt_cfg, stats, st, 0, 1, nullptr, &lps[i], j - i);
+            o.lps = &lps[i];
+            o.nst = j - i;
         } else {
             if (rg == 2)
                 return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq: warm-started frames are not implemented in the batched "
                                                        "reference chain (exec mode 1 / a model the resident kernels do not take)");
             // table of this run: cold stages i .. j-1, then the warm slice max(i, 2) .. j-1
-            std::vector<LossParams> tab(lps.begin() + i, lps.begin() + j);
+            tab.assign(lps.begin() + i, lps.begin() + j);
             const int wi = i > kWarmSkip ? i : kWarmSkip;
             const int wbegin = (int)tab.size();
             for (int k = wi; k < j; ++k) tab.push_back(wlps[k]);
             const int wend = (int)tab.size();
             rng.assign((size_t)B * 2, 0);
-            bool inactive = false;
             for (int b = 0; b < B; ++b) {
                 const bool wm = warm_host[b] != 0;
                 rng[2 * b] = wm ? wbegin : 0;
                 rng[2 * b + 1] = wm ? wend : j - i;
-                inactive |= wm && wbegin == wend;
+                o.some_inactive |= wm && wbegin == wend;
             }
             MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->stage_rng, rng.data(), rng.size() * sizeof(int), cudaMemcpyHostToDevice, st));
             MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));           // rng is reused by the next run
-            rc = run_stage(ctx, x_dev, final_loss_dev, opt_cfg, stats, st, 0, 1, nullptr, tab.data(), (int)tab.size(),
-                           reinterpret_cast<const int2*>(ctx->stage_rng), inactive);
+            o.lps = tab.data();
+            o.nst = (int)tab.size();
+            o.stage_rng = ctx->stage_rng;
         }
+        const int rc = run_stage(ctx, x_dev, final_loss_dev, opt_cfg, stats, st, o);
         if (rc) return rc;
         i = j;
     }
@@ -471,7 +503,7 @@ int mvs_lbfgs_run(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, const 
     if (!params_dev || !cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_run: NULL argument");
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     if (stats) memset(stats, 0, sizeof(*stats));
-    return run_stage(ctx, params_dev, final_loss_dev, cfg, stats, (cudaStream_t)stream);
+    return run_stage(ctx, params_dev, final_loss_dev, cfg, stats, (cudaStream_t)stream, RunOpts{});
 }
 
 int mvs_lbfgs_step(mvs_ctx* ctx, float* params_dev, float* loss_dev, float* last_grad_dev, const mvs_lbfgs_config* cfg,
@@ -483,7 +515,11 @@ int mvs_lbfgs_step(mvs_ctx* ctx, float* params_dev, float* loss_dev, float* last
     if (!reset && !ctx->lbfgs) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_step: reset=0 before any step");
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     if (stats) memset(stats, 0, sizeof(*stats));
-    return run_stage(ctx, params_dev, loss_dev, cfg, stats, (cudaStream_t)stream, 1, reset ? 1 : 0, last_grad_dev);
+    RunOpts o;
+    o.step = true;
+    o.reset = reset != 0;
+    o.last_grad = last_grad_dev;
+    return run_stage(ctx, params_dev, loss_dev, cfg, stats, (cudaStream_t)stream, o);
 }
 
 int mvs_fit_seq(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg,
@@ -527,7 +563,7 @@ int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, cons
         rc = ensure_state(ctx, H);
         if (rc) return rc;
     }
-    LbfgsState& S = *static_cast<LbfgsState*>(ctx->lbfgs);
+    LbfgsState& S = *ctx->lbfgs;
     float* x = S.x_fit;                              // [B][86] device copy of the parameters
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(x, params_host, (size_t)B * kParams * sizeof(float), cudaMemcpyHostToDevice, st));
     if (stats) memset(stats, 0, sizeof(*stats));

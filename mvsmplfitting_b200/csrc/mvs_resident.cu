@@ -193,19 +193,6 @@ frame_fwd_resident_kernel(ResidentModel m, const LossParams* __restrict__ lp_tab
     next_pose_forward(S, m, W, vp2, slot, b, Phi, PhiTc, At, ldA, slot_tr, nullptr, nullptr);
 }
 
-// ------------------------------------------------------------------------------------------------ dense regime
-// One round of the dense regime for one frame (multi-kernel path): see frame_step_body.
-__global__ void __launch_bounds__(kResThreads, 2)
-frame_step_kernel(FrameStepArgs a, const int* __restrict__ fidx, const int* __restrict__ na_ptr) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    // the model tables are constants of the run: staged while the previous kernel of the round drains
-    resident_setup(*reinterpret_cast<ResidentSmem*>(smem_raw), a.m);
-    pdl_wait();
-    const int slot = blockIdx.x;
-    if (slot >= *na_ptr) return;
-    frame_step_body(smem_raw, a, slot, fidx[slot]);
-}
-
 // ------------------------------------------------------------------------------------------------ host side
 static bool resident_supported(const mvs_ctx* ctx) {
     const DevModel& m = ctx->m;
@@ -283,12 +270,10 @@ bool resident_lbfgs_available_for(const mvs_ctx* ctx, const LossParams& lp, int 
 }
 bool resident_lbfgs_available(const mvs_ctx* ctx, int H) { return resident_lbfgs_available_for(ctx, ctx->loss, H); }
 
-int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const void* cfg_ptr, int H, const void* lp_tab_dev,
-                          const void* lp_tab_host, int nstages, void* sc_out, float* last_grad_dev, cudaStream_t st,
-                          const void* stage_rng_dev) {
+int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int H, const LossParams* lp_tab_dev,
+                          const LossParams* lph, int nstages, FrameScalars* sc_out, float* last_grad_dev, cudaStream_t st,
+                          const int2* stage_rng_dev) {
     Workspace& w = ctx->ws;
-    const LbfgsCfg& cfg = *static_cast<const LbfgsCfg*>(cfg_ptr);
-    const LossParams* lph = static_cast<const LossParams*>(lp_tab_host);
     int with_vposer = 0;
     for (int i = 0; i < nstages; ++i) with_vposer |= (lph[i].use_vposer == 2);
     const size_t smem = sizeof(ResidentSmem) + (size_t)2 * H * kParams * sizeof(float) + (with_vposer ? sizeof(VposerSmem) : 0);
@@ -298,10 +283,9 @@ int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const void* cfg_ptr, 
     }
     MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
                lbfgs_resident_kernel<<<w.B, kResThreads, smem, st>>>(make_resident_model(ctx), ctx->cams,
-                                                                     static_cast<const LossParams*>(lp_tab_dev), nstages, cfg,
-                                                                     params_dev, w.gt_uv, w.conf, w.joint_w, w.B, H,
-                                                                     static_cast<FrameScalars*>(sc_out), last_grad_dev, with_vposer,
-                                                                     static_cast<const int2*>(stage_rng_dev)));
+                                                                     lp_tab_dev, nstages, cfg, params_dev, w.gt_uv, w.conf,
+                                                                     w.joint_w, w.B, H, sc_out, last_grad_dev, with_vposer,
+                                                                     stage_rng_dev));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }
@@ -330,30 +314,27 @@ static int stages_with_vposer(const LbfgsState& L, int nstages) {
     return v;
 }
 
-FrameStepArgs make_frame_step_args(mvs_ctx* ctx, float* params_dev, const void* lbfgs_state, const void* lbfgs_cfg, int nstages) {
+static FrameStepArgs make_frame_step_args(mvs_ctx* ctx, float* params_dev, const LbfgsState& L, const LbfgsCfg& cfg, int nstages) {
     Workspace& w = ctx->ws;
     const DevModel& dm = ctx->m;
-    const LbfgsState& L = *static_cast<const LbfgsState*>(lbfgs_state);
     FrameStepArgs a;
     a.m = make_resident_model(ctx); a.cams = ctx->cams; a.lp_tab = L.lp_tab; a.nstages = nstages;
-    a.cfg = *static_cast<const LbfgsCfg*>(lbfgs_cfg); a.L = L; a.params = params_dev;
+    a.cfg = cfg; a.L = L; a.params = params_dev;
     a.gt_uv = w.gt_uv; a.conf = w.conf; a.joint_w = w.joint_w; a.B = w.B; a.N = dm.N;
     a.verts_ws = w.verts; a.poffT = tc_poffT(ctx); a.ST = dm.ST;
-    a.parts5 = w.sdf_parts5; a.part = w.sdf_part; a.pflag = w.sdf_pflag; a.box = reinterpret_cast<const FrameBox*>(w.sdf_box);
+    a.parts5 = w.sdf_parts5; a.part = w.sdf_part; a.pflag = w.sdf_pflag; a.box = w.sdf_box;
     a.Wd = dm.Wd; a.Phi = w.Phi; a.PhiTc = w.PhiTc; a.At = w.At; a.ldA = w.ldA; a.slot_tr = w.slot_tr;
     a.pose_cache = w.pose_cache; a.pose_valid = w.pose_valid; a.with_vposer = stages_with_vposer(L, nstages);
     return a;
 }
 
-size_t frame_step_smem(int H, bool with_vposer) {
+static size_t frame_step_smem(int H, bool with_vposer) {
     return sizeof(ResidentSmem) + (size_t)2 * H * kParams * sizeof(float) + (with_vposer ? sizeof(VposerSmem) : 0);
 }
 
-int launch_frame_step(mvs_ctx* ctx, float* params_dev, const void* lbfgs_state, const void* lbfgs_cfg, int nstages,
-                      cudaStream_t st) {
+int launch_frame_step(mvs_ctx* ctx, float* params_dev, const LbfgsState& L, const LbfgsCfg& cfg, int nstages, cudaStream_t st) {
     Workspace& w = ctx->ws;
-    const LbfgsState& L = *static_cast<const LbfgsState*>(lbfgs_state);
-    const FrameStepArgs a = make_frame_step_args(ctx, params_dev, lbfgs_state, lbfgs_cfg, nstages);
+    const FrameStepArgs a = make_frame_step_args(ctx, params_dev, L, cfg, nstages);
     const size_t smem = frame_step_smem(L.H, a.with_vposer != 0);
     if (!ctx->attr_done_step) {
         MVS_CUDA_OK(ctx, cudaFuncSetAttribute(frame_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -371,8 +352,7 @@ int launch_frame_step(mvs_ctx* ctx, float* params_dev, const void* lbfgs_state, 
 
 // slot-indexed pose forward of every active frame (run start, after a compaction); the axis-angle-only frame_fwd_kernel
 // serves runs without a device-decoded VPoser stage
-int launch_frame_fwd_dense(mvs_ctx* ctx, const float* x_dev, const void* lbfgs_state, int nstages, cudaStream_t st) {
-    const LbfgsState& L = *static_cast<const LbfgsState*>(lbfgs_state);
+int launch_frame_fwd_dense(mvs_ctx* ctx, const float* x_dev, const LbfgsState& L, int nstages, cudaStream_t st) {
     if (!stages_with_vposer(L, nstages)) return launch_frame_fwd(ctx, x_dev, st);
     Workspace& w = ctx->ws;
     if (!ctx->attr_done_step) {

@@ -1,6 +1,6 @@
-// Device-side building blocks of the frame-resident kernels (mvs_resident.cu) shared with the persistent dense-round
-// kernel (mvs_dense.cu): shared-memory layout of one frame, level-parallel kinematic chain, VPoser decoder, the closure,
-// the pose forward of the next trial point, and the per-frame half of a dense round (frame_step_body).
+// Device side of the frame-resident kernels (mvs_resident.cu): shared-memory layout of one frame, level-parallel kinematic
+// chain, VPoser decoder, the closure, the pose forward of the next trial point, and the per-frame half of a dense round
+// (frame_step_kernel).
 // A translation unit may define PHASE_MARK(i) before including this file (clock instrumentation); default: nothing.
 #pragma once
 #include <cstddef>
@@ -892,8 +892,7 @@ __device__ __forceinline__ void next_pose_forward(ResidentSmem& S, const Residen
     }
 }
 
-// Arguments of frame_step_body.  Everything except the model / camera / detection constants is rewritten every round by
-// other CTAs of the persistent dense-round kernel: plain pointers.
+// Arguments of frame_step_kernel
 struct FrameStepArgs {
     ResidentModel m; CamSet cams; const LossParams* lp_tab; int nstages; LbfgsCfg cfg; LbfgsState L; float* params;
     const float* gt_uv; const float* conf; const float* joint_w; int B, N;
@@ -906,11 +905,18 @@ struct FrameStepArgs {
 // frame's trial point, finishes the closure (keypoint term, adjoint, priors), advances the frame's L-BFGS state
 // machine and -- if the frame needs another evaluation -- runs the pose forward of the NEXT trial point and
 // writes its feature row / skinning transforms for the next dense vertex launch.
-// `smem_raw`: sizeof(ResidentSmem) + 2 H 86 floats (+ VposerSmem).  All kResThreads threads call; no trailing barrier
-// The caller stages the model tables (resident_setup) first: they are constants of the run.
-__device__ __forceinline__ void frame_step_body(unsigned char* smem_raw, const FrameStepArgs& a, const int slot, const int b) {
+// One CTA per slot; dynamic shared memory: sizeof(ResidentSmem) + 2 H 86 floats (+ VposerSmem).
+__global__ void __launch_bounds__(kResThreads, 2)
+frame_step_kernel(FrameStepArgs a, const int* __restrict__ fidx, const int* __restrict__ na_ptr) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
     ResidentSmem& S = *reinterpret_cast<ResidentSmem*>(smem_raw);
-    const ResidentModel& m = a.m; const CamSet& cams = a.cams; const LossParams* lp_tab = a.lp_tab; const int nstages = a.nstages;
+    // the model tables are constants of the run: staged while the previous kernel of the round drains
+    resident_setup(S, a.m);
+    pdl_wait();
+    const int slot = blockIdx.x;
+    if (slot >= *na_ptr) return;
+    const int b = fidx[slot];
+    const ResidentModel& m = a.m; const CamSet& cams = a.cams; const LossParams* lp_tab = a.lp_tab;
     const LbfgsCfg& cfg = a.cfg; const LbfgsState& L = a.L; float* params = a.params;
     const float* __restrict__ gt_uv = a.gt_uv; const float* __restrict__ conf = a.conf; const float* __restrict__ joint_w = a.joint_w;
     const int B = a.B, N = a.N, ldA = a.ldA, with_vposer = a.with_vposer;
@@ -1091,9 +1097,5 @@ __device__ __forceinline__ void frame_step_body(unsigned char* smem_raw, const F
     }
     PHASE_MARK(28);
 }
-
-// mvs_resident.cu (host)
-FrameStepArgs make_frame_step_args(mvs_ctx* ctx, float* params_dev, const void* lbfgs_state, const void* lbfgs_cfg, int nstages);
-size_t frame_step_smem(int H, bool with_vposer);
 
 }  // namespace mvs

@@ -19,7 +19,6 @@
 // gradients flow through the sample coordinates and through the bounding-box centre / scale, not through phi.
 #include <cstdlib>
 #include "mvs_internal.cuh"
-#include "mvs_lbfgs_core.cuh"
 // -DMVS_PHASE_DBG (scripts/sdf_phase_times.py): thread 0 of every sdf_fused CTA that runs to the end stamps clock64() at
 // entry (0), after pdl_wait (1), after the box fold and its barrier (2), once the cone/plane set-up and the chunk-cull
 // verdicts are ready (3), after sampling and its barrier (4) and after the block reduction and adjoint (5).  The intervals
@@ -466,18 +465,6 @@ static int ensure_sdf_bins_ws(mvs_ctx* ctx) {
     return MVS_OK;
 }
 
-// kAll = false: the reference call as written (the kernel sees triangle 0), the default and the benchmark's mode; kAll = true: the
-// intended all-faces field, over candidate lists or by brute force
-template <bool kAll>
-__global__ void __launch_bounds__(kSdfFThreads, 3)
-sdf_fused_kernel(SdfFusedArgs ar, const int* __restrict__ na_ptr, int passes) {
-    SDF_MARK(0);
-    pdl_wait();
-    SDF_MARK(1);
-    __shared__ SdfFusedSmem sm;
-    sdf_fused_body<kAll>(sm, ar, *na_ptr, (int)blockIdx.y, (int)blockIdx.x, passes);
-}
-
 int ensure_sdf_fused_ws(mvs_ctx* ctx) {
     Workspace& w = ctx->ws;
     const int B = w.B, N = ctx->m.N;
@@ -489,11 +476,7 @@ int ensure_sdf_fused_ws(mvs_ctx* ctx) {
         if ((rc = dev_alloc(ctx, &w.sdf_part, (size_t)B * nblocks * kPartFloats))) return rc;
         if ((rc = dev_alloc(ctx, &w.sdf_pflag, (size_t)B * nblocks))) return rc;
     }
-    if (!w.sdf_box) {
-        unsigned char* raw = nullptr;
-        if ((rc = dev_alloc(ctx, &raw, (size_t)B * sizeof(FrameBox)))) return rc;
-        w.sdf_box = raw;
-    }
+    if (!w.sdf_box && (rc = dev_alloc(ctx, &w.sdf_box, (size_t)B))) return rc;
     return MVS_OK;
 }
 
@@ -502,7 +485,7 @@ int ensure_sdf_setup_ws(mvs_ctx* ctx, cudaStream_t st) {
     int rc;
     if ((rc = ensure_sdf_fused_ws(ctx))) return rc;
     if (!w.sdf_setup) {
-        if ((rc = dev_alloc(ctx, &w.sdf_setup, (size_t)w.B * sizeof(SdfFrameSetup)))) return rc;
+        if ((rc = dev_alloc(ctx, &w.sdf_setup, (size_t)w.B))) return rc;
         if ((rc = dev_alloc(ctx, &w.sdf_arrive, (size_t)w.B))) return rc;
         MVS_CUDA_OK(ctx, cudaMemsetAsync(w.sdf_arrive, 0, (size_t)w.B * sizeof(int), st));
     }
@@ -513,7 +496,7 @@ SdfSetupArgs make_sdf_setup_args(mvs_ctx* ctx) {
     Workspace& w = ctx->ws;
     const DevModel& m = ctx->m;
     SdfSetupArgs a;
-    a.rec = reinterpret_cast<SdfFrameSetup*>(w.sdf_setup); a.boxout = reinterpret_cast<FrameBox*>(w.sdf_box);
+    a.rec = w.sdf_setup; a.boxout = w.sdf_box;
     a.arrive = w.sdf_arrive; a.slot_tr = w.slot_tr;
     a.f0 = m.tri0[0]; a.f1 = m.tri0[1]; a.f2 = m.tri0[2]; a.G = ctx->loss.sdf_grid;
     a.cull = ctx->loss.sdf_all_faces ? (m.F == 1) : 1;        // the cone/plane tests hold for a single face (num_faces == 1)
@@ -526,7 +509,7 @@ SdfFusedArgs make_sdf_fused_args(mvs_ctx* ctx) {
     const LossParams& lp = ctx->loss;
     SdfFusedArgs a;
     a.verts = w.verts; a.poffT = tc_poffT(ctx); a.Phi = w.Phi; a.ST = m.ST; a.slot_tr = w.slot_tr;
-    a.N = m.N; a.nbox = (m.N + 63) / 64; a.setup = reinterpret_cast<const SdfFrameSetup*>(w.sdf_setup); a.faces = m.faces;
+    a.N = m.N; a.nbox = (m.N + 63) / 64; a.setup = w.sdf_setup; a.faces = m.faces;
     a.num_faces = lp.sdf_all_faces ? m.F : 1; a.G = lp.sdf_grid;
     a.At = w.At; a.ldA = w.ldA; a.ell_j = m.ell_j; a.ell_w = m.ell_w; a.KW = m.KW; a.Wd = m.Wd; a.Qk = m.Qk;
     a.parts5 = w.sdf_parts5; a.part = w.sdf_part; a.pflag = w.sdf_pflag;
@@ -557,7 +540,7 @@ int launch_sdf_fused(mvs_ctx* ctx, cudaStream_t st) {
     if (ctx->loss.sdf_all_faces == 1) {                  // accelerated all-faces mode: this round's candidate lists first
         if ((rc = ensure_sdf_bins_ws(ctx))) return rc;
         SdfBinsArgs ba;
-        ba.verts = w.verts; ba.slot_tr = w.slot_tr; ba.setup = reinterpret_cast<const SdfFrameSetup*>(w.sdf_setup); ba.faces = m.faces;
+        ba.verts = w.verts; ba.slot_tr = w.slot_tr; ba.setup = w.sdf_setup; ba.faces = m.faces;
         ba.N = N; ba.F = m.F;
         ba.tri = w.bins_tri; ba.cell_ptr = w.bins_cell_ptr; ba.cell_idx = w.bins_cell_idx; ba.ray_ptr = w.bins_ray_ptr;
         ba.ray_idx = w.bins_ray_idx; ba.meta = w.bins_meta;
@@ -583,13 +566,11 @@ int launch_sdf_terms(mvs_ctx* ctx, const float* x_dev, cudaStream_t st) {
     const int nblk = (N + kSampleThreads - 1) / kSampleThreads;
     if (!w.sdf_frame) {
         int rc;
-        unsigned char* raw = nullptr;
-        if ((rc = dev_alloc(ctx, &raw, (size_t)B * sizeof(FrameBox)))) return rc;
-        w.sdf_frame = reinterpret_cast<float*>(raw);
+        if ((rc = dev_alloc(ctx, &w.sdf_frame, (size_t)B))) return rc;
         if (!w.sdf_gcoord && (rc = dev_alloc(ctx, &w.sdf_gcoord, (size_t)B * N * 3))) return rc;
         if ((rc = dev_alloc(ctx, &w.sdf_valpart, (size_t)B * nblk * 5))) return rc;
     }
-    FrameBox* box = reinterpret_cast<FrameBox*>(w.sdf_frame);
+    FrameBox* box = w.sdf_frame;
     MVS_LAUNCH(ctx, KID_SDF_BBOX, st, sdf_bbox_kernel<<<B, kBoxThreads, 0, st>>>(w.verts, x_dev, w.fidx, w.na, N, box));
     dim3 g(nblk, B);
     MVS_LAUNCH(ctx, KID_SDF_SAMPLE, st,

@@ -1,12 +1,12 @@
-// Device-side building blocks of the SDF interpenetration term (mvs_sdf.cu) shared with the persistent dense-round kernel
-// (mvs_dense.cu): the reference's geometric primitives and the fused sampling + sparse-adjoint CTA body.
+// Device side of the dense regime's SDF term (mvs_sdf.cu): the reference's geometric primitives and sdf_fused_kernel, the
+// fused sampling + sparse adjoint.
 #pragma once
 #include "mvs_internal.cuh"
 #include "mvs_tc_dev.cuh"
 #include "mvs_sdf_geom.cuh"
 #include "mvs_sdf_bins.cuh"
 
-// A translation unit may define SDF_MARK(i) before including this file (clock instrumentation of sdf_fused_body, see
+// A translation unit may define SDF_MARK(i) before including this file (clock instrumentation of sdf_fused_kernel, see
 // scripts/sdf_phase_times.py); default: nothing.
 #ifndef SDF_MARK
 #define SDF_MARK(i) do {} while (0)
@@ -60,8 +60,7 @@ struct SdfBinsDev {
     int F;
 };
 
-// Shared-memory working set of sdf_fused_body (static in sdf_fused_kernel, a slice of the dynamic buffer in the persistent
-// dense-round kernel)
+// Shared-memory working set of sdf_fused_kernel
 struct SdfFusedSmem {
     float ctab[256];
     float s_red[kSdfMaxPasses][8][5];
@@ -86,10 +85,17 @@ struct SdfFusedArgs {
     SdfBinsDev bins;
 };
 
-// One CTA of sdf_fused_kernel's virtual grid (pidx = block group of the frame in `slot`).  All kSdfFThreads threads call.
+// kAll = false: the reference call as written (the kernel sees triangle 0), the default and the benchmark's mode; kAll = true: the
+// intended all-faces field, over candidate lists or by brute force.  Grid (block groups, slots): CTA (pidx, slot) takes
+// `passes` blocks of 256 vertices of the frame in `slot`.
 template <bool kAll>
-__device__ __forceinline__ void sdf_fused_body(SdfFusedSmem& sm, const SdfFusedArgs& ar, const int na, const int slot, const int pidx,
-                                               const int passes) {
+__global__ void __launch_bounds__(kSdfFThreads, 3)
+sdf_fused_kernel(SdfFusedArgs ar, const int* __restrict__ na_ptr, int passes) {
+    SDF_MARK(0);
+    pdl_wait();
+    SDF_MARK(1);
+    __shared__ SdfFusedSmem sm;
+    const int na = *na_ptr, slot = blockIdx.y, pidx = blockIdx.x;
     const float* verts = ar.verts; const float* slot_tr = ar.slot_tr;
     const int N = ar.N, nbox = ar.nbox, num_faces = ar.num_faces, G = ar.G, ldA = ar.ldA, KW = ar.KW;
     const int* __restrict__ faces = ar.faces; const float* At = ar.At;

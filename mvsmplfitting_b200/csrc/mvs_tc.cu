@@ -169,18 +169,238 @@ posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_
     if (threadIdx.x == 0) TC_MARK(20);
 }
 
+// grid (nchunks, frame groups of 32); kSkinSmem bytes of dynamic shared memory
 __global__ void __launch_bounds__(kSkinThreads)
 skin_kernel(SkinArgs ar, const int* __restrict__ na_ptr, int cta_slots) {
     pdl_wait();
     extern __shared__ __align__(16) float sk[];
-    skin_body(sk, ar, *na_ptr, cta_slots, (int)blockIdx.x, (int)blockIdx.y);
+    const int na = *na_ptr;
+    const float* poffT = ar.poffT; const float* __restrict__ ST = ar.ST; const float* Phi = ar.Phi; const float* At = ar.At;
+    const int ldA = ar.ldA, KW = ar.KW, N = ar.N;
+    const int* __restrict__ ell_j = ar.ell_j; const float* __restrict__ ell_w = ar.ell_w;
+    float* vposed = ar.vposed; float* verts = ar.verts; float* bboxp = ar.bboxp;
+    float* As = sk;                                   // [24 joints][32 lanes][12]
+    float* Bs = As + kSkinFloats * 32;                // [10][32]
+    float* Ovp = Bs + kBetas * 32;                    // [32][193] (only when v_posed is stored)
+    float* Ov = vposed ? Ovp + 32 * kSkinOutLd : Ovp; // [32][193]
+    float* Bb = Ov + 32 * kSkinOutLd;                 // [8 warps][32 lanes][6] values, then [..][6] indices
+    float* Sts = Bb + 8 * 32 * 6 * 2;                 // [64][33] shapedirs rows | template of this CTA's vertices
+    float* Ews = Sts + kSkinV * 33;                   // [64][KW] skinning weights of the chunk
+    int* Ejs = reinterpret_cast<int*>(Ews + kSkinV * kSkinEllMax);   // [64][KW] their joints
+    const bool ell_smem = KW <= kSkinEllMax;
+    const int f0 = blockIdx.y * 32;
+    if (f0 >= na) return;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int slotc = min(f0 + lane, na - 1);
+    // chunks per CTA from the number of ACTIVE frame groups: one chunk each while the active CTAs fit in one wave
+    // (latency at the tail of a stage), several once they do not (the 36 KB of transforms are then loaded once)
+    const int nchunks = (N + kSkinV - 1) / kSkinV;
+    const int per_cta = (nchunks * ((na + 31) / 32) + cta_slots - 1) / cta_slots;
+    const int nx = (nchunks + per_cta - 1) / per_cta;
+    if ((int)blockIdx.x >= nx) return;
+    // the 32 frames' transforms and shape coefficients are loaded once and reused for every vertex chunk of this CTA
+    // layout [joint][lane][12]: a lane's 3x4 transform is three conflict-free LDS.128 (lane stride 48 B)
+    for (int e = tid; e < kSkinFloats * 32; e += kSkinThreads) {
+        const int jc = e >> 5, ln = e & 31;
+        As[((jc / 12) * 32 + ln) * 12 + jc % 12] = At[(size_t)jc * ldA + min(f0 + ln, na - 1)];
+    }
+    for (int e = tid; e < kBetas * 32; e += kSkinThreads)
+        Bs[e] = Phi[(size_t)min(f0 + (e & 31), na - 1) * kFeatPad + kPoseBasis + (e >> 5)];
+    constexpr int kVw = kSkinV / 8;                                       // vertices per warp and chunk
+    float beta[kBetas];
+    bool have_beta = false;
+    for (int ch = blockIdx.x; ch < nchunks; ch += nx) {
+        const int v0 = ch * kSkinV;
+        // pose offsets of this warp's vertices: 24 independent coalesced loads in flight before anything waits
+        float pf[kVw][3];
+#pragma unroll
+        for (int i = 0; i < kVw; ++i) {
+            const int n = v0 + warp * kVw + i;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) pf[i][c] = n < N ? poffT[(size_t)(3 * n + c) * ldA + slotc] : 0.f;
+        }
+        __syncthreads();                                                  // previous chunk's staging buffers are free
+        for (int e = tid; e < kSkinV * 33; e += kSkinThreads) Sts[e] = (v0 * 33 + e < N * 33) ? ST[(size_t)v0 * 33 + e] : 0.f;
+        if (ell_smem)
+            for (int e = tid; e < kSkinV * KW; e += kSkinThreads) {
+                const bool in = (size_t)v0 * KW + e < (size_t)N * KW;
+                Ews[e] = in ? ell_w[(size_t)v0 * KW + e] : 0.f;
+                Ejs[e] = in ? ell_j[(size_t)v0 * KW + e] : 0;
+            }
+        __syncthreads();
+        if (!have_beta) {
+#pragma unroll
+            for (int l = 0; l < kBetas; ++l) beta[l] = Bs[l * 32 + lane];
+            have_beta = true;
+        }
+        float blo[3] = {3e38f, 3e38f, 3e38f}, bhi[3] = {-3e38f, -3e38f, -3e38f};
+        int bilo[3] = {0, 0, 0}, bihi[3] = {0, 0, 0};
+#pragma unroll
+        for (int i = 0; i < kVw; ++i) {
+            const int li = warp * kVw + i;
+            const int n = v0 + li;
+            if (n < N) {
+                float vp[3], vvv[3];
+                skin_vertex(Sts + li * 33, beta, pf[i], ell_smem ? Ejs : ell_j, ell_smem ? Ews : ell_w, KW,
+                            ell_smem ? (size_t)li : (size_t)n,
+                            [&](int j, float* a12) {
+                                const float4* q = reinterpret_cast<const float4*>(As + (j * 32 + lane) * 12);
+                                const float4 q0 = q[0], q1 = q[1], q2 = q[2];
+                                a12[0] = q0.x; a12[1] = q0.y; a12[2] = q0.z; a12[3] = q0.w; a12[4] = q1.x; a12[5] = q1.y;
+                                a12[6] = q1.z; a12[7] = q1.w; a12[8] = q2.x; a12[9] = q2.y; a12[10] = q2.z; a12[11] = q2.w;
+                            }, vp, vvv);
+#pragma unroll
+                for (int r = 0; r < 3; ++r) {
+                    const float vv = vvv[r];
+                    if (vposed) Ovp[lane * kSkinOutLd + 3 * li + r] = vp[r];
+                    Ov[lane * kSkinOutLd + 3 * li + r] = vv;
+                    if (vv < blo[r]) { blo[r] = vv; bilo[r] = n; }       // strict: ties keep the lowest vertex index
+                    if (vv > bhi[r]) { bhi[r] = vv; bihi[r] = n; }
+                }
+            }
+        }
+        int* Bi = reinterpret_cast<int*>(Bb + 8 * 32 * 6);
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            Bb[(warp * 32 + lane) * 6 + r] = blo[r]; Bb[(warp * 32 + lane) * 6 + 3 + r] = bhi[r];
+            Bi[(warp * 32 + lane) * 6 + r] = bilo[r]; Bi[(warp * 32 + lane) * 6 + 3 + r] = bihi[r];
+        }
+        __syncthreads();
+        const int ncol = 3 * min(kSkinV, N - v0);                         // contiguous floats of this chunk per frame
+        for (int fl = warp; fl < 32; fl += 8) {                           // a warp stores one frame's row segment at a time
+            const int slot = f0 + fl;
+            if (slot >= na) break;
+            const size_t off = ((size_t)slot * N + v0) * 3;
+            for (int col = lane; col < ncol; col += 32) {
+                if (vposed) vposed[off + col] = Ovp[fl * kSkinOutLd + col];
+                verts[off + col] = Ov[fl * kSkinOutLd + col];
+            }
+        }
+        if (bboxp && warp == 0 && f0 + lane < na) {       // fold the 8 warps' vertex groups (ascending vertex index)
+            float lo[3], hi[3];
+            int ilo[3], ihi[3];
+#pragma unroll
+            for (int r = 0; r < 3; ++r) { lo[r] = Bb[lane * 6 + r]; hi[r] = Bb[lane * 6 + 3 + r]; ilo[r] = Bi[lane * 6 + r]; ihi[r] = Bi[lane * 6 + 3 + r]; }
+            for (int w2 = 1; w2 < 8; ++w2)
+#pragma unroll
+                for (int r = 0; r < 3; ++r) {
+                    const float l2 = Bb[(w2 * 32 + lane) * 6 + r], h2 = Bb[(w2 * 32 + lane) * 6 + 3 + r];
+                    if (l2 < lo[r]) { lo[r] = l2; ilo[r] = Bi[(w2 * 32 + lane) * 6 + r]; }
+                    if (h2 > hi[r]) { hi[r] = h2; ihi[r] = Bi[(w2 * 32 + lane) * 6 + 3 + r]; }
+                }
+            float* bp = bboxp + ((size_t)(f0 + lane) * nchunks + ch) * 12;
+#pragma unroll
+            for (int r = 0; r < 3; ++r) { bp[r] = lo[r]; bp[3 + r] = hi[r]; bp[6 + r] = __int_as_float(ilo[r]); bp[9 + r] = __int_as_float(ihi[r]); }
+        }
+    }
+    if (ar.sdf.rec != nullptr) {                          // per-frame SDF set-up by the last CTA of each frame (sdf_setup_frames)
+        __threadfence();
+        __syncthreads();
+        unsigned* s_mine = reinterpret_cast<unsigned*>(Bb);   // staging buffers are free once every thread is here
+        if (warp == 0) {
+            bool last = false;
+            if (f0 + lane < na) {
+                const int cnt = (nchunks - (int)blockIdx.x + nx - 1) / nx;        // chunks this CTA skinned for each frame
+                last = atomicAdd(ar.sdf.arrive + f0 + lane, cnt) + cnt == nchunks;
+            }
+            const unsigned m = __ballot_sync(0xffffffffu, last);
+            if (lane == 0) *s_mine = m;
+        }
+        __syncthreads();
+        sdf_setup_frames(ar.sdf, bboxp, verts, N, nchunks, f0, *s_mine, warp, lane, kSkinThreads / 32);
+    }
 }
 
+// The same for a handful of frames (the straggler tail of a fit): with lane = frame almost every lane of skin_kernel
+// idles and its fixed costs (36 KB of transforms per CTA, staging, three barriers per chunk) are pure latency.  Here
+// lane = vertex, a CTA owns one 64-vertex chunk (= one box partial) and loops over the <= kSkinSmallMax frames.
+constexpr int kSkinSmallMax = 8;
+constexpr int kSkinSmallThreads = 64;
+static_assert(kSkinSmallThreads == kSkinV, "one thread per vertex of a box chunk");
+
+struct SkinSmallSmem {
+    float As[kSkinSmallMax][kSkinFloats];
+    float Bs[kSkinSmallMax][kBetas];
+    float s_b[kSkinSmallMax][6];
+    int s_i[kSkinSmallMax][6];
+    unsigned mine;                         // frames whose SDF set-up this CTA computes
+};
+
+// one CTA per 64-vertex chunk, thread t = vertex of the chunk
 __global__ void __launch_bounds__(kSkinSmallThreads)
 skin_small_kernel(SkinArgs ar, const int* __restrict__ na_ptr) {
     __shared__ SkinSmallSmem sm;
     pdl_wait();
-    skin_small_body(sm, ar, *na_ptr, (int)blockIdx.x, (int)gridDim.x, (int)threadIdx.x, 0);
+    const int t = threadIdx.x, chunk = blockIdx.x, nchunks = gridDim.x;
+    const float* poffT = ar.poffT; const float* __restrict__ ST = ar.ST; const float* Phi = ar.Phi; const float* At = ar.At;
+    const int ldA = ar.ldA, KW = ar.KW, N = ar.N;
+    const int* __restrict__ ell_j = ar.ell_j; const float* __restrict__ ell_w = ar.ell_w;
+    float* vposed = ar.vposed; float* verts = ar.verts; float* bboxp = ar.bboxp;
+    auto& As = sm.As; auto& Bs = sm.Bs; auto& s_b = sm.s_b; auto& s_i = sm.s_i;
+    const int na = min(*na_ptr, kSkinSmallMax);
+    if (na <= 0) return;
+    const int lane = t & 31, warp = t >> 5;
+    const int n = chunk * kSkinSmallThreads + t;
+    for (int e = t; e < na * kSkinFloats; e += kSkinSmallThreads) As[e / kSkinFloats][e % kSkinFloats] = At[(size_t)(e % kSkinFloats) * ldA + e / kSkinFloats];
+    for (int e = t; e < na * kBetas; e += kSkinSmallThreads) Bs[e / kBetas][e % kBetas] = Phi[(size_t)(e / kBetas) * kFeatPad + kPoseBasis + e % kBetas];
+    float st[33];
+    if (n < N) {
+#pragma unroll
+        for (int q = 0; q < 33; ++q) st[q] = ST[(size_t)n * 33 + q];
+    }
+    __syncthreads();
+    for (int f = 0; f < na; ++f) {
+        float lo[3] = {3e38f, 3e38f, 3e38f}, hi[3] = {-3e38f, -3e38f, -3e38f};
+        int ilo[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff}, ihi[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff};
+        if (n < N) {
+            float poff[3], vp[3], vv[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) poff[c] = poffT[(size_t)(3 * n + c) * ldA + f];
+            skin_vertex(st, Bs[f], poff, ell_j, ell_w, KW, (size_t)n,
+                        [&](int j, float* a12) {
+#pragma unroll
+                            for (int c = 0; c < 12; ++c) a12[c] = As[f][j * 12 + c];
+                        }, vp, vv);
+            const size_t off = ((size_t)f * N + n) * 3;
+#pragma unroll
+            for (int r = 0; r < 3; ++r) {
+                if (vposed) vposed[off + r] = vp[r];
+                verts[off + r] = vv[r];
+                lo[r] = vv[r]; hi[r] = vv[r]; ilo[r] = n; ihi[r] = n;
+            }
+        }
+        if (bboxp) {               // box of the chunk: extreme value, ties -> lowest vertex index (as skin_kernel)
+#pragma unroll
+            for (int r = 0; r < 3; ++r) { warp_argmin(lo[r], ilo[r]); warp_argmax(hi[r], ihi[r]); }
+            if (warp == 1 && lane == 0) {
+#pragma unroll
+                for (int r = 0; r < 3; ++r) { s_b[f][r] = lo[r]; s_b[f][3 + r] = hi[r]; s_i[f][r] = ilo[r]; s_i[f][3 + r] = ihi[r]; }
+            }
+            __syncthreads();
+            if (warp == 0 && lane == 0) {
+                float* bp = bboxp + ((size_t)f * nchunks + chunk) * 12;
+#pragma unroll
+                for (int r = 0; r < 3; ++r) {
+                    const float l2 = s_b[f][r], h2 = s_b[f][3 + r];
+                    const int il2 = s_i[f][r], ih2 = s_i[f][3 + r];
+                    if (l2 < lo[r] || (l2 == lo[r] && il2 < ilo[r])) { lo[r] = l2; ilo[r] = il2; }
+                    if (h2 > hi[r] || (h2 == hi[r] && ih2 < ihi[r])) { hi[r] = h2; ihi[r] = ih2; }
+                    bp[r] = lo[r]; bp[3 + r] = hi[r]; bp[6 + r] = __int_as_float(ilo[r]); bp[9 + r] = __int_as_float(ihi[r]);
+                }
+            }
+        }
+    }
+    if (ar.sdf.rec != nullptr) {                          // per-frame SDF set-up by the last CTA of each frame (sdf_setup_frames)
+        __threadfence();
+        __syncthreads();
+        if (warp == 0) {
+            const bool last = lane < na && atomicAdd(ar.sdf.arrive + lane, 1) + 1 == nchunks;   // one chunk per CTA
+            const unsigned m = __ballot_sync(0xffffffffu, last);
+            if (lane == 0) sm.mine = m;
+        }
+        __syncthreads();
+        sdf_setup_frames(ar.sdf, bboxp, verts, N, nchunks, 0, sm.mine, warp, lane, kSkinSmallThreads / 32);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -236,7 +456,7 @@ static int tc_set_smem(mvs_ctx* ctx) {
 }
 
 int tc_prepare(mvs_ctx* ctx) {
-    TcState* T = static_cast<TcState*>(ctx->tc);
+    TcState* T = ctx->tc;
     Workspace& w = ctx->ws;
     const DevModel& m = ctx->m;
     if (!T) return set_error(ctx, MVS_ERR_INVALID, "tensor-core path not initialised (mvs_set_model)");
@@ -256,12 +476,10 @@ int tc_prepare(mvs_ctx* ctx) {
 }
 
 float* tc_poffT(mvs_ctx* ctx) {
-    TcState* T = static_cast<TcState*>(ctx->tc);
+    TcState* T = ctx->tc;
     if (!T || tc_prepare(ctx) != MVS_OK) return nullptr;
     return T->poffT;
 }
-
-int* tc_err_flag(mvs_ctx* ctx) { TcState* T = static_cast<TcState*>(ctx->tc); return T ? T->err : nullptr; }
 
 template <int NF>
 static cudaError_t launch_gemm(mvs_ctx* ctx, const TcState* T, int inst, dim3 grid, cudaStream_t st, int ntiles) {
@@ -271,7 +489,7 @@ static cudaError_t launch_gemm(mvs_ctx* ctx, const TcState* T, int inst, dim3 gr
 }
 
 int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool sdf_setup) {
-    TcState* T = static_cast<TcState*>(ctx->tc);
+    TcState* T = ctx->tc;
     Workspace& w = ctx->ws;
     const DevModel& m = ctx->m;
     { const int rc = tc_prepare(ctx); if (rc) return rc; }
@@ -307,7 +525,7 @@ int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool s
 }
 
 int tc_check_error(mvs_ctx* ctx) {          // host-side check after a synchronisation point
-    TcState* T = static_cast<TcState*>(ctx->tc);
+    TcState* T = ctx->tc;
     if (!T || !T->ready) return MVS_OK;
     int e = 0;
     MVS_CUDA_OK(ctx, cudaMemcpy(&e, T->err, sizeof(int), cudaMemcpyDeviceToHost));

@@ -224,9 +224,9 @@ __device__ __forceinline__ float vposed_of(const float* __restrict__ st11 /* sha
     return __fadd_rn(a, poff);
 }
 
-// Arguments of the skinning bodies.  poffT / Phi / At / verts / bboxp are rewritten every round by other CTAs of the
-// persistent dense-round kernel, so they are plain pointers (no __restrict__ / read-only path); the model constants may
-// use the read-only path.  vposed == nullptr: v_posed is not stored (the few consumers recompute it, vposed_of).
+// Arguments of the skinning kernels (mvs_tc.cu).  verts and bboxp are read back within the launch by the CTA that computes
+// a frame's SDF set-up (sdf_frame_setup), so they are plain pointers.  vposed == nullptr: v_posed is not stored (the few
+// consumers recompute it, vposed_of).
 struct SkinArgs {
     const float* poffT; const float* ST; const float* Phi; const float* At; int ldA;
     const int* ell_j; const float* ell_w; int KW; int N;
@@ -412,236 +412,6 @@ __device__ __forceinline__ void sdf_setup_frames(const SdfSetupArgs& sa, const f
     __threadfence();
     for (int k = 0; mine; mine &= mine - 1, ++k)
         if (k % nwarps == warp) sdf_frame_setup(sa, bboxp, verts, N, nbox, base + __ffs(mine) - 1, lane);
-}
-
-// skin_kernel's CTA (vbx, vby) of a virtual grid (nchunks, frame groups); `sk` = kSkinSmem bytes of shared memory.
-// All kSkinThreads threads must call.
-__device__ __forceinline__ void skin_body(float* sk, const SkinArgs& ar, const int na, const int cta_slots, const int vbx, const int vby) {
-    const float* poffT = ar.poffT; const float* __restrict__ ST = ar.ST; const float* Phi = ar.Phi; const float* At = ar.At;
-    const int ldA = ar.ldA, KW = ar.KW, N = ar.N;
-    const int* __restrict__ ell_j = ar.ell_j; const float* __restrict__ ell_w = ar.ell_w;
-    float* vposed = ar.vposed; float* verts = ar.verts; float* bboxp = ar.bboxp;
-    float* As = sk;                                   // [24 joints][32 lanes][12]
-    float* Bs = As + kSkinFloats * 32;                // [10][32]
-    float* Ovp = Bs + kBetas * 32;                    // [32][193] (only when v_posed is stored)
-    float* Ov = vposed ? Ovp + 32 * kSkinOutLd : Ovp; // [32][193]
-    float* Bb = Ov + 32 * kSkinOutLd;                 // [8 warps][32 lanes][6] values, then [..][6] indices
-    float* Sts = Bb + 8 * 32 * 6 * 2;                 // [64][33] shapedirs rows | template of this CTA's vertices
-    float* Ews = Sts + kSkinV * 33;                   // [64][KW] skinning weights of the chunk
-    int* Ejs = reinterpret_cast<int*>(Ews + kSkinV * kSkinEllMax);   // [64][KW] their joints
-    const bool ell_smem = KW <= kSkinEllMax;
-    const int f0 = vby * 32;
-    if (f0 >= na) return;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int slotc = min(f0 + lane, na - 1);
-    // chunks per CTA from the number of ACTIVE frame groups: one chunk each while the active CTAs fit in one wave
-    // (latency at the tail of a stage), several once they do not (the 36 KB of transforms are then loaded once)
-    const int nchunks = (N + kSkinV - 1) / kSkinV;
-    const int per_cta = (nchunks * ((na + 31) / 32) + cta_slots - 1) / cta_slots;
-    const int nx = (nchunks + per_cta - 1) / per_cta;
-    if (vbx >= nx) return;
-    // the 32 frames' transforms and shape coefficients are loaded once and reused for every vertex chunk of this CTA
-    // layout [joint][lane][12]: a lane's 3x4 transform is three conflict-free LDS.128 (lane stride 48 B)
-    for (int e = tid; e < kSkinFloats * 32; e += kSkinThreads) {
-        const int jc = e >> 5, ln = e & 31;
-        As[((jc / 12) * 32 + ln) * 12 + jc % 12] = At[(size_t)jc * ldA + min(f0 + ln, na - 1)];
-    }
-    for (int e = tid; e < kBetas * 32; e += kSkinThreads)
-        Bs[e] = Phi[(size_t)min(f0 + (e & 31), na - 1) * kFeatPad + kPoseBasis + (e >> 5)];
-    constexpr int kVw = kSkinV / 8;                                       // vertices per warp and chunk
-    float beta[kBetas];
-    bool have_beta = false;
-    for (int ch = vbx; ch < nchunks; ch += nx) {
-        const int v0 = ch * kSkinV;
-        // pose offsets of this warp's vertices: 24 independent coalesced loads in flight before anything waits
-        float pf[kVw][3];
-#pragma unroll
-        for (int i = 0; i < kVw; ++i) {
-            const int n = v0 + warp * kVw + i;
-#pragma unroll
-            for (int c = 0; c < 3; ++c) pf[i][c] = n < N ? poffT[(size_t)(3 * n + c) * ldA + slotc] : 0.f;
-        }
-        __syncthreads();                                                  // previous chunk's staging buffers are free
-        for (int e = tid; e < kSkinV * 33; e += kSkinThreads) Sts[e] = (v0 * 33 + e < N * 33) ? ST[(size_t)v0 * 33 + e] : 0.f;
-        if (ell_smem)
-            for (int e = tid; e < kSkinV * KW; e += kSkinThreads) {
-                const bool in = (size_t)v0 * KW + e < (size_t)N * KW;
-                Ews[e] = in ? ell_w[(size_t)v0 * KW + e] : 0.f;
-                Ejs[e] = in ? ell_j[(size_t)v0 * KW + e] : 0;
-            }
-        __syncthreads();
-        if (!have_beta) {
-#pragma unroll
-            for (int l = 0; l < kBetas; ++l) beta[l] = Bs[l * 32 + lane];
-            have_beta = true;
-        }
-        float blo[3] = {3e38f, 3e38f, 3e38f}, bhi[3] = {-3e38f, -3e38f, -3e38f};
-        int bilo[3] = {0, 0, 0}, bihi[3] = {0, 0, 0};
-#pragma unroll
-        for (int i = 0; i < kVw; ++i) {
-            const int li = warp * kVw + i;
-            const int n = v0 + li;
-            if (n < N) {
-                float vp[3], vvv[3];
-                skin_vertex(Sts + li * 33, beta, pf[i], ell_smem ? Ejs : ell_j, ell_smem ? Ews : ell_w, KW,
-                            ell_smem ? (size_t)li : (size_t)n,
-                            [&](int j, float* a12) {
-                                const float4* q = reinterpret_cast<const float4*>(As + (j * 32 + lane) * 12);
-                                const float4 q0 = q[0], q1 = q[1], q2 = q[2];
-                                a12[0] = q0.x; a12[1] = q0.y; a12[2] = q0.z; a12[3] = q0.w; a12[4] = q1.x; a12[5] = q1.y;
-                                a12[6] = q1.z; a12[7] = q1.w; a12[8] = q2.x; a12[9] = q2.y; a12[10] = q2.z; a12[11] = q2.w;
-                            }, vp, vvv);
-#pragma unroll
-                for (int r = 0; r < 3; ++r) {
-                    const float vv = vvv[r];
-                    if (vposed) Ovp[lane * kSkinOutLd + 3 * li + r] = vp[r];
-                    Ov[lane * kSkinOutLd + 3 * li + r] = vv;
-                    if (vv < blo[r]) { blo[r] = vv; bilo[r] = n; }       // strict: ties keep the lowest vertex index
-                    if (vv > bhi[r]) { bhi[r] = vv; bihi[r] = n; }
-                }
-            }
-        }
-        int* Bi = reinterpret_cast<int*>(Bb + 8 * 32 * 6);
-#pragma unroll
-        for (int r = 0; r < 3; ++r) {
-            Bb[(warp * 32 + lane) * 6 + r] = blo[r]; Bb[(warp * 32 + lane) * 6 + 3 + r] = bhi[r];
-            Bi[(warp * 32 + lane) * 6 + r] = bilo[r]; Bi[(warp * 32 + lane) * 6 + 3 + r] = bihi[r];
-        }
-        __syncthreads();
-        const int ncol = 3 * min(kSkinV, N - v0);                         // contiguous floats of this chunk per frame
-        for (int fl = warp; fl < 32; fl += 8) {                           // a warp stores one frame's row segment at a time
-            const int slot = f0 + fl;
-            if (slot >= na) break;
-            const size_t off = ((size_t)slot * N + v0) * 3;
-            for (int col = lane; col < ncol; col += 32) {
-                if (vposed) vposed[off + col] = Ovp[fl * kSkinOutLd + col];
-                verts[off + col] = Ov[fl * kSkinOutLd + col];
-            }
-        }
-        if (bboxp && warp == 0 && f0 + lane < na) {       // fold the 8 warps' vertex groups (ascending vertex index)
-            float lo[3], hi[3];
-            int ilo[3], ihi[3];
-#pragma unroll
-            for (int r = 0; r < 3; ++r) { lo[r] = Bb[lane * 6 + r]; hi[r] = Bb[lane * 6 + 3 + r]; ilo[r] = Bi[lane * 6 + r]; ihi[r] = Bi[lane * 6 + 3 + r]; }
-            for (int w2 = 1; w2 < 8; ++w2)
-#pragma unroll
-                for (int r = 0; r < 3; ++r) {
-                    const float l2 = Bb[(w2 * 32 + lane) * 6 + r], h2 = Bb[(w2 * 32 + lane) * 6 + 3 + r];
-                    if (l2 < lo[r]) { lo[r] = l2; ilo[r] = Bi[(w2 * 32 + lane) * 6 + r]; }
-                    if (h2 > hi[r]) { hi[r] = h2; ihi[r] = Bi[(w2 * 32 + lane) * 6 + 3 + r]; }
-                }
-            float* bp = bboxp + ((size_t)(f0 + lane) * nchunks + ch) * 12;
-#pragma unroll
-            for (int r = 0; r < 3; ++r) { bp[r] = lo[r]; bp[3 + r] = hi[r]; bp[6 + r] = __int_as_float(ilo[r]); bp[9 + r] = __int_as_float(ihi[r]); }
-        }
-    }
-    if (ar.sdf.rec != nullptr) {                          // per-frame SDF set-up by the last CTA of each frame (sdf_setup_frames)
-        __threadfence();
-        __syncthreads();
-        unsigned* s_mine = reinterpret_cast<unsigned*>(Bb);   // staging buffers are free once every thread is here
-        if (warp == 0) {
-            bool last = false;
-            if (f0 + lane < na) {
-                const int cnt = (nchunks - vbx + nx - 1) / nx;                    // chunks this CTA skinned for each frame
-                last = atomicAdd(ar.sdf.arrive + f0 + lane, cnt) + cnt == nchunks;
-            }
-            const unsigned m = __ballot_sync(0xffffffffu, last);
-            if (lane == 0) *s_mine = m;
-        }
-        __syncthreads();
-        sdf_setup_frames(ar.sdf, bboxp, verts, N, nchunks, f0, *s_mine, warp, lane, kSkinThreads / 32);
-    }
-    __syncthreads();
-}
-
-// The same for a handful of frames (the straggler tail of a fit): with lane = frame almost every lane of skin_kernel
-// idles and its fixed costs (36 KB of transforms per CTA, staging, three barriers per chunk) are pure latency.  Here
-// lane = vertex, a CTA owns one 64-vertex chunk (= one box partial) and loops over the <= kSkinSmallMax frames.
-constexpr int kSkinSmallMax = 8;
-constexpr int kSkinSmallThreads = 64;
-static_assert(kSkinSmallThreads == kSkinV, "one thread per vertex of a box chunk");
-
-struct SkinSmallSmem {
-    float As[kSkinSmallMax][kSkinFloats];
-    float Bs[kSkinSmallMax][kBetas];
-    float s_b[kSkinSmallMax][6];
-    int s_i[kSkinSmallMax][6];
-    unsigned mine;                         // frames whose SDF set-up this CTA computes
-};
-
-// skin_small_kernel's CTA for one 64-vertex chunk, executed by the kSkinSmallThreads threads t = 0..63 of a thread group
-// that synchronises on named barrier `bar` (0 with a 64-thread CTA = __syncthreads).
-__device__ __forceinline__ void skin_small_body(SkinSmallSmem& sm, const SkinArgs& ar, int na_in, const int chunk, const int nchunks,
-                                                const int t, const int bar) {
-    const float* poffT = ar.poffT; const float* __restrict__ ST = ar.ST; const float* Phi = ar.Phi; const float* At = ar.At;
-    const int ldA = ar.ldA, KW = ar.KW, N = ar.N;
-    const int* __restrict__ ell_j = ar.ell_j; const float* __restrict__ ell_w = ar.ell_w;
-    float* vposed = ar.vposed; float* verts = ar.verts; float* bboxp = ar.bboxp;
-    auto& As = sm.As; auto& Bs = sm.Bs; auto& s_b = sm.s_b; auto& s_i = sm.s_i;
-    const int na = min(na_in, kSkinSmallMax);
-    if (na <= 0) return;
-    const int lane = t & 31, warp = t >> 5;
-    const int n = chunk * kSkinSmallThreads + t;
-    for (int e = t; e < na * kSkinFloats; e += kSkinSmallThreads) As[e / kSkinFloats][e % kSkinFloats] = At[(size_t)(e % kSkinFloats) * ldA + e / kSkinFloats];
-    for (int e = t; e < na * kBetas; e += kSkinSmallThreads) Bs[e / kBetas][e % kBetas] = Phi[(size_t)(e / kBetas) * kFeatPad + kPoseBasis + e % kBetas];
-    float st[33];
-    if (n < N) {
-#pragma unroll
-        for (int q = 0; q < 33; ++q) st[q] = ST[(size_t)n * 33 + q];
-    }
-    asm volatile("bar.sync %0, %1;" ::"r"(bar), "r"(kSkinSmallThreads) : "memory");
-    for (int f = 0; f < na; ++f) {
-        float lo[3] = {3e38f, 3e38f, 3e38f}, hi[3] = {-3e38f, -3e38f, -3e38f};
-        int ilo[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff}, ihi[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff};
-        if (n < N) {
-            float poff[3], vp[3], vv[3];
-#pragma unroll
-            for (int c = 0; c < 3; ++c) poff[c] = poffT[(size_t)(3 * n + c) * ldA + f];
-            skin_vertex(st, Bs[f], poff, ell_j, ell_w, KW, (size_t)n,
-                        [&](int j, float* a12) {
-#pragma unroll
-                            for (int c = 0; c < 12; ++c) a12[c] = As[f][j * 12 + c];
-                        }, vp, vv);
-            const size_t off = ((size_t)f * N + n) * 3;
-#pragma unroll
-            for (int r = 0; r < 3; ++r) {
-                if (vposed) vposed[off + r] = vp[r];
-                verts[off + r] = vv[r];
-                lo[r] = vv[r]; hi[r] = vv[r]; ilo[r] = n; ihi[r] = n;
-            }
-        }
-        if (bboxp) {               // box of the chunk: extreme value, ties -> lowest vertex index (as skin_kernel)
-#pragma unroll
-            for (int r = 0; r < 3; ++r) { warp_argmin(lo[r], ilo[r]); warp_argmax(hi[r], ihi[r]); }
-            if (warp == 1 && lane == 0) {
-#pragma unroll
-                for (int r = 0; r < 3; ++r) { s_b[f][r] = lo[r]; s_b[f][3 + r] = hi[r]; s_i[f][r] = ilo[r]; s_i[f][3 + r] = ihi[r]; }
-            }
-            asm volatile("bar.sync %0, %1;" ::"r"(bar), "r"(kSkinSmallThreads) : "memory");
-            if (warp == 0 && lane == 0) {
-                float* bp = bboxp + ((size_t)f * nchunks + chunk) * 12;
-#pragma unroll
-                for (int r = 0; r < 3; ++r) {
-                    const float l2 = s_b[f][r], h2 = s_b[f][3 + r];
-                    const int il2 = s_i[f][r], ih2 = s_i[f][3 + r];
-                    if (l2 < lo[r] || (l2 == lo[r] && il2 < ilo[r])) { lo[r] = l2; ilo[r] = il2; }
-                    if (h2 > hi[r] || (h2 == hi[r] && ih2 < ihi[r])) { hi[r] = h2; ihi[r] = ih2; }
-                    bp[r] = lo[r]; bp[3 + r] = hi[r]; bp[6 + r] = __int_as_float(ilo[r]); bp[9 + r] = __int_as_float(ihi[r]);
-                }
-            }
-        }
-    }
-    if (ar.sdf.rec != nullptr) {                          // per-frame SDF set-up by the last CTA of each frame (sdf_setup_frames)
-        __threadfence();
-        asm volatile("bar.sync %0, %1;" ::"r"(bar), "r"(kSkinSmallThreads) : "memory");
-        if (warp == 0) {
-            const bool last = lane < na && atomicAdd(ar.sdf.arrive + lane, 1) + 1 == nchunks;   // one chunk per CTA
-            const unsigned m = __ballot_sync(0xffffffffu, last);
-            if (lane == 0) sm.mine = m;
-        }
-        asm volatile("bar.sync %0, %1;" ::"r"(bar), "r"(kSkinSmallThreads) : "memory");
-        sdf_setup_frames(ar.sdf, bboxp, verts, N, nchunks, 0, sm.mine, warp, lane, kSkinSmallThreads / 32);
-    }
 }
 
 }  // namespace mvs
