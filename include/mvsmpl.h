@@ -252,7 +252,8 @@ int mvs_sdf_grid(mvs_ctx* ctx, float* phi_dev, const int* faces_dev, int num_fac
  * L-BFGS stage -- out of shared memory;  1 = always the batched multi-kernel path (used by tests to cross-check);
  * 2 = like 0, but mvs_fit / mvs_fit_host keep a barrier between stages (one run per stage, as mvs_lbfgs_run);
  * 3 = like 0, and mvs_closure with the SDF term on (loss and gradient only) runs ONE evaluation through the dense-regime
- *     kernels the optimiser uses for SDF stages instead of the batched reference chain (parity tests; synchronises). */
+ *     kernels the optimiser uses for SDF stages instead of the batched reference chain (parity tests; synchronises).
+ *     Mode 3 affects mvs_closure only: the optimiser entry points (mvs_lbfgs_run, mvs_lbfgs_step, mvs_fit*) run as in 0. */
 int mvs_set_exec_mode(mvs_ctx* ctx, int mode);
 
 /* ---- measurement support (bench.py): per-kernel device time with CUDA events recorded on the launching

@@ -195,6 +195,26 @@ int mvs_set_model(mvs_ctx* ctx, const mvs_model_desc* d) {
     m.N = N;
     m.F = d->faces ? d->n_faces : 0;
     for (int j = 0; j < kJoints; ++j) ctx->parents.p[j] = d->parents[j];
+    {   // level schedule of the tree (ctx->chain is zero-initialised)
+        ChainSched& cs = ctx->chain;
+        int depth[kJoints];
+        depth[0] = 0;
+        int maxd = 0;
+        for (int j = 1; j < kJoints; ++j) { depth[j] = depth[d->parents[j]] + 1; if (depth[j] > maxd) maxd = depth[j]; }
+        cs.nlev = maxd + 1;
+        int o = 0;
+        for (int L = 0; L <= maxd; ++L) {
+            cs.lev_ptr[L] = (unsigned char)o;
+            for (int j = 0; j < kJoints; ++j) if (depth[j] == L) cs.lev_j[o++] = (unsigned char)j;
+        }
+        for (int L = maxd + 1; L <= kJoints; ++L) cs.lev_ptr[L] = (unsigned char)o;
+        o = 0;
+        for (int p = 0; p < kJoints; ++p) {
+            cs.ch_ptr[p] = (unsigned char)o;
+            for (int j = kJoints - 1; j >= 1; --j) if (d->parents[j] == p) cs.ch_j[o++] = (unsigned char)j;
+        }
+        cs.ch_ptr[kJoints] = (unsigned char)o;
+    }
 
     // Qk rows: [posedirs column | shapedirs row | v_template | pad]
     {
@@ -442,6 +462,9 @@ int mvs_set_batch(mvs_ctx* ctx, int B) {
     MVS_CUDA_OK(ctx, cudaMemset(w.At, 0, (size_t)kSkinFloats * w.ldA * sizeof(float)));
     MVS_CUDA_OK(ctx, cudaMemset(w.Phi, 0, (size_t)w.ldA * kFeatPad * sizeof(float)));
     MVS_CUDA_OK(ctx, cudaMemset(w.PhiTc, 0, (size_t)2 * w.ldA * kFeatPad * sizeof(float)));
+    if ((rc = closure_set_attributes(ctx)) || (rc = resident_set_attributes(ctx)) || (rc = tc_set_attributes(ctx)) ||
+        (rc = sdf_set_attributes(ctx)))
+        return rc;
     MVS_LAUNCH(ctx, KID_MISC, 0, iota_kernel<<<(B + 255) / 256, 256>>>(w.fidx, B, w.na));
     MVS_CUDA_OK(ctx, cudaDeviceSynchronize());
     return MVS_OK;
@@ -508,7 +531,7 @@ int mvs_closure(mvs_ctx* ctx, const float* params_dev, float* loss_dev, float* g
                 "mvs_closure: model, cameras, batch, keypoints and loss config must be set first");
     MVS_REQUIRE(ctx, params_dev, "mvs_closure: params_dev is NULL");
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    return launch_closure(ctx, params_dev, loss_dev, grad_dev, joints_dev, proj_dev, verts_dev, (cudaStream_t)stream);
+    return evaluate_closure(ctx, params_dev, loss_dev, grad_dev, joints_dev, proj_dev, verts_dev, (cudaStream_t)stream);
 }
 
 int mvs_forward(mvs_ctx* ctx, const float* params_dev, float* joints_dev, float* verts_dev, void* stream) {

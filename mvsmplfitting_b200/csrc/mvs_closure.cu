@@ -729,40 +729,33 @@ __global__ void fill_kernel(float* p, float v, size_t n) {
     if (i < n) p[i] = v;
 }
 
+int closure_set_attributes(mvs_ctx* ctx) {
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertFwdSmem));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertBwdSmem));
+    return MVS_OK;
+}
+
 int launch_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev,
                    float* proj_dev, float* verts_dev, cudaStream_t st, bool geometry_only) {
     DevModel& m = ctx->m;
     Workspace& w = ctx->ws;
     const LossParams& lp = ctx->loss;
     const int B = w.B;
-    const bool sdf_on = !geometry_only && lp.interpenetration && lp.coll_loss_weight > 0.f;
+    const bool sdf_on = !geometry_only && sdf_term_on(lp);
     const bool dense = sdf_on || verts_dev != nullptr;
     const bool have_grad = grad_dev != nullptr;
-    if (!dense && !geometry_only && resident_closure_available(ctx))     // sparse regime: one fused launch
-        return launch_closure_resident(ctx, x_dev, loss_dev, grad_dev, joints_dev, proj_dev, st);
-    if (sdf_on && ctx->exec_mode == 3 && !verts_dev && !joints_dev && !proj_dev && hybrid_available(ctx))
-        return dense_regime_closure(ctx, x_dev, loss_dev, grad_dev, st);       // the optimiser's own SDF-stage kernels
-    if (lp.use_vposer == 2 && !geometry_only)      // geometry only: the pose slot is axis-angle by definition (mvs_forward)
-        return set_error(ctx, MVS_ERR_INVALID, "use_vposer = 2 (VPoser decode on the device) is implemented in the "
-                                               "frame-resident closure only (no vertices, no SDF term, exec mode 0 or 2)");
     const int nv = dense ? m.N : m.nsup;
     const int* vlist = dense ? nullptr : m.sup;
     const Parents par = ctx->parents;
     const int ftiles = (B + kTileF - 1) / kTileF;
-
-    if (!ctx->attr_done) {
-        MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertFwdSmem));
-        MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertBwdSmem));
-        ctx->attr_done = true;
-    }
 
     MVS_LAUNCH(ctx, KID_FRAME_FWD, st,
                frame_fwd_kernel<<<B, kFrameThreads, 0, st>>>(x_dev, w.fidx, w.na, par, m.Jt, m.JS, w.Phi, w.PhiTc, w.At, w.ldA,
                                                              w.gchain, w.slot_tr));
     // with the SDF term this chain is the plain-fp32 cross-check of the dense-regime kernels: the sampled distances are
     // voxel-sized numbers, TF32 pose offsets would cost them 1e-5 .. 1e-4 relative (the dense-regime kernels re-evaluate
-    // the vertices that matter in fp32 instead, mvs_sdf_dev.cuh)
-    if (dense && !sdf_on && tc_available(ctx)) {
+    // the vertices that matter in fp32 instead, mvs_sdf_dev.cuh).  Exec mode 1 keeps the whole chain SIMT.
+    if (dense && !sdf_on && ctx->exec_mode != 1) {
         int rc = launch_vertex_fwd_tc(ctx, st, true, false);       // wgmma / TMA path (mvs_tc.cu)
         if (rc) return rc;
     } else {

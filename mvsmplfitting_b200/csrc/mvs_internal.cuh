@@ -23,6 +23,16 @@ constexpr int kPartFloats = kSkinFloats + kFeatPad; // per (strip, frame) partia
 
 struct Parents { int p[kJoints]; };
 
+// Depth-level schedule of the kinematic tree: joints of one level only depend on the level above (forward) / below
+// (adjoint), so a level is processed by parallel lane groups and the 23-step serial chain becomes <= 9 level steps
+// for SMPL.  Children are listed in DESCENDING index order: gathering them in that order reproduces the summation
+// order of the plain "for j = 23 .. 1" reverse sweep bit for bit.
+struct ChainSched {
+    int nlev;
+    unsigned char lev_ptr[kJoints + 1], lev_j[kJoints];
+    unsigned char ch_ptr[kJoints + 1], ch_j[kJoints];
+};
+
 struct CamSet {
     int num_views;
     CamF cam[kMaxViews];
@@ -36,6 +46,11 @@ struct LossParams {
     int num_gaussians;
     int anchor_on;
 };
+
+inline bool sdf_term_on(const LossParams& lp) { return lp.interpenetration && lp.coll_loss_weight > 0.f; }
+
+// execution regime of an optimiser run (DESIGN.md section 4)
+enum Regime { kResident, kDense, kBatched };
 
 // Model constants resident in HBM.  Layouts chosen for the kernels, not the reference's:
 //   Qk  [3N][224]   row (3n+c) = [posedirs[:,3n+c] (207) | shapedirs[n,c,:] (10) | v_template[n,c] | 0-pad]
@@ -204,10 +219,9 @@ struct mvs_ctx {
     mvs::LossParams loss{};
     mvs::Workspace ws;
     mvs::Parents parents{};
-    bool attr_done = false, attr_done_res = false, attr_done_step = false;
-    int attr_res_lbfgs_smem = 0;
+    mvs::ChainSched chain{};         // level schedule of parents
     bool anchor_enabled = false;
-    int exec_mode = 0;               // 0 auto (frame-resident kernels where they apply), 1 batched kernels only
+    int exec_mode = 0;               // mvs_set_exec_mode: 0 auto, 1 batched chain only, 2 stage barriers, 3 dense-round closures
     bool have_model = false, have_cams = false, have_kp = false, have_loss = false;
     std::vector<void*> allocs;       // everything cudaMalloc'ed, freed in mvs_destroy
     mvs::LbfgsState* lbfgs = nullptr;    // optimiser state (mvs_lbfgs.cu)
@@ -295,38 +309,40 @@ __device__ __forceinline__ void warp_argmax(float& v, int& idx) {
 template <class T> int dev_alloc(mvs_ctx* ctx, T** p, size_t count);
 template <class T> int dev_upload(mvs_ctx* ctx, T** p, const T* host, size_t count);
 
-// closure launcher (mvs_closure.cu): evaluates all active slots.  x_dev [B][86].
+// mvs_lbfgs.cu: mvs_closure through the frame-resident closure, a dense round or the batched chain
+int evaluate_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev, float* proj_dev,
+                     float* verts_dev, cudaStream_t st);
+// dynamic shared memory limits of each unit's kernels (largest launch), set by mvs_set_batch
+int closure_set_attributes(mvs_ctx* ctx);
+int resident_set_attributes(mvs_ctx* ctx);
+int tc_set_attributes(mvs_ctx* ctx);           // also encodes the tensor maps over Qk and PhiTc
+int sdf_set_attributes(mvs_ctx* ctx);
+// batched chain (mvs_closure.cu): evaluates all active slots.  x_dev [B][86].
 int launch_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev,
                    float* proj_dev, float* verts_dev, cudaStream_t st, bool geometry_only = false);
 int launch_sdf_terms(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);   // mvs_sdf.cu
 // mvs_resident.cu: frame-resident (one CTA per frame) closure and whole-stage optimiser for the sparse regime
-bool resident_closure_available(const mvs_ctx* ctx);
+bool resident_supported(const mvs_ctx* ctx);   // the model fits the frame-resident kernels
+bool dense_supported(const mvs_ctx* ctx);      // the mesh fits frame_step's list of 256-vertex blocks
 int launch_vposer_decode(mvs_ctx* ctx, const float* x_dev, float* body_pose_dev, cudaStream_t st);
 int launch_closure_resident(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev,
                             float* proj_dev, cudaStream_t st);
-bool resident_lbfgs_available(const mvs_ctx* ctx, int history);
 int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
                           const LossParams* lp_tab_host, int nstages, FrameScalars* frame_scalars_out, float* last_grad_dev,
                           cudaStream_t st, const int2* stage_rng_dev);
 // dense regime (SDF term): per round  posedirs_gemm_tc -> skin -> sdf_fused -> frame_step
-bool hybrid_available(const mvs_ctx* ctx);
 int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);                      // mvs_closure.cu
 int launch_sdf_fused(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu
 int ensure_sdf_setup_ws(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu: set-up records, arrival counters (zeroed on st), boxes
 SdfSetupArgs make_sdf_setup_args(mvs_ctx* ctx);          // mvs_sdf.cu
 // mvs_tc.cu: wgmma / TMA dense vertex forward
 int tc_upload_model(mvs_ctx* ctx);                 // after m.Qk is on the device
-bool tc_available(const mvs_ctx* ctx);
 int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool sdf_setup);
 int tc_check_error(mvs_ctx* ctx);
-float* tc_poffT(mvs_ctx* ctx);                 // [3N][ldA] pose offsets of the tensor-core contraction (allocated on first use)
-int tc_prepare(mvs_ctx* ctx);                  // tensor maps + pose-offset buffer (idempotent)
+float* tc_poffT(mvs_ctx* ctx);                 // [3N][ldA] pose offsets of the tensor-core contraction (written by launch_vertex_fwd_tc)
 int launch_frame_step(mvs_ctx* ctx, float* params_dev, const LbfgsState& L, const LbfgsCfg& cfg, int nstages, cudaStream_t st);
 int frame_step_begin_run(mvs_ctx* ctx, cudaStream_t st);                 // mvs_resident.cu
 int launch_frame_fwd_dense(mvs_ctx* ctx, const float* x_dev, const LbfgsState& L, int nstages, cudaStream_t st);   // mvs_resident.cu
-bool resident_lbfgs_available_for(const mvs_ctx* ctx, const LossParams& lp, int history);
-bool hybrid_available_for(const mvs_ctx* ctx, const LossParams& lp);
-int dense_regime_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, cudaStream_t st);   // mvs_lbfgs.cu
 int make_loss_params(mvs_ctx* ctx, const mvs_loss_config* c, LossParams* out);      // mvs_api.cu: validation + conversion
 int sdf_grid_launch(mvs_ctx* ctx, float* phi, const int* faces, int num_faces, const float* verts, int batch,
                     int n_verts, int G, cudaStream_t st);

@@ -7,7 +7,7 @@
 //   utils/fitting.py:71-142        FittingMonitor.run_fitting (NaN/Inf guard, ftol, gtol)
 //
 // The reference runs this loop in Python with a blocking float(closure()) per evaluation
-// (lbfgs_ls.py:251,281).  Here no scalar leaves the GPU.  run_stage picks one of three execution regimes per
+// (lbfgs_ls.py:251,281).  Here no scalar leaves the GPU.  stage_regime picks one of three execution regimes per
 // group of stages (DESIGN.md section 4):
 //   frame-resident   one CTA per frame runs closure + state machine for ALL stages of the group inside ONE launch
 //                    (mvs_resident.cu: lbfgs_resident_kernel)
@@ -187,7 +187,17 @@ struct RunOpts {
     bool some_inactive = false;       // some frame has no stage in this run
 };
 
-enum Regime { kResident, kDense, kBatched };
+// How a run evaluates the stage lp (step: mvs_lbfgs_step).  The frame-resident optimiser holds histories up to 100 and runs
+// whole stages; the dense rounds serve the SDF term, in step mode only with use_vposer = 2, which the batched chain lacks.
+static Regime stage_regime(const mvs_ctx* ctx, const LossParams& lp, int history, bool step) {
+    if (ctx->exec_mode == 1 || !resident_supported(ctx)) return kBatched;
+    if (!sdf_term_on(lp)) return !step && history <= 100 ? kResident : kBatched;
+    return (!step || lp.use_vposer == 2) && dense_supported(ctx) ? kDense : kBatched;
+}
+
+static bool resident_closure_applies(const mvs_ctx* ctx, bool want_verts) {
+    return !want_verts && !sdf_term_on(ctx->loss) && ctx->exec_mode != 1 && resident_supported(ctx);
+}
 
 // Shared set-up of a run: optimiser configuration, state for history size H, zeroed totals, stage table on the device
 static int begin_run(mvs_ctx* ctx, const mvs_lbfgs_config* c, bool step, const LossParams* lps, int nst, LbfgsCfg* cfg,
@@ -296,8 +306,8 @@ static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int n
     return tc_check_error(ctx);
 }
 
-// Batched chain: launch_closure + lbfgs_advance_kernel + lbfgs_compact_kernel per round, the host reads the active count
-// after every chunk of rounds
+// Batched chain: the closure (frame-resident where it applies, launch_closure otherwise) + lbfgs_advance_kernel +
+// lbfgs_compact_kernel per round, the host reads the active count after every chunk of rounds
 static int run_batched(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, bool vp2, cudaStream_t st) {
     LbfgsState& S = *ctx->lbfgs;
     Workspace& w = ctx->ws;
@@ -306,9 +316,11 @@ static int run_batched(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, boo
     const long long max_rounds = (long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8;
     long long rounds = 0;
     int na_host = B;
+    const bool resident = resident_closure_applies(ctx, false);     // (not the dense-round closure: it restarts the optimiser)
     while (na_host > 0 && rounds < max_rounds) {
         for (int r = 0; r < chunk; ++r) {
-            const int rc = launch_closure(ctx, S.x_eval, S.loss_eval, S.g_eval, nullptr, nullptr, nullptr, st);
+            const int rc = resident ? launch_closure_resident(ctx, S.x_eval, S.loss_eval, S.g_eval, nullptr, nullptr, st)
+                                    : launch_closure(ctx, S.x_eval, S.loss_eval, S.g_eval, nullptr, nullptr, nullptr, st);
             if (rc) return rc;
             MVS_LAUNCH(ctx, KID_LBFGS_ADVANCE, st, lbfgs_advance_kernel<<<B, 32, 0, st>>>(S, cfg, params_dev, w.fidx, w.na, vp2 ? 32 : kOffTransl - kOffPose));
             MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
@@ -356,24 +368,23 @@ static int run_stage(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, con
     LbfgsState& S = *ctx->lbfgs;
     Workspace& w = ctx->ws;
     const int B = w.B;
-    if (!o.step && resident_lbfgs_available(ctx, cfg.history)) {
+    const Regime rg = stage_regime(ctx, ctx->loss, cfg.history, o.step);
+    if (rg == kResident) {
         // sparse regime: every frame runs its whole stage inside one CTA (mvs_resident.cu): one launch, no rounds
         rc = launch_lbfgs_resident(ctx, params_dev, cfg, cfg.history, S.lp_tab, lps, nst, S.sc, o.last_grad, st, o.stage_rng);
         return rc ? rc : end_run(ctx, kResident, final_loss_dev, nullptr, stats, st);
     }
     // use_vposer = 2 (VPoser decode on the device) exists in the frame-resident closure and in the dense-regime kernels, not in
     // the SIMT reference chain.  mvs_lbfgs_step therefore runs its one step() per call through the dense rounds when the SDF
-    // term is on, and through launch_closure's frame-resident kernel + lbfgs_advance_kernel otherwise.
+    // term is on, and through the frame-resident closure + lbfgs_advance_kernel otherwise.
     const bool vp2 = ctx->loss.use_vposer == 2;
-    const bool sdf_on = ctx->loss.interpenetration && ctx->loss.coll_loss_weight > 0.f;
-    if (vp2 && (sdf_on ? !hybrid_available(ctx) : !resident_closure_available(ctx)))
+    if (rg == kBatched && vp2 && !resident_closure_applies(ctx, false))
         return set_error(ctx, MVS_ERR_INVALID, "use_vposer = 2 (VPoser decode on the device) is not implemented in the batched "
                                                "reference chain (exec mode 1): use use_vposer = 1 there");
     MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
     MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_init_kernel<<<B, 32, 0, st>>>(S, params_dev, B, o.reset ? 1 : 0, nst, o.stage_rng));
     if (o.some_inactive)                                    // frames without a stage in this run leave the active list now
         MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
-    const Regime rg = (!o.step || vp2) && hybrid_available(ctx) ? kDense : kBatched;
     rc = rg == kDense ? run_dense(ctx, params_dev, cfg, nst, st) : run_batched(ctx, params_dev, cfg, vp2, st);
     return rc ? rc : end_run(ctx, rg, final_loss_dev, o.last_grad, stats, st);
 }
@@ -381,7 +392,7 @@ static int run_stage(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, con
 // One closure evaluation through the dense-regime kernels (posedirs_gemm_tc -> skin -> sdf_fused -> frame_step with the
 // optimiser step switched off): mvs_closure in exec mode 3.  Exists so that parity tests can compare the loss and every
 // gradient segment of the kernels the optimiser actually runs with the SDF term on (DESIGN.md section 2).
-int dense_regime_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, cudaStream_t st) {
+static int dense_regime_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, cudaStream_t st) {
     const int B = ctx->ws.B;
     int rc = ensure_state(ctx, ctx->lbfgs ? ctx->lbfgs->H : 100);
     if (rc) return rc;
@@ -402,6 +413,22 @@ int dense_regime_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, floa
     if ((rc = tc_check_error(ctx))) return rc;
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
+}
+
+// mvs_closure: the frame-resident closure where it applies; in exec mode 3, loss and gradient with the SDF term through the
+// dense-round kernels the optimiser runs; the batched chain otherwise
+int evaluate_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev, float* proj_dev,
+                     float* verts_dev, cudaStream_t st) {
+    if (resident_closure_applies(ctx, verts_dev != nullptr))
+        return launch_closure_resident(ctx, x_dev, loss_dev, grad_dev, joints_dev, proj_dev, st);
+    if (ctx->exec_mode == 3 && sdf_term_on(ctx->loss) && !joints_dev && !proj_dev && !verts_dev && resident_supported(ctx) &&
+        dense_supported(ctx))
+        return dense_regime_closure(ctx, x_dev, loss_dev, grad_dev, st);
+    if (ctx->loss.use_vposer == 2)
+        return set_error(ctx, MVS_ERR_INVALID, "use_vposer = 2 (VPoser decode on the device) is implemented in the "
+                                               "frame-resident closure (no vertices, no SDF term, exec mode 0, 2 or 3) and in "
+                                               "the dense-round closure of exec mode 3 (SDF term, loss and gradient) only");
+    return launch_closure(ctx, x_dev, loss_dev, grad_dev, joints_dev, proj_dev, verts_dev, st);
 }
 
 // All stages of a fit.  Consecutive stages that run in the same regime are handed to ONE multi-stage run in which
@@ -437,20 +464,16 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
         }
     }
     const int H = opt_cfg->history_size > 0 ? opt_cfg->history_size : 100;
-    auto regime = [&](const LossParams& lp) {
-        if (resident_lbfgs_available_for(ctx, lp, H)) return 0;
-        if (hybrid_available_for(ctx, lp)) return 1;
-        return 2;
-    };
     const int max_run = any_warm ? kMaxStages / 2 : kMaxStages;       // the table holds the cold and the warm slice of a run
     std::vector<int> rng;
     std::vector<LossParams> tab;                                      // stage table of a warm run (read by run_stage)
     int i = 0;
     while (i < n_stages) {
-        const int rg = regime(lps[i]);
+        const Regime rg = stage_regime(ctx, lps[i], H, false);
         int j = i + 1;
-        while (ctx->exec_mode != 2 && rg != 2 && j < n_stages && j - i < max_run && regime(lps[j]) == rg &&
-               lps[j].sdf_grid == lps[i].sdf_grid && lps[j].sdf_all_faces == lps[i].sdf_all_faces)
+        while (ctx->exec_mode != 2 && rg != kBatched && j < n_stages && j - i < max_run &&
+               stage_regime(ctx, lps[j], H, false) == rg && lps[j].sdf_grid == lps[i].sdf_grid &&
+               lps[j].sdf_all_faces == lps[i].sdf_all_faces)
             ++j;
         ctx->loss = lps[i];
         ctx->have_loss = true;
@@ -459,7 +482,7 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
             o.lps = &lps[i];
             o.nst = j - i;
         } else {
-            if (rg == 2)
+            if (rg == kBatched)
                 return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq: warm-started frames are not implemented in the batched "
                                                        "reference chain (exec mode 1 / a model the resident kernels do not take)");
             // table of this run: cold stages i .. j-1, then the warm slice max(i, 2) .. j-1

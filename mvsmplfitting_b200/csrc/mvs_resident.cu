@@ -194,10 +194,30 @@ frame_fwd_resident_kernel(ResidentModel m, const LossParams* __restrict__ lp_tab
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-static bool resident_supported(const mvs_ctx* ctx) {
+bool resident_supported(const mvs_ctx* ctx) {
     const DevModel& m = ctx->m;
-    return ctx->exec_mode != 1 && m.supj_ptr != nullptr && m.nsup + 6 <= kResMaxSup && m.K <= kMaxKeypoints &&
+    return m.supj_ptr != nullptr && m.nsup + 6 <= kResMaxSup && m.K <= kMaxKeypoints &&
            ctx->cams.num_views * m.K <= kResMaxVK && m.M <= kResMaxM;
+}
+
+bool dense_supported(const mvs_ctx* ctx) { return (ctx->m.N + 255) / 256 <= 64; }     // frame_step's block list holds 64 entries
+
+// dynamic shared memory of lbfgs_resident_kernel and frame_step_kernel: one frame, history H (+ the VPoser decoder)
+static size_t frame_smem(int H, bool with_vposer) {
+    return sizeof(ResidentSmem) + (size_t)2 * H * kParams * sizeof(float) + (with_vposer ? sizeof(VposerSmem) : 0);
+}
+
+// lbfgs_resident_kernel runs histories up to 100 (stage_regime), frame_step_kernel up to 128 (the history_size limit)
+int resident_set_attributes(mvs_ctx* ctx) {
+    const int one_frame = (int)(sizeof(ResidentSmem) + sizeof(VposerSmem));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(closure_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, one_frame));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vposer_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, one_frame));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(frame_fwd_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, one_frame));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(lbfgs_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)frame_smem(100, true)));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(frame_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)frame_smem(128, true)));
+    return MVS_OK;
 }
 
 static ResidentModel make_resident_model(const mvs_ctx* ctx) {
@@ -213,39 +233,14 @@ static ResidentModel make_resident_model(const mvs_ctx* ctx) {
     r.vp_w1 = m.vp_w1; r.vp_w2 = m.vp_w2; r.vp_w3 = m.vp_w3; r.vp_w1t = m.vp_w1t; r.vp_w2t = m.vp_w2t; r.vp_w3t = m.vp_w3t;
     r.vp_b1 = m.vp_b1; r.vp_b2 = m.vp_b2; r.vp_b3 = m.vp_b3;
     r.par = ctx->parents;
-    // level schedule of the tree (parents[j] < j is checked in mvs_set_model)
-    int depth[kJoints];
-    depth[0] = 0;
-    int maxd = 0;
-    for (int j = 1; j < kJoints; ++j) { depth[j] = depth[r.par.p[j]] + 1; if (depth[j] > maxd) maxd = depth[j]; }
-    r.cs.nlev = maxd + 1;
-    int o = 0;
-    for (int L = 0; L <= maxd; ++L) {
-        r.cs.lev_ptr[L] = (unsigned char)o;
-        for (int j = 0; j < kJoints; ++j) if (depth[j] == L) r.cs.lev_j[o++] = (unsigned char)j;
-    }
-    for (int L = maxd + 1; L <= kJoints; ++L) r.cs.lev_ptr[L] = (unsigned char)o;
-    o = 0;
-    for (int p = 0; p < kJoints; ++p) {
-        r.cs.ch_ptr[p] = (unsigned char)o;
-        for (int j = kJoints - 1; j >= 1; --j) if (r.par.p[j] == p) r.cs.ch_j[o++] = (unsigned char)j;
-    }
-    r.cs.ch_ptr[kJoints] = (unsigned char)o;
-    for (int q = o; q < kJoints; ++q) r.cs.ch_j[q] = 0;
+    r.cs = ctx->chain;
     return r;
 }
-
-bool resident_closure_available(const mvs_ctx* ctx) { return resident_supported(ctx); }
 
 int launch_closure_resident(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev,
                             float* proj_dev, cudaStream_t st) {
     Workspace& w = ctx->ws;
     const size_t smem = sizeof(ResidentSmem) + (ctx->loss.use_vposer == 2 ? sizeof(VposerSmem) : 0);
-    if (!ctx->attr_done_res) {
-        MVS_CUDA_OK(ctx, cudaFuncSetAttribute(closure_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)(sizeof(ResidentSmem) + sizeof(VposerSmem))));
-        ctx->attr_done_res = true;
-    }
     MVS_LAUNCH(ctx, KID_RESIDENT_CLOSURE, st,
                closure_resident_kernel<<<w.B, kResThreads, smem, st>>>(make_resident_model(ctx), ctx->cams, ctx->loss, x_dev,
                                                                        w.fidx, w.na, w.gt_uv, w.conf, w.joint_w, w.B,
@@ -257,18 +252,11 @@ int launch_closure_resident(mvs_ctx* ctx, const float* x_dev, float* loss_dev, f
 
 int launch_vposer_decode(mvs_ctx* ctx, const float* x_dev, float* body_pose_dev, cudaStream_t st) {
     const size_t smem = sizeof(ResidentSmem) + sizeof(VposerSmem);
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vposer_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     MVS_LAUNCH(ctx, KID_MISC, st,
                vposer_decode_kernel<<<ctx->ws.B, kResThreads, smem, st>>>(make_resident_model(ctx), x_dev, ctx->ws.B, body_pose_dev));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }
-
-bool resident_lbfgs_available_for(const mvs_ctx* ctx, const LossParams& lp, int H) {
-    const bool sdf_on = lp.interpenetration && lp.coll_loss_weight > 0.f;
-    return resident_supported(ctx) && !sdf_on && H <= 100;
-}
-bool resident_lbfgs_available(const mvs_ctx* ctx, int H) { return resident_lbfgs_available_for(ctx, ctx->loss, H); }
 
 int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int H, const LossParams* lp_tab_dev,
                           const LossParams* lph, int nstages, FrameScalars* sc_out, float* last_grad_dev, cudaStream_t st,
@@ -276,11 +264,7 @@ int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, 
     Workspace& w = ctx->ws;
     int with_vposer = 0;
     for (int i = 0; i < nstages; ++i) with_vposer |= (lph[i].use_vposer == 2);
-    const size_t smem = sizeof(ResidentSmem) + (size_t)2 * H * kParams * sizeof(float) + (with_vposer ? sizeof(VposerSmem) : 0);
-    if (ctx->attr_res_lbfgs_smem < (int)smem) {
-        MVS_CUDA_OK(ctx, cudaFuncSetAttribute(lbfgs_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ctx->attr_res_lbfgs_smem = (int)smem;
-    }
+    const size_t smem = frame_smem(H, with_vposer != 0);
     MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
                lbfgs_resident_kernel<<<w.B, kResThreads, smem, st>>>(make_resident_model(ctx), ctx->cams,
                                                                      lp_tab_dev, nstages, cfg, params_dev, w.gt_uv, w.conf,
@@ -302,12 +286,6 @@ int frame_step_begin_run(mvs_ctx* ctx, cudaStream_t st) {
     return MVS_OK;
 }
 
-bool hybrid_available_for(const mvs_ctx* ctx, const LossParams& lp) {
-    const bool sdf_on = lp.interpenetration && lp.coll_loss_weight > 0.f;
-    return resident_supported(ctx) && sdf_on && (ctx->m.N + 255) / 256 <= 64;      // frame_step's block list holds 64 entries
-}
-bool hybrid_available(const mvs_ctx* ctx) { return hybrid_available_for(ctx, ctx->loss); }
-
 static int stages_with_vposer(const LbfgsState& L, int nstages) {
     int v = 0;
     for (int i = 0; i < nstages; ++i) v |= (L.lp_tab_host[i].use_vposer == 2);
@@ -328,21 +306,10 @@ static FrameStepArgs make_frame_step_args(mvs_ctx* ctx, float* params_dev, const
     return a;
 }
 
-static size_t frame_step_smem(int H, bool with_vposer) {
-    return sizeof(ResidentSmem) + (size_t)2 * H * kParams * sizeof(float) + (with_vposer ? sizeof(VposerSmem) : 0);
-}
-
 int launch_frame_step(mvs_ctx* ctx, float* params_dev, const LbfgsState& L, const LbfgsCfg& cfg, int nstages, cudaStream_t st) {
     Workspace& w = ctx->ws;
     const FrameStepArgs a = make_frame_step_args(ctx, params_dev, L, cfg, nstages);
-    const size_t smem = frame_step_smem(L.H, a.with_vposer != 0);
-    if (!ctx->attr_done_step) {
-        MVS_CUDA_OK(ctx, cudaFuncSetAttribute(frame_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)frame_step_smem(L.H, true)));
-        MVS_CUDA_OK(ctx, cudaFuncSetAttribute(frame_fwd_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)(sizeof(ResidentSmem) + sizeof(VposerSmem))));
-        ctx->attr_done_step = true;
-    }
+    const size_t smem = frame_smem(L.H, a.with_vposer != 0);
     MVS_LAUNCH(ctx, KID_FRAME_STEP, st,
                MVS_CUDA_OK(ctx, launch_pdl(frame_step_kernel, dim3(w.na_bound > 0 ? w.na_bound : w.B), dim3(kResThreads), smem, st,
                                            a, (const int*)w.fidx, (const int*)w.na)));
@@ -355,10 +322,6 @@ int launch_frame_step(mvs_ctx* ctx, float* params_dev, const LbfgsState& L, cons
 int launch_frame_fwd_dense(mvs_ctx* ctx, const float* x_dev, const LbfgsState& L, int nstages, cudaStream_t st) {
     if (!stages_with_vposer(L, nstages)) return launch_frame_fwd(ctx, x_dev, st);
     Workspace& w = ctx->ws;
-    if (!ctx->attr_done_step) {
-        MVS_CUDA_OK(ctx, cudaFuncSetAttribute(frame_fwd_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)(sizeof(ResidentSmem) + sizeof(VposerSmem))));
-    }
     MVS_LAUNCH(ctx, KID_FRAME_FWD, st,
                frame_fwd_resident_kernel<<<w.na_bound > 0 ? w.na_bound : w.B, kResThreads, sizeof(ResidentSmem) + sizeof(VposerSmem), st>>>(
                    make_resident_model(ctx), L.lp_tab, L.sc, x_dev, w.fidx, w.na, w.Phi, w.PhiTc, w.At, w.ldA, w.slot_tr));

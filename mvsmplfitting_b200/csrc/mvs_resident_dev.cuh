@@ -62,16 +62,6 @@ __device__ __forceinline__ float serial_sum8(int n, F v) {
     return a;
 }
 
-// Depth-level schedule of the kinematic tree: joints of one level only depend on the level above (forward) / below
-// (adjoint), so a level is processed by parallel lane groups and the 23-step serial chain becomes <= 9 level steps
-// for SMPL.  Children are listed in DESCENDING index order: gathering them in that order reproduces the summation
-// order of the plain "for j = 23 .. 1" reverse sweep bit for bit.
-struct ChainSched {
-    int nlev;
-    unsigned char lev_ptr[kJoints + 1], lev_j[kJoints];
-    unsigned char ch_ptr[kJoints + 1], ch_j[kJoints];
-};
-
 struct ResidentModel {                    // device pointers + sizes, by value
     const float* Qk; const float* Jt; const float* JS;
     const int* ell_j; const float* ell_w; int KW;

@@ -461,6 +461,10 @@ static int ensure_sdf_bins_ws(mvs_ctx* ctx) {
     if ((rc = dev_alloc(ctx, &w.bins_ray_ptr, B * (kBinRays + 1)))) return rc;
     if ((rc = dev_alloc(ctx, &w.bins_ray_idx, B * kBinCapR))) return rc;
     if ((rc = dev_alloc(ctx, &w.bins_meta, B * 8))) return rc;
+    return MVS_OK;
+}
+
+int sdf_set_attributes(mvs_ctx* ctx) {
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(sdf_bins_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBinsSmem));
     return MVS_OK;
 }

@@ -412,7 +412,6 @@ struct TcState {
     CUtensorMap map_f[kTcNumInst];  // PhiTc [2][ldA][224] (hi rows, then lo rows), box kTcInstances[i] rows x 32
     float* poffT = nullptr;         // [3N][ldA] pose offsets, frame fastest (output of the tensor-core contraction)
     int* err = nullptr;
-    bool ready = false;
 };
 
 static int encode_map(mvs_ctx* ctx, CUtensorMap* map, const float* ptr, uint64_t rows, uint32_t box_rows) {
@@ -445,41 +444,24 @@ int tc_upload_model(mvs_ctx* ctx) {
     return MVS_OK;
 }
 
-bool tc_available(const mvs_ctx* ctx) {
-    return ctx->exec_mode != 1 && ctx->tc != nullptr && ctx->ws.PhiTc != nullptr;
-}
-
-template <int NF>
-static int tc_set_smem(mvs_ctx* ctx) {
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<NF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(NF)));
+// kernel attributes and the tensor maps over the model's Qk rows and the batch's PhiTc
+int tc_set_attributes(mvs_ctx* ctx) {
+    TcState* T = ctx->tc;
+    const Workspace& w = ctx->ws;
+    int rc;
+    if ((rc = encode_map(ctx, &T->map_p, ctx->m.Qk, (uint64_t)3 * ctx->m.N, kTcRows))) return rc;
+    for (int i = 0; i < kTcNumInst; ++i)                                                           // hi rows, then lo rows
+        if ((rc = encode_map(ctx, &T->map_f[i], w.PhiTc, (uint64_t)2 * w.ldA, kTcInstances[i]))) return rc;
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(8)));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(16)));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(32)));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(64)));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(128)));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(skin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSkinSmem));
     return MVS_OK;
 }
 
-int tc_prepare(mvs_ctx* ctx) {
-    TcState* T = ctx->tc;
-    Workspace& w = ctx->ws;
-    const DevModel& m = ctx->m;
-    if (!T) return set_error(ctx, MVS_ERR_INVALID, "tensor-core path not initialised (mvs_set_model)");
-    if (!T->ready) {
-        int rc;
-        if ((rc = encode_map(ctx, &T->map_p, m.Qk, (uint64_t)3 * m.N, kTcRows))) return rc;
-        for (int i = 0; i < kTcNumInst; ++i)                                                       // hi rows, then lo rows
-            if ((rc = encode_map(ctx, &T->map_f[i], w.PhiTc, (uint64_t)2 * w.ldA, kTcInstances[i]))) return rc;
-        if ((rc = dev_alloc(ctx, &T->poffT, (size_t)3 * m.N * w.ldA))) return rc;
-        if ((rc = tc_set_smem<8>(ctx)) || (rc = tc_set_smem<16>(ctx)) || (rc = tc_set_smem<32>(ctx)) || (rc = tc_set_smem<64>(ctx)) ||
-            (rc = tc_set_smem<128>(ctx)))
-            return rc;
-        MVS_CUDA_OK(ctx, cudaFuncSetAttribute(skin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSkinSmem));
-        T->ready = true;
-    }
-    return MVS_OK;
-}
-
-float* tc_poffT(mvs_ctx* ctx) {
-    TcState* T = ctx->tc;
-    if (!T || tc_prepare(ctx) != MVS_OK) return nullptr;
-    return T->poffT;
-}
+float* tc_poffT(mvs_ctx* ctx) { return ctx->tc->poffT; }
 
 template <int NF>
 static cudaError_t launch_gemm(mvs_ctx* ctx, const TcState* T, int inst, dim3 grid, cudaStream_t st, int ntiles) {
@@ -492,7 +474,10 @@ int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool s
     TcState* T = ctx->tc;
     Workspace& w = ctx->ws;
     const DevModel& m = ctx->m;
-    { const int rc = tc_prepare(ctx); if (rc) return rc; }
+    if (!T->poffT) {                                    // allocated on first use: sparse-regime contexts never need it
+        const int rc = dev_alloc(ctx, &T->poffT, (size_t)3 * m.N * w.ldA);
+        if (rc) return rc;
+    }
     SdfSetupArgs sd{};
     if (sdf_setup) {                                    // the skinning kernel also computes each frame's SDF set-up
         const int rc = ensure_sdf_setup_ws(ctx, st);
@@ -526,7 +511,7 @@ int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool s
 
 int tc_check_error(mvs_ctx* ctx) {          // host-side check after a synchronisation point
     TcState* T = ctx->tc;
-    if (!T || !T->ready) return MVS_OK;
+    if (!T->poffT) return MVS_OK;                  // the kernel has never run
     int e = 0;
     MVS_CUDA_OK(ctx, cudaMemcpy(&e, T->err, sizeof(int), cudaMemcpyDeviceToHost));
     if (e) return set_error(ctx, MVS_ERR_CUDA, "vertex_fwd_tc_kernel: mbarrier wait timed out (pipeline protocol error)");
