@@ -132,6 +132,17 @@ int mvs_set_loss_config(mvs_ctx* ctx, const mvs_loss_config* cfg);
  *      anchor_dev and weight_dev are [B,86] device pointers, copied; enable = 0 switches the term off. */
 int mvs_set_anchor(mvs_ctx* ctx, const float* anchor_dev, const float* weight_dev, int enable, void* stream);
 
+/* ---- 3-D joint supervision: SMPLifyLoss(use_3d=True) (code/utils/fitting.py:318-324, targets from
+ *      code/utils/non_linear_solver.py:86-99): adds  data_weight^2 * sum_k conf[b,k]^2 * sum_c GMoF_rho(gt_xyz[b,k,c] - q[b,k,c])
+ *      to frame b's loss, q = the keypoints the 2-D term projects, with the stage's rho and data_weight; joint_weights and
+ *      use_joints_conf do not apply to it.  The confidences are taken as given (the reference zeroes hips 11 and 12 unless
+ *      use_hip is set; that is the caller's).  gt_xyz [B,K,3], conf [B,K]; on_device != 0: device pointers (copied D2D on
+ *      `stream`), else host pointers (copied before return).  enable = 0 switches the term off (the arrays are not read).
+ *      Needs the model and mvs_set_batch first: a context's batch size is fixed once set, so the targets always have its
+ *      B rows, and nothing from another batch size can be read.  Every later mvs_set_loss_config / mvs_fit stage sees the
+ *      term; mvs_init_guess aligns to the targets instead of the triangulated keypoints while it is on (init_guess.py:85-86). */
+int mvs_set_joints3d(mvs_ctx* ctx, const float* gt_xyz, const float* conf, int enable, int on_device, void* stream);
+
 /* ---- closure: replaces fitting_func() (code/utils/fitting.py:162-203) = SMPL.forward + SMPLifyLoss.forward
  *      + backward, for all B frames at once.  params_dev [B,86]; outputs (device, any may be NULL):
  *      loss_dev [B], grad_dev [B,86], joints_dev [B,K,3], proj_dev [V,B,K,2], verts_dev [B,n_verts,3].
@@ -221,7 +232,9 @@ int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, cons
  *      entries = hip_seed (fix_params; the reference uses 1.0; ignored when the loss config has use_vposer = 2, where
  *      the pose slots hold the latent code, which is zeroed as init_guess.py:96-98 does), transl = t, scale = s or
  *      fixed_scale.  Frames whose detections are degenerate (rank < 2) get the translation of the centroids only.
- *      params_dev [B,86] is overwritten; joints3d_dev [B,K,3] receives the triangulated keypoints (may be NULL).
+ *      With the 3-D joint term on (mvs_set_joints3d) the alignment target is the 3-D annotations instead of the triangulated
+ *      or depth-guessed keypoints (init_guess.py:85-86), and one view needs no keypoints 5, 6, 11, 12 unless use_torso is set.
+ *      params_dev [B,86] is overwritten; joints3d_dev [B,K,3] receives the alignment target (may be NULL).
  *      Uses the keypoints and cameras already uploaded; asynchronous on `stream`.  The rest joints are computed once per
  *      context and fixed_scale (seed + the 3-kernel geometry chain) and cached: a call is one launch afterwards.
  *      The warm start of sequences (load_init, init_guess.py:137-166) is a parameter copy and has no entry point: pass the

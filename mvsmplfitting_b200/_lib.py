@@ -62,7 +62,7 @@ EXPORTS = (
     "mvs_version", "mvs_build_id", "mvs_create", "mvs_destroy", "mvs_last_error", "mvs_launch_count", "mvs_set_model",
     "mvs_set_gmm_prior", "mvs_set_vposer", "mvs_vposer_decode", "mvs_set_cameras", "mvs_set_batch", "mvs_set_keypoints", "mvs_set_loss_config",
     "mvs_closure", "mvs_forward", "mvs_lbfgs_run", "mvs_lbfgs_step", "mvs_fit", "mvs_fit_seq", "mvs_fit_host", "mvs_sdf_grid", "mvs_profile", "mvs_profile_read",
-    "mvs_kernel_name", "mvs_set_exec_mode", "mvs_set_anchor", "mvs_init_guess",
+    "mvs_kernel_name", "mvs_set_exec_mode", "mvs_set_anchor", "mvs_set_joints3d", "mvs_init_guess",
 )
 NUM_KERNEL_IDS = 18
 
@@ -111,6 +111,7 @@ def load() -> ctypes.CDLL:
     lib.mvs_sdf_grid.argtypes = [vp, vp, vp, ci, vp, ci, ci, ci, vp]
     lib.mvs_set_exec_mode.argtypes = [vp, ci]
     lib.mvs_set_anchor.argtypes = [vp, vp, vp, ci, vp]
+    lib.mvs_set_joints3d.argtypes = [vp, vp, vp, ci, ci, vp]
     lib.mvs_profile.argtypes = [vp, ctypes.c_uint]
     lib.mvs_profile_read.argtypes = [vp, vp, vp]
     lib.mvs_kernel_name.argtypes = [ci]

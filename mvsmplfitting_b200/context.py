@@ -55,6 +55,7 @@ class FittingContext:
         self.K = 17
         self.N = 0
         self._loss_cfg = None
+        self._j3d_keep = None             # the 3-D targets while the term is on (set_joints3d)
 
     def close(self):
         if getattr(self, "h", None):
@@ -236,7 +237,8 @@ class FittingContext:
     def init_guess(self, estimate_scale: bool = True, fixed_scale: float = 1.0, use_torso: bool = True,
                    hip_seed: float = 1.0, want_joints3d: bool = True, umeyama_as_written: bool = False):
         """Initial parameter block of every frame from the uploaded detections (mvs_init_guess: triangulation -- or the
-        single-view depth guess -- + similarity alignment, init_guess.py:18-107 + fix_params :190-212).
+        single-view depth guess, or the 3-D targets of set_joints3d while they are on -- + similarity alignment,
+        init_guess.py:18-107 + fix_params :190-212).
         umeyama_as_written: evaluate code/utils/umeyama.py as written (see include/mvsmpl.h) instead of the published
         algorithm.  Returns (params [B,86], joints3d [B,K,3])."""
         params = torch.empty(self.B, 86, dtype=torch.float32, device=self.device)
@@ -305,6 +307,29 @@ class FittingContext:
             weight = weight[None].expand(self.B, -1).contiguous()
         assert tuple(anchor.shape) == (self.B, S.NUM_PARAMS) and tuple(weight.shape) == (self.B, S.NUM_PARAMS)
         _lib.check(self.h, self.lib.mvs_set_anchor(self.h, _ptr(anchor), _ptr(weight), 1, self._stream()), "mvs_set_anchor")
+
+    def set_joints3d(self, gt_xyz, conf=None):
+        """3-D joint targets of the SMPLifyLoss use_3d term (mvs_set_joints3d): gt_xyz [B,K,3], conf [B,K]; numpy (host) or
+        CUDA tensors.  gt_xyz=None switches the term off.  Takes effect with the next set_loss() / fit() and at once in
+        init_guess()."""
+        if gt_xyz is None:
+            _lib.check(self.h, self.lib.mvs_set_joints3d(self.h, None, None, 0, 0, self._stream()), "mvs_set_joints3d")
+            self._j3d_keep = None
+            return
+        if conf is None:
+            raise ValueError("set_joints3d: the 3-D term needs its confidences")
+        on_dev = isinstance(gt_xyz, torch.Tensor) and gt_xyz.is_cuda
+        if on_dev:
+            gt_xyz = gt_xyz.to(self.device, torch.float32).contiguous()
+            conf = torch.as_tensor(conf).to(self.device, torch.float32).contiguous()
+        else:
+            gt_xyz, conf = _f32(gt_xyz), _f32(conf)
+        if tuple(gt_xyz.shape) != (self.B, self.K, 3) or tuple(conf.shape) != (self.B, self.K):
+            raise ValueError("set_joints3d: want gt_xyz [%d,%d,3] and conf [%d,%d], got %s and %s"
+                             % (self.B, self.K, self.B, self.K, tuple(gt_xyz.shape), tuple(conf.shape)))
+        self._j3d_keep = (gt_xyz, conf)
+        _lib.check(self.h, self.lib.mvs_set_joints3d(self.h, _ptr(gt_xyz), _ptr(conf), 1, 1 if on_dev else 0, self._stream()),
+                   "mvs_set_joints3d")
 
     def set_exec_mode(self, mode: int):
         """0 = frame-resident kernels where they apply (default), 1 = batched kernels only"""

@@ -88,6 +88,7 @@ int make_loss_params(mvs_ctx* ctx, const mvs_loss_config* c, LossParams* out) {
     l.sdf_grid = c->sdf_grid > 0 ? c->sdf_grid : 128; l.sdf_all_faces = c->sdf_all_faces;
     l.frozen_mask = c->frozen_mask; l.num_gaussians = ctx->m.M;
     l.anchor_on = ctx->anchor_enabled ? 1 : 0;
+    l.j3d_on = ctx->j3d_enabled ? 1 : 0;
     *out = l;
     return MVS_OK;
 }
@@ -521,6 +522,29 @@ int mvs_set_anchor(mvs_ctx* ctx, const float* anchor_dev, const float* weight_de
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(w.anchor_w, weight_dev, (size_t)w.B * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
     ctx->loss.anchor_on = 1;
     ctx->anchor_enabled = true;
+    return MVS_OK;
+}
+
+int mvs_set_joints3d(mvs_ctx* ctx, const float* gt_xyz, const float* conf, int enable, int on_device, void* stream) {
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    MVS_REQUIRE(ctx, ctx->have_model && ctx->ws.B > 0, "mvs_set_joints3d: set the model and the batch first");
+    if (!enable) { ctx->loss.j3d_on = 0; ctx->j3d_enabled = false; return MVS_OK; }
+    MVS_REQUIRE(ctx, gt_xyz && conf, "mvs_set_joints3d: NULL array");
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    Workspace& w = ctx->ws;
+    const size_t n = (size_t)w.B * ctx->m.K;
+    int rc;
+    if (!w.j3d_xyz) {
+        if ((rc = dev_alloc(ctx, &w.j3d_xyz, n * 3))) return rc;
+        if ((rc = dev_alloc(ctx, &w.j3d_conf, n))) return rc;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(w.j3d_xyz, gt_xyz, n * 3 * sizeof(float), kind, st));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(w.j3d_conf, conf, n * sizeof(float), kind, st));
+    if (!on_device) MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    ctx->loss.j3d_on = 1;
+    ctx->j3d_enabled = true;
     return MVS_OK;
 }
 

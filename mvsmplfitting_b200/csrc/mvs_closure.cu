@@ -223,6 +223,7 @@ keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, 
                      KeypointModel km, const float* __restrict__ verts, int nv, int dense,
                      const float* __restrict__ gchain, CamSet cams, const float* __restrict__ gt_uv,
                      const float* __restrict__ conf, const float* __restrict__ joint_w, int B, LossParams lp,
+                     const float* __restrict__ j3d_xyz, const float* __restrict__ j3d_conf,
                      float* __restrict__ data_loss, float* __restrict__ dtransl, float* __restrict__ dv,
                      int dv_stride, float* __restrict__ dgchain, float* __restrict__ joints_out,
                      float* __restrict__ proj_out) {
@@ -236,6 +237,7 @@ keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, 
     __shared__ float contrib[kMaxViews * kMaxKeypoints * 3];
     __shared__ float lterm[kMaxViews * kMaxKeypoints];
     __shared__ float vsum[kMaxViews];
+    __shared__ float l3[kMaxKeypoints];
     const float* vf = verts + (size_t)slot * nv * 3;
     if (t < K) {
         float a0 = 0.f, a1 = 0.f, a2 = 0.f;
@@ -283,6 +285,16 @@ keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, 
         for (int v = 0; v < V; ++v) {
             a0 += contrib[3 * (v * K + t)]; a1 += contrib[3 * (v * K + t) + 1]; a2 += contrib[3 * (v * K + t) + 2];
         }
+        if (lp.j3d_on) {                  // 3-D joint term (fitting.py:318-324): targets of frame b, no joint_weights
+            const float c3 = j3d_conf[(size_t)b * K + t], c2 = c3 * c3;
+            const float* g3 = j3d_xyz + ((size_t)b * K + t) * 3;
+            float d0, d1, d2;
+            const float e0 = gmof(g3[0] - q[3 * t], rho2, &d0);
+            const float e1 = gmof(g3[1] - q[3 * t + 1], rho2, &d1);
+            const float e2 = gmof(g3[2] - q[3 * t + 2], rho2, &d2);
+            l3[t] = c2 * e0 + c2 * e1 + c2 * e2;
+            a0 += -(c2 * d0) * dw2; a1 += -(c2 * d1) * dw2; a2 += -(c2 * d2) * dw2;
+        }
         dq[3 * t] = a0; dq[3 * t + 1] = a1; dq[3 * t + 2] = a2;
     } else if (t >= 32 && t < 32 + V) {
         const int v = t - 32;
@@ -294,6 +306,11 @@ keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, 
     if (t == 0) {
         float a = 0.f;
         for (int v = 0; v < V; ++v) a += vsum[v];
+        if (lp.j3d_on) {                  // joint_loss + joints3d_loss, the first two terms of fitting.py:413
+            float s3 = 0.f;
+            for (int k = 0; k < K; ++k) s3 += l3[k];
+            a += s3 * dw2;
+        }
         data_loss[slot] = a;
     }
     if (t >= 32 && t < 35) {
@@ -770,11 +787,12 @@ int launch_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* gra
     }
     KeypointModel km{m.K, m.nsup, m.N, m.kp_ptr, m.kp_vidx, m.kp_spos, m.kp_w, m.kp_chain, m.sup, m.sup_ptr, m.sup_k, m.sup_w};
     CamSet cams = ctx->cams;
-    if (geometry_only) cams.num_views = 0;           // joints / vertices only: no projection, no detections read
+    LossParams kp_lp = lp;
+    if (geometry_only) { cams.num_views = 0; kp_lp.j3d_on = 0; }      // joints / vertices only: no detections or targets read
     MVS_LAUNCH(ctx, KID_KEYPOINT, st,
                keypoint_loss_kernel<<<B, kFrameThreads, 0, st>>>(x_dev, w.fidx, w.na, km, w.verts, nv, dense ? 1 : 0,
-                                                                 w.gchain, cams, w.gt_uv, w.conf, w.joint_w, B, lp,
-                                                                 w.data_loss, w.dtransl, w.dv, sdf_on ? m.nsup + m.N : m.nsup,
+                                                                 w.gchain, cams, w.gt_uv, w.conf, w.joint_w, B, kp_lp,
+                                                                 w.j3d_xyz, w.j3d_conf, w.data_loss, w.dtransl, w.dv, sdf_on ? m.nsup + m.N : m.nsup,
                                                                  w.dgchain, joints_dev, proj_dev));
     if (geometry_only) {
         if (verts_dev) {

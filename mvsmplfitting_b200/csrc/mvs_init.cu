@@ -25,10 +25,11 @@ __global__ void init_seed_kernel(float* __restrict__ params, int B, float scale)
 }
 
 // params [B,86] (written completely), rest [K,3] rest joints of the model (the same for every frame),
-// gt_uv [V,B,K,2], conf [V,B,K]; joints3d [B,K,3] or nullptr
+// gt_uv [V,B,K,2], conf [V,B,K]; targets [B,K,3] (3-D joint term on) or nullptr; joints3d [B,K,3] or nullptr
 __global__ void __launch_bounds__(128) init_guess_kernel(float* __restrict__ params, const float* __restrict__ rest,
                                                          CamSet cams, const float* __restrict__ gt_uv,
-                                                         const float* __restrict__ conf, int B, int K, int estimate_scale,
+                                                         const float* __restrict__ conf, const float* __restrict__ targets,
+                                                         int B, int K, int estimate_scale,
                                                          float fixed_scale, int use_torso, float hip_seed, int as_written,
                                                          float* __restrict__ joints3d) {
     __shared__ double s_dst[4][kMaxKeypoints * 3];
@@ -40,7 +41,9 @@ __global__ void __launch_bounds__(128) init_guess_kernel(float* __restrict__ par
     for (int i = lane; i < kParams; i += 32) x[i] = 0.f;
     if (lane < K) {
         double X[3];
-        if (cams.num_views == 1) {                        // init_guess.py:54-78: depth guess along the optical axis
+        if (targets) {                                    // init_guess.py:85-86: the 3-D annotations replace both guesses
+            for (int c = 0; c < 3; ++c) X[c] = (double)targets[((size_t)b * K + lane) * 3 + c];
+        } else if (cams.num_views == 1) {                 // init_guess.py:54-78: depth guess along the optical axis
             double rj[kMaxKeypoints * 3];
             for (int i = 0; i < K * 3; ++i) rj[i] = (double)rest[i];
             const double d = single_view_depth<double>(cams.cam[0], rj, gt_uv + (size_t)b * K * 2, conf + (size_t)b * K);
@@ -102,7 +105,8 @@ extern "C" int mvs_init_guess(mvs_ctx* ctx, float* params_dev, float* joints3d_d
     cudaStream_t st = (cudaStream_t)stream;
     Workspace& w = ctx->ws;
     if (K * 3 > kParams) return set_error(ctx, MVS_ERR_INVALID, "mvs_init_guess: more than 28 keypoints");
-    if (ctx->cams.num_views == 1 && K < 13)
+    const bool j3d = ctx->j3d_enabled;
+    if (ctx->cams.num_views == 1 && !j3d && K < 13)
         return set_error(ctx, MVS_ERR_INVALID, "mvs_init_guess: the single-view depth guess needs keypoints 5, 6, 11, 12");
     // Rest joints (zero pose, zero shape, scale = fixed_scale; init_guess.py:29-52) are a property of the model: computed once
     // per context and scale with the library's own forward pass (seed + the 3-kernel geometry chain), then cached, so that a
@@ -115,7 +119,7 @@ extern "C" int mvs_init_guess(mvs_ctx* ctx, float* params_dev, float* joints3d_d
         float* rest = w.grad_scratch;                      // [B,86] scratch of the closure; K*3 <= 86 floats per frame
         MVS_LAUNCH(ctx, KID_MISC, st, init_seed_kernel<<<(B * kParams + 255) / 256, 256, 0, st>>>(params_dev, B, cfg->fixed_scale));
         const int vposer = ctx->loss.use_vposer;           // the rest pose is body_pose = 0 whatever the pose encoding
-        ctx->loss.use_vposer = 0;
+        ctx->loss.use_vposer = 0;                          // (the geometry-only chain never reads the 3-D targets)
         const int rc = launch_closure(ctx, params_dev, nullptr, nullptr, rest, nullptr, nullptr, st, true);
         ctx->loss.use_vposer = vposer;
         if (rc) return rc;
@@ -123,7 +127,8 @@ extern "C" int mvs_init_guess(mvs_ctx* ctx, float* params_dev, float* joints3d_d
         ctx->rest_scale = cfg->fixed_scale;
     }
     MVS_LAUNCH(ctx, KID_MISC, st,
-               init_guess_kernel<<<(B + 3) / 4, 128, 0, st>>>(params_dev, ctx->rest_joints, ctx->cams, w.gt_uv, w.conf, B, K,
+               init_guess_kernel<<<(B + 3) / 4, 128, 0, st>>>(params_dev, ctx->rest_joints, ctx->cams, w.gt_uv, w.conf,
+                                                              j3d ? w.j3d_xyz : nullptr, B, K,
                                                               cfg->estimate_scale, cfg->fixed_scale, cfg->use_torso,
                                                               ctx->loss.use_vposer == 2 ? 0.f : cfg->hip_seed,
                                                               cfg->umeyama_as_written, joints3d_dev));

@@ -45,6 +45,7 @@ struct LossParams {
     unsigned frozen_mask;
     int num_gaussians;
     int anchor_on;
+    int j3d_on;                       // 3-D joint term (mvs_set_joints3d)
 };
 
 inline bool sdf_term_on(const LossParams& lp) { return lp.interpenetration && lp.coll_loss_weight > 0.f; }
@@ -135,6 +136,8 @@ struct Workspace {
     float* grad_scratch = nullptr;    // [B][86]
     float* anchor = nullptr;          // [B][86] quadratic anchor (sequence mode)
     float* anchor_w = nullptr;        // [B][86]
+    float* j3d_xyz = nullptr;         // [B][K][3] 3-D joint targets (mvs_set_joints3d)
+    float* j3d_conf = nullptr;        // [B][K]
     // SDF scratch
     FrameBox* sdf_frame = nullptr;    // [B] frame boxes of the batched chain's SDF term (launch_sdf_terms)
     float* sdf_gcoord = nullptr;      // [B][N][3]
@@ -221,6 +224,7 @@ struct mvs_ctx {
     mvs::Parents parents{};
     mvs::ChainSched chain{};         // level schedule of parents
     bool anchor_enabled = false;
+    bool j3d_enabled = false;
     int exec_mode = 0;               // mvs_set_exec_mode: 0 auto, 1 batched chain only, 2 stage barriers, 3 dense-round closures
     bool have_model = false, have_cams = false, have_kp = false, have_loss = false;
     std::vector<void*> allocs;       // everything cudaMalloc'ed, freed in mvs_destroy

@@ -230,6 +230,7 @@ static ResidentModel make_resident_model(const mvs_ctx* ctx) {
     r.supj_ptr = m.supj_ptr; r.supj_i = m.supj_i; r.supj_w = m.supj_w;
     r.M = m.M; r.gmm_means = m.gmm_means; r.gmm_prec = m.gmm_prec; r.gmm_lognllw = m.gmm_lognllw;
     r.anchor = ctx->ws.anchor; r.anchor_w = ctx->ws.anchor_w;
+    r.j3d_xyz = ctx->ws.j3d_xyz; r.j3d_conf = ctx->ws.j3d_conf;
     r.vp_w1 = m.vp_w1; r.vp_w2 = m.vp_w2; r.vp_w3 = m.vp_w3; r.vp_w1t = m.vp_w1t; r.vp_w2t = m.vp_w2t; r.vp_w3t = m.vp_w3t;
     r.vp_b1 = m.vp_b1; r.vp_b2 = m.vp_b2; r.vp_b3 = m.vp_b3;
     r.par = ctx->parents;

@@ -71,6 +71,7 @@ struct ResidentModel {                    // device pointers + sizes, by value
     const int* supj_ptr; const int* supj_i; const float* supj_w;      // per joint: (support index, weight)
     int M; const float* gmm_means; const float* gmm_prec; const float* gmm_lognllw;
     const float* anchor; const float* anchor_w;     // sequence mode (mvs_set_anchor)
+    const float* j3d_xyz; const float* j3d_conf;    // 3-D joint targets [B][K][3], [B][K] (mvs_set_joints3d)
     const float *vp_w1, *vp_w2, *vp_w3, *vp_w1t, *vp_w2t, *vp_w3t, *vp_b1, *vp_b2, *vp_b3;      // VPoser decoder
     Parents par;
     ChainSched cs;
@@ -89,7 +90,7 @@ struct ResidentSmem {
     // priors
     float gm_diff[kResMaxM * 69], gm_y[kResMaxM * 69], gm_ll[kResMaxM];
     float red[kResThreads];
-    float sc[16];                          // [0] data loss, [1] |theta|^2, [2] total loss
+    float sc[16];                          // [0] data loss, [1] |theta|^2, [2] total loss, [3] anchor, [4] 3-D joint loss
     // optimiser vectors (lbfgs_resident_kernel only)
     float lx[88], lg[88], ld[88], lprev_g[88], lx_init[88], lg_prev[88], lbg0[88], lbg1[88], lx_eval[88], lg_new[88];
     float ro[128], al[128];
@@ -564,12 +565,29 @@ static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m,
             }
             data_sync();
             PHASE_MARK(8);
-            if (t < K) {
-                float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-                for (int v = 0; v < V; ++v) {
-                    a0 += S.contrib[3 * (v * K + t)]; a1 += S.contrib[3 * (v * K + t) + 1]; a2 += S.contrib[3 * (v * K + t) + 2];
+            if (t < 32) {
+                float l3 = 0.f;
+                if (t < K) {
+                    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+                    for (int v = 0; v < V; ++v) {
+                        a0 += S.contrib[3 * (v * K + t)]; a1 += S.contrib[3 * (v * K + t) + 1]; a2 += S.contrib[3 * (v * K + t) + 2];
+                    }
+                    if (lp.j3d_on) {          // 3-D joint term (fitting.py:318-324): targets of frame b, no joint_weights
+                        const float c3 = m.j3d_conf[(size_t)b * K + t], c2 = c3 * c3;
+                        const float* g3 = m.j3d_xyz + ((size_t)b * K + t) * 3;
+                        float d0, d1, d2;
+                        const float e0 = gmof(g3[0] - S.q[3 * t], rho2, &d0);
+                        const float e1 = gmof(g3[1] - S.q[3 * t + 1], rho2, &d1);
+                        const float e2 = gmof(g3[2] - S.q[3 * t + 2], rho2, &d2);
+                        l3 = c2 * e0 + c2 * e1 + c2 * e2;
+                        a0 += -(c2 * d0) * dw2; a1 += -(c2 * d1) * dw2; a2 += -(c2 * d2) * dw2;
+                    }
+                    S.dq[3 * t] = a0; S.dq[3 * t + 1] = a1; S.dq[3 * t + 2] = a2;
                 }
-                S.dq[3 * t] = a0; S.dq[3 * t + 1] = a1; S.dq[3 * t + 2] = a2;
+                if (lp.j3d_on) {
+                    l3 = warp_sum(l3);
+                    if (t == 0) S.sc[4] = l3 * dw2;
+                }
             } else if (t >= 32 && t < 32 + V) {
                 const int v = t - 32;
                 float a = 0.f;
@@ -777,6 +795,7 @@ static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m,
     // ---- P12 total (same order as fitting.py:411-413) and the masked gradient
     if (t == 0) {
         float total = S.sc[0];
+        if (lp.j3d_on) total += S.sc[4];
         total += (pprior + l2extra);
         total += shape_loss;
         total += angle;

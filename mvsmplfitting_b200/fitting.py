@@ -2,7 +2,8 @@
 (code/utils/fitting.py:36-415), backed by the fused CUDA closure and the device-resident L-BFGS.
 
     monitor.create_fitting_closure(optimizer, body_model, camera=[...], gt_joints=[V,B,17,2],
-        joints_conf=[V x [B,17]], joint_weights=[1,17], loss=SMPLifyLoss, use_vposer=..., ...)
+        joints_conf=[V x [B,17]], joint_weights=[1,17], loss=SMPLifyLoss, use_vposer=...,
+        gt_joints3d=[B,17,3], joints3d_conf=[B,17] (3-D joint term, SMPLifyLoss(use_3d=True)), ...)
         -> fitting_func(backward=True) -> 0-dim loss tensor, gradients written to p.grad
     monitor.run_fitting(optimizer, closure, params, body_model, ...) -> final loss
 
@@ -123,8 +124,6 @@ def loss_config_from(loss, params_requires_grad: dict, use_vposer: bool):
         kind = "l2"
     else:
         kind = "none"
-    if getattr(loss, "use_3d", False):
-        raise NotImplementedError("use_3d (3-D joint supervision) is not on the B200 path")
     shape_prior = getattr(loss, "shape_prior", None)
     if shape_prior is not None and hasattr(shape_prior, "precisions"):
         raise NotImplementedError("only the L2 shape prior is on the B200 path")
@@ -143,7 +142,7 @@ class FittingClosure:
     """Callable returned by FittingMonitor.create_fitting_closure."""
 
     def __init__(self, optimizer, body_model, camera, gt_joints, loss, joints_conf, joint_weights, use_vposer, vposer,
-                 pose_embedding, return_verts=True):
+                 pose_embedding, return_verts=True, gt_joints3d=None, joints3d_conf=None):
         self.optimizer = optimizer
         self.body_model = body_model
         self.loss = loss
@@ -164,6 +163,14 @@ class FittingClosure:
             conf = torch.stack([torch.as_tensor(c).to(dev, torch.float32).reshape(B, K) for c in joints_conf]).contiguous()
         jw = torch.as_tensor(joint_weights).to(dev, torch.float32).reshape(-1)[:K].contiguous()
         self.ctx.set_keypoints(gt, conf, jw)
+        # 3-D joint term: on when the loss says so (SMPLifyLoss.use_3d, fitting.py:320), with the targets passed here
+        if getattr(loss, "use_3d", False):
+            if gt_joints3d is None or joints3d_conf is None:
+                raise ValueError("use_3d needs gt_joints3d and joints3d_conf (non_linear_solver.py:86-99)")
+            self.ctx.set_joints3d(torch.as_tensor(gt_joints3d).to(dev, torch.float32).reshape(B, K, 3),
+                                  torch.as_tensor(joints3d_conf).to(dev, torch.float32).reshape(B, K))
+        elif getattr(self.ctx, "_j3d_keep", None) is not None:      # the model's context had the term on: off again
+            self.ctx.set_joints3d(None)
         self._gmm_of = None
         self.last = None
         # VPoser: when the module exposes the reference's decoder layers (model/VPoser.py:190-197) the decode runs on
@@ -285,10 +292,11 @@ class FittingMonitor(object):
                                create_graph=False, use_3d=False, **kwargs):
         if create_graph:
             raise NotImplementedError("create_graph=True (second-order) is not on the B200 path")
-        if use_3d:
-            raise NotImplementedError("use_3d is not on the B200 path")
+        if use_3d and (gt_joints3d is None or joints3d_conf is None):
+            raise ValueError("use_3d needs gt_joints3d and joints3d_conf (non_linear_solver.py:86-99)")
         return FittingClosure(optimizer, body_model, camera, gt_joints, loss, joints_conf, joint_weights, use_vposer,
-                              vposer, pose_embedding, return_verts=return_verts)
+                              vposer, pose_embedding, return_verts=return_verts, gt_joints3d=gt_joints3d,
+                              joints3d_conf=joints3d_conf)
 
     def run_fitting_stages(self, optimizer, closure, opt_weights):
         """The stage loop of non_linear_solver.py:109-203 in ONE call.  The reference does, per entry of

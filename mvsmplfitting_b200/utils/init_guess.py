@@ -18,7 +18,7 @@ from ..fitting import model_context
 from ..seqio import camera_arrays
 
 
-def _run_device_guess(setting, data, use_torso, hip_seed, as_written=False):
+def _run_device_guess(setting, data, use_torso, hip_seed, as_written=False, joints3d=None):
     model = setting["model"]
     keypoints = data["keypoints"]
     est_scale = not setting["fix_scale"]                                                   # init_guess.py:24
@@ -29,19 +29,27 @@ def _run_device_guess(setting, data, use_torso, hip_seed, as_written=False):
     kp = np.stack([np.asarray(k, dtype=np.float32).reshape(ctx.B, -1, 3) for k in keypoints])      # [V,B,K,3]
     K = kp.shape[2]
     ctx.set_keypoints(np.ascontiguousarray(kp[..., :2]), np.ascontiguousarray(kp[..., 2]), np.ones(K, np.float32))
+    if joints3d is not None:                  # only the xyz steer the alignment; the loss gets its targets from the closure
+        ctx.set_joints3d(np.asarray(joints3d, dtype=np.float32).reshape(ctx.B, K, 3), np.ones((ctx.B, K), np.float32))
+    elif getattr(ctx, "_j3d_keep", None) is not None:
+        ctx.set_joints3d(None)
     params, joints3d = ctx.init_guess(estimate_scale=est_scale, fixed_scale=fixed_scale, use_torso=use_torso,
                                       hip_seed=hip_seed, umeyama_as_written=as_written)
+    if getattr(ctx, "_j3d_keep", None) is not None:
+        ctx.set_joints3d(None)                # the guess's stand-in confidences must not reach a later loss
     return params, joints3d, est_scale, fixed_scale
 
 
 def init_guess(setting, data, use_torso=False, **kwargs):
     """init_guess.py:18-107: resets the model to zero pose / shape, then sets transl, global_orient and scale from the
     similarity transform between the model's rest joints and the triangulated detections."""
-    if kwargs.get("use_3d") and data.get("3d_joint") is not None:
-        raise NotImplementedError("3-D joint annotations (init_guess.py:76-77) are outside the path (use_3d = False)")
+    j3 = None
+    if kwargs.get("use_3d") and data.get("3d_joint") is not None:     # init_guess.py:85-86: align to the annotations
+        j3 = np.asarray(data["3d_joint"][0])[..., :3]
     model = setting["model"]
     params, _, est_scale, fixed_scale = _run_device_guess(setting, data, use_torso, hip_seed=0.0,
-                                                          as_written=bool(kwargs.get("umeyama_as_written", False)))
+                                                          as_written=bool(kwargs.get("umeyama_as_written", False)),
+                                                          joints3d=j3)
     p = params.detach()
     dtype = setting.get("dtype", torch.float32)
     scale = p[:, 85:86].to(dtype) if est_scale else torch.full((p.shape[0], 1), fixed_scale, dtype=dtype, device=p.device)
