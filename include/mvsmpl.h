@@ -213,6 +213,35 @@ int mvs_fit_seq(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_co
                 const mvs_lbfgs_config* opt_cfg, const unsigned char* warm_host, float* final_loss_dev,
                 mvs_lbfgs_stats* stats, void* stream);
 
+/* ---- mvs_fit over a stream of F frames, F of any size relative to the context's batch B.  Every frame gets exactly what
+ *      mvs_fit gives it in a batch of any size, bit for bit: the same parameters, final loss and iteration / evaluation
+ *      counts.  Stages are grouped into runs as mvs_fit groups them; each run covers all F frames before the next starts
+ *      (one barrier per run for the whole stream).  A frame-resident run is one launch over the F frames.  A dense (SDF) run
+ *      keeps B frames in flight, one per slot: whenever a frame finishes, its slot takes the next frame of the stream at the
+ *      next compaction of the active list (every 8 rounds), so the tail of one batch overlaps the start of the next.
+ *      All arrays are device pointers.  stats sums over frames equal those of mvs_fit over the same frames; rounds and
+ *      dense_rounds are the rounds the stream ran.  Refused (MVS_ERR_UNSUPPORTED): stages that would run in the batched
+ *      reference chain (exec mode 1, history_size > 100 without the SDF term, a model the frame-resident / dense kernels do
+ *      not take) and the anchor term (mvs_set_anchor: it is per batch).  MVS_ERR_INVALID: NULL or empty arguments,
+ *      n_frames < 1, gt_xyz without conf3d.
+ *      Context state afterwards: the dense runs overwrite the slots' keypoint and 3-D target rows, so after the call the
+ *      context behaves as if no keypoints and no 3-D targets had been uploaded: entry points that need keypoints return
+ *      MVS_ERR_INVALID until mvs_set_keypoints is called again, and the 3-D term is off until mvs_set_joints3d enables it
+ *      again.  The stream never reads the context's own keypoints or 3-D targets.  Leaves the last stage's loss
+ *      configuration set (3-D term off).  Synchronises. */
+typedef struct {
+    int n_frames;                  /* F >= 1 */
+    float* params;                 /* [F,86] in/out: start point in, fitted parameters out */
+    const float* gt_uv;            /* [V,F,K,2] */
+    const float* conf;             /* [V,F,K] */
+    const float* joint_weights;    /* [K] */
+    const float* gt_xyz;           /* [F,K,3]: the 3-D joint term is on for this call iff non-NULL */
+    const float* conf3d;           /* [F,K], required with gt_xyz */
+    float* final_loss;             /* [F] or NULL */
+} mvs_frame_stream;
+int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
+                   const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream);
+
 /* ---- host-buffer entry point (what a caller without device memory uses): copies keypoints and
  *      parameters host->device, runs `n_stages` optimisation stages (one mvs_loss_config each, the weight
  *      schedule of code/utils/non_linear_solver.py:109-203), copies parameters and losses back.

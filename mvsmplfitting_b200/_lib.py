@@ -58,10 +58,17 @@ class InitConfig(ctypes.Structure):
                 ("hip_seed", ctypes.c_float), ("umeyama_as_written", ctypes.c_int)]
 
 
+class FrameStream(ctypes.Structure):
+    """mvs_frame_stream (include/mvsmpl.h)"""
+    _fields_ = [("n_frames", ctypes.c_int), ("params", ctypes.c_void_p), ("gt_uv", ctypes.c_void_p), ("conf", ctypes.c_void_p),
+                ("joint_weights", ctypes.c_void_p), ("gt_xyz", ctypes.c_void_p), ("conf3d", ctypes.c_void_p),
+                ("final_loss", ctypes.c_void_p)]
+
+
 EXPORTS = (
     "mvs_version", "mvs_build_id", "mvs_create", "mvs_destroy", "mvs_last_error", "mvs_launch_count", "mvs_set_model",
     "mvs_set_gmm_prior", "mvs_set_vposer", "mvs_vposer_decode", "mvs_set_cameras", "mvs_set_batch", "mvs_set_keypoints", "mvs_set_loss_config",
-    "mvs_closure", "mvs_forward", "mvs_lbfgs_run", "mvs_lbfgs_step", "mvs_fit", "mvs_fit_seq", "mvs_fit_host", "mvs_sdf_grid", "mvs_profile", "mvs_profile_read",
+    "mvs_closure", "mvs_forward", "mvs_lbfgs_run", "mvs_lbfgs_step", "mvs_fit", "mvs_fit_seq", "mvs_fit_stream", "mvs_fit_host", "mvs_sdf_grid", "mvs_profile", "mvs_profile_read",
     "mvs_kernel_name", "mvs_set_exec_mode", "mvs_set_anchor", "mvs_set_joints3d", "mvs_init_guess",
 )
 NUM_KERNEL_IDS = 18
@@ -106,6 +113,8 @@ def load() -> ctypes.CDLL:
     lib.mvs_fit.argtypes = [vp, vp, ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig), vp, ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_fit_seq.argtypes = [vp, vp, ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig), vp, vp,
                                 ctypes.POINTER(LbfgsStats), vp]
+    lib.mvs_fit_stream.argtypes = [vp, ctypes.POINTER(FrameStream), ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig),
+                                   ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_fit_host.argtypes = [vp, vp, vp, vp, vp, ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig), vp,
                                  ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_sdf_grid.argtypes = [vp, vp, vp, ci, vp, ci, ci, ci, vp]

@@ -269,6 +269,35 @@ class FittingContext:
                                                 ctypes.byref(st), self._stream()), "mvs_fit")
         return final, _stats_dict(st)
 
+    def fit_stream(self, params: torch.Tensor, gt_uv, conf, joint_weights, stage_cfgs, opt_cfg=None, joints3d=None,
+                   conf3d=None):
+        """mvs_fit over F frames of any number through the context's B slots (mvs_fit_stream): params [F,86] CUDA float32,
+        updated in place; gt_uv [V,F,K,2], conf [V,F,K], joint_weights [K] (numpy or tensors); joints3d [F,K,3] with conf3d
+        [F,K] switch the 3-D joint term on for this call.  Every frame gets the bits mvs_fit gives it.  Afterwards the context
+        holds no keypoints and no 3-D targets (set_keypoints / set_joints3d again before a closure or fit).
+        Returns (final_loss [F], stats)."""
+        assert params.is_cuda and params.dtype == torch.float32 and params.is_contiguous() and params.dim() == 2
+        F = params.shape[0]
+        dev = lambda a: None if a is None else torch.as_tensor(a).to(self.device, torch.float32).contiguous()
+        gt_uv, conf, jw = dev(gt_uv), dev(conf), dev(joint_weights).reshape(-1)
+        assert tuple(gt_uv.shape) == (self.V, F, self.K, 2) and tuple(conf.shape) == (self.V, F, self.K), \
+            (tuple(gt_uv.shape), tuple(conf.shape), (self.V, F, self.K))
+        if (joints3d is None) != (conf3d is None):
+            raise ValueError("fit_stream: joints3d and conf3d go together")
+        j3, c3 = dev(joints3d), dev(conf3d)
+        if j3 is not None and (tuple(j3.shape) != (F, self.K, 3) or tuple(c3.shape) != (F, self.K)):
+            raise ValueError("fit_stream: want joints3d [%d,%d,3] and conf3d [%d,%d], got %s and %s"
+                             % (F, self.K, F, self.K, tuple(j3.shape), tuple(c3.shape)))
+        final = torch.empty(F, dtype=torch.float32, device=self.device)
+        s = _lib.FrameStream(F, _ptr(params), _ptr(gt_uv), _ptr(conf), _ptr(jw), _ptr(j3), _ptr(c3), _ptr(final))
+        arr = (_lib.LossConfig * len(stage_cfgs))(*stage_cfgs)
+        cfg = opt_cfg or self.make_lbfgs_config()
+        st = _lib.LbfgsStats()
+        self._j3d_keep = None
+        _lib.check(self.h, self.lib.mvs_fit_stream(self.h, ctypes.byref(s), len(stage_cfgs), arr, ctypes.byref(cfg),
+                                                   ctypes.byref(st), self._stream()), "mvs_fit_stream")
+        return final, _stats_dict(st)
+
     def fit_host(self, params_host: np.ndarray, gt_uv: np.ndarray, conf: np.ndarray, joint_weights: np.ndarray,
                  stage_cfgs, opt_cfg=None):
         """Host-buffer entry point (mvs_fit_host): params_host [B,86] float32 updated in place."""

@@ -92,6 +92,19 @@ int make_loss_params(mvs_ctx* ctx, const mvs_loss_config* c, LossParams* out) {
     *out = l;
     return MVS_OK;
 }
+
+int ensure_keypoint_ws(mvs_ctx* ctx) {
+    Workspace& w = ctx->ws;
+    const int V = ctx->cams.num_views;
+    if (w.gt_uv && w.kp_views == V) return MVS_OK;
+    const size_t n = (size_t)V * w.B * ctx->m.K;
+    int rc;
+    if ((rc = dev_alloc(ctx, &w.gt_uv, n * 2))) return rc;
+    if ((rc = dev_alloc(ctx, &w.conf, n))) return rc;
+    if (!w.joint_w && (rc = dev_alloc(ctx, &w.joint_w, kMaxKeypoints))) return rc;
+    w.kp_views = V;
+    return MVS_OK;
+}
 }  // namespace mvs
 
 extern "C" {
@@ -479,12 +492,8 @@ int mvs_set_keypoints(mvs_ctx* ctx, const float* gt_uv, const float* conf, const
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     Workspace& w = ctx->ws;
     const size_t n = (size_t)ctx->cams.num_views * w.B * ctx->m.K;
-    int rc;
-    if (!w.gt_uv || !ctx->have_kp) {
-        if ((rc = dev_alloc(ctx, &w.gt_uv, n * 2))) return rc;
-        if ((rc = dev_alloc(ctx, &w.conf, n))) return rc;
-        if (!w.joint_w && (rc = dev_alloc(ctx, &w.joint_w, kMaxKeypoints))) return rc;
-    }
+    const int rc = ensure_keypoint_ws(ctx);
+    if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(w.gt_uv, gt_uv, n * 2 * sizeof(float), kind, st));

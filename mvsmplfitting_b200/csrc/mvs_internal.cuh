@@ -105,6 +105,14 @@ struct LbfgsState;
 struct LbfgsCfg;
 struct FrameScalars;
 struct TcState;
+struct StreamState;                   // mvs_fit_stream scratch (mvs_lbfgs.cu)
+
+// The frames a frame-resident run fits when they are not the context's batch (mvs_fit_stream): n frames, every array with
+// row stride n (gt_uv [V][n][K][2], conf [V][n][K], j3d_xyz [n][K][3], j3d_conf [n][K]; the 3-D pair may be NULL)
+struct FrameInputs {
+    int n;
+    const float *gt_uv, *conf, *joint_w, *j3d_xyz, *j3d_conf;
+};
 
 // Per-batch workspace (slot-indexed: slot = position in the active-frame list)
 struct Workspace {
@@ -129,6 +137,7 @@ struct Workspace {
     float* pen_loss = nullptr;        // [B]
     float* dtransl = nullptr;         // [B][3]
     float* dgchain = nullptr;         // [B][24][3]
+    int kp_views = 0;                 // V of the allocated gt_uv / conf
     float* gt_uv = nullptr;           // [V][B][K][2]
     float* conf = nullptr;            // [V][B][K]
     float* joint_w = nullptr;         // [K]
@@ -234,6 +243,7 @@ struct mvs_ctx {
     float* rest_joints = nullptr;    // [K,3] keypoints of the rest pose at scale rest_scale (mvs_init.cu), computed once
     float rest_scale = -1.f;
     int2* stage_rng = nullptr;       // [B] per-frame slice of the stage table (mvs_fit_seq), device
+    mvs::StreamState* fstream = nullptr;  // frame-stream scratch (mvs_fit_stream), created on first use
 };
 
 namespace mvs {
@@ -333,7 +343,7 @@ int launch_closure_resident(mvs_ctx* ctx, const float* x_dev, float* loss_dev, f
                             float* proj_dev, cudaStream_t st);
 int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
                           const LossParams* lp_tab_host, int nstages, FrameScalars* frame_scalars_out, float* last_grad_dev,
-                          cudaStream_t st, const int2* stage_rng_dev);
+                          cudaStream_t st, const int2* stage_rng_dev, const FrameInputs* frames = nullptr);
 // dense regime (SDF term): per round  posedirs_gemm_tc -> skin -> sdf_fused -> frame_step
 int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);                      // mvs_closure.cu
 int launch_sdf_fused(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu
@@ -348,6 +358,7 @@ int launch_frame_step(mvs_ctx* ctx, float* params_dev, const LbfgsState& L, cons
 int frame_step_begin_run(mvs_ctx* ctx, cudaStream_t st);                 // mvs_resident.cu
 int launch_frame_fwd_dense(mvs_ctx* ctx, const float* x_dev, const LbfgsState& L, int nstages, cudaStream_t st);   // mvs_resident.cu
 int make_loss_params(mvs_ctx* ctx, const mvs_loss_config* c, LossParams* out);      // mvs_api.cu: validation + conversion
+int ensure_keypoint_ws(mvs_ctx* ctx);          // mvs_api.cu: gt_uv / conf for the cameras' view count, joint weights
 int sdf_grid_launch(mvs_ctx* ctx, float* phi, const int* faces, int num_faces, const float* verts, int batch,
                     int n_verts, int G, cudaStream_t st);
 }  // namespace mvs

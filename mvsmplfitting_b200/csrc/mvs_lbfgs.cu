@@ -33,13 +33,12 @@
 
 namespace mvs {
 
-// reset != 0: fresh optimiser (new stage).  reset == 0: next step() of the same optimiser: history, d, t,
-// H_diag, prev_flat_grad, prev_loss and n_iter persist (lbfgs_ls.py:292-300,436-443).
-__global__ void lbfgs_init_kernel(LbfgsState S, const float* __restrict__ params, int B, int reset, int nstages,
-                                  const int2* __restrict__ stage_rng) {
-    const int b = blockIdx.x, lane = threadIdx.x;
-    if (b >= B) return;
-    VLOOP(i) S.x_eval[(size_t)b * kParams + i] = params[(size_t)b * kParams + i];
+// Start of frame b's run, one warp; x = its parameter row.  reset != 0: fresh optimiser (new stage).  reset == 0: next
+// step() of the same optimiser: history, d, t, H_diag, prev_flat_grad, prev_loss and n_iter persist
+// (lbfgs_ls.py:292-300,436-443).
+__device__ __forceinline__ void init_frame_state(const LbfgsState& S, const float* __restrict__ x, int b, int reset, int nstages,
+                                                 const int2* __restrict__ stage_rng, int lane) {
+    VLOOP(i) S.x_eval[(size_t)b * kParams + i] = x[i];
     if (lane == 0) {
         FrameScalars s;
         if (reset) {
@@ -58,6 +57,13 @@ __global__ void lbfgs_init_kernel(LbfgsState S, const float* __restrict__ params
         }
         S.sc[b] = s;
     }
+}
+
+__global__ void lbfgs_init_kernel(LbfgsState S, const float* __restrict__ params, int B, int reset, int nstages,
+                                  const int2* __restrict__ stage_rng) {
+    const int b = blockIdx.x;
+    if (b >= B) return;
+    init_frame_state(S, params + (size_t)b * kParams, b, reset, nstages, stage_rng, threadIdx.x);
 }
 
 __global__ void __launch_bounds__(32)
@@ -134,6 +140,108 @@ __global__ void iota2_kernel(int* p, int n, int* na) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) p[i] = i;
     if (i == 0) *na = n;
+}
+
+// mvs_fit_stream (DESIGN.md section 4): the context's B slots are lanes, each holding one frame of an F-frame stream
+struct StreamState {
+    int cap = 0;                        // entries of sc
+    FrameScalars* sc = nullptr;         // [cap] frame scalars of the frame-resident groups (one per frame of the stream)
+    int* lane_frame = nullptr;          // [B] frame held by each lane of a dense group, -1: none
+    long long* lane_start = nullptr;    // [B] round of the group in which the lane's frame started
+    float* lane_params = nullptr;       // [B][86] the lanes' parameters (what params_dev is to mvs_fit)
+    int* queue = nullptr;               // [1] next frame of the stream to enter a lane
+    long long* end_round = nullptr;     // [1] max over retired frames of start round + evaluations: the rounds the group ran
+    int* host = nullptr;                // pinned [2]: queue position of the two chunks in flight (next to their active counts)
+};
+
+struct StreamArgs {
+    int F, B, V, K, nstages;
+    float* params;                      // [F][86] the stream's parameters, in / out
+    float* final_loss;                  // [F] or NULL
+    const float *gt_uv, *conf;          // [V][F][K][2], [V][F][K]
+    const float *j3d_xyz, *j3d_conf;    // [F][K][3], [F][K]; NULL: 3-D term off
+    float *ws_gt_uv, *ws_conf, *ws_j3d_xyz, *ws_j3d_conf;     // the lanes' rows, read by the dense kernels
+    int* lane_frame; long long* lane_start; float* lane_params; int* queue; long long* end_round;
+    int* pose_valid;
+};
+
+// Runs just before lbfgs_compact_kernel at every compaction point of a dense group of mvs_fit_stream (and once before the
+// group's first round).  Every lane whose frame is done hands the frame's parameters, final loss and counts back to the
+// stream; the freed lanes then take the next queued frames in ascending lane order (ballot + prefix sum: no atomics decide
+// which lane gets which frame), and each new frame starts exactly as lbfgs_init_kernel starts a frame of mvs_fit, so that
+// its bits do not depend on the lane or on when it entered.  round: rounds of the group run so far (the new frames' first
+// round).  flush != 0: hand back every frame still in a lane, take none.
+__global__ void __launch_bounds__(1024) stream_refill_kernel(LbfgsState S, StreamArgs a, long long round, int flush) {
+    __shared__ int wsum[32];
+    __shared__ int qbase;
+    __shared__ int s_old[1024], s_new[1024];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    if (tid == 0) qbase = *a.queue;
+    __syncthreads();
+    for (int l0 = 0; l0 < a.B; l0 += 1024) {
+        const int l = l0 + tid;
+        int old = -1, fresh = -1;
+        bool freed = false;
+        if (l < a.B) {
+            old = a.lane_frame[l];
+            freed = old < 0 || flush || S.sc[l].phase == PH_DONE;
+            if (old >= 0 && freed) {                      // the frame's totals, as lbfgs_finalize_kernel counts them
+                const FrameScalars& s = S.sc[l];
+                if (a.final_loss) a.final_loss[old] = s.final_loss;
+                atomicAdd((unsigned long long*)&S.totals[0], (unsigned long long)s.iters);
+                atomicAdd((unsigned long long*)&S.totals[1], (unsigned long long)s.evals);
+                atomicAdd((unsigned long long*)&S.totals[2], (unsigned long long)(s.nan_flag + s.nan_acc));
+                atomicMax((unsigned long long*)a.end_round, (unsigned long long)(a.lane_start[l] + s.evals));
+            } else {
+                old = -1;
+            }
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, freed);
+        const int pre = __popc(m & ((1u << lane) - 1));
+        if (lane == 0) wsum[wid] = __popc(m);
+        __syncthreads();
+        if (freed) {
+            int f = qbase + pre;
+            for (int w = 0; w < wid; ++w) f += wsum[w];
+            fresh = (!flush && f < a.F) ? f : -1;
+            a.lane_frame[l] = fresh;
+            if (fresh >= 0) a.lane_start[l] = round;
+            else S.sc[l].phase = PH_DONE;                 // an empty lane stays out of the active list
+        }
+        s_old[tid] = old;
+        s_new[tid] = fresh;
+        __syncthreads();
+        if (tid == 0 && !flush) {
+            int tot = qbase;
+            for (int w = 0; w < 32; ++w) tot += wsum[w];
+            qbase = tot < a.F ? tot : a.F;
+        }
+        // parameters out and in, the new frame's detections into the lane's rows: one warp per lane
+        for (int j = wid; j < 1024 && l0 + j < a.B; j += 32) {
+            const int ln = l0 + j, fo = s_old[j], fn = s_new[j];
+            float* xl = a.lane_params + (size_t)ln * kParams;
+            if (fo >= 0) {
+                VLOOP(i) a.params[(size_t)fo * kParams + i] = xl[i];
+            }
+            if (fn < 0) continue;
+            VLOOP(i) xl[i] = a.params[(size_t)fn * kParams + i];
+            const int K = a.K;
+            for (int v = 0; v < a.V; ++v) {
+                const size_t dst = (size_t)v * a.B + ln, src = (size_t)v * a.F + fn;
+                for (int k = lane; k < 2 * K; k += 32) a.ws_gt_uv[dst * 2 * K + k] = a.gt_uv[src * 2 * K + k];
+                for (int k = lane; k < K; k += 32) a.ws_conf[dst * K + k] = a.conf[src * K + k];
+            }
+            if (a.j3d_xyz) {
+                for (int k = lane; k < 3 * K; k += 32) a.ws_j3d_xyz[(size_t)ln * 3 * K + k] = a.j3d_xyz[(size_t)fn * 3 * K + k];
+                for (int k = lane; k < K; k += 32) a.ws_j3d_conf[(size_t)ln * K + k] = a.j3d_conf[(size_t)fn * K + k];
+            }
+            __syncwarp();
+            init_frame_state(S, xl, ln, 1, a.nstages, nullptr, lane);
+            if (lane == 0) a.pose_valid[ln] = 0;           // the lane's pose cache belongs to its previous frame
+        }
+        __syncthreads();
+    }
+    if (tid == 0) *a.queue = qbase;
 }
 
 static int ensure_state(mvs_ctx* ctx, int H) {
@@ -242,13 +350,16 @@ static int dense_round(mvs_ctx* ctx, float* params_dev, const LbfgsState& S, con
 }
 
 // Dense regime (SDF term on): rounds of dense_round until no frame is active.  Finished frames are compacted out once per
-// chunk of rounds.
-static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int nst, cudaStream_t st) {
+// chunk of rounds.  fs (mvs_fit_stream): the finished frames' lanes are refilled from the stream's queue just before each
+// compaction.
+static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int nst, cudaStream_t st,
+                     const StreamArgs* fs = nullptr) {
     LbfgsState& S = *ctx->lbfgs;
     Workspace& w = ctx->ws;
     const int B = w.B;
     const int chunk = 8;
-    const long long max_rounds = ((long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8) * nst;
+    const long long frames_per_lane = fs ? (fs->F + B - 1) / B + 1 : 1;
+    const long long max_rounds = ((long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8) * nst * frames_per_lane;
     long long rounds = 0;
     int na_host = B;
     static const bool trace_na = getenv("MVS_TRACE_NA") != nullptr;       // debugging aid: active-list size per chunk
@@ -267,6 +378,8 @@ static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int n
         MVS_CUDA_OK(ctx, cudaEventCreateWithFlags(&S.na_event[1], cudaEventDisableTiming | cudaEventBlockingSync));
     }
     int* na_slots = reinterpret_cast<int*>(S.na_host);           // [0], [1]: two chunks in flight
+    int* queue_slots = fs ? ctx->fstream->host : nullptr;         // the same chunks' queue positions
+    bool drained = fs == nullptr;                                 // the host has seen the stream's queue empty
     int pending = -1;                                             // chunk whose count has not been read yet
     long long chunk_idx = 0;
     w.na_bound = B;                                               // grids shrink with the (lagging) host view of the count
@@ -275,20 +388,25 @@ static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int n
             if ((rc = dense_round(ctx, params_dev, S, cfg, nst, st))) return rc;
             ++rounds;
         }
+        if (fs) MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, stream_refill_kernel<<<1, 1024, 0, st>>>(S, *fs, rounds, 0));
         // compaction changes slot -> frame, so the surviving frames' Phi / transforms are rebuilt for their new slots
         MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
         if ((rc = launch_frame_fwd_dense(ctx, S.x_eval, S, nst, st))) return rc;
         const int cur = (int)(chunk_idx & 1);
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(&na_slots[cur], w.na, sizeof(int), cudaMemcpyDeviceToHost, st));
+        if (fs) MVS_CUDA_OK(ctx, cudaMemcpyAsync(&queue_slots[cur], fs->queue, sizeof(int), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaEventRecord(S.na_event[cur], st));
         if (pending >= 0) {
             const auto tb0 = std::chrono::steady_clock::now();
             MVS_CUDA_OK(ctx, cudaEventSynchronize(S.na_event[pending]));
             if (trace_host) blocked_us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - tb0).count();
             na_host = na_slots[pending];
+            if (!drained) drained = queue_slots[pending] >= fs->F;
             if (trace_na) fprintf(stderr, "[mvs] dense regime: chunk %lld, active frames %d\n", chunk_idx - 1, na_host);
-            if (na_host <= 0) break;
-            w.na_bound = na_host;                                 // the list only shrinks: still an upper bound
+            if (na_host <= 0) break;                              // (a refill leaves no lane idle while frames are queued)
+            // Without refills the list only shrinks, so the count is an upper bound for every later round.  Refills add
+            // frames back until the queue is empty: until the host has seen that, the grids keep all B slots.
+            w.na_bound = drained ? na_host : B;
         }
         pending = cur;
         ++chunk_idx;
@@ -431,6 +549,18 @@ int evaluate_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* g
     return launch_closure(ctx, x_dev, loss_dev, grad_dev, joints_dev, proj_dev, verts_dev, st);
 }
 
+// One past the last stage of the run that starts at stage i: the following stages of the same regime, SDF grid and face
+// mode, at most max_run of them (one stage per run in exec mode 2 and in the batched chain)
+static int stage_group_end(const mvs_ctx* ctx, const std::vector<LossParams>& lps, int i, int H, int max_run) {
+    const Regime rg = stage_regime(ctx, lps[i], H, false);
+    int j = i + 1;
+    while (ctx->exec_mode != 2 && rg != kBatched && j < (int)lps.size() && j - i < max_run &&
+           stage_regime(ctx, lps[j], H, false) == rg && lps[j].sdf_grid == lps[i].sdf_grid &&
+           lps[j].sdf_all_faces == lps[i].sdf_all_faces)
+        ++j;
+    return j;
+}
+
 // All stages of a fit.  Consecutive stages that run in the same regime are handed to ONE multi-stage run in which
 // every frame changes stage on its own (frames are independent problems, so a frame that converged need not wait at
 // the stage boundary for the slowest one; the per-frame arithmetic is the sequential schedule's).  exec_mode 2 keeps
@@ -470,11 +600,7 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
     int i = 0;
     while (i < n_stages) {
         const Regime rg = stage_regime(ctx, lps[i], H, false);
-        int j = i + 1;
-        while (ctx->exec_mode != 2 && rg != kBatched && j < n_stages && j - i < max_run &&
-               stage_regime(ctx, lps[j], H, false) == rg && lps[j].sdf_grid == lps[i].sdf_grid &&
-               lps[j].sdf_all_faces == lps[i].sdf_all_faces)
-            ++j;
+        const int j = stage_group_end(ctx, lps, i, H, max_run);
         ctx->loss = lps[i];
         ctx->have_loss = true;
         RunOpts o;
@@ -510,6 +636,149 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
     }
     ctx->loss = lps[n_stages - 1];
     return MVS_OK;
+}
+
+static void dev_free(mvs_ctx* ctx, void* p) {
+    for (auto it = ctx->allocs.begin(); it != ctx->allocs.end(); ++it)
+        if (*it == p) { ctx->allocs.erase(it); break; }
+    cudaFree(p);
+}
+
+// Lane state of the dense groups, and frame scalars for F frames when a frame-resident group runs (grow-only)
+static int ensure_stream_state(mvs_ctx* ctx, int F_resident) {
+    int rc;
+    if (!ctx->fstream) {
+        StreamState* ss = new StreamState();
+        ctx->fstream = ss;
+        const size_t B = (size_t)ctx->ws.B;
+        unsigned char* raw = nullptr;
+        if ((rc = dev_alloc(ctx, &ss->lane_frame, B))) return rc;
+        if ((rc = dev_alloc(ctx, &raw, B * sizeof(long long)))) return rc;
+        ss->lane_start = reinterpret_cast<long long*>(raw);
+        if ((rc = dev_alloc(ctx, &ss->lane_params, B * kParams))) return rc;
+        if ((rc = dev_alloc(ctx, &ss->queue, 1))) return rc;
+        if ((rc = dev_alloc(ctx, &raw, sizeof(long long)))) return rc;
+        ss->end_round = reinterpret_cast<long long*>(raw);
+        MVS_CUDA_OK(ctx, cudaMallocHost(&ss->host, 2 * sizeof(int)));
+    }
+    StreamState& ss = *ctx->fstream;
+    if (ss.cap < F_resident) {
+        if (ss.sc) dev_free(ctx, ss.sc);
+        ss.sc = nullptr;
+        ss.cap = 0;
+        unsigned char* raw = nullptr;
+        if ((rc = dev_alloc(ctx, &raw, (size_t)F_resident * sizeof(FrameScalars)))) return rc;
+        ss.sc = reinterpret_cast<FrameScalars*>(raw);
+        ss.cap = F_resident;
+    }
+    return MVS_OK;
+}
+
+// One run of mvs_fit_stream: stages lps[0 .. nst) of one regime over all F frames of the stream
+static int run_stream_group(mvs_ctx* ctx, const mvs_frame_stream* s, Regime rg, const LossParams* lps, int nst,
+                            const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats, cudaStream_t st) {
+    LbfgsCfg cfg;
+    int rc = begin_run(ctx, c, false, lps, nst, &cfg, st);
+    if (rc) return rc;
+    LbfgsState& S = *ctx->lbfgs;
+    StreamState& ss = *ctx->fstream;
+    Workspace& w = ctx->ws;
+    const int F = s->n_frames, B = w.B, K = ctx->m.K;
+    long long* th = reinterpret_cast<long long*>(S.na_host) + 1;      // [0..3] totals, [4] rounds of a dense group
+    if (rg == kResident) {
+        // one launch over all F frames, one CTA each: the block scheduler refills the SMs as frames finish
+        const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, s->gt_xyz, s->conf3d};
+        if ((rc = launch_lbfgs_resident(ctx, s->params, cfg, cfg.history, S.lp_tab, lps, nst, ss.sc, nullptr, st, nullptr, &in)))
+            return rc;
+        LbfgsState Sf = S;
+        Sf.sc = ss.sc;
+        MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_finalize_kernel<<<(F + 255) / 256, 256, 0, st>>>(Sf, F, s->final_loss, S.totals, 1));
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+        MVS_CUDA_OK(ctx, cudaGetLastError());
+        if (stats) {
+            stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
+            stats->rounds += (int)th[3];
+        }
+        return MVS_OK;
+    }
+    // dense rounds over B lanes fed from the queue
+    if ((rc = frame_step_begin_run(ctx, st))) return rc;                 // (allocates the pose cache on first use)
+    StreamArgs a;
+    a.F = F; a.B = B; a.V = ctx->cams.num_views; a.K = K; a.nstages = nst;
+    a.params = s->params; a.final_loss = s->final_loss; a.gt_uv = s->gt_uv; a.conf = s->conf;
+    a.j3d_xyz = s->gt_xyz; a.j3d_conf = s->conf3d;
+    a.ws_gt_uv = w.gt_uv; a.ws_conf = w.conf; a.ws_j3d_xyz = w.j3d_xyz; a.ws_j3d_conf = w.j3d_conf;
+    a.lane_frame = ss.lane_frame; a.lane_start = ss.lane_start; a.lane_params = ss.lane_params; a.queue = ss.queue;
+    a.end_round = ss.end_round; a.pose_valid = w.pose_valid;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(w.joint_w, s->joint_weights, (size_t)K * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.lane_frame, 0xff, (size_t)B * sizeof(int), st));
+    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.queue, 0, sizeof(int), st));
+    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.end_round, 0, sizeof(long long), st));
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
+    // the first min(F, B) frames enter through the same path as every later one
+    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, stream_refill_kernel<<<1, 1024, 0, st>>>(S, a, 0, 0));
+    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
+    if ((rc = run_dense(ctx, ss.lane_params, cfg, nst, st, &a))) return rc;
+    // whatever the round limit left in the lanes (nothing, when every frame finished)
+    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, stream_refill_kernel<<<1, 1024, 0, st>>>(S, a, 0, 1));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 3 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th + 4, ss.end_round, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    if (stats) {
+        stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
+        stats->rounds += (int)th[4];
+        stats->dense_frame_evals += th[1]; stats->dense_rounds += (int)th[4];
+    }
+    return MVS_OK;
+}
+
+// mvs_fit_stream: the stage groups of run_fit, each over all F frames before the next starts
+static int run_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
+                      const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, cudaStream_t st) {
+    if (n_stages > 64) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: at most 64 stages");
+    std::vector<LossParams> lps(n_stages);
+    for (int i = 0; i < n_stages; ++i) {
+        const int rc = make_loss_params(ctx, &stage_cfgs[i], &lps[i]);
+        if (rc) return rc;
+        lps[i].j3d_on = s->gt_xyz ? 1 : 0;          // the stream's own targets, never the context's
+    }
+    const int H = opt_cfg->history_size > 0 ? opt_cfg->history_size : 100;
+    std::vector<int> ends;
+    bool any_dense = false, any_resident = false;
+    for (int i = 0; i < n_stages; i = ends.back()) {
+        const Regime rg = stage_regime(ctx, lps[i], H, false);
+        if (rg == kBatched)
+            return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_stream: stage %d would run in the batched reference chain (exec "
+                                                       "mode 1, history_size > 100 without the SDF term, or a model the "
+                                                       "frame-resident and dense kernels do not take), which has no frame stream", i);
+        (rg == kDense ? any_dense : any_resident) = true;
+        ends.push_back(stage_group_end(ctx, lps, i, H, kMaxStages));
+    }
+    int rc = ensure_stream_state(ctx, any_resident ? s->n_frames : 0);
+    if (rc) return rc;
+    if (any_dense) {
+        Workspace& w = ctx->ws;
+        if ((rc = ensure_keypoint_ws(ctx))) return rc;
+        if (s->gt_xyz && !w.j3d_xyz) {
+            const size_t n = (size_t)w.B * ctx->m.K;
+            if ((rc = dev_alloc(ctx, &w.j3d_xyz, n * 3))) return rc;
+            if ((rc = dev_alloc(ctx, &w.j3d_conf, n))) return rc;
+        }
+    }
+    // the dense groups overwrite the lanes' keypoint and 3-D target rows: from here on the context holds neither
+    ctx->have_kp = false;
+    ctx->j3d_enabled = false;
+    for (int i = 0, g = 0; i < n_stages && !rc; i = ends[g++]) {
+        ctx->loss = lps[i];
+        ctx->have_loss = true;
+        rc = run_stream_group(ctx, s, stage_regime(ctx, lps[i], H, false), &lps[i], ends[g] - i, opt_cfg, stats, st);
+    }
+    ctx->loss = lps[n_stages - 1];
+    ctx->loss.j3d_on = 0;
+    return rc;
 }
 
 }  // namespace mvs
@@ -565,6 +834,24 @@ int mvs_fit(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_config
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     if (stats) memset(stats, 0, sizeof(*stats));
     return run_fit(ctx, params_dev, n_stages, stage_cfgs, opt_cfg, final_loss_dev, stats, (cudaStream_t)stream);
+}
+
+int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
+                   const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0))
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: model, cameras and batch must be set first");
+    if (!s || n_stages <= 0 || !stage_cfgs || !opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: NULL / empty argument");
+    if (s->n_frames < 1) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: n_frames must be >= 1 (got %d)", s->n_frames);
+    if (!s->params || !s->gt_uv || !s->conf || !s->joint_weights)
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: params, gt_uv, conf and joint_weights are required");
+    if (s->gt_xyz && !s->conf3d) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: gt_xyz needs conf3d");
+    if (ctx->anchor_enabled)
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_stream: the anchor term is per batch (sequence smoothness); switch it "
+                                                   "off (mvs_set_anchor enable = 0) to fit a frame stream");
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    if (stats) memset(stats, 0, sizeof(*stats));
+    return run_stream(ctx, s, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
 }
 
 int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, const float* conf_host,

@@ -261,16 +261,18 @@ int launch_vposer_decode(mvs_ctx* ctx, const float* x_dev, float* body_pose_dev,
 
 int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int H, const LossParams* lp_tab_dev,
                           const LossParams* lph, int nstages, FrameScalars* sc_out, float* last_grad_dev, cudaStream_t st,
-                          const int2* stage_rng_dev) {
-    Workspace& w = ctx->ws;
+                          const int2* stage_rng_dev, const FrameInputs* frames) {
+    const Workspace& w = ctx->ws;
     int with_vposer = 0;
     for (int i = 0; i < nstages; ++i) with_vposer |= (lph[i].use_vposer == 2);
     const size_t smem = frame_smem(H, with_vposer != 0);
+    const FrameInputs in = frames ? *frames : FrameInputs{w.B, w.gt_uv, w.conf, w.joint_w, w.j3d_xyz, w.j3d_conf};
+    ResidentModel rm = make_resident_model(ctx);
+    rm.j3d_xyz = in.j3d_xyz; rm.j3d_conf = in.j3d_conf;
     MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
-               lbfgs_resident_kernel<<<w.B, kResThreads, smem, st>>>(make_resident_model(ctx), ctx->cams,
-                                                                     lp_tab_dev, nstages, cfg, params_dev, w.gt_uv, w.conf,
-                                                                     w.joint_w, w.B, H, sc_out, last_grad_dev, with_vposer,
-                                                                     stage_rng_dev));
+               lbfgs_resident_kernel<<<in.n, kResThreads, smem, st>>>(rm, ctx->cams, lp_tab_dev, nstages, cfg, params_dev,
+                                                                      in.gt_uv, in.conf, in.joint_w, in.n, H, sc_out,
+                                                                      last_grad_dev, with_vposer, stage_rng_dev));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }

@@ -214,19 +214,48 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
     frame.  `ctx` is a FittingContext whose model, priors (GMM / VPoser decoder), cameras and batch (= number of frames) are
     set.  With use_vposer = 2 stage configurations (the reference's default, cfg_files/fit_smpl.yaml) the latent code
     starts at 0 (init_guess.py:96-98), and results carry the decoded pose plus 'pose_embedding' (utils.py:741-759).
-    Returns (params [B,86] numpy -- pose slot = latent code under VPoser --, final_loss [B], stats)."""
-    B = len(seq["frames"])
-    assert ctx.B == B, "context batch %d != frames %d" % (ctx.B, B)
+    A context batch smaller than the sequence works as a pool of slots: the initial guesses are computed ctx.B frames at a
+    time, then all frames go through ONE `mvs_fit_stream` call, which refills a slot as soon as its frame is done (the same
+    results bit for bit).
+    Returns (params [F,86] numpy -- pose slot = latent code under VPoser --, final_loss [F], stats)."""
+    F = len(seq["frames"])
+    assert ctx.B <= F, "context batch %d > frames %d" % (ctx.B, F)
     latent = _uses_latent_pose(stage_cfgs)
     _check_missing_views(seq, stage_cfgs)
-    ctx.set_keypoints(seq["gt_uv"], seq["conf"], joint_weights(pose_format, use_hip))
-    ctx.set_loss(config=stage_cfgs[0])           # mvs_init_guess zeroes the pose slot when it holds a latent code
-    params, _ = ctx.init_guess(estimate_scale=estimate_scale, fixed_scale=fixed_scale, use_torso=True, hip_seed=1.0,
-                               want_joints3d=False, umeyama_as_written=umeyama_as_written)
-    final, stats = ctx.fit(params, stage_cfgs, opt_cfg)
+    jw = joint_weights(pose_format, use_hip)
+    guess = dict(estimate_scale=estimate_scale, fixed_scale=fixed_scale, use_torso=True, hip_seed=1.0, want_joints3d=False,
+                 umeyama_as_written=umeyama_as_written)
+    if ctx.B == F:
+        ctx.set_keypoints(seq["gt_uv"], seq["conf"], jw)
+        ctx.set_loss(config=stage_cfgs[0])           # mvs_init_guess zeroes the pose slot when it holds a latent code
+        params, _ = ctx.init_guess(**guess)
+        final, stats = ctx.fit(params, stage_cfgs, opt_cfg)
+        loss = final.cpu().numpy()
+        if result_folder is not None:
+            _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces)
+        return params.cpu().numpy(), loss, stats
+    B = ctx.B
+    params = torch.empty(F, 86, dtype=torch.float32, device=ctx.device)
+    for c0 in range(0, F, B):                        # initial guesses per chunk of B frames; the last chunk is padded with
+        n = min(B, F - c0)                           # zero-confidence rows, which are dropped
+        gt = np.zeros((seq["gt_uv"].shape[0], B) + seq["gt_uv"].shape[2:], np.float32)
+        cf = np.zeros((seq["conf"].shape[0], B) + seq["conf"].shape[2:], np.float32)
+        gt[:, :n], cf[:, :n] = seq["gt_uv"][:, c0:c0 + n], seq["conf"][:, c0:c0 + n]
+        ctx.set_keypoints(gt, cf, jw)
+        ctx.set_loss(config=stage_cfgs[0])
+        x, _ = ctx.init_guess(**guess)
+        params[c0:c0 + n] = x[:n]
+    final, stats = ctx.fit_stream(params, seq["gt_uv"], seq["conf"], jw, stage_cfgs, opt_cfg)
     loss = final.cpu().numpy()
-    if result_folder is not None:
-        _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces)
+    if result_folder is not None:                    # the export takes whole batches: chunks of B rows, the last one padded
+        for c0 in range(0, F, B):
+            n = min(B, F - c0)
+            chunk = torch.zeros(B, 86, dtype=torch.float32, device=ctx.device)
+            chunk[:n] = params[c0:c0 + n]
+            lc = np.zeros(B, np.float32)
+            lc[:n] = loss[c0:c0 + n]
+            _export(ctx, seq, chunk, lc, latent, result_folder, mesh_folder, faces, frames=seq["frames"][c0:c0 + n],
+                    rows=range(n))
     return params.cpu().numpy(), loss, stats
 
 
