@@ -242,6 +242,43 @@ typedef struct {
 int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
                    const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream);
 
+/* ---- mvs_fit_seq over S video sequences of any number and length through the context's B slots (is_seq, code/main.py:76-79).
+ *      Sequence s owns frames [seq_offsets[s], seq_offsets[s+1]) of the F-frame arrays, in time order.  Every frame gets
+ *      exactly the parameters and final loss that mvs_fit_seq gives it when frame t of every sequence is fitted as one batch
+ *      of S (mvsmplfitting_b200.seqio.fit_sequences with a batch of S):
+ *        cold frame: the first frame of a sequence, or one whose predecessor's final loss is not <= reinit_loss (NaN is not).
+ *          It starts from its own params row -- the caller's cold start point, mvs_init_guess -- and runs every stage.
+ *        warm frame: starts from the predecessor's fitted row (load_init, code/utils/init_guess.py:137-166) with its own
+ *          params row's body-pose slot [13,82) (fix_params puts the pose back to the hip seed) unless the stages optimise a
+ *          latent code (use_vposer = 2: the whole row is carried), and runs stages 2 .. n-1 with stage 2's body_pose_weight
+ *          x 0.15 (code/utils/non_linear_solver.py:157-162).
+ *      Stages are grouped into runs as mvs_fit_seq groups them; stages 2 .. n-1 must form one run, the chaining run, in which
+ *      a finished frame hands its slot to its successor on the device (frame-resident: one CTA per sequence walks its frames
+ *      in one launch; dense: a lane takes the successor at the next compaction of the active list).  The runs before it take
+ *      cold frames as a frame stream (mvs_fit_stream); a sequence whose next frame is cold parks it until the next pass of
+ *      those runs.  All arrays except seq_offsets are device pointers.
+ *      stats: frame_iterations, frame_evals, frames_nan and dense_frame_evals are sums over the F frames; rounds and
+ *      dense_rounds count the rounds the call ran.  A frame-resident chaining run counts, per pass, the largest number of
+ *      closure evaluations one sequence's frames needed in it (the critical path of its launch) as rounds.
+ *      Refused (MVS_ERR_UNSUPPORTED): stages in the batched reference chain, the anchor term, stages 2 .. n-1 that do not
+ *      form one run (exec mode 2 with n_stages > 3, a change of regime, SDF grid or face mode between them).
+ *      MVS_ERR_INVALID: NULL or empty arguments, n_stages <= 2, seq_offsets not starting at 0 or not strictly ascending,
+ *      stages that mix use_vposer 2 with axis-angle poses.
+ *      Context state afterwards as after mvs_fit_stream: no keypoints, 3-D term off, the last stage's loss configuration set.
+ *      The 3-D joint term is not part of the call.  Synchronises. */
+typedef struct {
+    int n_sequences;               /* S >= 1 */
+    const int* seq_offsets;        /* HOST [S+1]: 0 = off[0] < off[1] < ... < off[S] = F (no empty sequence) */
+    float* params;                 /* [F,86] in: every frame's cold start point; out: fitted parameters */
+    const float* gt_uv;            /* [V,F,K,2] */
+    const float* conf;             /* [V,F,K] */
+    const float* joint_weights;    /* [K] */
+    float* final_loss;             /* [F] or NULL */
+    float reinit_loss;             /* 5000 in the reference (code/utils/init_guess.py:142) */
+} mvs_sequence_stream;
+int mvs_fit_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
+                       const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream);
+
 /* ---- host-buffer entry point (what a caller without device memory uses): copies keypoints and
  *      parameters host->device, runs `n_stages` optimisation stages (one mvs_loss_config each, the weight
  *      schedule of code/utils/non_linear_solver.py:109-203), copies parameters and losses back.
@@ -266,8 +303,8 @@ int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, cons
  *      params_dev [B,86] is overwritten; joints3d_dev [B,K,3] receives the alignment target (may be NULL).
  *      Uses the keypoints and cameras already uploaded; asynchronous on `stream`.  The rest joints are computed once per
  *      context and fixed_scale (seed + the 3-kernel geometry chain) and cached: a call is one launch afterwards.
- *      The warm start of sequences (load_init, init_guess.py:137-166) is a parameter copy and has no entry point: pass the
- *      previous result as params to mvs_fit with skip_stages (below). */
+ *      The warm start of sequences (load_init, init_guess.py:137-166) is a parameter copy done by mvs_fit_seq_stream on the
+ *      device; with mvs_fit_seq the caller passes the previous result as the frame's params row and marks it warm. */
 typedef struct {
     int estimate_scale;            /* not setting['fix_scale'] (init_guess.py:24) */
     float fixed_scale;             /* setting['fixed_scale'] or 1 (init_guess.py:25) */

@@ -65,10 +65,17 @@ class FrameStream(ctypes.Structure):
                 ("final_loss", ctypes.c_void_p)]
 
 
+class SequenceStream(ctypes.Structure):
+    """mvs_sequence_stream (include/mvsmpl.h)"""
+    _fields_ = [("n_sequences", ctypes.c_int), ("seq_offsets", ctypes.c_void_p), ("params", ctypes.c_void_p),
+                ("gt_uv", ctypes.c_void_p), ("conf", ctypes.c_void_p), ("joint_weights", ctypes.c_void_p),
+                ("final_loss", ctypes.c_void_p), ("reinit_loss", ctypes.c_float)]
+
+
 EXPORTS = (
     "mvs_version", "mvs_build_id", "mvs_create", "mvs_destroy", "mvs_last_error", "mvs_launch_count", "mvs_set_model",
     "mvs_set_gmm_prior", "mvs_set_vposer", "mvs_vposer_decode", "mvs_set_cameras", "mvs_set_batch", "mvs_set_keypoints", "mvs_set_loss_config",
-    "mvs_closure", "mvs_forward", "mvs_lbfgs_run", "mvs_lbfgs_step", "mvs_fit", "mvs_fit_seq", "mvs_fit_stream", "mvs_fit_host", "mvs_sdf_grid", "mvs_profile", "mvs_profile_read",
+    "mvs_closure", "mvs_forward", "mvs_lbfgs_run", "mvs_lbfgs_step", "mvs_fit", "mvs_fit_seq", "mvs_fit_stream", "mvs_fit_seq_stream", "mvs_fit_host", "mvs_sdf_grid", "mvs_profile", "mvs_profile_read",
     "mvs_kernel_name", "mvs_set_exec_mode", "mvs_set_anchor", "mvs_set_joints3d", "mvs_init_guess",
 )
 NUM_KERNEL_IDS = 18
@@ -115,6 +122,8 @@ def load() -> ctypes.CDLL:
                                 ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_fit_stream.argtypes = [vp, ctypes.POINTER(FrameStream), ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig),
                                    ctypes.POINTER(LbfgsStats), vp]
+    lib.mvs_fit_seq_stream.argtypes = [vp, ctypes.POINTER(SequenceStream), ci, ctypes.POINTER(LossConfig),
+                                       ctypes.POINTER(LbfgsConfig), ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_fit_host.argtypes = [vp, vp, vp, vp, vp, ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig), vp,
                                  ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_sdf_grid.argtypes = [vp, vp, vp, ci, vp, ci, ci, ci, vp]

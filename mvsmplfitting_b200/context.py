@@ -298,6 +298,35 @@ class FittingContext:
                                                    ctypes.byref(st), self._stream()), "mvs_fit_stream")
         return final, _stats_dict(st)
 
+    def fit_seq_stream(self, params: torch.Tensor, gt_uv, conf, joint_weights, lengths, stage_cfgs, opt_cfg=None,
+                       reinit_loss: float = 5000.0):
+        """mvs_fit_seq over S video sequences through the context's B slots (mvs_fit_seq_stream): the frames of sequence s are
+        the next lengths[s] rows, in time order.  params [F,86] CUDA float32 holds every frame's cold start point (init_guess)
+        and is updated in place; gt_uv [V,F,K,2], conf [V,F,K], joint_weights [K] (numpy or tensors).  A frame after the first
+        starts from its predecessor's result while that frame's final loss is <= reinit_loss (skipping stages 0 and 1), from
+        its own row otherwise.  Every frame gets the bits seqio.fit_sequences gives it with a batch of S.  Afterwards the
+        context holds no keypoints.  Returns (final_loss [F], stats)."""
+        assert params.is_cuda and params.dtype == torch.float32 and params.is_contiguous() and params.dim() == 2
+        F = params.shape[0]
+        lengths = [int(n) for n in lengths]
+        if not lengths or min(lengths) < 1 or sum(lengths) != F:
+            raise ValueError("fit_seq_stream: want sequence lengths >= 1 that add up to %d frames, got %s" % (F, lengths))
+        off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(lengths)]), dtype=np.int32)
+        dev = lambda a: torch.as_tensor(a).to(self.device, torch.float32).contiguous()
+        gt_uv, conf, jw = dev(gt_uv), dev(conf), dev(joint_weights).reshape(-1)
+        assert tuple(gt_uv.shape) == (self.V, F, self.K, 2) and tuple(conf.shape) == (self.V, F, self.K), \
+            (tuple(gt_uv.shape), tuple(conf.shape), (self.V, F, self.K))
+        final = torch.empty(F, dtype=torch.float32, device=self.device)
+        s = _lib.SequenceStream(len(lengths), _ptr(off), _ptr(params), _ptr(gt_uv), _ptr(conf), _ptr(jw), _ptr(final),
+                                float(reinit_loss))
+        arr = (_lib.LossConfig * len(stage_cfgs))(*stage_cfgs)
+        cfg = opt_cfg or self.make_lbfgs_config()
+        st = _lib.LbfgsStats()
+        self._j3d_keep = None
+        _lib.check(self.h, self.lib.mvs_fit_seq_stream(self.h, ctypes.byref(s), len(stage_cfgs), arr, ctypes.byref(cfg),
+                                                       ctypes.byref(st), self._stream()), "mvs_fit_seq_stream")
+        return final, _stats_dict(st)
+
     def fit_host(self, params_host: np.ndarray, gt_uv: np.ndarray, conf: np.ndarray, joint_weights: np.ndarray,
                  stage_cfgs, opt_cfg=None):
         """Host-buffer entry point (mvs_fit_host): params_host [B,86] float32 updated in place."""

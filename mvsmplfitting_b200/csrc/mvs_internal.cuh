@@ -106,12 +106,28 @@ struct LbfgsCfg;
 struct FrameScalars;
 struct TcState;
 struct StreamState;                   // mvs_fit_stream scratch (mvs_lbfgs.cu)
+struct SeqState;                      // mvs_fit_seq_stream scratch (mvs_lbfgs.cu)
 
 // The frames a frame-resident run fits when they are not the context's batch (mvs_fit_stream): n frames, every array with
 // row stride n (gt_uv [V][n][K][2], conf [V][n][K], j3d_xyz [n][K][3], j3d_conf [n][K]; the 3-D pair may be NULL)
 struct FrameInputs {
     int n;
     const float *gt_uv, *conf, *joint_w, *j3d_xyz, *j3d_conf;
+};
+
+// The chaining run of mvs_fit_seq_stream (DESIGN.md section 4): a finished frame hands its slot (a CTA of the frame-resident
+// kernel, a lane of the dense rounds) to its successor in the same sequence.  Frames of sequence s are [off[s], off[s+1]).
+struct SeqChain {
+    int n_act = 0;                    // sequences of this pass
+    const int* act = nullptr;         // [n_act] their indices, ascending
+    int* cur = nullptr;               // [S] in: each sequence's first frame of the pass (cold); out: its parked frame, -1 = done
+    const int* off = nullptr;         // [S+1]
+    int2 cold{0, 0}, warm{0, 0};      // slices of the run's stage table for cold and warm-started frames
+    float reinit_loss = 0.f;          // a successor is warm iff its predecessor's final loss <= reinit_loss
+    int park = 0;                     // 1: a cold successor leaves the run (it has earlier runs to pass first)
+    int keep_pose = 0;                // 1: a warm frame keeps its own body-pose slot (axis-angle stages; fix_params)
+    float* final_loss = nullptr;      // [F] or NULL
+    long long* totals = nullptr;      // [4] iters, evals, NaN stops, largest evaluations of one CTA (frame-resident kernel)
 };
 
 // Per-batch workspace (slot-indexed: slot = position in the active-frame list)
@@ -244,6 +260,7 @@ struct mvs_ctx {
     float rest_scale = -1.f;
     int2* stage_rng = nullptr;       // [B] per-frame slice of the stage table (mvs_fit_seq), device
     mvs::StreamState* fstream = nullptr;  // frame-stream scratch (mvs_fit_stream), created on first use
+    mvs::SeqState* sstream = nullptr;     // sequence-stream scratch (mvs_fit_seq_stream), created on first use
 };
 
 namespace mvs {
@@ -344,6 +361,10 @@ int launch_closure_resident(mvs_ctx* ctx, const float* x_dev, float* loss_dev, f
 int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
                           const LossParams* lp_tab_host, int nstages, FrameScalars* frame_scalars_out, float* last_grad_dev,
                           cudaStream_t st, const int2* stage_rng_dev, const FrameInputs* frames = nullptr);
+// the chaining run of mvs_fit_seq_stream in the frame-resident regime: one CTA per sequence of q.act
+int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
+                              const LossParams* lp_tab_host, int nstages, const FrameInputs& frames, const SeqChain& q,
+                              cudaStream_t st);
 // dense regime (SDF term): per round  posedirs_gemm_tc -> skin -> sdf_fused -> frame_step
 int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);                      // mvs_closure.cu
 int launch_sdf_fused(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu

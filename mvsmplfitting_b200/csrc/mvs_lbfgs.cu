@@ -244,6 +244,124 @@ __global__ void __launch_bounds__(1024) stream_refill_kernel(LbfgsState S, Strea
     if (tid == 0) *a.queue = qbase;
 }
 
+// mvs_fit_seq_stream's dense chaining run: a lane holds a sequence, the queue is q.act (sequences, not frames)
+struct SeqArgs {
+    StreamArgs f;                       // F: frames of the call; the lane arrays and the queue position as for a frame stream
+    SeqChain q;
+    int* lane_seq;                      // [B] sequence of each lane's frame
+};
+
+// stream_refill_kernel for sequences, at the same points of the dense run.  A lane whose frame is done hands the frame back
+// and takes its successor in the same sequence: warm from the frame's fitted row (body-pose slot from the successor's own
+// row unless the stages carry a latent code), cold from the successor's row unless cold frames park.  A lane whose
+// sequence ends or parks takes the next queued sequence's pending frame, in ascending lane order (ballot + prefix sum).
+// A lane that continues stays active and freed lanes only take from the queue, so the host's na_bound rule holds.
+__global__ void __launch_bounds__(1024) seq_refill_kernel(LbfgsState S, SeqArgs a, long long round, int flush) {
+    __shared__ int wsum[32];
+    __shared__ int qbase;
+    __shared__ int s_old[1024], s_new[1024];
+    __shared__ unsigned char s_warm[1024];
+    const StreamArgs& f = a.f;
+    const SeqChain& q = a.q;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    if (tid == 0) qbase = *f.queue;
+    __syncthreads();
+    for (int l0 = 0; l0 < f.B; l0 += 1024) {
+        const int l = l0 + tid;
+        int old = -1, fresh = -1;
+        bool fin = false, freed = false, warm = false;
+        if (l < f.B) {
+            old = f.lane_frame[l];
+            fin = old < 0 || flush || S.sc[l].phase == PH_DONE;
+            if (old >= 0 && fin) {
+                const FrameScalars& s = S.sc[l];
+                if (f.final_loss) f.final_loss[old] = s.final_loss;
+                atomicAdd((unsigned long long*)&S.totals[0], (unsigned long long)s.iters);
+                atomicAdd((unsigned long long*)&S.totals[1], (unsigned long long)s.evals);
+                atomicAdd((unsigned long long*)&S.totals[2], (unsigned long long)(s.nan_flag + s.nan_acc));
+                atomicMax((unsigned long long*)f.end_round, (unsigned long long)(f.lane_start[l] + s.evals));
+                const int sq = a.lane_seq[l], nx = old + 1;
+                const bool more = !flush && nx < q.off[sq + 1];
+                warm = more && s.final_loss <= q.reinit_loss;          // NaN is not
+                if (warm || (more && !q.park)) {
+                    fresh = nx;
+                } else {
+                    q.cur[sq] = more ? nx : -1;
+                    freed = true;
+                }
+            } else {
+                freed = fin;
+                old = -1;
+            }
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, freed);
+        const int pre = __popc(m & ((1u << lane) - 1));
+        if (lane == 0) wsum[wid] = __popc(m);
+        __syncthreads();
+        if (freed) {
+            int k = qbase + pre;
+            for (int w = 0; w < wid; ++w) k += wsum[w];
+            const int sq = (!flush && k < q.n_act) ? q.act[k] : -1;
+            if (sq >= 0) { fresh = q.cur[sq]; a.lane_seq[l] = sq; }
+        }
+        if (fin) {
+            f.lane_frame[l] = fresh;
+            if (fresh >= 0) f.lane_start[l] = round;
+            else S.sc[l].phase = PH_DONE;                 // an empty lane stays out of the active list
+        }
+        s_old[tid] = old;
+        s_new[tid] = fresh;
+        s_warm[tid] = warm ? 1 : 0;
+        __syncthreads();
+        if (tid == 0 && !flush) {
+            int tot = qbase;
+            for (int w = 0; w < 32; ++w) tot += wsum[w];
+            qbase = tot < q.n_act ? tot : q.n_act;
+        }
+        // parameters out and in, the new frame's detections into the lane's rows: one warp per lane
+        for (int j = wid; j < 1024 && l0 + j < f.B; j += 32) {
+            const int ln = l0 + j, fo = s_old[j], fn = s_new[j];
+            const bool wm = s_warm[j] != 0;
+            float* xl = f.lane_params + (size_t)ln * kParams;
+            if (fo >= 0) {
+                VLOOP(i) f.params[(size_t)fo * kParams + i] = xl[i];
+            }
+            if (fn < 0) continue;
+            VLOOP(i) {
+                if (!wm || (q.keep_pose && i >= kOffPose && i < kOffTransl)) xl[i] = f.params[(size_t)fn * kParams + i];
+            }
+            const int K = f.K;
+            for (int v = 0; v < f.V; ++v) {
+                const size_t dst = (size_t)v * f.B + ln, src = (size_t)v * f.F + fn;
+                for (int k = lane; k < 2 * K; k += 32) f.ws_gt_uv[dst * 2 * K + k] = f.gt_uv[src * 2 * K + k];
+                for (int k = lane; k < K; k += 32) f.ws_conf[dst * K + k] = f.conf[src * K + k];
+            }
+            __syncwarp();
+            init_frame_state(S, xl, ln, 1, f.nstages, nullptr, lane);
+            if (lane == 0) {
+                const int2 r = wm ? q.warm : q.cold;            // the frame's slice of the run's stage table
+                S.sc[ln].stage = r.x;
+                S.sc[ln].stage_end = r.y;
+                f.pose_valid[ln] = 0;                           // the lane's pose cache belongs to its previous frame
+            }
+        }
+        __syncthreads();
+    }
+    if (tid == 0) *f.queue = qbase;
+}
+
+// rows idx[0 .. n) of full [V][n_full][L] <-> packed [V][n][L]; to_full = 0 gathers, 1 scatters
+__global__ void copy_rows_kernel(float* __restrict__ packed, float* __restrict__ full, const int* __restrict__ idx, int n, int n_full,
+                                 int L, int to_full) {
+    const int i = blockIdx.x, v = blockIdx.y;
+    float* p = packed + ((size_t)v * n + i) * L;
+    float* g = full + ((size_t)v * n_full + idx[i]) * L;
+    for (int k = threadIdx.x; k < L; k += blockDim.x) {
+        if (to_full) g[k] = p[k];
+        else p[k] = g[k];
+    }
+}
+
 static int ensure_state(mvs_ctx* ctx, int H) {
     LbfgsState* S = ctx->lbfgs;
     const int B = ctx->ws.B;
@@ -351,14 +469,15 @@ static int dense_round(mvs_ctx* ctx, float* params_dev, const LbfgsState& S, con
 
 // Dense regime (SDF term on): rounds of dense_round until no frame is active.  Finished frames are compacted out once per
 // chunk of rounds.  fs (mvs_fit_stream): the finished frames' lanes are refilled from the stream's queue just before each
-// compaction.
+// compaction.  sq (mvs_fit_seq_stream, fs = &sq->f): the same with seq_refill_kernel, the queue holds sequences.
 static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int nst, cudaStream_t st,
-                     const StreamArgs* fs = nullptr) {
+                     const StreamArgs* fs = nullptr, const SeqArgs* sq = nullptr) {
     LbfgsState& S = *ctx->lbfgs;
     Workspace& w = ctx->ws;
     const int B = w.B;
     const int chunk = 8;
-    const long long frames_per_lane = fs ? (fs->F + B - 1) / B + 1 : 1;
+    // (a lane of a sequence stream may carry every frame of the call)
+    const long long frames_per_lane = sq ? fs->F + 1 : fs ? (fs->F + B - 1) / B + 1 : 1;
     const long long max_rounds = ((long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8) * nst * frames_per_lane;
     long long rounds = 0;
     int na_host = B;
@@ -388,7 +507,8 @@ static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int n
             if ((rc = dense_round(ctx, params_dev, S, cfg, nst, st))) return rc;
             ++rounds;
         }
-        if (fs) MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, stream_refill_kernel<<<1, 1024, 0, st>>>(S, *fs, rounds, 0));
+        if (sq) MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, seq_refill_kernel<<<1, 1024, 0, st>>>(S, *sq, rounds, 0));
+        else if (fs) MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, stream_refill_kernel<<<1, 1024, 0, st>>>(S, *fs, rounds, 0));
         // compaction changes slot -> frame, so the surviving frames' Phi / transforms are rebuilt for their new slots
         MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
         if ((rc = launch_frame_fwd_dense(ctx, S.x_eval, S, nst, st))) return rc;
@@ -401,7 +521,7 @@ static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int n
             MVS_CUDA_OK(ctx, cudaEventSynchronize(S.na_event[pending]));
             if (trace_host) blocked_us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - tb0).count();
             na_host = na_slots[pending];
-            if (!drained) drained = queue_slots[pending] >= fs->F;
+            if (!drained) drained = queue_slots[pending] >= (sq ? sq->q.n_act : fs->F);
             if (trace_na) fprintf(stderr, "[mvs] dense regime: chunk %lld, active frames %d\n", chunk_idx - 1, na_host);
             if (na_host <= 0) break;                              // (a refill leaves no lane idle while frames are queued)
             // Without refills the list only shrinks, so the count is an upper bound for every later round.  Refills add
@@ -781,6 +901,215 @@ static int run_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, con
     return rc;
 }
 
+// mvs_fit_seq_stream scratch, grow-only in the number of sequences
+struct SeqState {
+    int cap = 0;                        // sequences
+    int *off = nullptr, *cur = nullptr, *act = nullptr, *frames = nullptr;   // [cap+1], [cap], [cap], [cap]
+    int* lane_seq = nullptr;            // [B]
+    size_t packed_cap = 0;
+    float* packed = nullptr;            // the pending cold frames' rows for the runs before the chaining run
+};
+
+static int ensure_seq_state(mvs_ctx* ctx, int nseq, size_t packed_floats) {
+    int rc;
+    if (!ctx->sstream) {
+        ctx->sstream = new SeqState();
+        if ((rc = dev_alloc(ctx, &ctx->sstream->lane_seq, (size_t)ctx->ws.B))) return rc;
+    }
+    SeqState& q = *ctx->sstream;
+    if (q.cap < nseq) {
+        for (int* p : {q.off, q.cur, q.act, q.frames})
+            if (p) dev_free(ctx, p);
+        q.cap = 0;
+        if ((rc = dev_alloc(ctx, &q.off, (size_t)nseq + 1))) return rc;
+        if ((rc = dev_alloc(ctx, &q.cur, (size_t)nseq))) return rc;
+        if ((rc = dev_alloc(ctx, &q.act, (size_t)nseq))) return rc;
+        if ((rc = dev_alloc(ctx, &q.frames, (size_t)nseq))) return rc;
+        q.cap = nseq;
+    }
+    if (q.packed_cap < packed_floats) {
+        if (q.packed) dev_free(ctx, q.packed);
+        q.packed = nullptr;
+        q.packed_cap = 0;
+        if ((rc = dev_alloc(ctx, &q.packed, packed_floats))) return rc;
+        q.packed_cap = packed_floats;
+    }
+    return MVS_OK;
+}
+
+// The chaining run over the sequences of one pass (q.act): every frame of run `tab` from its sequence's pending frame on
+static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, int F, Regime rg, const std::vector<LossParams>& tab,
+                         const SeqChain& q0, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats, cudaStream_t st) {
+    const int nst = (int)tab.size();
+    LbfgsCfg cfg;
+    int rc = begin_run(ctx, c, false, tab.data(), nst, &cfg, st);
+    if (rc) return rc;
+    LbfgsState& S = *ctx->lbfgs;
+    Workspace& w = ctx->ws;
+    const int B = w.B, K = ctx->m.K;
+    long long* th = reinterpret_cast<long long*>(S.na_host) + 1;      // [0..3] totals, [4] rounds of a dense run
+    SeqChain q = q0;
+    q.final_loss = s->final_loss;
+    q.totals = S.totals;
+    if (rg == kResident) {
+        // one launch, one CTA per sequence; rounds: the largest number of evaluations one CTA ran (its frames' sum)
+        const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, nullptr, nullptr};
+        if ((rc = launch_lbfgs_resident_seq(ctx, s->params, cfg, cfg.history, S.lp_tab, tab.data(), nst, in, q, st))) return rc;
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+        MVS_CUDA_OK(ctx, cudaGetLastError());
+        if (stats) {
+            stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
+            stats->rounds += (int)th[3];
+        }
+        return MVS_OK;
+    }
+    // dense rounds over B lanes fed from the queue of sequences
+    StreamState& ss = *ctx->fstream;
+    if ((rc = frame_step_begin_run(ctx, st))) return rc;
+    SeqArgs a;
+    StreamArgs& f = a.f;
+    f.F = F; f.B = B; f.V = ctx->cams.num_views; f.K = K; f.nstages = nst;
+    f.params = s->params; f.final_loss = s->final_loss; f.gt_uv = s->gt_uv; f.conf = s->conf;
+    f.j3d_xyz = nullptr; f.j3d_conf = nullptr;
+    f.ws_gt_uv = w.gt_uv; f.ws_conf = w.conf; f.ws_j3d_xyz = nullptr; f.ws_j3d_conf = nullptr;
+    f.lane_frame = ss.lane_frame; f.lane_start = ss.lane_start; f.lane_params = ss.lane_params; f.queue = ss.queue;
+    f.end_round = ss.end_round; f.pose_valid = w.pose_valid;
+    a.q = q;
+    a.lane_seq = ctx->sstream->lane_seq;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(w.joint_w, s->joint_weights, (size_t)K * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.lane_frame, 0xff, (size_t)B * sizeof(int), st));
+    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.queue, 0, sizeof(int), st));
+    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.end_round, 0, sizeof(long long), st));
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
+    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, seq_refill_kernel<<<1, 1024, 0, st>>>(S, a, 0, 0));
+    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
+    if ((rc = run_dense(ctx, ss.lane_params, cfg, nst, st, &a.f, &a))) return rc;
+    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, seq_refill_kernel<<<1, 1024, 0, st>>>(S, a, 0, 1));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 3 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th + 4, ss.end_round, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    if (stats) {
+        stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
+        stats->rounds += (int)th[4];
+        stats->dense_frame_evals += th[1]; stats->dense_rounds += (int)th[4];
+    }
+    return MVS_OK;
+}
+
+// mvs_fit_seq_stream (DESIGN.md section 4).  Stages are grouped into runs as mvs_fit_seq groups them; run c holds stages
+// 2 .. n-1 and is the chaining run.  Each pass takes the pending cold frames P (at first: every sequence's first frame) through
+// the runs before c (as a frame stream of P's rows), then runs c over their sequences; a sequence whose next frame turns
+// out cold parks it for the next pass (c > 0 only: with c == 0 the cold frame stays in its slot with the cold slice).
+static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
+                          const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, cudaStream_t st) {
+    constexpr int kWarmSkip = 2;                                      // as run_fit
+    if (n_stages > 64) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: at most 64 stages");
+    const int NS = s->n_sequences;
+    const std::vector<int> off(s->seq_offsets, s->seq_offsets + NS + 1);
+    const int F = off[NS];
+    std::vector<LossParams> lps(n_stages), wlps;
+    int n_vp2 = 0;
+    for (int i = 0; i < n_stages; ++i) {
+        const int rc = make_loss_params(ctx, &stage_cfgs[i], &lps[i]);
+        if (rc) return rc;
+        lps[i].j3d_on = 0;
+        n_vp2 += lps[i].use_vposer == 2;
+    }
+    if (n_vp2 > 0 && n_vp2 < n_stages)
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: stages mix latent-code (use_vposer = 2) and axis-angle poses");
+    wlps = lps;
+    {
+        mvs_loss_config wc = stage_cfgs[kWarmSkip];
+        wc.body_pose_weight *= 0.15f;
+        const int rc = make_loss_params(ctx, &wc, &wlps[kWarmSkip]);
+        if (rc) return rc;
+        wlps[kWarmSkip].j3d_on = 0;
+    }
+    const int H = opt_cfg->history_size > 0 ? opt_cfg->history_size : 100;
+    std::vector<int> ends;
+    int c = -1, ic = 0;
+    bool any_dense = false, resident_before = false;
+    for (int i = 0; i < n_stages; i = ends.back()) {
+        const Regime rg = stage_regime(ctx, lps[i], H, false);
+        if (rg == kBatched)
+            return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_seq_stream: stage %d would run in the batched reference chain (exec "
+                                                       "mode 1, history_size > 100 without the SDF term, or a model the "
+                                                       "frame-resident and dense kernels do not take), which has no stream", i);
+        ends.push_back(stage_group_end(ctx, lps, i, H, kMaxStages / 2));
+        any_dense |= rg == kDense;
+        if (i <= kWarmSkip && kWarmSkip < ends.back()) { c = (int)ends.size() - 1; ic = i; }
+        else if (c < 0) resident_before |= rg == kResident;
+    }
+    if (ends[c] != n_stages)
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_seq_stream: stages %d .. %d do not form one run (the run holding stage "
+                                                   "%d ends at %d; exec mode 2, or a change of regime, SDF grid or face mode)",
+                         kWarmSkip, n_stages - 1, kWarmSkip, ends[c]);
+    // the chaining run's table: cold stages ic .. n-1, then the warm slice 2 .. n-1
+    std::vector<LossParams> tab(lps.begin() + ic, lps.end());
+    const int wbegin = (int)tab.size();
+    for (int k = kWarmSkip; k < n_stages; ++k) tab.push_back(wlps[k]);
+    SeqChain q;
+    q.cold = make_int2(0, wbegin);
+    q.warm = make_int2(wbegin, (int)tab.size());
+    q.reinit_loss = s->reinit_loss;
+    q.park = c > 0 ? 1 : 0;
+    q.keep_pose = n_vp2 == 0 ? 1 : 0;
+    const size_t row_floats = kParams + (size_t)ctx->cams.num_views * ctx->m.K * 3;   // params | gt_uv | conf of a frame
+    int rc = ensure_stream_state(ctx, resident_before ? NS : 0);
+    if (!rc) rc = ensure_seq_state(ctx, NS, c > 0 ? row_floats * NS : 0);
+    if (!rc && any_dense) rc = ensure_keypoint_ws(ctx);
+    if (rc) return rc;
+    SeqState& ss = *ctx->sstream;
+    q.off = ss.off;
+    q.cur = ss.cur;
+    q.act = ss.act;
+    // the dense runs overwrite the slots' keypoint rows: from here on the context holds none (and no 3-D targets)
+    ctx->have_kp = false;
+    ctx->j3d_enabled = false;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.off, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    std::vector<int> cur(off.begin(), off.end() - 1), act, frames;   // each sequence's pending cold frame, -1: done
+    const int V = ctx->cams.num_views, K = ctx->m.K;
+    while (!rc) {
+        act.clear();
+        frames.clear();
+        for (int k = 0; k < NS; ++k)
+            if (cur[k] >= 0) { act.push_back(k); frames.push_back(cur[k]); }
+        if (act.empty()) break;
+        const int n = (int)act.size();
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.cur, cur.data(), (size_t)NS * sizeof(int), cudaMemcpyHostToDevice, st));
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.act, act.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+        if (c > 0) {
+            // the pending frames through the runs before c, as a frame stream of their packed rows
+            MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.frames, frames.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+            float* px = ss.packed;
+            float* pg = px + (size_t)n * kParams;
+            float* pc = pg + (size_t)V * n * K * 2;
+            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, ss.frames, n, F, kParams, 0));
+            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pg, const_cast<float*>(s->gt_uv), ss.frames, n, F, 2 * K, 0));
+            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pc, const_cast<float*>(s->conf), ss.frames, n, F, K, 0));
+            const mvs_frame_stream fs{n, px, pg, pc, s->joint_weights, nullptr, nullptr, nullptr};
+            for (int i = 0, g = 0; g < c && !rc; i = ends[g++]) {
+                ctx->loss = lps[i];
+                ctx->have_loss = true;
+                rc = run_stream_group(ctx, &fs, stage_regime(ctx, lps[i], H, false), &lps[i], ends[g] - i, opt_cfg, stats, st);
+            }
+            if (rc) break;
+            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, ss.frames, n, F, kParams, 1));
+        }
+        q.n_act = n;
+        ctx->loss = lps[ic];
+        ctx->have_loss = true;
+        if ((rc = run_seq_chain(ctx, s, F, stage_regime(ctx, lps[ic], H, false), tab, q, opt_cfg, stats, st))) break;
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(cur.data(), ss.cur, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
+        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    }
+    ctx->loss = lps[n_stages - 1];
+    return rc;
+}
+
 }  // namespace mvs
 
 using namespace mvs;
@@ -852,6 +1181,31 @@ int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const 
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     if (stats) memset(stats, 0, sizeof(*stats));
     return run_stream(ctx, s, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
+}
+
+int mvs_fit_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
+                       const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0))
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: model, cameras and batch must be set first");
+    if (!s || !stage_cfgs || !opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: NULL argument");
+    if (n_stages <= 2)
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: warm-started frames skip the first 2 stages, %d given", n_stages);
+    if (s->n_sequences < 1 || !s->seq_offsets)
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: n_sequences must be >= 1 (got %d) with seq_offsets", s->n_sequences);
+    if (!s->params || !s->gt_uv || !s->conf || !s->joint_weights)
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: params, gt_uv, conf and joint_weights are required");
+    if (s->seq_offsets[0] != 0) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: seq_offsets[0] must be 0");
+    for (int k = 0; k < s->n_sequences; ++k)
+        if (s->seq_offsets[k + 1] <= s->seq_offsets[k])
+            return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: seq_offsets must ascend strictly (sequence %d is empty "
+                                                   "or negative)", k);
+    if (ctx->anchor_enabled)
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_seq_stream: the anchor term is per batch (sequence smoothness); switch "
+                                                   "it off (mvs_set_anchor enable = 0) to fit a sequence stream");
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    if (stats) memset(stats, 0, sizeof(*stats));
+    return run_seq_stream(ctx, s, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
 }
 
 int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, const float* conf_host,

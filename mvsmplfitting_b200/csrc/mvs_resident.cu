@@ -172,6 +172,98 @@ lbfgs_resident_kernel(ResidentModel m, CamSet cams, const LossParams* __restrict
     if (t == 0) sc_out[b] = S.fs;
 }
 
+// The chaining run of mvs_fit_seq_stream: ONE CTA owns ONE sequence (q.act[blockIdx.x]) and runs lbfgs_resident_kernel's
+// per-frame optimisation for each of its frames in turn, from its pending frame q.cur[seq] (cold) on.  After a frame it
+// writes the frame's parameters, final loss and counts, then starts the successor with a fresh optimiser: warm from the
+// fitted row in shared memory, cold from the successor's own row -- or, with q.park, leaves a cold successor to the next
+// pass.  B = F: the inputs' row stride.  Kept apart from lbfgs_resident_kernel so that kernel's code stays as it is.
+__global__ void __launch_bounds__(kResThreads, 2)
+lbfgs_resident_seq_kernel(ResidentModel m, CamSet cams, const LossParams* __restrict__ lp_tab, LbfgsCfg cfg,
+                          float* __restrict__ params, const float* __restrict__ gt_uv, const float* __restrict__ conf,
+                          const float* __restrict__ joint_w, int B, int H, int with_vposer, SeqChain q) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    ResidentSmem& S = *reinterpret_cast<ResidentSmem*>(smem_raw);
+    float* hy = reinterpret_cast<float*>(smem_raw + sizeof(ResidentSmem));
+    float* hs = hy + (size_t)H * kParams;
+    VposerSmem* W = with_vposer ? reinterpret_cast<VposerSmem*>(hs + (size_t)H * kParams) : nullptr;
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    if ((int)blockIdx.x >= q.n_act) return;
+    const int seq = q.act[blockIdx.x], seq_end = q.off[seq + 1];
+    int b = q.cur[seq];
+    int2 rng = q.cold;
+    long long seq_evals = 0;                                             // evaluations of this CTA's frames so far
+    resident_setup(S, m);
+    for (int i = t; i < kParams; i += kResThreads) { const float v = params[(size_t)b * kParams + i]; S.lx[i] = v; S.lx_eval[i] = v; }
+    LbfgsPtrs P{S.lx, S.lg, S.ld, S.lprev_g, S.lx_init, S.lg_prev, S.lbg0, S.lbg1, hy, hs, S.ro, S.al, S.lx_eval, S.lg_new, H,
+                S.gram, S.tl_scratch};
+    const long long eval_cap = (long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8;
+    while (true) {                                                       // frames of the sequence
+        if (t == 0) {
+            FrameScalars s;
+            memset(&s, 0, sizeof(s));
+            s.phase = PH_STEP_ENTRY;
+            s.H_diag = 1.f;
+            s.final_loss = __int_as_float(0x7fc00000);
+            s.stage = rng.x; s.stage_end = rng.y;
+            S.fs = s;
+        }
+        if (t < (int)(sizeof(LossParams) / 4)) reinterpret_cast<int*>(&S.lp)[t] = reinterpret_cast<const int*>(&lp_tab[rng.x])[t];
+        __syncthreads();
+        long long stage_ev0 = 0;
+        int cur_stage = rng.x;
+        while (true) {                                                   // as lbfgs_resident_kernel
+            for (int i = t; i < kParams; i += kResThreads) S.x[i] = S.lx_eval[i];
+            __syncthreads();
+            resident_closure(S, m, cams, S.lp, gt_uv, conf, joint_w, B, b, true, nullptr, nullptr, DenseIn{}, W);
+            if (warp == 0) {
+                FrameScalars s = S.fs;
+                lbfgs_advance_core(s, P, S.sc[2], cfg, lane, S.lp.use_vposer == 2 ? 32 : kOffTransl - kOffPose);
+                if (s.evals - stage_ev0 >= eval_cap && s.phase != PH_DONE) { s.phase = PH_DONE; s.nan_flag = 1; }
+                if (s.phase == PH_DONE && s.stage + 1 < s.stage_end) {
+                    next_stage_scalars(s);
+                    VLOOP(i) S.lx_eval[i] = S.lx[i];
+                }
+                if (lane == 0) S.fs = s;
+            }
+            __syncthreads();
+            if (S.fs.phase == PH_DONE) break;
+            if (S.fs.stage != cur_stage) {
+                cur_stage = S.fs.stage;
+                stage_ev0 = S.fs.evals;
+                if (t < (int)(sizeof(LossParams) / 4))
+                    reinterpret_cast<int*>(&S.lp)[t] = reinterpret_cast<const int*>(&lp_tab[cur_stage])[t];
+                __syncthreads();
+            }
+        }
+        for (int i = t; i < kParams; i += kResThreads) params[(size_t)b * kParams + i] = S.lx[i];
+        const FrameScalars& s = S.fs;
+        seq_evals += s.evals;
+        if (t == 0) {                                                    // the frame's totals, as lbfgs_finalize_kernel counts them
+            if (q.final_loss) q.final_loss[b] = s.final_loss;
+            atomicAdd((unsigned long long*)&q.totals[0], (unsigned long long)s.iters);
+            atomicAdd((unsigned long long*)&q.totals[1], (unsigned long long)s.evals);
+            atomicAdd((unsigned long long*)&q.totals[2], (unsigned long long)(s.nan_flag + s.nan_acc));
+        }
+        const int nx = b + 1;
+        const bool more = nx < seq_end, warm = more && s.final_loss <= q.reinit_loss;   // NaN is not <= reinit_loss
+        if (!more || (!warm && q.park)) {                                // sequence done, or parked for the earlier runs
+            if (t == 0) {
+                q.cur[seq] = more ? nx : -1;
+                atomicMax((unsigned long long*)&q.totals[3], (unsigned long long)seq_evals);
+            }
+            break;
+        }
+        for (int i = t; i < kParams; i += kResThreads) {                 // the successor's start point
+            const bool own = !warm || (q.keep_pose && i >= kOffPose && i < kOffTransl);
+            const float v = own ? params[(size_t)nx * kParams + i] : S.lx[i];
+            S.lx[i] = v; S.lx_eval[i] = v;
+        }
+        rng = warm ? q.warm : q.cold;
+        b = nx;
+        __syncthreads();                                                 // every thread has read S.fs before it is reset
+    }
+}
+
 // The same for every active slot at the start of a run and after a compaction (slots changed): the VPoser-capable
 // counterpart of frame_fwd_kernel (mvs_closure.cu), which only knows axis-angle poses.
 __global__ void __launch_bounds__(kResThreads, 2)
@@ -214,6 +306,8 @@ int resident_set_attributes(mvs_ctx* ctx) {
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vposer_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, one_frame));
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(frame_fwd_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, one_frame));
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(lbfgs_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)frame_smem(100, true)));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(lbfgs_resident_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           (int)frame_smem(100, true)));
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(frame_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           (int)frame_smem(128, true)));
@@ -273,6 +367,19 @@ int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, 
                lbfgs_resident_kernel<<<in.n, kResThreads, smem, st>>>(rm, ctx->cams, lp_tab_dev, nstages, cfg, params_dev,
                                                                       in.gt_uv, in.conf, in.joint_w, in.n, H, sc_out,
                                                                       last_grad_dev, with_vposer, stage_rng_dev));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    return MVS_OK;
+}
+
+int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int H, const LossParams* lp_tab_dev,
+                              const LossParams* lph, int nstages, const FrameInputs& in, const SeqChain& q, cudaStream_t st) {
+    int with_vposer = 0;
+    for (int i = 0; i < nstages; ++i) with_vposer |= (lph[i].use_vposer == 2);
+    const size_t smem = frame_smem(H, with_vposer != 0);
+    MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
+               lbfgs_resident_seq_kernel<<<q.n_act, kResThreads, smem, st>>>(make_resident_model(ctx), ctx->cams, lp_tab_dev, cfg,
+                                                                             params_dev, in.gt_uv, in.conf, in.joint_w, in.n, H,
+                                                                             with_vposer, q));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }

@@ -234,29 +234,42 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
         if result_folder is not None:
             _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces)
         return params.cpu().numpy(), loss, stats
-    B = ctx.B
-    params = torch.empty(F, 86, dtype=torch.float32, device=ctx.device)
-    for c0 in range(0, F, B):                        # initial guesses per chunk of B frames; the last chunk is padded with
-        n = min(B, F - c0)                           # zero-confidence rows, which are dropped
-        gt = np.zeros((seq["gt_uv"].shape[0], B) + seq["gt_uv"].shape[2:], np.float32)
-        cf = np.zeros((seq["conf"].shape[0], B) + seq["conf"].shape[2:], np.float32)
-        gt[:, :n], cf[:, :n] = seq["gt_uv"][:, c0:c0 + n], seq["conf"][:, c0:c0 + n]
-        ctx.set_keypoints(gt, cf, jw)
-        ctx.set_loss(config=stage_cfgs[0])
-        x, _ = ctx.init_guess(**guess)
-        params[c0:c0 + n] = x[:n]
+    params = _cold_guesses(ctx, seq["gt_uv"], seq["conf"], jw, stage_cfgs, guess)
     final, stats = ctx.fit_stream(params, seq["gt_uv"], seq["conf"], jw, stage_cfgs, opt_cfg)
     loss = final.cpu().numpy()
-    if result_folder is not None:                    # the export takes whole batches: chunks of B rows, the last one padded
-        for c0 in range(0, F, B):
-            n = min(B, F - c0)
-            chunk = torch.zeros(B, 86, dtype=torch.float32, device=ctx.device)
-            chunk[:n] = params[c0:c0 + n]
-            lc = np.zeros(B, np.float32)
-            lc[:n] = loss[c0:c0 + n]
-            _export(ctx, seq, chunk, lc, latent, result_folder, mesh_folder, faces, frames=seq["frames"][c0:c0 + n],
-                    rows=range(n))
+    if result_folder is not None:
+        _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces)
     return params.cpu().numpy(), loss, stats
+
+
+def _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess: dict) -> torch.Tensor:
+    """initial guesses (init_guess + fix_params) of F frames of any number, ctx.B frames at a time: params [F,86] on the
+    device.  The last chunk is padded with zero-confidence rows, which are dropped."""
+    F, B = gt_uv.shape[1], ctx.B
+    params = torch.empty(F, 86, dtype=torch.float32, device=ctx.device)
+    for c0 in range(0, F, B):
+        n = min(B, F - c0)
+        gt = np.zeros((gt_uv.shape[0], B) + gt_uv.shape[2:], np.float32)
+        cf = np.zeros((conf.shape[0], B) + conf.shape[2:], np.float32)
+        gt[:, :n], cf[:, :n] = gt_uv[:, c0:c0 + n], conf[:, c0:c0 + n]
+        ctx.set_keypoints(gt, cf, jw)
+        ctx.set_loss(config=stage_cfgs[0])           # mvs_init_guess zeroes the pose slot when it holds a latent code
+        x, _ = ctx.init_guess(**guess)
+        params[c0:c0 + n] = x[:n]
+    return params
+
+
+def _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces):
+    """_export of one sequence's F rows (params [F,86] on the device, loss [F]) in chunks of ctx.B rows, as the export takes
+    whole batches; the last chunk is padded"""
+    F, B = params.shape[0], ctx.B
+    for c0 in range(0, F, B):
+        n = min(B, F - c0)
+        chunk = torch.zeros(B, 86, dtype=torch.float32, device=ctx.device)
+        chunk[:n] = params[c0:c0 + n]
+        lc = np.zeros(B, np.float32)
+        lc[:n] = loss[c0:c0 + n]
+        _export(ctx, seq, chunk, lc, latent, result_folder, mesh_folder, faces, frames=seq["frames"][c0:c0 + n], rows=range(n))
 
 
 def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = False, fixed_scale: float = 1.0,
@@ -268,12 +281,19 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
     global_orient, transl, scale kept; body pose back to the hip seed, or the previous latent code under VPoser), skips
     stages 0 and 1 and damps stage 2's pose prior (non_linear_solver.py:157-162, `mvs_fit_seq`) -- unless the previous loss
     was above 5000, which re-runs the initial guess for that sequence (:141-144).  Sequences may differ in length.
+    A context batch other than S works as a pool of slots: the initial guesses of all frames are computed ctx.B frames at a
+    time, then all sequences go through ONE `mvs_fit_seq_stream` call, in which a slot takes the next frame of its sequence
+    as soon as a frame is done (the same results bit for bit; stats then also carry the dense-round counts).
     Returns a list (per sequence) of (params [T_s,86], loss [T_s]) and the summed stats."""
     S_ = len(seqs)
-    assert ctx.B == S_, "context batch %d != sequences %d" % (ctx.B, S_)
     latent = _uses_latent_pose(stage_cfgs)
     for q in seqs:
         _check_missing_views(q, stage_cfgs)
+    if ctx.B != S_:
+        return _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces,
+                                     pose_format, use_hip, dict(estimate_scale=estimate_scale, fixed_scale=fixed_scale,
+                                                                use_torso=True, hip_seed=1.0, want_joints3d=False,
+                                                                umeyama_as_written=umeyama_as_written))
     T = max(len(q["frames"]) for q in seqs)
     V = seqs[0]["gt_uv"].shape[0]
     jw = joint_weights(pose_format, use_hip)
@@ -316,3 +336,21 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
                 if live[s_]:
                     _export(ctx, q, params, prev_loss, latent, result_folder, mesh_folder, faces, frames=[q["frames"][t]], rows=[s_])
     return list(zip(out_x, out_l)), tot
+
+
+def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces, pose_format,
+                          use_hip, guess):
+    """fit_sequences through mvs_fit_seq_stream: the sequences' frames back to back, every frame's cold start point from
+    _cold_guesses"""
+    lengths = [len(q["frames"]) for q in seqs]
+    off = np.concatenate([[0], np.cumsum(lengths)])
+    gt_uv = np.concatenate([q["gt_uv"] for q in seqs], axis=1)
+    conf = np.concatenate([q["conf"] for q in seqs], axis=1)
+    jw = joint_weights(pose_format, use_hip)
+    params = _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess)
+    final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss)
+    x, loss = params.cpu().numpy(), final.cpu().numpy()
+    if result_folder is not None:
+        for s_, q in enumerate(seqs):
+            _export_rows(ctx, q, params[off[s_]:off[s_ + 1]], loss[off[s_]:off[s_ + 1]], latent, result_folder, mesh_folder, faces)
+    return [(x[off[s_]:off[s_ + 1]], loss[off[s_]:off[s_ + 1]]) for s_ in range(len(seqs))], stats
