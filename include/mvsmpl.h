@@ -265,7 +265,8 @@ int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const 
  *      MVS_ERR_INVALID: NULL or empty arguments, n_stages <= 2, seq_offsets not starting at 0 or not strictly ascending,
  *      stages that mix use_vposer 2 with axis-angle poses.
  *      Context state afterwards as after mvs_fit_stream: no keypoints, 3-D term off, the last stage's loss configuration set.
- *      The 3-D joint term is not part of the call.  Synchronises. */
+ *      The call never reads the context's own keypoints or 3-D targets; mvs_fit_seq_stream3d adds the 3-D joint term.
+ *      Synchronises. */
 typedef struct {
     int n_sequences;               /* S >= 1 */
     const int* seq_offsets;        /* HOST [S+1]: 0 = off[0] < off[1] < ... < off[S] = F (no empty sequence) */
@@ -278,6 +279,17 @@ typedef struct {
 } mvs_sequence_stream;
 int mvs_fit_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
                        const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream);
+
+/* ---- mvs_fit_seq_stream with the 3-D joint term (SMPLifyLoss use_3d, code/utils/fitting.py:318-324): gt_xyz [F,K,3] and
+ *      conf3d [F,K] (device pointers) are every frame's 3-D targets and confidences, rows in the order of the frames of s.
+ *      The term is on in every stage of every frame, cold and warm; a frame without annotations takes zero rows (confidence 0
+ *      gives, bit for bit, the result with the term off).  The bit-for-bit contract includes the term: every frame gets the
+ *      parameters and final loss that mvs_fit_seq gives it in a batch of S after mvs_set_joints3d with frame t's rows of the
+ *      S sequences.  Both pointers NULL: mvs_fit_seq_stream (which is this call with two NULLs).  Exactly one NULL:
+ *      MVS_ERR_INVALID.  Refusals and context state afterwards as mvs_fit_seq_stream.  Synchronises. */
+int mvs_fit_seq_stream3d(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int n_stages,
+                         const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
+                         void* stream);
 
 /* ---- host-buffer entry point (what a caller without device memory uses): copies keypoints and
  *      parameters host->device, runs `n_stages` optimisation stages (one mvs_loss_config each, the weight

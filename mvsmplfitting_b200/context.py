@@ -299,13 +299,15 @@ class FittingContext:
         return final, _stats_dict(st)
 
     def fit_seq_stream(self, params: torch.Tensor, gt_uv, conf, joint_weights, lengths, stage_cfgs, opt_cfg=None,
-                       reinit_loss: float = 5000.0):
+                       reinit_loss: float = 5000.0, joints3d=None, conf3d=None):
         """mvs_fit_seq over S video sequences through the context's B slots (mvs_fit_seq_stream): the frames of sequence s are
         the next lengths[s] rows, in time order.  params [F,86] CUDA float32 holds every frame's cold start point (init_guess)
         and is updated in place; gt_uv [V,F,K,2], conf [V,F,K], joint_weights [K] (numpy or tensors).  A frame after the first
         starts from its predecessor's result while that frame's final loss is <= reinit_loss (skipping stages 0 and 1), from
-        its own row otherwise.  Every frame gets the bits seqio.fit_sequences gives it with a batch of S.  Afterwards the
-        context holds no keypoints.  Returns (final_loss [F], stats)."""
+        its own row otherwise.  joints3d [F,K,3] with conf3d [F,K] switch the 3-D joint term on for every frame of the call
+        (mvs_fit_seq_stream3d; zero-confidence rows for frames without annotations).  Every frame gets the bits
+        seqio.fit_sequences gives it with a batch of S.  Afterwards the context holds no keypoints and no 3-D targets.
+        Returns (final_loss [F], stats)."""
         assert params.is_cuda and params.dtype == torch.float32 and params.is_contiguous() and params.dim() == 2
         F = params.shape[0]
         lengths = [int(n) for n in lengths]
@@ -316,6 +318,13 @@ class FittingContext:
         gt_uv, conf, jw = dev(gt_uv), dev(conf), dev(joint_weights).reshape(-1)
         assert tuple(gt_uv.shape) == (self.V, F, self.K, 2) and tuple(conf.shape) == (self.V, F, self.K), \
             (tuple(gt_uv.shape), tuple(conf.shape), (self.V, F, self.K))
+        if (joints3d is None) != (conf3d is None):
+            raise ValueError("fit_seq_stream: joints3d and conf3d go together")
+        j3 = None if joints3d is None else torch.as_tensor(joints3d).to(self.device, torch.float32).contiguous()
+        c3 = None if conf3d is None else torch.as_tensor(conf3d).to(self.device, torch.float32).contiguous()
+        if j3 is not None and (tuple(j3.shape) != (F, self.K, 3) or tuple(c3.shape) != (F, self.K)):
+            raise ValueError("fit_seq_stream: want joints3d [%d,%d,3] and conf3d [%d,%d], got %s and %s"
+                             % (F, self.K, F, self.K, tuple(j3.shape), tuple(c3.shape)))
         final = torch.empty(F, dtype=torch.float32, device=self.device)
         s = _lib.SequenceStream(len(lengths), _ptr(off), _ptr(params), _ptr(gt_uv), _ptr(conf), _ptr(jw), _ptr(final),
                                 float(reinit_loss))
@@ -323,8 +332,13 @@ class FittingContext:
         cfg = opt_cfg or self.make_lbfgs_config()
         st = _lib.LbfgsStats()
         self._j3d_keep = None
-        _lib.check(self.h, self.lib.mvs_fit_seq_stream(self.h, ctypes.byref(s), len(stage_cfgs), arr, ctypes.byref(cfg),
-                                                       ctypes.byref(st), self._stream()), "mvs_fit_seq_stream")
+        if j3 is None:
+            _lib.check(self.h, self.lib.mvs_fit_seq_stream(self.h, ctypes.byref(s), len(stage_cfgs), arr, ctypes.byref(cfg),
+                                                           ctypes.byref(st), self._stream()), "mvs_fit_seq_stream")
+        else:
+            _lib.check(self.h, self.lib.mvs_fit_seq_stream3d(self.h, ctypes.byref(s), _ptr(j3), _ptr(c3), len(stage_cfgs), arr,
+                                                             ctypes.byref(cfg), ctypes.byref(st), self._stream()),
+                       "mvs_fit_seq_stream3d")
         return final, _stats_dict(st)
 
     def fit_host(self, params_host: np.ndarray, gt_uv: np.ndarray, conf: np.ndarray, joint_weights: np.ndarray,

@@ -253,7 +253,8 @@ struct SeqArgs {
 
 // stream_refill_kernel for sequences, at the same points of the dense run.  A lane whose frame is done hands the frame back
 // and takes its successor in the same sequence: warm from the frame's fitted row (body-pose slot from the successor's own
-// row unless the stages carry a latent code), cold from the successor's row unless cold frames park.  A lane whose
+// row unless the stages carry a latent code), cold from the successor's row unless cold frames park.  Every frame that enters
+// a lane brings its detections and, with the 3-D term on, its 3-D targets into the lane's rows.  A lane whose
 // sequence ends or parks takes the next queued sequence's pending frame, in ascending lane order (ballot + prefix sum).
 // A lane that continues stays active and freed lanes only take from the queue, so the host's na_bound rule holds.
 __global__ void __launch_bounds__(1024) seq_refill_kernel(LbfgsState S, SeqArgs a, long long round, int flush) {
@@ -335,6 +336,10 @@ __global__ void __launch_bounds__(1024) seq_refill_kernel(LbfgsState S, SeqArgs 
                 const size_t dst = (size_t)v * f.B + ln, src = (size_t)v * f.F + fn;
                 for (int k = lane; k < 2 * K; k += 32) f.ws_gt_uv[dst * 2 * K + k] = f.gt_uv[src * 2 * K + k];
                 for (int k = lane; k < K; k += 32) f.ws_conf[dst * K + k] = f.conf[src * K + k];
+            }
+            if (f.j3d_xyz) {
+                for (int k = lane; k < 3 * K; k += 32) f.ws_j3d_xyz[(size_t)ln * 3 * K + k] = f.j3d_xyz[(size_t)fn * 3 * K + k];
+                for (int k = lane; k < K; k += 32) f.ws_j3d_conf[(size_t)ln * K + k] = f.j3d_conf[(size_t)fn * K + k];
             }
             __syncwarp();
             init_frame_state(S, xl, ln, 1, f.nstages, nullptr, lane);
@@ -938,8 +943,10 @@ static int ensure_seq_state(mvs_ctx* ctx, int nseq, size_t packed_floats) {
 }
 
 // The chaining run over the sequences of one pass (q.act): every frame of run `tab` from its sequence's pending frame on
-static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, int F, Regime rg, const std::vector<LossParams>& tab,
-                         const SeqChain& q0, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats, cudaStream_t st) {
+// (gt_xyz / conf3d [F][K][3] / [F][K]: the 3-D targets, both NULL when the term is off)
+static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int F, Regime rg,
+                         const std::vector<LossParams>& tab, const SeqChain& q0, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats,
+                         cudaStream_t st) {
     const int nst = (int)tab.size();
     LbfgsCfg cfg;
     int rc = begin_run(ctx, c, false, tab.data(), nst, &cfg, st);
@@ -953,7 +960,7 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, int F, Regi
     q.totals = S.totals;
     if (rg == kResident) {
         // one launch, one CTA per sequence; rounds: the largest number of evaluations one CTA ran (its frames' sum)
-        const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, nullptr, nullptr};
+        const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d};
         if ((rc = launch_lbfgs_resident_seq(ctx, s->params, cfg, cfg.history, S.lp_tab, tab.data(), nst, in, q, st))) return rc;
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
@@ -971,8 +978,8 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, int F, Regi
     StreamArgs& f = a.f;
     f.F = F; f.B = B; f.V = ctx->cams.num_views; f.K = K; f.nstages = nst;
     f.params = s->params; f.final_loss = s->final_loss; f.gt_uv = s->gt_uv; f.conf = s->conf;
-    f.j3d_xyz = nullptr; f.j3d_conf = nullptr;
-    f.ws_gt_uv = w.gt_uv; f.ws_conf = w.conf; f.ws_j3d_xyz = nullptr; f.ws_j3d_conf = nullptr;
+    f.j3d_xyz = gt_xyz; f.j3d_conf = conf3d;
+    f.ws_gt_uv = w.gt_uv; f.ws_conf = w.conf; f.ws_j3d_xyz = w.j3d_xyz; f.ws_j3d_conf = w.j3d_conf;
     f.lane_frame = ss.lane_frame; f.lane_start = ss.lane_start; f.lane_params = ss.lane_params; f.queue = ss.queue;
     f.end_round = ss.end_round; f.pose_valid = w.pose_valid;
     a.q = q;
@@ -1003,8 +1010,11 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, int F, Regi
 // 2 .. n-1 and is the chaining run.  Each pass takes the pending cold frames P (at first: every sequence's first frame) through
 // the runs before c (as a frame stream of P's rows), then runs c over their sequences; a sequence whose next frame turns
 // out cold parks it for the next pass (c > 0 only: with c == 0 the cold frame stays in its slot with the cold slice).
-static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
-                          const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, cudaStream_t st) {
+// gt_xyz / conf3d ([F][K][3] / [F][K], both NULL or both set): the 3-D joint term is on in every stage, cold and warm, iff set;
+// they travel with the frames as gt_uv / conf do.
+static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int n_stages,
+                          const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
+                          cudaStream_t st) {
     constexpr int kWarmSkip = 2;                                      // as run_fit
     if (n_stages > 64) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: at most 64 stages");
     const int NS = s->n_sequences;
@@ -1015,7 +1025,7 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stag
     for (int i = 0; i < n_stages; ++i) {
         const int rc = make_loss_params(ctx, &stage_cfgs[i], &lps[i]);
         if (rc) return rc;
-        lps[i].j3d_on = 0;
+        lps[i].j3d_on = gt_xyz ? 1 : 0;             // the call's own targets, never the context's
         n_vp2 += lps[i].use_vposer == 2;
     }
     if (n_vp2 > 0 && n_vp2 < n_stages)
@@ -1026,7 +1036,7 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stag
         wc.body_pose_weight *= 0.15f;
         const int rc = make_loss_params(ctx, &wc, &wlps[kWarmSkip]);
         if (rc) return rc;
-        wlps[kWarmSkip].j3d_on = 0;
+        wlps[kWarmSkip].j3d_on = gt_xyz ? 1 : 0;
     }
     const int H = opt_cfg->history_size > 0 ? opt_cfg->history_size : 100;
     std::vector<int> ends;
@@ -1057,10 +1067,15 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stag
     q.reinit_loss = s->reinit_loss;
     q.park = c > 0 ? 1 : 0;
     q.keep_pose = n_vp2 == 0 ? 1 : 0;
-    const size_t row_floats = kParams + (size_t)ctx->cams.num_views * ctx->m.K * 3;   // params | gt_uv | conf of a frame
+    // a frame's packed row: params | gt_uv | conf, then gt_xyz | conf3d with the 3-D term
+    const size_t row_floats = kParams + (size_t)ctx->cams.num_views * ctx->m.K * 3 + (gt_xyz ? (size_t)ctx->m.K * 4 : 0);
     int rc = ensure_stream_state(ctx, resident_before ? NS : 0);
     if (!rc) rc = ensure_seq_state(ctx, NS, c > 0 ? row_floats * NS : 0);
     if (!rc && any_dense) rc = ensure_keypoint_ws(ctx);
+    if (!rc && any_dense && gt_xyz && !ctx->ws.j3d_xyz) {           // the lanes' 3-D rows, as run_stream allocates them
+        const size_t n = (size_t)ctx->ws.B * ctx->m.K;
+        if (!(rc = dev_alloc(ctx, &ctx->ws.j3d_xyz, n * 3))) rc = dev_alloc(ctx, &ctx->ws.j3d_conf, n);
+    }
     if (rc) return rc;
     SeqState& ss = *ctx->sstream;
     q.off = ss.off;
@@ -1090,7 +1105,14 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stag
             MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, ss.frames, n, F, kParams, 0));
             MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pg, const_cast<float*>(s->gt_uv), ss.frames, n, F, 2 * K, 0));
             MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pc, const_cast<float*>(s->conf), ss.frames, n, F, K, 0));
-            const mvs_frame_stream fs{n, px, pg, pc, s->joint_weights, nullptr, nullptr, nullptr};
+            float *pj = nullptr, *pjc = nullptr;
+            if (gt_xyz) {
+                pj = pc + (size_t)V * n * K;
+                pjc = pj + (size_t)n * K * 3;
+                MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pj, const_cast<float*>(gt_xyz), ss.frames, n, F, 3 * K, 0));
+                MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pjc, const_cast<float*>(conf3d), ss.frames, n, F, K, 0));
+            }
+            const mvs_frame_stream fs{n, px, pg, pc, s->joint_weights, pj, pjc, nullptr};
             for (int i = 0, g = 0; g < c && !rc; i = ends[g++]) {
                 ctx->loss = lps[i];
                 ctx->have_loss = true;
@@ -1102,11 +1124,13 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stag
         q.n_act = n;
         ctx->loss = lps[ic];
         ctx->have_loss = true;
-        if ((rc = run_seq_chain(ctx, s, F, stage_regime(ctx, lps[ic], H, false), tab, q, opt_cfg, stats, st))) break;
+        if ((rc = run_seq_chain(ctx, s, gt_xyz, conf3d, F, stage_regime(ctx, lps[ic], H, false), tab, q, opt_cfg, stats, st)))
+            break;
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(cur.data(), ss.cur, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
     }
     ctx->loss = lps[n_stages - 1];
+    ctx->loss.j3d_on = 0;
     return rc;
 }
 
@@ -1183,9 +1207,10 @@ int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const 
     return run_stream(ctx, s, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
 }
 
-int mvs_fit_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
-                       const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
+int mvs_fit_seq_stream3d(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int n_stages,
+                         const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
     if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    if (!gt_xyz != !conf3d) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream3d: gt_xyz and conf3d go together");
     if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0))
         return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: model, cameras and batch must be set first");
     if (!s || !stage_cfgs || !opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: NULL argument");
@@ -1205,7 +1230,12 @@ int mvs_fit_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages,
                                                    "it off (mvs_set_anchor enable = 0) to fit a sequence stream");
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     if (stats) memset(stats, 0, sizeof(*stats));
-    return run_seq_stream(ctx, s, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
+    return run_seq_stream(ctx, s, gt_xyz, conf3d, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
+}
+
+int mvs_fit_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
+                       const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
+    return mvs_fit_seq_stream3d(ctx, s, nullptr, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
 }
 
 int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, const float* conf_host,

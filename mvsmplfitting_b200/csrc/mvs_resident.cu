@@ -376,8 +376,10 @@ int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& c
     int with_vposer = 0;
     for (int i = 0; i < nstages; ++i) with_vposer |= (lph[i].use_vposer == 2);
     const size_t smem = frame_smem(H, with_vposer != 0);
+    ResidentModel rm = make_resident_model(ctx);
+    rm.j3d_xyz = in.j3d_xyz; rm.j3d_conf = in.j3d_conf;              // row stride in.n, as gt_uv / conf
     MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
-               lbfgs_resident_seq_kernel<<<q.n_act, kResThreads, smem, st>>>(make_resident_model(ctx), ctx->cams, lp_tab_dev, cfg,
+               lbfgs_resident_seq_kernel<<<q.n_act, kResThreads, smem, st>>>(rm, ctx->cams, lp_tab_dev, cfg,
                                                                              params_dev, in.gt_uv, in.conf, in.joint_w, in.n, H,
                                                                              with_vposer, q));
     MVS_CUDA_OK(ctx, cudaGetLastError());

@@ -64,6 +64,23 @@ def read_keypoints(path: str, person: int = 0):
     return kp
 
 
+def read_joints(path: str, person: int = 0):
+    """data_parser.py:93-146 with use_hands = use_face = False: the 3-D annotation of one person, `pose_keypoints_3d` as
+    float32 rows (x, y, z, confidence) [N,4], N as the file gives it (unlike the 2-D reader, no truncation).  None where the
+    reference's reader gives None for the file: some person without `pose_keypoints_3d`, or with a length that does not
+    reshape to [-1,4] (its try / except drops the whole file); also None when the file lists fewer people.  A file without a
+    'people' list raises KeyError, as the reference's reader does."""
+    with open(path) as f:
+        data = json.load(f)
+    rows = []
+    for p in data["people"]:
+        try:
+            rows.append(np.array(p["pose_keypoints_3d"], dtype=np.float32).reshape([-1, 4]))
+        except Exception:
+            return None
+    return rows[person] if person < len(rows) else None
+
+
 def joint_weights(pose_format: str = "coco17", use_hip: bool = True) -> np.ndarray:
     """FittingData.get_joint_weights, data_parser.py:340-358: hips (11, 12) are ignored unless lsp14 with use_hip"""
     w = np.ones(NUM_BODY_JOINTS, dtype=np.float32)
@@ -86,11 +103,15 @@ def list_sequence(keyp_folder: str, serial: str):
     return cameras, sorted(frames)
 
 
-def load_sequence(keyp_folder: str, serial: str, cameras=None, frames=None, person: int = 0) -> dict:
+def load_sequence(keyp_folder: str, serial: str, cameras=None, frames=None, person: int = 0, use_3d: bool = False) -> dict:
     """All detections of a sequence as the arrays the device path takes: gt_uv [V,B,17,2], conf [V,B,17] float32.
     A (view, frame) without a keypoint file or without that person gets confidence 0 for every joint -- the reference
     drops such a view for that frame (main.py:45-56); with confidence 0 it weighs (w * conf)^2 = 0 in the data term
-    and 1e-6 in the triangulation (recompute3D.py:49)."""
+    and 1e-6 in the triangulation (recompute3D.py:49).
+    use_3d: also the 3-D annotations (data_parser.py:398-402): a frame's annotation is read_joints of the first of
+    `cameras`, in order, whose keypoint file exists and gives one.  Adds joints3d [B,17,3], conf3d [B,17] (column 3 as
+    written) and has3d [B] bool; a frame without annotation has zero rows and has3d False.  An annotation of other than 17
+    rows raises ValueError (the reference cannot broadcast it against the 17 keypoints, fitting.py:318-324)."""
     all_cams, all_frames = list_sequence(keyp_folder, serial)
     cameras = list(cameras) if cameras is not None else all_cams
     frames = list(frames) if frames is not None else all_frames
@@ -107,7 +128,23 @@ def load_sequence(keyp_folder: str, serial: str, cameras=None, frames=None, pers
             if kp is None or kp.shape[0] < NUM_BODY_JOINTS:
                 continue
             gt_uv[v, b], conf[v, b], present[v, b] = kp[:, :2], kp[:, 2], True
-    return dict(gt_uv=gt_uv, conf=conf, present=present, cameras=cameras, frames=frames, serial=serial)
+    out = dict(gt_uv=gt_uv, conf=conf, present=present, cameras=cameras, frames=frames, serial=serial)
+    if use_3d:
+        joints3d = np.zeros((B, NUM_BODY_JOINTS, 3), dtype=np.float32)
+        conf3d = np.zeros((B, NUM_BODY_JOINTS), dtype=np.float32)
+        has3d = np.zeros(B, dtype=bool)
+        for b, fr in enumerate(frames):
+            for cam in cameras:
+                fn = os.path.join(keyp_folder, serial, cam, fr + "_keypoints.json")
+                j = read_joints(fn, person) if os.path.exists(fn) else None
+                if j is None:
+                    continue
+                if j.shape[0] != NUM_BODY_JOINTS:
+                    raise ValueError("%s: pose_keypoints_3d has %d rows, want %d" % (fn, j.shape[0], NUM_BODY_JOINTS))
+                joints3d[b], conf3d[b], has3d[b] = j[:, :3], j[:, 3], True
+                break
+        out.update(joints3d=joints3d, conf3d=conf3d, has3d=has3d)
+    return out
 
 
 PARAM_SLICES = (("betas", 0, 10), ("global_orient", 10, 13), ("body_pose", 13, 82), ("transl", 82, 85), ("scale", 85, 86))
@@ -184,6 +221,42 @@ def _check_missing_views(seq: dict, stage_cfgs) -> None:
         raise ValueError("sequence has (view, frame) pairs without detections: every stage needs use_joints_conf = 1")
 
 
+def _targets_3d(seqs, stage_cfgs, use_hip: bool):
+    """use_3d (non_linear_solver.py:68-99) for sequences loaded with load_sequence(use_3d=True): per frame 3-D targets [F,17,3],
+    confidences [F,17] and has3d [F], the sequences' frames back to back.  A frame without annotation has no 3-D term (:68-69):
+    zero rows, which weigh nothing.  Hips 11 and 12 have confidence 0 unless use_hip (:92-94).  The confidences exist only
+    with use_joints_conf (:90-91), so every stage needs it."""
+    if not all(int(c.use_joints_conf) for c in stage_cfgs):
+        raise ValueError("use_3d needs use_joints_conf = 1 in every stage (the 3-D confidences are read with the 2-D ones)")
+    for q in seqs:
+        if "has3d" not in q:
+            raise ValueError("use_3d: sequence %s was loaded without its 3-D annotations (load_sequence(use_3d=True))"
+                             % q.get("serial"))
+    has = np.concatenate([q["has3d"] for q in seqs])
+    j3 = np.concatenate([q["joints3d"] for q in seqs]).astype(np.float32)
+    c3 = np.concatenate([q["conf3d"] for q in seqs]).astype(np.float32)
+    j3[~has], c3[~has] = 0.0, 0.0
+    if not use_hip:
+        c3[:, 11] = c3[:, 12] = 0.0
+    return j3, c3, has
+
+
+def _init_guess_3d(ctx, guess: dict, j3, c3, has):
+    """init_guess of one batch whose keypoints and loss configuration are set, under use_3d (init_guess.py:85-86): a frame
+    with annotation aligns to its 3-D targets, one without triangulates (or takes the depth guess).  A batch that mixes the
+    two runs the guess once with the targets and once without and takes each frame's row from its pass; the guess is per
+    frame, so each pass gives a frame the bits it gets alone.  Leaves the 3-D term set as the last pass left it."""
+    x = None
+    if has.any():
+        ctx.set_joints3d(j3, c3)
+        x, _ = ctx.init_guess(**guess)
+    if not has.all():
+        ctx.set_joints3d(None)
+        x0, _ = ctx.init_guess(**guess)
+        x = x0 if x is None else torch.where(torch.as_tensor(has, device=x.device)[:, None], x, x0).contiguous()
+    return x
+
+
 def _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces, frames=None, rows=None):
     """per-frame result pickles (+ meshes) of `rows` of the batch (default: all), named by `frames`"""
     x = params.cpu().numpy()
@@ -208,7 +281,7 @@ def _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces, f
 
 def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool = False, fixed_scale: float = 1.0,
                  use_hip: bool = True, pose_format: str = "coco17", result_folder: str | None = None,
-                 mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False):
+                 mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, use_3d: bool = False):
     """The frame loop of main.py:32-89 for one sequence as ONE batch (every frame from its own initial guess, is_seq = False):
     upload the detections, initial guess on the device (init_guess + fix_params), all stages (`mvs_fit`), results per
     frame.  `ctx` is a FittingContext whose model, priors (GMM / VPoser decoder), cameras and batch (= number of frames) are
@@ -217,34 +290,50 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
     A context batch smaller than the sequence works as a pool of slots: the initial guesses are computed ctx.B frames at a
     time, then all frames go through ONE `mvs_fit_stream` call, which refills a slot as soon as its frame is done (the same
     results bit for bit).
+    use_3d (the sequence loaded with load_sequence(use_3d=True)): the 3-D joint term for every frame with an annotation,
+    whose initial guess also aligns to it; frames without one fit as without the term (_targets_3d, _init_guess_3d).  The
+    context has the 3-D term off afterwards.
     Returns (params [F,86] numpy -- pose slot = latent code under VPoser --, final_loss [F], stats)."""
     F = len(seq["frames"])
     assert ctx.B <= F, "context batch %d > frames %d" % (ctx.B, F)
     latent = _uses_latent_pose(stage_cfgs)
     _check_missing_views(seq, stage_cfgs)
+    t3 = _targets_3d([seq], stage_cfgs, use_hip) if use_3d else None
     jw = joint_weights(pose_format, use_hip)
     guess = dict(estimate_scale=estimate_scale, fixed_scale=fixed_scale, use_torso=True, hip_seed=1.0, want_joints3d=False,
                  umeyama_as_written=umeyama_as_written)
     if ctx.B == F:
         ctx.set_keypoints(seq["gt_uv"], seq["conf"], jw)
         ctx.set_loss(config=stage_cfgs[0])           # mvs_init_guess zeroes the pose slot when it holds a latent code
-        params, _ = ctx.init_guess(**guess)
+        if t3 is None:
+            params, _ = ctx.init_guess(**guess)
+        else:
+            params = _init_guess_3d(ctx, guess, *t3)
+            ctx.set_joints3d(t3[0], t3[1])
         final, stats = ctx.fit(params, stage_cfgs, opt_cfg)
+        if t3 is not None:
+            ctx.set_joints3d(None)
         loss = final.cpu().numpy()
         if result_folder is not None:
             _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces)
         return params.cpu().numpy(), loss, stats
-    params = _cold_guesses(ctx, seq["gt_uv"], seq["conf"], jw, stage_cfgs, guess)
-    final, stats = ctx.fit_stream(params, seq["gt_uv"], seq["conf"], jw, stage_cfgs, opt_cfg)
+    params = _cold_guesses(ctx, seq["gt_uv"], seq["conf"], jw, stage_cfgs, guess, t3)
+    if t3 is None:
+        final, stats = ctx.fit_stream(params, seq["gt_uv"], seq["conf"], jw, stage_cfgs, opt_cfg)
+    else:
+        final, stats = ctx.fit_stream(params, seq["gt_uv"], seq["conf"], jw, stage_cfgs, opt_cfg, joints3d=t3[0], conf3d=t3[1])
+        ctx.set_joints3d(None)
     loss = final.cpu().numpy()
     if result_folder is not None:
         _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces)
     return params.cpu().numpy(), loss, stats
 
 
-def _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess: dict) -> torch.Tensor:
+def _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess: dict, t3=None) -> torch.Tensor:
     """initial guesses (init_guess + fix_params) of F frames of any number, ctx.B frames at a time: params [F,86] on the
-    device.  The last chunk is padded with zero-confidence rows, which are dropped."""
+    device.  The last chunk is padded with zero-confidence rows, which are dropped.  t3: _targets_3d of the F frames (use_3d),
+    each chunk's guesses then come from _init_guess_3d (padding rows count as frames without annotation only when the chunk
+    needs that pass anyway)."""
     F, B = gt_uv.shape[1], ctx.B
     params = torch.empty(F, 86, dtype=torch.float32, device=ctx.device)
     for c0 in range(0, F, B):
@@ -254,7 +343,14 @@ def _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess: dict) -> torch.Tensor
         gt[:, :n], cf[:, :n] = gt_uv[:, c0:c0 + n], conf[:, c0:c0 + n]
         ctx.set_keypoints(gt, cf, jw)
         ctx.set_loss(config=stage_cfgs[0])           # mvs_init_guess zeroes the pose slot when it holds a latent code
-        x, _ = ctx.init_guess(**guess)
+        if t3 is None:
+            x, _ = ctx.init_guess(**guess)
+        else:
+            j3 = np.zeros((B,) + t3[0].shape[1:], np.float32)
+            c3 = np.zeros((B,) + t3[1].shape[1:], np.float32)
+            has = np.full(B, bool(t3[2][c0:c0 + n].all()))
+            j3[:n], c3[:n], has[:n] = t3[0][c0:c0 + n], t3[1][c0:c0 + n], t3[2][c0:c0 + n]
+            x = _init_guess_3d(ctx, guess, j3, c3, has)
         params[c0:c0 + n] = x[:n]
     return params
 
@@ -274,7 +370,8 @@ def _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, fac
 
 def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = False, fixed_scale: float = 1.0,
                   use_hip: bool = True, pose_format: str = "coco17", result_folder: str | None = None,
-                  mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, reinit_loss: float = 5000.0):
+                  mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, reinit_loss: float = 5000.0,
+                  use_3d: bool = False):
     """main.py:32-89 with is_seq = True for S sequences in lock-step: the batch of step t is frame t of every sequence
     (context batch = S; same cameras).  A sequence's first frame gets the initial guess and every stage; a later frame
     starts from the previous frame's result as load_init + fix_params leave it (init_guess.py:137-166,190-212: betas,
@@ -284,18 +381,24 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
     A context batch other than S works as a pool of slots: the initial guesses of all frames are computed ctx.B frames at a
     time, then all sequences go through ONE `mvs_fit_seq_stream` call, in which a slot takes the next frame of its sequence
     as soon as a frame is done (the same results bit for bit; stats then also carry the dense-round counts).
+    use_3d (every sequence loaded with load_sequence(use_3d=True)): per frame, as non_linear_solver.py:68-99 decides it --
+    a frame with an annotation has the 3-D joint term in every stage it runs, warm or cold, and its cold start point aligns
+    to the annotation; a frame without one fits as without the term (_targets_3d, _init_guess_3d).  The context has the
+    3-D term off afterwards.
     Returns a list (per sequence) of (params [T_s,86], loss [T_s]) and the summed stats."""
     S_ = len(seqs)
     latent = _uses_latent_pose(stage_cfgs)
     for q in seqs:
         _check_missing_views(q, stage_cfgs)
+    t3 = _targets_3d(seqs, stage_cfgs, use_hip) if use_3d else None
     if ctx.B != S_:
         return _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces,
                                      pose_format, use_hip, dict(estimate_scale=estimate_scale, fixed_scale=fixed_scale,
                                                                 use_torso=True, hip_seed=1.0, want_joints3d=False,
-                                                                umeyama_as_written=umeyama_as_written))
+                                                                umeyama_as_written=umeyama_as_written), t3)
     T = max(len(q["frames"]) for q in seqs)
     V = seqs[0]["gt_uv"].shape[0]
+    off = np.concatenate([[0], np.cumsum([len(q["frames"]) for q in seqs])])
     jw = joint_weights(pose_format, use_hip)
     prev = None
     prev_loss = np.full(S_, np.inf, np.float32)
@@ -313,8 +416,15 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
                 gt[:, s_], cf[:, s_] = q["gt_uv"][:, -1], q["conf"][:, -1]
         ctx.set_keypoints(gt, cf, jw)
         ctx.set_loss(config=stage_cfgs[0])
-        cold, _ = ctx.init_guess(estimate_scale=estimate_scale, fixed_scale=fixed_scale, use_torso=True, hip_seed=1.0,
-                                 want_joints3d=False, umeyama_as_written=umeyama_as_written)
+        guess = dict(estimate_scale=estimate_scale, fixed_scale=fixed_scale, use_torso=True, hip_seed=1.0,
+                     want_joints3d=False, umeyama_as_written=umeyama_as_written)
+        if t3 is None:
+            cold, _ = ctx.init_guess(**guess)
+        else:                                  # frame t's 3-D rows (the last frame's for a finished sequence)
+            rows = [off[s_] + min(t, len(q["frames"]) - 1) for s_, q in enumerate(seqs)]
+            j3, c3, has = t3[0][rows], t3[1][rows], t3[2][rows]
+            cold = _init_guess_3d(ctx, guess, j3, c3, has)
+            ctx.set_joints3d(j3, c3)
         warm = np.zeros(S_, bool) if prev is None else (prev_loss <= reinit_loss)
         params = cold
         if warm.any():
@@ -335,20 +445,27 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
             for s_, q in enumerate(seqs):
                 if live[s_]:
                     _export(ctx, q, params, prev_loss, latent, result_folder, mesh_folder, faces, frames=[q["frames"][t]], rows=[s_])
+    if t3 is not None:
+        ctx.set_joints3d(None)
     return list(zip(out_x, out_l)), tot
 
 
 def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces, pose_format,
-                          use_hip, guess):
+                          use_hip, guess, t3=None):
     """fit_sequences through mvs_fit_seq_stream: the sequences' frames back to back, every frame's cold start point from
-    _cold_guesses"""
+    _cold_guesses; t3: _targets_3d of those frames (mvs_fit_seq_stream3d)"""
     lengths = [len(q["frames"]) for q in seqs]
     off = np.concatenate([[0], np.cumsum(lengths)])
     gt_uv = np.concatenate([q["gt_uv"] for q in seqs], axis=1)
     conf = np.concatenate([q["conf"] for q in seqs], axis=1)
     jw = joint_weights(pose_format, use_hip)
-    params = _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess)
-    final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss)
+    params = _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess, t3)
+    if t3 is None:
+        final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss)
+    else:
+        final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss,
+                                          joints3d=t3[0], conf3d=t3[1])
+        ctx.set_joints3d(None)
     x, loss = params.cpu().numpy(), final.cpu().numpy()
     if result_folder is not None:
         for s_, q in enumerate(seqs):
