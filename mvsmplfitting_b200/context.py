@@ -269,6 +269,21 @@ class FittingContext:
                                                 ctypes.byref(st), self._stream()), "mvs_fit")
         return final, _stats_dict(st)
 
+    def _stream_rows(self, who, F, gt_uv, conf, joint_weights, joints3d, conf3d):
+        """A stream's per-frame rows on the device, checked against F frames: gt_uv [V,F,K,2], conf [V,F,K], joint_weights
+        [K], and joints3d [F,K,3] with conf3d [F,K] or neither (None, None).  who: the public method, for the errors."""
+        dev = lambda a: None if a is None else torch.as_tensor(a).to(self.device, torch.float32).contiguous()
+        gt_uv, conf, jw = dev(gt_uv), dev(conf), dev(joint_weights).reshape(-1)
+        assert tuple(gt_uv.shape) == (self.V, F, self.K, 2) and tuple(conf.shape) == (self.V, F, self.K), \
+            (tuple(gt_uv.shape), tuple(conf.shape), (self.V, F, self.K))
+        if (joints3d is None) != (conf3d is None):
+            raise ValueError("%s: joints3d and conf3d go together" % who)
+        j3, c3 = dev(joints3d), dev(conf3d)
+        if j3 is not None and (tuple(j3.shape) != (F, self.K, 3) or tuple(c3.shape) != (F, self.K)):
+            raise ValueError("%s: want joints3d [%d,%d,3] and conf3d [%d,%d], got %s and %s"
+                             % (who, F, self.K, F, self.K, tuple(j3.shape), tuple(c3.shape)))
+        return gt_uv, conf, jw, j3, c3
+
     def fit_stream(self, params: torch.Tensor, gt_uv, conf, joint_weights, stage_cfgs, opt_cfg=None, joints3d=None,
                    conf3d=None):
         """mvs_fit over F frames of any number through the context's B slots (mvs_fit_stream): params [F,86] CUDA float32,
@@ -278,16 +293,7 @@ class FittingContext:
         Returns (final_loss [F], stats)."""
         assert params.is_cuda and params.dtype == torch.float32 and params.is_contiguous() and params.dim() == 2
         F = params.shape[0]
-        dev = lambda a: None if a is None else torch.as_tensor(a).to(self.device, torch.float32).contiguous()
-        gt_uv, conf, jw = dev(gt_uv), dev(conf), dev(joint_weights).reshape(-1)
-        assert tuple(gt_uv.shape) == (self.V, F, self.K, 2) and tuple(conf.shape) == (self.V, F, self.K), \
-            (tuple(gt_uv.shape), tuple(conf.shape), (self.V, F, self.K))
-        if (joints3d is None) != (conf3d is None):
-            raise ValueError("fit_stream: joints3d and conf3d go together")
-        j3, c3 = dev(joints3d), dev(conf3d)
-        if j3 is not None and (tuple(j3.shape) != (F, self.K, 3) or tuple(c3.shape) != (F, self.K)):
-            raise ValueError("fit_stream: want joints3d [%d,%d,3] and conf3d [%d,%d], got %s and %s"
-                             % (F, self.K, F, self.K, tuple(j3.shape), tuple(c3.shape)))
+        gt_uv, conf, jw, j3, c3 = self._stream_rows("fit_stream", F, gt_uv, conf, joint_weights, joints3d, conf3d)
         final = torch.empty(F, dtype=torch.float32, device=self.device)
         s = _lib.FrameStream(F, _ptr(params), _ptr(gt_uv), _ptr(conf), _ptr(jw), _ptr(j3), _ptr(c3), _ptr(final))
         arr = (_lib.LossConfig * len(stage_cfgs))(*stage_cfgs)
@@ -314,17 +320,7 @@ class FittingContext:
         if not lengths or min(lengths) < 1 or sum(lengths) != F:
             raise ValueError("fit_seq_stream: want sequence lengths >= 1 that add up to %d frames, got %s" % (F, lengths))
         off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(lengths)]), dtype=np.int32)
-        dev = lambda a: torch.as_tensor(a).to(self.device, torch.float32).contiguous()
-        gt_uv, conf, jw = dev(gt_uv), dev(conf), dev(joint_weights).reshape(-1)
-        assert tuple(gt_uv.shape) == (self.V, F, self.K, 2) and tuple(conf.shape) == (self.V, F, self.K), \
-            (tuple(gt_uv.shape), tuple(conf.shape), (self.V, F, self.K))
-        if (joints3d is None) != (conf3d is None):
-            raise ValueError("fit_seq_stream: joints3d and conf3d go together")
-        j3 = None if joints3d is None else torch.as_tensor(joints3d).to(self.device, torch.float32).contiguous()
-        c3 = None if conf3d is None else torch.as_tensor(conf3d).to(self.device, torch.float32).contiguous()
-        if j3 is not None and (tuple(j3.shape) != (F, self.K, 3) or tuple(c3.shape) != (F, self.K)):
-            raise ValueError("fit_seq_stream: want joints3d [%d,%d,3] and conf3d [%d,%d], got %s and %s"
-                             % (F, self.K, F, self.K, tuple(j3.shape), tuple(c3.shape)))
+        gt_uv, conf, jw, j3, c3 = self._stream_rows("fit_seq_stream", F, gt_uv, conf, joint_weights, joints3d, conf3d)
         final = torch.empty(F, dtype=torch.float32, device=self.device)
         s = _lib.SequenceStream(len(lengths), _ptr(off), _ptr(params), _ptr(gt_uv), _ptr(conf), _ptr(jw), _ptr(final),
                                 float(reinit_loss))

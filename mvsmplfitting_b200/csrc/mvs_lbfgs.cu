@@ -130,9 +130,7 @@ __global__ void lbfgs_finalize_kernel(LbfgsState S, int B, float* __restrict__ f
     if (b >= B) return;
     const FrameScalars s = S.sc[b];
     if (final_loss) final_loss[b] = s.final_loss;
-    atomicAdd((unsigned long long*)&totals[0], (unsigned long long)s.iters);
-    atomicAdd((unsigned long long*)&totals[1], (unsigned long long)s.evals);
-    atomicAdd((unsigned long long*)&totals[2], (unsigned long long)(s.nan_flag + s.nan_acc));
+    add_frame_totals(totals, s);
     if (max_evals_as_rounds) atomicMax((unsigned long long*)&totals[3], (unsigned long long)s.evals);
 }
 
@@ -142,154 +140,87 @@ __global__ void iota2_kernel(int* p, int n, int* na) {
     if (i == 0) *na = n;
 }
 
-// mvs_fit_stream (DESIGN.md section 4): the context's B slots are lanes, each holding one frame of an F-frame stream
+// mvs_fit_stream / mvs_fit_seq_stream (DESIGN.md section 4): the context's B slots are lanes, each holding one frame of the
+// call's F frames
 struct StreamState {
     int cap = 0;                        // entries of sc
     FrameScalars* sc = nullptr;         // [cap] frame scalars of the frame-resident groups (one per frame of the stream)
     int* lane_frame = nullptr;          // [B] frame held by each lane of a dense group, -1: none
     long long* lane_start = nullptr;    // [B] round of the group in which the lane's frame started
     float* lane_params = nullptr;       // [B][86] the lanes' parameters (what params_dev is to mvs_fit)
-    int* queue = nullptr;               // [1] next frame of the stream to enter a lane
+    int* queue = nullptr;               // [1] next queue entry to enter a lane
     long long* end_round = nullptr;     // [1] max over retired frames of start round + evaluations: the rounds the group ran
     int* host = nullptr;                // pinned [2]: queue position of the two chunks in flight (next to their active counts)
 };
 
-struct StreamArgs {
-    int F, B, V, K, nstages;
-    float* params;                      // [F][86] the stream's parameters, in / out
+// A dense run over the lanes, fed from a queue.  A frame stream is a sequence stream in which every sequence is one frame
+// long: its frames have no successor, and queue entry k is frame k.
+struct LaneArgs {
+    int F, B, V, K;
+    int n_queue;                        // queue entries: F (frame stream) or q.n_act (sequences of this pass)
+    float* params;                      // [F][86] the call's parameters, in / out
     float* final_loss;                  // [F] or NULL
     const float *gt_uv, *conf;          // [V][F][K][2], [V][F][K]
     const float *j3d_xyz, *j3d_conf;    // [F][K][3], [F][K]; NULL: 3-D term off
     float *ws_gt_uv, *ws_conf, *ws_j3d_xyz, *ws_j3d_conf;     // the lanes' rows, read by the dense kernels
     int* lane_frame; long long* lane_start; float* lane_params; int* queue; long long* end_round;
     int* pose_valid;
+    SeqChain q;                         // the sequences, queued by q.act; q.off == NULL: a frame stream (q.cold: its stage table)
+    int* lane_seq;                      // [B] sequence of each lane's frame (sequence stream)
 };
 
-// Runs just before lbfgs_compact_kernel at every compaction point of a dense group of mvs_fit_stream (and once before the
-// group's first round).  Every lane whose frame is done hands the frame's parameters, final loss and counts back to the
-// stream; the freed lanes then take the next queued frames in ascending lane order (ballot + prefix sum: no atomics decide
-// which lane gets which frame), and each new frame starts exactly as lbfgs_init_kernel starts a frame of mvs_fit, so that
-// its bits do not depend on the lane or on when it entered.  round: rounds of the group run so far (the new frames' first
-// round).  flush != 0: hand back every frame still in a lane, take none.
-__global__ void __launch_bounds__(1024) stream_refill_kernel(LbfgsState S, StreamArgs a, long long round, int flush) {
+// What follows a lane's finished frame `old` in the lane: its successor in the same sequence -- warm from the frame's
+// fitted row when the frame's loss is <= reinit_loss, else cold -- or -1 when the lane is freed: a frame stream's frames have
+// no successor, and a sequence that ends or parks a cold successor gives its lane up.
+__device__ __forceinline__ int lane_successor(const LaneArgs& a, int l, int old, float loss, int flush, bool& warm) {
+    warm = false;
+    if (!a.q.off) return -1;
+    const int sq = a.lane_seq[l], nx = old + 1;
+    const bool more = !flush && nx < a.q.off[sq + 1];
+    warm = more && loss <= a.q.reinit_loss;                         // NaN is not
+    if (warm || (more && !a.q.park)) return nx;
+    a.q.cur[sq] = more ? nx : -1;
+    return -1;
+}
+
+// The frame that queue entry k brings into lane l: frame k of a frame stream, the pending frame of sequence q.act[k] otherwise
+__device__ __forceinline__ int queued_frame(const LaneArgs& a, int l, int k) {
+    if (!a.q.off) return k;
+    const int sq = a.q.act[k];
+    a.lane_seq[l] = sq;
+    return a.q.cur[sq];
+}
+
+// Runs just before lbfgs_compact_kernel at every compaction point of a dense run over lanes (and once before the run's first
+// round).  Every lane whose frame is done hands the frame's parameters, final loss and counts back to the call and takes the
+// frame's successor in place (a lane that continues stays active).  The freed lanes then take the next queue entries in
+// ascending lane order (ballot + prefix sum: no atomics decide which lane gets which frame), so freed lanes only take from
+// the queue and the host's na_bound rule holds.  Every frame that enters a lane brings its detections and, with the 3-D term
+// on, its 3-D targets into the lane's rows, and starts as lbfgs_init_kernel starts a frame of mvs_fit, so that its bits do not
+// depend on the lane or on when it entered.  round: rounds of the run so far (the new frames' first round).  flush != 0: hand
+// back every frame still in a lane, take none.
+__global__ void __launch_bounds__(1024) lane_refill_kernel(LbfgsState S, LaneArgs a, long long round, int flush) {
     __shared__ int wsum[32];
     __shared__ int qbase;
     __shared__ int s_old[1024], s_new[1024];
+    __shared__ unsigned char s_warm[1024];
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     if (tid == 0) qbase = *a.queue;
     __syncthreads();
     for (int l0 = 0; l0 < a.B; l0 += 1024) {
         const int l = l0 + tid;
         int old = -1, fresh = -1;
-        bool freed = false;
+        bool fin = false, freed = false, warm = false;
         if (l < a.B) {
             old = a.lane_frame[l];
-            freed = old < 0 || flush || S.sc[l].phase == PH_DONE;
-            if (old >= 0 && freed) {                      // the frame's totals, as lbfgs_finalize_kernel counts them
+            fin = old < 0 || flush || S.sc[l].phase == PH_DONE;
+            if (old >= 0 && fin) {                        // the frame's totals, as lbfgs_finalize_kernel counts them
                 const FrameScalars& s = S.sc[l];
                 if (a.final_loss) a.final_loss[old] = s.final_loss;
-                atomicAdd((unsigned long long*)&S.totals[0], (unsigned long long)s.iters);
-                atomicAdd((unsigned long long*)&S.totals[1], (unsigned long long)s.evals);
-                atomicAdd((unsigned long long*)&S.totals[2], (unsigned long long)(s.nan_flag + s.nan_acc));
+                add_frame_totals(S.totals, s);
                 atomicMax((unsigned long long*)a.end_round, (unsigned long long)(a.lane_start[l] + s.evals));
-            } else {
-                old = -1;
-            }
-        }
-        const unsigned m = __ballot_sync(0xffffffffu, freed);
-        const int pre = __popc(m & ((1u << lane) - 1));
-        if (lane == 0) wsum[wid] = __popc(m);
-        __syncthreads();
-        if (freed) {
-            int f = qbase + pre;
-            for (int w = 0; w < wid; ++w) f += wsum[w];
-            fresh = (!flush && f < a.F) ? f : -1;
-            a.lane_frame[l] = fresh;
-            if (fresh >= 0) a.lane_start[l] = round;
-            else S.sc[l].phase = PH_DONE;                 // an empty lane stays out of the active list
-        }
-        s_old[tid] = old;
-        s_new[tid] = fresh;
-        __syncthreads();
-        if (tid == 0 && !flush) {
-            int tot = qbase;
-            for (int w = 0; w < 32; ++w) tot += wsum[w];
-            qbase = tot < a.F ? tot : a.F;
-        }
-        // parameters out and in, the new frame's detections into the lane's rows: one warp per lane
-        for (int j = wid; j < 1024 && l0 + j < a.B; j += 32) {
-            const int ln = l0 + j, fo = s_old[j], fn = s_new[j];
-            float* xl = a.lane_params + (size_t)ln * kParams;
-            if (fo >= 0) {
-                VLOOP(i) a.params[(size_t)fo * kParams + i] = xl[i];
-            }
-            if (fn < 0) continue;
-            VLOOP(i) xl[i] = a.params[(size_t)fn * kParams + i];
-            const int K = a.K;
-            for (int v = 0; v < a.V; ++v) {
-                const size_t dst = (size_t)v * a.B + ln, src = (size_t)v * a.F + fn;
-                for (int k = lane; k < 2 * K; k += 32) a.ws_gt_uv[dst * 2 * K + k] = a.gt_uv[src * 2 * K + k];
-                for (int k = lane; k < K; k += 32) a.ws_conf[dst * K + k] = a.conf[src * K + k];
-            }
-            if (a.j3d_xyz) {
-                for (int k = lane; k < 3 * K; k += 32) a.ws_j3d_xyz[(size_t)ln * 3 * K + k] = a.j3d_xyz[(size_t)fn * 3 * K + k];
-                for (int k = lane; k < K; k += 32) a.ws_j3d_conf[(size_t)ln * K + k] = a.j3d_conf[(size_t)fn * K + k];
-            }
-            __syncwarp();
-            init_frame_state(S, xl, ln, 1, a.nstages, nullptr, lane);
-            if (lane == 0) a.pose_valid[ln] = 0;           // the lane's pose cache belongs to its previous frame
-        }
-        __syncthreads();
-    }
-    if (tid == 0) *a.queue = qbase;
-}
-
-// mvs_fit_seq_stream's dense chaining run: a lane holds a sequence, the queue is q.act (sequences, not frames)
-struct SeqArgs {
-    StreamArgs f;                       // F: frames of the call; the lane arrays and the queue position as for a frame stream
-    SeqChain q;
-    int* lane_seq;                      // [B] sequence of each lane's frame
-};
-
-// stream_refill_kernel for sequences, at the same points of the dense run.  A lane whose frame is done hands the frame back
-// and takes its successor in the same sequence: warm from the frame's fitted row (body-pose slot from the successor's own
-// row unless the stages carry a latent code), cold from the successor's row unless cold frames park.  Every frame that enters
-// a lane brings its detections and, with the 3-D term on, its 3-D targets into the lane's rows.  A lane whose
-// sequence ends or parks takes the next queued sequence's pending frame, in ascending lane order (ballot + prefix sum).
-// A lane that continues stays active and freed lanes only take from the queue, so the host's na_bound rule holds.
-__global__ void __launch_bounds__(1024) seq_refill_kernel(LbfgsState S, SeqArgs a, long long round, int flush) {
-    __shared__ int wsum[32];
-    __shared__ int qbase;
-    __shared__ int s_old[1024], s_new[1024];
-    __shared__ unsigned char s_warm[1024];
-    const StreamArgs& f = a.f;
-    const SeqChain& q = a.q;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    if (tid == 0) qbase = *f.queue;
-    __syncthreads();
-    for (int l0 = 0; l0 < f.B; l0 += 1024) {
-        const int l = l0 + tid;
-        int old = -1, fresh = -1;
-        bool fin = false, freed = false, warm = false;
-        if (l < f.B) {
-            old = f.lane_frame[l];
-            fin = old < 0 || flush || S.sc[l].phase == PH_DONE;
-            if (old >= 0 && fin) {
-                const FrameScalars& s = S.sc[l];
-                if (f.final_loss) f.final_loss[old] = s.final_loss;
-                atomicAdd((unsigned long long*)&S.totals[0], (unsigned long long)s.iters);
-                atomicAdd((unsigned long long*)&S.totals[1], (unsigned long long)s.evals);
-                atomicAdd((unsigned long long*)&S.totals[2], (unsigned long long)(s.nan_flag + s.nan_acc));
-                atomicMax((unsigned long long*)f.end_round, (unsigned long long)(f.lane_start[l] + s.evals));
-                const int sq = a.lane_seq[l], nx = old + 1;
-                const bool more = !flush && nx < q.off[sq + 1];
-                warm = more && s.final_loss <= q.reinit_loss;          // NaN is not
-                if (warm || (more && !q.park)) {
-                    fresh = nx;
-                } else {
-                    q.cur[sq] = more ? nx : -1;
-                    freed = true;
-                }
+                fresh = lane_successor(a, l, old, s.final_loss, flush, warm);
+                freed = fresh < 0;
             } else {
                 freed = fin;
                 old = -1;
@@ -302,12 +233,11 @@ __global__ void __launch_bounds__(1024) seq_refill_kernel(LbfgsState S, SeqArgs 
         if (freed) {
             int k = qbase + pre;
             for (int w = 0; w < wid; ++w) k += wsum[w];
-            const int sq = (!flush && k < q.n_act) ? q.act[k] : -1;
-            if (sq >= 0) { fresh = q.cur[sq]; a.lane_seq[l] = sq; }
+            if (!flush && k < a.n_queue) fresh = queued_frame(a, l, k);
         }
         if (fin) {
-            f.lane_frame[l] = fresh;
-            if (fresh >= 0) f.lane_start[l] = round;
+            a.lane_frame[l] = fresh;
+            if (fresh >= 0) a.lane_start[l] = round;
             else S.sc[l].phase = PH_DONE;                 // an empty lane stays out of the active list
         }
         s_old[tid] = old;
@@ -317,42 +247,40 @@ __global__ void __launch_bounds__(1024) seq_refill_kernel(LbfgsState S, SeqArgs 
         if (tid == 0 && !flush) {
             int tot = qbase;
             for (int w = 0; w < 32; ++w) tot += wsum[w];
-            qbase = tot < q.n_act ? tot : q.n_act;
+            qbase = tot < a.n_queue ? tot : a.n_queue;
         }
         // parameters out and in, the new frame's detections into the lane's rows: one warp per lane
-        for (int j = wid; j < 1024 && l0 + j < f.B; j += 32) {
+        for (int j = wid; j < 1024 && l0 + j < a.B; j += 32) {
             const int ln = l0 + j, fo = s_old[j], fn = s_new[j];
             const bool wm = s_warm[j] != 0;
-            float* xl = f.lane_params + (size_t)ln * kParams;
+            float* xl = a.lane_params + (size_t)ln * kParams;
             if (fo >= 0) {
-                VLOOP(i) f.params[(size_t)fo * kParams + i] = xl[i];
+                VLOOP(i) a.params[(size_t)fo * kParams + i] = xl[i];
             }
             if (fn < 0) continue;
-            VLOOP(i) {
-                if (!wm || (q.keep_pose && i >= kOffPose && i < kOffTransl)) xl[i] = f.params[(size_t)fn * kParams + i];
+            VLOOP(i) {                                    // a warm frame keeps the fitted row (but its own body pose, keep_pose)
+                if (!wm || (a.q.keep_pose && i >= kOffPose && i < kOffTransl)) xl[i] = a.params[(size_t)fn * kParams + i];
             }
-            const int K = f.K;
-            for (int v = 0; v < f.V; ++v) {
-                const size_t dst = (size_t)v * f.B + ln, src = (size_t)v * f.F + fn;
-                for (int k = lane; k < 2 * K; k += 32) f.ws_gt_uv[dst * 2 * K + k] = f.gt_uv[src * 2 * K + k];
-                for (int k = lane; k < K; k += 32) f.ws_conf[dst * K + k] = f.conf[src * K + k];
+            const int K = a.K;
+            for (int v = 0; v < a.V; ++v) {
+                const size_t dst = (size_t)v * a.B + ln, src = (size_t)v * a.F + fn;
+                for (int k = lane; k < 2 * K; k += 32) a.ws_gt_uv[dst * 2 * K + k] = a.gt_uv[src * 2 * K + k];
+                for (int k = lane; k < K; k += 32) a.ws_conf[dst * K + k] = a.conf[src * K + k];
             }
-            if (f.j3d_xyz) {
-                for (int k = lane; k < 3 * K; k += 32) f.ws_j3d_xyz[(size_t)ln * 3 * K + k] = f.j3d_xyz[(size_t)fn * 3 * K + k];
-                for (int k = lane; k < K; k += 32) f.ws_j3d_conf[(size_t)ln * K + k] = f.j3d_conf[(size_t)fn * K + k];
+            if (a.j3d_xyz) {
+                for (int k = lane; k < 3 * K; k += 32) a.ws_j3d_xyz[(size_t)ln * 3 * K + k] = a.j3d_xyz[(size_t)fn * 3 * K + k];
+                for (int k = lane; k < K; k += 32) a.ws_j3d_conf[(size_t)ln * K + k] = a.j3d_conf[(size_t)fn * K + k];
             }
             __syncwarp();
-            init_frame_state(S, xl, ln, 1, f.nstages, nullptr, lane);
+            VLOOP(i) S.x_eval[(size_t)ln * kParams + i] = xl[i];
             if (lane == 0) {
-                const int2 r = wm ? q.warm : q.cold;            // the frame's slice of the run's stage table
-                S.sc[ln].stage = r.x;
-                S.sc[ln].stage_end = r.y;
-                f.pose_valid[ln] = 0;                           // the lane's pose cache belongs to its previous frame
+                S.sc[ln] = fresh_frame_scalars(wm ? a.q.warm : a.q.cold);     // the frame's slice of the run's stage table
+                a.pose_valid[ln] = 0;                     // the lane's pose cache belongs to its previous frame
             }
         }
         __syncthreads();
     }
-    if (tid == 0) *f.queue = qbase;
+    if (tid == 0) *a.queue = qbase;
 }
 
 // rows idx[0 .. n) of full [V][n_full][L] <-> packed [V][n][L]; to_full = 0 gathers, 1 scatters
@@ -430,10 +358,12 @@ static bool resident_closure_applies(const mvs_ctx* ctx, bool want_verts) {
     return !want_verts && !sdf_term_on(ctx->loss) && ctx->exec_mode != 1 && resident_supported(ctx);
 }
 
+static int history_size(const mvs_lbfgs_config* c) { return c->history_size > 0 ? c->history_size : 100; }
+
 // Shared set-up of a run: optimiser configuration, state for history size H, zeroed totals, stage table on the device
 static int begin_run(mvs_ctx* ctx, const mvs_lbfgs_config* c, bool step, const LossParams* lps, int nst, LbfgsCfg* cfg,
                      cudaStream_t st) {
-    const int H = c->history_size > 0 ? c->history_size : 100;
+    const int H = history_size(c);
     if (H > 128) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_run: history_size must be <= 128");
     int rc = ensure_state(ctx, H);
     if (rc) return rc;
@@ -473,16 +403,16 @@ static int dense_round(mvs_ctx* ctx, float* params_dev, const LbfgsState& S, con
 }
 
 // Dense regime (SDF term on): rounds of dense_round until no frame is active.  Finished frames are compacted out once per
-// chunk of rounds.  fs (mvs_fit_stream): the finished frames' lanes are refilled from the stream's queue just before each
-// compaction.  sq (mvs_fit_seq_stream, fs = &sq->f): the same with seq_refill_kernel, the queue holds sequences.
+// chunk of rounds.  la (mvs_fit_stream, mvs_fit_seq_stream): the finished frames' lanes are refilled from la's queue just
+// before each compaction.
 static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int nst, cudaStream_t st,
-                     const StreamArgs* fs = nullptr, const SeqArgs* sq = nullptr) {
+                     const LaneArgs* la = nullptr) {
     LbfgsState& S = *ctx->lbfgs;
     Workspace& w = ctx->ws;
     const int B = w.B;
     const int chunk = 8;
     // (a lane of a sequence stream may carry every frame of the call)
-    const long long frames_per_lane = sq ? fs->F + 1 : fs ? (fs->F + B - 1) / B + 1 : 1;
+    const long long frames_per_lane = !la ? 1 : la->q.off ? la->F + 1 : (la->F + B - 1) / B + 1;
     const long long max_rounds = ((long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8) * nst * frames_per_lane;
     long long rounds = 0;
     int na_host = B;
@@ -502,8 +432,8 @@ static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int n
         MVS_CUDA_OK(ctx, cudaEventCreateWithFlags(&S.na_event[1], cudaEventDisableTiming | cudaEventBlockingSync));
     }
     int* na_slots = reinterpret_cast<int*>(S.na_host);           // [0], [1]: two chunks in flight
-    int* queue_slots = fs ? ctx->fstream->host : nullptr;         // the same chunks' queue positions
-    bool drained = fs == nullptr;                                 // the host has seen the stream's queue empty
+    int* queue_slots = la ? ctx->fstream->host : nullptr;         // the same chunks' queue positions
+    bool drained = la == nullptr;                                 // the host has seen the queue empty
     int pending = -1;                                             // chunk whose count has not been read yet
     long long chunk_idx = 0;
     w.na_bound = B;                                               // grids shrink with the (lagging) host view of the count
@@ -512,21 +442,20 @@ static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int n
             if ((rc = dense_round(ctx, params_dev, S, cfg, nst, st))) return rc;
             ++rounds;
         }
-        if (sq) MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, seq_refill_kernel<<<1, 1024, 0, st>>>(S, *sq, rounds, 0));
-        else if (fs) MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, stream_refill_kernel<<<1, 1024, 0, st>>>(S, *fs, rounds, 0));
+        if (la) MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lane_refill_kernel<<<1, 1024, 0, st>>>(S, *la, rounds, 0));
         // compaction changes slot -> frame, so the surviving frames' Phi / transforms are rebuilt for their new slots
         MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
         if ((rc = launch_frame_fwd_dense(ctx, S.x_eval, S, nst, st))) return rc;
         const int cur = (int)(chunk_idx & 1);
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(&na_slots[cur], w.na, sizeof(int), cudaMemcpyDeviceToHost, st));
-        if (fs) MVS_CUDA_OK(ctx, cudaMemcpyAsync(&queue_slots[cur], fs->queue, sizeof(int), cudaMemcpyDeviceToHost, st));
+        if (la) MVS_CUDA_OK(ctx, cudaMemcpyAsync(&queue_slots[cur], la->queue, sizeof(int), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaEventRecord(S.na_event[cur], st));
         if (pending >= 0) {
             const auto tb0 = std::chrono::steady_clock::now();
             MVS_CUDA_OK(ctx, cudaEventSynchronize(S.na_event[pending]));
             if (trace_host) blocked_us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - tb0).count();
             na_host = na_slots[pending];
-            if (!drained) drained = queue_slots[pending] >= (sq ? sq->q.n_act : fs->F);
+            if (!drained) drained = queue_slots[pending] >= la->n_queue;
             if (trace_na) fprintf(stderr, "[mvs] dense regime: chunk %lld, active frames %d\n", chunk_idx - 1, na_host);
             if (na_host <= 0) break;                              // (a refill leaves no lane idle while frames are queued)
             // Without refills the list only shrinks, so the count is an upper bound for every later round.  Refills add
@@ -576,6 +505,15 @@ static int run_batched(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, boo
     return MVS_OK;
 }
 
+// Adds a run's totals th ([0..2] iterations, evaluations, NaN / Inf stops) and its rounds to stats, and to the dense counters
+// for a dense run
+static void add_totals(mvs_lbfgs_stats* stats, const long long* th, long long rounds, bool dense) {
+    if (!stats) return;
+    stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
+    stats->rounds += (int)rounds;
+    if (dense) { stats->dense_frame_evals += th[1]; stats->dense_rounds += (int)rounds; }
+}
+
 // End of a run: final losses and totals.  The frame-resident kernel wrote the last gradient itself and leaves the active
 // list alone; the round-based regimes copy the gradient and leave the context usable for plain closures (full active list).
 // The dense and frame-resident regimes report the largest per-frame evaluation count (the critical path) as rounds.
@@ -590,11 +528,7 @@ static int end_run(mvs_ctx* ctx, Regime rg, float* final_loss_dev, float* last_g
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
     if (rg != kResident) MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
     MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    if (stats) {
-        stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
-        stats->rounds += (int)th[3];
-        if (rg == kDense) { stats->dense_frame_evals += th[1]; stats->dense_rounds += (int)th[3]; }
-    }
+    add_totals(stats, th, th[3], rg == kDense);
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }
@@ -686,21 +620,58 @@ static int stage_group_end(const mvs_ctx* ctx, const std::vector<LossParams>& lp
     return j;
 }
 
+// warm-started frames (is_seq, non_linear_solver.py:157-162): no stage 0 and 1, stage 2 with 0.15 x body_pose_weight
+constexpr int kWarmSkip = 2;
+
+// The LossParams of a call's stages (at most 64; who names the entry point in the error).  j3d >= 0 sets the 3-D joint term
+// on (1) or off (0) in every stage: a stream's own targets, never the context's.
+static int stage_table(mvs_ctx* ctx, const char* who, int n_stages, const mvs_loss_config* cfgs, int j3d,
+                       std::vector<LossParams>* lps) {
+    if (n_stages > 64) return set_error(ctx, MVS_ERR_INVALID, "%s: at most 64 stages", who);
+    lps->resize(n_stages);
+    for (int i = 0; i < n_stages; ++i) {
+        const int rc = make_loss_params(ctx, &cfgs[i], &(*lps)[i]);
+        if (rc) return rc;
+        if (j3d >= 0) (*lps)[i].j3d_on = j3d;
+    }
+    return MVS_OK;
+}
+
+// The warm-started frames' copy of a stage table: stage kWarmSkip with 0.15 x its body-pose weight
+static int warm_stage_table(mvs_ctx* ctx, const mvs_loss_config* cfgs, int j3d, const std::vector<LossParams>& lps,
+                            std::vector<LossParams>* wlps) {
+    *wlps = lps;
+    mvs_loss_config wc = cfgs[kWarmSkip];
+    wc.body_pose_weight *= 0.15f;
+    const int rc = make_loss_params(ctx, &wc, &(*wlps)[kWarmSkip]);
+    if (!rc && j3d >= 0) (*wlps)[kWarmSkip].j3d_on = j3d;
+    return rc;
+}
+
+// The runs of a stream's stages, grouped as run_fit groups them (at most max_run stages each): ends[g] is one past run g's
+// last stage.  A stage of the batched reference chain is refused: that chain has no stream.
+static int stream_runs(mvs_ctx* ctx, const char* who, const std::vector<LossParams>& lps, int H, int max_run,
+                       std::vector<int>* ends) {
+    for (int i = 0; i < (int)lps.size(); i = ends->back()) {
+        if (stage_regime(ctx, lps[i], H, false) == kBatched)
+            return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: stage %d would run in the batched reference chain (exec mode 1, "
+                                                       "history_size > 100 without the SDF term, or a model the frame-resident "
+                                                       "and dense kernels do not take), which has no stream", who, i);
+        ends->push_back(stage_group_end(ctx, lps, i, H, max_run));
+    }
+    return MVS_OK;
+}
+
 // All stages of a fit.  Consecutive stages that run in the same regime are handed to ONE multi-stage run in which
 // every frame changes stage on its own (frames are independent problems, so a frame that converged need not wait at
 // the stage boundary for the slowest one; the per-frame arithmetic is the sequential schedule's).  exec_mode 2 keeps
 // the stage barrier (one run per stage).
 static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg,
                    float* final_loss_dev, mvs_lbfgs_stats* stats, cudaStream_t st, const unsigned char* warm_host = nullptr) {
-    if (n_stages > 64) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit: at most 64 stages");
-    std::vector<LossParams> lps(n_stages);
-    for (int i = 0; i < n_stages; ++i) {
-        const int rc = make_loss_params(ctx, &stage_cfgs[i], &lps[i]);
-        if (rc) return rc;
-    }
+    std::vector<LossParams> lps;
+    int rc = stage_table(ctx, "mvs_fit", n_stages, stage_cfgs, -1, &lps);
+    if (rc) return rc;
     const int B = ctx->ws.B;
-    // warm-started frames (is_seq, non_linear_solver.py:157-162): no stage 0 and 1, stage 2 with 0.15 x body_pose_weight
-    constexpr int kWarmSkip = 2;
     bool any_warm = false;
     if (warm_host)
         for (int b = 0; b < B; ++b) any_warm |= warm_host[b] != 0;
@@ -708,17 +679,10 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
         return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq: warm-started frames skip the first %d stages, %d given", kWarmSkip, n_stages);
     std::vector<LossParams> wlps;
     if (any_warm) {
-        wlps = lps;
-        std::vector<mvs_loss_config> wc(stage_cfgs, stage_cfgs + n_stages);
-        wc[kWarmSkip].body_pose_weight *= 0.15f;
-        const int rc = make_loss_params(ctx, &wc[kWarmSkip], &wlps[kWarmSkip]);
-        if (rc) return rc;
-        if (!ctx->stage_rng) {
-            const int rc2 = dev_alloc(ctx, &ctx->stage_rng, (size_t)B);
-            if (rc2) return rc2;
-        }
+        if ((rc = warm_stage_table(ctx, stage_cfgs, -1, lps, &wlps))) return rc;
+        if (!ctx->stage_rng && (rc = dev_alloc(ctx, &ctx->stage_rng, (size_t)B))) return rc;
     }
-    const int H = opt_cfg->history_size > 0 ? opt_cfg->history_size : 100;
+    const int H = history_size(opt_cfg);
     const int max_run = any_warm ? kMaxStages / 2 : kMaxStages;       // the table holds the cold and the warm slice of a run
     std::vector<int> rng;
     std::vector<LossParams> tab;                                      // stage table of a warm run (read by run_stage)
@@ -799,19 +763,65 @@ static int ensure_stream_state(mvs_ctx* ctx, int F_resident) {
     return MVS_OK;
 }
 
+// The lanes' keypoint rows, and their 3-D target rows when with_j3d
+static int ensure_lane_rows(mvs_ctx* ctx, bool with_j3d) {
+    Workspace& w = ctx->ws;
+    int rc = ensure_keypoint_ws(ctx);
+    if (!rc && with_j3d && !w.j3d_xyz) {
+        const size_t n = (size_t)w.B * ctx->m.K;
+        if (!(rc = dev_alloc(ctx, &w.j3d_xyz, n * 3))) rc = dev_alloc(ctx, &w.j3d_conf, n);
+    }
+    return rc;
+}
+
+// A dense run over the context's B lanes, fed from the queue that a describes (the caller sets F, n_queue, the call's arrays,
+// q.cold and, for a sequence stream, q and lane_seq): the first fill, the rounds, and the hand-back of whatever the round
+// limit left in the lanes.  Adds the run's totals to stats.
+static int run_lanes(mvs_ctx* ctx, LaneArgs& a, const float* joint_weights, const LbfgsCfg& cfg, int nst, mvs_lbfgs_stats* stats,
+                     cudaStream_t st) {
+    LbfgsState& S = *ctx->lbfgs;
+    StreamState& ss = *ctx->fstream;
+    Workspace& w = ctx->ws;
+    const int B = w.B, K = ctx->m.K;
+    long long* th = reinterpret_cast<long long*>(S.na_host) + 1;      // [0..2] totals, [4] rounds
+    int rc;
+    if ((rc = frame_step_begin_run(ctx, st))) return rc;                 // (allocates the pose cache on first use)
+    a.B = B; a.V = ctx->cams.num_views; a.K = K;
+    a.ws_gt_uv = w.gt_uv; a.ws_conf = w.conf; a.ws_j3d_xyz = w.j3d_xyz; a.ws_j3d_conf = w.j3d_conf;
+    a.lane_frame = ss.lane_frame; a.lane_start = ss.lane_start; a.lane_params = ss.lane_params; a.queue = ss.queue;
+    a.end_round = ss.end_round; a.pose_valid = w.pose_valid;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(w.joint_w, joint_weights, (size_t)K * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.lane_frame, 0xff, (size_t)B * sizeof(int), st));
+    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.queue, 0, sizeof(int), st));
+    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.end_round, 0, sizeof(long long), st));
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
+    // the first min(n_queue, B) queue entries enter through the same path as every later one
+    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lane_refill_kernel<<<1, 1024, 0, st>>>(S, a, 0, 0));
+    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
+    if ((rc = run_dense(ctx, ss.lane_params, cfg, nst, st, &a))) return rc;
+    // whatever the round limit left in the lanes (nothing, when every frame finished)
+    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lane_refill_kernel<<<1, 1024, 0, st>>>(S, a, 0, 1));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 3 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th + 4, ss.end_round, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    add_totals(stats, th, th[4], true);
+    return MVS_OK;
+}
+
 // One run of mvs_fit_stream: stages lps[0 .. nst) of one regime over all F frames of the stream
 static int run_stream_group(mvs_ctx* ctx, const mvs_frame_stream* s, Regime rg, const LossParams* lps, int nst,
                             const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats, cudaStream_t st) {
     LbfgsCfg cfg;
     int rc = begin_run(ctx, c, false, lps, nst, &cfg, st);
     if (rc) return rc;
-    LbfgsState& S = *ctx->lbfgs;
-    StreamState& ss = *ctx->fstream;
-    Workspace& w = ctx->ws;
-    const int F = s->n_frames, B = w.B, K = ctx->m.K;
-    long long* th = reinterpret_cast<long long*>(S.na_host) + 1;      // [0..3] totals, [4] rounds of a dense group
+    const int F = s->n_frames;
     if (rg == kResident) {
         // one launch over all F frames, one CTA each: the block scheduler refills the SMs as frames finish
+        LbfgsState& S = *ctx->lbfgs;
+        StreamState& ss = *ctx->fstream;
+        long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
         const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, s->gt_xyz, s->conf3d};
         if ((rc = launch_lbfgs_resident(ctx, s->params, cfg, cfg.history, S.lp_tab, lps, nst, ss.sc, nullptr, st, nullptr, &in)))
             return rc;
@@ -821,78 +831,31 @@ static int run_stream_group(mvs_ctx* ctx, const mvs_frame_stream* s, Regime rg, 
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
         MVS_CUDA_OK(ctx, cudaGetLastError());
-        if (stats) {
-            stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
-            stats->rounds += (int)th[3];
-        }
+        add_totals(stats, th, th[3], false);
         return MVS_OK;
     }
-    // dense rounds over B lanes fed from the queue
-    if ((rc = frame_step_begin_run(ctx, st))) return rc;                 // (allocates the pose cache on first use)
-    StreamArgs a;
-    a.F = F; a.B = B; a.V = ctx->cams.num_views; a.K = K; a.nstages = nst;
+    LaneArgs a{};
+    a.F = F; a.n_queue = F;
     a.params = s->params; a.final_loss = s->final_loss; a.gt_uv = s->gt_uv; a.conf = s->conf;
     a.j3d_xyz = s->gt_xyz; a.j3d_conf = s->conf3d;
-    a.ws_gt_uv = w.gt_uv; a.ws_conf = w.conf; a.ws_j3d_xyz = w.j3d_xyz; a.ws_j3d_conf = w.j3d_conf;
-    a.lane_frame = ss.lane_frame; a.lane_start = ss.lane_start; a.lane_params = ss.lane_params; a.queue = ss.queue;
-    a.end_round = ss.end_round; a.pose_valid = w.pose_valid;
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(w.joint_w, s->joint_weights, (size_t)K * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.lane_frame, 0xff, (size_t)B * sizeof(int), st));
-    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.queue, 0, sizeof(int), st));
-    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.end_round, 0, sizeof(long long), st));
-    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-    // the first min(F, B) frames enter through the same path as every later one
-    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, stream_refill_kernel<<<1, 1024, 0, st>>>(S, a, 0, 0));
-    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
-    if ((rc = run_dense(ctx, ss.lane_params, cfg, nst, st, &a))) return rc;
-    // whatever the round limit left in the lanes (nothing, when every frame finished)
-    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, stream_refill_kernel<<<1, 1024, 0, st>>>(S, a, 0, 1));
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 3 * sizeof(long long), cudaMemcpyDeviceToHost, st));
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th + 4, ss.end_round, sizeof(long long), cudaMemcpyDeviceToHost, st));
-    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    MVS_CUDA_OK(ctx, cudaGetLastError());
-    if (stats) {
-        stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
-        stats->rounds += (int)th[4];
-        stats->dense_frame_evals += th[1]; stats->dense_rounds += (int)th[4];
-    }
-    return MVS_OK;
+    a.q.cold = make_int2(0, nst);                                     // every frame runs the whole table
+    return run_lanes(ctx, a, s->joint_weights, cfg, nst, stats, st);
 }
 
 // mvs_fit_stream: the stage groups of run_fit, each over all F frames before the next starts
 static int run_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
                       const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, cudaStream_t st) {
-    if (n_stages > 64) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: at most 64 stages");
-    std::vector<LossParams> lps(n_stages);
-    for (int i = 0; i < n_stages; ++i) {
-        const int rc = make_loss_params(ctx, &stage_cfgs[i], &lps[i]);
-        if (rc) return rc;
-        lps[i].j3d_on = s->gt_xyz ? 1 : 0;          // the stream's own targets, never the context's
-    }
-    const int H = opt_cfg->history_size > 0 ? opt_cfg->history_size : 100;
+    const int H = history_size(opt_cfg);
+    std::vector<LossParams> lps;
     std::vector<int> ends;
-    bool any_dense = false, any_resident = false;
-    for (int i = 0; i < n_stages; i = ends.back()) {
-        const Regime rg = stage_regime(ctx, lps[i], H, false);
-        if (rg == kBatched)
-            return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_stream: stage %d would run in the batched reference chain (exec "
-                                                       "mode 1, history_size > 100 without the SDF term, or a model the "
-                                                       "frame-resident and dense kernels do not take), which has no frame stream", i);
-        (rg == kDense ? any_dense : any_resident) = true;
-        ends.push_back(stage_group_end(ctx, lps, i, H, kMaxStages));
-    }
-    int rc = ensure_stream_state(ctx, any_resident ? s->n_frames : 0);
+    int rc = stage_table(ctx, "mvs_fit_stream", n_stages, stage_cfgs, s->gt_xyz ? 1 : 0, &lps);
+    if (!rc) rc = stream_runs(ctx, "mvs_fit_stream", lps, H, kMaxStages, &ends);
     if (rc) return rc;
-    if (any_dense) {
-        Workspace& w = ctx->ws;
-        if ((rc = ensure_keypoint_ws(ctx))) return rc;
-        if (s->gt_xyz && !w.j3d_xyz) {
-            const size_t n = (size_t)w.B * ctx->m.K;
-            if ((rc = dev_alloc(ctx, &w.j3d_xyz, n * 3))) return rc;
-            if ((rc = dev_alloc(ctx, &w.j3d_conf, n))) return rc;
-        }
-    }
+    bool any_dense = false, any_resident = false;
+    for (int i = 0, g = 0; i < n_stages; i = ends[g++]) (stage_regime(ctx, lps[i], H, false) == kDense ? any_dense : any_resident) = true;
+    rc = ensure_stream_state(ctx, any_resident ? s->n_frames : 0);
+    if (!rc && any_dense) rc = ensure_lane_rows(ctx, s->gt_xyz != nullptr);
+    if (rc) return rc;
     // the dense groups overwrite the lanes' keypoint and 3-D target rows: from here on the context holds neither
     ctx->have_kp = false;
     ctx->j3d_enabled = false;
@@ -952,58 +915,27 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
     int rc = begin_run(ctx, c, false, tab.data(), nst, &cfg, st);
     if (rc) return rc;
     LbfgsState& S = *ctx->lbfgs;
-    Workspace& w = ctx->ws;
-    const int B = w.B, K = ctx->m.K;
-    long long* th = reinterpret_cast<long long*>(S.na_host) + 1;      // [0..3] totals, [4] rounds of a dense run
     SeqChain q = q0;
     q.final_loss = s->final_loss;
     q.totals = S.totals;
     if (rg == kResident) {
         // one launch, one CTA per sequence; rounds: the largest number of evaluations one CTA ran (its frames' sum)
+        long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
         const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d};
         if ((rc = launch_lbfgs_resident_seq(ctx, s->params, cfg, cfg.history, S.lp_tab, tab.data(), nst, in, q, st))) return rc;
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
         MVS_CUDA_OK(ctx, cudaGetLastError());
-        if (stats) {
-            stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
-            stats->rounds += (int)th[3];
-        }
+        add_totals(stats, th, th[3], false);
         return MVS_OK;
     }
-    // dense rounds over B lanes fed from the queue of sequences
-    StreamState& ss = *ctx->fstream;
-    if ((rc = frame_step_begin_run(ctx, st))) return rc;
-    SeqArgs a;
-    StreamArgs& f = a.f;
-    f.F = F; f.B = B; f.V = ctx->cams.num_views; f.K = K; f.nstages = nst;
-    f.params = s->params; f.final_loss = s->final_loss; f.gt_uv = s->gt_uv; f.conf = s->conf;
-    f.j3d_xyz = gt_xyz; f.j3d_conf = conf3d;
-    f.ws_gt_uv = w.gt_uv; f.ws_conf = w.conf; f.ws_j3d_xyz = w.j3d_xyz; f.ws_j3d_conf = w.j3d_conf;
-    f.lane_frame = ss.lane_frame; f.lane_start = ss.lane_start; f.lane_params = ss.lane_params; f.queue = ss.queue;
-    f.end_round = ss.end_round; f.pose_valid = w.pose_valid;
+    LaneArgs a{};
+    a.F = F; a.n_queue = q.n_act;
+    a.params = s->params; a.final_loss = s->final_loss; a.gt_uv = s->gt_uv; a.conf = s->conf;
+    a.j3d_xyz = gt_xyz; a.j3d_conf = conf3d;
     a.q = q;
     a.lane_seq = ctx->sstream->lane_seq;
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(w.joint_w, s->joint_weights, (size_t)K * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.lane_frame, 0xff, (size_t)B * sizeof(int), st));
-    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.queue, 0, sizeof(int), st));
-    MVS_CUDA_OK(ctx, cudaMemsetAsync(ss.end_round, 0, sizeof(long long), st));
-    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, seq_refill_kernel<<<1, 1024, 0, st>>>(S, a, 0, 0));
-    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
-    if ((rc = run_dense(ctx, ss.lane_params, cfg, nst, st, &a.f, &a))) return rc;
-    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, seq_refill_kernel<<<1, 1024, 0, st>>>(S, a, 0, 1));
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 3 * sizeof(long long), cudaMemcpyDeviceToHost, st));
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th + 4, ss.end_round, sizeof(long long), cudaMemcpyDeviceToHost, st));
-    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    MVS_CUDA_OK(ctx, cudaGetLastError());
-    if (stats) {
-        stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
-        stats->rounds += (int)th[4];
-        stats->dense_frame_evals += th[1]; stats->dense_rounds += (int)th[4];
-    }
-    return MVS_OK;
+    return run_lanes(ctx, a, s->joint_weights, cfg, nst, stats, st);
 }
 
 // mvs_fit_seq_stream (DESIGN.md section 4).  Stages are grouped into runs as mvs_fit_seq groups them; run c holds stages
@@ -1015,42 +947,27 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
 static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int n_stages,
                           const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
                           cudaStream_t st) {
-    constexpr int kWarmSkip = 2;                                      // as run_fit
-    if (n_stages > 64) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: at most 64 stages");
     const int NS = s->n_sequences;
     const std::vector<int> off(s->seq_offsets, s->seq_offsets + NS + 1);
     const int F = off[NS];
-    std::vector<LossParams> lps(n_stages), wlps;
+    const int j3d = gt_xyz ? 1 : 0;                                   // the call's own targets, never the context's
+    std::vector<LossParams> lps, wlps;
+    int rc = stage_table(ctx, "mvs_fit_seq_stream", n_stages, stage_cfgs, j3d, &lps);
+    if (rc) return rc;
     int n_vp2 = 0;
-    for (int i = 0; i < n_stages; ++i) {
-        const int rc = make_loss_params(ctx, &stage_cfgs[i], &lps[i]);
-        if (rc) return rc;
-        lps[i].j3d_on = gt_xyz ? 1 : 0;             // the call's own targets, never the context's
-        n_vp2 += lps[i].use_vposer == 2;
-    }
+    for (const LossParams& lp : lps) n_vp2 += lp.use_vposer == 2;
     if (n_vp2 > 0 && n_vp2 < n_stages)
         return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: stages mix latent-code (use_vposer = 2) and axis-angle poses");
-    wlps = lps;
-    {
-        mvs_loss_config wc = stage_cfgs[kWarmSkip];
-        wc.body_pose_weight *= 0.15f;
-        const int rc = make_loss_params(ctx, &wc, &wlps[kWarmSkip]);
-        if (rc) return rc;
-        wlps[kWarmSkip].j3d_on = gt_xyz ? 1 : 0;
-    }
-    const int H = opt_cfg->history_size > 0 ? opt_cfg->history_size : 100;
+    if ((rc = warm_stage_table(ctx, stage_cfgs, j3d, lps, &wlps))) return rc;
+    const int H = history_size(opt_cfg);
     std::vector<int> ends;
+    if ((rc = stream_runs(ctx, "mvs_fit_seq_stream", lps, H, kMaxStages / 2, &ends))) return rc;
     int c = -1, ic = 0;
     bool any_dense = false, resident_before = false;
-    for (int i = 0; i < n_stages; i = ends.back()) {
+    for (int i = 0, g = 0; i < n_stages; i = ends[g++]) {
         const Regime rg = stage_regime(ctx, lps[i], H, false);
-        if (rg == kBatched)
-            return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_seq_stream: stage %d would run in the batched reference chain (exec "
-                                                       "mode 1, history_size > 100 without the SDF term, or a model the "
-                                                       "frame-resident and dense kernels do not take), which has no stream", i);
-        ends.push_back(stage_group_end(ctx, lps, i, H, kMaxStages / 2));
         any_dense |= rg == kDense;
-        if (i <= kWarmSkip && kWarmSkip < ends.back()) { c = (int)ends.size() - 1; ic = i; }
+        if (i <= kWarmSkip && kWarmSkip < ends[g]) { c = g; ic = i; }
         else if (c < 0) resident_before |= rg == kResident;
     }
     if (ends[c] != n_stages)
@@ -1069,13 +986,9 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
     q.keep_pose = n_vp2 == 0 ? 1 : 0;
     // a frame's packed row: params | gt_uv | conf, then gt_xyz | conf3d with the 3-D term
     const size_t row_floats = kParams + (size_t)ctx->cams.num_views * ctx->m.K * 3 + (gt_xyz ? (size_t)ctx->m.K * 4 : 0);
-    int rc = ensure_stream_state(ctx, resident_before ? NS : 0);
+    rc = ensure_stream_state(ctx, resident_before ? NS : 0);
     if (!rc) rc = ensure_seq_state(ctx, NS, c > 0 ? row_floats * NS : 0);
-    if (!rc && any_dense) rc = ensure_keypoint_ws(ctx);
-    if (!rc && any_dense && gt_xyz && !ctx->ws.j3d_xyz) {           // the lanes' 3-D rows, as run_stream allocates them
-        const size_t n = (size_t)ctx->ws.B * ctx->m.K;
-        if (!(rc = dev_alloc(ctx, &ctx->ws.j3d_xyz, n * 3))) rc = dev_alloc(ctx, &ctx->ws.j3d_conf, n);
-    }
+    if (!rc && any_dense) rc = ensure_lane_rows(ctx, gt_xyz != nullptr);
     if (rc) return rc;
     SeqState& ss = *ctx->sstream;
     q.off = ss.off;
@@ -1252,7 +1165,7 @@ int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, cons
     int rc = mvs_set_keypoints(ctx, gt_uv_host, conf_host, joint_weights_host, 0, stream);
     if (rc) return rc;
     {
-        const int H = opt_cfg->history_size > 0 ? opt_cfg->history_size : 100;
+        const int H = history_size(opt_cfg);
         if (H > 128) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_host: history_size must be <= 128");
         rc = ensure_state(ctx, H);
         if (rc) return rc;

@@ -25,6 +25,38 @@ struct FrameScalars {
     long long iters, evals;
 };
 
+// A frame starting on its slice rng = [first, end) of the stage table, with a fresh optimiser
+__device__ __forceinline__ FrameScalars fresh_frame_scalars(int2 rng) {
+    FrameScalars s;
+    memset(&s, 0, sizeof(s));
+    s.phase = PH_STEP_ENTRY;
+    s.H_diag = 1.f;
+    s.final_loss = __int_as_float(0x7fc00000);
+    s.stage = rng.x; s.stage_end = rng.y;
+    return s;
+}
+
+// A frame that finished stage k of a multi-stage run starts stage k + 1 at once, with a fresh optimiser (the reference
+// builds one optimiser per stage, fitting.py / fit_single_frame) and the parameters it has: frames are independent
+// problems, so nothing makes a fast frame wait for the slowest one at a stage boundary.
+__device__ __forceinline__ void next_stage_scalars(FrameScalars& s) {
+    const long long it = s.iters, ev = s.evals;
+    const int st = s.stage + 1, nacc = s.nan_acc + s.nan_flag, end = s.stage_end;
+    memset(&s, 0, sizeof(s));
+    s.stage_end = end;
+    s.H_diag = 1.f;
+    s.phase = PH_STEP_ENTRY;
+    s.final_loss = __int_as_float(0x7fc00000);
+    s.iters = it; s.evals = ev; s.stage = st; s.nan_acc = nacc;
+}
+
+// A retiring frame's iterations, evaluations and NaN / Inf stops, added to totals[0 .. 2]
+__device__ __forceinline__ void add_frame_totals(long long* totals, const FrameScalars& s) {
+    atomicAdd((unsigned long long*)&totals[0], (unsigned long long)s.iters);
+    atomicAdd((unsigned long long*)&totals[1], (unsigned long long)s.evals);
+    atomicAdd((unsigned long long*)&totals[2], (unsigned long long)(s.nan_flag + s.nan_acc));
+}
+
 struct LbfgsState {
     int B = 0, H = 0;
     float *g = nullptr, *d = nullptr, *prev_g = nullptr, *x_init = nullptr, *g_prev = nullptr, *bg = nullptr;

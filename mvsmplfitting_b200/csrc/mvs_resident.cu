@@ -119,15 +119,7 @@ lbfgs_resident_kernel(ResidentModel m, CamSet cams, const LossParams* __restrict
     }
     resident_setup(S, m);
     for (int i = t; i < kParams; i += kResThreads) { const float v = params[(size_t)b * kParams + i]; S.lx[i] = v; S.lx_eval[i] = v; }
-    if (t == 0) {
-        FrameScalars s;
-        memset(&s, 0, sizeof(s));
-        s.phase = PH_STEP_ENTRY;
-        s.H_diag = 1.f;
-        s.final_loss = __int_as_float(0x7fc00000);
-        s.stage = st_begin; s.stage_end = st_end;
-        S.fs = s;
-    }
+    if (t == 0) S.fs = fresh_frame_scalars(make_int2(st_begin, st_end));
     if (t < (int)(sizeof(LossParams) / 4)) reinterpret_cast<int*>(&S.lp)[t] = reinterpret_cast<const int*>(&lp_tab[st_begin])[t];
     __syncthreads();
     LbfgsPtrs P{S.lx, S.lg, S.ld, S.lprev_g, S.lx_init, S.lg_prev, S.lbg0, S.lbg1, hy, hs, S.ro, S.al, S.lx_eval, S.lg_new, H,
@@ -198,15 +190,7 @@ lbfgs_resident_seq_kernel(ResidentModel m, CamSet cams, const LossParams* __rest
                 S.gram, S.tl_scratch};
     const long long eval_cap = (long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8;
     while (true) {                                                       // frames of the sequence
-        if (t == 0) {
-            FrameScalars s;
-            memset(&s, 0, sizeof(s));
-            s.phase = PH_STEP_ENTRY;
-            s.H_diag = 1.f;
-            s.final_loss = __int_as_float(0x7fc00000);
-            s.stage = rng.x; s.stage_end = rng.y;
-            S.fs = s;
-        }
+        if (t == 0) S.fs = fresh_frame_scalars(rng);
         if (t < (int)(sizeof(LossParams) / 4)) reinterpret_cast<int*>(&S.lp)[t] = reinterpret_cast<const int*>(&lp_tab[rng.x])[t];
         __syncthreads();
         long long stage_ev0 = 0;
@@ -240,9 +224,7 @@ lbfgs_resident_seq_kernel(ResidentModel m, CamSet cams, const LossParams* __rest
         seq_evals += s.evals;
         if (t == 0) {                                                    // the frame's totals, as lbfgs_finalize_kernel counts them
             if (q.final_loss) q.final_loss[b] = s.final_loss;
-            atomicAdd((unsigned long long*)&q.totals[0], (unsigned long long)s.iters);
-            atomicAdd((unsigned long long*)&q.totals[1], (unsigned long long)s.evals);
-            atomicAdd((unsigned long long*)&q.totals[2], (unsigned long long)(s.nan_flag + s.nan_acc));
+            add_frame_totals(q.totals, s);
         }
         const int nx = b + 1;
         const bool more = nx < seq_end, warm = more && s.final_loss <= q.reinit_loss;   // NaN is not <= reinit_loss

@@ -836,20 +836,6 @@ __device__ __forceinline__ void resident_setup(ResidentSmem& S, const ResidentMo
         }
 }
 
-// A frame that finished stage k of a multi-stage run starts stage k + 1 at once, with a fresh optimiser (the reference
-// builds one optimiser per stage, fitting.py / fit_single_frame) and the parameters it has: frames are independent
-// problems, so nothing makes a fast frame wait for the slowest one at a stage boundary.
-__device__ __forceinline__ void next_stage_scalars(FrameScalars& s) {
-    const long long it = s.iters, ev = s.evals;
-    const int st = s.stage + 1, nacc = s.nan_acc + s.nan_flag, end = s.stage_end;
-    memset(&s, 0, sizeof(s));
-    s.stage_end = end;
-    s.H_diag = 1.f;
-    s.phase = PH_STEP_ENTRY;
-    s.final_loss = __int_as_float(0x7fc00000);
-    s.iters = it; s.evals = ev; s.stage = st; s.nan_acc = nacc;
-}
-
 // Pose forward of the trial point in S.x for the dense kernels of the next round: feature row (fp32 and TF32), skinning
 // transforms (frame fastest), translation -- all addressed by the slot -- and the per-frame pose cache.  With vp2 the
 // body pose is decoded from the latent code first.  All threads; no trailing barrier.
