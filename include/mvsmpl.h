@@ -88,13 +88,33 @@ int mvs_set_vposer(mvs_ctx* ctx, const float* fc1_w, const float* fc1_b, const f
 int mvs_vposer_decode(mvs_ctx* ctx, const float* params_dev, float* body_pose_dev, void* stream);
 
 /* PerspectiveCamera list (code/camera.py:41-117, built in code/init.py:108-131): host arrays
- * R [V,3,3], t [V,3], f [V,2] (focal x,y), c [V,2] */
+ * R [V,3,3], t [V,3], f [V,2] (focal x,y), c [V,2].  The same as mvs_set_camera_rigs with one rig of scale 1. */
 int mvs_set_cameras(mvs_ctx* ctx, int num_views, const float* R, const float* t, const float* f, const float* c);
+
+/* ---- camera rigs: the frames of one context may come from different camera setups (the reference runs one camera file per
+ *      run, code/init.py cam_param).  A rig is num_views[r] <= 16 views plus a data-weight scale s_r.  A frame with rig r is
+ *      evaluated exactly as in a context whose only cameras are rig r's and whose stage configurations have
+ *      data_weight = fl32(data_weight * s_r): s_r scales the data weight of the 2-D term and of the 3-D joint term (e.g. the
+ *      reference's 500 / H for rigs of different image heights).  A scale of 1 is exact.
+ *      Host arrays padded to Vmax = max num_views: R [n_rigs,Vmax,3,3], t [n_rigs,Vmax,3], f and c [n_rigs,Vmax,2] (rows
+ *      v >= num_views[r] are not read); data_weight_scale [n_rigs] (finite, > 0) or NULL = all 1.  Replaces the previous rigs
+ *      or cameras (waits for the device first); keypoints and per-slot rigs must be set again.  Every detection array of the
+ *      context has Vmax view rows; rows v >= V_r of a frame with rig r are never read, and closure projections of those rows
+ *      are left untouched. */
+int mvs_set_camera_rigs(mvs_ctx* ctx, int n_rigs, const int* num_views, const float* R, const float* t, const float* f,
+                        const float* c, const float* data_weight_scale);
+
+/* The rig of every slot of the batch: rig_host [B] (HOST ints in [0, n_rigs)), validated and copied before return (waits for
+ *      the device first).  Read by mvs_closure, mvs_lbfgs_run, mvs_lbfgs_step, mvs_fit, mvs_fit_seq, mvs_fit_host and
+ *      mvs_init_guess.  With more than one rig, those entry points return MVS_ERR_INVALID unless per-slot rigs were given
+ *      since the last mvs_set_batch, mvs_set_camera_rigs / mvs_set_cameras or stream call; with one rig every slot has rig 0
+ *      unless told otherwise. */
+int mvs_set_frame_rigs(mvs_ctx* ctx, const int* rig_host);
 
 /* frames in flight (the reference is fixed to 1: code/utils/non_linear_solver.py:56); allocates workspace */
 int mvs_set_batch(mvs_ctx* ctx, int num_frames);
 
-/* 2-D detections: gt_uv [V,B,K,2], conf [V,B,K], joint_weights [K]
+/* 2-D detections: gt_uv [V,B,K,2], conf [V,B,K], joint_weights [K] (V = the rigs' largest view count)
  * (code/utils/non_linear_solver.py:77-101).  on_device != 0: device pointers (copied D2D on `stream`),
  * else host pointers (copied before return). */
 int mvs_set_keypoints(mvs_ctx* ctx, const float* gt_uv, const float* conf, const float* joint_weights,
@@ -242,6 +262,17 @@ typedef struct {
 int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
                    const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream);
 
+/* ---- mvs_fit_stream with a rig per frame (mvs_set_camera_rigs): rig_dev [F] (device ints) names each frame's rig; every frame
+ *      gets the bits mvs_fit gives it in a context whose only cameras are its rig's.  The indices are checked on the device
+ *      before any fitting work: one out of [0, n_rigs) returns MVS_ERR_INVALID naming the first such frame.  rig_dev = NULL:
+ *      every frame has rig 0, allowed with one rig only (MVS_ERR_INVALID otherwise); mvs_fit_stream is this call with NULL.
+ *      Context state afterwards as after mvs_fit_stream, and no per-slot rigs either (the lanes' rig rows were overwritten
+ *      with the keypoints): mvs_set_frame_rigs again before a batch entry point of a context with several rigs.
+ *      Synchronises. */
+int mvs_fit_stream_rigs(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig_dev, int n_stages,
+                        const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
+                        void* stream);
+
 /* ---- mvs_fit_seq over S video sequences of any number and length through the context's B slots (is_seq, code/main.py:76-79).
  *      Sequence s owns frames [seq_offsets[s], seq_offsets[s+1]) of the F-frame arrays, in time order.  Every frame gets
  *      exactly the parameters and final loss that mvs_fit_seq gives it when frame t of every sequence is fitted as one batch
@@ -290,6 +321,16 @@ int mvs_fit_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages,
 int mvs_fit_seq_stream3d(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int n_stages,
                          const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
                          void* stream);
+
+/* ---- mvs_fit_seq_stream3d with a rig per frame: rig_dev [F] (device ints, rows in the order of the frames of s) names each
+ *      frame's rig; the frames of one sequence may change rig.  Every frame gets the bits mvs_fit_seq gives it in a batch of S
+ *      (frame t of every sequence) with mvs_set_frame_rigs naming each slot's rig; a warm frame starts from its predecessor's
+ *      result whatever rig either has.  Checked on the device first: an index out of [0, n_rigs) returns MVS_ERR_INVALID
+ *      naming the first such frame.  rig_dev = NULL: every frame has rig 0, one rig only; mvs_fit_seq_stream3d and
+ *      mvs_fit_seq_stream are this call with NULL.  Context state afterwards as after mvs_fit_stream_rigs.  Synchronises. */
+int mvs_fit_seq_stream_rigs(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
+                            const int* rig_dev, int n_stages, const mvs_loss_config* stage_cfgs,
+                            const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream);
 
 /* ---- host-buffer entry point (what a caller without device memory uses): copies keypoints and
  *      parameters host->device, runs `n_stages` optimisation stages (one mvs_loss_config each, the weight

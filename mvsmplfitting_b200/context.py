@@ -51,7 +51,8 @@ class FittingContext:
         _lib.check(None, self.lib.mvs_create(self.device.index, ctypes.byref(h)), "mvs_create")
         self.h = h
         self.B = 0
-        self.V = 0
+        self.V = 0                        # view rows of every detection array: the rigs' largest view count
+        self.rig_views = []               # view count of each camera rig
         self.K = 17
         self.N = 0
         self._loss_cfg = None
@@ -134,6 +135,36 @@ class FittingContext:
         R, t, f, c = _f32(R), _f32(t), _f32(f), _f32(c)
         self.V = R.shape[0]
         _lib.check(self.h, self.lib.mvs_set_cameras(self.h, self.V, _ptr(R), _ptr(t), _ptr(f), _ptr(c)), "mvs_set_cameras")
+        self.rig_views = [self.V]
+
+    def set_camera_rigs(self, rigs, data_weight_scale=None):
+        """A table of camera rigs (mvs_set_camera_rigs): rigs is a list of dict(R [V_r,3,3], t [V_r,3], f [V_r,2], c [V_r,2])
+        such as seqio.camera_arrays returns; data_weight_scale [n_rigs] multiplies every stage's data_weight for the frames
+        of each rig (None: all 1).  Detection arrays then have V = max V_r view rows; rows v >= V_r of a frame with rig r are
+        not read.  Name each slot's rig with set_frame_rigs, or each frame's with fit_stream / fit_seq_stream(rig=...)."""
+        if not rigs:
+            raise ValueError("set_camera_rigs: want at least one rig")
+        nv = [int(np.asarray(r["R"]).shape[0]) for r in rigs]
+        V = max(nv)
+        pad = lambda a, n, shape: np.concatenate([_f32(a), np.zeros((V - n,) + shape, np.float32)]) if n < V else _f32(a)
+        R = _f32(np.stack([pad(r["R"], n, (3, 3)) for r, n in zip(rigs, nv)]))
+        t = _f32(np.stack([pad(r["t"], n, (3,)) for r, n in zip(rigs, nv)]))
+        f = _f32(np.stack([pad(r["f"], n, (2,)) for r, n in zip(rigs, nv)]))
+        c = _f32(np.stack([pad(r["c"], n, (2,)) for r, n in zip(rigs, nv)]))
+        scale = None if data_weight_scale is None else _f32(np.reshape(data_weight_scale, -1))
+        if scale is not None and scale.shape[0] != len(rigs):
+            raise ValueError("set_camera_rigs: %d rigs, %d data-weight scales" % (len(rigs), scale.shape[0]))
+        nva = _i32(nv)
+        _lib.check(self.h, self.lib.mvs_set_camera_rigs(self.h, len(rigs), _ptr(nva), _ptr(R), _ptr(t), _ptr(f), _ptr(c),
+                                                        _ptr(scale)), "mvs_set_camera_rigs")
+        self.V, self.rig_views = V, nv
+
+    def set_frame_rigs(self, rig):
+        """the rig of every slot of the batch (mvs_set_frame_rigs): rig [B] ints in [0, n_rigs)"""
+        r = _i32(np.reshape(rig, -1))
+        if r.shape[0] != self.B:
+            raise ValueError("set_frame_rigs: want %d rig indices, got %d" % (self.B, r.shape[0]))
+        _lib.check(self.h, self.lib.mvs_set_frame_rigs(self.h, _ptr(r)), "mvs_set_frame_rigs")
 
     def set_batch(self, B: int):
         _lib.check(self.h, self.lib.mvs_set_batch(self.h, int(B)), "mvs_set_batch")
@@ -284,36 +315,53 @@ class FittingContext:
                              % (who, F, self.K, F, self.K, tuple(j3.shape), tuple(c3.shape)))
         return gt_uv, conf, jw, j3, c3
 
+    def _stream_rigs(self, who, F, rig):
+        """a stream's per-frame rig indices [F] on the device (int32), or None"""
+        if rig is None:
+            return None
+        r = torch.as_tensor(np.asarray(rig.cpu() if isinstance(rig, torch.Tensor) else rig).astype(np.int32).reshape(-1))
+        if r.shape[0] != F:
+            raise ValueError("%s: want %d rig indices, got %d" % (who, F, r.shape[0]))
+        return r.to(self.device).contiguous()
+
     def fit_stream(self, params: torch.Tensor, gt_uv, conf, joint_weights, stage_cfgs, opt_cfg=None, joints3d=None,
-                   conf3d=None):
+                   conf3d=None, rig=None):
         """mvs_fit over F frames of any number through the context's B slots (mvs_fit_stream): params [F,86] CUDA float32,
         updated in place; gt_uv [V,F,K,2], conf [V,F,K], joint_weights [K] (numpy or tensors); joints3d [F,K,3] with conf3d
-        [F,K] switch the 3-D joint term on for this call.  Every frame gets the bits mvs_fit gives it.  Afterwards the context
-        holds no keypoints and no 3-D targets (set_keypoints / set_joints3d again before a closure or fit).
-        Returns (final_loss [F], stats)."""
+        [F,K] switch the 3-D joint term on for this call.  rig [F] (mvs_fit_stream_rigs) names each frame's camera rig
+        (set_camera_rigs; None: rig 0, one rig only).  Every frame gets the bits mvs_fit gives it.  Afterwards the context
+        holds no keypoints, no 3-D targets and no per-slot rigs (set_keypoints / set_joints3d / set_frame_rigs again before a
+        closure or fit).  Returns (final_loss [F], stats)."""
         assert params.is_cuda and params.dtype == torch.float32 and params.is_contiguous() and params.dim() == 2
         F = params.shape[0]
         gt_uv, conf, jw, j3, c3 = self._stream_rows("fit_stream", F, gt_uv, conf, joint_weights, joints3d, conf3d)
+        rg = self._stream_rigs("fit_stream", F, rig)
         final = torch.empty(F, dtype=torch.float32, device=self.device)
         s = _lib.FrameStream(F, _ptr(params), _ptr(gt_uv), _ptr(conf), _ptr(jw), _ptr(j3), _ptr(c3), _ptr(final))
         arr = (_lib.LossConfig * len(stage_cfgs))(*stage_cfgs)
         cfg = opt_cfg or self.make_lbfgs_config()
         st = _lib.LbfgsStats()
         self._j3d_keep = None
-        _lib.check(self.h, self.lib.mvs_fit_stream(self.h, ctypes.byref(s), len(stage_cfgs), arr, ctypes.byref(cfg),
-                                                   ctypes.byref(st), self._stream()), "mvs_fit_stream")
+        if rg is None:
+            _lib.check(self.h, self.lib.mvs_fit_stream(self.h, ctypes.byref(s), len(stage_cfgs), arr, ctypes.byref(cfg),
+                                                       ctypes.byref(st), self._stream()), "mvs_fit_stream")
+        else:
+            _lib.check(self.h, self.lib.mvs_fit_stream_rigs(self.h, ctypes.byref(s), _ptr(rg), len(stage_cfgs), arr,
+                                                            ctypes.byref(cfg), ctypes.byref(st), self._stream()),
+                       "mvs_fit_stream_rigs")
         return final, _stats_dict(st)
 
     def fit_seq_stream(self, params: torch.Tensor, gt_uv, conf, joint_weights, lengths, stage_cfgs, opt_cfg=None,
-                       reinit_loss: float = 5000.0, joints3d=None, conf3d=None):
+                       reinit_loss: float = 5000.0, joints3d=None, conf3d=None, rig=None):
         """mvs_fit_seq over S video sequences through the context's B slots (mvs_fit_seq_stream): the frames of sequence s are
         the next lengths[s] rows, in time order.  params [F,86] CUDA float32 holds every frame's cold start point (init_guess)
         and is updated in place; gt_uv [V,F,K,2], conf [V,F,K], joint_weights [K] (numpy or tensors).  A frame after the first
         starts from its predecessor's result while that frame's final loss is <= reinit_loss (skipping stages 0 and 1), from
         its own row otherwise.  joints3d [F,K,3] with conf3d [F,K] switch the 3-D joint term on for every frame of the call
-        (mvs_fit_seq_stream3d; zero-confidence rows for frames without annotations).  Every frame gets the bits
-        seqio.fit_sequences gives it with a batch of S.  Afterwards the context holds no keypoints and no 3-D targets.
-        Returns (final_loss [F], stats)."""
+        (mvs_fit_seq_stream3d; zero-confidence rows for frames without annotations).  rig [F] (mvs_fit_seq_stream_rigs)
+        names each frame's camera rig (set_camera_rigs; None: rig 0, one rig only).  Every frame gets the bits
+        seqio.fit_sequences gives it with a batch of S.  Afterwards the context holds no keypoints, no 3-D targets and no
+        per-slot rigs.  Returns (final_loss [F], stats)."""
         assert params.is_cuda and params.dtype == torch.float32 and params.is_contiguous() and params.dim() == 2
         F = params.shape[0]
         lengths = [int(n) for n in lengths]
@@ -321,6 +369,7 @@ class FittingContext:
             raise ValueError("fit_seq_stream: want sequence lengths >= 1 that add up to %d frames, got %s" % (F, lengths))
         off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(lengths)]), dtype=np.int32)
         gt_uv, conf, jw, j3, c3 = self._stream_rows("fit_seq_stream", F, gt_uv, conf, joint_weights, joints3d, conf3d)
+        rg = self._stream_rigs("fit_seq_stream", F, rig)
         final = torch.empty(F, dtype=torch.float32, device=self.device)
         s = _lib.SequenceStream(len(lengths), _ptr(off), _ptr(params), _ptr(gt_uv), _ptr(conf), _ptr(jw), _ptr(final),
                                 float(reinit_loss))
@@ -328,7 +377,11 @@ class FittingContext:
         cfg = opt_cfg or self.make_lbfgs_config()
         st = _lib.LbfgsStats()
         self._j3d_keep = None
-        if j3 is None:
+        if rg is not None:
+            _lib.check(self.h, self.lib.mvs_fit_seq_stream_rigs(self.h, ctypes.byref(s), _ptr(j3), _ptr(c3), _ptr(rg),
+                                                                len(stage_cfgs), arr, ctypes.byref(cfg), ctypes.byref(st),
+                                                                self._stream()), "mvs_fit_seq_stream_rigs")
+        elif j3 is None:
             _lib.check(self.h, self.lib.mvs_fit_seq_stream(self.h, ctypes.byref(s), len(stage_cfgs), arr, ctypes.byref(cfg),
                                                            ctypes.byref(st), self._stream()), "mvs_fit_seq_stream")
         else:

@@ -95,7 +95,7 @@ int make_loss_params(mvs_ctx* ctx, const mvs_loss_config* c, LossParams* out) {
 
 int ensure_keypoint_ws(mvs_ctx* ctx) {
     Workspace& w = ctx->ws;
-    const int V = ctx->cams.num_views;
+    const int V = ctx->vmax;
     if (w.gt_uv && w.kp_views == V) return MVS_OK;
     const size_t n = (size_t)V * w.B * ctx->m.K;
     int rc;
@@ -103,6 +103,35 @@ int ensure_keypoint_ws(mvs_ctx* ctx) {
     if ((rc = dev_alloc(ctx, &w.conf, n))) return rc;
     if (!w.joint_w && (rc = dev_alloc(ctx, &w.joint_w, kMaxKeypoints))) return rc;
     w.kp_views = V;
+    return MVS_OK;
+}
+
+int batch_rigs(mvs_ctx* ctx, const char* who) {
+    if (ctx->rigs.size() > 1 && !ctx->slot_rigs)
+        return set_error(ctx, MVS_ERR_INVALID, "%s: the context has %d camera rigs and no per-slot rigs were given since the last "
+                                               "mvs_set_batch, mvs_set_camera_rigs or stream call (mvs_set_frame_rigs)",
+                         who, (int)ctx->rigs.size());
+    return MVS_OK;
+}
+
+__global__ void rig_check_kernel(const int* __restrict__ rig, int n, int n_rigs, int* __restrict__ first_bad) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && (unsigned)rig[i] >= (unsigned)n_rigs) atomicMin(first_bad, i);
+}
+
+int check_frame_rigs(mvs_ctx* ctx, const char* who, const int* rig_dev, int n, cudaStream_t st) {
+    int rc;
+    if (!ctx->rig_bad && (rc = dev_alloc(ctx, &ctx->rig_bad, 1))) return rc;
+    MVS_CUDA_OK(ctx, cudaMemsetAsync(ctx->rig_bad, 0x7f, sizeof(int), st));         // 0x7f7f7f7f: no bad frame
+    MVS_LAUNCH(ctx, KID_MISC, st, rig_check_kernel<<<(n + 255) / 256, 256, 0, st>>>(rig_dev, n, (int)ctx->rigs.size(), ctx->rig_bad));
+    int bad = 0;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(&bad, ctx->rig_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    if (bad < n) {
+        int r = 0;
+        MVS_CUDA_OK(ctx, cudaMemcpy(&r, rig_dev + bad, sizeof(int), cudaMemcpyDeviceToHost));
+        return set_error(ctx, MVS_ERR_INVALID, "%s: frame %d names rig %d, the context has %d", who, bad, r, (int)ctx->rigs.size());
+    }
     return MVS_OK;
 }
 }  // namespace mvs
@@ -426,18 +455,77 @@ int mvs_set_vposer(mvs_ctx* ctx, const float* fc1_w, const float* fc1_b, const f
     return MVS_OK;
 }
 
+int mvs_set_camera_rigs(mvs_ctx* ctx, int n_rigs, const int* num_views, const float* R, const float* t, const float* f,
+                        const float* c, const float* data_weight_scale) {
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    MVS_REQUIRE(ctx, n_rigs > 0 && num_views && R && t && f && c, "mvs_set_camera_rigs: need n_rigs >= 1 and the camera arrays");
+    int vmax = 0;
+    for (int r = 0; r < n_rigs; ++r) {
+        MVS_REQUIRE(ctx, num_views[r] > 0 && num_views[r] <= kMaxViews, "mvs_set_camera_rigs: rig %d has %d views (1..%d)", r,
+                    num_views[r], kMaxViews);
+        MVS_REQUIRE(ctx, !data_weight_scale || (isfinite(data_weight_scale[r]) && data_weight_scale[r] > 0.f),
+                    "mvs_set_camera_rigs: rig %d has data_weight_scale %g (want a finite positive scale)", r,
+                    data_weight_scale ? data_weight_scale[r] : 1.f);
+        vmax = std::max(vmax, num_views[r]);
+    }
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    std::vector<Rig> rigs((size_t)n_rigs);
+    for (int r = 0; r < n_rigs; ++r) {
+        Rig& g = rigs[r];
+        memset(&g, 0, sizeof(g));
+        g.num_views = num_views[r];
+        g.dw_scale = data_weight_scale ? data_weight_scale[r] : 1.f;
+        for (int v = 0; v < g.num_views; ++v) {
+            const size_t i = (size_t)r * vmax + v;           // host arrays padded to vmax views
+            memcpy(g.cam[v].R, R + 9 * i, 9 * sizeof(float));
+            memcpy(g.cam[v].t, t + 3 * i, 3 * sizeof(float));
+            memcpy(g.cam[v].f, f + 2 * i, 2 * sizeof(float));
+            memcpy(g.cam[v].c, c + 2 * i, 2 * sizeof(float));
+        }
+    }
+    // no kernel may still read the table it replaces
+    MVS_CUDA_OK(ctx, cudaDeviceSynchronize());
+    if (ctx->rigs_cap < n_rigs) {
+        if (ctx->rigs_dev) {
+            ctx->allocs.erase(std::find(ctx->allocs.begin(), ctx->allocs.end(), (void*)ctx->rigs_dev));
+            cudaFree(ctx->rigs_dev);
+            ctx->rigs_dev = nullptr;
+        }
+        ctx->rigs_cap = 0;
+        void* d = nullptr;
+        MVS_CUDA_OK(ctx, cudaMalloc(&d, (size_t)n_rigs * sizeof(Rig)));
+        ctx->allocs.push_back(d);
+        ctx->rigs_dev = static_cast<Rig*>(d);
+        ctx->rigs_cap = n_rigs;
+    }
+    MVS_CUDA_OK(ctx, cudaMemcpy(ctx->rigs_dev, rigs.data(), (size_t)n_rigs * sizeof(Rig), cudaMemcpyHostToDevice));
+    ctx->rigs = std::move(rigs);
+    ctx->vmax = vmax;
+    ctx->have_cams = true;
+    ctx->have_kp = false;                                   // keypoints are per view: must be set again
+    ctx->slot_rigs = nullptr;                               // so are the slots' rigs
+    return MVS_OK;
+}
+
 int mvs_set_cameras(mvs_ctx* ctx, int V, const float* R, const float* t, const float* f, const float* c) {
     if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
     MVS_REQUIRE(ctx, V > 0 && V <= kMaxViews && R && t && f && c, "mvs_set_cameras: need 1..%d views", kMaxViews);
-    ctx->cams.num_views = V;
-    for (int v = 0; v < V; ++v) {
-        memcpy(ctx->cams.cam[v].R, R + 9 * v, 9 * sizeof(float));
-        memcpy(ctx->cams.cam[v].t, t + 3 * v, 3 * sizeof(float));
-        memcpy(ctx->cams.cam[v].f, f + 2 * v, 2 * sizeof(float));
-        memcpy(ctx->cams.cam[v].c, c + 2 * v, 2 * sizeof(float));
-    }
-    ctx->have_cams = true;
-    ctx->have_kp = false;                                   // keypoints are per view: must be set again
+    return mvs_set_camera_rigs(ctx, 1, &V, R, t, f, c, nullptr);
+}
+
+int mvs_set_frame_rigs(mvs_ctx* ctx, const int* rig_host) {
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    MVS_REQUIRE(ctx, ctx->ws.B > 0 && ctx->have_cams, "mvs_set_frame_rigs: set cameras and batch first");
+    MVS_REQUIRE(ctx, rig_host, "mvs_set_frame_rigs: NULL array");
+    const int B = ctx->ws.B, n = (int)ctx->rigs.size();
+    for (int b = 0; b < B; ++b)
+        MVS_REQUIRE(ctx, rig_host[b] >= 0 && rig_host[b] < n, "mvs_set_frame_rigs: slot %d names rig %d, the context has %d", b,
+                    rig_host[b], n);
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    MVS_CUDA_OK(ctx, cudaDeviceSynchronize());              // no kernel may still read the rows it replaces
+    MVS_CUDA_OK(ctx, cudaMemcpy(ctx->ws.slot_rig, rig_host, (size_t)B * sizeof(int), cudaMemcpyHostToDevice));
+    ctx->slot_rig_host.assign(rig_host, rig_host + B);
+    ctx->slot_rigs = ctx->ws.slot_rig;
     return MVS_OK;
 }
 
@@ -457,6 +545,8 @@ int mvs_set_batch(mvs_ctx* ctx, int B) {
     int rc;
     if ((rc = dev_alloc(ctx, &w.fidx, B))) return rc;
     if ((rc = dev_alloc(ctx, &w.na, 1))) return rc;
+    if ((rc = dev_alloc(ctx, &w.slot_rig, B))) return rc;
+    ctx->slot_rigs = nullptr;
     if ((rc = dev_alloc(ctx, &w.Phi, (size_t)w.ldA * kFeatPad))) return rc;
     if ((rc = dev_alloc(ctx, &w.PhiTc, (size_t)2 * w.ldA * kFeatPad))) return rc;
     if ((rc = dev_alloc(ctx, &w.bboxp, (size_t)B * ((m.N + 63) / 64) * 12))) return rc;
@@ -491,7 +581,7 @@ int mvs_set_keypoints(mvs_ctx* ctx, const float* gt_uv, const float* conf, const
     MVS_REQUIRE(ctx, gt_uv && conf && joint_weights, "mvs_set_keypoints: NULL array");
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     Workspace& w = ctx->ws;
-    const size_t n = (size_t)ctx->cams.num_views * w.B * ctx->m.K;
+    const size_t n = (size_t)ctx->vmax * w.B * ctx->m.K;
     const int rc = ensure_keypoint_ws(ctx);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
@@ -563,6 +653,7 @@ int mvs_closure(mvs_ctx* ctx, const float* params_dev, float* loss_dev, float* g
     MVS_REQUIRE(ctx, ctx->have_model && ctx->have_cams && ctx->have_kp && ctx->have_loss && ctx->ws.B > 0,
                 "mvs_closure: model, cameras, batch, keypoints and loss config must be set first");
     MVS_REQUIRE(ctx, params_dev, "mvs_closure: params_dev is NULL");
+    if (int rc = batch_rigs(ctx, "mvs_closure")) return rc;
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     return evaluate_closure(ctx, params_dev, loss_dev, grad_dev, joints_dev, proj_dev, verts_dev, (cudaStream_t)stream);
 }

@@ -221,7 +221,7 @@ struct KeypointModel {
 __global__ void __launch_bounds__(kFrameThreads)
 keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, const int* __restrict__ na_ptr,
                      KeypointModel km, const float* __restrict__ verts, int nv, int dense,
-                     const float* __restrict__ gchain, CamSet cams, const float* __restrict__ gt_uv,
+                     const float* __restrict__ gchain, RigSet rigs, int with_views, const float* __restrict__ gt_uv,
                      const float* __restrict__ conf, const float* __restrict__ joint_w, int B, LossParams lp,
                      const float* __restrict__ j3d_xyz, const float* __restrict__ j3d_conf,
                      float* __restrict__ data_loss, float* __restrict__ dtransl, float* __restrict__ dv,
@@ -231,7 +231,9 @@ keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, 
     if (slot >= *na_ptr) return;
     const int b = fidx[slot];
     const int t = threadIdx.x;
-    const int K = km.K, V = cams.num_views;
+    // with_views == 0 (joints / vertices only): no rig, no detections read
+    const FrameRig rig = with_views ? frame_rig(rigs, b) : FrameRig{nullptr, 0, 1.f};
+    const int K = km.K, V = rig.num_views;                         // V: the views of this frame's rig
     __shared__ float q[kMaxKeypoints * 3];
     __shared__ float dq[kMaxKeypoints * 3];
     __shared__ float contrib[kMaxViews * kMaxKeypoints * 3];
@@ -260,11 +262,13 @@ keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, 
     }
     __syncthreads();
     const float rho2 = lp.rho * lp.rho;
-    const float dw2 = lp.data_weight * lp.data_weight;
+    const float dw = lp.data_weight * rig.dw_scale;                 // the rig's data weight (x 1: exact)
+    const float dw2 = dw * dw;
     for (int idx = t; idx < V * K; idx += blockDim.x) {
         const int v = idx / K, k = idx % K;
         float xc[3], uv[2];
-        project_fwd(cams.cam[v], &q[3 * k], xc, uv);
+        const CamF cam = rig_camera(rig, v);
+        project_fwd(cam, &q[3 * k], xc, uv);
         const size_t o = ((size_t)v * B + b) * K + k;
         if (proj_out) { proj_out[2 * o] = uv[0]; proj_out[2 * o + 1] = uv[1]; }
         float w = joint_w[k];
@@ -276,7 +280,7 @@ keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, 
         lterm[idx] = w2 * g0 + w2 * g1;
         const float duv[2] = {-(w2 * d0) * dw2, -(w2 * d1) * dw2};
         float dqv[3] = {0.f, 0.f, 0.f};
-        project_bwd(cams.cam[v], xc, duv, dqv);
+        project_bwd(cam, xc, duv, dqv);
         contrib[3 * idx] = dqv[0]; contrib[3 * idx + 1] = dqv[1]; contrib[3 * idx + 2] = dqv[2];
     }
     __syncthreads();
@@ -786,12 +790,12 @@ int launch_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* gra
         if (rc) return rc;
     }
     KeypointModel km{m.K, m.nsup, m.N, m.kp_ptr, m.kp_vidx, m.kp_spos, m.kp_w, m.kp_chain, m.sup, m.sup_ptr, m.sup_k, m.sup_w};
-    CamSet cams = ctx->cams;
     LossParams kp_lp = lp;
-    if (geometry_only) { cams.num_views = 0; kp_lp.j3d_on = 0; }      // joints / vertices only: no detections or targets read
+    if (geometry_only) kp_lp.j3d_on = 0;                    // joints / vertices only: no detections or targets read
+    const RigSet rigs = geometry_only ? RigSet{nullptr, nullptr} : slot_rig_set(ctx);     // (mvs_forward needs no cameras)
     MVS_LAUNCH(ctx, KID_KEYPOINT, st,
                keypoint_loss_kernel<<<B, kFrameThreads, 0, st>>>(x_dev, w.fidx, w.na, km, w.verts, nv, dense ? 1 : 0,
-                                                                 w.gchain, cams, w.gt_uv, w.conf, w.joint_w, B, kp_lp,
+                                                                 w.gchain, rigs, geometry_only ? 0 : 1, w.gt_uv, w.conf, w.joint_w, B, kp_lp,
                                                                  w.j3d_xyz, w.j3d_conf, w.data_loss, w.dtransl, w.dv, sdf_on ? m.nsup + m.N : m.nsup,
                                                                  w.dgchain, joints_dev, proj_dev));
     if (geometry_only) {

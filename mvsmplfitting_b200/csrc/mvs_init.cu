@@ -25,9 +25,9 @@ __global__ void init_seed_kernel(float* __restrict__ params, int B, float scale)
 }
 
 // params [B,86] (written completely), rest [K,3] rest joints of the model (the same for every frame),
-// gt_uv [V,B,K,2], conf [V,B,K]; targets [B,K,3] (3-D joint term on) or nullptr; joints3d [B,K,3] or nullptr
+// gt_uv [Vmax,B,K,2], conf [Vmax,B,K] (rows v < the frame's rig's view count are read); targets [B,K,3] (3-D joint term on) or nullptr; joints3d [B,K,3] or nullptr
 __global__ void __launch_bounds__(128) init_guess_kernel(float* __restrict__ params, const float* __restrict__ rest,
-                                                         CamSet cams, const float* __restrict__ gt_uv,
+                                                         RigSet rigs, const float* __restrict__ gt_uv,
                                                          const float* __restrict__ conf, const float* __restrict__ targets,
                                                          int B, int K, int estimate_scale,
                                                          float fixed_scale, int use_torso, float hip_seed, int as_written,
@@ -40,6 +40,7 @@ __global__ void __launch_bounds__(128) init_guess_kernel(float* __restrict__ par
     float* x = params + (size_t)b * kParams;
     for (int i = lane; i < kParams; i += 32) x[i] = 0.f;
     if (lane < K) {
+        const FrameRig cams = frame_rig(rigs, b);            // this frame's rig: its views, or one view's depth guess
         double X[3];
         if (targets) {                                    // init_guess.py:85-86: the 3-D annotations replace both guesses
             for (int c = 0; c < 3; ++c) X[c] = (double)targets[((size_t)b * K + lane) * 3 + c];
@@ -98,6 +99,7 @@ extern "C" int mvs_init_guess(mvs_ctx* ctx, float* params_dev, float* joints3d_d
     if (!(ctx->have_model && ctx->have_cams && ctx->have_kp && ctx->ws.B > 0))
         return set_error(ctx, MVS_ERR_INVALID, "mvs_init_guess: model, cameras, batch and keypoints must be set first");
     if (!params_dev || !cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_init_guess: NULL argument");
+    if (int rc = batch_rigs(ctx, "mvs_init_guess")) return rc;
     const int K = ctx->m.K, B = ctx->ws.B;
     if (cfg->use_torso && K < 13) return set_error(ctx, MVS_ERR_INVALID, "mvs_init_guess: use_torso needs keypoints 5, 6, 11, 12");
     if (!(cfg->fixed_scale > 0.f)) return set_error(ctx, MVS_ERR_INVALID, "mvs_init_guess: fixed_scale must be positive");
@@ -106,8 +108,11 @@ extern "C" int mvs_init_guess(mvs_ctx* ctx, float* params_dev, float* joints3d_d
     Workspace& w = ctx->ws;
     if (K * 3 > kParams) return set_error(ctx, MVS_ERR_INVALID, "mvs_init_guess: more than 28 keypoints");
     const bool j3d = ctx->j3d_enabled;
-    if (ctx->cams.num_views == 1 && !j3d && K < 13)
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_init_guess: the single-view depth guess needs keypoints 5, 6, 11, 12");
+    if (!j3d && K < 13)                                    // per frame: the frames whose rig has one view
+        for (int b = 0; b < B; ++b)
+            if (ctx->rigs[ctx->slot_rigs ? ctx->slot_rig_host[b] : 0].num_views == 1)
+                return set_error(ctx, MVS_ERR_INVALID, "mvs_init_guess: the single-view depth guess (frame %d) needs keypoints 5, 6, "
+                                                       "11, 12", b);
     // Rest joints (zero pose, zero shape, scale = fixed_scale; init_guess.py:29-52) are a property of the model: computed once
     // per context and scale with the library's own forward pass (seed + the 3-kernel geometry chain), then cached, so that a
     // call is ONE launch afterwards.
@@ -127,7 +132,7 @@ extern "C" int mvs_init_guess(mvs_ctx* ctx, float* params_dev, float* joints3d_d
         ctx->rest_scale = cfg->fixed_scale;
     }
     MVS_LAUNCH(ctx, KID_MISC, st,
-               init_guess_kernel<<<(B + 3) / 4, 128, 0, st>>>(params_dev, ctx->rest_joints, ctx->cams, w.gt_uv, w.conf,
+               init_guess_kernel<<<(B + 3) / 4, 128, 0, st>>>(params_dev, ctx->rest_joints, slot_rig_set(ctx), w.gt_uv, w.conf,
                                                               j3d ? w.j3d_xyz : nullptr, B, K,
                                                               cfg->estimate_scale, cfg->fixed_scale, cfg->use_torso,
                                                               ctx->loss.use_vposer == 2 ? 0.f : cfg->hip_seed,

@@ -33,10 +33,44 @@ struct ChainSched {
     unsigned char ch_ptr[kJoints + 1], ch_j[kJoints];
 };
 
-struct CamSet {
-    int num_views;
+// One camera rig of the context's table (mvs_set_camera_rigs): its views, their number and the scale of every stage's
+// data_weight for the frames that name it.  Lives in device memory; kernels reach it through frame_rig() only.
+struct __align__(16) Rig {
     CamF cam[kMaxViews];
+    int num_views;
+    float dw_scale;
+    int pad[2];
 };
+static_assert(sizeof(CamF) == 64 && sizeof(Rig) % 16 == 0, "rig layout (float4 loads of a camera)");
+
+// Where a kernel finds each frame's rig: the context's table and the rig index of every row it indexes frames by (frame of
+// a stream, slot of a batch or lane of a dense run); of == NULL: every row has rig 0 (a table of one rig).
+struct RigSet {
+    const Rig* rig;
+    const int* of;
+};
+
+// What a kernel reads of a frame's rig: the rig's cameras (device memory), view count and data-weight scale
+struct FrameRig {
+    const CamF* cam;
+    int num_views;
+    float dw_scale;
+};
+#ifdef __CUDACC__
+__device__ __forceinline__ FrameRig frame_rig(const RigSet& rs, int row) {
+    const Rig* r = rs.rig + (rs.of ? __ldg(rs.of + row) : 0);
+    return FrameRig{r->cam, __ldg(&r->num_views), __ldg(&r->dw_scale)};
+}
+// camera v of a frame's rig, into registers (four 16-byte loads)
+__device__ __forceinline__ CamF rig_camera(const FrameRig& fr, int v) {
+    const float4* p = reinterpret_cast<const float4*>(fr.cam + v);
+    CamF c;
+    float4* d = reinterpret_cast<float4*>(&c);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) d[i] = __ldg(p + i);
+    return c;
+}
+#endif
 
 // Everything a kernel needs to know about the loss (passed by value)
 struct LossParams {
@@ -109,10 +143,12 @@ struct StreamState;                   // mvs_fit_stream scratch (mvs_lbfgs.cu)
 struct SeqState;                      // mvs_fit_seq_stream scratch (mvs_lbfgs.cu)
 
 // The frames a frame-resident run fits when they are not the context's batch (mvs_fit_stream): n frames, every array with
-// row stride n (gt_uv [V][n][K][2], conf [V][n][K], j3d_xyz [n][K][3], j3d_conf [n][K]; the 3-D pair may be NULL)
+// row stride n (gt_uv [V][n][K][2], conf [V][n][K], j3d_xyz [n][K][3], j3d_conf [n][K]; the 3-D pair may be NULL; rig [n]
+// or NULL: every frame has rig 0)
 struct FrameInputs {
     int n;
     const float *gt_uv, *conf, *joint_w, *j3d_xyz, *j3d_conf;
+    const int* rig;
 };
 
 // The chaining run of mvs_fit_seq_stream (DESIGN.md section 4): a finished frame hands its slot (a CTA of the frame-resident
@@ -153,7 +189,8 @@ struct Workspace {
     float* pen_loss = nullptr;        // [B]
     float* dtransl = nullptr;         // [B][3]
     float* dgchain = nullptr;         // [B][24][3]
-    int kp_views = 0;                 // V of the allocated gt_uv / conf
+    int kp_views = 0;                 // V of the allocated gt_uv / conf (the rig table's largest view count)
+    int* slot_rig = nullptr;          // [B] rig of each slot (mvs_set_frame_rigs) or of each lane's frame (dense stream runs)
     float* gt_uv = nullptr;           // [V][B][K][2]
     float* conf = nullptr;            // [V][B][K]
     float* joint_w = nullptr;         // [K]
@@ -243,7 +280,14 @@ struct mvs_ctx {
     std::string err;
     long long launches = 0;
     mvs::DevModel m;
-    mvs::CamSet cams{};
+    // camera rigs (mvs_set_camera_rigs; mvs_set_cameras is a table of one): host copy and device table
+    std::vector<mvs::Rig> rigs;
+    mvs::Rig* rigs_dev = nullptr;
+    int rigs_cap = 0;                // rigs the device table holds
+    int vmax = 0;                    // largest view count of the table: the view rows of every detection array
+    std::vector<int> slot_rig_host;  // [B] per-slot rigs of mvs_set_frame_rigs
+    const int* slot_rigs = nullptr;  // per-slot rigs the batch entry points read (ws.slot_rig), NULL: none given (rig 0)
+    int* rig_bad = nullptr;          // [1] first frame of a stream whose rig index is out of range (check_frame_rigs)
     mvs::LossParams loss{};
     mvs::Workspace ws;
     mvs::Parents parents{};
@@ -379,7 +423,14 @@ int launch_frame_step(mvs_ctx* ctx, float* params_dev, const LbfgsState& L, cons
 int frame_step_begin_run(mvs_ctx* ctx, cudaStream_t st);                 // mvs_resident.cu
 int launch_frame_fwd_dense(mvs_ctx* ctx, const float* x_dev, const LbfgsState& L, int nstages, cudaStream_t st);   // mvs_resident.cu
 int make_loss_params(mvs_ctx* ctx, const mvs_loss_config* c, LossParams* out);      // mvs_api.cu: validation + conversion
-int ensure_keypoint_ws(mvs_ctx* ctx);          // mvs_api.cu: gt_uv / conf for the cameras' view count, joint weights
+int ensure_keypoint_ws(mvs_ctx* ctx);          // mvs_api.cu: gt_uv / conf for the rigs' largest view count, joint weights
+// mvs_api.cu: the rigs of the batch's slots (ctx->slot_rigs); MVS_ERR_INVALID when the table has several rigs and no per-slot
+// rigs were given
+int batch_rigs(mvs_ctx* ctx, const char* who);
+inline RigSet slot_rig_set(const mvs_ctx* ctx) { return RigSet{ctx->rigs_dev, ctx->slot_rigs}; }
+// mvs_api.cu: every entry of rig_dev [n] names a rig of the table; MVS_ERR_INVALID naming the first frame that does not.
+// Synchronises st.
+int check_frame_rigs(mvs_ctx* ctx, const char* who, const int* rig_dev, int n, cudaStream_t st);
 int sdf_grid_launch(mvs_ctx* ctx, float* phi, const int* faces, int num_faces, const float* verts, int batch,
                     int n_verts, int G, cudaStream_t st);
 }  // namespace mvs

@@ -156,13 +156,16 @@ struct StreamState {
 // A dense run over the lanes, fed from a queue.  A frame stream is a sequence stream in which every sequence is one frame
 // long: its frames have no successor, and queue entry k is frame k.
 struct LaneArgs {
-    int F, B, V, K;
+    int F, B, K;
     int n_queue;                        // queue entries: F (frame stream) or q.n_act (sequences of this pass)
     float* params;                      // [F][86] the call's parameters, in / out
     float* final_loss;                  // [F] or NULL
     const float *gt_uv, *conf;          // [V][F][K][2], [V][F][K]
     const float *j3d_xyz, *j3d_conf;    // [F][K][3], [F][K]; NULL: 3-D term off
+    const Rig* rigs;                    // the context's rig table
+    const int* rig;                     // [F] rig of each frame; NULL: every frame has rig 0
     float *ws_gt_uv, *ws_conf, *ws_j3d_xyz, *ws_j3d_conf;     // the lanes' rows, read by the dense kernels
+    int* ws_rig;                        // [B] the rig of each lane's frame (with rig)
     int* lane_frame; long long* lane_start; float* lane_params; int* queue; long long* end_round;
     int* pose_valid;
     SeqChain q;                         // the sequences, queued by q.act; q.off == NULL: a frame stream (q.cold: its stage table)
@@ -195,8 +198,8 @@ __device__ __forceinline__ int queued_frame(const LaneArgs& a, int l, int k) {
 // round).  Every lane whose frame is done hands the frame's parameters, final loss and counts back to the call and takes the
 // frame's successor in place (a lane that continues stays active).  The freed lanes then take the next queue entries in
 // ascending lane order (ballot + prefix sum: no atomics decide which lane gets which frame), so freed lanes only take from
-// the queue and the host's na_bound rule holds.  Every frame that enters a lane brings its detections and, with the 3-D term
-// on, its 3-D targets into the lane's rows, and starts as lbfgs_init_kernel starts a frame of mvs_fit, so that its bits do not
+// the queue and the host's na_bound rule holds.  Every frame that enters a lane brings its rig index, the detections of its
+// rig's views and, with the 3-D term on, its 3-D targets into the lane's rows, and starts as lbfgs_init_kernel starts a frame of mvs_fit, so that its bits do not
 // depend on the lane or on when it entered.  round: rounds of the run so far (the new frames' first round).  flush != 0: hand
 // back every frame still in a lane, take none.
 __global__ void __launch_bounds__(1024) lane_refill_kernel(LbfgsState S, LaneArgs a, long long round, int flush) {
@@ -261,8 +264,10 @@ __global__ void __launch_bounds__(1024) lane_refill_kernel(LbfgsState S, LaneArg
             VLOOP(i) {                                    // a warm frame keeps the fitted row (but its own body pose, keep_pose)
                 if (!wm || (a.q.keep_pose && i >= kOffPose && i < kOffTransl)) xl[i] = a.params[(size_t)fn * kParams + i];
             }
-            const int K = a.K;
-            for (int v = 0; v < a.V; ++v) {
+            const int K = a.K, rg = a.rig ? a.rig[fn] : 0;
+            if (a.rig && lane == 0) a.ws_rig[ln] = rg;
+            const int nv = a.rigs[rg].num_views;          // rows v >= nv of the frame are not read
+            for (int v = 0; v < nv; ++v) {
                 const size_t dst = (size_t)v * a.B + ln, src = (size_t)v * a.F + fn;
                 for (int k = lane; k < 2 * K; k += 32) a.ws_gt_uv[dst * 2 * K + k] = a.gt_uv[src * 2 * K + k];
                 for (int k = lane; k < K; k += 32) a.ws_conf[dst * K + k] = a.conf[src * K + k];
@@ -283,12 +288,15 @@ __global__ void __launch_bounds__(1024) lane_refill_kernel(LbfgsState S, LaneArg
     if (tid == 0) *a.queue = qbase;
 }
 
-// rows idx[0 .. n) of full [V][n_full][L] <-> packed [V][n][L]; to_full = 0 gathers, 1 scatters
-__global__ void copy_rows_kernel(float* __restrict__ packed, float* __restrict__ full, const int* __restrict__ idx, int n, int n_full,
-                                 int L, int to_full) {
+// rows idx[0 .. n) of full [V][n_full][L] <-> packed [V][n][L]; to_full = 0 gathers, 1 scatters.  With rig (per-view rows of
+// frames with rigs rig[n_full]): view v of a frame whose rig has no view v is skipped.
+template <class T>
+__global__ void copy_rows_kernel(T* __restrict__ packed, T* __restrict__ full, const int* __restrict__ idx, int n, int n_full,
+                                 int L, int to_full, const Rig* __restrict__ rigs = nullptr, const int* __restrict__ rig = nullptr) {
     const int i = blockIdx.x, v = blockIdx.y;
-    float* p = packed + ((size_t)v * n + i) * L;
-    float* g = full + ((size_t)v * n_full + idx[i]) * L;
+    if (rig && v >= rigs[rig[idx[i]]].num_views) return;
+    T* p = packed + ((size_t)v * n + i) * L;
+    T* g = full + ((size_t)v * n_full + idx[i]) * L;
     for (int k = threadIdx.x; k < L; k += blockDim.x) {
         if (to_full) g[k] = p[k];
         else p[k] = g[k];
@@ -786,8 +794,10 @@ static int run_lanes(mvs_ctx* ctx, LaneArgs& a, const float* joint_weights, cons
     long long* th = reinterpret_cast<long long*>(S.na_host) + 1;      // [0..2] totals, [4] rounds
     int rc;
     if ((rc = frame_step_begin_run(ctx, st))) return rc;                 // (allocates the pose cache on first use)
-    a.B = B; a.V = ctx->cams.num_views; a.K = K;
-    a.ws_gt_uv = w.gt_uv; a.ws_conf = w.conf; a.ws_j3d_xyz = w.j3d_xyz; a.ws_j3d_conf = w.j3d_conf;
+    a.B = B; a.K = K;
+    a.rigs = ctx->rigs_dev;
+    a.ws_gt_uv = w.gt_uv; a.ws_conf = w.conf; a.ws_j3d_xyz = w.j3d_xyz; a.ws_j3d_conf = w.j3d_conf; a.ws_rig = w.slot_rig;
+    ctx->slot_rigs = a.rig ? w.slot_rig : nullptr;                       // the dense kernels read each lane's rig
     a.lane_frame = ss.lane_frame; a.lane_start = ss.lane_start; a.lane_params = ss.lane_params; a.queue = ss.queue;
     a.end_round = ss.end_round; a.pose_valid = w.pose_valid;
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(w.joint_w, joint_weights, (size_t)K * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -811,7 +821,7 @@ static int run_lanes(mvs_ctx* ctx, LaneArgs& a, const float* joint_weights, cons
 }
 
 // One run of mvs_fit_stream: stages lps[0 .. nst) of one regime over all F frames of the stream
-static int run_stream_group(mvs_ctx* ctx, const mvs_frame_stream* s, Regime rg, const LossParams* lps, int nst,
+static int run_stream_group(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig, Regime rg, const LossParams* lps, int nst,
                             const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats, cudaStream_t st) {
     LbfgsCfg cfg;
     int rc = begin_run(ctx, c, false, lps, nst, &cfg, st);
@@ -822,7 +832,7 @@ static int run_stream_group(mvs_ctx* ctx, const mvs_frame_stream* s, Regime rg, 
         LbfgsState& S = *ctx->lbfgs;
         StreamState& ss = *ctx->fstream;
         long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
-        const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, s->gt_xyz, s->conf3d};
+        const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, s->gt_xyz, s->conf3d, rig};
         if ((rc = launch_lbfgs_resident(ctx, s->params, cfg, cfg.history, S.lp_tab, lps, nst, ss.sc, nullptr, st, nullptr, &in)))
             return rc;
         LbfgsState Sf = S;
@@ -837,13 +847,13 @@ static int run_stream_group(mvs_ctx* ctx, const mvs_frame_stream* s, Regime rg, 
     LaneArgs a{};
     a.F = F; a.n_queue = F;
     a.params = s->params; a.final_loss = s->final_loss; a.gt_uv = s->gt_uv; a.conf = s->conf;
-    a.j3d_xyz = s->gt_xyz; a.j3d_conf = s->conf3d;
+    a.j3d_xyz = s->gt_xyz; a.j3d_conf = s->conf3d; a.rig = rig;
     a.q.cold = make_int2(0, nst);                                     // every frame runs the whole table
     return run_lanes(ctx, a, s->joint_weights, cfg, nst, stats, st);
 }
 
-// mvs_fit_stream: the stage groups of run_fit, each over all F frames before the next starts
-static int run_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
+// mvs_fit_stream: the stage groups of run_fit, each over all F frames before the next starts (rig [F] or NULL: rig 0)
+static int run_stream(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig, int n_stages, const mvs_loss_config* stage_cfgs,
                       const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, cudaStream_t st) {
     const int H = history_size(opt_cfg);
     std::vector<LossParams> lps;
@@ -856,16 +866,18 @@ static int run_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, con
     rc = ensure_stream_state(ctx, any_resident ? s->n_frames : 0);
     if (!rc && any_dense) rc = ensure_lane_rows(ctx, s->gt_xyz != nullptr);
     if (rc) return rc;
-    // the dense groups overwrite the lanes' keypoint and 3-D target rows: from here on the context holds neither
+    // the dense groups overwrite the lanes' keypoint, 3-D target and rig rows: from here on the context holds none of them
     ctx->have_kp = false;
     ctx->j3d_enabled = false;
+    ctx->slot_rigs = nullptr;
     for (int i = 0, g = 0; i < n_stages && !rc; i = ends[g++]) {
         ctx->loss = lps[i];
         ctx->have_loss = true;
-        rc = run_stream_group(ctx, s, stage_regime(ctx, lps[i], H, false), &lps[i], ends[g] - i, opt_cfg, stats, st);
+        rc = run_stream_group(ctx, s, rig, stage_regime(ctx, lps[i], H, false), &lps[i], ends[g] - i, opt_cfg, stats, st);
     }
     ctx->loss = lps[n_stages - 1];
     ctx->loss.j3d_on = 0;
+    ctx->slot_rigs = nullptr;
     return rc;
 }
 
@@ -876,6 +888,7 @@ struct SeqState {
     int* lane_seq = nullptr;            // [B]
     size_t packed_cap = 0;
     float* packed = nullptr;            // the pending cold frames' rows for the runs before the chaining run
+    int* packed_rig = nullptr;          // [cap] their rigs
 };
 
 static int ensure_seq_state(mvs_ctx* ctx, int nseq, size_t packed_floats) {
@@ -886,13 +899,14 @@ static int ensure_seq_state(mvs_ctx* ctx, int nseq, size_t packed_floats) {
     }
     SeqState& q = *ctx->sstream;
     if (q.cap < nseq) {
-        for (int* p : {q.off, q.cur, q.act, q.frames})
+        for (int* p : {q.off, q.cur, q.act, q.frames, q.packed_rig})
             if (p) dev_free(ctx, p);
         q.cap = 0;
         if ((rc = dev_alloc(ctx, &q.off, (size_t)nseq + 1))) return rc;
         if ((rc = dev_alloc(ctx, &q.cur, (size_t)nseq))) return rc;
         if ((rc = dev_alloc(ctx, &q.act, (size_t)nseq))) return rc;
         if ((rc = dev_alloc(ctx, &q.frames, (size_t)nseq))) return rc;
+        if ((rc = dev_alloc(ctx, &q.packed_rig, (size_t)nseq))) return rc;
         q.cap = nseq;
     }
     if (q.packed_cap < packed_floats) {
@@ -907,8 +921,8 @@ static int ensure_seq_state(mvs_ctx* ctx, int nseq, size_t packed_floats) {
 
 // The chaining run over the sequences of one pass (q.act): every frame of run `tab` from its sequence's pending frame on
 // (gt_xyz / conf3d [F][K][3] / [F][K]: the 3-D targets, both NULL when the term is off)
-static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int F, Regime rg,
-                         const std::vector<LossParams>& tab, const SeqChain& q0, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats,
+static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig, int F,
+                         Regime rg, const std::vector<LossParams>& tab, const SeqChain& q0, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats,
                          cudaStream_t st) {
     const int nst = (int)tab.size();
     LbfgsCfg cfg;
@@ -921,7 +935,7 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
     if (rg == kResident) {
         // one launch, one CTA per sequence; rounds: the largest number of evaluations one CTA ran (its frames' sum)
         long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
-        const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d};
+        const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d, rig};
         if ((rc = launch_lbfgs_resident_seq(ctx, s->params, cfg, cfg.history, S.lp_tab, tab.data(), nst, in, q, st))) return rc;
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
@@ -932,7 +946,7 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
     LaneArgs a{};
     a.F = F; a.n_queue = q.n_act;
     a.params = s->params; a.final_loss = s->final_loss; a.gt_uv = s->gt_uv; a.conf = s->conf;
-    a.j3d_xyz = gt_xyz; a.j3d_conf = conf3d;
+    a.j3d_xyz = gt_xyz; a.j3d_conf = conf3d; a.rig = rig;
     a.q = q;
     a.lane_seq = ctx->sstream->lane_seq;
     return run_lanes(ctx, a, s->joint_weights, cfg, nst, stats, st);
@@ -943,8 +957,9 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
 // the runs before c (as a frame stream of P's rows), then runs c over their sequences; a sequence whose next frame turns
 // out cold parks it for the next pass (c > 0 only: with c == 0 the cold frame stays in its slot with the cold slice).
 // gt_xyz / conf3d ([F][K][3] / [F][K], both NULL or both set): the 3-D joint term is on in every stage, cold and warm, iff set;
-// they travel with the frames as gt_uv / conf do.
-static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int n_stages,
+// they travel with the frames as gt_uv / conf do, and so does rig ([F] or NULL: every frame has rig 0).
+static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig,
+                          int n_stages,
                           const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
                           cudaStream_t st) {
     const int NS = s->n_sequences;
@@ -985,7 +1000,7 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
     q.park = c > 0 ? 1 : 0;
     q.keep_pose = n_vp2 == 0 ? 1 : 0;
     // a frame's packed row: params | gt_uv | conf, then gt_xyz | conf3d with the 3-D term
-    const size_t row_floats = kParams + (size_t)ctx->cams.num_views * ctx->m.K * 3 + (gt_xyz ? (size_t)ctx->m.K * 4 : 0);
+    const size_t row_floats = kParams + (size_t)ctx->vmax * ctx->m.K * 3 + (gt_xyz ? (size_t)ctx->m.K * 4 : 0);
     rc = ensure_stream_state(ctx, resident_before ? NS : 0);
     if (!rc) rc = ensure_seq_state(ctx, NS, c > 0 ? row_floats * NS : 0);
     if (!rc && any_dense) rc = ensure_lane_rows(ctx, gt_xyz != nullptr);
@@ -994,12 +1009,14 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
     q.off = ss.off;
     q.cur = ss.cur;
     q.act = ss.act;
-    // the dense runs overwrite the slots' keypoint rows: from here on the context holds none (and no 3-D targets)
+    // the dense runs overwrite the slots' keypoint rows: from here on the context holds none (and no 3-D targets or rigs)
     ctx->have_kp = false;
     ctx->j3d_enabled = false;
+    ctx->slot_rigs = nullptr;
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.off, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     std::vector<int> cur(off.begin(), off.end() - 1), act, frames;   // each sequence's pending cold frame, -1: done
-    const int V = ctx->cams.num_views, K = ctx->m.K;
+    const int V = ctx->vmax, K = ctx->m.K;
+    const Rig* rigs = ctx->rigs_dev;
     while (!rc) {
         act.clear();
         frames.clear();
@@ -1016,8 +1033,12 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
             float* pg = px + (size_t)n * kParams;
             float* pc = pg + (size_t)V * n * K * 2;
             MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, ss.frames, n, F, kParams, 0));
-            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pg, const_cast<float*>(s->gt_uv), ss.frames, n, F, 2 * K, 0));
-            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pc, const_cast<float*>(s->conf), ss.frames, n, F, K, 0));
+            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pg, const_cast<float*>(s->gt_uv), ss.frames, n, F, 2 * K, 0,
+                                                                                     rigs, rig));
+            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pc, const_cast<float*>(s->conf), ss.frames, n, F, K, 0,
+                                                                                     rigs, rig));
+            if (rig)
+                MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 32, 0, st>>>(ss.packed_rig, const_cast<int*>(rig), ss.frames, n, F, 1, 0));
             float *pj = nullptr, *pjc = nullptr;
             if (gt_xyz) {
                 pj = pc + (size_t)V * n * K;
@@ -1029,7 +1050,8 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
             for (int i = 0, g = 0; g < c && !rc; i = ends[g++]) {
                 ctx->loss = lps[i];
                 ctx->have_loss = true;
-                rc = run_stream_group(ctx, &fs, stage_regime(ctx, lps[i], H, false), &lps[i], ends[g] - i, opt_cfg, stats, st);
+                rc = run_stream_group(ctx, &fs, rig ? ss.packed_rig : nullptr, stage_regime(ctx, lps[i], H, false), &lps[i],
+                                      ends[g] - i, opt_cfg, stats, st);
             }
             if (rc) break;
             MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, ss.frames, n, F, kParams, 1));
@@ -1037,13 +1059,14 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
         q.n_act = n;
         ctx->loss = lps[ic];
         ctx->have_loss = true;
-        if ((rc = run_seq_chain(ctx, s, gt_xyz, conf3d, F, stage_regime(ctx, lps[ic], H, false), tab, q, opt_cfg, stats, st)))
+        if ((rc = run_seq_chain(ctx, s, gt_xyz, conf3d, rig, F, stage_regime(ctx, lps[ic], H, false), tab, q, opt_cfg, stats, st)))
             break;
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(cur.data(), ss.cur, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
     }
     ctx->loss = lps[n_stages - 1];
     ctx->loss.j3d_on = 0;
+    ctx->slot_rigs = nullptr;
     return rc;
 }
 
@@ -1059,6 +1082,7 @@ int mvs_lbfgs_run(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, const 
     if (!(ctx->have_model && ctx->have_cams && ctx->have_kp && ctx->have_loss && ctx->ws.B > 0))
         return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_run: model, cameras, batch, keypoints and loss config must be set first");
     if (!params_dev || !cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_run: NULL argument");
+    if (int rc = batch_rigs(ctx, "mvs_lbfgs_run")) return rc;
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     if (stats) memset(stats, 0, sizeof(*stats));
     return run_stage(ctx, params_dev, final_loss_dev, cfg, stats, (cudaStream_t)stream, RunOpts{});
@@ -1071,6 +1095,7 @@ int mvs_lbfgs_step(mvs_ctx* ctx, float* params_dev, float* loss_dev, float* last
         return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_step: model, cameras, batch, keypoints and loss config must be set first");
     if (!params_dev || !cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_step: NULL argument");
     if (!reset && !ctx->lbfgs) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_step: reset=0 before any step");
+    if (int rc = batch_rigs(ctx, "mvs_lbfgs_step")) return rc;
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     if (stats) memset(stats, 0, sizeof(*stats));
     RunOpts o;
@@ -1086,6 +1111,7 @@ int mvs_fit_seq(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_co
     if (!(ctx->have_model && ctx->have_cams && ctx->have_kp && ctx->ws.B > 0))
         return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq: model, cameras, batch and keypoints must be set first");
     if (!params_dev || n_stages <= 0 || !stage_cfgs || !opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq: NULL / empty argument");
+    if (int rc = batch_rigs(ctx, "mvs_fit_seq")) return rc;
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     if (stats) memset(stats, 0, sizeof(*stats));
     return run_fit(ctx, params_dev, n_stages, stage_cfgs, opt_cfg, final_loss_dev, stats, (cudaStream_t)stream, warm_host);
@@ -1097,13 +1123,14 @@ int mvs_fit(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_config
     if (!(ctx->have_model && ctx->have_cams && ctx->have_kp && ctx->ws.B > 0))
         return set_error(ctx, MVS_ERR_INVALID, "mvs_fit: model, cameras, batch and keypoints must be set first");
     if (!params_dev || n_stages <= 0 || !stage_cfgs || !opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit: NULL / empty argument");
+    if (int rc = batch_rigs(ctx, "mvs_fit")) return rc;
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     if (stats) memset(stats, 0, sizeof(*stats));
     return run_fit(ctx, params_dev, n_stages, stage_cfgs, opt_cfg, final_loss_dev, stats, (cudaStream_t)stream);
 }
 
-int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
-                   const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
+int mvs_fit_stream_rigs(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig_dev, int n_stages, const mvs_loss_config* stage_cfgs,
+                        const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
     if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
     if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0))
         return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: model, cameras and batch must be set first");
@@ -1115,13 +1142,25 @@ int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const 
     if (ctx->anchor_enabled)
         return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_stream: the anchor term is per batch (sequence smoothness); switch it "
                                                    "off (mvs_set_anchor enable = 0) to fit a frame stream");
+    if (!rig_dev && ctx->rigs.size() > 1)
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: the context has %d camera rigs: give each frame's rig "
+                                               "(mvs_fit_stream_rigs)", (int)ctx->rigs.size());
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    if (rig_dev) {
+        if (int rc = check_frame_rigs(ctx, "mvs_fit_stream_rigs", rig_dev, s->n_frames, (cudaStream_t)stream)) return rc;
+    }
     if (stats) memset(stats, 0, sizeof(*stats));
-    return run_stream(ctx, s, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
+    return run_stream(ctx, s, rig_dev, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
 }
 
-int mvs_fit_seq_stream3d(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int n_stages,
-                         const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
+int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
+                   const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
+    return mvs_fit_stream_rigs(ctx, s, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
+}
+
+int mvs_fit_seq_stream_rigs(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig_dev,
+                            int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
+                            void* stream) {
     if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
     if (!gt_xyz != !conf3d) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream3d: gt_xyz and conf3d go together");
     if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0))
@@ -1141,14 +1180,26 @@ int mvs_fit_seq_stream3d(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
     if (ctx->anchor_enabled)
         return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_seq_stream: the anchor term is per batch (sequence smoothness); switch "
                                                    "it off (mvs_set_anchor enable = 0) to fit a sequence stream");
+    if (!rig_dev && ctx->rigs.size() > 1)
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: the context has %d camera rigs: give each frame's rig "
+                                               "(mvs_fit_seq_stream_rigs)", (int)ctx->rigs.size());
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    if (rig_dev) {
+        const int F = s->seq_offsets[s->n_sequences];
+        if (int rc = check_frame_rigs(ctx, "mvs_fit_seq_stream_rigs", rig_dev, F, (cudaStream_t)stream)) return rc;
+    }
     if (stats) memset(stats, 0, sizeof(*stats));
-    return run_seq_stream(ctx, s, gt_xyz, conf3d, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
+    return run_seq_stream(ctx, s, gt_xyz, conf3d, rig_dev, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
+}
+
+int mvs_fit_seq_stream3d(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int n_stages,
+                         const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
+    return mvs_fit_seq_stream_rigs(ctx, s, gt_xyz, conf3d, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
 }
 
 int mvs_fit_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
                        const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
-    return mvs_fit_seq_stream3d(ctx, s, nullptr, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
+    return mvs_fit_seq_stream_rigs(ctx, s, nullptr, nullptr, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
 }
 
 int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, const float* conf_host,
@@ -1159,6 +1210,7 @@ int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, cons
         return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_host: model, cameras and batch must be set first");
     if (!params_host || !gt_uv_host || !conf_host || !joint_weights_host || n_stages <= 0 || !stage_cfgs || !opt_cfg)
         return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_host: NULL / empty argument");
+    if (int rc = batch_rigs(ctx, "mvs_fit_host")) return rc;
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = (cudaStream_t)stream;
     const int B = ctx->ws.B;

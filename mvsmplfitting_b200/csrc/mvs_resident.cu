@@ -58,7 +58,7 @@ namespace mvs {
 
 // ------------------------------------------------------------------------------------------------ single closure
 __global__ void __launch_bounds__(kResThreads, 2)
-closure_resident_kernel(ResidentModel m, CamSet cams, LossParams lp, const float* __restrict__ x,
+closure_resident_kernel(ResidentModel m, RigSet rigs, LossParams lp, const float* __restrict__ x,
                         const int* __restrict__ fidx, const int* __restrict__ na_ptr, const float* __restrict__ gt_uv,
                         const float* __restrict__ conf, const float* __restrict__ joint_w, int B, int have_grad,
                         float* __restrict__ loss_out, float* __restrict__ grad_out, float* __restrict__ joints_out,
@@ -68,11 +68,12 @@ closure_resident_kernel(ResidentModel m, CamSet cams, LossParams lp, const float
     const int slot = blockIdx.x;
     if (slot >= *na_ptr) return;
     const int b = fidx[slot];
+    const FrameRig rig = frame_rig(rigs, b);
     resident_setup(S, m);
     for (int i = threadIdx.x; i < kParams; i += kResThreads) S.x[i] = x[(size_t)b * kParams + i];
     __syncthreads();
     VposerSmem* W = lp.use_vposer == 2 ? reinterpret_cast<VposerSmem*>(smem_raw + sizeof(ResidentSmem)) : nullptr;
-    resident_closure(S, m, cams, lp, gt_uv, conf, joint_w, B, b, have_grad != 0, joints_out, proj_out, DenseIn{}, W);
+    resident_closure(S, m, rig, lp, gt_uv, conf, joint_w, B, b, have_grad != 0, joints_out, proj_out, DenseIn{}, W);
     if (threadIdx.x == 0) loss_out[b] = S.sc[2];
     if (have_grad)
         for (int i = threadIdx.x; i < kParams; i += kResThreads) grad_out[(size_t)b * kParams + i] = S.lg_new[i];
@@ -94,7 +95,7 @@ vposer_decode_kernel(ResidentModel m, const float* __restrict__ x, int B, float*
 
 // ------------------------------------------------------------------------------------------------ whole stage
 __global__ void __launch_bounds__(kResThreads, 2)
-lbfgs_resident_kernel(ResidentModel m, CamSet cams, const LossParams* __restrict__ lp_tab, int nstages, LbfgsCfg cfg,
+lbfgs_resident_kernel(ResidentModel m, RigSet rigs, const LossParams* __restrict__ lp_tab, int nstages, LbfgsCfg cfg,
                       float* __restrict__ params, const float* __restrict__ gt_uv, const float* __restrict__ conf,
                       const float* __restrict__ joint_w, int B, int H, FrameScalars* __restrict__ sc_out,
                       float* __restrict__ last_grad_out, int with_vposer, const int2* __restrict__ stage_rng) {
@@ -117,6 +118,7 @@ lbfgs_resident_kernel(ResidentModel m, CamSet cams, const LossParams* __restrict
         }
         return;
     }
+    const FrameRig rig = frame_rig(rigs, b);
     resident_setup(S, m);
     for (int i = t; i < kParams; i += kResThreads) { const float v = params[(size_t)b * kParams + i]; S.lx[i] = v; S.lx_eval[i] = v; }
     if (t == 0) S.fs = fresh_frame_scalars(make_int2(st_begin, st_end));
@@ -134,7 +136,7 @@ lbfgs_resident_kernel(ResidentModel m, CamSet cams, const LossParams* __restrict
         for (int i = t; i < kParams; i += kResThreads) S.x[i] = S.lx_eval[i];
         __syncthreads();
         PHASE_MARK(1);
-        resident_closure(S, m, cams, S.lp, gt_uv, conf, joint_w, B, b, true, nullptr, nullptr, DenseIn{}, W);
+        resident_closure(S, m, rig, S.lp, gt_uv, conf, joint_w, B, b, true, nullptr, nullptr, DenseIn{}, W);
         PHASE_MARK(23);
         if (warp == 0) {
             FrameScalars s = S.fs;
@@ -170,7 +172,7 @@ lbfgs_resident_kernel(ResidentModel m, CamSet cams, const LossParams* __restrict
 // fitted row in shared memory, cold from the successor's own row -- or, with q.park, leaves a cold successor to the next
 // pass.  B = F: the inputs' row stride.  Kept apart from lbfgs_resident_kernel so that kernel's code stays as it is.
 __global__ void __launch_bounds__(kResThreads, 2)
-lbfgs_resident_seq_kernel(ResidentModel m, CamSet cams, const LossParams* __restrict__ lp_tab, LbfgsCfg cfg,
+lbfgs_resident_seq_kernel(ResidentModel m, RigSet rigs, const LossParams* __restrict__ lp_tab, LbfgsCfg cfg,
                           float* __restrict__ params, const float* __restrict__ gt_uv, const float* __restrict__ conf,
                           const float* __restrict__ joint_w, int B, int H, int with_vposer, SeqChain q) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -190,6 +192,7 @@ lbfgs_resident_seq_kernel(ResidentModel m, CamSet cams, const LossParams* __rest
                 S.gram, S.tl_scratch};
     const long long eval_cap = (long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8;
     while (true) {                                                       // frames of the sequence
+        const FrameRig rig = frame_rig(rigs, b);                         // a sequence's frames may change rig
         if (t == 0) S.fs = fresh_frame_scalars(rng);
         if (t < (int)(sizeof(LossParams) / 4)) reinterpret_cast<int*>(&S.lp)[t] = reinterpret_cast<const int*>(&lp_tab[rng.x])[t];
         __syncthreads();
@@ -198,7 +201,7 @@ lbfgs_resident_seq_kernel(ResidentModel m, CamSet cams, const LossParams* __rest
         while (true) {                                                   // as lbfgs_resident_kernel
             for (int i = t; i < kParams; i += kResThreads) S.x[i] = S.lx_eval[i];
             __syncthreads();
-            resident_closure(S, m, cams, S.lp, gt_uv, conf, joint_w, B, b, true, nullptr, nullptr, DenseIn{}, W);
+            resident_closure(S, m, rig, S.lp, gt_uv, conf, joint_w, B, b, true, nullptr, nullptr, DenseIn{}, W);
             if (warp == 0) {
                 FrameScalars s = S.fs;
                 lbfgs_advance_core(s, P, S.sc[2], cfg, lane, S.lp.use_vposer == 2 ? 32 : kOffTransl - kOffPose);
@@ -271,7 +274,7 @@ frame_fwd_resident_kernel(ResidentModel m, const LossParams* __restrict__ lp_tab
 bool resident_supported(const mvs_ctx* ctx) {
     const DevModel& m = ctx->m;
     return m.supj_ptr != nullptr && m.nsup + 6 <= kResMaxSup && m.K <= kMaxKeypoints &&
-           ctx->cams.num_views * m.K <= kResMaxVK && m.M <= kResMaxM;
+           ctx->vmax * m.K <= kResMaxVK && m.M <= kResMaxM;
 }
 
 bool dense_supported(const mvs_ctx* ctx) { return (ctx->m.N + 255) / 256 <= 64; }     // frame_step's block list holds 64 entries
@@ -319,7 +322,7 @@ int launch_closure_resident(mvs_ctx* ctx, const float* x_dev, float* loss_dev, f
     Workspace& w = ctx->ws;
     const size_t smem = sizeof(ResidentSmem) + (ctx->loss.use_vposer == 2 ? sizeof(VposerSmem) : 0);
     MVS_LAUNCH(ctx, KID_RESIDENT_CLOSURE, st,
-               closure_resident_kernel<<<w.B, kResThreads, smem, st>>>(make_resident_model(ctx), ctx->cams, ctx->loss, x_dev,
+               closure_resident_kernel<<<w.B, kResThreads, smem, st>>>(make_resident_model(ctx), slot_rig_set(ctx), ctx->loss, x_dev,
                                                                        w.fidx, w.na, w.gt_uv, w.conf, w.joint_w, w.B,
                                                                        grad_dev ? 1 : 0, loss_dev ? loss_dev : w.loss_scratch,
                                                                        grad_dev, joints_dev, proj_dev));
@@ -342,11 +345,11 @@ int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, 
     int with_vposer = 0;
     for (int i = 0; i < nstages; ++i) with_vposer |= (lph[i].use_vposer == 2);
     const size_t smem = frame_smem(H, with_vposer != 0);
-    const FrameInputs in = frames ? *frames : FrameInputs{w.B, w.gt_uv, w.conf, w.joint_w, w.j3d_xyz, w.j3d_conf};
+    const FrameInputs in = frames ? *frames : FrameInputs{w.B, w.gt_uv, w.conf, w.joint_w, w.j3d_xyz, w.j3d_conf, ctx->slot_rigs};
     ResidentModel rm = make_resident_model(ctx);
     rm.j3d_xyz = in.j3d_xyz; rm.j3d_conf = in.j3d_conf;
     MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
-               lbfgs_resident_kernel<<<in.n, kResThreads, smem, st>>>(rm, ctx->cams, lp_tab_dev, nstages, cfg, params_dev,
+               lbfgs_resident_kernel<<<in.n, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev, in.rig}, lp_tab_dev, nstages, cfg, params_dev,
                                                                       in.gt_uv, in.conf, in.joint_w, in.n, H, sc_out,
                                                                       last_grad_dev, with_vposer, stage_rng_dev));
     MVS_CUDA_OK(ctx, cudaGetLastError());
@@ -361,7 +364,7 @@ int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& c
     ResidentModel rm = make_resident_model(ctx);
     rm.j3d_xyz = in.j3d_xyz; rm.j3d_conf = in.j3d_conf;              // row stride in.n, as gt_uv / conf
     MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
-               lbfgs_resident_seq_kernel<<<q.n_act, kResThreads, smem, st>>>(rm, ctx->cams, lp_tab_dev, cfg,
+               lbfgs_resident_seq_kernel<<<q.n_act, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev, in.rig}, lp_tab_dev, cfg,
                                                                              params_dev, in.gt_uv, in.conf, in.joint_w, in.n, H,
                                                                              with_vposer, q));
     MVS_CUDA_OK(ctx, cudaGetLastError());
@@ -390,7 +393,7 @@ static FrameStepArgs make_frame_step_args(mvs_ctx* ctx, float* params_dev, const
     Workspace& w = ctx->ws;
     const DevModel& dm = ctx->m;
     FrameStepArgs a;
-    a.m = make_resident_model(ctx); a.cams = ctx->cams; a.lp_tab = L.lp_tab; a.nstages = nstages;
+    a.m = make_resident_model(ctx); a.rigs = slot_rig_set(ctx); a.lp_tab = L.lp_tab; a.nstages = nstages;
     a.cfg = cfg; a.L = L; a.params = params_dev;
     a.gt_uv = w.gt_uv; a.conf = w.conf; a.joint_w = w.joint_w; a.B = w.B; a.N = dm.N;
     a.verts_ws = w.verts; a.poffT = tc_poffT(ctx); a.ST = dm.ST;

@@ -374,13 +374,13 @@ __device__ __forceinline__ void dphi_col(ResidentSmem& S, const ResidentModel& m
 // ------------------------------------------------------------------------------------------------
 // One closure evaluation at S.x (already loaded).  Writes S.sc[2] = total loss and S.lg_new = gradient
 // (frozen segments zeroed).  All kResThreads threads must call it.
-static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m, const CamSet& cams, const LossParams& lp,
+static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m, const FrameRig& rig, const LossParams& lp,
                                  const float* __restrict__ gt_uv, const float* __restrict__ conf,
                                  const float* __restrict__ joint_w, int B, int b, bool have_grad,
                                  float* __restrict__ joints_out, float* __restrict__ proj_out, const DenseIn& din,
                                  VposerSmem* W = nullptr) {
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    const int nsup = m.nsup, K = m.K, V = cams.num_views, ncol = 3 * nsup;
+    const int nsup = m.nsup, K = m.K, V = rig.num_views, ncol = 3 * nsup;          // V: the views of this frame's rig
     // use_vposer == 2: the body pose is decoded from the latent code in the pose slot (fitting.py:121-123)
     const bool vp2 = (lp.use_vposer == 2) && W != nullptr;
     if (vp2) vposer_decode(S, m, *W);
@@ -544,11 +544,13 @@ static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m,
         data_sync();
         PHASE_MARK(7);
         {
-            const float rho2 = lp.rho * lp.rho, dw2 = lp.data_weight * lp.data_weight;
+            const float dw = lp.data_weight * rig.dw_scale;                         // the rig's data weight (x 1: exact)
+            const float rho2 = lp.rho * lp.rho, dw2 = dw * dw;
             for (int idx = t; idx < V * K; idx += kDataThreads) {
                 const int v = idx / K, k = idx % K;
                 float xc[3], uv[2];
-                project_fwd(cams.cam[v], &S.q[3 * k], xc, uv);
+                const CamF cam = rig_camera(rig, v);
+                project_fwd(cam, &S.q[3 * k], xc, uv);
                 const size_t o = ((size_t)v * B + b) * K + k;
                 if (proj_out) { proj_out[2 * o] = uv[0]; proj_out[2 * o + 1] = uv[1]; }
                 float w = joint_w[k];
@@ -560,7 +562,7 @@ static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m,
                 S.lterm[idx] = w2 * g0 + w2 * g1;
                 const float duv[2] = {-(w2 * d0) * dw2, -(w2 * d1) * dw2};
                 float dqv[3] = {0.f, 0.f, 0.f};
-                project_bwd(cams.cam[v], xc, duv, dqv);
+                project_bwd(cam, xc, duv, dqv);
                 S.contrib[3 * idx] = dqv[0]; S.contrib[3 * idx + 1] = dqv[1]; S.contrib[3 * idx + 2] = dqv[2];
             }
             data_sync();
@@ -889,7 +891,7 @@ __device__ __forceinline__ void next_pose_forward(ResidentSmem& S, const Residen
 
 // Arguments of frame_step_kernel
 struct FrameStepArgs {
-    ResidentModel m; CamSet cams; const LossParams* lp_tab; int nstages; LbfgsCfg cfg; LbfgsState L; float* params;
+    ResidentModel m; RigSet rigs; const LossParams* lp_tab; int nstages; LbfgsCfg cfg; LbfgsState L; float* params;
     const float* gt_uv; const float* conf; const float* joint_w; int B, N;
     const float* verts_ws; const float* poffT; const float* ST;
     const float* parts5; const float* part; const int* pflag; const FrameBox* box; const float* Wd;
@@ -911,7 +913,8 @@ frame_step_kernel(FrameStepArgs a, const int* __restrict__ fidx, const int* __re
     const int slot = blockIdx.x;
     if (slot >= *na_ptr) return;
     const int b = fidx[slot];
-    const ResidentModel& m = a.m; const CamSet& cams = a.cams; const LossParams* lp_tab = a.lp_tab;
+    const FrameRig rig = frame_rig(a.rigs, b);                  // the cameras of this frame (issued ahead of the closure)
+    const ResidentModel& m = a.m; const LossParams* lp_tab = a.lp_tab;
     const LbfgsCfg& cfg = a.cfg; const LbfgsState& L = a.L; float* params = a.params;
     const float* __restrict__ gt_uv = a.gt_uv; const float* __restrict__ conf = a.conf; const float* __restrict__ joint_w = a.joint_w;
     const int B = a.B, N = a.N, ldA = a.ldA, with_vposer = a.with_vposer;
@@ -1032,7 +1035,7 @@ frame_step_kernel(FrameStepArgs a, const int* __restrict__ fidx, const int* __re
     din.fl = S.fl;
     din.nfl = S.nfl;
     din.pose_ready = pose_ready;
-    resident_closure(S, m, cams, S.lp, gt_uv, conf, joint_w, B, b, true, nullptr, nullptr, din, W);
+    resident_closure(S, m, rig, S.lp, gt_uv, conf, joint_w, B, b, true, nullptr, nullptr, din, W);
     for (int i = t; i < kParams; i += kResThreads) L.g_eval[(size_t)b * kParams + i] = S.lg_new[i];
     cp_async_wait_all();                               // group 1: history, curvature scalars, block Gram
     __syncthreads();

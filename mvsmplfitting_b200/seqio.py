@@ -214,10 +214,12 @@ def _uses_latent_pose(stage_cfgs) -> bool:
     return kinds == {2}
 
 
-def _check_missing_views(seq: dict, stage_cfgs) -> None:
+def _check_missing_views(seq: dict, stage_cfgs, views: int | None = None) -> None:
     """a (view, frame) without detections carries confidence 0; that only removes it from the data term when the loss uses the
-    confidences (the reference drops such a view from the camera list instead, main.py:45-56)"""
-    if not seq["present"].all() and not all(int(c.use_joints_conf) for c in stage_cfgs):
+    confidences (the reference drops such a view from the camera list instead, main.py:45-56).  views: the number of views
+    of the sequence's rig (default: all rows), the only ones its frames have"""
+    present = seq["present"] if views is None else seq["present"][:views]
+    if not present.all() and not all(int(c.use_joints_conf) for c in stage_cfgs):
         raise ValueError("sequence has (view, frame) pairs without detections: every stage needs use_joints_conf = 1")
 
 
@@ -255,6 +257,16 @@ def _init_guess_3d(ctx, guess: dict, j3, c3, has):
         x0, _ = ctx.init_guess(**guess)
         x = x0 if x is None else torch.where(torch.as_tensor(has, device=x.device)[:, None], x, x0).contiguous()
     return x
+
+
+def _pad_views(seq: dict, V: int) -> dict:
+    """seq with its per-view arrays (gt_uv, conf, present) padded to V view rows (zeros; rows beyond the sequence's own views
+    are never read)"""
+    n = seq["gt_uv"].shape[0]
+    if n == V:
+        return seq
+    pad = lambda a: np.concatenate([a, np.zeros((V - n,) + a.shape[1:], a.dtype)])
+    return dict(seq, gt_uv=pad(seq["gt_uv"]), conf=pad(seq["conf"]), present=pad(seq["present"]))
 
 
 def _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces, frames=None, rows=None):
@@ -329,18 +341,25 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
     return params.cpu().numpy(), loss, stats
 
 
-def _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess: dict, t3=None) -> torch.Tensor:
+def _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess: dict, t3=None, rig=None, rig_views=None) -> torch.Tensor:
     """initial guesses (init_guess + fix_params) of F frames of any number, ctx.B frames at a time: params [F,86] on the
     device.  The last chunk is padded with zero-confidence rows, which are dropped.  t3: _targets_3d of the F frames (use_3d),
     each chunk's guesses then come from _init_guess_3d (padding rows count as frames without annotation only when the chunk
-    needs that pass anyway)."""
+    needs that pass anyway).  rig [F] (the rig of each frame, views rig_views[r]): every chunk names its slots' rigs, and a
+    frame's rows beyond its rig's views are not taken (padding rows take the chunk's first rig)."""
     F, B = gt_uv.shape[1], ctx.B
     params = torch.empty(F, 86, dtype=torch.float32, device=ctx.device)
     for c0 in range(0, F, B):
         n = min(B, F - c0)
         gt = np.zeros((gt_uv.shape[0], B) + gt_uv.shape[2:], np.float32)
         cf = np.zeros((conf.shape[0], B) + conf.shape[2:], np.float32)
-        gt[:, :n], cf[:, :n] = gt_uv[:, c0:c0 + n], conf[:, c0:c0 + n]
+        if rig is None:
+            gt[:, :n], cf[:, :n] = gt_uv[:, c0:c0 + n], conf[:, c0:c0 + n]
+        else:
+            for j in range(n):
+                nv = rig_views[rig[c0 + j]]
+                gt[:nv, j], cf[:nv, j] = gt_uv[:nv, c0 + j], conf[:nv, c0 + j]
+            ctx.set_frame_rigs(np.concatenate([rig[c0:c0 + n], np.full(B - n, rig[c0], np.int32)]))
         ctx.set_keypoints(gt, cf, jw)
         ctx.set_loss(config=stage_cfgs[0])           # mvs_init_guess zeroes the pose slot when it holds a latent code
         if t3 is None:
@@ -371,9 +390,9 @@ def _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, fac
 def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = False, fixed_scale: float = 1.0,
                   use_hip: bool = True, pose_format: str = "coco17", result_folder: str | None = None,
                   mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, reinit_loss: float = 5000.0,
-                  use_3d: bool = False):
+                  use_3d: bool = False, rigs=None, rig_data_weight_scale=None):
     """main.py:32-89 with is_seq = True for S sequences in lock-step: the batch of step t is frame t of every sequence
-    (context batch = S; same cameras).  A sequence's first frame gets the initial guess and every stage; a later frame
+    (context batch = S).  A sequence's first frame gets the initial guess and every stage; a later frame
     starts from the previous frame's result as load_init + fix_params leave it (init_guess.py:137-166,190-212: betas,
     global_orient, transl, scale kept; body pose back to the hip seed, or the previous latent code under VPoser), skips
     stages 0 and 1 and damps stage 2's pose prior (non_linear_solver.py:157-162, `mvs_fit_seq`) -- unless the previous loss
@@ -385,17 +404,35 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
     a frame with an annotation has the 3-D joint term in every stage it runs, warm or cold, and its cold start point aligns
     to the annotation; a frame without one fits as without the term (_targets_3d, _init_guess_3d).  The context has the
     3-D term off afterwards.
+    Without rigs every sequence was seen by the context's cameras.  rigs (a list of camera dicts, seqio.camera_arrays) fits
+    sequences of several camera setups in the same call: sequence q was seen by rigs[q["rig"]] and has that rig's number of
+    view rows; rig_data_weight_scale [n_rigs] (None: all 1) scales every stage's data_weight per rig (the reference's
+    500 / H for rigs of different image heights).  The rigs are set on the context (set_camera_rigs), detections are padded
+    to the largest view count, and every frame gets what a context with only its rig's cameras gives it.
     Returns a list (per sequence) of (params [T_s,86], loss [T_s]) and the summed stats."""
     S_ = len(seqs)
     latent = _uses_latent_pose(stage_cfgs)
-    for q in seqs:
-        _check_missing_views(q, stage_cfgs)
+    seq_rig = rig_views = None
+    if rigs is not None:
+        rig_views = [int(np.asarray(r["R"]).shape[0]) for r in rigs]
+        seq_rig = np.array([int(q["rig"]) for q in seqs], np.int32)
+        for q, r in zip(seqs, seq_rig):
+            if not 0 <= r < len(rigs):
+                raise ValueError("fit_sequences: sequence %s names rig %d of %d" % (q.get("serial"), r, len(rigs)))
+            if q["gt_uv"].shape[0] != rig_views[r]:
+                raise ValueError("fit_sequences: sequence %s has %d views, its rig %d has %d"
+                                 % (q.get("serial"), q["gt_uv"].shape[0], r, rig_views[r]))
+        ctx.set_camera_rigs(rigs, rig_data_weight_scale)
+        V = max(rig_views)
+        seqs = [_pad_views(q, V) for q in seqs]
+    for s_, q in enumerate(seqs):
+        _check_missing_views(q, stage_cfgs, None if seq_rig is None else rig_views[seq_rig[s_]])
     t3 = _targets_3d(seqs, stage_cfgs, use_hip) if use_3d else None
     if ctx.B != S_:
         return _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces,
                                      pose_format, use_hip, dict(estimate_scale=estimate_scale, fixed_scale=fixed_scale,
                                                                 use_torso=True, hip_seed=1.0, want_joints3d=False,
-                                                                umeyama_as_written=umeyama_as_written), t3)
+                                                                umeyama_as_written=umeyama_as_written), t3, seq_rig, rig_views)
     T = max(len(q["frames"]) for q in seqs)
     V = seqs[0]["gt_uv"].shape[0]
     off = np.concatenate([[0], np.cumsum([len(q["frames"]) for q in seqs])])
@@ -414,6 +451,8 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
                 gt[:, s_], cf[:, s_] = q["gt_uv"][:, t], q["conf"][:, t]
             else:                              # a finished sequence idles on its last frame (results are not kept)
                 gt[:, s_], cf[:, s_] = q["gt_uv"][:, -1], q["conf"][:, -1]
+        if seq_rig is not None:
+            ctx.set_frame_rigs(seq_rig)
         ctx.set_keypoints(gt, cf, jw)
         ctx.set_loss(config=stage_cfgs[0])
         guess = dict(estimate_scale=estimate_scale, fixed_scale=fixed_scale, use_torso=True, hip_seed=1.0,
@@ -451,20 +490,23 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
 
 
 def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces, pose_format,
-                          use_hip, guess, t3=None):
+                          use_hip, guess, t3=None, seq_rig=None, rig_views=None):
     """fit_sequences through mvs_fit_seq_stream: the sequences' frames back to back, every frame's cold start point from
-    _cold_guesses; t3: _targets_3d of those frames (mvs_fit_seq_stream3d)"""
+    _cold_guesses; t3: _targets_3d of those frames (mvs_fit_seq_stream3d); seq_rig [S]: each sequence's rig, which every
+    one of its frames takes (mvs_fit_seq_stream_rigs)"""
     lengths = [len(q["frames"]) for q in seqs]
     off = np.concatenate([[0], np.cumsum(lengths)])
     gt_uv = np.concatenate([q["gt_uv"] for q in seqs], axis=1)
     conf = np.concatenate([q["conf"] for q in seqs], axis=1)
     jw = joint_weights(pose_format, use_hip)
-    params = _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess, t3)
+    rig = None if seq_rig is None else np.repeat(seq_rig, lengths).astype(np.int32)
+    params = _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess, t3, rig, rig_views)
+    kw = {} if rig is None else dict(rig=rig)
     if t3 is None:
-        final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss)
+        final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss, **kw)
     else:
         final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss,
-                                          joints3d=t3[0], conf3d=t3[1])
+                                          joints3d=t3[0], conf3d=t3[1], **kw)
         ctx.set_joints3d(None)
     x, loss = params.cpu().numpy(), final.cpu().numpy()
     if result_folder is not None:
