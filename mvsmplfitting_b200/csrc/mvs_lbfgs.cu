@@ -1235,4 +1235,83 @@ int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, cons
     return MVS_OK;
 }
 
+// Testing aids, not part of the ABI (tests/test_gpu_lbfgs_transitions.py): they let a test drive the optimiser's state machine
+// from the host, one transition at a time, and compare every transition with a float64 restatement.
+//
+// mvs_debug_lbfgs_layout: sizeof(FrameScalars) and the byte offset of each of its fields, in declaration order (arrays: the
+// offset of their first element), so that a host mirror of the struct cannot drift from it.  Needs no context and no device.
+extern "C" int mvs_debug_lbfgs_layout(int* out) {
+#define MVS_OFF(f) (int)offsetof(FrameScalars, f)
+    const int v[] = {(int)sizeof(FrameScalars),
+                     MVS_OFF(phase), MVS_OFF(outer_n), MVS_OFF(state_n_iter), MVS_OFF(n_iter), MVS_OFF(current_evals),
+                     MVS_OFF(ls_iter), MVS_OFF(ls_evals), MVS_OFF(ls_first), MVS_OFF(low), MVS_OFF(high), MVS_OFF(done),
+                     MVS_OFF(insuf), MVS_OFF(have_prev), MVS_OFF(hist_len), MVS_OFF(hist_head), MVS_OFF(nan_flag),
+                     MVS_OFF(pushed_slot), MVS_OFF(stage), MVS_OFF(stage_end), MVS_OFF(nan_acc),
+                     MVS_OFF(t), MVS_OFF(H_diag), MVS_OFF(gtd0), MVS_OFF(t_prev), MVS_OFF(gtd_prev), MVS_OFF(d_norm),
+                     MVS_OFF(bt), MVS_OFF(bgtd), MVS_OFF(bf),
+                     MVS_OFF(loss), MVS_OFF(prev_loss), MVS_OFF(orig_loss), MVS_OFF(f_prev), MVS_OFF(mon_prev_loss),
+                     MVS_OFF(final_loss), MVS_OFF(iters), MVS_OFF(evals)};
+#undef MVS_OFF
+    const int n = (int)(sizeof(v) / sizeof(v[0]));
+    if (out)
+        for (int i = 0; i < n; ++i) out[i] = v[i];
+    return n;
+}
+
+// mvs_debug_lbfgs_state: copies the context's optimiser state of all B frames (history size H) to (write == 0) or from
+// (write != 0) host buffers; null pointers are skipped.  sc [B] FrameScalars; x [B][86] (the parameters that
+// mvs_debug_lbfgs_advance updates); g, d, prev_g, x_init, g_prev [B][86]; bg [B][2][86]; the ring hist_s, hist_y [B][H][86]
+// and ro [B][H]; gram [B][16][8][8]; x_eval, g_eval [B][86]; loss_eval [B].  A write first allocates the state for H
+// (ensure_state); a read needs the state to exist with history size H.  Synchronises the device first.
+extern "C" int mvs_debug_lbfgs_state(mvs_ctx* ctx, int write, int H, void* sc, float* x, float* g, float* d, float* prev_g,
+                                     float* x_init, float* g_prev, float* bg, float* hist_s, float* hist_y, float* ro,
+                                     float* gram, float* x_eval, float* g_eval, float* loss_eval) {
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    if (ctx->ws.B <= 0) return set_error(ctx, MVS_ERR_INVALID, "mvs_debug_lbfgs_state: set the batch first");
+    if (H < 1 || H > 128) return set_error(ctx, MVS_ERR_INVALID, "mvs_debug_lbfgs_state: history size %d", H);
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    MVS_CUDA_OK(ctx, cudaDeviceSynchronize());
+    if (write) {
+        if (int rc = ensure_state(ctx, H)) return rc;
+    } else if (!ctx->lbfgs || ctx->lbfgs->H != H) {
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_debug_lbfgs_state: no optimiser state with history size %d", H);
+    }
+    const LbfgsState& S = *ctx->lbfgs;
+    const size_t B = (size_t)S.B, V = B * kParams * sizeof(float), R = V * (size_t)H;
+    struct { void* host; void* dev; size_t bytes; } cp[] = {
+        {sc, S.sc, B * sizeof(FrameScalars)}, {x, S.x_fit, V}, {g, S.g, V}, {d, S.d, V}, {prev_g, S.prev_g, V},
+        {x_init, S.x_init, V}, {g_prev, S.g_prev, V}, {bg, S.bg, 2 * V}, {hist_s, S.hist_s, R}, {hist_y, S.hist_y, R},
+        {ro, S.ro, B * H * sizeof(float)}, {gram, S.gram, B * kGramFloats * sizeof(float)}, {x_eval, S.x_eval, V},
+        {g_eval, S.g_eval, V}, {loss_eval, S.loss_eval, B * sizeof(float)}};
+    for (auto& c : cp)
+        if (c.host)
+            MVS_CUDA_OK(ctx, write ? cudaMemcpy(c.dev, c.host, c.bytes, cudaMemcpyHostToDevice)
+                                   : cudaMemcpy(c.host, c.dev, c.bytes, cudaMemcpyDeviceToHost));
+    return MVS_OK;
+}
+
+// mvs_debug_lbfgs_advance: one launch of the production lbfgs_advance_kernel over every frame of the context that is not
+// PH_DONE (the active list of lbfgs_compact_kernel), on the context's state, with the LbfgsCfg that begin_run builds from cfg
+// and the given step_mode and pose_len (69: body_pose, 32: pose_embedding).  The parameters it updates are the state's x
+// (mvs_debug_lbfgs_state).  Synchronises before it returns.
+extern "C" int mvs_debug_lbfgs_advance(mvs_ctx* ctx, const mvs_lbfgs_config* c, int step_mode, int pose_len) {
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    if (!c || ctx->ws.B <= 0) return set_error(ctx, MVS_ERR_INVALID, "mvs_debug_lbfgs_advance: NULL config or no batch");
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    const cudaStream_t st = 0;
+    LbfgsCfg cfg;
+    if (int rc = begin_run(ctx, c, step_mode != 0, &ctx->loss, 1, &cfg, st)) return rc;
+    cfg.step_mode = step_mode;
+    LbfgsState& S = *ctx->lbfgs;
+    Workspace& w = ctx->ws;
+    const int B = w.B;
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
+    MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
+    MVS_LAUNCH(ctx, KID_LBFGS_ADVANCE, st, lbfgs_advance_kernel<<<B, 32, 0, st>>>(S, cfg, S.x_fit, w.fidx, w.na, pose_len));
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    return MVS_OK;
+}
+
 }  // extern "C"

@@ -413,7 +413,9 @@ __device__ __forceinline__ void lbfgs_advance_core(FrameScalars& s, const LbfgsP
                 VLOOP(i) bgl[i] = g_new[i];
             }
             __syncwarp();
-            if (fabsf(s.bt[1] - s.bt[0]) * s.d_norm < cfg.tol_change) { label = L_LS_FINISH; break; }
+            // the reference's step() calls _strong_Wolfe without tolerance_change (lbfgs_ls.py:393-397), so the bracket
+            // width is always tested against its default 1e-9, whatever tolerance_change the optimiser was given
+            if (fabsf(s.bt[1] - s.bt[0]) * s.d_norm < 1e-9f) { label = L_LS_FINISH; break; }
             label = L_ZOOM_HEAD;
             break;
         }
