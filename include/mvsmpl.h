@@ -196,7 +196,7 @@ typedef struct {
     int rounds;                    /* batched closure launches */
     int frames_nan;                /* frames stopped by the NaN/Inf guard (fitting.py:101-107) */
     long long dense_frame_evals;   /* of frame_evals: those evaluated by dense (SDF) rounds */
-    int dense_rounds;              /* of rounds: dense rounds (gemm -> skin -> sdf_fused -> frame_step each) */
+    int dense_rounds;              /* of rounds: dense rounds (gemm -> skin -> sdf_setup -> sdf_fused -> frame_step each) */
     int reserved;
 } mvs_lbfgs_stats;
 /* params_dev [B,86] in/out; final_loss_dev [B] or NULL (run_fitting's return value per frame).
@@ -392,7 +392,7 @@ int mvs_set_exec_mode(mvs_ctx* ctx, int mode);
  *      stream around every launch whose kernel id bit is set in `mask` (0 = off, the default).
  *      mvs_profile_read synchronises the device, adds up the elapsed times since the last mvs_profile call
  *      and writes, for kernel id k < MVS_NUM_KERNEL_IDS, ms[k] and launches[k]. */
-#define MVS_NUM_KERNEL_IDS 18
+#define MVS_NUM_KERNEL_IDS 19
 int mvs_profile(mvs_ctx* ctx, unsigned mask);
 int mvs_profile_read(mvs_ctx* ctx, double* ms, long long* launches);
 const char* mvs_kernel_name(int kernel_id);

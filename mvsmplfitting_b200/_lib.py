@@ -79,7 +79,7 @@ EXPORTS = (
     "mvs_fit_stream_rigs", "mvs_fit_seq_stream_rigs", "mvs_fit_host", "mvs_sdf_grid", "mvs_profile", "mvs_profile_read",
     "mvs_kernel_name", "mvs_set_exec_mode", "mvs_set_anchor", "mvs_set_joints3d", "mvs_init_guess",
 )
-NUM_KERNEL_IDS = 18
+NUM_KERNEL_IDS = 19
 
 _lib = None
 

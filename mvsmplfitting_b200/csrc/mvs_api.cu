@@ -174,7 +174,8 @@ int mvs_create(int device, mvs_ctx** out) {
 
 static const char* kKernelNames[KID_COUNT] = {
     "frame_fwd", "vertex_fwd", "sdf_bbox", "sdf_sample", "sdf_finalize", "keypoint_loss", "vertex_bwd", "frame_bwd",
-    "lbfgs_advance", "lbfgs_compact", "sdf_grid", "misc", "closure_resident", "lbfgs_resident", "sdf_fused", "frame_step", "posedirs_gemm_tc", "skin"};
+    "lbfgs_advance", "lbfgs_compact", "sdf_grid", "misc", "closure_resident", "lbfgs_resident", "sdf_fused", "frame_step", "posedirs_gemm_tc", "skin",
+    "sdf_setup"};
 
 const char* mvs_kernel_name(int k) { return (k >= 0 && k < KID_COUNT) ? kKernelNames[k] : ""; }
 

@@ -210,8 +210,8 @@ struct Workspace {
     float* sdf_part = nullptr;        // [B][P][512] unit-factor partial adjoints (288 skin | 224 feature)
     int* sdf_pflag = nullptr;         // [B][P] 1 iff the block has vertices with a non-zero sample gradient
     FrameBox* sdf_box = nullptr;      // [B] frame boxes of the dense rounds, written with the set-up, read by frame_step
-    SdfFrameSetup* sdf_setup = nullptr;   // [B] written by the skinning kernel's last CTA of each frame
-    int* sdf_arrive = nullptr;        // [B] chunk boxes of the frame written so far this round (0 between rounds)
+    SdfFrameSetup* sdf_setup = nullptr;   // [B] by sdf_setup_kernel (at <= 4 frames by skin_small_kernel's last CTA of a frame)
+    int* sdf_arrive = nullptr;        // [B] skin_small_kernel: chunk boxes of a frame written so far this round (0 between rounds)
     // accelerated all-faces SDF (mvs_sdf_bins.cuh): per slot triangle corners, cell lists, ray-bin lists, meta (s_lo, s_scale, overflow)
     float* bins_tri = nullptr; int* bins_cell_ptr = nullptr; unsigned short* bins_cell_idx = nullptr;
     int* bins_ray_ptr = nullptr; unsigned short* bins_ray_idx = nullptr; float* bins_meta = nullptr;
@@ -227,8 +227,8 @@ struct FrameBox {                     // bounding box of one frame's mesh (fitti
 
 // What sdf_fused needs of a frame before it touches a vertex: the frame box, triangle 0 in box coordinates, the cone it
 // spans from the corner (-1,-1,-1) and the triangle's plane with their margins, the vertex-level pads, and the chunk-cull
-// verdict of every 64-vertex chunk.  Computed once per frame and round by the skinning kernel (sdf_frame_setup in
-// mvs_tc_dev.cuh) instead of by every sdf_fused CTA.
+// verdict of every 64-vertex chunk.  Computed once per frame and round (sdf_frame_setup in mvs_tc_dev.cuh), by sdf_setup_kernel
+// after the skinning kernel or by skin_small_kernel's tail (<= 4 frames), instead of by every sdf_fused CTA.
 constexpr int kSdfSkipWords = 8;      // chunk-cull bits for up to 256 chunks (16384 vertices); larger meshes are not culled
 struct __align__(16) SdfFrameSetup {
     FrameBox fb;
@@ -241,7 +241,7 @@ struct __align__(16) SdfFrameSetup {
 };
 static_assert(sizeof(SdfFrameSetup) == 208, "SdfFrameSetup layout");
 
-// Per-launch arguments of the set-up; rec == nullptr: the skinning kernel does not compute it (SDF term off)
+// Per-launch arguments of the set-up; rec == nullptr: skin_small_kernel does not compute it (SDF term off)
 struct SdfSetupArgs {
     SdfFrameSetup* rec; FrameBox* boxout; int* arrive; const float* slot_tr;
     int f0, f1, f2, G, cull;          // triangle 0, grid size, cone/plane culls on (as-written semantics: one face)
@@ -262,7 +262,7 @@ __host__ __device__ inline int sdf_passes_for(int na, int nblocks, int cta_slots
 enum KernelId {
     KID_FRAME_FWD = 0, KID_VERTEX_FWD, KID_SDF_BBOX, KID_SDF_SAMPLE, KID_SDF_FINALIZE, KID_KEYPOINT, KID_VERTEX_BWD,
     KID_FRAME_BWD, KID_LBFGS_ADVANCE, KID_LBFGS_COMPACT, KID_SDF_GRID, KID_MISC, KID_RESIDENT_CLOSURE, KID_RESIDENT_LBFGS,
-    KID_SDF_FRAME, KID_FRAME_STEP, KID_VERTEX_FWD_TC, KID_SKIN, KID_COUNT
+    KID_SDF_FRAME, KID_FRAME_STEP, KID_VERTEX_FWD_TC, KID_SKIN, KID_SDF_SETUP, KID_COUNT
 };
 static_assert(KID_COUNT == MVS_NUM_KERNEL_IDS, "kernel id table out of sync with mvsmpl.h");
 
@@ -409,7 +409,8 @@ int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, 
 int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
                               const LossParams* lp_tab_host, int nstages, const FrameInputs& frames, const SeqChain& q,
                               cudaStream_t st);
-// dense regime (SDF term): per round  posedirs_gemm_tc -> skin -> sdf_fused -> frame_step
+// dense regime (SDF term): per round  posedirs_gemm_tc -> skin -> sdf_setup -> sdf_fused -> frame_step (skin_small in place of
+// skin at <= 8 frames; at <= 4 frames skin_small computes the set-ups itself and sdf_setup is not launched)
 int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);                      // mvs_closure.cu
 int launch_sdf_fused(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu
 int ensure_sdf_setup_ws(mvs_ctx* ctx, cudaStream_t st);   // mvs_sdf.cu: set-up records, arrival counters (zeroed on st), boxes

@@ -11,9 +11,9 @@
 // group of stages (DESIGN.md section 4):
 //   frame-resident   one CTA per frame runs closure + state machine for ALL stages of the group inside ONE launch
 //                    (mvs_resident.cu: lbfgs_resident_kernel)
-//   dense rounds     SDF term on: per round posedirs_gemm_tc -> skin -> sdf_fused -> frame_step; finished frames are
-//                    compacted out every 8 rounds; the host reads the active count one chunk late (the next chunk is
-//                    already enqueued) and only uses it to size grids and to stop
+//   dense rounds     SDF term on: per round posedirs_gemm_tc -> skin -> sdf_setup (above 4 frames) -> sdf_fused ->
+//                    frame_step; finished frames are compacted out every 8 rounds; the host reads the active count
+//                    one chunk late (the next chunk is already enqueued) and only uses it to size grids and to stop
 //   batched chain    the reference SIMT path (launch_closure + lbfgs_advance_kernel + lbfgs_compact_kernel), also
 //                    what mvs_lbfgs_step (one LBFGS.step per call, state persistent in the context) uses
 // run_fit hands consecutive stages of the same regime to one run in which every frame changes stage on its own.
@@ -400,9 +400,9 @@ static int dense_begin(mvs_ctx* ctx, const LbfgsState& S, int nst, cudaStream_t 
     return rc ? rc : frame_step_begin_run(ctx, st);
 }
 
-// One dense round: pose blend shapes of the active frames (wgmma GEMM), skinning + box partials + each frame's SDF set-up,
-// the SDF term with the adjoint of its (short) vertex list, and the per-frame closure adjoint + optimiser step + next pose
-// forward
+// One dense round: pose blend shapes of the active frames (wgmma GEMM), skinning + box partials, each frame's SDF set-up
+// (sdf_setup, one warp per frame; at <= 4 frames the tail of skin_small instead), the SDF term with the adjoint of its
+// (short) vertex list, and the per-frame closure adjoint + optimiser step + next pose forward
 static int dense_round(mvs_ctx* ctx, float* params_dev, const LbfgsState& S, const LbfgsCfg& cfg, int nst, cudaStream_t st) {
     int rc;
     if ((rc = launch_vertex_fwd_tc(ctx, st, false, true))) return rc;
@@ -574,8 +574,8 @@ static int run_stage(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, con
     return rc ? rc : end_run(ctx, rg, final_loss_dev, o.last_grad, stats, st);
 }
 
-// One closure evaluation through the dense-regime kernels (posedirs_gemm_tc -> skin -> sdf_fused -> frame_step with the
-// optimiser step switched off): mvs_closure in exec mode 3.  Exists so that parity tests can compare the loss and every
+// One closure evaluation through the dense-regime kernels (dense_round: posedirs_gemm_tc -> skin -> sdf_setup -> sdf_fused
+// -> frame_step, with the optimiser step switched off): mvs_closure in exec mode 3.  Exists so that parity tests can compare the loss and every
 // gradient segment of the kernels the optimiser actually runs with the SDF term on (DESIGN.md section 2).
 static int dense_regime_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, cudaStream_t st) {
     const int B = ctx->ws.B;

@@ -351,7 +351,7 @@ sdf_bins_kernel(SdfBinsArgs a, const int* __restrict__ na_ptr) {
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     const float* vf = a.verts + (size_t)slot * a.N * 3;
     const float tr[3] = {a.slot_tr[4 * slot], a.slot_tr[4 * slot + 1], a.slot_tr[4 * slot + 2]};
-    // ---- frame box: the set-up the skinning kernel computed for this frame (the box sdf_fused uses)
+    // ---- frame box: the set-up sdf_setup_kernel (or skin_small_kernel) computed for this frame (the box sdf_fused uses)
     const FrameBox& fbx = a.setup[slot].fb;
     const float centre[3] = {fbx.centre[0], fbx.centre[1], fbx.centre[2]}, scale = fbx.scale;
     float* wb = reinterpret_cast<float*>(hist);                // [32][4] scratch of the projected-box fold
@@ -606,6 +606,15 @@ extern "C" int mvs_debug_sdf_state(mvs_ctx* ctx, float* bboxp, float* slot_tr, v
     for (auto& c : cp)
         if (c.dst && cudaMemcpy(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
     return 0;
+}
+
+// Testing aid, not part of the ABI (tests/test_gpu_sdf_setup_kernel.py): copies the SdfFrameSetup record of every slot
+// [B][208 B] as the last dense round left it.  Synchronises the device first.
+extern "C" int mvs_debug_sdf_setup(mvs_ctx* ctx, void* rec) {
+    const mvs::Workspace& w = ctx->ws;
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+    if (!w.sdf_setup) return -2;
+    return cudaMemcpy(rec, w.sdf_setup, (size_t)w.B * sizeof(mvs::SdfFrameSetup), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
 }
 
 #ifdef MVS_PHASE_DBG

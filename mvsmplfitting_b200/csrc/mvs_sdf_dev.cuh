@@ -16,7 +16,7 @@ namespace mvs {
 
 // ---------------------------------------------------------------------------------- dense regime, v4: fused adjoint
 // sdf_fused_kernel: P CTAs per frame, 1 to kSdfMaxPasses blocks of 256 vertices each.  Per CTA: load the frame's set-up record
-// (box, triangle 0, cone / plane, chunk-cull verdicts; written once per frame by the skinning kernel), sample phi at the <= 8 voxels around each vertex, compact the vertices with a non-zero sample gradient
+// (box, triangle 0, cone / plane, chunk-cull verdicts; written once per frame by sdf_setup_kernel or skin_small_kernel), sample phi at the <= 8 voxels around each vertex, compact the vertices with a non-zero sample gradient
 // (deterministic order: warp, pass, lane) and -- because with the as-written semantics that list holds a handful of
 // vertices -- run the adjoint of the vertex stage for exactly those vertices right here:
 //     d v_posed = T_3x3^T g,   dA_j += W[n,j] [g (x) v_posed | g],   dPhi += d v_posed . Qk[rows of n]
@@ -108,8 +108,8 @@ sdf_fused_kernel(SdfFusedArgs ar, const int* __restrict__ na_ptr, int passes) {
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     if (slot >= na) return;
     if (pidx * passes * kSdfFThreads >= N) return;
-    // ---- prologue: the frame's set-up (box, triangle 0, cone / plane, chunk-cull verdicts; computed once per frame by the
-    //      skinning kernel, sdf_frame_setup), its translation and this CTA's first vertices, all addressed by the slot alone:
+    // ---- prologue: the frame's set-up (box, triangle 0, cone / plane, chunk-cull verdicts; computed once per frame before
+    //      this launch, sdf_frame_setup), its translation and this CTA's first vertices, all addressed by the slot alone:
     //      one round trip
     const SdfFrameSetup* rec = ar.setup + slot;
     const float* vf = verts + (size_t)slot * N * 3;

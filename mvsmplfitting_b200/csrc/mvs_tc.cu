@@ -293,28 +293,19 @@ skin_kernel(SkinArgs ar, const int* __restrict__ na_ptr, int cta_slots) {
             for (int r = 0; r < 3; ++r) { bp[r] = lo[r]; bp[3 + r] = hi[r]; bp[6 + r] = __int_as_float(ilo[r]); bp[9 + r] = __int_as_float(ihi[r]); }
         }
     }
-    if (ar.sdf.rec != nullptr) {                          // per-frame SDF set-up by the last CTA of each frame (sdf_setup_frames)
-        __threadfence();
-        __syncthreads();
-        unsigned* s_mine = reinterpret_cast<unsigned*>(Bb);   // staging buffers are free once every thread is here
-        if (warp == 0) {
-            bool last = false;
-            if (f0 + lane < na) {
-                const int cnt = (nchunks - (int)blockIdx.x + nx - 1) / nx;        // chunks this CTA skinned for each frame
-                last = atomicAdd(ar.sdf.arrive + f0 + lane, cnt) + cnt == nchunks;
-            }
-            const unsigned m = __ballot_sync(0xffffffffu, last);
-            if (lane == 0) *s_mine = m;
-        }
-        __syncthreads();
-        sdf_setup_frames(ar.sdf, bboxp, verts, N, nchunks, f0, *s_mine, warp, lane, kSkinThreads / 32);
-    }
+    // (SDF term on: the frames' set-ups are sdf_setup_kernel's, the next launch)
 }
 
 // The same for a handful of frames (the straggler tail of a fit): with lane = frame almost every lane of skin_kernel
 // idles and its fixed costs (36 KB of transforms per CTA, staging, three barriers per chunk) are pure latency.  Here
-// lane = vertex, a CTA owns one 64-vertex chunk (= one box partial) and loops over the <= kSkinSmallMax frames.
+// lane = vertex, a CTA owns one 64-vertex chunk (= one box partial) and loops over the <= kSkinSmallMax frames.  With the
+// SDF term on and at most kSkinSetupMax frames it also computes the frames' set-ups at its end (sdf_setup_frames), so the
+// smallest rounds keep the four launches the dispatch tests fix (tests/test_gpu_dispatch.py runs 4 frames; DESIGN.md
+// section 5); its 2 warps take ceil(na / 2) set-ups each, one after the other.  Above that
+// sdf_setup_kernel computes them, one set-up deep plus a dependent launch: at 8 frames a round takes 127 us instead of 137
+// (H100, scripts/round_times.py; DESIGN.md section 5 has the sizes below).
 constexpr int kSkinSmallMax = 8;
+constexpr int kSkinSetupMax = 4;
 constexpr int kSkinSmallThreads = 64;
 static_assert(kSkinSmallThreads == kSkinV, "one thread per vertex of a box chunk");
 
@@ -403,6 +394,20 @@ skin_small_kernel(SkinArgs ar, const int* __restrict__ na_ptr) {
     }
 }
 
+// The per-frame SDF set-up after the skinning kernel (SDF term on, more than kSkinSetupMax frames): one warp per active
+// slot calls sdf_frame_setup on the chunk boxes and vertices the previous launch wrote.  In skin_kernel the CTA that
+// completed a frame's chunks computed it, usually the same CTA for all 32 frames of a group, so its 8 warps ran 4 set-ups
+// each, one after the other, at the end of the launch.  Here every frame's set-up runs in parallel with the others.
+constexpr int kSetupWarps = 4;                             // frames per CTA
+__global__ void __launch_bounds__(32 * kSetupWarps)
+sdf_setup_kernel(const SdfSetupArgs sa, const float* bboxp, const float* verts, const int N, const int nbox,
+                 const int* __restrict__ na_ptr) {
+    pdl_wait();                                            // every thread: sdf_fused's wait then also covers the skinning
+    const int slot = blockIdx.x * kSetupWarps + (threadIdx.x >> 5);
+    if (slot >= *na_ptr) return;                           // whole warps: the set-up uses warp-wide reductions
+    sdf_frame_setup(sa, bboxp, verts, N, nbox, slot, threadIdx.x & 31);
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 constexpr int kTcInstances[] = {8, 16, 32, 64, 128};       // wgmma N instances of posedirs_gemm_tc_kernel
 constexpr int kTcNumInst = 5;
@@ -478,13 +483,15 @@ int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool s
         const int rc = dev_alloc(ctx, &T->poffT, (size_t)3 * m.N * w.ldA);
         if (rc) return rc;
     }
+    const int nb = w.na_bound > 0 ? w.na_bound : w.B;             // upper bound of the active-frame count
+    // each frame's SDF set-up: skin_small_kernel's tail at <= kSkinSetupMax frames, else sdf_setup_kernel after the skinning
+    const bool setup_in_skin = sdf_setup && nb <= kSkinSetupMax;
     SdfSetupArgs sd{};
-    if (sdf_setup) {                                    // the skinning kernel also computes each frame's SDF set-up
+    if (sdf_setup) {
         const int rc = ensure_sdf_setup_ws(ctx, st);
         if (rc) return rc;
         sd = make_sdf_setup_args(ctx);
     }
-    const int nb = w.na_bound > 0 ? w.na_bound : w.B;             // upper bound of the active-frame count
     const int ntiles = (3 * m.N + kTcRows - 1) / kTcRows;
     const int nf = tc_cols_for(nb);
     dim3 grid(std::min(ctx->sm_count, ntiles), (nb + kTcCols - 1) / kTcCols);   // surplus CTAs exit: the kernel splits the tiles from *na
@@ -495,7 +502,8 @@ int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool s
                                 : nf == 64 ? launch_gemm<64>(ctx, T, 3, grid, st, ntiles)
                                            : launch_gemm<128>(ctx, T, 4, grid, st, ntiles)));
     const int nchunks = (m.N + kSkinV - 1) / kSkinV, fgroups = (nb + 31) / 32;
-    const SkinArgs sa{T->poffT, m.ST, w.Phi, w.At, w.ldA, m.ell_j, m.ell_w, m.KW, m.N, need_vposed ? w.vposed : nullptr, w.verts, w.bboxp, sd};
+    const SkinArgs sa{T->poffT, m.ST, w.Phi, w.At, w.ldA, m.ell_j, m.ell_w, m.KW, m.N, need_vposed ? w.vposed : nullptr, w.verts, w.bboxp,
+                      setup_in_skin ? sd : SdfSetupArgs{}};
     if (nb <= kSkinSmallMax) {                          // straggler tail: lane = vertex, one chunk per CTA
         MVS_LAUNCH(ctx, KID_SKIN, st,
                    MVS_CUDA_OK(ctx, launch_pdl(skin_small_kernel, dim3(nchunks), dim3(kSkinSmallThreads), 0, st, sa, (const int*)w.na)));
@@ -505,6 +513,10 @@ int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool s
         MVS_LAUNCH(ctx, KID_SKIN, st,
                    MVS_CUDA_OK(ctx, launch_pdl(skin_kernel, g2, dim3(kSkinThreads), kSkinSmem, st, sa, (const int*)w.na, 2 * ctx->sm_count)));
     }
+    if (sdf_setup && !setup_in_skin)
+        MVS_LAUNCH(ctx, KID_SDF_SETUP, st,
+                   MVS_CUDA_OK(ctx, launch_pdl(sdf_setup_kernel, dim3((nb + kSetupWarps - 1) / kSetupWarps), dim3(32 * kSetupWarps), 0, st,
+                                               sd, (const float*)w.bboxp, (const float*)w.verts, m.N, nchunks, (const int*)w.na)));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }

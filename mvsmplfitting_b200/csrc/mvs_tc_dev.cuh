@@ -224,9 +224,10 @@ __device__ __forceinline__ float vposed_of(const float* __restrict__ st11 /* sha
     return __fadd_rn(a, poff);
 }
 
-// Arguments of the skinning kernels (mvs_tc.cu).  verts and bboxp are read back within the launch by the CTA that computes
-// a frame's SDF set-up (sdf_frame_setup), so they are plain pointers.  vposed == nullptr: v_posed is not stored (the few
-// consumers recompute it, vposed_of).
+// Arguments of the skinning kernels (mvs_tc.cu).  verts and bboxp are read back within skin_small_kernel's launch by the CTA
+// that computes a frame's SDF set-up (sdf_frame_setup), so they are plain pointers.  sdf: read by skin_small_kernel only, set
+// at <= kSkinSetupMax frames (otherwise sdf_setup_kernel computes the set-ups).  vposed == nullptr: v_posed is not stored
+// (the few consumers recompute it, vposed_of).
 struct SkinArgs {
     const float* poffT; const float* ST; const float* Phi; const float* At; int ldA;
     const int* ell_j; const float* ell_w; int KW; int N;
@@ -238,8 +239,10 @@ struct SkinArgs {
 // One warp computes frame `slot`'s SdfFrameSetup from the frame's nbox chunk boxes and skinned vertices, with the
 // expressions sdf_fused used to evaluate in every CTA: the box (ties -> lowest vertex index), triangle 0 in box coordinates
 // (fitting.py:362-363), the cone of planes it spans from the corner (-1,-1,-1), the plane of the triangle, the vertex-level
-// pads and the chunk-cull verdicts.  The chunk boxes and vertices were written by other CTAs of the same launch, so they are
-// read through L2 (__ldcg).  Resets the frame's arrival counter for the next round.
+// pads and the chunk-cull verdicts.  Called by sdf_setup_kernel (mvs_tc.cu: one warp per slot, after the skinning kernel)
+// and at the end of skin_small_kernel at <= 4 frames (sdf_setup_frames).  The chunk boxes and vertices were written by other
+// CTAs, in skin_small_kernel of the same launch, so they are read through L2 (__ldcg).  Resets the frame's arrival counter
+// for the next round (sdf_setup_kernel finds it at 0 and leaves it there).
 static __device__ __noinline__ void sdf_frame_setup(const SdfSetupArgs sa, const float* bboxp, const float* verts, const int N,
                                              const int nbox, const int slot, const int lane) {
     const float tr[3] = {sa.slot_tr[4 * slot], sa.slot_tr[4 * slot + 1], sa.slot_tr[4 * slot + 2]};
@@ -398,7 +401,10 @@ static __device__ __noinline__ void sdf_frame_setup(const SdfSetupArgs sa, const
     }
 }
 
-// Arrival protocol of the skinning kernels (SDF term on).  Every CTA has written its chunk boxes and vertices; each thread
+// Arrival protocol of skin_small_kernel (SDF term on, at most kSkinSetupMax frames; with more frames the skinning kernels
+// write only the chunk boxes and vertices, and sdf_setup_kernel computes every frame's set-up in the next launch, one warp
+// per frame).
+// Every CTA has written its chunk boxes and vertices; each thread
 // fences its own writes (__threadfence: visible device-wide before anything it does later), the CTA barrier orders all of
 // them before the one atomicAdd per frame that adds the CTA's chunk count to the frame's counter.  Exactly one CTA sees its
 // add complete the frame's nbox: every other CTA's fence-then-add precedes it in the counter's modification order, so

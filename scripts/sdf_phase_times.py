@@ -2,7 +2,7 @@
 
     python scripts/sdf_phase_times.py [B ...]
 
-Runs dense-regime closures (exec mode 3: posedirs_gemm_tc -> skin -> sdf_fused -> frame_step, one round each) at every batch
+Runs dense-regime closures (exec mode 3: posedirs_gemm_tc -> skin -> sdf_setup -> sdf_fused -> frame_step, one round each) at every batch
 size and prints, per CTA that ran to the end, the mean and the largest time of each phase (see the SDF_MARK stamps in
 mvs_sdf.cu), then the CTAs per launch, the waves they make at 3 CTAs/SM and waves x mean CTA time against the kernel's event
 time per launch (profiled in a separate loop of the same build)."""
