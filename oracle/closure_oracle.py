@@ -39,9 +39,12 @@ class OracleModel:
     faces: torch.Tensor | None
     model_type: str = "smpllsp"
     dtype: torch.dtype = torch.float32
+    joint_map: tuple | None = None          # keypoint k = source joint_map[k]; None: MAP_LSP14 / MAP_COCO17 by model_type
+    extra_vertex_ids: tuple | None = None   # vertices appended to the source joints; None: FACE_IDS
 
     @staticmethod
-    def from_numpy(model: dict, dtype=torch.float32, model_type="smpllsp") -> "OracleModel":
+    def from_numpy(model: dict, dtype=torch.float32, model_type="smpllsp", joint_map=None,
+                   extra_vertex_ids=None) -> "OracleModel":
         t = lambda a: torch.tensor(np.asarray(a, dtype=np.float64), dtype=dtype)
         pd = np.reshape(np.asarray(model["posedirs"]), [-1, model["posedirs"].shape[-1]]).T
         parents = [int(x) for x in np.asarray(model["kintree_table"][0]).astype(np.int64)]
@@ -51,7 +54,9 @@ class OracleModel:
             J_regressor=t(model["J_regressor"]), parents=parents, lbs_weights=t(model["weights"]),
             lsp_regressor=t(model["lsp_regressor"]),
             faces=None if model.get("f") is None else torch.tensor(np.asarray(model["f"], dtype=np.int64)),
-            model_type=model_type, dtype=dtype)
+            model_type=model_type, dtype=dtype,
+            joint_map=None if joint_map is None else tuple(int(j) for j in joint_map),
+            extra_vertex_ids=None if extra_vertex_ids is None else tuple(int(v) for v in extra_vertex_ids))
 
 
 def rodrigues(rot_vecs: torch.Tensor) -> torch.Tensor:
@@ -100,7 +105,7 @@ def rigid_chain(rot_mats, joints, parents, scale):
 def smpl_forward(om: OracleModel, betas, global_orient, body_pose, transl, scale):
     """body_models_scale.py:327-412 + lbs.py:135-222 for ONE frame.
     Inputs are [1,10],[1,3],[1,69],[1,3],[1,1].  Returns vertices [N,3] (with transl),
-    keypoints [17,3], full_pose [1,72]."""
+    keypoints [K,3] (K = 17 for the default keypoint maps), full_pose [1,72]."""
     full_pose = torch.cat([global_orient, body_pose], dim=1)
     v_shaped = om.v_template + torch.einsum("bl,mkl->bmk", betas, om.shapedirs)[0]   # lbs.py:179,265
     J = torch.einsum("ik,ji->jk", v_shaped, om.J_regressor)                           # lbs.py:183,242
@@ -117,7 +122,10 @@ def smpl_forward(om: OracleModel, betas, global_orient, body_pose, transl, scale
     else:
         joints = posed_joints
         jmap = MAP_COCO17
-    joints = torch.cat([joints, verts[list(FACE_IDS)]], dim=0)                        # vertex_joint_selector.py:73-77
+    if om.joint_map is not None:
+        jmap = om.joint_map
+    extra = FACE_IDS if om.extra_vertex_ids is None else om.extra_vertex_ids
+    joints = torch.cat([joints, verts[list(extra)]], dim=0)                           # vertex_joint_selector.py:73-77
     joints = joints[list(jmap)]                                                       # utils/utils.py:420-424
     joints = joints + transl                                                          # body_models_scale.py:401-403
     verts = verts + transl

@@ -13,6 +13,11 @@ them, parameters), so its float64 result is the same operation carried out in hi
 own: vertices and joints relative to that frame's largest |coordinate|, the loss relative to itself, and every gradient
 segment (betas, orient, pose, transl, scale) relative to its own largest entry.
 
+The same matrix runs at the limits of the frame-resident kernels (EDGE_CONFIGS, built by tests/model_variants.py): 1, 8 and
+9 GMM components, 86, 90 and 91 support vertices, keypoint entries and support-joint pairs past what shared memory stages,
+9 skinning weights per vertex, custom keypoint sets of 18 and 32 keypoints on both sides of the view-keypoint limit, and
+poses on both sides of the pose-prior and bending cut-offs.  Each case asserts which kernels ran.
+
 Each bar below is at most about 4x the worst value measured on an NVIDIA H100 80GB HBM3 (400 W power limit) and never
 looser than the 1e-4 parity bar used elsewhere in the suite; the measured worst case is written next to it.  Every test
 prints its worst errors next to its bars (run with -s).
@@ -25,6 +30,7 @@ from mvsmplfitting_b200 import synthetic as S
 from oracle import closure_oracle as O
 from oracle import sdf_oracle
 from tests import golden_util as G
+from tests import model_variants as MV
 
 pytestmark = pytest.mark.gpu
 
@@ -34,6 +40,8 @@ EDGE_FRAMES = sorted({0} | {b - 1 for b in BATCHES} | {e + d for e in range(32, 
 SEGS = dict(betas=(0, 10), global_orient=(10, 13), body_pose=(13, 82), transl=(82, 85), scale=(85, 86))
 # bench.py's stage 2 (cfg_files/fit_smpl.yaml stage 3 of 4), the first stage with the SDF term
 W2 = dict(data_weight=500.0 / 1536, body_pose_weight=57.4, shape_weight=10.0, bending_prior_weight=3.17 * 57.4)
+# bench.py's last stage (4 of 4): the GMM pose prior is active (its minimum NLL x 4.78^2 stays under the 5e4 cut-off)
+W3 = dict(data_weight=500.0 / 1536, body_pose_weight=4.78, shape_weight=5.0, bending_prior_weight=3.17 * 4.78)
 F64 = torch.float64
 
 # ---- bars (measured worst on the H100 in the comment)
@@ -41,15 +49,22 @@ BAR_GEOM = 1e-6            # A: vertices / joints, both exec modes, both joint s
 BAR_LOSS = 1.5e-6          # B: loss, exec modes 0, 1 and 3 (worst 4.4e-7)
 BAR_GRAD = dict(betas=5e-6, global_orient=1e-4, body_pose=1e-6, transl=1e-4, scale=1e-4)
 #                 B: per segment (worst 1.4e-6, 5.0e-5, 2.5e-7, 2.9e-5, 7.8e-5)
+# B at the limits of the frame-resident kernels (EDGE_CONFIGS), exec modes 0, 1 and 3.  The active GMM prior adds a
+# 69-term product with the float32 precision matrices to the pose gradient, and the cut-off cases run extreme poses.
+BAR_EDGE_LOSS = 1.5e-6     # worst 4.1e-7 (K32_V9)
+BAR_EDGE_GRAD = dict(betas=1e-5, global_orient=2e-5, body_pose=5e-6, transl=1.5e-5, scale=1e-4)
+#                 worst 2.6e-6 (gmm1), 4.7e-6 (kpe_wide), 1.3e-6 (gmm8), 4.5e-6 (gmm8), 5.2e-5 (cut_l2_s2)
+BAR_EDGE_JOINTS = 5e-6     # keypoints relative to the frame's largest |coordinate| (worst 1.3e-6, cut_l2_s3)
+BAR_PROJ = 5e-7            # projections relative to the frame's largest |uv| (worst 1.2e-7, cut_l2_s3)
 BAR_SDF_LOSS = 2e-5        # C: loss with the real SDF weight (worst 5.2e-6)
 BAR_SDF_GRAD = 4e-4        # C: per segment, plus float32 noise (FP32_NOISE); worst 1.4e-4 without the noise allowance,
 #                            0.64 of the allowance with it (scale, frame 159)
 
 
-def make_ctx(model, gmm, cams, B, model_type="smpllsp", mode=0):
+def make_ctx(model, gmm, cams, B, model_type="smpllsp", mode=0, jmap=None):
     from mvsmplfitting_b200.context import FittingContext
     ctx = FittingContext(0)
-    ctx.set_model(model, model_type=model_type)
+    ctx.set_model(model, model_type=model_type, **(jmap or {}))
     ctx.set_gmm_from_dict(gmm)
     ctx.set_cameras(cams["R"], cams["t"], cams["f"], cams["c"])
     ctx.set_batch(B)
@@ -60,10 +75,11 @@ def make_ctx(model, gmm, cams, B, model_type="smpllsp", mode=0):
 _OM = {}
 
 
-def oracle_model(model, model_type, dtype=F64):
-    key = (model_type, dtype)
+def oracle_model(model, model_type, dtype=F64, variant=None, jmap=None):
+    key = (model_type, dtype, variant, jmap)
     if key not in _OM:
-        _OM[key] = O.OracleModel.from_numpy(model, dtype=dtype, model_type=model_type)
+        kp = MV.KEYPOINT_SETS[jmap] if jmap else {}
+        _OM[key] = O.OracleModel.from_numpy(MV.make_variant(variant, model), dtype=dtype, model_type=model_type, **kp)
     return _OM[key]
 
 
@@ -182,21 +198,129 @@ CONFIGS = dict(
     V2=dict(V=2),
     V16=dict(V=16),
 )
+_SEED_INDEX = {n: i for i, n in enumerate(sorted(CONFIGS))}
+# The limits of the frame-resident kernels (tests/model_variants.py), each from one side or both.  Keys: model (a variant of
+# make_model(0)), gmm_m (components of make_gmm(7, M)), jmap (a custom keypoint set), V, pose (how the checked frames' poses
+# are chosen), cut (prior cut-off case: prior kind and body_pose_weight).  The GMM variants run at the last stage's weights
+# (W3), where the prior is active, with each checked frame posed near one component's mean so that every component index
+# (the last one included) is the minimum somewhere.
+EDGE_CONFIGS = dict(
+    gmm1=dict(gmm_m=1, weights=W3, pose="gmm_means"),
+    gmm8=dict(gmm_m=8, weights=W3, pose="gmm_means"),                    # M = kResMaxM
+    gmm9=dict(gmm_m=9, weights=W3, pose="gmm_means"),                    # batched chain
+    sup86=dict(model="sup86"),                                           # the real SMPL's support size
+    sup90=dict(model="sup90"),                                           # nsup + 6 = kResMaxSup: full support arrays
+    sup91=dict(model="sup91"),                                           # batched chain
+    kpe_wide=dict(model="kpe_wide"),                                     # 269 keypoint entries: kp_on = 0
+    skin_dense=dict(model="skin_dense"),                                 # 531 support-joint pairs: sj_on = 0; KW = 8
+    skin_kw9=dict(model="skin_kw9"),                                     # KW = 9: skin_kernel reads the ELL from global
+    K18_V15=dict(jmap="K18", V=15),                                      # 270 view-keypoints
+    K18_V16=dict(jmap="K18", V=16),                                      # 288: batched chain
+    K32_V8=dict(jmap="K32", V=8),                                        # 256
+    K32_V9=dict(jmap="K32", V=9),                                        # 288: batched chain
+    V16_smpl=dict(model_type="smpl", V=16),                              # 272 with the chain-joint keypoints
+    cut_gmm_s3=dict(cut=("gmm", 4.78)),
+    cut_gmm_s2=dict(cut=("gmm", 57.4)),
+    cut_l2_s3=dict(cut=("l2", 4.78)),
+    cut_l2_s2=dict(cut=("l2", 57.4)),
+)
+_SEED_INDEX.update({n: 100 + i for i, n in enumerate(EDGE_CONFIGS)})
+CONFIGS.update(EDGE_CONFIGS)
 B_SMALL, B_LARGE = 5, 40            # skin_small_kernel + N = 8;  skin_kernel over two 32-frame groups + N = 64
 CHECK_FRAMES = (0, 1, 2, 3, 4, 30, 31, 32, 33, 39)
 CW_SMALL = 3e-3                   # SDF term on, but its oracle value stays below 1e-7 of every frame's loss
+PPRIOR_CUT, ANGLE_CUT = 5e4, 1e4  # fitting.py:334-335, :349-350
+GATE_MARGIN = 1e-3                # no checked frame this close (relative) to a cut-off: the terms are discontinuous there
+
+_VARIANTS, _GMMS = {}, {}
 
 
-def config_case(model, name, V=None, seed=700):
-    """frames, parameters, loss settings and the float64 oracle of the CHECK_FRAMES for configuration `name`"""
+def variant_model(model, name):
+    if name not in _VARIANTS:
+        _VARIANTS[name] = MV.make_variant(name, model)
+    return _VARIANTS[name]
+
+
+def variant_gmm(gmm, M):
+    if M is None:
+        return gmm
+    if M not in _GMMS:
+        _GMMS[M] = S.make_gmm(7, num_gaussians=M)
+    return _GMMS[M]
+
+
+def _frame_rank(i):
+    """position of frame i among the checked frames (its own index for the others)"""
+    return CHECK_FRAMES.index(i) if i in CHECK_FRAMES else i
+
+
+def _custom_keypoints(case, rng):
+    """detections for a custom keypoint set: the float64 oracle keypoints of the generator's ground truth, projected, plus
+    noise; confidences with zeros, one whole view of frame 2 among them; joint_weights of length K"""
+    om = oracle_model(case["base"], case["model_type"], variant=case["variant"], jmap=case["jmap"])
+    Xg = S.pack_params(case["fr"]["gt"])
+    joints = np.stack([oracle_forward(om, Xg[i])[1].numpy() for i in range(B_LARGE)])
+    V, K = case["V"], joints.shape[1]
+    uv = S.project_np(case["cams"], joints) + rng.normal(0, 5.0, size=(V, B_LARGE, K, 2))
+    conf = rng.uniform(0.6, 0.95, size=(V, B_LARGE, K))
+    conf[rng.uniform(size=conf.shape) < 0.1] = 0.0
+    conf[V - 1, 2] = 0.0
+    fr = dict(case["fr"], gt_uv=uv.astype(np.float32), conf=conf.astype(np.float32),
+              joint_weights=rng.uniform(0.5, 1.5, K).astype(np.float32))
+    return fr
+
+
+def _pose_at_gates(X, i, kind, bpw, gmm32, rng):
+    """pose of frame i with its pose prior and bending term on chosen sides of their cut-offs: the bending entry
+    (52, 55, 9 or 12 by frame) sets the bending term, then the other entries are scaled until the pose prior hits its target"""
+    k = _frame_rank(i)
+    bend = 3.17 * bpw
+    p_above, a_above = k % 2 == 1, (k // 2) % 2 == 1
+    pose = X[i, 13:82].astype(np.float64)
+    e = MV.ANGLE_IDX[k % 4]
+    sg = MV.ANGLE_SIGN[k % 4]
+    r_a = rng.uniform(1.5, 3.0) if a_above else rng.uniform(0.2, 0.6)
+    rest = pose.copy()
+    rest[list(MV.ANGLE_IDX)] = 0.0
+    base = np.zeros(69)
+    base[list(MV.ANGLE_IDX)] = pose[list(MV.ANGLE_IDX)] * 0.1
+    others = bend * sum(np.exp(base[j] * s) ** 2 for j, s in zip(MV.ANGLE_IDX, MV.ANGLE_SIGN) if j != e)
+    base[e] = sg * 0.5 * np.log((r_a * ANGLE_CUT - others) / bend)
+    f = lambda s: MV.prior_gates(base + s * rest, kind, bpw, bend, gmm32)[0]
+    if kind == "gmm" and bpw > 10:            # min NLL >= 65 for make_gmm: always above the cut-off at this weight
+        s = 1.0
+    else:
+        target = PPRIOR_CUT * (rng.uniform(2.0, 4.0) if p_above else rng.uniform(0.5, 0.9))
+        lo, hi = 0.0, 1.0
+        assert f(lo) < target, (i, f(lo), target)
+        while f(hi) < target:
+            hi *= 2.0
+        for _ in range(80):
+            mid = 0.5 * (lo + hi)
+            lo, hi = (mid, hi) if f(mid) < target else (lo, mid)
+        s = 0.5 * (lo + hi)
+    X[i, 13:82] = (base + s * rest).astype(np.float32)
+
+
+def config_case(model, gmm, name, V=None, seed=700):
+    """frames, parameters and loss settings of configuration `name`: the model variant, GMM and keypoint set it names, and
+    which side of each kernel limit it is on"""
     c = CONFIGS[name]
     V = V if V is not None else c.get("V", 4)
     model_type = c.get("model_type", "smpllsp")
-    loss = dict(body_prior="gmm", **W2)
+    variant, jmap, M = c.get("model"), c.get("jmap"), c.get("gmm_m")
+    mdl, gm = variant_model(model, variant), variant_gmm(gmm, M)
+    weights = c.get("weights", W2)
+    if "cut" in c:
+        kind, bpw = c["cut"]
+        weights = dict(W2 if bpw > 10 else W3, body_pose_weight=bpw, bending_prior_weight=3.17 * bpw)
+    loss = dict(body_prior="gmm", **weights)
+    if "cut" in c:
+        loss["body_prior"] = c["cut"][0]
     loss.update(c.get("loss", {}))
     frozen = loss.get("frozen", ())
     cams = S.make_cameras(V)
-    fr = S.make_frames(model, cams, B_LARGE, seed=seed + sorted(CONFIGS).index(name), model_type=model_type)
+    fr = S.make_frames(mdl, cams, B_LARGE, seed=seed + _SEED_INDEX[name], model_type=model_type)
     rng = np.random.RandomState(seed)
     X = S.pack_params(fr["init"])
     X[:, 0:10] = 0.5 * fr["gt"]["betas"]
@@ -205,15 +329,46 @@ def config_case(model, name, V=None, seed=700):
     if c.get("anchor"):
         anchor = (X + rng.normal(0, 0.05, X.shape)).astype(np.float32)
         weight = rng.uniform(0, 3, X.shape).astype(np.float32)
-    return dict(V=V, model_type=model_type, loss=loss, frozen=frozen, cams=cams, fr=fr, X=X, anchor=anchor, weight=weight)
+    kp = MV.KEYPOINT_SETS[jmap] if jmap else {}
+    bk = MV.bookkeeping(mdl, model_type, **kp)
+    case = dict(name=name, V=V, model_type=model_type, loss=loss, frozen=frozen, cams=cams, fr=fr, X=X, anchor=anchor,
+                weight=weight, base=model, variant=variant, jmap=jmap, model=mdl, gmm=gm, kp=kp, bk=bk,
+                branches=MV.branches(bk, V, gm["means"].shape[0]))
+    if jmap:
+        case["fr"] = _custom_keypoints(case, rng)
+    gmm32 = MV.gmm_buffers_f32(gm)
+    if c.get("pose") == "gmm_means":          # frame i near component (its rank mod M)
+        for i in range(B_LARGE):
+            X[i, 13:82] = gm["means"][_frame_rank(i) % M] + rng.normal(0, 0.05, 69)
+        best = [MV.gmm_nll_min(gmm32, X[i, 13:82])[1] for i in CHECK_FRAMES]
+        assert best == [k % M for k in range(len(CHECK_FRAMES))], best
+        assert max(MV.prior_gates(X[i, 13:82], "gmm", loss["body_pose_weight"], loss["bending_prior_weight"], gmm32)[0]
+                   for i in CHECK_FRAMES) < 0.5 * PPRIOR_CUT
+    if "cut" in c:
+        kind, bpw = c["cut"]
+        for i in range(B_LARGE):
+            _pose_at_gates(X, i, kind, bpw, gmm32, rng)
+        g = np.array([MV.prior_gates(X[i, 13:82], kind, bpw, 3.17 * bpw, gmm32) for i in CHECK_FRAMES])
+        for col, cut in ((0, PPRIOR_CUT), (1, ANGLE_CUT)):
+            assert np.abs(g[:, col] / cut - 1.0).min() > GATE_MARGIN, (name, col, g[:, col])
+        above = g / np.array([PPRIOR_CUT, ANGLE_CUT]) > 1.0
+        assert (above[:, 1].sum() >= 3 and (~above[:, 1]).sum() >= 3), (name, g[:, 1])
+        if kind == "gmm" and bpw > 10:
+            assert above[:, 0].all(), (name, g[:, 0])            # the GMM term is always cut at this weight
+        else:
+            assert above[:, 0].sum() >= 3 and (~above[:, 0]).sum() >= 3, (name, g[:, 0])
+        case["gates"] = g
+    return case
 
 
-def oracle_case(case, model, gmm):
-    om = oracle_model(model, case["model_type"])
+def oracle_case(case):
+    """the float64 oracle of the CHECK_FRAMES of a case"""
+    om = oracle_model(case["base"], case["model_type"], variant=case["variant"], jmap=case["jmap"])
     lo = case["loss"]
     cfg = O.LossConfig(rho=lo.get("rho", 100.0), use_joints_conf=lo.get("use_joints_conf", True),
-                       fix_shape=lo.get("fix_shape", False), **W2)
-    pri = oracle_priors(gmm, lo["body_prior"])
+                       fix_shape=lo.get("fix_shape", False),
+                       **{k: lo[k] for k in ("data_weight", "body_pose_weight", "shape_weight", "bending_prior_weight")})
+    pri = oracle_priors(case["gmm"], lo["body_prior"])
     cams_t = O.cams_to_torch(case["cams"], F64)
     fr, X = case["fr"], case["X"]
     ref = {}
@@ -229,12 +384,15 @@ def oracle_case(case, model, gmm):
             a, e = SEGS[f]
             grad[a:e] = 0.0
         res = np.abs(fr["gt_uv"][:, i].astype(np.float64) - r["proj"]).max()
-        ref[i] = dict(loss=loss, grad=grad, res=res)
+        ref[i] = dict(loss=loss, grad=grad, res=res, joints=r["joints"], proj=r["proj"])
     return ref
 
 
+def case_ctx(case, B, mode=0):
+    return make_ctx(case["model"], case["gmm"], case["cams"], B, case["model_type"], mode, case["kp"])
 
-def run_closure(ctx, case, B, mode, sdf):
+
+def run_closure(ctx, case, B, mode, sdf, want_geom=False):
     fr, X = case["fr"], case["X"]
     ctx.set_exec_mode(mode)
     ctx.set_keypoints(*batch_frames(fr, range(B)), fr["joint_weights"])
@@ -246,20 +404,25 @@ def run_closure(ctx, case, B, mode, sdf):
     ctx.set_loss(**kw)
     x = torch.tensor(X[:B], device="cuda")
     ctx.profile(0xFFFFFFFF)
-    out = ctx.closure(x)
+    out = ctx.closure(x, want_joints=want_geom, want_proj=want_geom)
     prof = ctx.profile_read()
     ctx.profile(0)
-    return out["loss"].cpu().numpy(), out["grad"].cpu().numpy(), prof
+    res = (out["loss"].cpu().numpy(), out["grad"].cpu().numpy(), prof)
+    if want_geom:
+        res += (out["joints"].cpu().numpy(), out["proj"].cpu().numpy())
+    return res
 
 
 def compare_case(worst, tag, case, ref, loss, grad, B):
+    edge = case["name"] in EDGE_CONFIGS
+    bar_loss, bar_grad = (BAR_EDGE_LOSS, BAR_EDGE_GRAD) if edge else (BAR_LOSS, BAR_GRAD)
     for i in (i for i in CHECK_FRAMES if i < B):
-        worst.add(tag + " loss", abs(float(loss[i]) - ref[i]["loss"]) / abs(ref[i]["loss"]), BAR_LOSS, (B, i))
+        worst.add(tag + " loss", abs(float(loss[i]) - ref[i]["loss"]) / abs(ref[i]["loss"]), bar_loss, (B, i))
         for n, (a, e) in SEGS.items():
             if n in case["frozen"]:
                 assert np.all(grad[i, a:e] == 0.0), (tag, B, i, n, "frozen segment must be exactly zero")
                 continue
-            worst.add(tag + " grad " + n, G.relmax(grad[i, a:e], ref[i]["grad"][a:e]), BAR_GRAD[n], (B, i))
+            worst.add(tag + " grad " + n, G.relmax(grad[i, a:e], ref[i]["grad"][a:e]), bar_grad[n], (B, i))
 
 
 @pytest.mark.parametrize("name", list(CONFIGS))
@@ -269,10 +432,11 @@ def test_dense_closure_matches_float64(name, syn_model, syn_gmm):
     the 32-frame edge at B = 40 (skin_kernel, N = 64, 2 blocks per sdf_fused CTA).  The SDF term is on with a weight so small
     that the oracle's penetration term stays below 1e-7 of every compared loss (asserted), so the comparison isolates the
     data and prior arithmetic from the discontinuous as-written SDF field.  Frozen segments must be exactly zero, and frames
-    0-4 must give the same bits at B = 5 and at B = 40."""
-    case = config_case(syn_model, name)
-    ref = oracle_case(case, syn_model, syn_gmm)
-    om = oracle_model(syn_model, case["model_type"])
+    0-4 must give the same bits at B = 5 and at B = 40.  A configuration outside the frame-resident envelope (more support
+    vertices, view-keypoints or GMM components than frame_step holds) must run the batched chain instead."""
+    case = config_case(syn_model, syn_gmm, name)
+    ref = oracle_case(case)
+    om = oracle_model(syn_model, case["model_type"], variant=case["variant"], jmap=case["jmap"])
     pen_ratio = max(oracle_penetration(om, case["X"][i], CW_SMALL, 128) / ref[i]["loss"] for i in CHECK_FRAMES)
     assert pen_ratio < 1e-7, pen_ratio
     if name == "rho10":         # frames whose residuals reach GMoF's saturating region
@@ -280,11 +444,14 @@ def test_dense_closure_matches_float64(name, syn_model, syn_gmm):
     worst = Worst("B dense " + name)
     bits = {}
     for B in (B_SMALL, B_LARGE):
-        ctx = make_ctx(syn_model, syn_gmm, case["cams"], B, case["model_type"])
+        ctx = case_ctx(case, B)
         loss, grad, prof = run_closure(ctx, case, B, 3, sdf=True)
         ctx.close()
-        assert prof.get("frame_step", (0, 0))[1] == 1 and prof.get("skin", (0, 0))[1] == 1, prof
-        assert "keypoint_loss" not in prof, prof                # not the batched reference chain
+        if case["branches"]["resident"]:
+            assert prof.get("frame_step", (0, 0))[1] == 1 and prof.get("skin", (0, 0))[1] == 1, prof
+            assert "keypoint_loss" not in prof, prof                # not the batched reference chain
+        else:
+            assert "keypoint_loss" in prof and "frame_step" not in prof and "skin" not in prof, prof
         compare_case(worst, "mode3", case, ref, loss, grad, B)
         bits[B] = (loss[:B_SMALL], grad[:B_SMALL])
     assert np.array_equal(bits[B_SMALL][0], bits[B_LARGE][0]) and np.array_equal(bits[B_SMALL][1], bits[B_LARGE][1])
@@ -293,19 +460,51 @@ def test_dense_closure_matches_float64(name, syn_model, syn_gmm):
 
 
 @pytest.mark.parametrize("V", [1, 2])
-@pytest.mark.parametrize("name", [n for n in CONFIGS if not n.startswith("V")])
+@pytest.mark.parametrize("name", [n for n in CONFIGS if not n.startswith("V") and n not in EDGE_CONFIGS])
 def test_resident_and_batched_closure_match_float64_few_views(name, V, syn_model, syn_gmm):
     """The configuration matrix of test_dense_closure_matches_float64 without the SDF term, at one and two views, through the
     frame-resident closure (exec mode 0) and the batched kernel chain (exec mode 1), against closure_eval in float64."""
-    case = config_case(syn_model, name, V=V)
-    ref = oracle_case(case, syn_model, syn_gmm)
+    case = config_case(syn_model, syn_gmm, name, V=V)
+    ref = oracle_case(case)
     worst = Worst("B V=%d %s" % (V, name))
     for B in (B_SMALL, B_LARGE):
-        ctx = make_ctx(syn_model, syn_gmm, case["cams"], B, case["model_type"])
+        ctx = case_ctx(case, B)
         for mode, kid in ((0, "closure_resident"), (1, "keypoint_loss")):
             loss, grad, prof = run_closure(ctx, case, B, mode, sdf=False)
             assert kid in prof, (mode, prof)
             compare_case(worst, "mode%d" % mode, case, ref, loss, grad, B)
+        ctx.close()
+    worst.report()
+
+
+@pytest.mark.parametrize("name", list(EDGE_CONFIGS))
+def test_closure_at_the_resident_limits_matches_float64(name, syn_model, syn_gmm):
+    """Exec mode 0 (the frame-resident closure where the configuration fits it, the batched chain where it does not) and
+    exec mode 1 (the batched chain) at the limits of the frame-resident kernels: loss, keypoints, projections and every
+    gradient segment of the checked frames against closure_eval in float64, at B = 5 and B = 40.  Which kernel ran is read
+    from the profile; the branch each configuration reaches inside the kernel is asserted from the host mirror of
+    mvs_set_model (tests/test_model_variants.py)."""
+    case = config_case(syn_model, syn_gmm, name)
+    ref = oracle_case(case)
+    br = case["branches"]
+    if "gates" in case:
+        print("[B limits %s] pose prior / 5e4: %s   bending / 1e4: %s" % (
+            name, np.round(case["gates"][:, 0] / PPRIOR_CUT, 2).tolist(), np.round(case["gates"][:, 1] / ANGLE_CUT, 2).tolist()))
+    worst = Worst("B limits " + name)
+    for B in (B_SMALL, B_LARGE):
+        ctx = case_ctx(case, B)
+        for mode in (0, 1):
+            loss, grad, prof, joints, proj = run_closure(ctx, case, B, mode, sdf=False, want_geom=True)
+            if mode == 0 and br["resident"]:
+                assert "closure_resident" in prof and "keypoint_loss" not in prof, prof
+            else:
+                assert "keypoint_loss" in prof and "closure_resident" not in prof, (mode, prof)
+            tag = "mode%d" % mode
+            compare_case(worst, tag, case, ref, loss, grad, B)
+            for i in (i for i in CHECK_FRAMES if i < B):
+                jo, po = ref[i]["joints"], ref[i]["proj"]
+                worst.add(tag + " joints", np.abs(joints[i] - jo).max() / np.abs(jo).max(), BAR_EDGE_JOINTS, (B, i))
+                worst.add(tag + " proj", np.abs(proj[:, i] - po).max() / np.abs(po).max(), BAR_PROJ, (B, i))
         ctx.close()
     worst.report()
 

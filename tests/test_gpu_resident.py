@@ -121,3 +121,44 @@ def test_dense_regime_lbfgs_matches_batched_lbfgs(syn_model, syn_gmm):
     assert abs(a["st"]["frame_evals"] - b["st"]["frame_evals"]) <= b["st"]["frame_evals"] // 4
     # (final losses are NOT compared: with a discontinuous term the two arithmetic paths legitimately end in
     #  different local minima for some frames; every single evaluation is what must agree, checked above)
+
+
+# the configurations of test_gpu_dense_parity.py that sit inside the frame-resident envelope at one of its limits:
+# 8 GMM components, 90 support vertices, kp_on = 0, sj_on = 0, 32 keypoints x 8 views, 16 views x 17 chain-joint keypoints
+RESIDENT_LIMITS = ("gmm8", "sup90", "kpe_wide", "skin_dense", "K32_V8", "V16_smpl")
+
+
+@pytest.mark.parametrize("name", RESIDENT_LIMITS)
+def test_resident_lbfgs_first_step_at_the_limits_follows_float64_gradient(name, syn_model, syn_gmm):
+    """lbfgs_resident_kernel through the same branches as the closure kernel: one L-BFGS iteration of frames 0-4 in exec
+    mode 0.  The loss at entry must equal the frame-resident closure's loss, and the first step is steepest descent, so on
+    every frame that moved it must point along the float64 oracle's negative gradient."""
+    from tests import test_gpu_dense_parity as P
+    case = P.config_case(syn_model, syn_gmm, name)
+    assert case["branches"]["resident"], case["branches"]
+    ref = P.oracle_case(case)
+    B = P.B_SMALL
+    ctx = P.case_ctx(case, B)
+    ctx.set_keypoints(*P.batch_frames(case["fr"], range(B)), case["fr"]["joint_weights"])
+    ctx.set_loss(**case["loss"])
+    x0 = torch.tensor(case["X"][:B], device="cuda")
+    c0 = ctx.closure(x0)["loss"].cpu().numpy()
+    x1 = x0.clone()
+    ctx.profile(0xFFFFFFFF)
+    f1, st = ctx.lbfgs_run(x1, ctx.make_lbfgs_config(max_outer=1, max_iter=1))
+    prof = ctx.profile_read()
+    ctx.profile(0)
+    f1, step = f1.cpu().numpy(), x1.cpu().numpy() - case["X"][:B]
+    ctx.close()
+    assert "lbfgs_resident" in prof and "keypoint_loss" not in prof, prof
+    assert st["frames_nan"] == 0
+    assert G.relmax(f1, c0.astype(np.float64)) < 1e-6, (f1, c0)
+    moved = np.abs(step).max(axis=1) > 0
+    assert moved.sum() >= B - 1, moved
+    cos = []
+    for i in np.flatnonzero(moved):
+        g = ref[i]["grad"]
+        cos.append(-(step[i] * g).sum() / (np.linalg.norm(step[i]) * np.linalg.norm(g)))
+    print("[resident lbfgs %s] entry loss vs closure %.1e, cos(step, -grad64) min %.7f over %d frames" % (
+        name, G.relmax(f1, c0.astype(np.float64)), min(cos), len(cos)))
+    assert min(cos) > 0.9999, cos
