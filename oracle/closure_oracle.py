@@ -290,10 +290,15 @@ def closure_eval_batch(om, cfg, pri, cams_t, X, gt_uv, conf, joint_weights, back
 
 
 def closure_eval_vposer(om: OracleModel, cfg: LossConfig, pri: OraclePriors, cams_t: dict, x86: np.ndarray, z: np.ndarray,
-                        vposer_w: dict, gt_uv: np.ndarray, conf: np.ndarray, joint_weights: np.ndarray):
+                        vposer_w: dict, gt_uv: np.ndarray, conf: np.ndarray, joint_weights: np.ndarray, body_pose=None):
     """fitting_func() with use_vposer=True for ONE frame (fitting.py:162-203): body_pose = VPoser.decode(z, 'aa');
     the 69 pose entries of x86 are ignored.  Returns dict(loss, grad_* for betas / global_orient / transl / scale /
-    pose_embedding, joints, body_pose)."""
+    pose_embedding / body_pose (the decoded pose), joints, proj [V,K,2], body_pose, terms (per-term values of
+    smplify_loss)).
+
+    The decoder runs in om.dtype: float32 weights (what a device context uploads) are widened exactly to float64.
+    body_pose [69]: evaluate at this pose instead of decode(z) -- the caller decoded it (use_vposer = 1, the drop-in
+    mode); z then only enters the |z|^2 prior, and g_pose_embedding is that prior's gradient alone."""
     from . import vposer_oracle as VO
     dt = om.dtype
     x = torch.tensor(np.asarray(x86, dtype=np.float64), dtype=dt)
@@ -302,13 +307,18 @@ def closure_eval_vposer(om: OracleModel, cfg: LossConfig, pri: OraclePriors, cam
     tr = x[82:85].clone().view(1, 3).requires_grad_(True)
     sc = x[85:86].clone().view(1, 1).requires_grad_(True)
     emb = torch.tensor(np.asarray(z, dtype=np.float64), dtype=dt).view(1, 32).requires_grad_(True)
-    bp = VO.decode_aa(vposer_w, emb)
+    if body_pose is None:
+        bp = VO.decode_aa(vposer_w, emb)
+    else:
+        bp = torch.tensor(np.asarray(body_pose, dtype=np.float64), dtype=dt).view(1, 69).requires_grad_(True)
     verts, joints, full_pose = smpl_forward(om, betas, go, bp, tr, sc)
-    total, proj = smplify_loss(om, cfg, pri, cams_t, verts, joints, full_pose, betas, bp, torch.tensor(gt_uv, dtype=dt),
-                               torch.tensor(conf, dtype=dt), torch.tensor(joint_weights, dtype=dt), pose_embedding=emb)
-    g = torch.autograd.grad(total, [betas, go, tr, sc, emb])
-    names = ("betas", "global_orient", "transl", "scale", "pose_embedding")
-    out = dict(loss=float(total), joints=joints.detach().numpy().copy(), body_pose=bp.detach().numpy()[0].copy())
+    total, proj, terms = smplify_loss(om, cfg, pri, cams_t, verts, joints, full_pose, betas, bp,
+                                      torch.tensor(gt_uv, dtype=dt), torch.tensor(conf, dtype=dt),
+                                      torch.tensor(joint_weights, dtype=dt), pose_embedding=emb, return_terms=True)
+    g = torch.autograd.grad(total, [betas, go, tr, sc, emb, bp])
+    names = ("betas", "global_orient", "transl", "scale", "pose_embedding", "body_pose")
+    out = dict(loss=float(total), joints=joints.detach().numpy().copy(), body_pose=bp.detach().numpy()[0].copy(),
+               proj=proj.detach().numpy().copy(), terms=terms)
     for n, gg in zip(names, g):
         out["g_" + n] = gg.reshape(-1).numpy().copy()
     return out

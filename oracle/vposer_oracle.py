@@ -67,3 +67,29 @@ def decode_aa(w: dict, z: torch.Tensor) -> torch.Tensor:
     n = z.shape[0]
     R = cont6d_to_matrot(decode_6d(w, z))
     return quaternion_to_angle_axis(matrot_to_quaternion(R)).reshape(n, -1)
+
+
+def rotation_branches(w: dict, z, eps: float = 1e-6) -> dict:
+    """Where each decoded joint rotation of decode(z, 'aa') sits in the branch structure of matrot_to_quaternion and
+    quaternion_to_angle_axis, in float64 (float32 weights are widened exactly).  z [n, 32] -> arrays [n, 23]:
+
+    branch    0-3, the quaternion formula rotation_matrix_to_quaternion picks (m = R^T: 0 if m22 < eps and m00 > m11,
+              1 if m22 < eps otherwise, 2 if m22 >= eps and m00 < -m11, 3 otherwise)
+    surface   [n, 23, 3] signed distances to the three branch surfaces: m22 - eps, m00 - m11, m00 + m11.  Rotation-matrix
+              entries lie in [-1, 1], so these are relative distances as they stand
+    margin    distance to the nearest surface that decides this rotation's branch: m22 = eps, and m00 = m11 below it or
+              m00 = -m11 above it (the other one is not tested, so a rotation may sit on it: the identity has m00 = m11)
+    cos_neg   the quaternion's scalar part is negative (the atan2(-sin, -cos) side of quaternion_to_angle_axis)
+    angle     the rotation angle |aa| in [0, pi]"""
+    z = torch.as_tensor(np.asarray(z, dtype=np.float64))
+    n = z.shape[0]
+    R = cont6d_to_matrot(decode_6d(w, z))
+    m = R.transpose(1, 2)
+    d2 = m[:, 2, 2] < eps
+    br = torch.where(d2, torch.where(m[:, 0, 0] > m[:, 1, 1], 0, 1), torch.where(m[:, 0, 0] < -m[:, 1, 1], 2, 3))
+    surface = torch.stack([m[:, 2, 2] - eps, m[:, 0, 0] - m[:, 1, 1], m[:, 0, 0] + m[:, 1, 1]], -1)
+    margin = torch.minimum(surface[:, 0].abs(), torch.where(d2, surface[:, 1], surface[:, 2]).abs())
+    q = matrot_to_quaternion(R)
+    aa = quaternion_to_angle_axis(q)
+    return dict(branch=br.reshape(n, -1).numpy(), surface=surface.reshape(n, -1, 3).numpy(), margin=margin.reshape(n, -1).numpy(),
+                cos_neg=(q[:, 0] < 0).reshape(n, -1).numpy(), angle=aa.norm(dim=-1).reshape(n, -1).numpy())
