@@ -233,6 +233,21 @@ int mvs_fit_seq(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_co
                 const mvs_lbfgs_config* opt_cfg, const unsigned char* warm_host, float* final_loss_dev,
                 mvs_lbfgs_stats* stats, void* stream);
 
+/* ---- mvs_fit_seq with a causal temporal term (NOT in the reference: smoother video fits).  temporal_w_host [86] (HOST floats,
+ *      finite, >= 0, the same for every frame) adds  sum_i w[i] * (x[b,i] - prev[b,i])^2  to the loss of every stage a WARM
+ *      frame b runs (stages 2 .. n-1; the weight is not scaled by the stage, the 0.15 damping of stage 2 or a rig's data-weight
+ *      scale); cold frames never carry it.  prev_dev [B,86] (device) holds each warm frame's predecessor's FITTED row as
+ *      mvs_fit_seq returned it (before load_init / fix_params: without VPoser the anchor keeps the fitted body pose while the
+ *      start point has the hip seed; with use_vposer = 2 the latent code is anchored); rows of cold frames are not read.
+ *      A warm frame gets exactly what mvs_fit gives it alone on its slice of the stages after
+ *      mvs_set_anchor(row = prev[b], weight = w).  temporal_w_host NULL or all zero: mvs_fit_seq, bit for bit.
+ *      Refused: MVS_ERR_INVALID for a weight entry that is negative or not finite and for n_stages <= 2; MVS_ERR_UNSUPPORTED in
+ *      exec mode 1 and while mvs_set_anchor is on.  Afterwards the anchor term is off, as it had to be before the call (the
+ *      context's anchor rows and weights are overwritten); otherwise the context is as after mvs_fit_seq.  Synchronises. */
+int mvs_fit_seq_temporal(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_config* stage_cfgs,
+                         const mvs_lbfgs_config* opt_cfg, const unsigned char* warm_host, const float* prev_dev,
+                         const float* temporal_w_host, float* final_loss_dev, mvs_lbfgs_stats* stats, void* stream);
+
 /* ---- mvs_fit over a stream of F frames, F of any size relative to the context's batch B.  Every frame gets exactly what
  *      mvs_fit gives it in a batch of any size, bit for bit: the same parameters, final loss and iteration / evaluation
  *      counts.  Stages are grouped into runs as mvs_fit groups them; each run covers all F frames before the next starts
@@ -331,6 +346,20 @@ int mvs_fit_seq_stream3d(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
 int mvs_fit_seq_stream_rigs(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
                             const int* rig_dev, int n_stages, const mvs_loss_config* stage_cfgs,
                             const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream);
+
+/* ---- mvs_fit_seq_stream_rigs with the causal temporal term of mvs_fit_seq_temporal: temporal_w_host [86] (HOST floats, finite,
+ *      >= 0).  Every warm frame's stages 2 .. n-1 carry  sum_i w[i] * (x_i - x^_i)^2, x^ = its predecessor's fitted row, which
+ *      the device hands over with the slot (never passed in): the frame-resident chaining run anchors to the row it has just
+ *      written to params, a dense lane copies the fitted row into its anchor row before the successor's start point replaces
+ *      it.  Every frame gets exactly the parameters and final loss that mvs_fit_seq_temporal gives it in a batch of S
+ *      (seqio.fit_sequences with a batch of S and the same weight), in both chaining regimes, with rigs and the 3-D term.
+ *      temporal_w_host NULL or all zero: mvs_fit_seq_stream_rigs, bit for bit (which is this call with NULL).  Refusals as
+ *      mvs_fit_seq_temporal adds them to those of mvs_fit_seq_stream_rigs; context state afterwards as after
+ *      mvs_fit_seq_stream_rigs, anchor term off.  Synchronises. */
+int mvs_fit_seq_stream_temporal(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
+                                const int* rig_dev, const float* temporal_w_host, int n_stages,
+                                const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
+                                void* stream);
 
 /* ---- host-buffer entry point (what a caller without device memory uses): copies keypoints and
  *      parameters host->device, runs `n_stages` optimisation stages (one mvs_loss_config each, the weight

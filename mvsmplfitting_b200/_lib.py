@@ -77,7 +77,8 @@ EXPORTS = (
     "mvs_set_gmm_prior", "mvs_set_vposer", "mvs_vposer_decode", "mvs_set_cameras", "mvs_set_camera_rigs", "mvs_set_frame_rigs", "mvs_set_batch", "mvs_set_keypoints", "mvs_set_loss_config",
     "mvs_closure", "mvs_forward", "mvs_lbfgs_run", "mvs_lbfgs_step", "mvs_fit", "mvs_fit_seq", "mvs_fit_stream", "mvs_fit_seq_stream", "mvs_fit_seq_stream3d",
     "mvs_fit_stream_rigs", "mvs_fit_seq_stream_rigs", "mvs_fit_host", "mvs_sdf_grid", "mvs_profile", "mvs_profile_read",
-    "mvs_kernel_name", "mvs_set_exec_mode", "mvs_set_anchor", "mvs_set_joints3d", "mvs_init_guess",
+    "mvs_kernel_name", "mvs_set_exec_mode", "mvs_set_anchor", "mvs_set_joints3d", "mvs_init_guess", "mvs_fit_seq_temporal",
+    "mvs_fit_seq_stream_temporal",
 )
 NUM_KERNEL_IDS = 19
 
@@ -123,6 +124,8 @@ def load() -> ctypes.CDLL:
     lib.mvs_fit.argtypes = [vp, vp, ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig), vp, ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_fit_seq.argtypes = [vp, vp, ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig), vp, vp,
                                 ctypes.POINTER(LbfgsStats), vp]
+    lib.mvs_fit_seq_temporal.argtypes = [vp, vp, ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig), vp, vp, vp, vp,
+                                         ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_fit_stream.argtypes = [vp, ctypes.POINTER(FrameStream), ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig),
                                    ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_fit_seq_stream.argtypes = [vp, ctypes.POINTER(SequenceStream), ci, ctypes.POINTER(LossConfig),
@@ -133,6 +136,8 @@ def load() -> ctypes.CDLL:
                                         ctypes.POINTER(LbfgsConfig), ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_fit_seq_stream_rigs.argtypes = [vp, ctypes.POINTER(SequenceStream), vp, vp, vp, ci, ctypes.POINTER(LossConfig),
                                             ctypes.POINTER(LbfgsConfig), ctypes.POINTER(LbfgsStats), vp]
+    lib.mvs_fit_seq_stream_temporal.argtypes = [vp, ctypes.POINTER(SequenceStream), vp, vp, vp, vp, ci, ctypes.POINTER(LossConfig),
+                                                ctypes.POINTER(LbfgsConfig), ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_fit_host.argtypes = [vp, vp, vp, vp, vp, ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig), vp,
                                  ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_sdf_grid.argtypes = [vp, vp, vp, ci, vp, ci, ci, ci, vp]

@@ -33,6 +33,14 @@ def _ptr(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 
 
+def _temporal_weight(w) -> np.ndarray:
+    """a temporal weight as the C ABI takes it: 86 host float32 (checked there)"""
+    w = _f32(w.cpu() if isinstance(w, torch.Tensor) else w).reshape(-1)
+    if w.shape[0] != S.NUM_PARAMS:
+        raise ValueError("temporal_weight: want %d entries, got %d" % (S.NUM_PARAMS, w.shape[0]))
+    return w
+
+
 def _stats_dict(st) -> dict:
     return dict(frame_iterations=st.frame_iterations, frame_evals=st.frame_evals, rounds=st.rounds, frames_nan=st.frames_nan,
                 dense_frame_evals=st.dense_frame_evals, dense_rounds=st.dense_rounds)
@@ -280,17 +288,27 @@ class FittingContext:
                    "mvs_init_guess")
         return params, j3
 
-    def fit(self, params: torch.Tensor, stage_cfgs, opt_cfg=None, warm=None):
+    def fit(self, params: torch.Tensor, stage_cfgs, opt_cfg=None, warm=None, prev=None, temporal_weight=None):
         """All stages of a fit on device buffers (mvs_fit): params [B,86] CUDA float32, updated in place.  Frames move
         from stage to stage on their own; returns (final_loss [B], stats).  warm [B] bool (mvs_fit_seq): frames that
         continue a video sequence from the previous frame's result skip stages 0, 1 and damp stage 2's pose prior
-        (non_linear_solver.py:157-162)."""
+        (non_linear_solver.py:157-162).  temporal_weight [86] (mvs_fit_seq_temporal, needs warm and prev [B,86] CUDA float32,
+        the previous frames' fitted rows): every warm frame's stages add sum_i w_i (x_i - prev_i)^2."""
         assert params.is_cuda and params.dtype == torch.float32 and params.is_contiguous()
         arr = (_lib.LossConfig * len(stage_cfgs))(*stage_cfgs)
         cfg = opt_cfg or self.make_lbfgs_config()
         final = torch.empty(self.B, dtype=torch.float32, device=self.device)
         st = _lib.LbfgsStats()
-        if warm is not None:
+        if temporal_weight is not None:
+            if warm is None or prev is None:
+                raise ValueError("fit: temporal_weight needs warm and prev")
+            assert prev.is_cuda and prev.dtype == torch.float32 and prev.is_contiguous() and tuple(prev.shape) == (self.B, 86)
+            wm = np.ascontiguousarray(np.asarray(warm).astype(np.uint8).reshape(self.B))
+            tw = _temporal_weight(temporal_weight)
+            _lib.check(self.h, self.lib.mvs_fit_seq_temporal(self.h, _ptr(params), len(stage_cfgs), arr, ctypes.byref(cfg),
+                                                             _ptr(wm), _ptr(prev), _ptr(tw), _ptr(final), ctypes.byref(st),
+                                                             self._stream()), "mvs_fit_seq_temporal")
+        elif warm is not None:
             wm = np.ascontiguousarray(np.asarray(warm).astype(np.uint8).reshape(self.B))
             _lib.check(self.h, self.lib.mvs_fit_seq(self.h, _ptr(params), len(stage_cfgs), arr, ctypes.byref(cfg),
                                                     wm.ctypes.data_as(ctypes.c_void_p), _ptr(final), ctypes.byref(st),
@@ -352,7 +370,7 @@ class FittingContext:
         return final, _stats_dict(st)
 
     def fit_seq_stream(self, params: torch.Tensor, gt_uv, conf, joint_weights, lengths, stage_cfgs, opt_cfg=None,
-                       reinit_loss: float = 5000.0, joints3d=None, conf3d=None, rig=None):
+                       reinit_loss: float = 5000.0, joints3d=None, conf3d=None, rig=None, temporal_weight=None):
         """mvs_fit_seq over S video sequences through the context's B slots (mvs_fit_seq_stream): the frames of sequence s are
         the next lengths[s] rows, in time order.  params [F,86] CUDA float32 holds every frame's cold start point (init_guess)
         and is updated in place; gt_uv [V,F,K,2], conf [V,F,K], joint_weights [K] (numpy or tensors).  A frame after the first
@@ -360,8 +378,9 @@ class FittingContext:
         its own row otherwise.  joints3d [F,K,3] with conf3d [F,K] switch the 3-D joint term on for every frame of the call
         (mvs_fit_seq_stream3d; zero-confidence rows for frames without annotations).  rig [F] (mvs_fit_seq_stream_rigs)
         names each frame's camera rig (set_camera_rigs; None: rig 0, one rig only).  Every frame gets the bits
-        seqio.fit_sequences gives it with a batch of S.  Afterwards the context holds no keypoints, no 3-D targets and no
-        per-slot rigs.  Returns (final_loss [F], stats)."""
+        seqio.fit_sequences gives it with a batch of S.  temporal_weight [86] (mvs_fit_seq_stream_temporal): every warm frame's
+        stages add sum_i w_i (x_i - x^_i)^2, x^ = its predecessor's fitted row.  Afterwards the context holds no keypoints,
+        no 3-D targets and no per-slot rigs.  Returns (final_loss [F], stats)."""
         assert params.is_cuda and params.dtype == torch.float32 and params.is_contiguous() and params.dim() == 2
         F = params.shape[0]
         lengths = [int(n) for n in lengths]
@@ -377,7 +396,12 @@ class FittingContext:
         cfg = opt_cfg or self.make_lbfgs_config()
         st = _lib.LbfgsStats()
         self._j3d_keep = None
-        if rg is not None:
+        if temporal_weight is not None:
+            tw = _temporal_weight(temporal_weight)
+            _lib.check(self.h, self.lib.mvs_fit_seq_stream_temporal(self.h, ctypes.byref(s), _ptr(j3), _ptr(c3), _ptr(rg), _ptr(tw),
+                                                                    len(stage_cfgs), arr, ctypes.byref(cfg), ctypes.byref(st),
+                                                                    self._stream()), "mvs_fit_seq_stream_temporal")
+        elif rg is not None:
             _lib.check(self.h, self.lib.mvs_fit_seq_stream_rigs(self.h, ctypes.byref(s), _ptr(j3), _ptr(c3), _ptr(rg),
                                                                 len(stage_cfgs), arr, ctypes.byref(cfg), ctypes.byref(st),
                                                                 self._stream()), "mvs_fit_seq_stream_rigs")

@@ -405,10 +405,12 @@ int launch_closure_resident(mvs_ctx* ctx, const float* x_dev, float* loss_dev, f
 int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
                           const LossParams* lp_tab_host, int nstages, FrameScalars* frame_scalars_out, float* last_grad_dev,
                           cudaStream_t st, const int2* stage_rng_dev, const FrameInputs* frames = nullptr);
-// the chaining run of mvs_fit_seq_stream in the frame-resident regime: one CTA per sequence of q.act
+// the chaining run of mvs_fit_seq_stream in the frame-resident regime: one CTA per sequence of q.act.  temporal_w [F][86]
+// (mvs_fit_seq_stream_temporal; NULL: term off) are the anchor weights of the warm stages, whose anchor row is the
+// predecessor's fitted row of params_dev
 int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
                               const LossParams* lp_tab_host, int nstages, const FrameInputs& frames, const SeqChain& q,
-                              cudaStream_t st);
+                              cudaStream_t st, const float* temporal_w = nullptr);
 // dense regime (SDF term): per round  posedirs_gemm_tc -> skin -> sdf_setup -> sdf_fused -> frame_step (skin_small in place of
 // skin at <= 8 frames; at <= 4 frames skin_small computes the set-ups itself and sdf_setup is not launched)
 int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);                      // mvs_closure.cu

@@ -170,6 +170,7 @@ struct LaneArgs {
     int* pose_valid;
     SeqChain q;                         // the sequences, queued by q.act; q.off == NULL: a frame stream (q.cold: its stage table)
     int* lane_seq;                      // [B] sequence of each lane's frame (sequence stream)
+    float* anchor;                      // [B][86] the lanes' anchor rows (temporal term of a sequence stream), NULL: term off
 };
 
 // What follows a lane's finished frame `old` in the lane: its successor in the same sequence -- warm from the frame's
@@ -262,6 +263,7 @@ __global__ void __launch_bounds__(1024) lane_refill_kernel(LbfgsState S, LaneArg
             }
             if (fn < 0) continue;
             VLOOP(i) {                                    // a warm frame keeps the fitted row (but its own body pose, keep_pose)
+                if (wm && a.anchor) a.anchor[(size_t)ln * kParams + i] = xl[i];      // its anchor: the fitted row as returned
                 if (!wm || (a.q.keep_pose && i >= kOffPose && i < kOffTransl)) xl[i] = a.params[(size_t)fn * kParams + i];
             }
             const int K = a.K, rg = a.rig ? a.rig[fn] : 0;
@@ -286,6 +288,13 @@ __global__ void __launch_bounds__(1024) lane_refill_kernel(LbfgsState S, LaneArg
         __syncthreads();
     }
     if (tid == 0) *a.queue = qbase;
+}
+
+// rows [0, n) of dst [n][86] = w (the temporal weight: the same for every frame of a call)
+struct Row86 { float v[kParams]; };
+__global__ void fill_rows_kernel(float* __restrict__ dst, Row86 w, int n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < (size_t)n * kParams) dst[i] = w.v[i % kParams];
 }
 
 // rows idx[0 .. n) of full [V][n_full][L] <-> packed [V][n][L]; to_full = 0 gathers, 1 scatters.  With rig (per-view rows of
@@ -645,14 +654,17 @@ static int stage_table(mvs_ctx* ctx, const char* who, int n_stages, const mvs_lo
     return MVS_OK;
 }
 
-// The warm-started frames' copy of a stage table: stage kWarmSkip with 0.15 x its body-pose weight
+// The warm-started frames' copy of a stage table: stage kWarmSkip with 0.15 x its body-pose weight.  temporal: every stage
+// the warm frames run (kWarmSkip .. n-1) carries the anchor term, whose rows and weights the caller has set up.
 static int warm_stage_table(mvs_ctx* ctx, const mvs_loss_config* cfgs, int j3d, const std::vector<LossParams>& lps,
-                            std::vector<LossParams>* wlps) {
+                            std::vector<LossParams>* wlps, bool temporal = false) {
     *wlps = lps;
     mvs_loss_config wc = cfgs[kWarmSkip];
     wc.body_pose_weight *= 0.15f;
     const int rc = make_loss_params(ctx, &wc, &(*wlps)[kWarmSkip]);
     if (!rc && j3d >= 0) (*wlps)[kWarmSkip].j3d_on = j3d;
+    if (temporal)
+        for (size_t k = kWarmSkip; k < wlps->size(); ++k) (*wlps)[k].anchor_on = 1;
     return rc;
 }
 
@@ -674,8 +686,10 @@ static int stream_runs(mvs_ctx* ctx, const char* who, const std::vector<LossPara
 // every frame changes stage on its own (frames are independent problems, so a frame that converged need not wait at
 // the stage boundary for the slowest one; the per-frame arithmetic is the sequential schedule's).  exec_mode 2 keeps
 // the stage barrier (one run per stage).
+// temporal (mvs_fit_seq_temporal): the warm frames' stages carry the anchor term of the rows the caller put in ws.anchor / anchor_w.
 static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg,
-                   float* final_loss_dev, mvs_lbfgs_stats* stats, cudaStream_t st, const unsigned char* warm_host = nullptr) {
+                   float* final_loss_dev, mvs_lbfgs_stats* stats, cudaStream_t st, const unsigned char* warm_host = nullptr,
+                   bool temporal = false) {
     std::vector<LossParams> lps;
     int rc = stage_table(ctx, "mvs_fit", n_stages, stage_cfgs, -1, &lps);
     if (rc) return rc;
@@ -687,7 +701,7 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
         return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq: warm-started frames skip the first %d stages, %d given", kWarmSkip, n_stages);
     std::vector<LossParams> wlps;
     if (any_warm) {
-        if ((rc = warm_stage_table(ctx, stage_cfgs, -1, lps, &wlps))) return rc;
+        if ((rc = warm_stage_table(ctx, stage_cfgs, -1, lps, &wlps, temporal))) return rc;
         if (!ctx->stage_rng && (rc = dev_alloc(ctx, &ctx->stage_rng, (size_t)B))) return rc;
     }
     const int H = history_size(opt_cfg);
@@ -889,6 +903,8 @@ struct SeqState {
     size_t packed_cap = 0;
     float* packed = nullptr;            // the pending cold frames' rows for the runs before the chaining run
     int* packed_rig = nullptr;          // [cap] their rigs
+    size_t tw_cap = 0;
+    float* tw = nullptr;                // [tw_cap / 86][86] the temporal weight, one row per frame (frame-resident chaining)
 };
 
 static int ensure_seq_state(mvs_ctx* ctx, int nseq, size_t packed_floats) {
@@ -919,11 +935,27 @@ static int ensure_seq_state(mvs_ctx* ctx, int nseq, size_t packed_floats) {
     return MVS_OK;
 }
 
+// The slots' anchor rows and weights (as mvs_set_anchor allocates them), weights set to w for every slot
+static int temporal_slot_rows(mvs_ctx* ctx, const float* w, cudaStream_t st) {
+    Workspace& ws = ctx->ws;
+    int rc;
+    if (!ws.anchor) {
+        if ((rc = dev_alloc(ctx, &ws.anchor, (size_t)ws.B * kParams))) return rc;
+        if ((rc = dev_alloc(ctx, &ws.anchor_w, (size_t)ws.B * kParams))) return rc;
+    }
+    Row86 r;
+    for (int i = 0; i < kParams; ++i) r.v[i] = w[i];
+    MVS_LAUNCH(ctx, KID_MISC, st, fill_rows_kernel<<<(ws.B * kParams + 255) / 256, 256, 0, st>>>(ws.anchor_w, r, ws.B));
+    return MVS_OK;
+}
+
 // The chaining run over the sequences of one pass (q.act): every frame of run `tab` from its sequence's pending frame on
 // (gt_xyz / conf3d [F][K][3] / [F][K]: the 3-D targets, both NULL when the term is off)
+// temporal: the warm stages of tab carry the anchor term; its weight rows are set up (sstream->tw for the frame-resident
+// regime, ws.anchor_w for the dense one), and the anchor rows are the predecessors' fitted rows, handed over on the device.
 static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig, int F,
                          Regime rg, const std::vector<LossParams>& tab, const SeqChain& q0, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats,
-                         cudaStream_t st) {
+                         cudaStream_t st, bool temporal) {
     const int nst = (int)tab.size();
     LbfgsCfg cfg;
     int rc = begin_run(ctx, c, false, tab.data(), nst, &cfg, st);
@@ -936,7 +968,9 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
         // one launch, one CTA per sequence; rounds: the largest number of evaluations one CTA ran (its frames' sum)
         long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
         const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d, rig};
-        if ((rc = launch_lbfgs_resident_seq(ctx, s->params, cfg, cfg.history, S.lp_tab, tab.data(), nst, in, q, st))) return rc;
+        if ((rc = launch_lbfgs_resident_seq(ctx, s->params, cfg, cfg.history, S.lp_tab, tab.data(), nst, in, q, st,
+                                            temporal ? ctx->sstream->tw : nullptr)))
+            return rc;
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
         MVS_CUDA_OK(ctx, cudaGetLastError());
@@ -949,6 +983,7 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
     a.j3d_xyz = gt_xyz; a.j3d_conf = conf3d; a.rig = rig;
     a.q = q;
     a.lane_seq = ctx->sstream->lane_seq;
+    a.anchor = temporal ? ctx->ws.anchor : nullptr;
     return run_lanes(ctx, a, s->joint_weights, cfg, nst, stats, st);
 }
 
@@ -958,10 +993,11 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
 // out cold parks it for the next pass (c > 0 only: with c == 0 the cold frame stays in its slot with the cold slice).
 // gt_xyz / conf3d ([F][K][3] / [F][K], both NULL or both set): the 3-D joint term is on in every stage, cold and warm, iff set;
 // they travel with the frames as gt_uv / conf do, and so does rig ([F] or NULL: every frame has rig 0).
+// tw ([86] host, NULL: off): the temporal weight; every warm frame's stages carry sum_i tw_i (x_i - predecessor's fitted x_i)^2.
 static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig,
                           int n_stages,
                           const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
-                          cudaStream_t st) {
+                          cudaStream_t st, const float* tw = nullptr) {
     const int NS = s->n_sequences;
     const std::vector<int> off(s->seq_offsets, s->seq_offsets + NS + 1);
     const int F = off[NS];
@@ -973,7 +1009,7 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
     for (const LossParams& lp : lps) n_vp2 += lp.use_vposer == 2;
     if (n_vp2 > 0 && n_vp2 < n_stages)
         return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: stages mix latent-code (use_vposer = 2) and axis-angle poses");
-    if ((rc = warm_stage_table(ctx, stage_cfgs, j3d, lps, &wlps))) return rc;
+    if ((rc = warm_stage_table(ctx, stage_cfgs, j3d, lps, &wlps, tw != nullptr))) return rc;
     const int H = history_size(opt_cfg);
     std::vector<int> ends;
     if ((rc = stream_runs(ctx, "mvs_fit_seq_stream", lps, H, kMaxStages / 2, &ends))) return rc;
@@ -1006,6 +1042,21 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
     if (!rc && any_dense) rc = ensure_lane_rows(ctx, gt_xyz != nullptr);
     if (rc) return rc;
     SeqState& ss = *ctx->sstream;
+    const Regime rg_chain = stage_regime(ctx, lps[ic], H, false);
+    if (tw && rg_chain == kResident) {                                // a weight row per frame, as the closure indexes them
+        if (ss.tw_cap < (size_t)F * kParams) {
+            if (ss.tw) dev_free(ctx, ss.tw);
+            ss.tw = nullptr;
+            ss.tw_cap = 0;
+            if ((rc = dev_alloc(ctx, &ss.tw, (size_t)F * kParams))) return rc;
+            ss.tw_cap = (size_t)F * kParams;
+        }
+        Row86 r;
+        for (int i = 0; i < kParams; ++i) r.v[i] = tw[i];
+        MVS_LAUNCH(ctx, KID_MISC, st, fill_rows_kernel<<<(F * kParams + 255) / 256, 256, 0, st>>>(ss.tw, r, F));
+    } else if (tw && (rc = temporal_slot_rows(ctx, tw, st))) {         // dense: per lane
+        return rc;
+    }
     q.off = ss.off;
     q.cur = ss.cur;
     q.act = ss.act;
@@ -1059,8 +1110,7 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
         q.n_act = n;
         ctx->loss = lps[ic];
         ctx->have_loss = true;
-        if ((rc = run_seq_chain(ctx, s, gt_xyz, conf3d, rig, F, stage_regime(ctx, lps[ic], H, false), tab, q, opt_cfg, stats, st)))
-            break;
+        if ((rc = run_seq_chain(ctx, s, gt_xyz, conf3d, rig, F, rg_chain, tab, q, opt_cfg, stats, st, tw != nullptr))) break;
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(cur.data(), ss.cur, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
     }
@@ -1068,6 +1118,28 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
     ctx->loss.j3d_on = 0;
     ctx->slot_rigs = nullptr;
     return rc;
+}
+
+// The temporal weight of mvs_fit_seq_temporal / mvs_fit_seq_stream_temporal (who: the entry point): NULL, or 86 finite entries
+// >= 0 with n_stages > 2, outside exec mode 1 and with mvs_set_anchor off.  *on: some entry is non-zero (all zero: the term
+// is off, and the call is the one it extends).
+static int check_temporal_weight(mvs_ctx* ctx, const char* who, const float* w, int n_stages, bool* on) {
+    *on = false;
+    if (!w) return MVS_OK;
+    for (int i = 0; i < kParams; ++i) {
+        if (!(w[i] >= 0.f) || !isfinite(w[i]))
+            return set_error(ctx, MVS_ERR_INVALID, "%s: temporal weight %d is %g (want finite and >= 0)", who, i, (double)w[i]);
+        *on |= w[i] != 0.f;
+    }
+    if (n_stages <= kWarmSkip)
+        return set_error(ctx, MVS_ERR_INVALID, "%s: the temporal term is on the warm frames' stages %d .. n-1, %d stages given", who,
+                         kWarmSkip, n_stages);
+    if (ctx->exec_mode == 1)
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: warm-started frames are not implemented in the batched reference chain "
+                                                   "(exec mode 1)", who);
+    if (ctx->anchor_enabled)
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the temporal term uses the anchor rows; switch mvs_set_anchor off first", who);
+    return MVS_OK;
 }
 
 }  // namespace mvs
@@ -1117,6 +1189,27 @@ int mvs_fit_seq(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_co
     return run_fit(ctx, params_dev, n_stages, stage_cfgs, opt_cfg, final_loss_dev, stats, (cudaStream_t)stream, warm_host);
 }
 
+int mvs_fit_seq_temporal(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_config* stage_cfgs,
+                         const mvs_lbfgs_config* opt_cfg, const unsigned char* warm_host, const float* prev_dev,
+                         const float* temporal_w_host, float* final_loss_dev, mvs_lbfgs_stats* stats, void* stream) {
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    bool on = false;
+    if (int rc = check_temporal_weight(ctx, "mvs_fit_seq_temporal", temporal_w_host, n_stages, &on)) return rc;
+    if (!on) return mvs_fit_seq(ctx, params_dev, n_stages, stage_cfgs, opt_cfg, warm_host, final_loss_dev, stats, stream);
+    if (!(ctx->have_model && ctx->have_cams && ctx->have_kp && ctx->ws.B > 0))
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_temporal: model, cameras, batch and keypoints must be set first");
+    if (!params_dev || !stage_cfgs || !opt_cfg || !prev_dev)
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_temporal: NULL argument");
+    if (int rc = batch_rigs(ctx, "mvs_fit_seq_temporal")) return rc;
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    if (stats) memset(stats, 0, sizeof(*stats));
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = temporal_slot_rows(ctx, temporal_w_host, st)) return rc;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->ws.anchor, prev_dev, (size_t)ctx->ws.B * kParams * sizeof(float), cudaMemcpyDeviceToDevice,
+                                     st));
+    return run_fit(ctx, params_dev, n_stages, stage_cfgs, opt_cfg, final_loss_dev, stats, st, warm_host, true);
+}
+
 int mvs_fit(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg,
             float* final_loss_dev, mvs_lbfgs_stats* stats, void* stream) {
     if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
@@ -1158,10 +1251,12 @@ int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const 
     return mvs_fit_stream_rigs(ctx, s, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
 }
 
-int mvs_fit_seq_stream_rigs(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig_dev,
-                            int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
-                            void* stream) {
+int mvs_fit_seq_stream_temporal(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
+                                const int* rig_dev, const float* temporal_w_host, int n_stages, const mvs_loss_config* stage_cfgs,
+                                const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
     if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    bool on = false;
+    if (int rc = check_temporal_weight(ctx, "mvs_fit_seq_stream_temporal", temporal_w_host, n_stages, &on)) return rc;
     if (!gt_xyz != !conf3d) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream3d: gt_xyz and conf3d go together");
     if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0))
         return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: model, cameras and batch must be set first");
@@ -1189,7 +1284,14 @@ int mvs_fit_seq_stream_rigs(mvs_ctx* ctx, const mvs_sequence_stream* s, const fl
         if (int rc = check_frame_rigs(ctx, "mvs_fit_seq_stream_rigs", rig_dev, F, (cudaStream_t)stream)) return rc;
     }
     if (stats) memset(stats, 0, sizeof(*stats));
-    return run_seq_stream(ctx, s, gt_xyz, conf3d, rig_dev, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
+    return run_seq_stream(ctx, s, gt_xyz, conf3d, rig_dev, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream,
+                          on ? temporal_w_host : nullptr);
+}
+
+int mvs_fit_seq_stream_rigs(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig_dev,
+                            int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
+                            void* stream) {
+    return mvs_fit_seq_stream_temporal(ctx, s, gt_xyz, conf3d, rig_dev, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
 }
 
 int mvs_fit_seq_stream3d(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int n_stages,

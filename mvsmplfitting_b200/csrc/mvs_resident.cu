@@ -357,12 +357,20 @@ int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, 
 }
 
 int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int H, const LossParams* lp_tab_dev,
-                              const LossParams* lph, int nstages, const FrameInputs& in, const SeqChain& q, cudaStream_t st) {
+                              const LossParams* lph, int nstages, const FrameInputs& in, const SeqChain& q, cudaStream_t st,
+                              const float* temporal_w) {
     int with_vposer = 0;
     for (int i = 0; i < nstages; ++i) with_vposer |= (lph[i].use_vposer == 2);
     const size_t smem = frame_smem(H, with_vposer != 0);
     ResidentModel rm = make_resident_model(ctx);
     rm.j3d_xyz = in.j3d_xyz; rm.j3d_conf = in.j3d_conf;              // row stride in.n, as gt_uv / conf
+    if (temporal_w) {
+        // the closure reads frame b's anchor row at anchor + 86 b: here the row of frame b - 1 in params, which the CTA wrote
+        // (the frame's fitted row) before the barrier that starts warm frame b.  Cold frames run no anchored stage, so the
+        // row before params is never read.
+        rm.anchor = params_dev - kParams;
+        rm.anchor_w = temporal_w;
+    }
     MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
                lbfgs_resident_seq_kernel<<<q.n_act, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev, in.rig}, lp_tab_dev, cfg,
                                                                              params_dev, in.gt_uv, in.conf, in.joint_w, in.n, H,

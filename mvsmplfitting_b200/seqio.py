@@ -387,10 +387,24 @@ def _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, fac
         _export(ctx, seq, chunk, lc, latent, result_folder, mesh_folder, faces, frames=seq["frames"][c0:c0 + n], rows=range(n))
 
 
+def temporal_weight_vector(temporal_weight):
+    """fit_sequences' temporal_weight as the 86 per-parameter weights the device takes: None stays None, a scalar lam is
+    lam x sequence.smooth_mask() (global orientation, the pose slot and translation), an array is taken as the 86-vector"""
+    if temporal_weight is None:
+        return None
+    if np.ndim(temporal_weight) == 0:
+        from .sequence import smooth_mask
+        return np.float32(temporal_weight) * smooth_mask().numpy().astype(np.float32)
+    w = np.ascontiguousarray(temporal_weight, dtype=np.float32).reshape(-1)
+    if w.shape[0] != 86:
+        raise ValueError("temporal_weight: want a scalar or 86 entries, got %d" % w.shape[0])
+    return w
+
+
 def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = False, fixed_scale: float = 1.0,
                   use_hip: bool = True, pose_format: str = "coco17", result_folder: str | None = None,
                   mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, reinit_loss: float = 5000.0,
-                  use_3d: bool = False, rigs=None, rig_data_weight_scale=None):
+                  use_3d: bool = False, rigs=None, rig_data_weight_scale=None, temporal_weight=None):
     """main.py:32-89 with is_seq = True for S sequences in lock-step: the batch of step t is frame t of every sequence
     (context batch = S).  A sequence's first frame gets the initial guess and every stage; a later frame
     starts from the previous frame's result as load_init + fix_params leave it (init_guess.py:137-166,190-212: betas,
@@ -409,8 +423,13 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
     view rows; rig_data_weight_scale [n_rigs] (None: all 1) scales every stage's data_weight per rig (the reference's
     500 / H for rigs of different image heights).  The rigs are set on the context (set_camera_rigs), detections are padded
     to the largest view count, and every frame gets what a context with only its rig's cameras gives it.
+    temporal_weight (None: off; a scalar lam, or 86 weights w, see temporal_weight_vector) pulls every warm frame towards its
+    predecessor's fitted row: its stages add sum_i w_i (x_i - x^_{t-1,i})^2 (mvs_fit_seq_temporal in lock-step, after step
+    t-1 with that step's fitted rows; mvs_fit_seq_stream_temporal otherwise, with the same bits).  Cold frames are fitted as
+    without it.
     Returns a list (per sequence) of (params [T_s,86], loss [T_s]) and the summed stats."""
     S_ = len(seqs)
+    tw = temporal_weight_vector(temporal_weight)
     latent = _uses_latent_pose(stage_cfgs)
     seq_rig = rig_views = None
     if rigs is not None:
@@ -432,7 +451,7 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
         return _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces,
                                      pose_format, use_hip, dict(estimate_scale=estimate_scale, fixed_scale=fixed_scale,
                                                                 use_torso=True, hip_seed=1.0, want_joints3d=False,
-                                                                umeyama_as_written=umeyama_as_written), t3, seq_rig, rig_views)
+                                                                umeyama_as_written=umeyama_as_written), t3, seq_rig, rig_views, tw)
     T = max(len(q["frames"]) for q in seqs)
     V = seqs[0]["gt_uv"].shape[0]
     off = np.concatenate([[0], np.cumsum([len(q["frames"]) for q in seqs])])
@@ -472,7 +491,10 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
                 carried[:, 13:82] = cold[:, 13:82]
             wm = torch.as_tensor(warm, device=params.device)
             params = torch.where(wm[:, None], carried, cold).contiguous()
-        final, st = ctx.fit(params, stage_cfgs, opt_cfg, warm=warm if warm.any() else None)
+        if tw is not None and warm.any():      # prev: step t-1's fitted rows, before load_init / fix_params
+            final, st = ctx.fit(params, stage_cfgs, opt_cfg, warm=warm, prev=prev, temporal_weight=tw)
+        else:
+            final, st = ctx.fit(params, stage_cfgs, opt_cfg, warm=warm if warm.any() else None)
         for k in tot:
             tot[k] += st[k]
         prev, prev_loss = params, final.cpu().numpy()
@@ -490,10 +512,10 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
 
 
 def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces, pose_format,
-                          use_hip, guess, t3=None, seq_rig=None, rig_views=None):
+                          use_hip, guess, t3=None, seq_rig=None, rig_views=None, tw=None):
     """fit_sequences through mvs_fit_seq_stream: the sequences' frames back to back, every frame's cold start point from
     _cold_guesses; t3: _targets_3d of those frames (mvs_fit_seq_stream3d); seq_rig [S]: each sequence's rig, which every
-    one of its frames takes (mvs_fit_seq_stream_rigs)"""
+    one of its frames takes (mvs_fit_seq_stream_rigs); tw [86]: the temporal weight (mvs_fit_seq_stream_temporal)"""
     lengths = [len(q["frames"]) for q in seqs]
     off = np.concatenate([[0], np.cumsum(lengths)])
     gt_uv = np.concatenate([q["gt_uv"] for q in seqs], axis=1)
@@ -502,6 +524,8 @@ def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, r
     rig = None if seq_rig is None else np.repeat(seq_rig, lengths).astype(np.int32)
     params = _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess, t3, rig, rig_views)
     kw = {} if rig is None else dict(rig=rig)
+    if tw is not None:
+        kw["temporal_weight"] = tw
     if t3 is None:
         final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss, **kw)
     else:
