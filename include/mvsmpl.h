@@ -361,6 +361,34 @@ int mvs_fit_seq_stream_temporal(mvs_ctx* ctx, const mvs_sequence_stream* s, cons
                                 const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
                                 void* stream);
 
+/* ---- one body shape per video sequence (NOT in the reference, whose only tool is fix_shape with a hand-typed shape): for
+ *      sequence q of s and the one stage configuration `stage` (normally the schedule's last), minimises
+ *        E_q = sum_{t in q} L(x_t with betas <- beta, scale <- s)
+ *      over beta, s and the other entries of every frame's row x_t, L = what mvs_closure returns for that row under `stage`
+ *      (2-D term, priors with each frame's own shape prior, the 3-D term with gt_xyz, the rig's data-weight scale).  scale
+ *      is shared unless `stage` freezes it (frozen_mask bit 4, fix_scale): a frozen scale stays at each row's own value.
+ *      Block-coordinate descent, n_sweeps >= 1 times:
+ *        consensus: beta (, s) = the mean over the sequence's frames whose rows are all finite (double, frame order); a
+ *          sequence without a finite row is skipped: its rows are left as they are, its losses are NaN;
+ *        shape step: one L-BFGS problem per sequence over its shared entries with the poses held (the 86-vector state machine
+ *          of mvs_fit's frames, with run_fitting's NaN / ftol / gtol rules and opt_cfg), the context's B sequences at a time;
+ *          its closure adds the frames' mvs_closure losses and shared gradient entries in double, in frame order;
+ *        pose step: the shared entries written into every row of the sequence, then every frame runs `stage` from its row with
+ *          betas (and a shared scale) frozen: exactly mvs_fit_stream's bits for that row.
+ *      s->params [F,86] holds the fitted rows on entry and the result on exit (s->reinit_loss is not read); s->final_loss [F]
+ *      (may be NULL) receives each frame's pose-step result of the last sweep; seq_loss_dev [S] (device, may be NULL) each
+ *      sequence's run_fitting value of its last shape step.  gt_xyz, conf3d and rig_dev as in mvs_fit_seq_stream_rigs.
+ *      shape_stats counts the sequence problems' iterations and evaluations, pose_stats what mvs_fit_stream reports (both
+ *      summed over the sweeps).  Refused: MVS_ERR_INVALID for NULL or empty arguments, n_sweeps < 1, bad seq_offsets, exactly
+ *      one of gt_xyz / conf3d, betas frozen in `stage` (frozen_mask bit 0: the shape is given) and a rig index out of range
+ *      (checked on the device); MVS_ERR_UNSUPPORTED for stage.interpenetration (the shape closure has no SDF term), the anchor
+ *      term, and what mvs_fit_stream refuses (exec mode 1, history_size > 100).  Context state afterwards as after
+ *      mvs_fit_stream.  Synchronises. */
+int mvs_fit_shared_shape(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
+                         const int* rig_dev, const mvs_loss_config* stage, const mvs_lbfgs_config* opt_cfg,
+                         int n_sweeps, float* seq_loss_dev, mvs_lbfgs_stats* shape_stats,
+                         mvs_lbfgs_stats* pose_stats, void* stream);
+
 /* ---- host-buffer entry point (what a caller without device memory uses): copies keypoints and
  *      parameters host->device, runs `n_stages` optimisation stages (one mvs_loss_config each, the weight
  *      schedule of code/utils/non_linear_solver.py:109-203), copies parameters and losses back.

@@ -414,6 +414,35 @@ class FittingContext:
                        "mvs_fit_seq_stream3d")
         return final, _stats_dict(st)
 
+    def fit_shared_shape(self, params: torch.Tensor, gt_uv, conf, joint_weights, lengths, stage_cfg, opt_cfg=None, sweeps=1,
+                         joints3d=None, conf3d=None, rig=None):
+        """One body shape per video sequence (mvs_fit_shared_shape): the frames of sequence s are the next lengths[s] rows of
+        params [F,86] (CUDA float32, fitted rows in, result out).  `sweeps` rounds of: each sequence's betas (and scale, unless
+        stage_cfg freezes it) fitted to all of its frames with the poses held, from the mean over its finite rows; then every
+        frame refits stage_cfg with the shared entries frozen.  gt_uv [V,F,K,2], conf [V,F,K], joint_weights [K], joints3d /
+        conf3d and rig as in fit_seq_stream.  Afterwards the context holds no keypoints, no 3-D targets and no per-slot rigs.
+        Returns (final_loss [F], seq_loss [S], shape_stats, pose_stats)."""
+        assert params.is_cuda and params.dtype == torch.float32 and params.is_contiguous() and params.dim() == 2
+        F = params.shape[0]
+        lengths = [int(n) for n in lengths]
+        if not lengths or min(lengths) < 1 or sum(lengths) != F:
+            raise ValueError("fit_shared_shape: want sequence lengths >= 1 that add up to %d frames, got %s" % (F, lengths))
+        if int(sweeps) < 1:
+            raise ValueError("fit_shared_shape: want sweeps >= 1, got %s" % sweeps)
+        off = np.ascontiguousarray(np.concatenate([[0], np.cumsum(lengths)]), dtype=np.int32)
+        gt_uv, conf, jw, j3, c3 = self._stream_rows("fit_shared_shape", F, gt_uv, conf, joint_weights, joints3d, conf3d)
+        rg = self._stream_rigs("fit_shared_shape", F, rig)
+        final = torch.empty(F, dtype=torch.float32, device=self.device)
+        seq_loss = torch.empty(len(lengths), dtype=torch.float32, device=self.device)
+        s = _lib.SequenceStream(len(lengths), _ptr(off), _ptr(params), _ptr(gt_uv), _ptr(conf), _ptr(jw), _ptr(final), 0.0)
+        cfg = opt_cfg or self.make_lbfgs_config()
+        sh, po = _lib.LbfgsStats(), _lib.LbfgsStats()
+        self._j3d_keep = None
+        _lib.check(self.h, self.lib.mvs_fit_shared_shape(self.h, ctypes.byref(s), _ptr(j3), _ptr(c3), _ptr(rg), ctypes.byref(stage_cfg),
+                                                         ctypes.byref(cfg), int(sweeps), _ptr(seq_loss), ctypes.byref(sh),
+                                                         ctypes.byref(po), self._stream()), "mvs_fit_shared_shape")
+        return final, seq_loss, _stats_dict(sh), _stats_dict(po)
+
     def fit_host(self, params_host: np.ndarray, gt_uv: np.ndarray, conf: np.ndarray, joint_weights: np.ndarray,
                  stage_cfgs, opt_cfg=None):
         """Host-buffer entry point (mvs_fit_host): params_host [B,86] float32 updated in place."""

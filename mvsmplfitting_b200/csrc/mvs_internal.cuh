@@ -141,6 +141,7 @@ struct FrameScalars;
 struct TcState;
 struct StreamState;                   // mvs_fit_stream scratch (mvs_lbfgs.cu)
 struct SeqState;                      // mvs_fit_seq_stream scratch (mvs_lbfgs.cu)
+struct ShapeState;                    // mvs_fit_shared_shape scratch (mvs_lbfgs.cu)
 
 // The frames a frame-resident run fits when they are not the context's batch (mvs_fit_stream): n frames, every array with
 // row stride n (gt_uv [V][n][K][2], conf [V][n][K], j3d_xyz [n][K][3], j3d_conf [n][K]; the 3-D pair may be NULL; rig [n]
@@ -149,6 +150,19 @@ struct FrameInputs {
     int n;
     const float *gt_uv, *conf, *joint_w, *j3d_xyz, *j3d_conf;
     const int* rig;
+};
+
+// The shape step of mvs_fit_shared_shape (DESIGN.md section 4): sequences base .. base + n - 1 of the call, in the optimiser's
+// slots 0 .. n - 1, whose frames are f0 .. f0 + nf - 1 of the call's F frames (in.n = F: the row stride of every input)
+struct ShapeArgs {
+    FrameInputs in;
+    const float* params;              // [F][86] the frames' rows (poses held)
+    const int* off;                   // [S+1] device: sequence q owns frames [off[q], off[q+1])
+    const int* seq_of;                // [F] sequence of each frame
+    int base, n, f0, nf;
+    int share_scale;                  // 1: scale (entry 85) is shared, 0: it stays per frame
+    float* loss;                      // [F] per-frame scratch
+    float* grad;                      // [F][86]
 };
 
 // The chaining run of mvs_fit_seq_stream (DESIGN.md section 4): a finished frame hands its slot (a CTA of the frame-resident
@@ -305,6 +319,7 @@ struct mvs_ctx {
     int2* stage_rng = nullptr;       // [B] per-frame slice of the stage table (mvs_fit_seq), device
     mvs::StreamState* fstream = nullptr;  // frame-stream scratch (mvs_fit_stream), created on first use
     mvs::SeqState* sstream = nullptr;     // sequence-stream scratch (mvs_fit_seq_stream), created on first use
+    mvs::ShapeState* shape = nullptr;     // shared-shape scratch (mvs_fit_shared_shape), created on first use
 };
 
 namespace mvs {
@@ -411,6 +426,9 @@ int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, 
 int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
                               const LossParams* lp_tab_host, int nstages, const FrameInputs& frames, const SeqChain& q,
                               cudaStream_t st, const float* temporal_w = nullptr);
+// the shape closure of mvs_fit_shared_shape: per frame (shape_closure_kernel), then per sequence (shape_reduce_kernel) into
+// L.loss_eval / L.g_eval of the chunk's slots; slots whose problem is done are skipped
+int launch_shape_closure(mvs_ctx* ctx, const ShapeArgs& a, const LossParams& lp, const LbfgsState& L, cudaStream_t st);
 // dense regime (SDF term): per round  posedirs_gemm_tc -> skin -> sdf_setup -> sdf_fused -> frame_step (skin_small in place of
 // skin at <= 8 frames; at <= 4 frames skin_small computes the set-ups itself and sdf_setup is not launched)
 int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);                      // mvs_closure.cu

@@ -28,6 +28,7 @@
 #include <cstdio>
 #include <vector>
 #include <cstdlib>
+#include <functional>
 #include "mvs_internal.cuh"
 #include "mvs_lbfgs_core.cuh"
 
@@ -495,9 +496,11 @@ static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int n
     return tc_check_error(ctx);
 }
 
-// Batched chain: the closure (frame-resident where it applies, launch_closure otherwise) + lbfgs_advance_kernel +
-// lbfgs_compact_kernel per round, the host reads the active count after every chunk of rounds
-static int run_batched(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, bool vp2, cudaStream_t st) {
+// Batched chain: the closure (frame-resident where it applies, launch_closure otherwise; closure: the caller's, which fills
+// S.loss_eval / S.g_eval of the active slots) + lbfgs_advance_kernel + lbfgs_compact_kernel per round, the host reads the active
+// count after every chunk of rounds
+static int run_batched(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, bool vp2, cudaStream_t st,
+                       const std::function<int()>& closure = nullptr) {
     LbfgsState& S = *ctx->lbfgs;
     Workspace& w = ctx->ws;
     const int B = w.B;
@@ -508,8 +511,9 @@ static int run_batched(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, boo
     const bool resident = resident_closure_applies(ctx, false);     // (not the dense-round closure: it restarts the optimiser)
     while (na_host > 0 && rounds < max_rounds) {
         for (int r = 0; r < chunk; ++r) {
-            const int rc = resident ? launch_closure_resident(ctx, S.x_eval, S.loss_eval, S.g_eval, nullptr, nullptr, st)
-                                    : launch_closure(ctx, S.x_eval, S.loss_eval, S.g_eval, nullptr, nullptr, nullptr, st);
+            const int rc = closure ? closure()
+                         : resident ? launch_closure_resident(ctx, S.x_eval, S.loss_eval, S.g_eval, nullptr, nullptr, st)
+                         : launch_closure(ctx, S.x_eval, S.loss_eval, S.g_eval, nullptr, nullptr, nullptr, st);
             if (rc) return rc;
             MVS_LAUNCH(ctx, KID_LBFGS_ADVANCE, st, lbfgs_advance_kernel<<<B, 32, 0, st>>>(S, cfg, params_dev, w.fidx, w.na, vp2 ? 32 : kOffTransl - kOffPose));
             MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
@@ -1142,6 +1146,243 @@ static int check_temporal_weight(mvs_ctx* ctx, const char* who, const float* w, 
     return MVS_OK;
 }
 
+// mvs_fit_shared_shape scratch (DESIGN.md section 4), grow-only in sequences and frames
+struct ShapeState {
+    int s_cap = 0, f_cap = 0;
+    int *off = nullptr, *ok = nullptr;  // [s_cap+1], [s_cap] (ok: the sequence has a finite row)
+    float* rows = nullptr;              // [s_cap + B][86] each sequence's shared row: the x of its problem (B rows of padding
+                                        // for the slots a last chunk leaves empty)
+    float* seq_final = nullptr;         // [B] run_fitting's value of each slot's problem
+    int *seq_of = nullptr, *frames = nullptr, *packed_rig = nullptr;    // [f_cap] each
+    float *loss = nullptr, *grad = nullptr;                             // [f_cap], [f_cap][86] the shape closure's per-frame terms
+    size_t packed_cap = 0;
+    float* packed = nullptr;            // the pose step's frame stream: rows, detections, 3-D targets, final losses
+};
+
+static int ensure_shape_state(mvs_ctx* ctx, int NS, int F, size_t packed_floats) {
+    int rc;
+    if (!ctx->shape) ctx->shape = new ShapeState();
+    ShapeState& h = *ctx->shape;
+    const int B = ctx->ws.B;
+    if (!h.seq_final && (rc = dev_alloc(ctx, &h.seq_final, (size_t)B))) return rc;
+    if (h.s_cap < NS) {
+        for (void* p : {(void*)h.off, (void*)h.ok, (void*)h.rows})
+            if (p) dev_free(ctx, p);
+        h.s_cap = 0;
+        if ((rc = dev_alloc(ctx, &h.off, (size_t)NS + 1)) || (rc = dev_alloc(ctx, &h.ok, (size_t)NS)) ||
+            (rc = dev_alloc(ctx, &h.rows, ((size_t)NS + B) * kParams)))
+            return rc;
+        h.s_cap = NS;
+    }
+    if (h.f_cap < F) {
+        for (void* p : {(void*)h.seq_of, (void*)h.frames, (void*)h.packed_rig, (void*)h.loss, (void*)h.grad})
+            if (p) dev_free(ctx, p);
+        h.f_cap = 0;
+        if ((rc = dev_alloc(ctx, &h.seq_of, (size_t)F)) || (rc = dev_alloc(ctx, &h.frames, (size_t)F)) ||
+            (rc = dev_alloc(ctx, &h.packed_rig, (size_t)F)) || (rc = dev_alloc(ctx, &h.loss, (size_t)F)) ||
+            (rc = dev_alloc(ctx, &h.grad, (size_t)F * kParams)))
+            return rc;
+        h.f_cap = F;
+    }
+    if (h.packed_cap < packed_floats) {
+        if (h.packed) dev_free(ctx, h.packed);
+        h.packed = nullptr;
+        h.packed_cap = 0;
+        if ((rc = dev_alloc(ctx, &h.packed, packed_floats))) return rc;
+        h.packed_cap = packed_floats;
+    }
+    return MVS_OK;
+}
+
+// Per sequence (one warp): the mean of the shared entries (betas, and scale with share_scale) over the frames whose rows are
+// all finite, accumulated in double in frame order, into rows[q] (zeros elsewhere); ok[q] = 0 when no row is finite.  Once the
+// shared entries of a sequence's rows are equal (after a sweep), the mean reproduces them bit for bit.
+__global__ void shape_consensus_kernel(const float* __restrict__ params, const int* __restrict__ off, int share_scale,
+                                       float* __restrict__ rows, int* __restrict__ ok) {
+    const int q = blockIdx.x, lane = threadIdx.x;
+    const int e = lane < kOffOrient ? lane : (lane == kOffOrient && share_scale) ? kOffScale : -1;
+    double acc = 0.0;
+    int n = 0;
+    for (int f = off[q]; f < off[q + 1]; ++f) {
+        const float* x = params + (size_t)f * kParams;
+        bool fin = true;
+        for (int i = lane; i < kParams; i += 32) fin = fin && isfinite(x[i]);
+        if (!__all_sync(0xffffffffu, fin)) continue;
+        ++n;
+        if (e >= 0) acc += (double)x[e];
+    }
+    float* r = rows + (size_t)q * kParams;
+    for (int i = lane; i < kParams; i += 32) r[i] = 0.f;
+    __syncwarp();
+    if (e >= 0 && n > 0) r[e] = (float)(acc / (double)n);
+    if (lane == 0) ok[q] = n > 0 ? 1 : 0;
+}
+
+// The shared entries of every frame of a sequence with a finite row: its sequence's row
+__global__ void shape_write_kernel(float* __restrict__ params, const int* __restrict__ seq_of, const float* __restrict__ rows,
+                                   const int* __restrict__ ok, int F, int share_scale) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= F || !ok[seq_of[f]]) return;
+    const float* r = rows + (size_t)seq_of[f] * kParams;
+    float* x = params + (size_t)f * kParams;
+    for (int i = kOffBetas; i < kOffOrient; ++i) x[i] = r[i];
+    if (share_scale) x[kOffScale] = r[kOffScale];
+}
+
+// The slots of one chunk of sequence problems: slot j < n holds sequence base + j from its shared row (rows[base + j]) with a
+// fresh optimiser, unless the sequence has no finite row (ok); the other slots have no stage and leave the active list
+static int shape_chunk_start(mvs_ctx* ctx, int base, int n, const std::vector<int>& ok, cudaStream_t st) {
+    LbfgsState& S = *ctx->lbfgs;
+    Workspace& w = ctx->ws;
+    const int B = w.B;
+    int rc;
+    if (!ctx->stage_rng && (rc = dev_alloc(ctx, &ctx->stage_rng, (size_t)B))) return rc;
+    std::vector<int> rng((size_t)B * 2, 0);
+    bool some_inactive = false;
+    for (int j = 0; j < B; ++j) {
+        const bool on = j < n && ok[base + j];
+        rng[2 * j + 1] = on ? 1 : 0;
+        some_inactive |= !on;
+    }
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->stage_rng, rng.data(), rng.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
+    MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_init_kernel<<<B, 32, 0, st>>>(S, ctx->shape->rows + (size_t)base * kParams, B, 1, 1,
+                                                                       ctx->stage_rng));
+    if (some_inactive) MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
+    return MVS_OK;
+}
+
+// The shape closure's arguments for sequences base .. base + n - 1 (off: the host copy of the offsets)
+static ShapeArgs shape_chunk_args(const ShapeArgs& a0, const std::vector<int>& off, int base, int n) {
+    ShapeArgs a = a0;
+    a.base = base; a.n = n;
+    a.f0 = off[base]; a.nf = off[base + n] - off[base];
+    return a;
+}
+
+// The shape step: every sequence's L-BFGS problem over its shared entries, the context's B at a time, run as run_fitting runs a
+// frame's stage (lbfgs_init / advance / compact of the batched chain, with the shape closure as the closure)
+static int shape_step(mvs_ctx* ctx, const ShapeArgs& a0, const std::vector<int>& off, const std::vector<int>& ok,
+                      const LossParams& lp, const mvs_lbfgs_config* c, float* seq_loss, mvs_lbfgs_stats* stats, cudaStream_t st) {
+    const int NS = (int)off.size() - 1, B = ctx->ws.B;
+    ShapeState& h = *ctx->shape;
+    for (int base = 0; base < NS; base += B) {
+        const int n = std::min(B, NS - base);
+        LbfgsCfg cfg;
+        int rc = begin_run(ctx, c, false, &lp, 1, &cfg, st);
+        if (!rc) rc = shape_chunk_start(ctx, base, n, ok, st);
+        if (rc) return rc;
+        const LbfgsState S = *ctx->lbfgs;
+        const ShapeArgs a = shape_chunk_args(a0, off, base, n);
+        const std::function<int()> closure = [&]() { return launch_shape_closure(ctx, a, lp, S, st); };
+        if ((rc = run_batched(ctx, h.rows + (size_t)base * kParams, cfg, lp.use_vposer == 2, st, closure))) return rc;
+        if ((rc = end_run(ctx, kBatched, h.seq_final, nullptr, stats, st))) return rc;
+        if (seq_loss)
+            MVS_CUDA_OK(ctx, cudaMemcpyAsync(seq_loss + base, h.seq_final, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    }
+    return MVS_OK;
+}
+
+// The pose step: the frames of `frames` (ascending; the sequences with a finite row) as one frame stream of their packed rows
+// through run_stream under the one stage cfg; their rows and final losses go back to the call's arrays
+static int shape_pose_step(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig,
+                           const std::vector<int>& frames, const mvs_loss_config& cfg, const mvs_lbfgs_config* c,
+                           mvs_lbfgs_stats* stats, cudaStream_t st) {
+    const int n = (int)frames.size(), F = s->seq_offsets[s->n_sequences], V = ctx->vmax, K = ctx->m.K;
+    if (n == 0) return MVS_OK;
+    ShapeState& h = *ctx->shape;
+    const Rig* rigs = ctx->rigs_dev;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.frames, frames.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+    float* px = h.packed;
+    float* pg = px + (size_t)n * kParams;
+    float* pc = pg + (size_t)V * n * K * 2;
+    float* pf = pc + (size_t)V * n * K;
+    float* pj = gt_xyz ? pf + n : nullptr;
+    float* pjc = gt_xyz ? pj + (size_t)n * K * 3 : nullptr;
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, h.frames, n, F, kParams, 0));
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pg, const_cast<float*>(s->gt_uv), h.frames, n, F,
+                                                                             2 * K, 0, rigs, rig));
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pc, const_cast<float*>(s->conf), h.frames, n, F, K,
+                                                                             0, rigs, rig));
+    if (rig)
+        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 32, 0, st>>>(h.packed_rig, const_cast<int*>(rig), h.frames, n,
+                                                                                F, 1, 0));
+    if (gt_xyz) {
+        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pj, const_cast<float*>(gt_xyz), h.frames, n, F,
+                                                                                 3 * K, 0));
+        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pjc, const_cast<float*>(conf3d), h.frames, n, F,
+                                                                                 K, 0));
+    }
+    const mvs_frame_stream fs{n, px, pg, pc, s->joint_weights, pj, pjc, pf};
+    int rc = run_stream(ctx, &fs, rig ? h.packed_rig : nullptr, 1, &cfg, c, stats, st);
+    if (rc) return rc;
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, h.frames, n, F, kParams, 1));
+    if (s->final_loss)
+        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 32, 0, st>>>(pf, s->final_loss, h.frames, n, F, 1, 1));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    return MVS_OK;
+}
+
+// What mvs_fit_shared_shape and mvs_debug_shape_closure share: the checks of the call, the stage's LossParams (3-D term as the
+// call says), the offsets on the host, and the scratch with the offsets and each frame's sequence on the device.  a0 gets the
+// shape closure's arguments except the chunk.
+static int shape_prepare(mvs_ctx* ctx, const char* who, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
+                         const int* rig, const mvs_loss_config* stage, int H, LossParams* lp, std::vector<int>* off,
+                         ShapeArgs* a0, cudaStream_t st) {
+    if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0))
+        return set_error(ctx, MVS_ERR_INVALID, "%s: model, cameras and batch must be set first", who);
+    if (!s || !stage) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    if (s->n_sequences < 1 || !s->seq_offsets)
+        return set_error(ctx, MVS_ERR_INVALID, "%s: n_sequences must be >= 1 (got %d) with seq_offsets", who, s->n_sequences);
+    if (!s->params || !s->gt_uv || !s->conf || !s->joint_weights)
+        return set_error(ctx, MVS_ERR_INVALID, "%s: params, gt_uv, conf and joint_weights are required", who);
+    if (s->seq_offsets[0] != 0) return set_error(ctx, MVS_ERR_INVALID, "%s: seq_offsets[0] must be 0", who);
+    for (int k = 0; k < s->n_sequences; ++k)
+        if (s->seq_offsets[k + 1] <= s->seq_offsets[k])
+            return set_error(ctx, MVS_ERR_INVALID, "%s: seq_offsets must ascend strictly (sequence %d is empty or negative)", who, k);
+    if (!gt_xyz != !conf3d) return set_error(ctx, MVS_ERR_INVALID, "%s: gt_xyz and conf3d go together", who);
+    if (stage->frozen_mask & 1u)
+        return set_error(ctx, MVS_ERR_INVALID, "%s: the stage freezes betas (fix_shape): the shape is given, there is nothing to "
+                                               "share", who);
+    if (stage->interpenetration)
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the shape closure is the frame-resident closure, which has no "
+                                                   "interpenetration (SDF) term", who);
+    if (ctx->anchor_enabled)
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the anchor term is per batch; switch it off (mvs_set_anchor enable = 0)", who);
+    if (!rig && ctx->rigs.size() > 1)
+        return set_error(ctx, MVS_ERR_INVALID, "%s: the context has %d camera rigs: give each frame's rig", who, (int)ctx->rigs.size());
+    int rc = make_loss_params(ctx, stage, lp);
+    if (rc) return rc;
+    lp->j3d_on = gt_xyz ? 1 : 0;
+    if (stage_regime(ctx, *lp, H, false) != kResident)
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the stage would not run in the frame-resident kernels (exec mode 1, "
+                                                   "history_size > 100, or a model they do not take)", who);
+    const int NS = s->n_sequences, F = s->seq_offsets[NS];
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    if (rig && (rc = check_frame_rigs(ctx, who, rig, F, st))) return rc;
+    off->assign(s->seq_offsets, s->seq_offsets + NS + 1);
+    const size_t packed = (size_t)F * (kParams + 1 + (size_t)ctx->vmax * ctx->m.K * 3 + (gt_xyz ? (size_t)ctx->m.K * 4 : 0));
+    if ((rc = ensure_shape_state(ctx, NS, F, packed))) return rc;
+    ShapeState& h = *ctx->shape;
+    std::vector<int> seq_of((size_t)F);
+    for (int q = 0; q < NS; ++q)
+        for (int f = (*off)[q]; f < (*off)[q + 1]; ++f) seq_of[f] = q;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.off, off->data(), off->size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.seq_of, seq_of.data(), (size_t)F * sizeof(int), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    *a0 = ShapeArgs{};
+    a0->in = FrameInputs{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d, rig};
+    a0->params = s->params;
+    a0->off = h.off;
+    a0->seq_of = h.seq_of;
+    a0->share_scale = (stage->frozen_mask >> 4 & 1u) ? 0 : 1;
+    a0->loss = h.loss;
+    a0->grad = h.grad;
+    return MVS_OK;
+}
+
 }  // namespace mvs
 
 using namespace mvs;
@@ -1304,6 +1545,43 @@ int mvs_fit_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages,
     return mvs_fit_seq_stream_rigs(ctx, s, nullptr, nullptr, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
 }
 
+int mvs_fit_shared_shape(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig_dev,
+                         const mvs_loss_config* stage, const mvs_lbfgs_config* opt_cfg, int n_sweeps, float* seq_loss_dev,
+                         mvs_lbfgs_stats* shape_stats, mvs_lbfgs_stats* pose_stats, void* stream) {
+    static const char* who = "mvs_fit_shared_shape";
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    if (!opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    if (n_sweeps < 1) return set_error(ctx, MVS_ERR_INVALID, "%s: n_sweeps must be >= 1 (got %d)", who, n_sweeps);
+    const cudaStream_t st = (cudaStream_t)stream;
+    LossParams lp;
+    std::vector<int> off;
+    ShapeArgs a0;
+    int rc = shape_prepare(ctx, who, s, gt_xyz, conf3d, rig_dev, stage, history_size(opt_cfg), &lp, &off, &a0, st);
+    if (rc) return rc;
+    if (shape_stats) memset(shape_stats, 0, sizeof(*shape_stats));
+    if (pose_stats) memset(pose_stats, 0, sizeof(*pose_stats));
+    const int NS = s->n_sequences, F = off[NS];
+    ShapeState& h = *ctx->shape;
+    mvs_loss_config pose_cfg = *stage;                                   // the pose step: the shared entries held
+    pose_cfg.frozen_mask |= 1u | (a0.share_scale ? 16u : 0u);
+    if (s->final_loss) MVS_CUDA_OK(ctx, cudaMemsetAsync(s->final_loss, 0xff, (size_t)F * sizeof(float), st));   // NaN: skipped
+    std::vector<int> ok((size_t)NS), frames;
+    for (int sweep = 0; sweep < n_sweeps && !rc; ++sweep) {
+        MVS_LAUNCH(ctx, KID_MISC, st, shape_consensus_kernel<<<NS, 32, 0, st>>>(s->params, h.off, a0.share_scale, h.rows, h.ok));
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ok.data(), h.ok, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
+        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+        if ((rc = shape_step(ctx, a0, off, ok, lp, opt_cfg, seq_loss_dev, shape_stats, st))) break;
+        MVS_LAUNCH(ctx, KID_MISC, st, shape_write_kernel<<<(F + 127) / 128, 128, 0, st>>>(s->params, h.seq_of, h.rows, h.ok, F,
+                                                                                        a0.share_scale));
+        frames.clear();
+        for (int q = 0; q < NS; ++q)
+            if (ok[q])
+                for (int f = off[q]; f < off[q + 1]; ++f) frames.push_back(f);
+        rc = shape_pose_step(ctx, s, gt_xyz, conf3d, rig_dev, frames, pose_cfg, opt_cfg, pose_stats, st);
+    }
+    return rc;
+}
+
 int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, const float* conf_host,
                  const float* joint_weights_host, int n_stages, const mvs_loss_config* stage_cfgs,
                  const mvs_lbfgs_config* opt_cfg, float* final_loss_host, mvs_lbfgs_stats* stats, void* stream) {
@@ -1414,6 +1692,42 @@ extern "C" int mvs_debug_lbfgs_advance(mvs_ctx* ctx, const mvs_lbfgs_config* c, 
     MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
+}
+
+// mvs_debug_shape_closure (tests/test_gpu_shared_shape.py): the shape closure of mvs_fit_shared_shape evaluated once, with the
+// same arguments, at the shared rows rows_dev [S][86] (device; the shared entries are read): loss_dev [S] and grad_dev [S][86]
+// (device) receive what the optimiser sees as loss_eval / g_eval of each sequence's problem.  Uses the context's optimiser state
+// (history size 100 when there is none).  Synchronises.
+extern "C" int mvs_debug_shape_closure(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
+                                       const int* rig_dev, const mvs_loss_config* stage, const float* rows_dev, float* loss_dev,
+                                       float* grad_dev, void* stream) {
+    static const char* who = "mvs_debug_shape_closure";
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    if (!rows_dev || !loss_dev || !grad_dev) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    const cudaStream_t st = (cudaStream_t)stream;
+    LossParams lp;
+    std::vector<int> off;
+    ShapeArgs a0;
+    int rc = shape_prepare(ctx, who, s, gt_xyz, conf3d, rig_dev, stage, 100, &lp, &off, &a0, st);
+    if (!rc) rc = ensure_state(ctx, ctx->lbfgs ? ctx->lbfgs->H : 100);
+    if (rc) return rc;
+    const int NS = s->n_sequences, B = ctx->ws.B;
+    ShapeState& h = *ctx->shape;
+    const std::vector<int> ok((size_t)NS, 1);
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.rows, rows_dev, (size_t)NS * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    for (int base = 0; base < NS && !rc; base += B) {
+        const int n = std::min(B, NS - base);
+        if ((rc = shape_chunk_start(ctx, base, n, ok, st))) break;
+        const LbfgsState& S = *ctx->lbfgs;
+        if ((rc = launch_shape_closure(ctx, shape_chunk_args(a0, off, base, n), lp, S, st))) break;
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(loss_dev + base, S.loss_eval, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(grad_dev + (size_t)base * kParams, S.g_eval, (size_t)n * kParams * sizeof(float),
+                                         cudaMemcpyDeviceToDevice, st));
+    }
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(ctx->ws.fidx, B, ctx->ws.na));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    return rc;
 }
 
 }  // extern "C"

@@ -293,7 +293,8 @@ def _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces, f
 
 def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool = False, fixed_scale: float = 1.0,
                  use_hip: bool = True, pose_format: str = "coco17", result_folder: str | None = None,
-                 mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, use_3d: bool = False):
+                 mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, use_3d: bool = False,
+                 shared_shape: int = 0):
     """The frame loop of main.py:32-89 for one sequence as ONE batch (every frame from its own initial guess, is_seq = False):
     upload the detections, initial guess on the device (init_guess + fix_params), all stages (`mvs_fit`), results per
     frame.  `ctx` is a FittingContext whose model, priors (GMM / VPoser decoder), cameras and batch (= number of frames) are
@@ -305,7 +306,10 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
     use_3d (the sequence loaded with load_sequence(use_3d=True)): the 3-D joint term for every frame with an annotation,
     whose initial guess also aligns to it; frames without one fit as without the term (_targets_3d, _init_guess_3d).  The
     context has the 3-D term off afterwards.
+    shared_shape (sweeps, 0: off): the sequence is one subject -- after the fit, one fit_shared_shape call gives all of its
+    frames one betas (and scale) under the last stage, see share_shape; results are written after it.
     Returns (params [F,86] numpy -- pose slot = latent code under VPoser --, final_loss [F], stats)."""
+    _check_shared_shape(shared_shape, None)
     F = len(seq["frames"])
     assert ctx.B <= F, "context batch %d > frames %d" % (ctx.B, F)
     latent = _uses_latent_pose(stage_cfgs)
@@ -325,6 +329,8 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
         final, stats = ctx.fit(params, stage_cfgs, opt_cfg)
         if t3 is not None:
             ctx.set_joints3d(None)
+        if shared_shape:
+            final = share_shape(ctx, params, seq["gt_uv"], seq["conf"], jw, [F], stage_cfgs, opt_cfg, shared_shape, t3, stats=stats)
         loss = final.cpu().numpy()
         if result_folder is not None:
             _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces)
@@ -335,6 +341,8 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
     else:
         final, stats = ctx.fit_stream(params, seq["gt_uv"], seq["conf"], jw, stage_cfgs, opt_cfg, joints3d=t3[0], conf3d=t3[1])
         ctx.set_joints3d(None)
+    if shared_shape:
+        final = share_shape(ctx, params, seq["gt_uv"], seq["conf"], jw, [F], stage_cfgs, opt_cfg, shared_shape, t3, stats=stats)
     loss = final.cpu().numpy()
     if result_folder is not None:
         _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces)
@@ -387,6 +395,28 @@ def _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, fac
         _export(ctx, seq, chunk, lc, latent, result_folder, mesh_folder, faces, frames=seq["frames"][c0:c0 + n], rows=range(n))
 
 
+def _check_shared_shape(shared_shape, temporal_weight) -> None:
+    if isinstance(shared_shape, bool) or int(shared_shape) != shared_shape or shared_shape < 0:
+        raise ValueError("shared_shape: want a number of sweeps >= 0 (0: off), got %r" % (shared_shape,))
+    if shared_shape and temporal_weight is not None:
+        raise ValueError("shared_shape and temporal_weight do not combine: the shared shape's pose step fits frames "
+                         "independently, so the causal temporal term cannot be honoured")
+
+
+def share_shape(ctx, params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, sweeps, t3=None, rig=None, stats=None):
+    """The shared shape of fit_sequences / fit_sequence: ONE fit_shared_shape call over the fitted rows params [F,86] (device,
+    updated in place) of all sequences (lengths), under the last stage configuration; t3 (_targets_3d of the frames) adds the
+    3-D term, rig [F] each frame's rig.  Returns the frames' final losses [F]; stats (a dict) gets 'shared_shape': the shape
+    and pose steps' counts."""
+    kw = {} if rig is None else dict(rig=rig)
+    if t3 is not None:
+        kw.update(joints3d=t3[0], conf3d=t3[1])
+    final, _, sh, po = ctx.fit_shared_shape(params, gt_uv, conf, jw, lengths, stage_cfgs[-1], opt_cfg, sweeps=int(sweeps), **kw)
+    if stats is not None:
+        stats["shared_shape"] = dict(shape=sh, pose=po)
+    return final
+
+
 def temporal_weight_vector(temporal_weight):
     """fit_sequences' temporal_weight as the 86 per-parameter weights the device takes: None stays None, a scalar lam is
     lam x sequence.smooth_mask() (global orientation, the pose slot and translation), an array is taken as the 86-vector"""
@@ -404,7 +434,7 @@ def temporal_weight_vector(temporal_weight):
 def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = False, fixed_scale: float = 1.0,
                   use_hip: bool = True, pose_format: str = "coco17", result_folder: str | None = None,
                   mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, reinit_loss: float = 5000.0,
-                  use_3d: bool = False, rigs=None, rig_data_weight_scale=None, temporal_weight=None):
+                  use_3d: bool = False, rigs=None, rig_data_weight_scale=None, temporal_weight=None, shared_shape: int = 0):
     """main.py:32-89 with is_seq = True for S sequences in lock-step: the batch of step t is frame t of every sequence
     (context batch = S).  A sequence's first frame gets the initial guess and every stage; a later frame
     starts from the previous frame's result as load_init + fix_params leave it (init_guess.py:137-166,190-212: betas,
@@ -427,7 +457,11 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
     predecessor's fitted row: its stages add sum_i w_i (x_i - x^_{t-1,i})^2 (mvs_fit_seq_temporal in lock-step, after step
     t-1 with that step's fitted rows; mvs_fit_seq_stream_temporal otherwise, with the same bits).  Cold frames are fitted as
     without it.
+    shared_shape (a number of sweeps, 0: off) gives every sequence one body shape: after the fit, ONE fit_shared_shape call
+    over all frames under the last stage configuration (the same call in lock-step and stream mode; see share_shape), and the
+    results and meshes are written after it.  It does not combine with temporal_weight (ValueError).
     Returns a list (per sequence) of (params [T_s,86], loss [T_s]) and the summed stats."""
+    _check_shared_shape(shared_shape, temporal_weight)
     S_ = len(seqs)
     tw = temporal_weight_vector(temporal_weight)
     latent = _uses_latent_pose(stage_cfgs)
@@ -451,7 +485,8 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
         return _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces,
                                      pose_format, use_hip, dict(estimate_scale=estimate_scale, fixed_scale=fixed_scale,
                                                                 use_torso=True, hip_seed=1.0, want_joints3d=False,
-                                                                umeyama_as_written=umeyama_as_written), t3, seq_rig, rig_views, tw)
+                                                                umeyama_as_written=umeyama_as_written), t3, seq_rig, rig_views, tw,
+                                     shared_shape)
     T = max(len(q["frames"]) for q in seqs)
     V = seqs[0]["gt_uv"].shape[0]
     off = np.concatenate([[0], np.cumsum([len(q["frames"]) for q in seqs])])
@@ -502,20 +537,34 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
         for s_, q in enumerate(seqs):
             if live[s_]:
                 out_x[s_][t], out_l[s_][t] = x[s_], prev_loss[s_]
-        if result_folder is not None:
+        if result_folder is not None and not shared_shape:
             for s_, q in enumerate(seqs):
                 if live[s_]:
                     _export(ctx, q, params, prev_loss, latent, result_folder, mesh_folder, faces, frames=[q["frames"][t]], rows=[s_])
     if t3 is not None:
         ctx.set_joints3d(None)
+    if shared_shape:
+        lengths = [len(q["frames"]) for q in seqs]
+        x = torch.as_tensor(np.concatenate(out_x), device=ctx.device).contiguous()
+        rig = None if seq_rig is None else np.repeat(seq_rig, lengths).astype(np.int32)
+        final = share_shape(ctx, x, np.concatenate([q["gt_uv"] for q in seqs], axis=1),
+                            np.concatenate([q["conf"] for q in seqs], axis=1), jw, lengths, stage_cfgs, opt_cfg, shared_shape, t3,
+                            rig, tot).cpu().numpy()
+        xs = x.cpu().numpy()
+        out_x = [xs[off[s_]:off[s_ + 1]] for s_ in range(S_)]
+        out_l = [final[off[s_]:off[s_ + 1]] for s_ in range(S_)]
+        if result_folder is not None:
+            for s_, q in enumerate(seqs):
+                _export_rows(ctx, q, x[off[s_]:off[s_ + 1]], out_l[s_], latent, result_folder, mesh_folder, faces)
     return list(zip(out_x, out_l)), tot
 
 
 def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces, pose_format,
-                          use_hip, guess, t3=None, seq_rig=None, rig_views=None, tw=None):
+                          use_hip, guess, t3=None, seq_rig=None, rig_views=None, tw=None, shared_shape=0):
     """fit_sequences through mvs_fit_seq_stream: the sequences' frames back to back, every frame's cold start point from
     _cold_guesses; t3: _targets_3d of those frames (mvs_fit_seq_stream3d); seq_rig [S]: each sequence's rig, which every
-    one of its frames takes (mvs_fit_seq_stream_rigs); tw [86]: the temporal weight (mvs_fit_seq_stream_temporal)"""
+    one of its frames takes (mvs_fit_seq_stream_rigs); tw [86]: the temporal weight (mvs_fit_seq_stream_temporal);
+    shared_shape: sweeps of share_shape after the fit (0: off)"""
     lengths = [len(q["frames"]) for q in seqs]
     off = np.concatenate([[0], np.cumsum(lengths)])
     gt_uv = np.concatenate([q["gt_uv"] for q in seqs], axis=1)
@@ -532,6 +581,8 @@ def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, r
         final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss,
                                           joints3d=t3[0], conf3d=t3[1], **kw)
         ctx.set_joints3d(None)
+    if shared_shape:
+        final = share_shape(ctx, params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, shared_shape, t3, rig, stats)
     x, loss = params.cpu().numpy(), final.cpu().numpy()
     if result_folder is not None:
         for s_, q in enumerate(seqs):
