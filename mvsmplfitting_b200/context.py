@@ -299,23 +299,16 @@ class FittingContext:
         cfg = opt_cfg or self.make_lbfgs_config()
         final = torch.empty(self.B, dtype=torch.float32, device=self.device)
         st = _lib.LbfgsStats()
+        tw = None
         if temporal_weight is not None:
             if warm is None or prev is None:
                 raise ValueError("fit: temporal_weight needs warm and prev")
             assert prev.is_cuda and prev.dtype == torch.float32 and prev.is_contiguous() and tuple(prev.shape) == (self.B, 86)
-            wm = np.ascontiguousarray(np.asarray(warm).astype(np.uint8).reshape(self.B))
             tw = _temporal_weight(temporal_weight)
-            _lib.check(self.h, self.lib.mvs_fit_seq_temporal(self.h, _ptr(params), len(stage_cfgs), arr, ctypes.byref(cfg),
-                                                             _ptr(wm), _ptr(prev), _ptr(tw), _ptr(final), ctypes.byref(st),
-                                                             self._stream()), "mvs_fit_seq_temporal")
-        elif warm is not None:
-            wm = np.ascontiguousarray(np.asarray(warm).astype(np.uint8).reshape(self.B))
-            _lib.check(self.h, self.lib.mvs_fit_seq(self.h, _ptr(params), len(stage_cfgs), arr, ctypes.byref(cfg),
-                                                    wm.ctypes.data_as(ctypes.c_void_p), _ptr(final), ctypes.byref(st),
-                                                    self._stream()), "mvs_fit_seq")
-        else:
-            _lib.check(self.h, self.lib.mvs_fit(self.h, _ptr(params), len(stage_cfgs), arr, ctypes.byref(cfg), _ptr(final),
-                                                ctypes.byref(st), self._stream()), "mvs_fit")
+        wm = None if warm is None else np.ascontiguousarray(np.asarray(warm).astype(np.uint8).reshape(self.B))
+        _lib.check(self.h, self.lib.mvs_fit_seq_temporal(self.h, _ptr(params), len(stage_cfgs), arr, ctypes.byref(cfg), _ptr(wm),
+                                                         _ptr(prev if tw is not None else None), _ptr(tw), _ptr(final),
+                                                         ctypes.byref(st), self._stream()), "mvs_fit_seq_temporal")
         return final, _stats_dict(st)
 
     def _stream_rows(self, who, F, gt_uv, conf, joint_weights, joints3d, conf3d):
@@ -360,13 +353,8 @@ class FittingContext:
         cfg = opt_cfg or self.make_lbfgs_config()
         st = _lib.LbfgsStats()
         self._j3d_keep = None
-        if rg is None:
-            _lib.check(self.h, self.lib.mvs_fit_stream(self.h, ctypes.byref(s), len(stage_cfgs), arr, ctypes.byref(cfg),
-                                                       ctypes.byref(st), self._stream()), "mvs_fit_stream")
-        else:
-            _lib.check(self.h, self.lib.mvs_fit_stream_rigs(self.h, ctypes.byref(s), _ptr(rg), len(stage_cfgs), arr,
-                                                            ctypes.byref(cfg), ctypes.byref(st), self._stream()),
-                       "mvs_fit_stream_rigs")
+        _lib.check(self.h, self.lib.mvs_fit_stream_rigs(self.h, ctypes.byref(s), _ptr(rg), len(stage_cfgs), arr, ctypes.byref(cfg),
+                                                        ctypes.byref(st), self._stream()), "mvs_fit_stream_rigs")
         return final, _stats_dict(st)
 
     def fit_seq_stream(self, params: torch.Tensor, gt_uv, conf, joint_weights, lengths, stage_cfgs, opt_cfg=None,
@@ -396,22 +384,10 @@ class FittingContext:
         cfg = opt_cfg or self.make_lbfgs_config()
         st = _lib.LbfgsStats()
         self._j3d_keep = None
-        if temporal_weight is not None:
-            tw = _temporal_weight(temporal_weight)
-            _lib.check(self.h, self.lib.mvs_fit_seq_stream_temporal(self.h, ctypes.byref(s), _ptr(j3), _ptr(c3), _ptr(rg), _ptr(tw),
-                                                                    len(stage_cfgs), arr, ctypes.byref(cfg), ctypes.byref(st),
-                                                                    self._stream()), "mvs_fit_seq_stream_temporal")
-        elif rg is not None:
-            _lib.check(self.h, self.lib.mvs_fit_seq_stream_rigs(self.h, ctypes.byref(s), _ptr(j3), _ptr(c3), _ptr(rg),
+        tw = None if temporal_weight is None else _temporal_weight(temporal_weight)
+        _lib.check(self.h, self.lib.mvs_fit_seq_stream_temporal(self.h, ctypes.byref(s), _ptr(j3), _ptr(c3), _ptr(rg), _ptr(tw),
                                                                 len(stage_cfgs), arr, ctypes.byref(cfg), ctypes.byref(st),
-                                                                self._stream()), "mvs_fit_seq_stream_rigs")
-        elif j3 is None:
-            _lib.check(self.h, self.lib.mvs_fit_seq_stream(self.h, ctypes.byref(s), len(stage_cfgs), arr, ctypes.byref(cfg),
-                                                           ctypes.byref(st), self._stream()), "mvs_fit_seq_stream")
-        else:
-            _lib.check(self.h, self.lib.mvs_fit_seq_stream3d(self.h, ctypes.byref(s), _ptr(j3), _ptr(c3), len(stage_cfgs), arr,
-                                                             ctypes.byref(cfg), ctypes.byref(st), self._stream()),
-                       "mvs_fit_seq_stream3d")
+                                                                self._stream()), "mvs_fit_seq_stream_temporal")
         return final, _stats_dict(st)
 
     def fit_shared_shape(self, params: torch.Tensor, gt_uv, conf, joint_weights, lengths, stage_cfg, opt_cfg=None, sweeps=1,

@@ -8,6 +8,7 @@
 #include <string.h>
 
 #include "mvs_internal.cuh"
+#include "mvs_lbfgs_core.cuh"
 
 static std::string g_last_error;
 
@@ -31,6 +32,11 @@ template <class T> int dev_alloc(mvs_ctx* ctx, T** p, size_t count) {
     *p = static_cast<T*>(d);
     return MVS_OK;
 }
+void dev_free(mvs_ctx* ctx, void* p) {
+    if (!p) return;
+    ctx->allocs.erase(std::find(ctx->allocs.begin(), ctx->allocs.end(), p));
+    cudaFree(p);
+}
 template <class T> int dev_upload(mvs_ctx* ctx, T** p, const T* host, size_t count) {
     int rc = dev_alloc(ctx, p, count);
     if (rc) return rc;
@@ -45,6 +51,10 @@ template int dev_alloc<unsigned char>(mvs_ctx*, unsigned char**, size_t);
 template int dev_alloc<int2>(mvs_ctx*, int2**, size_t);
 template int dev_alloc<FrameBox>(mvs_ctx*, FrameBox**, size_t);
 template int dev_alloc<SdfFrameSetup>(mvs_ctx*, SdfFrameSetup**, size_t);
+template int dev_alloc<long long>(mvs_ctx*, long long**, size_t);
+template int dev_alloc<Rig>(mvs_ctx*, Rig**, size_t);
+template int dev_alloc<LossParams>(mvs_ctx*, LossParams**, size_t);
+template int dev_alloc<FrameScalars>(mvs_ctx*, FrameScalars**, size_t);
 template int dev_upload<float>(mvs_ctx*, float**, const float*, size_t);
 template int dev_upload<int>(mvs_ctx*, int**, const int*, size_t);
 
@@ -220,6 +230,8 @@ void mvs_destroy(mvs_ctx* ctx) {
     cudaDeviceSynchronize();
     for (int k = 0; k < KID_COUNT; ++k)
         for (cudaEvent_t e : ctx->prof.ev[k]) cudaEventDestroy(e);
+    release_fit_state(ctx);
+    release_tc_state(ctx);
     for (void* p : ctx->allocs) cudaFree(p);
     delete ctx;
 }
@@ -486,20 +498,8 @@ int mvs_set_camera_rigs(mvs_ctx* ctx, int n_rigs, const int* num_views, const fl
     }
     // no kernel may still read the table it replaces
     MVS_CUDA_OK(ctx, cudaDeviceSynchronize());
-    if (ctx->rigs_cap < n_rigs) {
-        if (ctx->rigs_dev) {
-            ctx->allocs.erase(std::find(ctx->allocs.begin(), ctx->allocs.end(), (void*)ctx->rigs_dev));
-            cudaFree(ctx->rigs_dev);
-            ctx->rigs_dev = nullptr;
-        }
-        ctx->rigs_cap = 0;
-        void* d = nullptr;
-        MVS_CUDA_OK(ctx, cudaMalloc(&d, (size_t)n_rigs * sizeof(Rig)));
-        ctx->allocs.push_back(d);
-        ctx->rigs_dev = static_cast<Rig*>(d);
-        ctx->rigs_cap = n_rigs;
-    }
-    MVS_CUDA_OK(ctx, cudaMemcpy(ctx->rigs_dev, rigs.data(), (size_t)n_rigs * sizeof(Rig), cudaMemcpyHostToDevice));
+    if (int rc = dev_grow(ctx, ctx->rigs_dev, (size_t)n_rigs)) return rc;
+    MVS_CUDA_OK(ctx, cudaMemcpy(ctx->rigs_dev.p, rigs.data(), (size_t)n_rigs * sizeof(Rig), cudaMemcpyHostToDevice));
     ctx->rigs = std::move(rigs);
     ctx->vmax = vmax;
     ctx->have_cams = true;

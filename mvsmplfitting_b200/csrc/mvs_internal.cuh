@@ -140,8 +140,13 @@ struct LbfgsCfg;
 struct FrameScalars;
 struct TcState;
 struct StreamState;                   // mvs_fit_stream scratch (mvs_lbfgs.cu)
-struct SeqState;                      // mvs_fit_seq_stream scratch (mvs_lbfgs.cu)
-struct ShapeState;                    // mvs_fit_shared_shape scratch (mvs_lbfgs.cu)
+struct SeqState;                      // mvs_fit_seq_stream and mvs_fit_shared_shape scratch (mvs_lbfgs.cu)
+
+// A device array of the context that only grows (dev_grow): cap elements at p
+template <class T> struct DevBuf {
+    T* p = nullptr;
+    size_t cap = 0;
+};
 
 // The frames a frame-resident run fits when they are not the context's batch (mvs_fit_stream): n frames, every array with
 // row stride n (gt_uv [V][n][K][2], conf [V][n][K], j3d_xyz [n][K][3], j3d_conf [n][K]; the 3-D pair may be NULL; rig [n]
@@ -296,8 +301,7 @@ struct mvs_ctx {
     mvs::DevModel m;
     // camera rigs (mvs_set_camera_rigs; mvs_set_cameras is a table of one): host copy and device table
     std::vector<mvs::Rig> rigs;
-    mvs::Rig* rigs_dev = nullptr;
-    int rigs_cap = 0;                // rigs the device table holds
+    mvs::DevBuf<mvs::Rig> rigs_dev;
     int vmax = 0;                    // largest view count of the table: the view rows of every detection array
     std::vector<int> slot_rig_host;  // [B] per-slot rigs of mvs_set_frame_rigs
     const int* slot_rigs = nullptr;  // per-slot rigs the batch entry points read (ws.slot_rig), NULL: none given (rig 0)
@@ -310,7 +314,8 @@ struct mvs_ctx {
     bool j3d_enabled = false;
     int exec_mode = 0;               // mvs_set_exec_mode: 0 auto, 1 batched chain only, 2 stage barriers, 3 dense-round closures
     bool have_model = false, have_cams = false, have_kp = false, have_loss = false;
-    std::vector<void*> allocs;       // everything cudaMalloc'ed, freed in mvs_destroy
+    std::vector<void*> allocs;       // everything cudaMalloc'ed, freed in mvs_destroy (dev_alloc / dev_free)
+    // The state objects below are set only once complete, and released by mvs_destroy (release_fit_state, release_tc_state)
     mvs::LbfgsState* lbfgs = nullptr;    // optimiser state (mvs_lbfgs.cu)
     mvs::Profiler prof;
     mvs::TcState* tc = nullptr;          // tensor-core path state (mvs_tc.cu)
@@ -318,8 +323,7 @@ struct mvs_ctx {
     float rest_scale = -1.f;
     int2* stage_rng = nullptr;       // [B] per-frame slice of the stage table (mvs_fit_seq), device
     mvs::StreamState* fstream = nullptr;  // frame-stream scratch (mvs_fit_stream), created on first use
-    mvs::SeqState* sstream = nullptr;     // sequence-stream scratch (mvs_fit_seq_stream), created on first use
-    mvs::ShapeState* shape = nullptr;     // shared-shape scratch (mvs_fit_shared_shape), created on first use
+    mvs::SeqState* sstream = nullptr;     // sequence-stream and shared-shape scratch, created on first use
 };
 
 namespace mvs {
@@ -397,6 +401,17 @@ __device__ __forceinline__ void warp_argmax(float& v, int& idx) {
 }
 
 template <class T> int dev_alloc(mvs_ctx* ctx, T** p, size_t count);
+void dev_free(mvs_ctx* ctx, void* p);          // a dev_alloc'ed array (NULL: nothing)
+// Room for n elements in b: a larger array replaces a smaller one (its contents are lost).  b.cap counts only what is
+// allocated: after a failed allocation b is empty.
+template <class T> int dev_grow(mvs_ctx* ctx, DevBuf<T>& b, size_t n) {
+    if (b.cap >= n) return MVS_OK;
+    dev_free(ctx, b.p);
+    b = DevBuf<T>{};
+    if (int rc = dev_alloc(ctx, &b.p, n)) return rc;
+    b.cap = n;
+    return MVS_OK;
+}
 template <class T> int dev_upload(mvs_ctx* ctx, T** p, const T* host, size_t count);
 
 // mvs_lbfgs.cu: mvs_closure through the frame-resident closure, a dense round or the batched chain
@@ -448,10 +463,12 @@ int ensure_keypoint_ws(mvs_ctx* ctx);          // mvs_api.cu: gt_uv / conf for t
 // mvs_api.cu: the rigs of the batch's slots (ctx->slot_rigs); MVS_ERR_INVALID when the table has several rigs and no per-slot
 // rigs were given
 int batch_rigs(mvs_ctx* ctx, const char* who);
-inline RigSet slot_rig_set(const mvs_ctx* ctx) { return RigSet{ctx->rigs_dev, ctx->slot_rigs}; }
+inline RigSet slot_rig_set(const mvs_ctx* ctx) { return RigSet{ctx->rigs_dev.p, ctx->slot_rigs}; }
 // mvs_api.cu: every entry of rig_dev [n] names a rig of the table; MVS_ERR_INVALID naming the first frame that does not.
 // Synchronises st.
 int check_frame_rigs(mvs_ctx* ctx, const char* who, const int* rig_dev, int n, cudaStream_t st);
+void release_fit_state(mvs_ctx* ctx);          // mvs_lbfgs.cu: the optimiser state and the stream scratch (mvs_destroy)
+void release_tc_state(mvs_ctx* ctx);           // mvs_tc.cu (mvs_destroy)
 int sdf_grid_launch(mvs_ctx* ctx, float* phi, const int* faces, int num_faces, const float* verts, int batch,
                     int n_verts, int G, cudaStream_t st);
 }  // namespace mvs

@@ -29,6 +29,7 @@
 #include <vector>
 #include <cstdlib>
 #include <functional>
+#include <memory>
 #include "mvs_internal.cuh"
 #include "mvs_lbfgs_core.cuh"
 
@@ -144,8 +145,7 @@ __global__ void iota2_kernel(int* p, int n, int* na) {
 // mvs_fit_stream / mvs_fit_seq_stream (DESIGN.md section 4): the context's B slots are lanes, each holding one frame of the
 // call's F frames
 struct StreamState {
-    int cap = 0;                        // entries of sc
-    FrameScalars* sc = nullptr;         // [cap] frame scalars of the frame-resident groups (one per frame of the stream)
+    DevBuf<FrameScalars> sc;            // frame scalars of the frame-resident groups (one per frame of the stream)
     int* lane_frame = nullptr;          // [B] frame held by each lane of a dense group, -1: none
     long long* lane_start = nullptr;    // [B] round of the group in which the lane's frame started
     float* lane_params = nullptr;       // [B][86] the lanes' parameters (what params_dev is to mvs_fit)
@@ -313,42 +313,46 @@ __global__ void copy_rows_kernel(T* __restrict__ packed, T* __restrict__ full, c
     }
 }
 
+// The host resources of the state objects; their device arrays belong to ctx->allocs
+static void release(LbfgsState* S) {
+    if (!S) return;
+    cudaFreeHost(S->na_host);
+    cudaFreeHost(S->lp_tab_host);
+    for (cudaEvent_t e : S->na_event)
+        if (e) cudaEventDestroy(e);
+    delete S;
+}
+static void release(StreamState* ss) {
+    if (!ss) return;
+    cudaFreeHost(ss->host);
+    delete ss;
+}
+struct ReleaseState { template <class T> void operator()(T* p) const { release(p); } };
+
 static int ensure_state(mvs_ctx* ctx, int H) {
-    LbfgsState* S = ctx->lbfgs;
     const int B = ctx->ws.B;
-    if (S && S->B == B && S->H == H) return MVS_OK;
-    if (S) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_run: history_size changed between calls (%d -> %d)", S->H, H);
-    S = new LbfgsState();
+    if (ctx->lbfgs && ctx->lbfgs->B == B && ctx->lbfgs->H == H) return MVS_OK;
+    if (ctx->lbfgs)
+        return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_run: history_size changed between calls (%d -> %d)", ctx->lbfgs->H, H);
+    std::unique_ptr<LbfgsState, ReleaseState> S(new LbfgsState());
     S->B = B; S->H = H;
     int rc;
     const size_t V = (size_t)B * kParams;
-    if ((rc = dev_alloc(ctx, &S->g, V))) return rc;
-    if ((rc = dev_alloc(ctx, &S->d, V))) return rc;
-    if ((rc = dev_alloc(ctx, &S->prev_g, V))) return rc;
-    if ((rc = dev_alloc(ctx, &S->x_init, V))) return rc;
-    if ((rc = dev_alloc(ctx, &S->g_prev, V))) return rc;
-    if ((rc = dev_alloc(ctx, &S->bg, 2 * V))) return rc;
-    if ((rc = dev_alloc(ctx, &S->hist_y, V * H))) return rc;
-    if ((rc = dev_alloc(ctx, &S->hist_s, V * H))) return rc;
-    if ((rc = dev_alloc(ctx, &S->ro, (size_t)B * H))) return rc;
-    if ((rc = dev_alloc(ctx, &S->gram, (size_t)B * kGramFloats))) return rc;
-    if ((rc = dev_alloc(ctx, &S->x_eval, V))) return rc;
-    if ((rc = dev_alloc(ctx, &S->loss_eval, B))) return rc;
-    if ((rc = dev_alloc(ctx, &S->g_eval, V))) return rc;
-    if ((rc = dev_alloc(ctx, &S->x_fit, V))) return rc;
-    if ((rc = dev_alloc(ctx, &S->final_fit, B))) return rc;
-    unsigned char* raw = nullptr;
-    if ((rc = dev_alloc(ctx, &raw, (size_t)B * sizeof(FrameScalars)))) return rc;
-    S->sc = reinterpret_cast<FrameScalars*>(raw);
-    unsigned char* raw2 = nullptr;
-    if ((rc = dev_alloc(ctx, &raw2, 4 * sizeof(long long)))) return rc;
-    S->totals = reinterpret_cast<long long*>(raw2);
+    if ((rc = dev_alloc(ctx, &S->g, V)) || (rc = dev_alloc(ctx, &S->d, V)) || (rc = dev_alloc(ctx, &S->prev_g, V)) ||
+        (rc = dev_alloc(ctx, &S->x_init, V)) || (rc = dev_alloc(ctx, &S->g_prev, V)) || (rc = dev_alloc(ctx, &S->bg, 2 * V)) ||
+        (rc = dev_alloc(ctx, &S->hist_y, V * H)) || (rc = dev_alloc(ctx, &S->hist_s, V * H)) ||
+        (rc = dev_alloc(ctx, &S->ro, (size_t)B * H)) || (rc = dev_alloc(ctx, &S->gram, (size_t)B * kGramFloats)) ||
+        (rc = dev_alloc(ctx, &S->x_eval, V)) || (rc = dev_alloc(ctx, &S->loss_eval, B)) || (rc = dev_alloc(ctx, &S->g_eval, V)) ||
+        (rc = dev_alloc(ctx, &S->x_fit, V)) || (rc = dev_alloc(ctx, &S->final_fit, B)) || (rc = dev_alloc(ctx, &S->sc, B)) ||
+        (rc = dev_alloc(ctx, &S->totals, 4)) || (rc = dev_alloc(ctx, &S->lp_tab, kMaxStages)))
+        return rc;
     MVS_CUDA_OK(ctx, cudaMallocHost(&S->na_host, 8 * sizeof(long long)));
     MVS_CUDA_OK(ctx, cudaMallocHost(&S->lp_tab_host, kMaxStages * sizeof(LossParams)));
-    unsigned char* raw3 = nullptr;
-    if ((rc = dev_alloc(ctx, &raw3, kMaxStages * sizeof(LossParams)))) return rc;
-    S->lp_tab = reinterpret_cast<LossParams*>(raw3);
-    ctx->lbfgs = S;
+    // blocking sync: the host thread sleeps while it waits for a chunk of dense rounds (several contexts are driven by as many
+    // host threads; spinning ones would compete with the threads that have launches to enqueue)
+    for (cudaEvent_t& e : S->na_event)
+        MVS_CUDA_OK(ctx, cudaEventCreateWithFlags(&e, cudaEventDisableTiming | cudaEventBlockingSync));
+    ctx->lbfgs = S.release();
     return MVS_OK;
 }
 
@@ -443,12 +447,6 @@ static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int n
     if (rc) return rc;
     // The host only needs the active count to know when to stop, so chunk k+1 is enqueued BEFORE the count of
     // chunk k is awaited (kernels exit at once when the list is empty): the GPU never idles on the host round trip.
-    if (!S.na_event[0]) {
-        // blocking sync: the host thread sleeps while it waits for a chunk (several contexts are driven by as many host
-        // threads; spinning ones would compete with the threads that have launches to enqueue)
-        MVS_CUDA_OK(ctx, cudaEventCreateWithFlags(&S.na_event[0], cudaEventDisableTiming | cudaEventBlockingSync));
-        MVS_CUDA_OK(ctx, cudaEventCreateWithFlags(&S.na_event[1], cudaEventDisableTiming | cudaEventBlockingSync));
-    }
     int* na_slots = reinterpret_cast<int*>(S.na_host);           // [0], [1]: two chunks in flight
     int* queue_slots = la ? ctx->fstream->host : nullptr;         // the same chunks' queue positions
     bool drained = la == nullptr;                                 // the host has seen the queue empty
@@ -526,13 +524,20 @@ static int run_batched(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, boo
     return MVS_OK;
 }
 
-// Adds a run's totals th ([0..2] iterations, evaluations, NaN / Inf stops) and its rounds to stats, and to the dense counters
-// for a dense run
-static void add_totals(mvs_lbfgs_stats* stats, const long long* th, long long rounds, bool dense) {
-    if (!stats) return;
+// End of every run: waits for st, then adds the run's totals (S.totals: iterations, evaluations, NaN / Inf stops) and its
+// rounds (S.totals[3], or *rounds_dev when given) to stats, and to the dense counters for a dense run
+static int read_totals(mvs_ctx* ctx, const long long* rounds_dev, bool dense, mvs_lbfgs_stats* stats, cudaStream_t st) {
+    LbfgsState& S = *ctx->lbfgs;
+    long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    if (rounds_dev) MVS_CUDA_OK(ctx, cudaMemcpyAsync(th + 3, rounds_dev, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    if (!stats) return MVS_OK;
     stats->frame_iterations += th[0]; stats->frame_evals += th[1]; stats->frames_nan += (int)th[2];
-    stats->rounds += (int)rounds;
-    if (dense) { stats->dense_frame_evals += th[1]; stats->dense_rounds += (int)rounds; }
+    stats->rounds += (int)th[3];
+    if (dense) { stats->dense_frame_evals += th[1]; stats->dense_rounds += (int)th[3]; }
+    return MVS_OK;
 }
 
 // End of a run: final losses and totals.  The frame-resident kernel wrote the last gradient itself and leaves the active
@@ -545,13 +550,8 @@ static int end_run(mvs_ctx* ctx, Regime rg, float* final_loss_dev, float* last_g
     MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_finalize_kernel<<<(B + 255) / 256, 256, 0, st>>>(S, B, final_loss_dev, S.totals, rg != kBatched));
     if (rg != kResident && last_grad_dev)
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(last_grad_dev, S.g_eval, (size_t)B * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
     if (rg != kResident) MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    add_totals(stats, th, th[3], rg == kDense);
-    MVS_CUDA_OK(ctx, cudaGetLastError());
-    return MVS_OK;
+    return read_totals(ctx, nullptr, rg == kDense, stats, st);
 }
 
 // Runs the stages o.lps[0 .. o.nst) (default: ctx->loss).  nst > 1 requires that all of them run in the same regime
@@ -686,28 +686,40 @@ static int stream_runs(mvs_ctx* ctx, const char* who, const std::vector<LossPara
     return MVS_OK;
 }
 
-// All stages of a fit.  Consecutive stages that run in the same regime are handed to ONE multi-stage run in which
-// every frame changes stage on its own (frames are independent problems, so a frame that converged need not wait at
-// the stage boundary for the slowest one; the per-frame arithmetic is the sequential schedule's).  exec_mode 2 keeps
-// the stage barrier (one run per stage).
+// The stage a run starts with becomes the context's loss config (what the kernels and a later mvs_lbfgs_run read)
+static void use_stage(mvs_ctx* ctx, const LossParams& lp) {
+    ctx->loss = lp;
+    ctx->have_loss = true;
+}
+
+// Each slot's slice [rng[2b], rng[2b+1]) of the next run's stage table, in ctx->stage_rng.  Synchronises: rng is reused.
+static int upload_stage_rng(mvs_ctx* ctx, const std::vector<int>& rng, cudaStream_t st) {
+    int rc;
+    if (!ctx->stage_rng && (rc = dev_alloc(ctx, &ctx->stage_rng, (size_t)ctx->ws.B))) return rc;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->stage_rng, rng.data(), rng.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    return MVS_OK;
+}
+
+// All stages of a fit (who: the entry point called).  Consecutive stages that run in the same regime are handed to ONE
+// multi-stage run in which every frame changes stage on its own (frames are independent problems, so a frame that converged
+// need not wait at the stage boundary for the slowest one; the per-frame arithmetic is the sequential schedule's).  exec_mode 2
+// keeps the stage barrier (one run per stage).
 // temporal (mvs_fit_seq_temporal): the warm frames' stages carry the anchor term of the rows the caller put in ws.anchor / anchor_w.
-static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg,
-                   float* final_loss_dev, mvs_lbfgs_stats* stats, cudaStream_t st, const unsigned char* warm_host = nullptr,
-                   bool temporal = false) {
+static int run_fit(mvs_ctx* ctx, const char* who, float* x_dev, int n_stages, const mvs_loss_config* stage_cfgs,
+                   const mvs_lbfgs_config* opt_cfg, float* final_loss_dev, mvs_lbfgs_stats* stats, cudaStream_t st,
+                   const unsigned char* warm_host = nullptr, bool temporal = false) {
     std::vector<LossParams> lps;
-    int rc = stage_table(ctx, "mvs_fit", n_stages, stage_cfgs, -1, &lps);
+    int rc = stage_table(ctx, who, n_stages, stage_cfgs, -1, &lps);
     if (rc) return rc;
     const int B = ctx->ws.B;
     bool any_warm = false;
     if (warm_host)
         for (int b = 0; b < B; ++b) any_warm |= warm_host[b] != 0;
     if (any_warm && n_stages <= kWarmSkip)
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq: warm-started frames skip the first %d stages, %d given", kWarmSkip, n_stages);
+        return set_error(ctx, MVS_ERR_INVALID, "%s: warm-started frames skip the first %d stages, %d given", who, kWarmSkip, n_stages);
     std::vector<LossParams> wlps;
-    if (any_warm) {
-        if ((rc = warm_stage_table(ctx, stage_cfgs, -1, lps, &wlps, temporal))) return rc;
-        if (!ctx->stage_rng && (rc = dev_alloc(ctx, &ctx->stage_rng, (size_t)B))) return rc;
-    }
+    if (any_warm && (rc = warm_stage_table(ctx, stage_cfgs, -1, lps, &wlps, temporal))) return rc;
     const int H = history_size(opt_cfg);
     const int max_run = any_warm ? kMaxStages / 2 : kMaxStages;       // the table holds the cold and the warm slice of a run
     std::vector<int> rng;
@@ -716,16 +728,15 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
     while (i < n_stages) {
         const Regime rg = stage_regime(ctx, lps[i], H, false);
         const int j = stage_group_end(ctx, lps, i, H, max_run);
-        ctx->loss = lps[i];
-        ctx->have_loss = true;
+        use_stage(ctx, lps[i]);
         RunOpts o;
         if (!any_warm) {
             o.lps = &lps[i];
             o.nst = j - i;
         } else {
             if (rg == kBatched)
-                return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq: warm-started frames are not implemented in the batched "
-                                                       "reference chain (exec mode 1 / a model the resident kernels do not take)");
+                return set_error(ctx, MVS_ERR_INVALID, "%s: warm-started frames are not implemented in the batched reference "
+                                                       "chain (exec mode 1 / a model the resident kernels do not take)", who);
             // table of this run: cold stages i .. j-1, then the warm slice max(i, 2) .. j-1
             tab.assign(lps.begin() + i, lps.begin() + j);
             const int wi = i > kWarmSkip ? i : kWarmSkip;
@@ -739,8 +750,7 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
                 rng[2 * b + 1] = wm ? wend : j - i;
                 o.some_inactive |= wm && wbegin == wend;
             }
-            MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->stage_rng, rng.data(), rng.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-            MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));           // rng is reused by the next run
+            if ((rc = upload_stage_rng(ctx, rng, st))) return rc;
             o.lps = tab.data();
             o.nst = (int)tab.size();
             o.stage_rng = ctx->stage_rng;
@@ -753,40 +763,20 @@ static int run_fit(mvs_ctx* ctx, float* x_dev, int n_stages, const mvs_loss_conf
     return MVS_OK;
 }
 
-static void dev_free(mvs_ctx* ctx, void* p) {
-    for (auto it = ctx->allocs.begin(); it != ctx->allocs.end(); ++it)
-        if (*it == p) { ctx->allocs.erase(it); break; }
-    cudaFree(p);
-}
-
 // Lane state of the dense groups, and frame scalars for F frames when a frame-resident group runs (grow-only)
 static int ensure_stream_state(mvs_ctx* ctx, int F_resident) {
-    int rc;
     if (!ctx->fstream) {
-        StreamState* ss = new StreamState();
-        ctx->fstream = ss;
+        std::unique_ptr<StreamState, ReleaseState> ss(new StreamState());
         const size_t B = (size_t)ctx->ws.B;
-        unsigned char* raw = nullptr;
-        if ((rc = dev_alloc(ctx, &ss->lane_frame, B))) return rc;
-        if ((rc = dev_alloc(ctx, &raw, B * sizeof(long long)))) return rc;
-        ss->lane_start = reinterpret_cast<long long*>(raw);
-        if ((rc = dev_alloc(ctx, &ss->lane_params, B * kParams))) return rc;
-        if ((rc = dev_alloc(ctx, &ss->queue, 1))) return rc;
-        if ((rc = dev_alloc(ctx, &raw, sizeof(long long)))) return rc;
-        ss->end_round = reinterpret_cast<long long*>(raw);
+        int rc;
+        if ((rc = dev_alloc(ctx, &ss->lane_frame, B)) || (rc = dev_alloc(ctx, &ss->lane_start, B)) ||
+            (rc = dev_alloc(ctx, &ss->lane_params, B * kParams)) || (rc = dev_alloc(ctx, &ss->queue, 1)) ||
+            (rc = dev_alloc(ctx, &ss->end_round, 1)))
+            return rc;
         MVS_CUDA_OK(ctx, cudaMallocHost(&ss->host, 2 * sizeof(int)));
+        ctx->fstream = ss.release();
     }
-    StreamState& ss = *ctx->fstream;
-    if (ss.cap < F_resident) {
-        if (ss.sc) dev_free(ctx, ss.sc);
-        ss.sc = nullptr;
-        ss.cap = 0;
-        unsigned char* raw = nullptr;
-        if ((rc = dev_alloc(ctx, &raw, (size_t)F_resident * sizeof(FrameScalars)))) return rc;
-        ss.sc = reinterpret_cast<FrameScalars*>(raw);
-        ss.cap = F_resident;
-    }
-    return MVS_OK;
+    return dev_grow(ctx, ctx->fstream->sc, (size_t)F_resident);
 }
 
 // The lanes' keypoint rows, and their 3-D target rows when with_j3d
@@ -809,11 +799,10 @@ static int run_lanes(mvs_ctx* ctx, LaneArgs& a, const float* joint_weights, cons
     StreamState& ss = *ctx->fstream;
     Workspace& w = ctx->ws;
     const int B = w.B, K = ctx->m.K;
-    long long* th = reinterpret_cast<long long*>(S.na_host) + 1;      // [0..2] totals, [4] rounds
     int rc;
     if ((rc = frame_step_begin_run(ctx, st))) return rc;                 // (allocates the pose cache on first use)
     a.B = B; a.K = K;
-    a.rigs = ctx->rigs_dev;
+    a.rigs = ctx->rigs_dev.p;
     a.ws_gt_uv = w.gt_uv; a.ws_conf = w.conf; a.ws_j3d_xyz = w.j3d_xyz; a.ws_j3d_conf = w.j3d_conf; a.ws_rig = w.slot_rig;
     ctx->slot_rigs = a.rig ? w.slot_rig : nullptr;                       // the dense kernels read each lane's rig
     a.lane_frame = ss.lane_frame; a.lane_start = ss.lane_start; a.lane_params = ss.lane_params; a.queue = ss.queue;
@@ -829,18 +818,14 @@ static int run_lanes(mvs_ctx* ctx, LaneArgs& a, const float* joint_weights, cons
     if ((rc = run_dense(ctx, ss.lane_params, cfg, nst, st, &a))) return rc;
     // whatever the round limit left in the lanes (nothing, when every frame finished)
     MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lane_refill_kernel<<<1, 1024, 0, st>>>(S, a, 0, 1));
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 3 * sizeof(long long), cudaMemcpyDeviceToHost, st));
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(th + 4, ss.end_round, sizeof(long long), cudaMemcpyDeviceToHost, st));
     MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    MVS_CUDA_OK(ctx, cudaGetLastError());
-    add_totals(stats, th, th[4], true);
-    return MVS_OK;
+    return read_totals(ctx, ss.end_round, true, stats, st);
 }
 
 // One run of mvs_fit_stream: stages lps[0 .. nst) of one regime over all F frames of the stream
 static int run_stream_group(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig, Regime rg, const LossParams* lps, int nst,
                             const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats, cudaStream_t st) {
+    use_stage(ctx, lps[0]);
     LbfgsCfg cfg;
     int rc = begin_run(ctx, c, false, lps, nst, &cfg, st);
     if (rc) return rc;
@@ -848,19 +833,14 @@ static int run_stream_group(mvs_ctx* ctx, const mvs_frame_stream* s, const int* 
     if (rg == kResident) {
         // one launch over all F frames, one CTA each: the block scheduler refills the SMs as frames finish
         LbfgsState& S = *ctx->lbfgs;
-        StreamState& ss = *ctx->fstream;
-        long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
+        FrameScalars* sc = ctx->fstream->sc.p;
         const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, s->gt_xyz, s->conf3d, rig};
-        if ((rc = launch_lbfgs_resident(ctx, s->params, cfg, cfg.history, S.lp_tab, lps, nst, ss.sc, nullptr, st, nullptr, &in)))
+        if ((rc = launch_lbfgs_resident(ctx, s->params, cfg, cfg.history, S.lp_tab, lps, nst, sc, nullptr, st, nullptr, &in)))
             return rc;
         LbfgsState Sf = S;
-        Sf.sc = ss.sc;
+        Sf.sc = sc;
         MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_finalize_kernel<<<(F + 255) / 256, 256, 0, st>>>(Sf, F, s->final_loss, S.totals, 1));
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
-        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-        MVS_CUDA_OK(ctx, cudaGetLastError());
-        add_totals(stats, th, th[3], false);
-        return MVS_OK;
+        return read_totals(ctx, nullptr, false, stats, st);
     }
     LaneArgs a{};
     a.F = F; a.n_queue = F;
@@ -870,73 +850,112 @@ static int run_stream_group(mvs_ctx* ctx, const mvs_frame_stream* s, const int* 
     return run_lanes(ctx, a, s->joint_weights, cfg, nst, stats, st);
 }
 
-// mvs_fit_stream: the stage groups of run_fit, each over all F frames before the next starts (rig [F] or NULL: rig 0)
-static int run_stream(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig, int n_stages, const mvs_loss_config* stage_cfgs,
-                      const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, cudaStream_t st) {
+// A stream call's writes to the context.  Its dense runs overwrite the slots' keypoint, 3-D target and rig rows, so from the
+// start the context holds none of them; at the end its loss config is the call's last stage, without the call's 3-D term.
+static void stream_call_begin(mvs_ctx* ctx) {
+    ctx->have_kp = false;
+    ctx->j3d_enabled = false;
+    ctx->slot_rigs = nullptr;
+}
+static void stream_call_end(mvs_ctx* ctx, const LossParams& last) {
+    ctx->loss = last;
+    ctx->loss.j3d_on = 0;
+    ctx->slot_rigs = nullptr;
+}
+
+// mvs_fit_stream (who: the entry point called): the stage groups of run_fit, each over all F frames before the next starts
+// (rig [F] or NULL: rig 0)
+static int run_stream(mvs_ctx* ctx, const char* who, const mvs_frame_stream* s, const int* rig, int n_stages,
+                      const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, cudaStream_t st) {
     const int H = history_size(opt_cfg);
     std::vector<LossParams> lps;
     std::vector<int> ends;
-    int rc = stage_table(ctx, "mvs_fit_stream", n_stages, stage_cfgs, s->gt_xyz ? 1 : 0, &lps);
-    if (!rc) rc = stream_runs(ctx, "mvs_fit_stream", lps, H, kMaxStages, &ends);
+    int rc = stage_table(ctx, who, n_stages, stage_cfgs, s->gt_xyz ? 1 : 0, &lps);
+    if (!rc) rc = stream_runs(ctx, who, lps, H, kMaxStages, &ends);
     if (rc) return rc;
     bool any_dense = false, any_resident = false;
     for (int i = 0, g = 0; i < n_stages; i = ends[g++]) (stage_regime(ctx, lps[i], H, false) == kDense ? any_dense : any_resident) = true;
     rc = ensure_stream_state(ctx, any_resident ? s->n_frames : 0);
     if (!rc && any_dense) rc = ensure_lane_rows(ctx, s->gt_xyz != nullptr);
     if (rc) return rc;
-    // the dense groups overwrite the lanes' keypoint, 3-D target and rig rows: from here on the context holds none of them
-    ctx->have_kp = false;
-    ctx->j3d_enabled = false;
-    ctx->slot_rigs = nullptr;
-    for (int i = 0, g = 0; i < n_stages && !rc; i = ends[g++]) {
-        ctx->loss = lps[i];
-        ctx->have_loss = true;
+    stream_call_begin(ctx);
+    for (int i = 0, g = 0; i < n_stages && !rc; i = ends[g++])
         rc = run_stream_group(ctx, s, rig, stage_regime(ctx, lps[i], H, false), &lps[i], ends[g] - i, opt_cfg, stats, st);
-    }
-    ctx->loss = lps[n_stages - 1];
-    ctx->loss.j3d_on = 0;
-    ctx->slot_rigs = nullptr;
+    stream_call_end(ctx, lps[n_stages - 1]);
     return rc;
 }
 
-// mvs_fit_seq_stream scratch, grow-only in the number of sequences
+// mvs_fit_seq_stream and mvs_fit_shared_shape scratch (DESIGN.md section 4), every array grow-only.  A context runs one call at
+// a time, so the two share it: off and the gathered frames (gather_frames) serve both.
 struct SeqState {
-    int cap = 0;                        // sequences
-    int *off = nullptr, *cur = nullptr, *act = nullptr, *frames = nullptr;   // [cap+1], [cap], [cap], [cap]
-    int* lane_seq = nullptr;            // [B]
-    size_t packed_cap = 0;
-    float* packed = nullptr;            // the pending cold frames' rows for the runs before the chaining run
-    int* packed_rig = nullptr;          // [cap] their rigs
-    size_t tw_cap = 0;
-    float* tw = nullptr;                // [tw_cap / 86][86] the temporal weight, one row per frame (frame-resident chaining)
+    DevBuf<int> off;                    // [S+1] the call's sequence offsets
+    DevBuf<int> frames, packed_rig;     // [n] the gathered frames, their rigs
+    DevBuf<float> packed;               // their packed rows (gather_floats)
+    DevBuf<int> cur, act, lane_seq;     // sequence stream: [S], [S], [B] (SeqChain, LaneArgs)
+    DevBuf<float> tw;                   // [F][86] the temporal weight, one row per frame (frame-resident chaining)
+    DevBuf<int> ok, seq_of;             // shared shape: [S] the sequence has a finite row, [F] each frame's sequence
+    DevBuf<float> rows;                 // [S + B][86] each sequence's shared row: the x of its problem (B rows of padding for
+                                        // the slots a last chunk leaves empty)
+    DevBuf<float> seq_final;            // [B] run_fitting's value of each slot's problem
+    DevBuf<float> loss, grad;           // [F], [F][86] the shape closure's per-frame terms
 };
 
-static int ensure_seq_state(mvs_ctx* ctx, int nseq, size_t packed_floats) {
-    int rc;
-    if (!ctx->sstream) {
-        ctx->sstream = new SeqState();
-        if ((rc = dev_alloc(ctx, &ctx->sstream->lane_seq, (size_t)ctx->ws.B))) return rc;
-    }
+static SeqState& seq_state(mvs_ctx* ctx) {
+    if (!ctx->sstream) ctx->sstream = new SeqState();
+    return *ctx->sstream;
+}
+
+// The floats of n gathered frames' packed rows: params | gt_uv | conf, a final loss each with with_loss, then gt_xyz | conf3d
+// with the 3-D term
+static size_t gather_floats(const mvs_ctx* ctx, int n, bool with_loss, bool j3d) {
+    const size_t K = (size_t)ctx->m.K;
+    return (size_t)n * (kParams + (size_t)ctx->vmax * K * 3 + (with_loss ? 1 : 0) + (j3d ? K * 4 : 0));
+}
+
+// Frames idx[0 .. n) of a sequence-stream call's arrays (gt_xyz / conf3d and rig as the call gives them, both NULL / NULL: none)
+// packed into the scratch as the frame stream *fs of n frames, with final-loss rows when with_loss; *prig: their rigs, NULL
+// without rig
+static int gather_frames(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig,
+                         const std::vector<int>& idx, bool with_loss, mvs_frame_stream* fs, const int** prig, cudaStream_t st) {
     SeqState& q = *ctx->sstream;
-    if (q.cap < nseq) {
-        for (int* p : {q.off, q.cur, q.act, q.frames, q.packed_rig})
-            if (p) dev_free(ctx, p);
-        q.cap = 0;
-        if ((rc = dev_alloc(ctx, &q.off, (size_t)nseq + 1))) return rc;
-        if ((rc = dev_alloc(ctx, &q.cur, (size_t)nseq))) return rc;
-        if ((rc = dev_alloc(ctx, &q.act, (size_t)nseq))) return rc;
-        if ((rc = dev_alloc(ctx, &q.frames, (size_t)nseq))) return rc;
-        if ((rc = dev_alloc(ctx, &q.packed_rig, (size_t)nseq))) return rc;
-        q.cap = nseq;
+    const int n = (int)idx.size(), F = s->seq_offsets[s->n_sequences], V = ctx->vmax, K = ctx->m.K;
+    int rc;
+    if ((rc = dev_grow(ctx, q.frames, (size_t)n)) || (rc = dev_grow(ctx, q.packed_rig, (size_t)n)) ||
+        (rc = dev_grow(ctx, q.packed, gather_floats(ctx, n, with_loss, gt_xyz != nullptr))))
+        return rc;
+    const int* fr = q.frames.p;
+    const Rig* rigs = ctx->rigs_dev.p;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(q.frames.p, idx.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+    float* px = q.packed.p;
+    float* pg = px + (size_t)n * kParams;
+    float* pc = pg + (size_t)V * n * K * 2;
+    float* pf = pc + (size_t)V * n * K;
+    float* pj = gt_xyz ? pf + (with_loss ? n : 0) : nullptr;
+    float* pjc = gt_xyz ? pj + (size_t)n * K * 3 : nullptr;
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, fr, n, F, kParams, 0));
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pg, const_cast<float*>(s->gt_uv), fr, n, F, 2 * K, 0,
+                                                                             rigs, rig));
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pc, const_cast<float*>(s->conf), fr, n, F, K, 0,
+                                                                             rigs, rig));
+    if (rig)
+        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 32, 0, st>>>(q.packed_rig.p, const_cast<int*>(rig), fr, n, F, 1, 0));
+    if (gt_xyz) {
+        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pj, const_cast<float*>(gt_xyz), fr, n, F, 3 * K, 0));
+        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pjc, const_cast<float*>(conf3d), fr, n, F, K, 0));
     }
-    if (q.packed_cap < packed_floats) {
-        if (q.packed) dev_free(ctx, q.packed);
-        q.packed = nullptr;
-        q.packed_cap = 0;
-        if ((rc = dev_alloc(ctx, &q.packed, packed_floats))) return rc;
-        q.packed_cap = packed_floats;
-    }
+    *fs = mvs_frame_stream{n, px, pg, pc, s->joint_weights, pj, pjc, with_loss ? pf : nullptr};
+    *prig = rig ? q.packed_rig.p : nullptr;
     return MVS_OK;
+}
+
+// The gathered frames' rows (gather_frames) back to the call's parameters, and their final losses when fs has them and the
+// call wants them
+static void scatter_frames(mvs_ctx* ctx, const mvs_sequence_stream* s, const mvs_frame_stream& fs, cudaStream_t st) {
+    const int n = fs.n_frames, F = s->seq_offsets[s->n_sequences];
+    const int* fr = ctx->sstream->frames.p;
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(fs.params, s->params, fr, n, F, kParams, 1));
+    if (fs.final_loss && s->final_loss)
+        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 32, 0, st>>>(fs.final_loss, s->final_loss, fr, n, F, 1, 1));
 }
 
 // The slots' anchor rows and weights (as mvs_set_anchor allocates them), weights set to w for every slot
@@ -961,6 +980,7 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
                          Regime rg, const std::vector<LossParams>& tab, const SeqChain& q0, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats,
                          cudaStream_t st, bool temporal) {
     const int nst = (int)tab.size();
+    use_stage(ctx, tab[0]);
     LbfgsCfg cfg;
     int rc = begin_run(ctx, c, false, tab.data(), nst, &cfg, st);
     if (rc) return rc;
@@ -970,53 +990,48 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
     q.totals = S.totals;
     if (rg == kResident) {
         // one launch, one CTA per sequence; rounds: the largest number of evaluations one CTA ran (its frames' sum)
-        long long* th = reinterpret_cast<long long*>(S.na_host) + 1;
         const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d, rig};
         if ((rc = launch_lbfgs_resident_seq(ctx, s->params, cfg, cfg.history, S.lp_tab, tab.data(), nst, in, q, st,
-                                            temporal ? ctx->sstream->tw : nullptr)))
+                                            temporal ? ctx->sstream->tw.p : nullptr)))
             return rc;
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(th, S.totals, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
-        MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-        MVS_CUDA_OK(ctx, cudaGetLastError());
-        add_totals(stats, th, th[3], false);
-        return MVS_OK;
+        return read_totals(ctx, nullptr, false, stats, st);
     }
     LaneArgs a{};
     a.F = F; a.n_queue = q.n_act;
     a.params = s->params; a.final_loss = s->final_loss; a.gt_uv = s->gt_uv; a.conf = s->conf;
     a.j3d_xyz = gt_xyz; a.j3d_conf = conf3d; a.rig = rig;
     a.q = q;
-    a.lane_seq = ctx->sstream->lane_seq;
+    a.lane_seq = ctx->sstream->lane_seq.p;
     a.anchor = temporal ? ctx->ws.anchor : nullptr;
     return run_lanes(ctx, a, s->joint_weights, cfg, nst, stats, st);
 }
 
-// mvs_fit_seq_stream (DESIGN.md section 4).  Stages are grouped into runs as mvs_fit_seq groups them; run c holds stages
-// 2 .. n-1 and is the chaining run.  Each pass takes the pending cold frames P (at first: every sequence's first frame) through
-// the runs before c (as a frame stream of P's rows), then runs c over their sequences; a sequence whose next frame turns
-// out cold parks it for the next pass (c > 0 only: with c == 0 the cold frame stays in its slot with the cold slice).
+// mvs_fit_seq_stream (DESIGN.md section 4; who: the entry point called).  Stages are grouped into runs as mvs_fit_seq groups
+// them; run c holds stages 2 .. n-1 and is the chaining run.  Each pass takes the pending cold frames P (at first: every
+// sequence's first frame) through the runs before c (as a frame stream of P's rows), then runs c over their sequences; a
+// sequence whose next frame turns out cold parks it for the next pass (c > 0 only: with c == 0 the cold frame stays in its slot
+// with the cold slice).
 // gt_xyz / conf3d ([F][K][3] / [F][K], both NULL or both set): the 3-D joint term is on in every stage, cold and warm, iff set;
 // they travel with the frames as gt_uv / conf do, and so does rig ([F] or NULL: every frame has rig 0).
 // tw ([86] host, NULL: off): the temporal weight; every warm frame's stages carry sum_i tw_i (x_i - predecessor's fitted x_i)^2.
-static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig,
-                          int n_stages,
-                          const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
-                          cudaStream_t st, const float* tw = nullptr) {
+static int run_seq_stream(mvs_ctx* ctx, const char* who, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
+                          const int* rig, int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg,
+                          mvs_lbfgs_stats* stats, cudaStream_t st, const float* tw) {
     const int NS = s->n_sequences;
     const std::vector<int> off(s->seq_offsets, s->seq_offsets + NS + 1);
     const int F = off[NS];
     const int j3d = gt_xyz ? 1 : 0;                                   // the call's own targets, never the context's
     std::vector<LossParams> lps, wlps;
-    int rc = stage_table(ctx, "mvs_fit_seq_stream", n_stages, stage_cfgs, j3d, &lps);
+    int rc = stage_table(ctx, who, n_stages, stage_cfgs, j3d, &lps);
     if (rc) return rc;
     int n_vp2 = 0;
     for (const LossParams& lp : lps) n_vp2 += lp.use_vposer == 2;
     if (n_vp2 > 0 && n_vp2 < n_stages)
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: stages mix latent-code (use_vposer = 2) and axis-angle poses");
+        return set_error(ctx, MVS_ERR_INVALID, "%s: stages mix latent-code (use_vposer = 2) and axis-angle poses", who);
     if ((rc = warm_stage_table(ctx, stage_cfgs, j3d, lps, &wlps, tw != nullptr))) return rc;
     const int H = history_size(opt_cfg);
     std::vector<int> ends;
-    if ((rc = stream_runs(ctx, "mvs_fit_seq_stream", lps, H, kMaxStages / 2, &ends))) return rc;
+    if ((rc = stream_runs(ctx, who, lps, H, kMaxStages / 2, &ends))) return rc;
     int c = -1, ic = 0;
     bool any_dense = false, resident_before = false;
     for (int i = 0, g = 0; i < n_stages; i = ends[g++]) {
@@ -1026,9 +1041,9 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
         else if (c < 0) resident_before |= rg == kResident;
     }
     if (ends[c] != n_stages)
-        return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_seq_stream: stages %d .. %d do not form one run (the run holding stage "
-                                                   "%d ends at %d; exec mode 2, or a change of regime, SDF grid or face mode)",
-                         kWarmSkip, n_stages - 1, kWarmSkip, ends[c]);
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: stages %d .. %d do not form one run (the run holding stage %d ends at %d; "
+                                                   "exec mode 2, or a change of regime, SDF grid or face mode)",
+                         who, kWarmSkip, n_stages - 1, kWarmSkip, ends[c]);
     // the chaining run's table: cold stages ic .. n-1, then the warm slice 2 .. n-1
     std::vector<LossParams> tab(lps.begin() + ic, lps.end());
     const int wbegin = (int)tab.size();
@@ -1039,39 +1054,28 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
     q.reinit_loss = s->reinit_loss;
     q.park = c > 0 ? 1 : 0;
     q.keep_pose = n_vp2 == 0 ? 1 : 0;
-    // a frame's packed row: params | gt_uv | conf, then gt_xyz | conf3d with the 3-D term
-    const size_t row_floats = kParams + (size_t)ctx->vmax * ctx->m.K * 3 + (gt_xyz ? (size_t)ctx->m.K * 4 : 0);
+    SeqState& ss = seq_state(ctx);
     rc = ensure_stream_state(ctx, resident_before ? NS : 0);
-    if (!rc) rc = ensure_seq_state(ctx, NS, c > 0 ? row_floats * NS : 0);
+    if (!rc && !(rc = dev_grow(ctx, ss.off, (size_t)NS + 1)) && !(rc = dev_grow(ctx, ss.cur, (size_t)NS)) &&
+        !(rc = dev_grow(ctx, ss.act, (size_t)NS)))
+        rc = dev_grow(ctx, ss.lane_seq, (size_t)ctx->ws.B);
     if (!rc && any_dense) rc = ensure_lane_rows(ctx, gt_xyz != nullptr);
     if (rc) return rc;
-    SeqState& ss = *ctx->sstream;
     const Regime rg_chain = stage_regime(ctx, lps[ic], H, false);
     if (tw && rg_chain == kResident) {                                // a weight row per frame, as the closure indexes them
-        if (ss.tw_cap < (size_t)F * kParams) {
-            if (ss.tw) dev_free(ctx, ss.tw);
-            ss.tw = nullptr;
-            ss.tw_cap = 0;
-            if ((rc = dev_alloc(ctx, &ss.tw, (size_t)F * kParams))) return rc;
-            ss.tw_cap = (size_t)F * kParams;
-        }
+        if ((rc = dev_grow(ctx, ss.tw, (size_t)F * kParams))) return rc;
         Row86 r;
         for (int i = 0; i < kParams; ++i) r.v[i] = tw[i];
-        MVS_LAUNCH(ctx, KID_MISC, st, fill_rows_kernel<<<(F * kParams + 255) / 256, 256, 0, st>>>(ss.tw, r, F));
+        MVS_LAUNCH(ctx, KID_MISC, st, fill_rows_kernel<<<(F * kParams + 255) / 256, 256, 0, st>>>(ss.tw.p, r, F));
     } else if (tw && (rc = temporal_slot_rows(ctx, tw, st))) {         // dense: per lane
         return rc;
     }
-    q.off = ss.off;
-    q.cur = ss.cur;
-    q.act = ss.act;
-    // the dense runs overwrite the slots' keypoint rows: from here on the context holds none (and no 3-D targets or rigs)
-    ctx->have_kp = false;
-    ctx->j3d_enabled = false;
-    ctx->slot_rigs = nullptr;
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.off, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    q.off = ss.off.p;
+    q.cur = ss.cur.p;
+    q.act = ss.act.p;
+    stream_call_begin(ctx);
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.off.p, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     std::vector<int> cur(off.begin(), off.end() - 1), act, frames;   // each sequence's pending cold frame, -1: done
-    const int V = ctx->vmax, K = ctx->m.K;
-    const Rig* rigs = ctx->rigs_dev;
     while (!rc) {
         act.clear();
         frames.clear();
@@ -1079,48 +1083,24 @@ static int run_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, const floa
             if (cur[k] >= 0) { act.push_back(k); frames.push_back(cur[k]); }
         if (act.empty()) break;
         const int n = (int)act.size();
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.cur, cur.data(), (size_t)NS * sizeof(int), cudaMemcpyHostToDevice, st));
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.act, act.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.cur.p, cur.data(), (size_t)NS * sizeof(int), cudaMemcpyHostToDevice, st));
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.act.p, act.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
         if (c > 0) {
             // the pending frames through the runs before c, as a frame stream of their packed rows
-            MVS_CUDA_OK(ctx, cudaMemcpyAsync(ss.frames, frames.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
-            float* px = ss.packed;
-            float* pg = px + (size_t)n * kParams;
-            float* pc = pg + (size_t)V * n * K * 2;
-            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, ss.frames, n, F, kParams, 0));
-            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pg, const_cast<float*>(s->gt_uv), ss.frames, n, F, 2 * K, 0,
-                                                                                     rigs, rig));
-            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pc, const_cast<float*>(s->conf), ss.frames, n, F, K, 0,
-                                                                                     rigs, rig));
-            if (rig)
-                MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 32, 0, st>>>(ss.packed_rig, const_cast<int*>(rig), ss.frames, n, F, 1, 0));
-            float *pj = nullptr, *pjc = nullptr;
-            if (gt_xyz) {
-                pj = pc + (size_t)V * n * K;
-                pjc = pj + (size_t)n * K * 3;
-                MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pj, const_cast<float*>(gt_xyz), ss.frames, n, F, 3 * K, 0));
-                MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pjc, const_cast<float*>(conf3d), ss.frames, n, F, K, 0));
-            }
-            const mvs_frame_stream fs{n, px, pg, pc, s->joint_weights, pj, pjc, nullptr};
-            for (int i = 0, g = 0; g < c && !rc; i = ends[g++]) {
-                ctx->loss = lps[i];
-                ctx->have_loss = true;
-                rc = run_stream_group(ctx, &fs, rig ? ss.packed_rig : nullptr, stage_regime(ctx, lps[i], H, false), &lps[i],
-                                      ends[g] - i, opt_cfg, stats, st);
-            }
+            mvs_frame_stream fs;
+            const int* prig;
+            if ((rc = gather_frames(ctx, s, gt_xyz, conf3d, rig, frames, false, &fs, &prig, st))) break;
+            for (int i = 0, g = 0; g < c && !rc; i = ends[g++])
+                rc = run_stream_group(ctx, &fs, prig, stage_regime(ctx, lps[i], H, false), &lps[i], ends[g] - i, opt_cfg, stats, st);
             if (rc) break;
-            MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, ss.frames, n, F, kParams, 1));
+            scatter_frames(ctx, s, fs, st);
         }
         q.n_act = n;
-        ctx->loss = lps[ic];
-        ctx->have_loss = true;
         if ((rc = run_seq_chain(ctx, s, gt_xyz, conf3d, rig, F, rg_chain, tab, q, opt_cfg, stats, st, tw != nullptr))) break;
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(cur.data(), ss.cur, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(cur.data(), ss.cur.p, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
     }
-    ctx->loss = lps[n_stages - 1];
-    ctx->loss.j3d_on = 0;
-    ctx->slot_rigs = nullptr;
+    stream_call_end(ctx, lps[n_stages - 1]);
     return rc;
 }
 
@@ -1143,54 +1123,6 @@ static int check_temporal_weight(mvs_ctx* ctx, const char* who, const float* w, 
                                                    "(exec mode 1)", who);
     if (ctx->anchor_enabled)
         return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the temporal term uses the anchor rows; switch mvs_set_anchor off first", who);
-    return MVS_OK;
-}
-
-// mvs_fit_shared_shape scratch (DESIGN.md section 4), grow-only in sequences and frames
-struct ShapeState {
-    int s_cap = 0, f_cap = 0;
-    int *off = nullptr, *ok = nullptr;  // [s_cap+1], [s_cap] (ok: the sequence has a finite row)
-    float* rows = nullptr;              // [s_cap + B][86] each sequence's shared row: the x of its problem (B rows of padding
-                                        // for the slots a last chunk leaves empty)
-    float* seq_final = nullptr;         // [B] run_fitting's value of each slot's problem
-    int *seq_of = nullptr, *frames = nullptr, *packed_rig = nullptr;    // [f_cap] each
-    float *loss = nullptr, *grad = nullptr;                             // [f_cap], [f_cap][86] the shape closure's per-frame terms
-    size_t packed_cap = 0;
-    float* packed = nullptr;            // the pose step's frame stream: rows, detections, 3-D targets, final losses
-};
-
-static int ensure_shape_state(mvs_ctx* ctx, int NS, int F, size_t packed_floats) {
-    int rc;
-    if (!ctx->shape) ctx->shape = new ShapeState();
-    ShapeState& h = *ctx->shape;
-    const int B = ctx->ws.B;
-    if (!h.seq_final && (rc = dev_alloc(ctx, &h.seq_final, (size_t)B))) return rc;
-    if (h.s_cap < NS) {
-        for (void* p : {(void*)h.off, (void*)h.ok, (void*)h.rows})
-            if (p) dev_free(ctx, p);
-        h.s_cap = 0;
-        if ((rc = dev_alloc(ctx, &h.off, (size_t)NS + 1)) || (rc = dev_alloc(ctx, &h.ok, (size_t)NS)) ||
-            (rc = dev_alloc(ctx, &h.rows, ((size_t)NS + B) * kParams)))
-            return rc;
-        h.s_cap = NS;
-    }
-    if (h.f_cap < F) {
-        for (void* p : {(void*)h.seq_of, (void*)h.frames, (void*)h.packed_rig, (void*)h.loss, (void*)h.grad})
-            if (p) dev_free(ctx, p);
-        h.f_cap = 0;
-        if ((rc = dev_alloc(ctx, &h.seq_of, (size_t)F)) || (rc = dev_alloc(ctx, &h.frames, (size_t)F)) ||
-            (rc = dev_alloc(ctx, &h.packed_rig, (size_t)F)) || (rc = dev_alloc(ctx, &h.loss, (size_t)F)) ||
-            (rc = dev_alloc(ctx, &h.grad, (size_t)F * kParams)))
-            return rc;
-        h.f_cap = F;
-    }
-    if (h.packed_cap < packed_floats) {
-        if (h.packed) dev_free(ctx, h.packed);
-        h.packed = nullptr;
-        h.packed_cap = 0;
-        if ((rc = dev_alloc(ctx, &h.packed, packed_floats))) return rc;
-        h.packed_cap = packed_floats;
-    }
     return MVS_OK;
 }
 
@@ -1235,8 +1167,6 @@ static int shape_chunk_start(mvs_ctx* ctx, int base, int n, const std::vector<in
     LbfgsState& S = *ctx->lbfgs;
     Workspace& w = ctx->ws;
     const int B = w.B;
-    int rc;
-    if (!ctx->stage_rng && (rc = dev_alloc(ctx, &ctx->stage_rng, (size_t)B))) return rc;
     std::vector<int> rng((size_t)B * 2, 0);
     bool some_inactive = false;
     for (int j = 0; j < B; ++j) {
@@ -1244,10 +1174,9 @@ static int shape_chunk_start(mvs_ctx* ctx, int base, int n, const std::vector<in
         rng[2 * j + 1] = on ? 1 : 0;
         some_inactive |= !on;
     }
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->stage_rng, rng.data(), rng.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    if (int rc = upload_stage_rng(ctx, rng, st)) return rc;
     MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-    MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_init_kernel<<<B, 32, 0, st>>>(S, ctx->shape->rows + (size_t)base * kParams, B, 1, 1,
+    MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_init_kernel<<<B, 32, 0, st>>>(S, ctx->sstream->rows.p + (size_t)base * kParams, B, 1, 1,
                                                                        ctx->stage_rng));
     if (some_inactive) MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
     return MVS_OK;
@@ -1266,7 +1195,7 @@ static ShapeArgs shape_chunk_args(const ShapeArgs& a0, const std::vector<int>& o
 static int shape_step(mvs_ctx* ctx, const ShapeArgs& a0, const std::vector<int>& off, const std::vector<int>& ok,
                       const LossParams& lp, const mvs_lbfgs_config* c, float* seq_loss, mvs_lbfgs_stats* stats, cudaStream_t st) {
     const int NS = (int)off.size() - 1, B = ctx->ws.B;
-    ShapeState& h = *ctx->shape;
+    SeqState& h = *ctx->sstream;
     for (int base = 0; base < NS; base += B) {
         const int n = std::min(B, NS - base);
         LbfgsCfg cfg;
@@ -1276,10 +1205,10 @@ static int shape_step(mvs_ctx* ctx, const ShapeArgs& a0, const std::vector<int>&
         const LbfgsState S = *ctx->lbfgs;
         const ShapeArgs a = shape_chunk_args(a0, off, base, n);
         const std::function<int()> closure = [&]() { return launch_shape_closure(ctx, a, lp, S, st); };
-        if ((rc = run_batched(ctx, h.rows + (size_t)base * kParams, cfg, lp.use_vposer == 2, st, closure))) return rc;
-        if ((rc = end_run(ctx, kBatched, h.seq_final, nullptr, stats, st))) return rc;
+        if ((rc = run_batched(ctx, h.rows.p + (size_t)base * kParams, cfg, lp.use_vposer == 2, st, closure))) return rc;
+        if ((rc = end_run(ctx, kBatched, h.seq_final.p, nullptr, stats, st))) return rc;
         if (seq_loss)
-            MVS_CUDA_OK(ctx, cudaMemcpyAsync(seq_loss + base, h.seq_final, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+            MVS_CUDA_OK(ctx, cudaMemcpyAsync(seq_loss + base, h.seq_final.p, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
     }
     return MVS_OK;
 }
@@ -1289,51 +1218,101 @@ static int shape_step(mvs_ctx* ctx, const ShapeArgs& a0, const std::vector<int>&
 static int shape_pose_step(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig,
                            const std::vector<int>& frames, const mvs_loss_config& cfg, const mvs_lbfgs_config* c,
                            mvs_lbfgs_stats* stats, cudaStream_t st) {
-    const int n = (int)frames.size(), F = s->seq_offsets[s->n_sequences], V = ctx->vmax, K = ctx->m.K;
-    if (n == 0) return MVS_OK;
-    ShapeState& h = *ctx->shape;
-    const Rig* rigs = ctx->rigs_dev;
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.frames, frames.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
-    float* px = h.packed;
-    float* pg = px + (size_t)n * kParams;
-    float* pc = pg + (size_t)V * n * K * 2;
-    float* pf = pc + (size_t)V * n * K;
-    float* pj = gt_xyz ? pf + n : nullptr;
-    float* pjc = gt_xyz ? pj + (size_t)n * K * 3 : nullptr;
-    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, h.frames, n, F, kParams, 0));
-    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pg, const_cast<float*>(s->gt_uv), h.frames, n, F,
-                                                                             2 * K, 0, rigs, rig));
-    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pc, const_cast<float*>(s->conf), h.frames, n, F, K,
-                                                                             0, rigs, rig));
-    if (rig)
-        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 32, 0, st>>>(h.packed_rig, const_cast<int*>(rig), h.frames, n,
-                                                                                F, 1, 0));
-    if (gt_xyz) {
-        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pj, const_cast<float*>(gt_xyz), h.frames, n, F,
-                                                                                 3 * K, 0));
-        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pjc, const_cast<float*>(conf3d), h.frames, n, F,
-                                                                                 K, 0));
-    }
-    const mvs_frame_stream fs{n, px, pg, pc, s->joint_weights, pj, pjc, pf};
-    int rc = run_stream(ctx, &fs, rig ? h.packed_rig : nullptr, 1, &cfg, c, stats, st);
+    if (frames.empty()) return MVS_OK;
+    mvs_frame_stream fs;
+    const int* prig;
+    int rc = gather_frames(ctx, s, gt_xyz, conf3d, rig, frames, true, &fs, &prig, st);
+    if (!rc) rc = run_stream(ctx, "mvs_fit_shared_shape", &fs, prig, 1, &cfg, c, stats, st);
     if (rc) return rc;
-    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, h.frames, n, F, kParams, 1));
-    if (s->final_loss)
-        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 32, 0, st>>>(pf, s->final_loss, h.frames, n, F, 1, 1));
+    scatter_frames(ctx, s, fs, st);
     MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }
 
-// What mvs_fit_shared_shape and mvs_debug_shape_closure share: the checks of the call, the stage's LossParams (3-D term as the
-// call says), the offsets on the host, and the scratch with the offsets and each frame's sequence on the device.  a0 gets the
-// shape closure's arguments except the chunk.
+// What mvs_fit_shared_shape and mvs_debug_shape_closure share once check_seq_stream has passed: the checks of the stage, its
+// LossParams (3-D term as the call says), the offsets on the host, and the scratch with the offsets and each frame's sequence on
+// the device.  a0 gets the shape closure's arguments except the chunk.
 static int shape_prepare(mvs_ctx* ctx, const char* who, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
                          const int* rig, const mvs_loss_config* stage, int H, LossParams* lp, std::vector<int>* off,
                          ShapeArgs* a0, cudaStream_t st) {
-    if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0))
-        return set_error(ctx, MVS_ERR_INVALID, "%s: model, cameras and batch must be set first", who);
-    if (!s || !stage) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    if (!stage) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    if (stage->frozen_mask & 1u)
+        return set_error(ctx, MVS_ERR_INVALID, "%s: the stage freezes betas (fix_shape): the shape is given, there is nothing to "
+                                               "share", who);
+    if (stage->interpenetration)
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the shape closure is the frame-resident closure, which has no "
+                                                   "interpenetration (SDF) term", who);
+    int rc = make_loss_params(ctx, stage, lp);
+    if (rc) return rc;
+    lp->j3d_on = gt_xyz ? 1 : 0;
+    if (stage_regime(ctx, *lp, H, false) != kResident)
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the stage would not run in the frame-resident kernels (exec mode 1, "
+                                                   "history_size > 100, or a model they do not take)", who);
+    const int NS = s->n_sequences, F = s->seq_offsets[NS], B = ctx->ws.B;
+    off->assign(s->seq_offsets, s->seq_offsets + NS + 1);
+    SeqState& h = seq_state(ctx);
+    if ((rc = dev_grow(ctx, h.off, (size_t)NS + 1)) || (rc = dev_grow(ctx, h.ok, (size_t)NS)) ||
+        (rc = dev_grow(ctx, h.rows, ((size_t)NS + B) * kParams)) || (rc = dev_grow(ctx, h.seq_final, (size_t)B)) ||
+        (rc = dev_grow(ctx, h.seq_of, (size_t)F)) || (rc = dev_grow(ctx, h.loss, (size_t)F)) ||
+        (rc = dev_grow(ctx, h.grad, (size_t)F * kParams)))
+        return rc;
+    std::vector<int> seq_of((size_t)F);
+    for (int q = 0; q < NS; ++q)
+        for (int f = (*off)[q]; f < (*off)[q + 1]; ++f) seq_of[f] = q;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.off.p, off->data(), off->size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.seq_of.p, seq_of.data(), (size_t)F * sizeof(int), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    *a0 = ShapeArgs{};
+    a0->in = FrameInputs{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d, rig};
+    a0->params = s->params;
+    a0->off = h.off.p;
+    a0->seq_of = h.seq_of.p;
+    a0->share_scale = (stage->frozen_mask >> 4 & 1u) ? 0 : 1;
+    a0->loss = h.loss.p;
+    a0->grad = h.grad.p;
+    return MVS_OK;
+}
+
+// Refuses a call (who: the entry point called) before the context has model, cameras and batch, and the keypoints (kp) and the
+// loss config (loss) where the call reads them
+static int check_ready(mvs_ctx* ctx, const char* who, bool kp = false, bool loss = false) {
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0) || (kp && !ctx->have_kp) || (loss && !ctx->have_loss))
+        return set_error(ctx, MVS_ERR_INVALID, "%s: %s must be set first", who,
+                         loss ? "model, cameras, batch, keypoints and loss config"
+                         : kp ? "model, cameras, batch and keypoints" : "model, cameras and batch");
+    return MVS_OK;
+}
+
+// The preamble of the batch entry points: check_ready, the arguments (args_ok: none is NULL or empty) and the slots' rigs; then
+// the device and zeroed stats
+static int begin_batch_call(mvs_ctx* ctx, const char* who, bool kp, bool loss, bool args_ok, mvs_lbfgs_stats* stats) {
+    if (int rc = check_ready(ctx, who, kp, loss)) return rc;
+    if (!args_ok) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL / empty argument", who);
+    if (int rc = batch_rigs(ctx, who)) return rc;
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    if (stats) memset(stats, 0, sizeof(*stats));
+    return MVS_OK;
+}
+
+// What every stream call checks last (who: the entry point called; F frames): the anchor term off, and a rig per frame when
+// the context has several, its indices checked on the device
+static int check_stream_rigs(mvs_ctx* ctx, const char* who, const int* rig, int F, cudaStream_t st) {
+    if (ctx->anchor_enabled)
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the anchor term is per batch (sequence smoothness); switch it off "
+                                                   "(mvs_set_anchor enable = 0) to fit a stream", who);
+    if (!rig && ctx->rigs.size() > 1)
+        return set_error(ctx, MVS_ERR_INVALID, "%s: the context has %d camera rigs: give each frame's rig", who, (int)ctx->rigs.size());
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    return rig ? check_frame_rigs(ctx, who, rig, F, st) : MVS_OK;
+}
+
+// The checks of a sequence stream s and its gt_xyz, conf3d and rig (who: the entry point called)
+static int check_seq_stream(mvs_ctx* ctx, const char* who, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
+                            const int* rig, cudaStream_t st) {
+    if (int rc = check_ready(ctx, who)) return rc;
+    if (!s) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
     if (s->n_sequences < 1 || !s->seq_offsets)
         return set_error(ctx, MVS_ERR_INVALID, "%s: n_sequences must be >= 1 (got %d) with seq_offsets", who, s->n_sequences);
     if (!s->params || !s->gt_uv || !s->conf || !s->joint_weights)
@@ -1343,44 +1322,64 @@ static int shape_prepare(mvs_ctx* ctx, const char* who, const mvs_sequence_strea
         if (s->seq_offsets[k + 1] <= s->seq_offsets[k])
             return set_error(ctx, MVS_ERR_INVALID, "%s: seq_offsets must ascend strictly (sequence %d is empty or negative)", who, k);
     if (!gt_xyz != !conf3d) return set_error(ctx, MVS_ERR_INVALID, "%s: gt_xyz and conf3d go together", who);
-    if (stage->frozen_mask & 1u)
-        return set_error(ctx, MVS_ERR_INVALID, "%s: the stage freezes betas (fix_shape): the shape is given, there is nothing to "
-                                               "share", who);
-    if (stage->interpenetration)
-        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the shape closure is the frame-resident closure, which has no "
-                                                   "interpenetration (SDF) term", who);
-    if (ctx->anchor_enabled)
-        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the anchor term is per batch; switch it off (mvs_set_anchor enable = 0)", who);
-    if (!rig && ctx->rigs.size() > 1)
-        return set_error(ctx, MVS_ERR_INVALID, "%s: the context has %d camera rigs: give each frame's rig", who, (int)ctx->rigs.size());
-    int rc = make_loss_params(ctx, stage, lp);
+    return check_stream_rigs(ctx, who, rig, s->seq_offsets[s->n_sequences], st);
+}
+
+// mvs_fit, mvs_fit_seq and mvs_fit_seq_temporal (who: the entry point called): warm_host NULL: every frame is cold;
+// temporal_w_host NULL or all zero: no temporal term, and prev_dev is not read
+static int fit_batch(mvs_ctx* ctx, const char* who, float* params_dev, int n_stages, const mvs_loss_config* stage_cfgs,
+                     const mvs_lbfgs_config* opt_cfg, const unsigned char* warm_host, const float* prev_dev,
+                     const float* temporal_w_host, float* final_loss_dev, mvs_lbfgs_stats* stats, void* stream) {
+    const cudaStream_t st = (cudaStream_t)stream;
+    bool on = false;
+    int rc = begin_batch_call(ctx, who, true, false, params_dev && n_stages > 0 && stage_cfgs && opt_cfg, stats);
+    if (!rc) rc = check_temporal_weight(ctx, who, temporal_w_host, n_stages, &on);
+    if (!rc && on && !prev_dev) rc = set_error(ctx, MVS_ERR_INVALID, "%s: NULL / empty argument", who);
+    if (!rc && on) rc = temporal_slot_rows(ctx, temporal_w_host, st);
     if (rc) return rc;
-    lp->j3d_on = gt_xyz ? 1 : 0;
-    if (stage_regime(ctx, *lp, H, false) != kResident)
-        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the stage would not run in the frame-resident kernels (exec mode 1, "
-                                                   "history_size > 100, or a model they do not take)", who);
-    const int NS = s->n_sequences, F = s->seq_offsets[NS];
-    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    if (rig && (rc = check_frame_rigs(ctx, who, rig, F, st))) return rc;
-    off->assign(s->seq_offsets, s->seq_offsets + NS + 1);
-    const size_t packed = (size_t)F * (kParams + 1 + (size_t)ctx->vmax * ctx->m.K * 3 + (gt_xyz ? (size_t)ctx->m.K * 4 : 0));
-    if ((rc = ensure_shape_state(ctx, NS, F, packed))) return rc;
-    ShapeState& h = *ctx->shape;
-    std::vector<int> seq_of((size_t)F);
-    for (int q = 0; q < NS; ++q)
-        for (int f = (*off)[q]; f < (*off)[q + 1]; ++f) seq_of[f] = q;
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.off, off->data(), off->size() * sizeof(int), cudaMemcpyHostToDevice, st));
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.seq_of, seq_of.data(), (size_t)F * sizeof(int), cudaMemcpyHostToDevice, st));
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    *a0 = ShapeArgs{};
-    a0->in = FrameInputs{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d, rig};
-    a0->params = s->params;
-    a0->off = h.off;
-    a0->seq_of = h.seq_of;
-    a0->share_scale = (stage->frozen_mask >> 4 & 1u) ? 0 : 1;
-    a0->loss = h.loss;
-    a0->grad = h.grad;
-    return MVS_OK;
+    if (on)
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->ws.anchor, prev_dev, (size_t)ctx->ws.B * kParams * sizeof(float),
+                                         cudaMemcpyDeviceToDevice, st));
+    return run_fit(ctx, who, params_dev, n_stages, stage_cfgs, opt_cfg, final_loss_dev, stats, st, warm_host, on);
+}
+
+// mvs_fit_stream and mvs_fit_stream_rigs (who: the entry point called)
+static int fit_stream(mvs_ctx* ctx, const char* who, const mvs_frame_stream* s, const int* rig, int n_stages,
+                      const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = check_ready(ctx, who)) return rc;
+    if (!s || n_stages <= 0 || !stage_cfgs || !opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL / empty argument", who);
+    if (s->n_frames < 1) return set_error(ctx, MVS_ERR_INVALID, "%s: n_frames must be >= 1 (got %d)", who, s->n_frames);
+    if (!s->params || !s->gt_uv || !s->conf || !s->joint_weights)
+        return set_error(ctx, MVS_ERR_INVALID, "%s: params, gt_uv, conf and joint_weights are required", who);
+    if (s->gt_xyz && !s->conf3d) return set_error(ctx, MVS_ERR_INVALID, "%s: gt_xyz needs conf3d", who);
+    if (int rc = check_stream_rigs(ctx, who, rig, s->n_frames, st)) return rc;
+    if (stats) memset(stats, 0, sizeof(*stats));
+    return run_stream(ctx, who, s, rig, n_stages, stage_cfgs, opt_cfg, stats, st);
+}
+
+// The mvs_fit_seq_stream entry points (who: the one called)
+static int fit_seq_stream(mvs_ctx* ctx, const char* who, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
+                          const int* rig, const float* temporal_w_host, int n_stages, const mvs_loss_config* stage_cfgs,
+                          const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
+    const cudaStream_t st = (cudaStream_t)stream;
+    bool on = false;
+    if (int rc = check_seq_stream(ctx, who, s, gt_xyz, conf3d, rig, st)) return rc;
+    if (!stage_cfgs || !opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    if (n_stages <= kWarmSkip)
+        return set_error(ctx, MVS_ERR_INVALID, "%s: warm-started frames skip the first %d stages, %d given", who, kWarmSkip, n_stages);
+    if (int rc = check_temporal_weight(ctx, who, temporal_w_host, n_stages, &on)) return rc;
+    if (stats) memset(stats, 0, sizeof(*stats));
+    return run_seq_stream(ctx, who, s, gt_xyz, conf3d, rig, n_stages, stage_cfgs, opt_cfg, stats, st, on ? temporal_w_host : nullptr);
+}
+
+void release_fit_state(mvs_ctx* ctx) {
+    release(ctx->lbfgs);
+    release(ctx->fstream);
+    delete ctx->sstream;
+    ctx->lbfgs = nullptr;
+    ctx->fstream = nullptr;
+    ctx->sstream = nullptr;
 }
 
 }  // namespace mvs
@@ -1391,26 +1390,14 @@ extern "C" {
 
 int mvs_lbfgs_run(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, const mvs_lbfgs_config* cfg,
                   mvs_lbfgs_stats* stats, void* stream) {
-    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
-    if (!(ctx->have_model && ctx->have_cams && ctx->have_kp && ctx->have_loss && ctx->ws.B > 0))
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_run: model, cameras, batch, keypoints and loss config must be set first");
-    if (!params_dev || !cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_run: NULL argument");
-    if (int rc = batch_rigs(ctx, "mvs_lbfgs_run")) return rc;
-    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    if (stats) memset(stats, 0, sizeof(*stats));
+    if (int rc = begin_batch_call(ctx, "mvs_lbfgs_run", true, true, params_dev && cfg, stats)) return rc;
     return run_stage(ctx, params_dev, final_loss_dev, cfg, stats, (cudaStream_t)stream, RunOpts{});
 }
 
 int mvs_lbfgs_step(mvs_ctx* ctx, float* params_dev, float* loss_dev, float* last_grad_dev, const mvs_lbfgs_config* cfg,
                    int reset, mvs_lbfgs_stats* stats, void* stream) {
-    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
-    if (!(ctx->have_model && ctx->have_cams && ctx->have_kp && ctx->have_loss && ctx->ws.B > 0))
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_step: model, cameras, batch, keypoints and loss config must be set first");
-    if (!params_dev || !cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_step: NULL argument");
+    if (int rc = begin_batch_call(ctx, "mvs_lbfgs_step", true, true, params_dev && cfg, stats)) return rc;
     if (!reset && !ctx->lbfgs) return set_error(ctx, MVS_ERR_INVALID, "mvs_lbfgs_step: reset=0 before any step");
-    if (int rc = batch_rigs(ctx, "mvs_lbfgs_step")) return rc;
-    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    if (stats) memset(stats, 0, sizeof(*stats));
     RunOpts o;
     o.step = true;
     o.reset = reset != 0;
@@ -1418,160 +1405,88 @@ int mvs_lbfgs_step(mvs_ctx* ctx, float* params_dev, float* loss_dev, float* last
     return run_stage(ctx, params_dev, loss_dev, cfg, stats, (cudaStream_t)stream, o);
 }
 
-int mvs_fit_seq(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg,
-                const unsigned char* warm_host, float* final_loss_dev, mvs_lbfgs_stats* stats, void* stream) {
-    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
-    if (!(ctx->have_model && ctx->have_cams && ctx->have_kp && ctx->ws.B > 0))
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq: model, cameras, batch and keypoints must be set first");
-    if (!params_dev || n_stages <= 0 || !stage_cfgs || !opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq: NULL / empty argument");
-    if (int rc = batch_rigs(ctx, "mvs_fit_seq")) return rc;
-    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    if (stats) memset(stats, 0, sizeof(*stats));
-    return run_fit(ctx, params_dev, n_stages, stage_cfgs, opt_cfg, final_loss_dev, stats, (cudaStream_t)stream, warm_host);
-}
-
 int mvs_fit_seq_temporal(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_config* stage_cfgs,
                          const mvs_lbfgs_config* opt_cfg, const unsigned char* warm_host, const float* prev_dev,
                          const float* temporal_w_host, float* final_loss_dev, mvs_lbfgs_stats* stats, void* stream) {
-    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
-    bool on = false;
-    if (int rc = check_temporal_weight(ctx, "mvs_fit_seq_temporal", temporal_w_host, n_stages, &on)) return rc;
-    if (!on) return mvs_fit_seq(ctx, params_dev, n_stages, stage_cfgs, opt_cfg, warm_host, final_loss_dev, stats, stream);
-    if (!(ctx->have_model && ctx->have_cams && ctx->have_kp && ctx->ws.B > 0))
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_temporal: model, cameras, batch and keypoints must be set first");
-    if (!params_dev || !stage_cfgs || !opt_cfg || !prev_dev)
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_temporal: NULL argument");
-    if (int rc = batch_rigs(ctx, "mvs_fit_seq_temporal")) return rc;
-    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    if (stats) memset(stats, 0, sizeof(*stats));
-    const cudaStream_t st = (cudaStream_t)stream;
-    if (int rc = temporal_slot_rows(ctx, temporal_w_host, st)) return rc;
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->ws.anchor, prev_dev, (size_t)ctx->ws.B * kParams * sizeof(float), cudaMemcpyDeviceToDevice,
-                                     st));
-    return run_fit(ctx, params_dev, n_stages, stage_cfgs, opt_cfg, final_loss_dev, stats, st, warm_host, true);
+    return fit_batch(ctx, "mvs_fit_seq_temporal", params_dev, n_stages, stage_cfgs, opt_cfg, warm_host, prev_dev, temporal_w_host,
+                     final_loss_dev, stats, stream);
+}
+
+int mvs_fit_seq(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg,
+                const unsigned char* warm_host, float* final_loss_dev, mvs_lbfgs_stats* stats, void* stream) {
+    return fit_batch(ctx, "mvs_fit_seq", params_dev, n_stages, stage_cfgs, opt_cfg, warm_host, nullptr, nullptr, final_loss_dev,
+                     stats, stream);
 }
 
 int mvs_fit(mvs_ctx* ctx, float* params_dev, int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg,
             float* final_loss_dev, mvs_lbfgs_stats* stats, void* stream) {
-    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
-    if (!(ctx->have_model && ctx->have_cams && ctx->have_kp && ctx->ws.B > 0))
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit: model, cameras, batch and keypoints must be set first");
-    if (!params_dev || n_stages <= 0 || !stage_cfgs || !opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit: NULL / empty argument");
-    if (int rc = batch_rigs(ctx, "mvs_fit")) return rc;
-    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    if (stats) memset(stats, 0, sizeof(*stats));
-    return run_fit(ctx, params_dev, n_stages, stage_cfgs, opt_cfg, final_loss_dev, stats, (cudaStream_t)stream);
+    return fit_batch(ctx, "mvs_fit", params_dev, n_stages, stage_cfgs, opt_cfg, nullptr, nullptr, nullptr, final_loss_dev, stats,
+                     stream);
 }
 
 int mvs_fit_stream_rigs(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig_dev, int n_stages, const mvs_loss_config* stage_cfgs,
                         const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
-    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
-    if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0))
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: model, cameras and batch must be set first");
-    if (!s || n_stages <= 0 || !stage_cfgs || !opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: NULL / empty argument");
-    if (s->n_frames < 1) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: n_frames must be >= 1 (got %d)", s->n_frames);
-    if (!s->params || !s->gt_uv || !s->conf || !s->joint_weights)
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: params, gt_uv, conf and joint_weights are required");
-    if (s->gt_xyz && !s->conf3d) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: gt_xyz needs conf3d");
-    if (ctx->anchor_enabled)
-        return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_stream: the anchor term is per batch (sequence smoothness); switch it "
-                                                   "off (mvs_set_anchor enable = 0) to fit a frame stream");
-    if (!rig_dev && ctx->rigs.size() > 1)
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_stream: the context has %d camera rigs: give each frame's rig "
-                                               "(mvs_fit_stream_rigs)", (int)ctx->rigs.size());
-    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    if (rig_dev) {
-        if (int rc = check_frame_rigs(ctx, "mvs_fit_stream_rigs", rig_dev, s->n_frames, (cudaStream_t)stream)) return rc;
-    }
-    if (stats) memset(stats, 0, sizeof(*stats));
-    return run_stream(ctx, s, rig_dev, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream);
+    return fit_stream(ctx, "mvs_fit_stream_rigs", s, rig_dev, n_stages, stage_cfgs, opt_cfg, stats, stream);
 }
 
 int mvs_fit_stream(mvs_ctx* ctx, const mvs_frame_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
                    const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
-    return mvs_fit_stream_rigs(ctx, s, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
+    return fit_stream(ctx, "mvs_fit_stream", s, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
 }
 
 int mvs_fit_seq_stream_temporal(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
                                 const int* rig_dev, const float* temporal_w_host, int n_stages, const mvs_loss_config* stage_cfgs,
                                 const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
-    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
-    bool on = false;
-    if (int rc = check_temporal_weight(ctx, "mvs_fit_seq_stream_temporal", temporal_w_host, n_stages, &on)) return rc;
-    if (!gt_xyz != !conf3d) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream3d: gt_xyz and conf3d go together");
-    if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0))
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: model, cameras and batch must be set first");
-    if (!s || !stage_cfgs || !opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: NULL argument");
-    if (n_stages <= 2)
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: warm-started frames skip the first 2 stages, %d given", n_stages);
-    if (s->n_sequences < 1 || !s->seq_offsets)
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: n_sequences must be >= 1 (got %d) with seq_offsets", s->n_sequences);
-    if (!s->params || !s->gt_uv || !s->conf || !s->joint_weights)
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: params, gt_uv, conf and joint_weights are required");
-    if (s->seq_offsets[0] != 0) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: seq_offsets[0] must be 0");
-    for (int k = 0; k < s->n_sequences; ++k)
-        if (s->seq_offsets[k + 1] <= s->seq_offsets[k])
-            return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: seq_offsets must ascend strictly (sequence %d is empty "
-                                                   "or negative)", k);
-    if (ctx->anchor_enabled)
-        return set_error(ctx, MVS_ERR_UNSUPPORTED, "mvs_fit_seq_stream: the anchor term is per batch (sequence smoothness); switch "
-                                                   "it off (mvs_set_anchor enable = 0) to fit a sequence stream");
-    if (!rig_dev && ctx->rigs.size() > 1)
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_seq_stream: the context has %d camera rigs: give each frame's rig "
-                                               "(mvs_fit_seq_stream_rigs)", (int)ctx->rigs.size());
-    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
-    if (rig_dev) {
-        const int F = s->seq_offsets[s->n_sequences];
-        if (int rc = check_frame_rigs(ctx, "mvs_fit_seq_stream_rigs", rig_dev, F, (cudaStream_t)stream)) return rc;
-    }
-    if (stats) memset(stats, 0, sizeof(*stats));
-    return run_seq_stream(ctx, s, gt_xyz, conf3d, rig_dev, n_stages, stage_cfgs, opt_cfg, stats, (cudaStream_t)stream,
-                          on ? temporal_w_host : nullptr);
+    return fit_seq_stream(ctx, "mvs_fit_seq_stream_temporal", s, gt_xyz, conf3d, rig_dev, temporal_w_host, n_stages, stage_cfgs,
+                          opt_cfg, stats, stream);
 }
 
 int mvs_fit_seq_stream_rigs(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig_dev,
                             int n_stages, const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats,
                             void* stream) {
-    return mvs_fit_seq_stream_temporal(ctx, s, gt_xyz, conf3d, rig_dev, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
+    return fit_seq_stream(ctx, "mvs_fit_seq_stream_rigs", s, gt_xyz, conf3d, rig_dev, nullptr, n_stages, stage_cfgs, opt_cfg, stats,
+                          stream);
 }
 
 int mvs_fit_seq_stream3d(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, int n_stages,
                          const mvs_loss_config* stage_cfgs, const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
-    return mvs_fit_seq_stream_rigs(ctx, s, gt_xyz, conf3d, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
+    return fit_seq_stream(ctx, "mvs_fit_seq_stream3d", s, gt_xyz, conf3d, nullptr, nullptr, n_stages, stage_cfgs, opt_cfg, stats,
+                          stream);
 }
 
 int mvs_fit_seq_stream(mvs_ctx* ctx, const mvs_sequence_stream* s, int n_stages, const mvs_loss_config* stage_cfgs,
                        const mvs_lbfgs_config* opt_cfg, mvs_lbfgs_stats* stats, void* stream) {
-    return mvs_fit_seq_stream_rigs(ctx, s, nullptr, nullptr, nullptr, n_stages, stage_cfgs, opt_cfg, stats, stream);
+    return fit_seq_stream(ctx, "mvs_fit_seq_stream", s, nullptr, nullptr, nullptr, nullptr, n_stages, stage_cfgs, opt_cfg, stats,
+                          stream);
 }
 
 int mvs_fit_shared_shape(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig_dev,
                          const mvs_loss_config* stage, const mvs_lbfgs_config* opt_cfg, int n_sweeps, float* seq_loss_dev,
                          mvs_lbfgs_stats* shape_stats, mvs_lbfgs_stats* pose_stats, void* stream) {
     static const char* who = "mvs_fit_shared_shape";
-    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
-    if (!opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
-    if (n_sweeps < 1) return set_error(ctx, MVS_ERR_INVALID, "%s: n_sweeps must be >= 1 (got %d)", who, n_sweeps);
     const cudaStream_t st = (cudaStream_t)stream;
     LossParams lp;
     std::vector<int> off;
     ShapeArgs a0;
-    int rc = shape_prepare(ctx, who, s, gt_xyz, conf3d, rig_dev, stage, history_size(opt_cfg), &lp, &off, &a0, st);
+    int rc = check_seq_stream(ctx, who, s, gt_xyz, conf3d, rig_dev, st);
+    if (!rc && !opt_cfg) rc = set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    if (!rc && n_sweeps < 1) rc = set_error(ctx, MVS_ERR_INVALID, "%s: n_sweeps must be >= 1 (got %d)", who, n_sweeps);
+    if (!rc) rc = shape_prepare(ctx, who, s, gt_xyz, conf3d, rig_dev, stage, history_size(opt_cfg), &lp, &off, &a0, st);
     if (rc) return rc;
     if (shape_stats) memset(shape_stats, 0, sizeof(*shape_stats));
     if (pose_stats) memset(pose_stats, 0, sizeof(*pose_stats));
     const int NS = s->n_sequences, F = off[NS];
-    ShapeState& h = *ctx->shape;
+    SeqState& h = *ctx->sstream;
     mvs_loss_config pose_cfg = *stage;                                   // the pose step: the shared entries held
     pose_cfg.frozen_mask |= 1u | (a0.share_scale ? 16u : 0u);
     if (s->final_loss) MVS_CUDA_OK(ctx, cudaMemsetAsync(s->final_loss, 0xff, (size_t)F * sizeof(float), st));   // NaN: skipped
     std::vector<int> ok((size_t)NS), frames;
     for (int sweep = 0; sweep < n_sweeps && !rc; ++sweep) {
-        MVS_LAUNCH(ctx, KID_MISC, st, shape_consensus_kernel<<<NS, 32, 0, st>>>(s->params, h.off, a0.share_scale, h.rows, h.ok));
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ok.data(), h.ok, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
+        MVS_LAUNCH(ctx, KID_MISC, st, shape_consensus_kernel<<<NS, 32, 0, st>>>(s->params, h.off.p, a0.share_scale, h.rows.p, h.ok.p));
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ok.data(), h.ok.p, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
         if ((rc = shape_step(ctx, a0, off, ok, lp, opt_cfg, seq_loss_dev, shape_stats, st))) break;
-        MVS_LAUNCH(ctx, KID_MISC, st, shape_write_kernel<<<(F + 127) / 128, 128, 0, st>>>(s->params, h.seq_of, h.rows, h.ok, F,
+        MVS_LAUNCH(ctx, KID_MISC, st, shape_write_kernel<<<(F + 127) / 128, 128, 0, st>>>(s->params, h.seq_of.p, h.rows.p, h.ok.p, F,
                                                                                         a0.share_scale));
         frames.clear();
         for (int q = 0; q < NS; ++q)
@@ -1585,29 +1500,20 @@ int mvs_fit_shared_shape(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
 int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, const float* conf_host,
                  const float* joint_weights_host, int n_stages, const mvs_loss_config* stage_cfgs,
                  const mvs_lbfgs_config* opt_cfg, float* final_loss_host, mvs_lbfgs_stats* stats, void* stream) {
-    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
-    if (!(ctx->have_model && ctx->have_cams && ctx->ws.B > 0))
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_host: model, cameras and batch must be set first");
-    if (!params_host || !gt_uv_host || !conf_host || !joint_weights_host || n_stages <= 0 || !stage_cfgs || !opt_cfg)
-        return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_host: NULL / empty argument");
-    if (int rc = batch_rigs(ctx, "mvs_fit_host")) return rc;
-    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    static const char* who = "mvs_fit_host";
+    int rc = begin_batch_call(ctx, who, false, false, params_host && gt_uv_host && conf_host && joint_weights_host && n_stages > 0 &&
+                              stage_cfgs && opt_cfg, stats);
+    if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int B = ctx->ws.B;
-    int rc = mvs_set_keypoints(ctx, gt_uv_host, conf_host, joint_weights_host, 0, stream);
-    if (rc) return rc;
-    {
-        const int H = history_size(opt_cfg);
-        if (H > 128) return set_error(ctx, MVS_ERR_INVALID, "mvs_fit_host: history_size must be <= 128");
-        rc = ensure_state(ctx, H);
-        if (rc) return rc;
-    }
+    if ((rc = mvs_set_keypoints(ctx, gt_uv_host, conf_host, joint_weights_host, 0, stream))) return rc;
+    const int H = history_size(opt_cfg);
+    if (H > 128) return set_error(ctx, MVS_ERR_INVALID, "%s: history_size must be <= 128", who);
+    if ((rc = ensure_state(ctx, H))) return rc;
     LbfgsState& S = *ctx->lbfgs;
     float* x = S.x_fit;                              // [B][86] device copy of the parameters
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(x, params_host, (size_t)B * kParams * sizeof(float), cudaMemcpyHostToDevice, st));
-    if (stats) memset(stats, 0, sizeof(*stats));
-    rc = run_fit(ctx, x, n_stages, stage_cfgs, opt_cfg, S.final_fit, stats, st);
-    if (rc) return rc;
+    if ((rc = run_fit(ctx, who, x, n_stages, stage_cfgs, opt_cfg, S.final_fit, stats, st))) return rc;
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(params_host, x, (size_t)B * kParams * sizeof(float), cudaMemcpyDeviceToHost, st));
     if (final_loss_host)
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(final_loss_host, S.final_fit, (size_t)B * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -1702,19 +1608,18 @@ extern "C" int mvs_debug_shape_closure(mvs_ctx* ctx, const mvs_sequence_stream* 
                                        const int* rig_dev, const mvs_loss_config* stage, const float* rows_dev, float* loss_dev,
                                        float* grad_dev, void* stream) {
     static const char* who = "mvs_debug_shape_closure";
-    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
-    if (!rows_dev || !loss_dev || !grad_dev) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
     const cudaStream_t st = (cudaStream_t)stream;
     LossParams lp;
     std::vector<int> off;
     ShapeArgs a0;
-    int rc = shape_prepare(ctx, who, s, gt_xyz, conf3d, rig_dev, stage, 100, &lp, &off, &a0, st);
+    int rc = check_seq_stream(ctx, who, s, gt_xyz, conf3d, rig_dev, st);
+    if (!rc && (!rows_dev || !loss_dev || !grad_dev)) rc = set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    if (!rc) rc = shape_prepare(ctx, who, s, gt_xyz, conf3d, rig_dev, stage, 100, &lp, &off, &a0, st);
     if (!rc) rc = ensure_state(ctx, ctx->lbfgs ? ctx->lbfgs->H : 100);
     if (rc) return rc;
     const int NS = s->n_sequences, B = ctx->ws.B;
-    ShapeState& h = *ctx->shape;
     const std::vector<int> ok((size_t)NS, 1);
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.rows, rows_dev, (size_t)NS * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->sstream->rows.p, rows_dev, (size_t)NS * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
     for (int base = 0; base < NS && !rc; base += B) {
         const int n = std::min(B, NS - base);
         if ((rc = shape_chunk_start(ctx, base, n, ok, st))) break;

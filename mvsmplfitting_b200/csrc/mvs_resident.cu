@@ -379,7 +379,7 @@ int launch_shape_closure(mvs_ctx* ctx, const ShapeArgs& a, const LossParams& lp,
     ResidentModel rm = make_resident_model(ctx);
     rm.j3d_xyz = a.in.j3d_xyz; rm.j3d_conf = a.in.j3d_conf;           // row stride a.in.n, as gt_uv / conf
     MVS_LAUNCH(ctx, KID_RESIDENT_CLOSURE, st,
-               shape_closure_kernel<<<a.nf, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev, a.in.rig}, lp, L, a));
+               shape_closure_kernel<<<a.nf, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev.p, a.in.rig}, lp, L, a));
     MVS_LAUNCH(ctx, KID_MISC, st, shape_reduce_kernel<<<a.n, 32, 0, st>>>(L, a));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
@@ -404,7 +404,7 @@ int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, 
     ResidentModel rm = make_resident_model(ctx);
     rm.j3d_xyz = in.j3d_xyz; rm.j3d_conf = in.j3d_conf;
     MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
-               lbfgs_resident_kernel<<<in.n, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev, in.rig}, lp_tab_dev, nstages, cfg, params_dev,
+               lbfgs_resident_kernel<<<in.n, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev.p, in.rig}, lp_tab_dev, nstages, cfg, params_dev,
                                                                       in.gt_uv, in.conf, in.joint_w, in.n, H, sc_out,
                                                                       last_grad_dev, with_vposer, stage_rng_dev));
     MVS_CUDA_OK(ctx, cudaGetLastError());
@@ -427,7 +427,7 @@ int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& c
         rm.anchor_w = temporal_w;
     }
     MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
-               lbfgs_resident_seq_kernel<<<q.n_act, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev, in.rig}, lp_tab_dev, cfg,
+               lbfgs_resident_seq_kernel<<<q.n_act, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev.p, in.rig}, lp_tab_dev, cfg,
                                                                              params_dev, in.gt_uv, in.conf, in.joint_w, in.n, H,
                                                                              with_vposer, q));
     MVS_CUDA_OK(ctx, cudaGetLastError());

@@ -441,12 +441,17 @@ static int encode_map(mvs_ctx* ctx, CUtensorMap* map, const float* ptr, uint64_t
 
 // state of the tensor path (called from mvs_set_model once the Qk rows are on the device: the kernel reads them directly)
 int tc_upload_model(mvs_ctx* ctx) {
-    TcState* T = new TcState();
-    ctx->tc = T;
-    int rc;
-    if ((rc = dev_alloc(ctx, &T->err, 1))) return rc;
-    MVS_CUDA_OK(ctx, cudaMemset(T->err, 0, sizeof(int)));
+    int* err = nullptr;
+    if (int rc = dev_alloc(ctx, &err, 1)) return rc;
+    MVS_CUDA_OK(ctx, cudaMemset(err, 0, sizeof(int)));
+    ctx->tc = new TcState();
+    ctx->tc->err = err;
     return MVS_OK;
+}
+
+void release_tc_state(mvs_ctx* ctx) {
+    delete ctx->tc;
+    ctx->tc = nullptr;
 }
 
 // kernel attributes and the tensor maps over the model's Qk rows and the batch's PhiTc

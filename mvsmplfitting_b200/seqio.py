@@ -575,11 +575,10 @@ def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, r
     kw = {} if rig is None else dict(rig=rig)
     if tw is not None:
         kw["temporal_weight"] = tw
-    if t3 is None:
-        final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss, **kw)
-    else:
-        final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss,
-                                          joints3d=t3[0], conf3d=t3[1], **kw)
+    if t3 is not None:
+        kw.update(joints3d=t3[0], conf3d=t3[1])
+    final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss, **kw)
+    if t3 is not None:
         ctx.set_joints3d(None)
     if shared_shape:
         final = share_shape(ctx, params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, shared_shape, t3, rig, stats)
