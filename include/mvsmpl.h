@@ -389,6 +389,35 @@ int mvs_fit_shared_shape(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
                          int n_sweeps, float* seq_loss_dev, mvs_lbfgs_stats* shape_stats,
                          mvs_lbfgs_stats* pose_stats, void* stream);
 
+/* ---- refine the camera rigs' extrinsics from fitted bodies (NOT in the reference, whose calibration is fixed): for the frames
+ *      of s and the one stage configuration `stage` (normally the schedule's last), minimises  sum_f L(x_f; cameras of rig(f))
+ *      (L = what mvs_closure returns for row x_f under `stage`) by block-coordinate descent, n_sweeps >= 1 times:
+ *        held keypoints: each frame's keypoints (the points the 2-D term projects) from its row;
+ *        camera step: one L-BFGS problem per view v >= 1 of every rig r with frames in the call (the 86-vector state machine of
+ *          mvs_fit's frames, with run_fitting's NaN / ftol / gtol rules and opt_cfg), the context's B at a time.  Its loss is
+ *          view v's 2-D data term of mvs_closure, summed over the frames with rig r at their held keypoints (in double, in
+ *          call order).  Variables: a rotation update w and a camera-centre update, R = Rod(w) R0 and
+ *          x_cam = Rod(w) (R0 (q - dC) + t0), exactly (R0, t0) at 0.  View 0 is held; view 1 keeps its distance to view 0
+ *          (its centre moves on that sphere: 2 centre variables); views 2 .. V_r - 1 have 3.  The solved cameras replace the
+ *          calibrated ones in the context's rig table;
+ *        body step: every frame runs `stage` from its row against the refined table: exactly mvs_fit_stream_rigs's bits.
+ *      A frame whose row is not all finite takes no part: its row is kept and its final loss is NaN.  Intrinsics, distortion and
+ *      the data-weight scales are not refined; a view without a confident detection in the call and a rig of one view keep
+ *      their cameras bit for bit.
+ *      s->params [F,86] holds the fitted rows on entry and the result on exit; s->final_loss [F] (may be NULL) receives each
+ *      frame's body-step result of the last sweep; s->gt_xyz / conf3d switch the 3-D term of the body step on.  rig_dev as in
+ *      mvs_fit_stream_rigs.  R_host [n_rigs,Vmax,3,3] and t_host [n_rigs,Vmax,3] (HOST, each may be NULL) receive the refined
+ *      table (rows v >= V_r are zero).  camera_stats counts the view problems' iterations and evaluations, pose_stats what
+ *      mvs_fit_stream reports (both summed over the sweeps).  SDF stages are taken (the body step runs them as mvs_fit_stream).
+ *      Refused: MVS_ERR_INVALID for NULL or empty arguments, n_sweeps < 1, exactly one of gt_xyz / conf3d, several rigs
+ *      without rig_dev and a rig index out of range (checked on the device); MVS_ERR_UNSUPPORTED for the anchor term, exec
+ *      mode 1, history_size > 100 and what mvs_fit_stream refuses.  Nothing is changed by a refused call.
+ *      Context state afterwards as after mvs_fit_stream (no keypoints, 3-D term off, no per-slot rigs), and the rig table
+ *      holds the refined extrinsics (f, c and the scales unchanged).  Synchronises. */
+int mvs_refine_cameras(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig_dev, const mvs_loss_config* stage,
+                       const mvs_lbfgs_config* opt_cfg, int n_sweeps, float* R_host, float* t_host,
+                       mvs_lbfgs_stats* camera_stats, mvs_lbfgs_stats* pose_stats, void* stream);
+
 /* ---- host-buffer entry point (what a caller without device memory uses): copies keypoints and
  *      parameters host->device, runs `n_stages` optimisation stages (one mvs_loss_config each, the weight
  *      schedule of code/utils/non_linear_solver.py:109-203), copies parameters and losses back.

@@ -78,7 +78,7 @@ EXPORTS = (
     "mvs_closure", "mvs_forward", "mvs_lbfgs_run", "mvs_lbfgs_step", "mvs_fit", "mvs_fit_seq", "mvs_fit_stream", "mvs_fit_seq_stream", "mvs_fit_seq_stream3d",
     "mvs_fit_stream_rigs", "mvs_fit_seq_stream_rigs", "mvs_fit_host", "mvs_sdf_grid", "mvs_profile", "mvs_profile_read",
     "mvs_kernel_name", "mvs_set_exec_mode", "mvs_set_anchor", "mvs_set_joints3d", "mvs_init_guess", "mvs_fit_seq_temporal",
-    "mvs_fit_seq_stream_temporal", "mvs_fit_shared_shape",
+    "mvs_fit_seq_stream_temporal", "mvs_fit_shared_shape", "mvs_refine_cameras",
 )
 NUM_KERNEL_IDS = 19
 
@@ -141,6 +141,8 @@ def load() -> ctypes.CDLL:
     lib.mvs_fit_shared_shape.argtypes = [vp, ctypes.POINTER(SequenceStream), vp, vp, vp, ctypes.POINTER(LossConfig),
                                          ctypes.POINTER(LbfgsConfig), ci, vp, ctypes.POINTER(LbfgsStats), ctypes.POINTER(LbfgsStats),
                                          vp]
+    lib.mvs_refine_cameras.argtypes = [vp, ctypes.POINTER(FrameStream), vp, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig),
+                                       ci, vp, vp, ctypes.POINTER(LbfgsStats), ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_fit_host.argtypes = [vp, vp, vp, vp, vp, ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig), vp,
                                  ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_sdf_grid.argtypes = [vp, vp, vp, ci, vp, ci, ci, ci, vp]

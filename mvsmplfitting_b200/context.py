@@ -65,6 +65,7 @@ class FittingContext:
         self.N = 0
         self._loss_cfg = None
         self._j3d_keep = None             # the 3-D targets while the term is on (set_joints3d)
+        self._rigs = []                   # the camera table as set: dict(R, t, f, c) float32 per rig (refine_cameras updates R, t)
 
     def close(self):
         if getattr(self, "h", None):
@@ -144,6 +145,7 @@ class FittingContext:
         self.V = R.shape[0]
         _lib.check(self.h, self.lib.mvs_set_cameras(self.h, self.V, _ptr(R), _ptr(t), _ptr(f), _ptr(c)), "mvs_set_cameras")
         self.rig_views = [self.V]
+        self._rigs = [dict(R=R.copy(), t=t.copy(), f=f.copy(), c=c.copy())]
 
     def set_camera_rigs(self, rigs, data_weight_scale=None):
         """A table of camera rigs (mvs_set_camera_rigs): rigs is a list of dict(R [V_r,3,3], t [V_r,3], f [V_r,2], c [V_r,2])
@@ -166,6 +168,7 @@ class FittingContext:
         _lib.check(self.h, self.lib.mvs_set_camera_rigs(self.h, len(rigs), _ptr(nva), _ptr(R), _ptr(t), _ptr(f), _ptr(c),
                                                         _ptr(scale)), "mvs_set_camera_rigs")
         self.V, self.rig_views = V, nv
+        self._rigs = [dict(R=R[r, :n].copy(), t=t[r, :n].copy(), f=f[r, :n].copy(), c=c[r, :n].copy()) for r, n in enumerate(nv)]
 
     def set_frame_rigs(self, rig):
         """the rig of every slot of the batch (mvs_set_frame_rigs): rig [B] ints in [0, n_rigs)"""
@@ -418,6 +421,37 @@ class FittingContext:
                                                          ctypes.byref(cfg), int(sweeps), _ptr(seq_loss), ctypes.byref(sh),
                                                          ctypes.byref(po), self._stream()), "mvs_fit_shared_shape")
         return final, seq_loss, _stats_dict(sh), _stats_dict(po)
+
+    def refine_cameras(self, params: torch.Tensor, gt_uv, conf, joint_weights, stage_cfg, opt_cfg=None, sweeps=1, joints3d=None,
+                       conf3d=None, rig=None):
+        """Refine every rig's extrinsics from fitted bodies (mvs_refine_cameras): `sweeps` rounds of: each view v >= 1 of every rig
+        fitted to the keypoints of the frames with that rig, held from their rows (view 0 fixed, view 1 at its distance to
+        view 0); then every frame refits stage_cfg from its row against the refined cameras.  params [F,86] CUDA float32, fitted
+        rows in, result out; gt_uv [V,F,K,2], conf [V,F,K], joint_weights [K], joints3d / conf3d and rig as in fit_stream.  The
+        context keeps the refined cameras; afterwards it holds no keypoints, no 3-D targets and no per-slot rigs.  Returns
+        (final_loss [F], rigs, camera_stats, pose_stats), rigs: the refined table as the list of dict(R, t, f, c) that
+        set_camera_rigs takes (same views per rig, f and c unchanged)."""
+        assert params.is_cuda and params.dtype == torch.float32 and params.is_contiguous() and params.dim() == 2
+        F = params.shape[0]
+        if isinstance(sweeps, bool) or int(sweeps) != sweeps or sweeps < 1:
+            raise ValueError("refine_cameras: want sweeps >= 1, got %r" % (sweeps,))
+        gt_uv, conf, jw, j3, c3 = self._stream_rows("refine_cameras", F, gt_uv, conf, joint_weights, joints3d, conf3d)
+        rg = self._stream_rigs("refine_cameras", F, rig)
+        final = torch.empty(F, dtype=torch.float32, device=self.device)
+        s = _lib.FrameStream(F, _ptr(params), _ptr(gt_uv), _ptr(conf), _ptr(jw), _ptr(j3), _ptr(c3), _ptr(final))
+        cfg = opt_cfg or self.make_lbfgs_config()
+        n = len(self.rig_views)
+        R = np.zeros((n, self.V, 3, 3), np.float32)
+        t = np.zeros((n, self.V, 3), np.float32)
+        ca, po = _lib.LbfgsStats(), _lib.LbfgsStats()
+        self._j3d_keep = None
+        _lib.check(self.h, self.lib.mvs_refine_cameras(self.h, ctypes.byref(s), _ptr(rg), ctypes.byref(stage_cfg), ctypes.byref(cfg),
+                                                       int(sweeps), _ptr(R), _ptr(t), ctypes.byref(ca), ctypes.byref(po),
+                                                       self._stream()), "mvs_refine_cameras")
+        for r, nv in enumerate(self.rig_views):
+            self._rigs[r] = dict(self._rigs[r], R=R[r, :nv].copy(), t=t[r, :nv].copy())
+        rigs = [{k: v.copy() for k, v in d.items()} for d in self._rigs]
+        return final, rigs, _stats_dict(ca), _stats_dict(po)
 
     def fit_host(self, params_host: np.ndarray, gt_uv: np.ndarray, conf: np.ndarray, joint_weights: np.ndarray,
                  stage_cfgs, opt_cfg=None):

@@ -53,6 +53,8 @@ template int dev_alloc<FrameBox>(mvs_ctx*, FrameBox**, size_t);
 template int dev_alloc<SdfFrameSetup>(mvs_ctx*, SdfFrameSetup**, size_t);
 template int dev_alloc<long long>(mvs_ctx*, long long**, size_t);
 template int dev_alloc<Rig>(mvs_ctx*, Rig**, size_t);
+template int dev_alloc<CamRefine>(mvs_ctx*, CamRefine**, size_t);
+template int dev_alloc<CameraProblem>(mvs_ctx*, CameraProblem**, size_t);
 template int dev_alloc<LossParams>(mvs_ctx*, LossParams**, size_t);
 template int dev_alloc<FrameScalars>(mvs_ctx*, FrameScalars**, size_t);
 template int dev_upload<float>(mvs_ctx*, float**, const float*, size_t);

@@ -140,7 +140,7 @@ struct LbfgsCfg;
 struct FrameScalars;
 struct TcState;
 struct StreamState;                   // mvs_fit_stream scratch (mvs_lbfgs.cu)
-struct SeqState;                      // mvs_fit_seq_stream and mvs_fit_shared_shape scratch (mvs_lbfgs.cu)
+struct SeqState;                      // mvs_fit_seq_stream, mvs_fit_shared_shape and mvs_refine_cameras scratch (mvs_lbfgs.cu)
 
 // A device array of the context that only grows (dev_grow): cap elements at p
 template <class T> struct DevBuf {
@@ -168,6 +168,30 @@ struct ShapeArgs {
     int share_scale;                  // 1: scale (entry 85) is shared, 0: it stays per frame
     float* loss;                      // [F] per-frame scratch
     float* grad;                      // [F][86]
+};
+
+// One view problem of mvs_refine_cameras: view `view` of rig `rig`, whose frames are frames[fbeg .. fbeg + nf) of the call's
+// rig-grouped frame list (the frames with that rig and a finite row, in call order) and whose closure work items (one warp
+// per frame) are item0 .. item0 + nf - 1
+struct CameraProblem {
+    int rig, view, fbeg, nf, item0;
+};
+
+// The camera step of mvs_refine_cameras (DESIGN.md section 4): view problems base .. base + n - 1 in the optimiser's slots
+// 0 .. n - 1, whose work items are i0 .. i0 + ni - 1.  A problem's variables are the entries kOffOrient .. +2 (rotation
+// update) and kOffTransl .. +2 (centre update) of its slot's row; its closure is the 2-D data term of its view over its frames
+// at the held keypoints q.
+struct CameraArgs {
+    FrameInputs in;                   // the call's frames (in.n = F: the row stride of gt_uv / conf)
+    const float* q;                   // [F][K][3] held keypoints (with translation)
+    const CamRefine* cr;              // [P] each problem's calibrated camera and centre map
+    const CameraProblem* prob;        // [P]
+    const int* frames;                // the rig-grouped frame list
+    const int* item_prob;             // [items] problem of each work item
+    const Rig* rigs;                  // the context's rig table (intrinsics and data-weight scale)
+    int K;
+    int base, n, i0, ni;
+    float* part;                      // [items][8] per work item: loss, rotation gradient [3], centre gradient [3]
 };
 
 // The chaining run of mvs_fit_seq_stream (DESIGN.md section 4): a finished frame hands its slot (a CTA of the frame-resident
@@ -323,7 +347,7 @@ struct mvs_ctx {
     float rest_scale = -1.f;
     int2* stage_rng = nullptr;       // [B] per-frame slice of the stage table (mvs_fit_seq), device
     mvs::StreamState* fstream = nullptr;  // frame-stream scratch (mvs_fit_stream), created on first use
-    mvs::SeqState* sstream = nullptr;     // sequence-stream and shared-shape scratch, created on first use
+    mvs::SeqState* sstream = nullptr;     // sequence-stream, shared-shape and camera-refinement scratch, created on first use
 };
 
 namespace mvs {
@@ -444,6 +468,17 @@ int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& c
 // the shape closure of mvs_fit_shared_shape: per frame (shape_closure_kernel), then per sequence (shape_reduce_kernel) into
 // L.loss_eval / L.g_eval of the chunk's slots; slots whose problem is done are skipped
 int launch_shape_closure(mvs_ctx* ctx, const ShapeArgs& a, const LossParams& lp, const LbfgsState& L, cudaStream_t st);
+// mvs_refine_cameras (mvs_resident.cu): the keypoints q [F][K][3] (with translation) of frames[0 .. n), the rows of params [F][86],
+// from resident_closure's joints output under lp (in: the call's frames, for the rigs)
+int launch_camera_joints(mvs_ctx* ctx, const FrameInputs& in, const float* params, const int* frames, int n, const LossParams& lp,
+                         float* q, cudaStream_t st);
+// mvs_camera.cu: the camera closure of one chunk of view problems, per work item (camera_closure_kernel) and per problem
+// (camera_reduce_kernel) into L.loss_eval / L.g_eval of the chunk's slots; slots whose problem is done are skipped
+int launch_camera_closure(mvs_ctx* ctx, const CameraArgs& a, const LossParams& lp, const LbfgsState& L, cudaStream_t st);
+// mvs_camera.cu: the cameras of problems 0 .. P-1 at their rows x [P][86] into the device rig table
+int launch_camera_write(mvs_ctx* ctx, const CamRefine* cr, const CameraProblem* prob, int P, const float* x, cudaStream_t st);
+// mvs_camera.cu: fin[f] = 1 iff row f of params [F][86] is all finite
+int launch_row_finite(mvs_ctx* ctx, const float* params, int F, int* fin, cudaStream_t st);
 // dense regime (SDF term): per round  posedirs_gemm_tc -> skin -> sdf_setup -> sdf_fused -> frame_step (skin_small in place of
 // skin at <= 8 frames; at <= 4 frames skin_small computes the set-ups itself and sdf_setup is not launched)
 int launch_frame_fwd(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);                      // mvs_closure.cu

@@ -898,6 +898,13 @@ struct SeqState {
                                         // the slots a last chunk leaves empty)
     DevBuf<float> seq_final;            // [B] run_fitting's value of each slot's problem
     DevBuf<float> loss, grad;           // [F], [F][86] the shape closure's per-frame terms
+    // camera refinement (rows and seq_final above serve its view problems)
+    DevBuf<int> fin, body;              // [F] the row is all finite, [n] the frames with a finite row (ascending)
+    DevBuf<float> held;                 // [F][K][3] held keypoints
+    DevBuf<int> cam_frames, item_prob;  // the rig-grouped frame list, the problem of each work item
+    DevBuf<CameraProblem> prob;         // [P]
+    DevBuf<CamRefine> cr;               // [P]
+    DevBuf<float> part;                 // [items][8] the camera closure's per-frame terms
 };
 
 static SeqState& seq_state(mvs_ctx* ctx) {
@@ -1373,6 +1380,218 @@ static int fit_seq_stream(mvs_ctx* ctx, const char* who, const mvs_sequence_stre
     return run_seq_stream(ctx, who, s, gt_xyz, conf3d, rig, n_stages, stage_cfgs, opt_cfg, stats, st, on ? temporal_w_host : nullptr);
 }
 
+// The view problems of a mvs_refine_cameras call: the frames with a finite row, ascending (body), grouped by rig in call
+// order (frames), and one problem per view 1 .. V_r - 1 of every rig with such frames
+struct CameraPlan {
+    std::vector<int> body, frames;
+    std::vector<CameraProblem> prob;
+    int items = 0;
+};
+
+// What mvs_refine_cameras and mvs_debug_camera_closure check before anything changes (who: the entry point called), and the
+// stage's LossParams (3-D term as the call says)
+static int camera_check(mvs_ctx* ctx, const char* who, const mvs_frame_stream* s, const int* rig, const mvs_loss_config* stage,
+                        int H, LossParams* lp, cudaStream_t st) {
+    if (int rc = check_ready(ctx, who)) return rc;
+    if (!s || !stage) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    if (s->n_frames < 1) return set_error(ctx, MVS_ERR_INVALID, "%s: n_frames must be >= 1 (got %d)", who, s->n_frames);
+    if (!s->params || !s->gt_uv || !s->conf || !s->joint_weights)
+        return set_error(ctx, MVS_ERR_INVALID, "%s: params, gt_uv, conf and joint_weights are required", who);
+    if (!s->gt_xyz != !s->conf3d) return set_error(ctx, MVS_ERR_INVALID, "%s: gt_xyz and conf3d go together", who);
+    if (ctx->exec_mode == 1 || H > 100 || !resident_supported(ctx))
+        return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the held keypoints come from the frame-resident closure, and the body step "
+                                                   "is a frame stream (exec mode 1, history_size > 100, or a model the "
+                                                   "frame-resident kernels do not take)", who);
+    std::vector<LossParams> lps;
+    std::vector<int> ends;
+    int rc = stage_table(ctx, who, 1, stage, s->gt_xyz ? 1 : 0, &lps);
+    if (!rc) rc = stream_runs(ctx, who, lps, H, kMaxStages, &ends);
+    if (!rc) rc = check_stream_rigs(ctx, who, rig, s->n_frames, st);
+    if (rc) return rc;
+    *lp = lps[0];
+    return MVS_OK;
+}
+
+// The call's plan (finite rows and rigs read back once) and its scratch on the device
+static int camera_plan(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig, CameraPlan* plan, cudaStream_t st) {
+    const int F = s->n_frames, B = ctx->ws.B, nr = (int)ctx->rigs.size();
+    SeqState& h = seq_state(ctx);
+    int rc;
+    if ((rc = dev_grow(ctx, h.fin, (size_t)F)) || (rc = launch_row_finite(ctx, s->params, F, h.fin.p, st))) return rc;
+    std::vector<int> fin((size_t)F), rg((size_t)F, 0);
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(fin.data(), h.fin.p, (size_t)F * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (rig) MVS_CUDA_OK(ctx, cudaMemcpyAsync(rg.data(), rig, (size_t)F * sizeof(int), cudaMemcpyDeviceToHost, st));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    *plan = CameraPlan{};
+    std::vector<std::vector<int>> of((size_t)nr);
+    for (int f = 0; f < F; ++f)
+        if (fin[f]) { plan->body.push_back(f); of[rg[f]].push_back(f); }
+    std::vector<int> item_prob;
+    for (int r = 0; r < nr; ++r) {
+        const int fbeg = (int)plan->frames.size(), nf = (int)of[r].size();
+        plan->frames.insert(plan->frames.end(), of[r].begin(), of[r].end());
+        if (nf == 0) continue;
+        for (int v = 1; v < ctx->rigs[r].num_views; ++v) {
+            plan->prob.push_back(CameraProblem{r, v, fbeg, nf, plan->items});
+            item_prob.insert(item_prob.end(), (size_t)nf, (int)plan->prob.size() - 1);
+            plan->items += nf;
+        }
+    }
+    const size_t P = plan->prob.size(), n = plan->body.size();
+    if ((rc = dev_grow(ctx, h.body, std::max<size_t>(n, 1))) || (rc = dev_grow(ctx, h.held, (size_t)F * ctx->m.K * 3)) ||
+        (rc = dev_grow(ctx, h.cam_frames, std::max<size_t>(n, 1))) ||
+        (rc = dev_grow(ctx, h.item_prob, std::max<size_t>(plan->items, 1))) || (rc = dev_grow(ctx, h.prob, std::max<size_t>(P, 1))) ||
+        (rc = dev_grow(ctx, h.cr, std::max<size_t>(P, 1))) || (rc = dev_grow(ctx, h.part, (size_t)std::max(plan->items, 1) * 8)) ||
+        (rc = dev_grow(ctx, h.rows, (P + B) * kParams)) || (rc = dev_grow(ctx, h.seq_final, (size_t)B)))
+        return rc;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.body.p, plan->body.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.cam_frames.p, plan->frames.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.item_prob.p, item_prob.data(), item_prob.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.prob.p, plan->prob.data(), P * sizeof(CameraProblem), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    return MVS_OK;
+}
+
+// Each problem's calibrated camera, from the context's rig table as it stands (host copy): view 1 moves on the sphere about view
+// 0's centre through its own centre, with a basis computed in double
+static int camera_refs(mvs_ctx* ctx, const CameraPlan& plan, cudaStream_t st) {
+    std::vector<CamRefine> cr(plan.prob.size());
+    auto centre = [](const CamF& c, double* C) {                   // -R^T t
+        for (int i = 0; i < 3; ++i) C[i] = -((double)c.R[i] * c.t[0] + (double)c.R[3 + i] * c.t[1] + (double)c.R[6 + i] * c.t[2]);
+    };
+    for (size_t p = 0; p < cr.size(); ++p) {
+        const Rig& rg = ctx->rigs[plan.prob[p].rig];
+        const CamF& cam = rg.cam[plan.prob[p].view];
+        CamRefine& c = cr[p];
+        memset(&c, 0, sizeof(c));
+        memcpy(c.R0, cam.R, sizeof(c.R0));
+        memcpy(c.t0, cam.t, sizeof(c.t0));
+        if (plan.prob[p].view != 1) continue;
+        c.sphere = 1;
+        double C0[3], C1[3], d[3], r = 0.0;
+        centre(rg.cam[0], C0);
+        centre(cam, C1);
+        for (int i = 0; i < 3; ++i) { d[i] = C1[i] - C0[i]; r += d[i] * d[i]; }
+        r = sqrt(r);
+        if (!(r > 0.0)) continue;                                  // coincident centres: view 1 only rotates
+        for (int i = 0; i < 3; ++i) d[i] /= r;
+        const int k = fabs(d[0]) <= fabs(d[1]) && fabs(d[0]) <= fabs(d[2]) ? 0 : fabs(d[1]) <= fabs(d[2]) ? 1 : 2;
+        double a[3] = {0.0, 0.0, 0.0}, e1[3], e2[3];
+        a[k] = 1.0;                                                // the axis least aligned with d
+        e1[0] = d[1] * a[2] - d[2] * a[1]; e1[1] = d[2] * a[0] - d[0] * a[2]; e1[2] = d[0] * a[1] - d[1] * a[0];
+        const double l = sqrt(e1[0] * e1[0] + e1[1] * e1[1] + e1[2] * e1[2]);
+        for (int i = 0; i < 3; ++i) e1[i] /= l;
+        e2[0] = d[1] * e1[2] - d[2] * e1[1]; e2[1] = d[2] * e1[0] - d[0] * e1[2]; e2[2] = d[0] * e1[1] - d[1] * e1[0];
+        for (int i = 0; i < 3; ++i) {
+            c.E[2 * i] = (float)(r * e1[i]);
+            c.E[2 * i + 1] = (float)(r * e2[i]);
+            c.n[i] = (float)(r * d[i]);
+        }
+    }
+    if (!cr.empty())
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->sstream->cr.p, cr.data(), cr.size() * sizeof(CamRefine), cudaMemcpyHostToDevice, st));
+    return MVS_OK;
+}
+
+// The camera closure's arguments for problems base .. base + n - 1
+static CameraArgs camera_chunk_args(const CameraArgs& a0, const CameraPlan& plan, int base, int n) {
+    CameraArgs a = a0;
+    a.base = base; a.n = n;
+    a.i0 = plan.prob[base].item0;
+    a.ni = plan.prob[base + n - 1].item0 + plan.prob[base + n - 1].nf - a.i0;
+    return a;
+}
+
+static CameraArgs camera_args(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig) {
+    SeqState& h = *ctx->sstream;
+    CameraArgs a{};
+    a.in = FrameInputs{s->n_frames, s->gt_uv, s->conf, s->joint_weights, nullptr, nullptr, rig};
+    a.q = h.held.p; a.cr = h.cr.p; a.prob = h.prob.p; a.frames = h.cam_frames.p; a.item_prob = h.item_prob.p;
+    a.rigs = ctx->rigs_dev.p; a.K = ctx->m.K; a.part = h.part.p;
+    return a;
+}
+
+// The camera step: every view problem from 0, the context's B at a time, run as run_fitting runs a frame's stage (the batched
+// chain's lbfgs_init / advance / compact with the camera closure); then the solved cameras into the table and its host copy
+static int camera_step(mvs_ctx* ctx, const CameraArgs& a0, const CameraPlan& plan, const LossParams& lp, const mvs_lbfgs_config* c,
+                       mvs_lbfgs_stats* stats, cudaStream_t st) {
+    const int P = (int)plan.prob.size(), B = ctx->ws.B;
+    if (P == 0) return MVS_OK;
+    SeqState& h = *ctx->sstream;
+    MVS_CUDA_OK(ctx, cudaMemsetAsync(h.rows.p, 0, (size_t)P * kParams * sizeof(float), st));
+    const std::vector<int> ok((size_t)P, 1);
+    for (int base = 0; base < P; base += B) {
+        const int n = std::min(B, P - base);
+        LbfgsCfg cfg;
+        int rc = begin_run(ctx, c, false, &lp, 1, &cfg, st);
+        if (!rc) rc = shape_chunk_start(ctx, base, n, ok, st);
+        if (rc) return rc;
+        const LbfgsState S = *ctx->lbfgs;
+        const CameraArgs a = camera_chunk_args(a0, plan, base, n);
+        const std::function<int()> closure = [&]() { return launch_camera_closure(ctx, a, lp, S, st); };
+        if ((rc = run_batched(ctx, h.rows.p + (size_t)base * kParams, cfg, false, st, closure))) return rc;
+        if ((rc = end_run(ctx, kBatched, h.seq_final.p, nullptr, stats, st))) return rc;
+    }
+    if (int rc = launch_camera_write(ctx, h.cr.p, h.prob.p, P, h.rows.p, st)) return rc;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->rigs.data(), ctx->rigs_dev.p, ctx->rigs.size() * sizeof(Rig), cudaMemcpyDeviceToHost, st));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    return MVS_OK;
+}
+
+// The body step: the frames with a finite row as one frame stream of their packed rows through run_stream under the stage,
+// against the refined table; their rows and final losses go back to the call's arrays
+static int camera_body_step(mvs_ctx* ctx, const char* who, const mvs_frame_stream* s, const int* rig, const CameraPlan& plan,
+                            const mvs_loss_config* stage, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats, cudaStream_t st) {
+    if (plan.body.empty()) return MVS_OK;
+    const int off[2] = {0, s->n_frames};
+    const mvs_sequence_stream ss{1, off, s->params, s->gt_uv, s->conf, s->joint_weights, s->final_loss, 0.f};
+    mvs_frame_stream fs;
+    const int* prig;
+    int rc = gather_frames(ctx, &ss, s->gt_xyz, s->conf3d, rig, plan.body, true, &fs, &prig, st);
+    if (!rc) rc = run_stream(ctx, who, &fs, prig, 1, stage, c, stats, st);
+    if (rc) return rc;
+    scatter_frames(ctx, &ss, fs, st);
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    return MVS_OK;
+}
+
+// mvs_refine_cameras (DESIGN.md section 4)
+static int refine_cameras(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig, const mvs_loss_config* stage,
+                          const mvs_lbfgs_config* opt_cfg, int n_sweeps, float* R_host, float* t_host, mvs_lbfgs_stats* camera_stats,
+                          mvs_lbfgs_stats* pose_stats, cudaStream_t st) {
+    static const char* who = "mvs_refine_cameras";
+    LossParams lp;
+    int rc = check_ready(ctx, who);
+    if (!rc && !opt_cfg) rc = set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    if (!rc && n_sweeps < 1) rc = set_error(ctx, MVS_ERR_INVALID, "%s: n_sweeps must be >= 1 (got %d)", who, n_sweeps);
+    if (!rc) rc = camera_check(ctx, who, s, rig, stage, history_size(opt_cfg), &lp, st);
+    if (rc) return rc;
+    if (camera_stats) memset(camera_stats, 0, sizeof(*camera_stats));
+    if (pose_stats) memset(pose_stats, 0, sizeof(*pose_stats));
+    CameraPlan plan;
+    if ((rc = camera_plan(ctx, s, rig, &plan, st))) return rc;
+    const CameraArgs a0 = camera_args(ctx, s, rig);
+    const FrameInputs in = a0.in;
+    stream_call_begin(ctx);
+    if (s->final_loss) MVS_CUDA_OK(ctx, cudaMemsetAsync(s->final_loss, 0xff, (size_t)s->n_frames * sizeof(float), st));   // NaN
+    for (int sweep = 0; sweep < n_sweeps && !rc; ++sweep) {
+        if ((rc = launch_camera_joints(ctx, in, s->params, ctx->sstream->body.p, (int)plan.body.size(), lp, ctx->sstream->held.p, st)) ||
+            (rc = camera_refs(ctx, plan, st)) || (rc = camera_step(ctx, a0, plan, lp, opt_cfg, camera_stats, st)))
+            break;
+        rc = camera_body_step(ctx, who, s, rig, plan, stage, opt_cfg, pose_stats, st);
+    }
+    stream_call_end(ctx, lp);
+    if (rc) return rc;
+    const int V = ctx->vmax;
+    for (size_t r = 0; r < ctx->rigs.size(); ++r)
+        for (int v = 0; v < V; ++v) {
+            if (R_host) memcpy(R_host + (r * V + v) * 9, ctx->rigs[r].cam[v].R, 9 * sizeof(float));
+            if (t_host) memcpy(t_host + (r * V + v) * 3, ctx->rigs[r].cam[v].t, 3 * sizeof(float));
+        }
+    return MVS_OK;
+}
+
 void release_fit_state(mvs_ctx* ctx) {
     release(ctx->lbfgs);
     release(ctx->fstream);
@@ -1495,6 +1714,12 @@ int mvs_fit_shared_shape(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
         rc = shape_pose_step(ctx, s, gt_xyz, conf3d, rig_dev, frames, pose_cfg, opt_cfg, pose_stats, st);
     }
     return rc;
+}
+
+int mvs_refine_cameras(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig_dev, const mvs_loss_config* stage,
+                       const mvs_lbfgs_config* opt_cfg, int n_sweeps, float* R_host, float* t_host, mvs_lbfgs_stats* camera_stats,
+                       mvs_lbfgs_stats* pose_stats, void* stream) {
+    return refine_cameras(ctx, s, rig_dev, stage, opt_cfg, n_sweeps, R_host, t_host, camera_stats, pose_stats, (cudaStream_t)stream);
 }
 
 int mvs_fit_host(mvs_ctx* ctx, float* params_host, const float* gt_uv_host, const float* conf_host,
@@ -1625,6 +1850,50 @@ extern "C" int mvs_debug_shape_closure(mvs_ctx* ctx, const mvs_sequence_stream* 
         if ((rc = shape_chunk_start(ctx, base, n, ok, st))) break;
         const LbfgsState& S = *ctx->lbfgs;
         if ((rc = launch_shape_closure(ctx, shape_chunk_args(a0, off, base, n), lp, S, st))) break;
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(loss_dev + base, S.loss_eval, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(grad_dev + (size_t)base * kParams, S.g_eval, (size_t)n * kParams * sizeof(float),
+                                         cudaMemcpyDeviceToDevice, st));
+    }
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(ctx->ws.fidx, B, ctx->ws.na));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    return rc;
+}
+
+// mvs_debug_camera_closure (tests/test_gpu_camera_refine.py): the camera closure of mvs_refine_cameras evaluated once, with the
+// same arguments, the context's rig table as the calibration and the keypoints of s->params held.  *n_prob receives the number
+// P of view problems and prob_host [P][2] (may be NULL) their (rig, view), in the order of the rows.  With rows_dev [P][86]
+// (device; entries 10..12 and 82..84 are read) loss_dev [P] and grad_dev [P][86] (device) receive what the optimiser sees as
+// loss_eval / g_eval of each problem; rows_dev NULL: only the problems are reported.  Uses the context's optimiser state
+// (history size 100 when there is none).  Synchronises.
+extern "C" int mvs_debug_camera_closure(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig_dev, const mvs_loss_config* stage,
+                                        const float* rows_dev, float* loss_dev, float* grad_dev, int* prob_host, int* n_prob,
+                                        void* stream) {
+    static const char* who = "mvs_debug_camera_closure";
+    const cudaStream_t st = (cudaStream_t)stream;
+    LossParams lp;
+    int rc = camera_check(ctx, who, s, rig_dev, stage, 100, &lp, st);
+    if (!rc && (!n_prob || (rows_dev && (!loss_dev || !grad_dev)))) rc = set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    CameraPlan plan;
+    if (!rc) rc = camera_plan(ctx, s, rig_dev, &plan, st);
+    if (rc) return rc;
+    const int P = (int)plan.prob.size(), B = ctx->ws.B;
+    *n_prob = P;
+    for (int p = 0; p < P && prob_host; ++p) { prob_host[2 * p] = plan.prob[p].rig; prob_host[2 * p + 1] = plan.prob[p].view; }
+    if (!rows_dev || P == 0) return MVS_OK;
+    if ((rc = ensure_state(ctx, ctx->lbfgs ? ctx->lbfgs->H : 100))) return rc;
+    SeqState& h = *ctx->sstream;
+    const CameraArgs a0 = camera_args(ctx, s, rig_dev);
+    if ((rc = launch_camera_joints(ctx, a0.in, s->params, h.body.p, (int)plan.body.size(), lp, h.held.p, st)) ||
+        (rc = camera_refs(ctx, plan, st)))
+        return rc;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.rows.p, rows_dev, (size_t)P * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    const std::vector<int> ok((size_t)P, 1);
+    for (int base = 0; base < P && !rc; base += B) {
+        const int n = std::min(B, P - base);
+        if ((rc = shape_chunk_start(ctx, base, n, ok, st))) break;
+        const LbfgsState& S = *ctx->lbfgs;
+        if ((rc = launch_camera_closure(ctx, camera_chunk_args(a0, plan, base, n), lp, S, st))) break;
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(loss_dev + base, S.loss_eval, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(grad_dev + (size_t)base * kParams, S.g_eval, (size_t)n * kParams * sizeof(float),
                                          cudaMemcpyDeviceToDevice, st));

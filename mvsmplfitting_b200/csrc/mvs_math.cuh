@@ -305,6 +305,134 @@ template <class T, class C> MVS_HD void project_bwd(const C& cam, const T* x, co
     dq[1] += T(cam.R[1]) * dx0 + T(cam.R[4]) * dx1 + T(cam.R[7]) * dx2;
     dq[2] += T(cam.R[2]) * dx0 + T(cam.R[5]) * dx1 + T(cam.R[8]) * dx2;
 }
+// dx = the camera-space adjoint of the perspective divide (the first half of project_bwd)
+template <class T, class C> MVS_HD void project_bwd_x(const C& cam, const T* x, const T* duv, T* dx) {
+    const T iz = T(1) / x[2];
+    dx[0] = duv[0] * T(cam.f[0]) * iz;
+    dx[1] = duv[1] * T(cam.f[1]) * iz;
+    dx[2] = -(dx[0] * x[0] + dx[1] * x[1]) * iz;
+}
+
+// ---------------------------------------------------------------- camera refinement (mvs_refine_cameras, DESIGN.md section 4)
+// A refined view's camera from its update (w, c):  R = Rod(w) R0,  t = Rod(w) (t0 - R0 dC),  i.e.  x_cam = Rod(w) (R0 (q - dC) + t0).
+// Rod(w) = I + D,  D = A K + B K^2,  K = [w]x,  A = sin th / th,  B = (1 - cos th) / th^2,  th = |w|  (series below th^2 = 0.1),
+// so D = 0 exactly at w = 0 (rodrigues_fwd's +1e-8 shift is not).  dC is the camera-centre update: c itself for a free view; for
+// the view that keeps its distance r to view 0 (sphere), dC = (E u - n (s - 1)) / s with u = (c0, c1), s = sqrt(1 + |u|^2),
+// E = r [e1 e2] and n = r d (d: unit vector from view 0's centre to this one's, e1, e2 orthonormal and normal to it): the new
+// centre is view 0's + r (d + e1 u0 + e2 u1) / s.  Every entry adds its increment to the calibrated one, and an increment that
+// is zero keeps the calibrated bits (a -0 entry stays -0): at w = c = 0 the camera IS (R0, t0).
+struct CamRefine {
+    float R0[9], t0[3];
+    float E[6];                       // [3][2] row-major (sphere only)
+    float n[3];                       // (sphere only)
+    int sphere;
+};
+
+template <class T> struct CamDeltaState { T K[9], K2[9], D[9], p[3], a[3], A, B, dA, dB, s, nu, m; };
+
+// A, B and their derivatives with respect to th2 = th^2
+template <class T> MVS_HD void rotvec_coeffs(T th2, T* A, T* B, T* dA, T* dB) {
+    if (th2 < T(0.1)) {
+        *A = T(1) + th2 * (T(-1) / T(6) + th2 * (T(1) / T(120) + th2 * (T(-1) / T(5040))));
+        *B = T(0.5) + th2 * (T(-1) / T(24) + th2 * (T(1) / T(720) + th2 * (T(-1) / T(40320))));
+        *dA = T(-1) / T(6) + th2 * (T(1) / T(60) + th2 * (T(-1) / T(1680) + th2 * (T(1) / T(90720))));
+        *dB = T(-1) / T(24) + th2 * (T(1) / T(360) + th2 * (T(-1) / T(13440) + th2 * (T(1) / T(907200))));
+    } else {
+        const T th = mvs_sqrt(th2), s = mvs_sin(th), c = mvs_cos(th);
+        *A = s / th;
+        *B = (T(1) - c) / th2;
+        *dA = (th * c - s) / (T(2) * th2 * th);
+        *dB = (th * s - T(2) * (T(1) - c)) / (T(2) * th2 * th2);
+    }
+}
+
+template <class T> MVS_HD T add_increment(float base, T inc) { return inc == T(0) ? T(base) : T(base) + inc; }
+
+template <class T> MVS_HD void cam_from_delta(const CamRefine& cr, const T* w, const T* c, T* R, T* t, CamDeltaState<T>& S) {
+    const T th2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
+    rotvec_coeffs(th2, &S.A, &S.B, &S.dA, &S.dB);
+    const T K[9] = {T(0), -w[2], w[1], w[2], T(0), -w[0], -w[1], w[0], T(0)};
+#pragma unroll
+    for (int i = 0; i < 9; ++i) S.K[i] = K[i];
+    mat3_mul(S.K, S.K, S.K2);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) S.D[i] = S.A * S.K[i] + S.B * S.K2[i];
+    T dC[3];
+    if (cr.sphere) {
+        S.nu = c[0] * c[0] + c[1] * c[1];
+        S.s = mvs_sqrt(T(1) + S.nu);
+        S.m = S.nu / (S.s + T(1));                                     // s - 1 without the cancellation
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            S.a[i] = T(cr.E[2 * i]) * c[0] + T(cr.E[2 * i + 1]) * c[1] - T(cr.n[i]) * S.m;
+            dC[i] = S.a[i] / S.s;
+        }
+    } else {
+        dC[0] = c[0]; dC[1] = c[1]; dC[2] = c[2];
+    }
+    T R0[9], wv[3], Dp[3], RD[9];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) R0[i] = T(cr.R0[i]);
+    mat3_mul(S.D, R0, RD);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) R[i] = add_increment(cr.R0[i], RD[i]);
+    mat3_vec(R0, dC, wv);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) S.p[i] = T(cr.t0[i]) - wv[i];
+    mat3_vec(S.D, S.p, Dp);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) t[i] = add_increment(cr.t0[i], Dp[i] - wv[i]);
+}
+
+// (gw, gc) = the adjoint of cam_from_delta for the camera's adjoint (dR, dt); gc[2] = 0 for a sphere view
+template <class T> MVS_HD void cam_from_delta_bwd(const CamRefine& cr, const T* w, const T* c, const CamDeltaState<T>& S,
+                                                  const T* dR, const T* dt, T* gw, T* gc) {
+    T R0[9], dD[9], t1[9], t2[9], dp[3], dwv[3], ddC[3];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) R0[i] = T(cr.R0[i]);
+    mat3_mul_nt(dR, R0, dD);                                           // R = R0 + D R0
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int k = 0; k < 3; ++k) dD[3 * r + k] += dt[r] * S.p[k];   // t = t0 - R0 dC + D p
+    mat3_tvec(S.D, dt, dp);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) dwv[i] = -dt[i] - dp[i];
+    mat3_tvec(R0, dwv, ddC);
+    // D = A K + B K K
+    T dA = T(0), dB = T(0);
+#pragma unroll
+    for (int i = 0; i < 9; ++i) { dA += dD[i] * S.K[i]; dB += dD[i] * S.K2[i]; }
+    mat3_mul_nt(dD, S.K, t1);
+    mat3_mul_tn(S.K, dD, t2);
+    T dK[9];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) dK[i] = S.A * dD[i] + S.B * (t1[i] + t2[i]);
+    const T dth2 = dA * S.dA + dB * S.dB;
+    gw[0] = dK[7] - dK[5] + T(2) * w[0] * dth2;
+    gw[1] = dK[2] - dK[6] + T(2) * w[1] * dth2;
+    gw[2] = dK[3] - dK[1] + T(2) * w[2] * dth2;
+    if (cr.sphere) {
+        // dC = a / s,  a = E u - n m,  m = nu / (s + 1),  s = sqrt(1 + nu),  nu = |u|^2
+        T da[3], ds = T(0), dm = T(0);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            da[i] = ddC[i] / S.s;
+            ds -= ddC[i] * S.a[i] / (S.s * S.s);
+            dm -= T(cr.n[i]) * da[i];
+        }
+        const T sp1 = S.s + T(1);
+        T dnu = dm / sp1;
+        ds -= dm * S.nu / (sp1 * sp1);
+        dnu += ds / (T(2) * S.s);
+        gc[0] = T(cr.E[0]) * da[0] + T(cr.E[2]) * da[1] + T(cr.E[4]) * da[2] + T(2) * c[0] * dnu;
+        gc[1] = T(cr.E[1]) * da[0] + T(cr.E[3]) * da[1] + T(cr.E[5]) * da[2] + T(2) * c[1] * dnu;
+        gc[2] = T(0);
+    } else {
+        gc[0] = ddC[0]; gc[1] = ddC[1]; gc[2] = ddC[2];
+    }
+}
+
 // GMoF (utils/utils.py:427-438): rho^2 e^2 / (e^2 + rho^2) ; returns value, *dval = d/de
 template <class T> MVS_HD T gmof(T e, T rho2, T* dval) {
     const T sq = e * e, den = sq + rho2;

@@ -122,6 +122,22 @@ shape_reduce_kernel(LbfgsState L, ShapeArgs a) {
     if (lane == kOffOrient + 1) L.loss_eval[j] = (float)acc;
 }
 
+// The held keypoints of mvs_refine_cameras: ONE CTA per frame of `frames`, resident_closure's joints output (the keypoints the
+// 2-D term projects, with translation; VPoser decoded under use_vposer = 2) of the frame's row, into q [F][K][3]
+__global__ void __launch_bounds__(kResThreads, 2)
+camera_joints_kernel(ResidentModel m, RigSet rigs, LossParams lp, FrameInputs in, const float* __restrict__ params,
+                     const int* __restrict__ frames, float* __restrict__ q) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    ResidentSmem& S = *reinterpret_cast<ResidentSmem*>(smem_raw);
+    const int f = frames[blockIdx.x];
+    const FrameRig rig = frame_rig(rigs, f);
+    resident_setup(S, m);
+    for (int i = threadIdx.x; i < kParams; i += kResThreads) S.x[i] = params[(size_t)f * kParams + i];
+    __syncthreads();
+    VposerSmem* W = lp.use_vposer == 2 ? reinterpret_cast<VposerSmem*>(smem_raw + sizeof(ResidentSmem)) : nullptr;
+    resident_closure(S, m, rig, lp, in.gt_uv, in.conf, in.joint_w, in.n, f, false, q, nullptr, DenseIn{}, W);
+}
+
 // VPoser.decode(z, 'aa') alone (result export: code/utils/utils.py:741-743 decodes the fitted latent code before saving)
 __global__ void __launch_bounds__(kResThreads, 2)
 vposer_decode_kernel(ResidentModel m, const float* __restrict__ x, int B, float* __restrict__ body_pose) {
@@ -332,6 +348,7 @@ int resident_set_attributes(mvs_ctx* ctx) {
     const int one_frame = (int)(sizeof(ResidentSmem) + sizeof(VposerSmem));
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(closure_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, one_frame));
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(shape_closure_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, one_frame));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(camera_joints_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, one_frame));
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vposer_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, one_frame));
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(frame_fwd_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, one_frame));
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(lbfgs_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -381,6 +398,20 @@ int launch_shape_closure(mvs_ctx* ctx, const ShapeArgs& a, const LossParams& lp,
     MVS_LAUNCH(ctx, KID_RESIDENT_CLOSURE, st,
                shape_closure_kernel<<<a.nf, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev.p, a.in.rig}, lp, L, a));
     MVS_LAUNCH(ctx, KID_MISC, st, shape_reduce_kernel<<<a.n, 32, 0, st>>>(L, a));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    return MVS_OK;
+}
+
+int launch_camera_joints(mvs_ctx* ctx, const FrameInputs& in, const float* params, const int* frames, int n, const LossParams& lp,
+                         float* q, cudaStream_t st) {
+    if (n <= 0) return MVS_OK;
+    LossParams l = lp;
+    l.j3d_on = 0;                                                     // only the keypoints are read: no 3-D targets, no anchor
+    l.anchor_on = 0;
+    const size_t smem = sizeof(ResidentSmem) + (l.use_vposer == 2 ? sizeof(VposerSmem) : 0);
+    MVS_LAUNCH(ctx, KID_RESIDENT_CLOSURE, st,
+               camera_joints_kernel<<<n, kResThreads, smem, st>>>(make_resident_model(ctx), RigSet{ctx->rigs_dev.p, in.rig}, l, in,
+                                                                  params, frames, q));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }

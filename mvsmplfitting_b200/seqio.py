@@ -52,6 +52,36 @@ def camera_arrays(extris, intris, views=None) -> dict:
                 c=f32(np.stack([intris[:, 0, 2], intris[:, 1, 2]], 1)))
 
 
+def camera_matrices(cams: dict):
+    """The inverse of camera_arrays: a camera dict R [V,3,3], t [V,3], f [V,2], c [V,2] -> (extrinsics [V,4,4], intrinsics
+    [V,3,3]) float64, the layout load_camera_para returns"""
+    R, t = np.asarray(cams["R"], np.float64), np.asarray(cams["t"], np.float64)
+    f, c = np.asarray(cams["f"], np.float64), np.asarray(cams["c"], np.float64)
+    V = R.shape[0]
+    extris = np.zeros((V, 4, 4))
+    extris[:, :3, :3], extris[:, :3, 3], extris[:, 3, 3] = R, t, 1.0
+    intris = np.zeros((V, 3, 3))
+    intris[:, 0, 0], intris[:, 1, 1], intris[:, 0, 2], intris[:, 1, 2], intris[:, 2, 2] = f[:, 0], f[:, 1], c[:, 0], c[:, 1], 1.0
+    return extris, intris
+
+
+def write_camera_para(path: str, extris, intris) -> None:
+    """A camera file in the reference's layout (what load_camera_para reads): per view its index line, the three intrinsic
+    rows, '0 0' (no distortion), the three [R | t] rows and a blank line.  Numbers are written with repr, so float32 inputs
+    read back as the same float32 values."""
+    extris, intris = np.asarray(extris), np.asarray(intris)
+    row = lambda r: " ".join(repr(float(x)) for x in r) + " \n"
+    with open(path, "w") as fh:
+        for v in range(extris.shape[0]):
+            fh.write("%d\n" % v)
+            for r in intris[v]:
+                fh.write(row(r))
+            fh.write("0 0\n")
+            for r in extris[v][:3]:
+                fh.write(row(r))
+            fh.write("\n")
+
+
 def read_keypoints(path: str, person: int = 0):
     """data_parser.py:42-90 with use_hands = use_face = False: the first 17 (u, v, confidence) triplets of
     `pose_keypoints_2d` of one person as float32 [17,3]; None if the file lists fewer people."""
@@ -294,7 +324,7 @@ def _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces, f
 def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool = False, fixed_scale: float = 1.0,
                  use_hip: bool = True, pose_format: str = "coco17", result_folder: str | None = None,
                  mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, use_3d: bool = False,
-                 shared_shape: int = 0):
+                 shared_shape: int = 0, refine_cameras: int = 0):
     """The frame loop of main.py:32-89 for one sequence as ONE batch (every frame from its own initial guess, is_seq = False):
     upload the detections, initial guess on the device (init_guess + fix_params), all stages (`mvs_fit`), results per
     frame.  `ctx` is a FittingContext whose model, priors (GMM / VPoser decoder), cameras and batch (= number of frames) are
@@ -308,8 +338,12 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
     context has the 3-D term off afterwards.
     shared_shape (sweeps, 0: off): the sequence is one subject -- after the fit, one fit_shared_shape call gives all of its
     frames one betas (and scale) under the last stage, see share_shape; results are written after it.
+    refine_cameras (sweeps, 0: off): after the fit, one FittingContext.refine_cameras call over all frames refines the context's
+    camera extrinsics from them (before shared_shape when both are given), see refine_rigs; the refined rigs go into stats and,
+    with result_folder, into cameras_rig<r>.txt there.
     Returns (params [F,86] numpy -- pose slot = latent code under VPoser --, final_loss [F], stats)."""
     _check_shared_shape(shared_shape, None)
+    _check_refine_cameras(refine_cameras, None)
     F = len(seq["frames"])
     assert ctx.B <= F, "context batch %d > frames %d" % (ctx.B, F)
     latent = _uses_latent_pose(stage_cfgs)
@@ -329,6 +363,9 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
         final, stats = ctx.fit(params, stage_cfgs, opt_cfg)
         if t3 is not None:
             ctx.set_joints3d(None)
+        if refine_cameras:
+            final = refine_rigs(ctx, params, seq["gt_uv"], seq["conf"], jw, stage_cfgs, opt_cfg, refine_cameras, t3, stats=stats,
+                                result_folder=result_folder)
         if shared_shape:
             final = share_shape(ctx, params, seq["gt_uv"], seq["conf"], jw, [F], stage_cfgs, opt_cfg, shared_shape, t3, stats=stats)
         loss = final.cpu().numpy()
@@ -341,6 +378,9 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
     else:
         final, stats = ctx.fit_stream(params, seq["gt_uv"], seq["conf"], jw, stage_cfgs, opt_cfg, joints3d=t3[0], conf3d=t3[1])
         ctx.set_joints3d(None)
+    if refine_cameras:
+        final = refine_rigs(ctx, params, seq["gt_uv"], seq["conf"], jw, stage_cfgs, opt_cfg, refine_cameras, t3, stats=stats,
+                            result_folder=result_folder)
     if shared_shape:
         final = share_shape(ctx, params, seq["gt_uv"], seq["conf"], jw, [F], stage_cfgs, opt_cfg, shared_shape, t3, stats=stats)
     loss = final.cpu().numpy()
@@ -403,6 +443,33 @@ def _check_shared_shape(shared_shape, temporal_weight) -> None:
                          "independently, so the causal temporal term cannot be honoured")
 
 
+def _check_refine_cameras(refine_cameras, temporal_weight) -> None:
+    if isinstance(refine_cameras, bool) or int(refine_cameras) != refine_cameras or refine_cameras < 0:
+        raise ValueError("refine_cameras: want a number of sweeps >= 0 (0: off), got %r" % (refine_cameras,))
+    if refine_cameras and temporal_weight is not None:
+        raise ValueError("refine_cameras and temporal_weight do not combine: the camera refinement's body step fits frames "
+                         "independently, so the causal temporal term cannot be honoured")
+
+
+def refine_rigs(ctx, params, gt_uv, conf, jw, stage_cfgs, opt_cfg, sweeps, t3=None, rig=None, stats=None, result_folder=None):
+    """The camera refinement of fit_sequences / fit_sequence: ONE refine_cameras call over the fitted rows params [F,86]
+    (device, updated in place) of all frames, under the last stage configuration; t3 (_targets_3d of the frames) adds the
+    3-D term, rig [F] each frame's rig.  Returns the frames' final losses [F]; stats (a dict) gets 'refine_cameras': the
+    refined rigs (camera dicts, as set_camera_rigs takes them) and the camera and body steps' counts.  With result_folder,
+    rig r's refined calibration is written to <result_folder>/cameras_rig<r>.txt (write_camera_para)."""
+    kw = {} if rig is None else dict(rig=rig)
+    if t3 is not None:
+        kw.update(joints3d=t3[0], conf3d=t3[1])
+    final, rigs, ca, po = ctx.refine_cameras(params, gt_uv, conf, jw, stage_cfgs[-1], opt_cfg, sweeps=int(sweeps), **kw)
+    if stats is not None:
+        stats["refine_cameras"] = dict(rigs=rigs, camera=ca, pose=po)
+    if result_folder is not None:
+        os.makedirs(result_folder, exist_ok=True)
+        for r, cams in enumerate(rigs):
+            write_camera_para(os.path.join(result_folder, "cameras_rig%d.txt" % r), *camera_matrices(cams))
+    return final
+
+
 def share_shape(ctx, params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, sweeps, t3=None, rig=None, stats=None):
     """The shared shape of fit_sequences / fit_sequence: ONE fit_shared_shape call over the fitted rows params [F,86] (device,
     updated in place) of all sequences (lengths), under the last stage configuration; t3 (_targets_3d of the frames) adds the
@@ -434,7 +501,8 @@ def temporal_weight_vector(temporal_weight):
 def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = False, fixed_scale: float = 1.0,
                   use_hip: bool = True, pose_format: str = "coco17", result_folder: str | None = None,
                   mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, reinit_loss: float = 5000.0,
-                  use_3d: bool = False, rigs=None, rig_data_weight_scale=None, temporal_weight=None, shared_shape: int = 0):
+                  use_3d: bool = False, rigs=None, rig_data_weight_scale=None, temporal_weight=None, shared_shape: int = 0,
+                  refine_cameras: int = 0):
     """main.py:32-89 with is_seq = True for S sequences in lock-step: the batch of step t is frame t of every sequence
     (context batch = S).  A sequence's first frame gets the initial guess and every stage; a later frame
     starts from the previous frame's result as load_init + fix_params leave it (init_guess.py:137-166,190-212: betas,
@@ -460,8 +528,13 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
     shared_shape (a number of sweeps, 0: off) gives every sequence one body shape: after the fit, ONE fit_shared_shape call
     over all frames under the last stage configuration (the same call in lock-step and stream mode; see share_shape), and the
     results and meshes are written after it.  It does not combine with temporal_weight (ValueError).
+    refine_cameras (a number of sweeps, 0: off) refines every rig's camera extrinsics from the fitted bodies: after the fit, ONE
+    refine_cameras call over all frames with each frame's rig (see refine_rigs), before shared_shape when both are given; the
+    refined rigs go into stats['refine_cameras'] and, with result_folder, into cameras_rig<r>.txt there.  The context keeps
+    the refined cameras.  It does not combine with temporal_weight (ValueError).
     Returns a list (per sequence) of (params [T_s,86], loss [T_s]) and the summed stats."""
     _check_shared_shape(shared_shape, temporal_weight)
+    _check_refine_cameras(refine_cameras, temporal_weight)
     S_ = len(seqs)
     tw = temporal_weight_vector(temporal_weight)
     latent = _uses_latent_pose(stage_cfgs)
@@ -486,7 +559,7 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
                                      pose_format, use_hip, dict(estimate_scale=estimate_scale, fixed_scale=fixed_scale,
                                                                 use_torso=True, hip_seed=1.0, want_joints3d=False,
                                                                 umeyama_as_written=umeyama_as_written), t3, seq_rig, rig_views, tw,
-                                     shared_shape)
+                                     shared_shape, refine_cameras)
     T = max(len(q["frames"]) for q in seqs)
     V = seqs[0]["gt_uv"].shape[0]
     off = np.concatenate([[0], np.cumsum([len(q["frames"]) for q in seqs])])
@@ -537,19 +610,23 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
         for s_, q in enumerate(seqs):
             if live[s_]:
                 out_x[s_][t], out_l[s_][t] = x[s_], prev_loss[s_]
-        if result_folder is not None and not shared_shape:
+        if result_folder is not None and not (shared_shape or refine_cameras):
             for s_, q in enumerate(seqs):
                 if live[s_]:
                     _export(ctx, q, params, prev_loss, latent, result_folder, mesh_folder, faces, frames=[q["frames"][t]], rows=[s_])
     if t3 is not None:
         ctx.set_joints3d(None)
-    if shared_shape:
+    if shared_shape or refine_cameras:
         lengths = [len(q["frames"]) for q in seqs]
         x = torch.as_tensor(np.concatenate(out_x), device=ctx.device).contiguous()
         rig = None if seq_rig is None else np.repeat(seq_rig, lengths).astype(np.int32)
-        final = share_shape(ctx, x, np.concatenate([q["gt_uv"] for q in seqs], axis=1),
-                            np.concatenate([q["conf"] for q in seqs], axis=1), jw, lengths, stage_cfgs, opt_cfg, shared_shape, t3,
-                            rig, tot).cpu().numpy()
+        gt_all = np.concatenate([q["gt_uv"] for q in seqs], axis=1)
+        conf_all = np.concatenate([q["conf"] for q in seqs], axis=1)
+        if refine_cameras:
+            final = refine_rigs(ctx, x, gt_all, conf_all, jw, stage_cfgs, opt_cfg, refine_cameras, t3, rig, tot, result_folder)
+        if shared_shape:
+            final = share_shape(ctx, x, gt_all, conf_all, jw, lengths, stage_cfgs, opt_cfg, shared_shape, t3, rig, tot)
+        final = final.cpu().numpy()
         xs = x.cpu().numpy()
         out_x = [xs[off[s_]:off[s_ + 1]] for s_ in range(S_)]
         out_l = [final[off[s_]:off[s_ + 1]] for s_ in range(S_)]
@@ -560,11 +637,11 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
 
 
 def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces, pose_format,
-                          use_hip, guess, t3=None, seq_rig=None, rig_views=None, tw=None, shared_shape=0):
+                          use_hip, guess, t3=None, seq_rig=None, rig_views=None, tw=None, shared_shape=0, refine_cameras=0):
     """fit_sequences through mvs_fit_seq_stream: the sequences' frames back to back, every frame's cold start point from
     _cold_guesses; t3: _targets_3d of those frames (mvs_fit_seq_stream3d); seq_rig [S]: each sequence's rig, which every
     one of its frames takes (mvs_fit_seq_stream_rigs); tw [86]: the temporal weight (mvs_fit_seq_stream_temporal);
-    shared_shape: sweeps of share_shape after the fit (0: off)"""
+    shared_shape: sweeps of share_shape after the fit (0: off); refine_cameras: sweeps of refine_rigs before it (0: off)"""
     lengths = [len(q["frames"]) for q in seqs]
     off = np.concatenate([[0], np.cumsum(lengths)])
     gt_uv = np.concatenate([q["gt_uv"] for q in seqs], axis=1)
@@ -580,6 +657,8 @@ def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, r
     final, stats = ctx.fit_seq_stream(params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, reinit_loss=reinit_loss, **kw)
     if t3 is not None:
         ctx.set_joints3d(None)
+    if refine_cameras:
+        final = refine_rigs(ctx, params, gt_uv, conf, jw, stage_cfgs, opt_cfg, refine_cameras, t3, rig, stats, result_folder)
     if shared_shape:
         final = share_shape(ctx, params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, shared_shape, t3, rig, stats)
     x, loss = params.cpu().numpy(), final.cpu().numpy()
