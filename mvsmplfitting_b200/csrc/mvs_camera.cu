@@ -17,14 +17,14 @@ __device__ __noinline__ void build_camera(const CamRefine& cr, const float* w, c
 // that view: the same projection, weights, GMoF and dw^2, the keypoints' terms added in keypoint order.  Its gradient with
 // respect to the camera (R, t) is summed over the keypoints, then taken back to the problem's variables.
 __global__ void __launch_bounds__(128)
-camera_closure_kernel(LossParams lp, LbfgsState L, CameraArgs a) {
+camera_closure_kernel(LossParams lp, LbfgsState L, CameraArgs a, ProblemChunk ch) {
     const int lane = threadIdx.x & 31;
-    const int item = a.i0 + blockIdx.x * 4 + (threadIdx.x >> 5);
-    if (item >= a.i0 + a.ni) return;
-    const int p = a.item_prob[item], j = p - a.base;
+    const int item = ch.i0 + blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (item >= ch.i0 + ch.ni) return;
+    const int p = ch.item_of[item], j = p - ch.base;
     if (L.sc[j].phase == PH_DONE) return;                                // the problem has finished
     const CameraProblem P = a.prob[p];
-    const int f = a.frames[P.fbeg + item - P.item0], K = a.K, F = a.in.n;
+    const int f = a.frames[P.fbeg + item - ch.beg[p]], K = a.K, F = a.in.n;
     const CamRefine cr = a.cr[p];
     const float* xe = L.x_eval + (size_t)j * kParams;
     const float w[3] = {xe[kOffOrient], xe[kOffOrient + 1], xe[kOffOrient + 2]};
@@ -70,29 +70,11 @@ camera_closure_kernel(LossParams lp, LbfgsState L, CameraArgs a) {
     if (lane == 0) {
         float gw[3], gc[3];
         cam_from_delta_bwd(cr, w, c, S, g, g + 9, gw, gc);
-        float* out = a.part + (size_t)item * 8;
+        float* out = ch.part + (size_t)item * kPartCols;
         out[0] = acc * dw2;
         out[1] = gw[0]; out[2] = gw[1]; out[3] = gw[2];
         out[4] = gc[0]; out[5] = gc[1]; out[6] = gc[2];
     }
-}
-
-// Per problem (one warp, block j = slot j): its work items' losses and gradient entries added in double, in the rig's frame
-// order, into the slot's loss_eval / g_eval (zeros elsewhere).  The order depends on the problem's frames only.
-__global__ void __launch_bounds__(32)
-camera_reduce_kernel(LbfgsState L, CameraArgs a) {
-    const int j = blockIdx.x, lane = threadIdx.x;
-    if (L.sc[j].phase == PH_DONE) return;
-    const CameraProblem P = a.prob[a.base + j];
-    double acc = 0.0;
-    if (lane < 7)
-        for (int i = P.item0; i < P.item0 + P.nf; ++i) acc += (double)a.part[(size_t)i * 8 + lane];
-    float* g = L.g_eval + (size_t)j * kParams;
-    for (int i = lane; i < kParams; i += 32) g[i] = 0.f;
-    __syncwarp();
-    if (lane == 0) L.loss_eval[j] = (float)acc;
-    else if (lane < 4) g[kOffOrient + lane - 1] = (float)acc;
-    else if (lane < 7) g[kOffTransl + lane - 4] = (float)acc;
 }
 
 // One thread per problem: the camera at the problem's row into its rig's view
@@ -122,10 +104,10 @@ __global__ void row_finite_kernel(const float* __restrict__ params, int F, int* 
     if (lane == 0) fin[f] = ok ? 1 : 0;
 }
 
-int launch_camera_closure(mvs_ctx* ctx, const CameraArgs& a, const LossParams& lp, const LbfgsState& L, cudaStream_t st) {
-    if (a.ni > 0)
-        MVS_LAUNCH(ctx, KID_MISC, st, camera_closure_kernel<<<(a.ni + 3) / 4, 128, 0, st>>>(lp, L, a));
-    MVS_LAUNCH(ctx, KID_MISC, st, camera_reduce_kernel<<<a.n, 32, 0, st>>>(L, a));
+int launch_camera_closure(mvs_ctx* ctx, const CameraArgs& a, const ProblemChunk& c, const LossParams& lp, const LbfgsState& L,
+                          cudaStream_t st) {
+    if (c.ni > 0)
+        MVS_LAUNCH(ctx, KID_MISC, st, camera_closure_kernel<<<(c.ni + 3) / 4, 128, 0, st>>>(lp, L, a, c));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }

@@ -157,28 +157,33 @@ struct FrameInputs {
     const int* rig;
 };
 
-// The shape step of mvs_fit_shared_shape (DESIGN.md section 4): sequences base .. base + n - 1 of the call, in the optimiser's
-// slots 0 .. n - 1, whose frames are f0 .. f0 + nf - 1 of the call's F frames (in.n = F: the row stride of every input)
+// One chunk of a set of small problems solved by the batched chain's L-BFGS (DESIGN.md section 4): problems base .. base + n - 1
+// in the optimiser's slots 0 .. n - 1, whose work items are i0 .. i0 + ni - 1.  Problem p owns the work items [beg[p], beg[p+1])
+// and item i belongs to problem item_of[i].  Each work item writes its row of part: its loss, then its problem's gradient
+// entries of the call (at most kPartCols - 1, the same for every item); the driver adds the rows per problem.
+constexpr int kPartCols = 12;
+struct ProblemChunk {
+    const int* beg;                   // [P+1]
+    const int* item_of;               // [items]
+    float* part;                      // [items][kPartCols]
+    int base, n, i0, ni;
+};
+
+// The shape step of mvs_fit_shared_shape (DESIGN.md section 4): a problem per sequence, a work item per frame (in.n = F: the
+// row stride of every input)
 struct ShapeArgs {
     FrameInputs in;
     const float* params;              // [F][86] the frames' rows (poses held)
-    const int* off;                   // [S+1] device: sequence q owns frames [off[q], off[q+1])
-    const int* seq_of;                // [F] sequence of each frame
-    int base, n, f0, nf;
     int share_scale;                  // 1: scale (entry 85) is shared, 0: it stays per frame
-    float* loss;                      // [F] per-frame scratch
-    float* grad;                      // [F][86]
 };
 
-// One view problem of mvs_refine_cameras: view `view` of rig `rig`, whose frames are frames[fbeg .. fbeg + nf) of the call's
-// rig-grouped frame list (the frames with that rig and a finite row, in call order) and whose closure work items (one warp
-// per frame) are item0 .. item0 + nf - 1
+// One view problem of mvs_refine_cameras: view `view` of rig `rig`, whose frames are frames[fbeg ..) of the call's rig-grouped
+// frame list (the frames with that rig and a finite row, in call order), one work item each
 struct CameraProblem {
-    int rig, view, fbeg, nf, item0;
+    int rig, view, fbeg;
 };
 
-// The camera step of mvs_refine_cameras (DESIGN.md section 4): view problems base .. base + n - 1 in the optimiser's slots
-// 0 .. n - 1, whose work items are i0 .. i0 + ni - 1.  A problem's variables are the entries kOffOrient .. +2 (rotation
+// The camera step of mvs_refine_cameras (DESIGN.md section 4).  A problem's variables are the entries kOffOrient .. +2 (rotation
 // update) and kOffTransl .. +2 (centre update) of its slot's row; its closure is the 2-D data term of its view over its frames
 // at the held keypoints q.
 struct CameraArgs {
@@ -187,11 +192,8 @@ struct CameraArgs {
     const CamRefine* cr;              // [P] each problem's calibrated camera and centre map
     const CameraProblem* prob;        // [P]
     const int* frames;                // the rig-grouped frame list
-    const int* item_prob;             // [items] problem of each work item
     const Rig* rigs;                  // the context's rig table (intrinsics and data-weight scale)
     int K;
-    int base, n, i0, ni;
-    float* part;                      // [items][8] per work item: loss, rotation gradient [3], centre gradient [3]
 };
 
 // The chaining run of mvs_fit_seq_stream (DESIGN.md section 4): a finished frame hands its slot (a CTA of the frame-resident
@@ -465,16 +467,18 @@ int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, 
 int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
                               const LossParams* lp_tab_host, int nstages, const FrameInputs& frames, const SeqChain& q,
                               cudaStream_t st, const float* temporal_w = nullptr);
-// the shape closure of mvs_fit_shared_shape: per frame (shape_closure_kernel), then per sequence (shape_reduce_kernel) into
-// L.loss_eval / L.g_eval of the chunk's slots; slots whose problem is done are skipped
-int launch_shape_closure(mvs_ctx* ctx, const ShapeArgs& a, const LossParams& lp, const LbfgsState& L, cudaStream_t st);
+// the shape closure of mvs_fit_shared_shape: the part rows of chunk c's frames (loss, betas, scale); frames whose problem is
+// done are skipped
+int launch_shape_closure(mvs_ctx* ctx, const ShapeArgs& a, const ProblemChunk& c, const LossParams& lp, const LbfgsState& L,
+                         cudaStream_t st);
 // mvs_refine_cameras (mvs_resident.cu): the keypoints q [F][K][3] (with translation) of frames[0 .. n), the rows of params [F][86],
 // from resident_closure's joints output under lp (in: the call's frames, for the rigs)
 int launch_camera_joints(mvs_ctx* ctx, const FrameInputs& in, const float* params, const int* frames, int n, const LossParams& lp,
                          float* q, cudaStream_t st);
-// mvs_camera.cu: the camera closure of one chunk of view problems, per work item (camera_closure_kernel) and per problem
-// (camera_reduce_kernel) into L.loss_eval / L.g_eval of the chunk's slots; slots whose problem is done are skipped
-int launch_camera_closure(mvs_ctx* ctx, const CameraArgs& a, const LossParams& lp, const LbfgsState& L, cudaStream_t st);
+// mvs_camera.cu: the camera closure of one chunk of view problems: the part rows of its work items (loss, rotation gradient [3],
+// centre gradient [3]); items whose problem is done are skipped
+int launch_camera_closure(mvs_ctx* ctx, const CameraArgs& a, const ProblemChunk& c, const LossParams& lp, const LbfgsState& L,
+                          cudaStream_t st);
 // mvs_camera.cu: the cameras of problems 0 .. P-1 at their rows x [P][86] into the device rig table
 int launch_camera_write(mvs_ctx* ctx, const CamRefine* cr, const CameraProblem* prob, int P, const float* x, cudaStream_t st);
 // mvs_camera.cu: fin[f] = 1 iff row f of params [F][86] is all finite

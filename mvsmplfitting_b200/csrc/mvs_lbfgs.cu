@@ -885,26 +885,27 @@ static int run_stream(mvs_ctx* ctx, const char* who, const mvs_frame_stream* s, 
     return rc;
 }
 
-// mvs_fit_seq_stream and mvs_fit_shared_shape scratch (DESIGN.md section 4), every array grow-only.  A context runs one call at
-// a time, so the two share it: off and the gathered frames (gather_frames) serve both.
+// mvs_fit_seq_stream, mvs_fit_shared_shape and mvs_refine_cameras scratch (DESIGN.md section 4), every array grow-only.  A
+// context runs one call at a time, so they share it: the gathered frames (gather_frames) serve all three, and off, item_of,
+// part, rows and seq_final describe the small problems of the two alternating calls (solve_problems).
 struct SeqState {
-    DevBuf<int> off;                    // [S+1] the call's sequence offsets
+    DevBuf<int> off;                    // [S+1] the call's sequence offsets; alternating calls: [P+1] problem p owns the
+                                        // work items [off[p], off[p+1]) (shared shape: a problem per sequence, an item per frame)
     DevBuf<int> frames, packed_rig;     // [n] the gathered frames, their rigs
     DevBuf<float> packed;               // their packed rows (gather_floats)
     DevBuf<int> cur, act, lane_seq;     // sequence stream: [S], [S], [B] (SeqChain, LaneArgs)
     DevBuf<float> tw;                   // [F][86] the temporal weight, one row per frame (frame-resident chaining)
-    DevBuf<int> ok, seq_of;             // shared shape: [S] the sequence has a finite row, [F] each frame's sequence
-    DevBuf<float> rows;                 // [S + B][86] each sequence's shared row: the x of its problem (B rows of padding for
-                                        // the slots a last chunk leaves empty)
+    DevBuf<int> item_of;                // [items] the problem of each work item
+    DevBuf<float> part;                 // [items][kPartCols] each work item's loss and gradient entries
+    DevBuf<float> rows;                 // [P + B][86] each problem's x (B rows of padding for the slots a last chunk leaves empty)
     DevBuf<float> seq_final;            // [B] run_fitting's value of each slot's problem
-    DevBuf<float> loss, grad;           // [F], [F][86] the shape closure's per-frame terms
-    // camera refinement (rows and seq_final above serve its view problems)
+    DevBuf<int> ok;                     // shared shape: [S] the sequence has a finite row
+    // camera refinement
     DevBuf<int> fin, body;              // [F] the row is all finite, [n] the frames with a finite row (ascending)
     DevBuf<float> held;                 // [F][K][3] held keypoints
-    DevBuf<int> cam_frames, item_prob;  // the rig-grouped frame list, the problem of each work item
+    DevBuf<int> cam_frames;             // the rig-grouped frame list
     DevBuf<CameraProblem> prob;         // [P]
     DevBuf<CamRefine> cr;               // [P]
-    DevBuf<float> part;                 // [items][8] the camera closure's per-frame terms
 };
 
 static SeqState& seq_state(mvs_ctx* ctx) {
@@ -919,13 +920,14 @@ static size_t gather_floats(const mvs_ctx* ctx, int n, bool with_loss, bool j3d)
     return (size_t)n * (kParams + (size_t)ctx->vmax * K * 3 + (with_loss ? 1 : 0) + (j3d ? K * 4 : 0));
 }
 
-// Frames idx[0 .. n) of a sequence-stream call's arrays (gt_xyz / conf3d and rig as the call gives them, both NULL / NULL: none)
-// packed into the scratch as the frame stream *fs of n frames, with final-loss rows when with_loss; *prig: their rigs, NULL
-// without rig
-static int gather_frames(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig,
-                         const std::vector<int>& idx, bool with_loss, mvs_frame_stream* fs, const int** prig, cudaStream_t st) {
+// Frames idx[0 .. n) of a call's frames `in` and their rows params [in.n][86] packed into the scratch as the frame stream *fs of
+// n frames, with final-loss rows when with_loss; *prig: their rigs, NULL without in.rig
+static int gather_frames(mvs_ctx* ctx, const FrameInputs& in, float* params, const std::vector<int>& idx, bool with_loss,
+                         mvs_frame_stream* fs, const int** prig, cudaStream_t st) {
     SeqState& q = *ctx->sstream;
-    const int n = (int)idx.size(), F = s->seq_offsets[s->n_sequences], V = ctx->vmax, K = ctx->m.K;
+    const int n = (int)idx.size(), F = in.n, V = ctx->vmax, K = ctx->m.K;
+    const float *gt_xyz = in.j3d_xyz, *conf3d = in.j3d_conf;
+    const int* rig = in.rig;
     int rc;
     if ((rc = dev_grow(ctx, q.frames, (size_t)n)) || (rc = dev_grow(ctx, q.packed_rig, (size_t)n)) ||
         (rc = dev_grow(ctx, q.packed, gather_floats(ctx, n, with_loss, gt_xyz != nullptr))))
@@ -939,10 +941,10 @@ static int gather_frames(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
     float* pf = pc + (size_t)V * n * K;
     float* pj = gt_xyz ? pf + (with_loss ? n : 0) : nullptr;
     float* pjc = gt_xyz ? pj + (size_t)n * K * 3 : nullptr;
-    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, s->params, fr, n, F, kParams, 0));
-    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pg, const_cast<float*>(s->gt_uv), fr, n, F, 2 * K, 0,
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(px, params, fr, n, F, kParams, 0));
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pg, const_cast<float*>(in.gt_uv), fr, n, F, 2 * K, 0,
                                                                              rigs, rig));
-    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pc, const_cast<float*>(s->conf), fr, n, F, K, 0,
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, V), 128, 0, st>>>(pc, const_cast<float*>(in.conf), fr, n, F, K, 0,
                                                                              rigs, rig));
     if (rig)
         MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 32, 0, st>>>(q.packed_rig.p, const_cast<int*>(rig), fr, n, F, 1, 0));
@@ -950,19 +952,19 @@ static int gather_frames(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
         MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pj, const_cast<float*>(gt_xyz), fr, n, F, 3 * K, 0));
         MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(pjc, const_cast<float*>(conf3d), fr, n, F, K, 0));
     }
-    *fs = mvs_frame_stream{n, px, pg, pc, s->joint_weights, pj, pjc, with_loss ? pf : nullptr};
+    *fs = mvs_frame_stream{n, px, pg, pc, in.joint_w, pj, pjc, with_loss ? pf : nullptr};
     *prig = rig ? q.packed_rig.p : nullptr;
     return MVS_OK;
 }
 
-// The gathered frames' rows (gather_frames) back to the call's parameters, and their final losses when fs has them and the
-// call wants them
-static void scatter_frames(mvs_ctx* ctx, const mvs_sequence_stream* s, const mvs_frame_stream& fs, cudaStream_t st) {
-    const int n = fs.n_frames, F = s->seq_offsets[s->n_sequences];
+// The gathered frames' rows (gather_frames) back to the call's rows params [F][86], and their final losses to final_loss [F]
+// when fs has them and final_loss is not NULL
+static void scatter_frames(mvs_ctx* ctx, int F, float* params, float* final_loss, const mvs_frame_stream& fs, cudaStream_t st) {
+    const int n = fs.n_frames;
     const int* fr = ctx->sstream->frames.p;
-    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(fs.params, s->params, fr, n, F, kParams, 1));
-    if (fs.final_loss && s->final_loss)
-        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 32, 0, st>>>(fs.final_loss, s->final_loss, fr, n, F, 1, 1));
+    MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 128, 0, st>>>(fs.params, params, fr, n, F, kParams, 1));
+    if (fs.final_loss && final_loss)
+        MVS_LAUNCH(ctx, KID_MISC, st, copy_rows_kernel<<<dim3(n, 1), 32, 0, st>>>(fs.final_loss, final_loss, fr, n, F, 1, 1));
 }
 
 // The slots' anchor rows and weights (as mvs_set_anchor allocates them), weights set to w for every slot
@@ -980,11 +982,11 @@ static int temporal_slot_rows(mvs_ctx* ctx, const float* w, cudaStream_t st) {
 }
 
 // The chaining run over the sequences of one pass (q.act): every frame of run `tab` from its sequence's pending frame on
-// (gt_xyz / conf3d [F][K][3] / [F][K]: the 3-D targets, both NULL when the term is off)
+// (in: the call's frames, F = in.n)
 // temporal: the warm stages of tab carry the anchor term; its weight rows are set up (sstream->tw for the frame-resident
 // regime, ws.anchor_w for the dense one), and the anchor rows are the predecessors' fitted rows, handed over on the device.
-static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig, int F,
-                         Regime rg, const std::vector<LossParams>& tab, const SeqChain& q0, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats,
+static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const FrameInputs& in, Regime rg,
+                         const std::vector<LossParams>& tab, const SeqChain& q0, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats,
                          cudaStream_t st, bool temporal) {
     const int nst = (int)tab.size();
     use_stage(ctx, tab[0]);
@@ -997,20 +999,19 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
     q.totals = S.totals;
     if (rg == kResident) {
         // one launch, one CTA per sequence; rounds: the largest number of evaluations one CTA ran (its frames' sum)
-        const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d, rig};
         if ((rc = launch_lbfgs_resident_seq(ctx, s->params, cfg, cfg.history, S.lp_tab, tab.data(), nst, in, q, st,
                                             temporal ? ctx->sstream->tw.p : nullptr)))
             return rc;
         return read_totals(ctx, nullptr, false, stats, st);
     }
     LaneArgs a{};
-    a.F = F; a.n_queue = q.n_act;
-    a.params = s->params; a.final_loss = s->final_loss; a.gt_uv = s->gt_uv; a.conf = s->conf;
-    a.j3d_xyz = gt_xyz; a.j3d_conf = conf3d; a.rig = rig;
+    a.F = in.n; a.n_queue = q.n_act;
+    a.params = s->params; a.final_loss = s->final_loss; a.gt_uv = in.gt_uv; a.conf = in.conf;
+    a.j3d_xyz = in.j3d_xyz; a.j3d_conf = in.j3d_conf; a.rig = in.rig;
     a.q = q;
     a.lane_seq = ctx->sstream->lane_seq.p;
     a.anchor = temporal ? ctx->ws.anchor : nullptr;
-    return run_lanes(ctx, a, s->joint_weights, cfg, nst, stats, st);
+    return run_lanes(ctx, a, in.joint_w, cfg, nst, stats, st);
 }
 
 // mvs_fit_seq_stream (DESIGN.md section 4; who: the entry point called).  Stages are grouped into runs as mvs_fit_seq groups
@@ -1027,6 +1028,7 @@ static int run_seq_stream(mvs_ctx* ctx, const char* who, const mvs_sequence_stre
     const int NS = s->n_sequences;
     const std::vector<int> off(s->seq_offsets, s->seq_offsets + NS + 1);
     const int F = off[NS];
+    const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d, rig};
     const int j3d = gt_xyz ? 1 : 0;                                   // the call's own targets, never the context's
     std::vector<LossParams> lps, wlps;
     int rc = stage_table(ctx, who, n_stages, stage_cfgs, j3d, &lps);
@@ -1096,14 +1098,14 @@ static int run_seq_stream(mvs_ctx* ctx, const char* who, const mvs_sequence_stre
             // the pending frames through the runs before c, as a frame stream of their packed rows
             mvs_frame_stream fs;
             const int* prig;
-            if ((rc = gather_frames(ctx, s, gt_xyz, conf3d, rig, frames, false, &fs, &prig, st))) break;
+            if ((rc = gather_frames(ctx, in, s->params, frames, false, &fs, &prig, st))) break;
             for (int i = 0, g = 0; g < c && !rc; i = ends[g++])
                 rc = run_stream_group(ctx, &fs, prig, stage_regime(ctx, lps[i], H, false), &lps[i], ends[g] - i, opt_cfg, stats, st);
             if (rc) break;
-            scatter_frames(ctx, s, fs, st);
+            scatter_frames(ctx, F, s->params, nullptr, fs, st);
         }
         q.n_act = n;
-        if ((rc = run_seq_chain(ctx, s, gt_xyz, conf3d, rig, F, rg_chain, tab, q, opt_cfg, stats, st, tw != nullptr))) break;
+        if ((rc = run_seq_chain(ctx, s, in, rg_chain, tab, q, opt_cfg, stats, st, tw != nullptr))) break;
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(cur.data(), ss.cur.p, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
     }
@@ -1158,91 +1160,171 @@ __global__ void shape_consensus_kernel(const float* __restrict__ params, const i
 }
 
 // The shared entries of every frame of a sequence with a finite row: its sequence's row
-__global__ void shape_write_kernel(float* __restrict__ params, const int* __restrict__ seq_of, const float* __restrict__ rows,
+__global__ void shape_write_kernel(float* __restrict__ params, const int* __restrict__ item_of, const float* __restrict__ rows,
                                    const int* __restrict__ ok, int F, int share_scale) {
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
-    if (f >= F || !ok[seq_of[f]]) return;
-    const float* r = rows + (size_t)seq_of[f] * kParams;
+    if (f >= F || !ok[item_of[f]]) return;
+    const float* r = rows + (size_t)item_of[f] * kParams;
     float* x = params + (size_t)f * kParams;
     for (int i = kOffBetas; i < kOffOrient; ++i) x[i] = r[i];
     if (share_scale) x[kOffScale] = r[kOffScale];
 }
 
-// The slots of one chunk of sequence problems: slot j < n holds sequence base + j from its shared row (rows[base + j]) with a
-// fresh optimiser, unless the sequence has no finite row (ok); the other slots have no stage and leave the active list
-static int shape_chunk_start(mvs_ctx* ctx, int base, int n, const std::vector<int>& ok, cudaStream_t st) {
+// The small problems of mvs_fit_shared_shape (a sequence's shape) and mvs_refine_cameras (a view's extrinsics), solved by one
+// driver (DESIGN.md section 4).  Problem p's x is sstream->rows[p]; it owns the work items [beg[p], beg[p+1]) (device copy:
+// sstream->off, with sstream->item_of), and each item's closure kernel writes the item's part row: its loss, then the gradient
+// entries ent.e[0 .. ent.n) of its problem.
+struct PartEntries {
+    int n, e[kPartCols - 1];
+};
+struct ProblemSet {
+    std::vector<int> beg;               // [P+1] host
+    std::vector<int> on;                // [P] 0: the problem is not solved and its row stays (a sequence without a finite row)
+    PartEntries ent;
+    bool vp2 = false;                   // the pose entries of x hold a latent code (lbfgs_advance's pose length)
+};
+// The closure kernel of one chunk: the part rows of the chunk's work items
+using ChunkClosure = std::function<int(const ProblemChunk&, const LbfgsState&)>;
+
+// Per problem of a chunk (one warp, block j = slot j): lane k adds column k of the part rows of the problem's work items in
+// double, in item order; column 0 goes to the slot's loss_eval, column 1 + k to entry ent.e[k] of its g_eval (zeros elsewhere).
+// The order depends on the problem's items only.  Problems that have finished are skipped.
+__global__ void __launch_bounds__(32)
+problem_reduce_kernel(LbfgsState L, ProblemChunk c, PartEntries ent) {
+    const int j = blockIdx.x, lane = threadIdx.x, p = c.base + j;
+    if (L.sc[j].phase == PH_DONE) return;
+    double acc = 0.0;
+    if (lane <= ent.n)
+        for (int i = c.beg[p]; i < c.beg[p + 1]; ++i) acc += (double)c.part[(size_t)i * kPartCols + lane];
+    int e = -1;
+#pragma unroll
+    for (int k = 0; k < kPartCols - 1; ++k)
+        if (lane == k + 1 && k < ent.n) e = ent.e[k];
+    float* g = L.g_eval + (size_t)j * kParams;
+    for (int i = lane; i < kParams; i += 32) g[i] = 0.f;
+    __syncwarp();
+    if (lane == 0) L.loss_eval[j] = (float)acc;
+    else if (e >= 0) g[e] = (float)acc;
+}
+
+// The scratch of ps (rows for P problems and B slots of padding, each slot's final value, a part row per work item) and its
+// beg / item_of on the device
+static int problem_scratch(mvs_ctx* ctx, const ProblemSet& ps, cudaStream_t st) {
+    SeqState& h = seq_state(ctx);
+    const int P = (int)ps.beg.size() - 1, items = ps.beg[P], B = ctx->ws.B;
+    std::vector<int> item_of((size_t)items);
+    for (int p = 0; p < P; ++p)
+        for (int i = ps.beg[p]; i < ps.beg[p + 1]; ++i) item_of[i] = p;
+    int rc;
+    if ((rc = dev_grow(ctx, h.off, (size_t)P + 1)) || (rc = dev_grow(ctx, h.item_of, (size_t)std::max(items, 1))) ||
+        (rc = dev_grow(ctx, h.part, (size_t)std::max(items, 1) * kPartCols)) ||
+        (rc = dev_grow(ctx, h.rows, ((size_t)P + B) * kParams)) || (rc = dev_grow(ctx, h.seq_final, (size_t)B)))
+        return rc;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.off.p, ps.beg.data(), ps.beg.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.item_of.p, item_of.data(), (size_t)items * sizeof(int), cudaMemcpyHostToDevice, st));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    return MVS_OK;
+}
+
+// Chunk *c of ps: problems base .. base + n - 1, the context's B at most, in slots 0 .. n - 1, each from its row with a fresh
+// optimiser unless it is off; the other slots have no stage and leave the active list
+static int chunk_start(mvs_ctx* ctx, const ProblemSet& ps, int base, ProblemChunk* c, cudaStream_t st) {
     LbfgsState& S = *ctx->lbfgs;
     Workspace& w = ctx->ws;
-    const int B = w.B;
+    SeqState& h = *ctx->sstream;
+    const int B = w.B, n = std::min(B, (int)ps.beg.size() - 1 - base);
+    *c = ProblemChunk{h.off.p, h.item_of.p, h.part.p, base, n, ps.beg[base], ps.beg[base + n] - ps.beg[base]};
     std::vector<int> rng((size_t)B * 2, 0);
     bool some_inactive = false;
     for (int j = 0; j < B; ++j) {
-        const bool on = j < n && ok[base + j];
+        const bool on = j < n && ps.on[base + j];
         rng[2 * j + 1] = on ? 1 : 0;
         some_inactive |= !on;
     }
     if (int rc = upload_stage_rng(ctx, rng, st)) return rc;
     MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-    MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_init_kernel<<<B, 32, 0, st>>>(S, ctx->sstream->rows.p + (size_t)base * kParams, B, 1, 1,
-                                                                       ctx->stage_rng));
+    MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_init_kernel<<<B, 32, 0, st>>>(S, h.rows.p + (size_t)base * kParams, B, 1, 1, ctx->stage_rng));
     if (some_inactive) MVS_LAUNCH(ctx, KID_LBFGS_COMPACT, st, lbfgs_compact_kernel<<<1, 1024, 0, st>>>(S, B, w.fidx, w.na));
     return MVS_OK;
 }
 
-// The shape closure's arguments for sequences base .. base + n - 1 (off: the host copy of the offsets)
-static ShapeArgs shape_chunk_args(const ShapeArgs& a0, const std::vector<int>& off, int base, int n) {
-    ShapeArgs a = a0;
-    a.base = base; a.n = n;
-    a.f0 = off[base]; a.nf = off[base + n] - off[base];
-    return a;
+// One evaluation of chunk c: the closure's part rows, then their sums per problem into the slots' loss_eval / g_eval
+static int eval_chunk(mvs_ctx* ctx, const ProblemSet& ps, const ProblemChunk& c, const ChunkClosure& closure, cudaStream_t st) {
+    const LbfgsState& S = *ctx->lbfgs;
+    if (int rc = closure(c, S)) return rc;
+    MVS_LAUNCH(ctx, KID_MISC, st, problem_reduce_kernel<<<c.n, 32, 0, st>>>(S, c, ps.ent));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    return MVS_OK;
 }
 
-// The shape step: every sequence's L-BFGS problem over its shared entries, the context's B at a time, run as run_fitting runs a
-// frame's stage (lbfgs_init / advance / compact of the batched chain, with the shape closure as the closure)
-static int shape_step(mvs_ctx* ctx, const ShapeArgs& a0, const std::vector<int>& off, const std::vector<int>& ok,
-                      const LossParams& lp, const mvs_lbfgs_config* c, float* seq_loss, mvs_lbfgs_stats* stats, cudaStream_t st) {
-    const int NS = (int)off.size() - 1, B = ctx->ws.B;
+// Every problem of ps that is on, from its row, the context's B at a time, run as run_fitting runs a frame's stage (the batched
+// chain's lbfgs_init / advance / compact with the chunk's evaluation as the closure); final [P] (device, or NULL): run_fitting's
+// value of each problem
+static int solve_problems(mvs_ctx* ctx, const ProblemSet& ps, const ChunkClosure& closure, const LossParams& lp,
+                          const mvs_lbfgs_config* c, float* final, mvs_lbfgs_stats* stats, cudaStream_t st) {
     SeqState& h = *ctx->sstream;
-    for (int base = 0; base < NS; base += B) {
-        const int n = std::min(B, NS - base);
+    for (int base = 0; base < (int)ps.beg.size() - 1; base += ctx->ws.B) {
         LbfgsCfg cfg;
+        ProblemChunk ch;
         int rc = begin_run(ctx, c, false, &lp, 1, &cfg, st);
-        if (!rc) rc = shape_chunk_start(ctx, base, n, ok, st);
+        if (!rc) rc = chunk_start(ctx, ps, base, &ch, st);
         if (rc) return rc;
-        const LbfgsState S = *ctx->lbfgs;
-        const ShapeArgs a = shape_chunk_args(a0, off, base, n);
-        const std::function<int()> closure = [&]() { return launch_shape_closure(ctx, a, lp, S, st); };
-        if ((rc = run_batched(ctx, h.rows.p + (size_t)base * kParams, cfg, lp.use_vposer == 2, st, closure))) return rc;
+        const std::function<int()> eval = [&]() { return eval_chunk(ctx, ps, ch, closure, st); };
+        if ((rc = run_batched(ctx, h.rows.p + (size_t)base * kParams, cfg, ps.vp2, st, eval))) return rc;
         if ((rc = end_run(ctx, kBatched, h.seq_final.p, nullptr, stats, st))) return rc;
-        if (seq_loss)
-            MVS_CUDA_OK(ctx, cudaMemcpyAsync(seq_loss + base, h.seq_final.p, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        if (final)
+            MVS_CUDA_OK(ctx, cudaMemcpyAsync(final + base, h.seq_final.p, (size_t)ch.n * sizeof(float), cudaMemcpyDeviceToDevice, st));
     }
     return MVS_OK;
 }
 
-// The pose step: the frames of `frames` (ascending; the sequences with a finite row) as one frame stream of their packed rows
-// through run_stream under the one stage cfg; their rows and final losses go back to the call's arrays
-static int shape_pose_step(mvs_ctx* ctx, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d, const int* rig,
-                           const std::vector<int>& frames, const mvs_loss_config& cfg, const mvs_lbfgs_config* c,
-                           mvs_lbfgs_stats* stats, cudaStream_t st) {
+// The debug closures: every problem of ps evaluated once at rows [P][86] (device): loss [P] and grad [P][86] (device) receive
+// what the optimiser sees as loss_eval / g_eval.  Uses the context's optimiser state (history size 100 when there is none).
+// Synchronises.
+static int eval_problems(mvs_ctx* ctx, const ProblemSet& ps, const ChunkClosure& closure, const float* rows, float* loss,
+                         float* grad, cudaStream_t st) {
+    const int P = (int)ps.beg.size() - 1, B = ctx->ws.B;
+    int rc = ensure_state(ctx, ctx->lbfgs ? ctx->lbfgs->H : 100);
+    if (rc) return rc;
+    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->sstream->rows.p, rows, (size_t)P * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    for (int base = 0; base < P && !rc; base += B) {
+        ProblemChunk ch;
+        if ((rc = chunk_start(ctx, ps, base, &ch, st)) || (rc = eval_chunk(ctx, ps, ch, closure, st))) break;
+        const LbfgsState& S = *ctx->lbfgs;
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(loss + base, S.loss_eval, (size_t)ch.n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(grad + (size_t)base * kParams, S.g_eval, (size_t)ch.n * kParams * sizeof(float),
+                                         cudaMemcpyDeviceToDevice, st));
+    }
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(ctx->ws.fidx, B, ctx->ws.na));
+    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    return rc;
+}
+
+// The body step of an alternating call (who: the entry point called): `frames` (ascending) of the call's frames `in` as one
+// frame stream of their packed rows through run_stream under the one stage cfg; their rows and final losses go back to params
+// and final_loss (may be NULL)
+static int refit_bodies(mvs_ctx* ctx, const char* who, const FrameInputs& in, float* params, float* final_loss,
+                        const std::vector<int>& frames, const mvs_loss_config* cfg, const mvs_lbfgs_config* c,
+                        mvs_lbfgs_stats* stats, cudaStream_t st) {
     if (frames.empty()) return MVS_OK;
     mvs_frame_stream fs;
     const int* prig;
-    int rc = gather_frames(ctx, s, gt_xyz, conf3d, rig, frames, true, &fs, &prig, st);
-    if (!rc) rc = run_stream(ctx, "mvs_fit_shared_shape", &fs, prig, 1, &cfg, c, stats, st);
+    int rc = gather_frames(ctx, in, params, frames, true, &fs, &prig, st);
+    if (!rc) rc = run_stream(ctx, who, &fs, prig, 1, cfg, c, stats, st);
     if (rc) return rc;
-    scatter_frames(ctx, s, fs, st);
+    scatter_frames(ctx, in.n, params, final_loss, fs, st);
     MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }
 
 // What mvs_fit_shared_shape and mvs_debug_shape_closure share once check_seq_stream has passed: the checks of the stage, its
-// LossParams (3-D term as the call says), the offsets on the host, and the scratch with the offsets and each frame's sequence on
-// the device.  a0 gets the shape closure's arguments except the chunk.
+// LossParams (3-D term as the call says), the sequences as problems (a work item per frame, the shared entries as variables)
+// with their scratch, and the shape closure's arguments a
 static int shape_prepare(mvs_ctx* ctx, const char* who, const mvs_sequence_stream* s, const float* gt_xyz, const float* conf3d,
-                         const int* rig, const mvs_loss_config* stage, int H, LossParams* lp, std::vector<int>* off,
-                         ShapeArgs* a0, cudaStream_t st) {
+                         const int* rig, const mvs_loss_config* stage, int H, LossParams* lp, ProblemSet* ps, ShapeArgs* a,
+                         cudaStream_t st) {
     if (!stage) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
     if (stage->frozen_mask & 1u)
         return set_error(ctx, MVS_ERR_INVALID, "%s: the stage freezes betas (fix_shape): the shape is given, there is nothing to "
@@ -1256,29 +1338,18 @@ static int shape_prepare(mvs_ctx* ctx, const char* who, const mvs_sequence_strea
     if (stage_regime(ctx, *lp, H, false) != kResident)
         return set_error(ctx, MVS_ERR_UNSUPPORTED, "%s: the stage would not run in the frame-resident kernels (exec mode 1, "
                                                    "history_size > 100, or a model they do not take)", who);
-    const int NS = s->n_sequences, F = s->seq_offsets[NS], B = ctx->ws.B;
-    off->assign(s->seq_offsets, s->seq_offsets + NS + 1);
-    SeqState& h = seq_state(ctx);
-    if ((rc = dev_grow(ctx, h.off, (size_t)NS + 1)) || (rc = dev_grow(ctx, h.ok, (size_t)NS)) ||
-        (rc = dev_grow(ctx, h.rows, ((size_t)NS + B) * kParams)) || (rc = dev_grow(ctx, h.seq_final, (size_t)B)) ||
-        (rc = dev_grow(ctx, h.seq_of, (size_t)F)) || (rc = dev_grow(ctx, h.loss, (size_t)F)) ||
-        (rc = dev_grow(ctx, h.grad, (size_t)F * kParams)))
-        return rc;
-    std::vector<int> seq_of((size_t)F);
-    for (int q = 0; q < NS; ++q)
-        for (int f = (*off)[q]; f < (*off)[q + 1]; ++f) seq_of[f] = q;
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.off.p, off->data(), off->size() * sizeof(int), cudaMemcpyHostToDevice, st));
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.seq_of.p, seq_of.data(), (size_t)F * sizeof(int), cudaMemcpyHostToDevice, st));
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    *a0 = ShapeArgs{};
-    a0->in = FrameInputs{F, s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d, rig};
-    a0->params = s->params;
-    a0->off = h.off.p;
-    a0->seq_of = h.seq_of.p;
-    a0->share_scale = (stage->frozen_mask >> 4 & 1u) ? 0 : 1;
-    a0->loss = h.loss.p;
-    a0->grad = h.grad.p;
-    return MVS_OK;
+    const int NS = s->n_sequences;
+    *a = ShapeArgs{FrameInputs{s->seq_offsets[NS], s->gt_uv, s->conf, s->joint_weights, gt_xyz, conf3d, rig}, s->params,
+                   (stage->frozen_mask >> 4 & 1u) ? 0 : 1};
+    *ps = ProblemSet{};
+    ps->beg.assign(s->seq_offsets, s->seq_offsets + NS + 1);
+    ps->on.assign((size_t)NS, 1);
+    ps->ent.n = kOffOrient + a->share_scale;                         // betas, then scale
+    for (int e = 0; e < kOffOrient; ++e) ps->ent.e[e] = kOffBetas + e;
+    ps->ent.e[kOffOrient] = kOffScale;
+    ps->vp2 = lp->use_vposer == 2;
+    if ((rc = dev_grow(ctx, seq_state(ctx).ok, (size_t)NS))) return rc;
+    return problem_scratch(ctx, *ps, st);
 }
 
 // Refuses a call (who: the entry point called) before the context has model, cameras and batch, and the keypoints (kp) and the
@@ -1300,6 +1371,21 @@ static int begin_batch_call(mvs_ctx* ctx, const char* who, bool kp, bool loss, b
     if (int rc = batch_rigs(ctx, who)) return rc;
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     if (stats) memset(stats, 0, sizeof(*stats));
+    return MVS_OK;
+}
+
+// The alternating calls (mvs_fit_shared_shape, mvs_refine_cameras; who: the one called): what they check of their sweeps
+// (check_sweeps), and how they start once every check has passed (start_sweeps: both stats zeroed, the F final losses NaN, as
+// the frames without a finite row keep them)
+static int check_sweeps(mvs_ctx* ctx, const char* who, const mvs_lbfgs_config* opt_cfg, int n_sweeps) {
+    if (!opt_cfg) return set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
+    if (n_sweeps < 1) return set_error(ctx, MVS_ERR_INVALID, "%s: n_sweeps must be >= 1 (got %d)", who, n_sweeps);
+    return MVS_OK;
+}
+static int start_sweeps(mvs_ctx* ctx, int F, float* final_loss, mvs_lbfgs_stats* a, mvs_lbfgs_stats* b, cudaStream_t st) {
+    if (a) memset(a, 0, sizeof(*a));
+    if (b) memset(b, 0, sizeof(*b));
+    if (final_loss) MVS_CUDA_OK(ctx, cudaMemsetAsync(final_loss, 0xff, (size_t)F * sizeof(float), st));
     return MVS_OK;
 }
 
@@ -1381,11 +1467,11 @@ static int fit_seq_stream(mvs_ctx* ctx, const char* who, const mvs_sequence_stre
 }
 
 // The view problems of a mvs_refine_cameras call: the frames with a finite row, ascending (body), grouped by rig in call
-// order (frames), and one problem per view 1 .. V_r - 1 of every rig with such frames
+// order (frames), and one problem per view 1 .. V_r - 1 of every rig with such frames, a work item per frame of its rig (ps)
 struct CameraPlan {
     std::vector<int> body, frames;
     std::vector<CameraProblem> prob;
-    int items = 0;
+    ProblemSet ps;
 };
 
 // What mvs_refine_cameras and mvs_debug_camera_closure check before anything changes (who: the entry point called), and the
@@ -1414,7 +1500,7 @@ static int camera_check(mvs_ctx* ctx, const char* who, const mvs_frame_stream* s
 
 // The call's plan (finite rows and rigs read back once) and its scratch on the device
 static int camera_plan(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig, CameraPlan* plan, cudaStream_t st) {
-    const int F = s->n_frames, B = ctx->ws.B, nr = (int)ctx->rigs.size();
+    const int F = s->n_frames, nr = (int)ctx->rigs.size();
     SeqState& h = seq_state(ctx);
     int rc;
     if ((rc = dev_grow(ctx, h.fin, (size_t)F)) || (rc = launch_row_finite(ctx, s->params, F, h.fin.p, st))) return rc;
@@ -1426,30 +1512,28 @@ static int camera_plan(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig, 
     std::vector<std::vector<int>> of((size_t)nr);
     for (int f = 0; f < F; ++f)
         if (fin[f]) { plan->body.push_back(f); of[rg[f]].push_back(f); }
-    std::vector<int> item_prob;
+    ProblemSet& ps = plan->ps;
+    ps.beg.assign(1, 0);
     for (int r = 0; r < nr; ++r) {
         const int fbeg = (int)plan->frames.size(), nf = (int)of[r].size();
         plan->frames.insert(plan->frames.end(), of[r].begin(), of[r].end());
         if (nf == 0) continue;
         for (int v = 1; v < ctx->rigs[r].num_views; ++v) {
-            plan->prob.push_back(CameraProblem{r, v, fbeg, nf, plan->items});
-            item_prob.insert(item_prob.end(), (size_t)nf, (int)plan->prob.size() - 1);
-            plan->items += nf;
+            plan->prob.push_back(CameraProblem{r, v, fbeg});
+            ps.beg.push_back(ps.beg.back() + nf);
         }
     }
     const size_t P = plan->prob.size(), n = plan->body.size();
+    ps.on.assign(P, 1);
+    ps.ent = PartEntries{6, {kOffOrient, kOffOrient + 1, kOffOrient + 2, kOffTransl, kOffTransl + 1, kOffTransl + 2}};
     if ((rc = dev_grow(ctx, h.body, std::max<size_t>(n, 1))) || (rc = dev_grow(ctx, h.held, (size_t)F * ctx->m.K * 3)) ||
-        (rc = dev_grow(ctx, h.cam_frames, std::max<size_t>(n, 1))) ||
-        (rc = dev_grow(ctx, h.item_prob, std::max<size_t>(plan->items, 1))) || (rc = dev_grow(ctx, h.prob, std::max<size_t>(P, 1))) ||
-        (rc = dev_grow(ctx, h.cr, std::max<size_t>(P, 1))) || (rc = dev_grow(ctx, h.part, (size_t)std::max(plan->items, 1) * 8)) ||
-        (rc = dev_grow(ctx, h.rows, (P + B) * kParams)) || (rc = dev_grow(ctx, h.seq_final, (size_t)B)))
+        (rc = dev_grow(ctx, h.cam_frames, std::max<size_t>(n, 1))) || (rc = dev_grow(ctx, h.prob, std::max<size_t>(P, 1))) ||
+        (rc = dev_grow(ctx, h.cr, std::max<size_t>(P, 1))))
         return rc;
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.body.p, plan->body.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.cam_frames.p, plan->frames.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.item_prob.p, item_prob.data(), item_prob.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.prob.p, plan->prob.data(), P * sizeof(CameraProblem), cudaMemcpyHostToDevice, st));
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    return MVS_OK;
+    return problem_scratch(ctx, ps, st);
 }
 
 // Each problem's calibrated camera, from the context's rig table as it stands (host copy): view 1 moves on the sphere about view
@@ -1493,66 +1577,23 @@ static int camera_refs(mvs_ctx* ctx, const CameraPlan& plan, cudaStream_t st) {
     return MVS_OK;
 }
 
-// The camera closure's arguments for problems base .. base + n - 1
-static CameraArgs camera_chunk_args(const CameraArgs& a0, const CameraPlan& plan, int base, int n) {
-    CameraArgs a = a0;
-    a.base = base; a.n = n;
-    a.i0 = plan.prob[base].item0;
-    a.ni = plan.prob[base + n - 1].item0 + plan.prob[base + n - 1].nf - a.i0;
-    return a;
-}
-
-static CameraArgs camera_args(mvs_ctx* ctx, const mvs_frame_stream* s, const int* rig) {
+static CameraArgs camera_args(mvs_ctx* ctx, const FrameInputs& in) {
     SeqState& h = *ctx->sstream;
-    CameraArgs a{};
-    a.in = FrameInputs{s->n_frames, s->gt_uv, s->conf, s->joint_weights, nullptr, nullptr, rig};
-    a.q = h.held.p; a.cr = h.cr.p; a.prob = h.prob.p; a.frames = h.cam_frames.p; a.item_prob = h.item_prob.p;
-    a.rigs = ctx->rigs_dev.p; a.K = ctx->m.K; a.part = h.part.p;
-    return a;
+    return CameraArgs{in, h.held.p, h.cr.p, h.prob.p, h.cam_frames.p, ctx->rigs_dev.p, ctx->m.K};
 }
 
-// The camera step: every view problem from 0, the context's B at a time, run as run_fitting runs a frame's stage (the batched
-// chain's lbfgs_init / advance / compact with the camera closure); then the solved cameras into the table and its host copy
-static int camera_step(mvs_ctx* ctx, const CameraArgs& a0, const CameraPlan& plan, const LossParams& lp, const mvs_lbfgs_config* c,
-                       mvs_lbfgs_stats* stats, cudaStream_t st) {
-    const int P = (int)plan.prob.size(), B = ctx->ws.B;
+// The camera step: every view problem from a zero update (solve_problems with the camera closure); then the solved cameras into
+// the table and its host copy
+static int solve_cameras(mvs_ctx* ctx, const CameraPlan& plan, const ChunkClosure& closure, const LossParams& lp,
+                         const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats, cudaStream_t st) {
+    const int P = (int)plan.prob.size();
     if (P == 0) return MVS_OK;
     SeqState& h = *ctx->sstream;
     MVS_CUDA_OK(ctx, cudaMemsetAsync(h.rows.p, 0, (size_t)P * kParams * sizeof(float), st));
-    const std::vector<int> ok((size_t)P, 1);
-    for (int base = 0; base < P; base += B) {
-        const int n = std::min(B, P - base);
-        LbfgsCfg cfg;
-        int rc = begin_run(ctx, c, false, &lp, 1, &cfg, st);
-        if (!rc) rc = shape_chunk_start(ctx, base, n, ok, st);
-        if (rc) return rc;
-        const LbfgsState S = *ctx->lbfgs;
-        const CameraArgs a = camera_chunk_args(a0, plan, base, n);
-        const std::function<int()> closure = [&]() { return launch_camera_closure(ctx, a, lp, S, st); };
-        if ((rc = run_batched(ctx, h.rows.p + (size_t)base * kParams, cfg, false, st, closure))) return rc;
-        if ((rc = end_run(ctx, kBatched, h.seq_final.p, nullptr, stats, st))) return rc;
-    }
+    if (int rc = solve_problems(ctx, plan.ps, closure, lp, c, nullptr, stats, st)) return rc;
     if (int rc = launch_camera_write(ctx, h.cr.p, h.prob.p, P, h.rows.p, st)) return rc;
     MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->rigs.data(), ctx->rigs_dev.p, ctx->rigs.size() * sizeof(Rig), cudaMemcpyDeviceToHost, st));
     MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    return MVS_OK;
-}
-
-// The body step: the frames with a finite row as one frame stream of their packed rows through run_stream under the stage,
-// against the refined table; their rows and final losses go back to the call's arrays
-static int camera_body_step(mvs_ctx* ctx, const char* who, const mvs_frame_stream* s, const int* rig, const CameraPlan& plan,
-                            const mvs_loss_config* stage, const mvs_lbfgs_config* c, mvs_lbfgs_stats* stats, cudaStream_t st) {
-    if (plan.body.empty()) return MVS_OK;
-    const int off[2] = {0, s->n_frames};
-    const mvs_sequence_stream ss{1, off, s->params, s->gt_uv, s->conf, s->joint_weights, s->final_loss, 0.f};
-    mvs_frame_stream fs;
-    const int* prig;
-    int rc = gather_frames(ctx, &ss, s->gt_xyz, s->conf3d, rig, plan.body, true, &fs, &prig, st);
-    if (!rc) rc = run_stream(ctx, who, &fs, prig, 1, stage, c, stats, st);
-    if (rc) return rc;
-    scatter_frames(ctx, &ss, fs, st);
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }
 
@@ -1563,23 +1604,22 @@ static int refine_cameras(mvs_ctx* ctx, const mvs_frame_stream* s, const int* ri
     static const char* who = "mvs_refine_cameras";
     LossParams lp;
     int rc = check_ready(ctx, who);
-    if (!rc && !opt_cfg) rc = set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
-    if (!rc && n_sweeps < 1) rc = set_error(ctx, MVS_ERR_INVALID, "%s: n_sweeps must be >= 1 (got %d)", who, n_sweeps);
+    if (!rc) rc = check_sweeps(ctx, who, opt_cfg, n_sweeps);
     if (!rc) rc = camera_check(ctx, who, s, rig, stage, history_size(opt_cfg), &lp, st);
     if (rc) return rc;
-    if (camera_stats) memset(camera_stats, 0, sizeof(*camera_stats));
-    if (pose_stats) memset(pose_stats, 0, sizeof(*pose_stats));
+    const FrameInputs in{s->n_frames, s->gt_uv, s->conf, s->joint_weights, s->gt_xyz, s->conf3d, rig};
+    if ((rc = start_sweeps(ctx, in.n, s->final_loss, camera_stats, pose_stats, st))) return rc;
     CameraPlan plan;
     if ((rc = camera_plan(ctx, s, rig, &plan, st))) return rc;
-    const CameraArgs a0 = camera_args(ctx, s, rig);
-    const FrameInputs in = a0.in;
+    SeqState& h = *ctx->sstream;
+    const CameraArgs a = camera_args(ctx, in);
+    const ChunkClosure closure = [&](const ProblemChunk& c, const LbfgsState& S) { return launch_camera_closure(ctx, a, c, lp, S, st); };
     stream_call_begin(ctx);
-    if (s->final_loss) MVS_CUDA_OK(ctx, cudaMemsetAsync(s->final_loss, 0xff, (size_t)s->n_frames * sizeof(float), st));   // NaN
     for (int sweep = 0; sweep < n_sweeps && !rc; ++sweep) {
-        if ((rc = launch_camera_joints(ctx, in, s->params, ctx->sstream->body.p, (int)plan.body.size(), lp, ctx->sstream->held.p, st)) ||
-            (rc = camera_refs(ctx, plan, st)) || (rc = camera_step(ctx, a0, plan, lp, opt_cfg, camera_stats, st)))
+        if ((rc = launch_camera_joints(ctx, in, s->params, h.body.p, (int)plan.body.size(), lp, h.held.p, st)) ||
+            (rc = camera_refs(ctx, plan, st)) || (rc = solve_cameras(ctx, plan, closure, lp, opt_cfg, camera_stats, st)))
             break;
-        rc = camera_body_step(ctx, who, s, rig, plan, stage, opt_cfg, pose_stats, st);
+        rc = refit_bodies(ctx, who, in, s->params, s->final_loss, plan.body, stage, opt_cfg, pose_stats, st);
     }
     stream_call_end(ctx, lp);
     if (rc) return rc;
@@ -1685,33 +1725,31 @@ int mvs_fit_shared_shape(mvs_ctx* ctx, const mvs_sequence_stream* s, const float
     static const char* who = "mvs_fit_shared_shape";
     const cudaStream_t st = (cudaStream_t)stream;
     LossParams lp;
-    std::vector<int> off;
-    ShapeArgs a0;
+    ProblemSet ps;
+    ShapeArgs a;
     int rc = check_seq_stream(ctx, who, s, gt_xyz, conf3d, rig_dev, st);
-    if (!rc && !opt_cfg) rc = set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
-    if (!rc && n_sweeps < 1) rc = set_error(ctx, MVS_ERR_INVALID, "%s: n_sweeps must be >= 1 (got %d)", who, n_sweeps);
-    if (!rc) rc = shape_prepare(ctx, who, s, gt_xyz, conf3d, rig_dev, stage, history_size(opt_cfg), &lp, &off, &a0, st);
+    if (!rc) rc = check_sweeps(ctx, who, opt_cfg, n_sweeps);
+    if (!rc) rc = shape_prepare(ctx, who, s, gt_xyz, conf3d, rig_dev, stage, history_size(opt_cfg), &lp, &ps, &a, st);
+    if (!rc) rc = start_sweeps(ctx, a.in.n, s->final_loss, shape_stats, pose_stats, st);
     if (rc) return rc;
-    if (shape_stats) memset(shape_stats, 0, sizeof(*shape_stats));
-    if (pose_stats) memset(pose_stats, 0, sizeof(*pose_stats));
-    const int NS = s->n_sequences, F = off[NS];
+    const int NS = s->n_sequences, F = a.in.n;
     SeqState& h = *ctx->sstream;
     mvs_loss_config pose_cfg = *stage;                                   // the pose step: the shared entries held
-    pose_cfg.frozen_mask |= 1u | (a0.share_scale ? 16u : 0u);
-    if (s->final_loss) MVS_CUDA_OK(ctx, cudaMemsetAsync(s->final_loss, 0xff, (size_t)F * sizeof(float), st));   // NaN: skipped
-    std::vector<int> ok((size_t)NS), frames;
+    pose_cfg.frozen_mask |= 1u | (a.share_scale ? 16u : 0u);
+    const ChunkClosure closure = [&](const ProblemChunk& c, const LbfgsState& S) { return launch_shape_closure(ctx, a, c, lp, S, st); };
+    std::vector<int> frames;
     for (int sweep = 0; sweep < n_sweeps && !rc; ++sweep) {
-        MVS_LAUNCH(ctx, KID_MISC, st, shape_consensus_kernel<<<NS, 32, 0, st>>>(s->params, h.off.p, a0.share_scale, h.rows.p, h.ok.p));
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ok.data(), h.ok.p, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
+        MVS_LAUNCH(ctx, KID_MISC, st, shape_consensus_kernel<<<NS, 32, 0, st>>>(s->params, h.off.p, a.share_scale, h.rows.p, h.ok.p));
+        MVS_CUDA_OK(ctx, cudaMemcpyAsync(ps.on.data(), h.ok.p, (size_t)NS * sizeof(int), cudaMemcpyDeviceToHost, st));
         MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-        if ((rc = shape_step(ctx, a0, off, ok, lp, opt_cfg, seq_loss_dev, shape_stats, st))) break;
-        MVS_LAUNCH(ctx, KID_MISC, st, shape_write_kernel<<<(F + 127) / 128, 128, 0, st>>>(s->params, h.seq_of.p, h.rows.p, h.ok.p, F,
-                                                                                        a0.share_scale));
+        if ((rc = solve_problems(ctx, ps, closure, lp, opt_cfg, seq_loss_dev, shape_stats, st))) break;
+        MVS_LAUNCH(ctx, KID_MISC, st, shape_write_kernel<<<(F + 127) / 128, 128, 0, st>>>(s->params, h.item_of.p, h.rows.p, h.ok.p, F,
+                                                                                        a.share_scale));
         frames.clear();
         for (int q = 0; q < NS; ++q)
-            if (ok[q])
-                for (int f = off[q]; f < off[q + 1]; ++f) frames.push_back(f);
-        rc = shape_pose_step(ctx, s, gt_xyz, conf3d, rig_dev, frames, pose_cfg, opt_cfg, pose_stats, st);
+            if (ps.on[q])
+                for (int f = ps.beg[q]; f < ps.beg[q + 1]; ++f) frames.push_back(f);
+        rc = refit_bodies(ctx, who, a.in, s->params, s->final_loss, frames, &pose_cfg, opt_cfg, pose_stats, st);
     }
     return rc;
 }
@@ -1835,29 +1873,14 @@ extern "C" int mvs_debug_shape_closure(mvs_ctx* ctx, const mvs_sequence_stream* 
     static const char* who = "mvs_debug_shape_closure";
     const cudaStream_t st = (cudaStream_t)stream;
     LossParams lp;
-    std::vector<int> off;
-    ShapeArgs a0;
+    ProblemSet ps;
+    ShapeArgs a;
     int rc = check_seq_stream(ctx, who, s, gt_xyz, conf3d, rig_dev, st);
     if (!rc && (!rows_dev || !loss_dev || !grad_dev)) rc = set_error(ctx, MVS_ERR_INVALID, "%s: NULL argument", who);
-    if (!rc) rc = shape_prepare(ctx, who, s, gt_xyz, conf3d, rig_dev, stage, 100, &lp, &off, &a0, st);
-    if (!rc) rc = ensure_state(ctx, ctx->lbfgs ? ctx->lbfgs->H : 100);
+    if (!rc) rc = shape_prepare(ctx, who, s, gt_xyz, conf3d, rig_dev, stage, 100, &lp, &ps, &a, st);
     if (rc) return rc;
-    const int NS = s->n_sequences, B = ctx->ws.B;
-    const std::vector<int> ok((size_t)NS, 1);
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(ctx->sstream->rows.p, rows_dev, (size_t)NS * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    for (int base = 0; base < NS && !rc; base += B) {
-        const int n = std::min(B, NS - base);
-        if ((rc = shape_chunk_start(ctx, base, n, ok, st))) break;
-        const LbfgsState& S = *ctx->lbfgs;
-        if ((rc = launch_shape_closure(ctx, shape_chunk_args(a0, off, base, n), lp, S, st))) break;
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(loss_dev + base, S.loss_eval, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(grad_dev + (size_t)base * kParams, S.g_eval, (size_t)n * kParams * sizeof(float),
-                                         cudaMemcpyDeviceToDevice, st));
-    }
-    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(ctx->ws.fidx, B, ctx->ws.na));
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    MVS_CUDA_OK(ctx, cudaGetLastError());
-    return rc;
+    const ChunkClosure closure = [&](const ProblemChunk& c, const LbfgsState& S) { return launch_shape_closure(ctx, a, c, lp, S, st); };
+    return eval_problems(ctx, ps, closure, rows_dev, loss_dev, grad_dev, st);
 }
 
 // mvs_debug_camera_closure (tests/test_gpu_camera_refine.py): the camera closure of mvs_refine_cameras evaluated once, with the
@@ -1877,31 +1900,16 @@ extern "C" int mvs_debug_camera_closure(mvs_ctx* ctx, const mvs_frame_stream* s,
     CameraPlan plan;
     if (!rc) rc = camera_plan(ctx, s, rig_dev, &plan, st);
     if (rc) return rc;
-    const int P = (int)plan.prob.size(), B = ctx->ws.B;
+    const int P = (int)plan.prob.size();
     *n_prob = P;
     for (int p = 0; p < P && prob_host; ++p) { prob_host[2 * p] = plan.prob[p].rig; prob_host[2 * p + 1] = plan.prob[p].view; }
     if (!rows_dev || P == 0) return MVS_OK;
-    if ((rc = ensure_state(ctx, ctx->lbfgs ? ctx->lbfgs->H : 100))) return rc;
-    SeqState& h = *ctx->sstream;
-    const CameraArgs a0 = camera_args(ctx, s, rig_dev);
-    if ((rc = launch_camera_joints(ctx, a0.in, s->params, h.body.p, (int)plan.body.size(), lp, h.held.p, st)) ||
+    const CameraArgs a = camera_args(ctx, FrameInputs{s->n_frames, s->gt_uv, s->conf, s->joint_weights, s->gt_xyz, s->conf3d, rig_dev});
+    if ((rc = launch_camera_joints(ctx, a.in, s->params, ctx->sstream->body.p, (int)plan.body.size(), lp, ctx->sstream->held.p, st)) ||
         (rc = camera_refs(ctx, plan, st)))
         return rc;
-    MVS_CUDA_OK(ctx, cudaMemcpyAsync(h.rows.p, rows_dev, (size_t)P * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    const std::vector<int> ok((size_t)P, 1);
-    for (int base = 0; base < P && !rc; base += B) {
-        const int n = std::min(B, P - base);
-        if ((rc = shape_chunk_start(ctx, base, n, ok, st))) break;
-        const LbfgsState& S = *ctx->lbfgs;
-        if ((rc = launch_camera_closure(ctx, camera_chunk_args(a0, plan, base, n), lp, S, st))) break;
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(loss_dev + base, S.loss_eval, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        MVS_CUDA_OK(ctx, cudaMemcpyAsync(grad_dev + (size_t)base * kParams, S.g_eval, (size_t)n * kParams * sizeof(float),
-                                         cudaMemcpyDeviceToDevice, st));
-    }
-    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(ctx->ws.fidx, B, ctx->ws.na));
-    MVS_CUDA_OK(ctx, cudaStreamSynchronize(st));
-    MVS_CUDA_OK(ctx, cudaGetLastError());
-    return rc;
+    const ChunkClosure closure = [&](const ProblemChunk& c, const LbfgsState& S) { return launch_camera_closure(ctx, a, c, lp, S, st); };
+    return eval_problems(ctx, plan.ps, closure, rows_dev, loss_dev, grad_dev, st);
 }
 
 }  // extern "C"

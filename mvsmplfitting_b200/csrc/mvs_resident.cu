@@ -79,17 +79,17 @@ closure_resident_kernel(ResidentModel m, RigSet rigs, LossParams lp, const float
         for (int i = threadIdx.x; i < kParams; i += kResThreads) grad_out[(size_t)b * kParams + i] = S.lg_new[i];
 }
 
-// The shape step of mvs_fit_shared_shape: ONE CTA per frame of the sequences in the optimiser's slots (sequence a.base + j in
-// slot j).  The frame's row with its sequence's shared entries (betas, and scale with a.share_scale) taken from the slot's
-// x_eval, evaluated by resident_closure under the stage lp; loss and gradient go to the per-frame scratch.
+// The shape step of mvs_fit_shared_shape: ONE CTA per frame of chunk c (its sequence's problem in slot j).  The frame's row with
+// its sequence's shared entries (betas, and scale with a.share_scale) taken from the slot's x_eval, evaluated by resident_closure
+// under the stage lp; its part row: the loss, the betas' gradient, then scale's.
 __device__ __forceinline__ bool shape_shared(int i, int share_scale) { return i < kOffOrient || (share_scale && i == kOffScale); }
 
 __global__ void __launch_bounds__(kResThreads, 2)
-shape_closure_kernel(ResidentModel m, RigSet rigs, LossParams lp, LbfgsState L, ShapeArgs a) {
+shape_closure_kernel(ResidentModel m, RigSet rigs, LossParams lp, LbfgsState L, ShapeArgs a, ProblemChunk c) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     ResidentSmem& S = *reinterpret_cast<ResidentSmem*>(smem_raw);
-    const int f = a.f0 + blockIdx.x;
-    const int j = a.seq_of[f] - a.base;
+    const int f = c.i0 + blockIdx.x;
+    const int j = c.item_of[f] - c.base;
     if (L.sc[j].phase == PH_DONE) return;                               // the sequence's problem has finished
     const FrameRig rig = frame_rig(rigs, f);
     resident_setup(S, m);
@@ -98,28 +98,9 @@ shape_closure_kernel(ResidentModel m, RigSet rigs, LossParams lp, LbfgsState L, 
     __syncthreads();
     VposerSmem* W = lp.use_vposer == 2 ? reinterpret_cast<VposerSmem*>(smem_raw + sizeof(ResidentSmem)) : nullptr;
     resident_closure(S, m, rig, lp, a.in.gt_uv, a.in.conf, a.in.joint_w, a.in.n, f, true, nullptr, nullptr, DenseIn{}, W);
-    if (threadIdx.x == 0) a.loss[f] = S.sc[2];
-    for (int i = threadIdx.x; i < kParams; i += kResThreads) a.grad[(size_t)f * kParams + i] = S.lg_new[i];
-}
-
-// Per sequence (one warp, block j = slot j): the frames' losses and shared gradient entries added in double, in frame order,
-// into the slot's loss_eval / g_eval (zeros outside the shared entries).  The order depends on the sequence only.
-__global__ void __launch_bounds__(kResThreads, 2)
-shape_reduce_kernel(LbfgsState L, ShapeArgs a) {
-    const int j = blockIdx.x, lane = threadIdx.x;
-    if (L.sc[j].phase == PH_DONE) return;
-    const int q = a.base + j, f0 = a.off[q], f1 = a.off[q + 1];
-    // lane 0..9: betas, lane 10: scale, lane 11: the loss
-    const int e = lane < kOffOrient ? lane : lane == kOffOrient ? kOffScale : -1;
-    const bool on = lane == kOffOrient + 1 || (e >= 0 && shape_shared(e, a.share_scale));
-    double acc = 0.0;
-    if (on)
-        for (int f = f0; f < f1; ++f) acc += e >= 0 ? (double)a.grad[(size_t)f * kParams + e] : (double)a.loss[f];
-    float* g = L.g_eval + (size_t)j * kParams;
-    for (int i = lane; i < kParams; i += 32)
-        if (!shape_shared(i, a.share_scale)) g[i] = 0.f;
-    if (e >= 0 && on) g[e] = (float)acc;
-    if (lane == kOffOrient + 1) L.loss_eval[j] = (float)acc;
+    float* row = c.part + (size_t)f * kPartCols;
+    if (threadIdx.x == 0) row[0] = S.sc[2];
+    if (threadIdx.x <= kOffOrient) row[1 + threadIdx.x] = S.lg_new[threadIdx.x < kOffOrient ? threadIdx.x : kOffScale];
 }
 
 // The held keypoints of mvs_refine_cameras: ONE CTA per frame of `frames`, resident_closure's joints output (the keypoints the
@@ -391,13 +372,13 @@ int launch_closure_resident(mvs_ctx* ctx, const float* x_dev, float* loss_dev, f
     return MVS_OK;
 }
 
-int launch_shape_closure(mvs_ctx* ctx, const ShapeArgs& a, const LossParams& lp, const LbfgsState& L, cudaStream_t st) {
+int launch_shape_closure(mvs_ctx* ctx, const ShapeArgs& a, const ProblemChunk& c, const LossParams& lp, const LbfgsState& L,
+                         cudaStream_t st) {
     const size_t smem = sizeof(ResidentSmem) + (lp.use_vposer == 2 ? sizeof(VposerSmem) : 0);
     ResidentModel rm = make_resident_model(ctx);
     rm.j3d_xyz = a.in.j3d_xyz; rm.j3d_conf = a.in.j3d_conf;           // row stride a.in.n, as gt_uv / conf
     MVS_LAUNCH(ctx, KID_RESIDENT_CLOSURE, st,
-               shape_closure_kernel<<<a.nf, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev.p, a.in.rig}, lp, L, a));
-    MVS_LAUNCH(ctx, KID_MISC, st, shape_reduce_kernel<<<a.n, 32, 0, st>>>(L, a));
+               shape_closure_kernel<<<c.ni, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev.p, a.in.rig}, lp, L, a, c));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }

@@ -342,8 +342,8 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
     camera extrinsics from them (before shared_shape when both are given), see refine_rigs; the refined rigs go into stats and,
     with result_folder, into cameras_rig<r>.txt there.
     Returns (params [F,86] numpy -- pose slot = latent code under VPoser --, final_loss [F], stats)."""
-    _check_shared_shape(shared_shape, None)
-    _check_refine_cameras(refine_cameras, None)
+    _check_sweeps("shared_shape", shared_shape, None, "the shared shape's pose step")
+    _check_sweeps("refine_cameras", refine_cameras, None, "the camera refinement's body step")
     F = len(seq["frames"])
     assert ctx.B <= F, "context batch %d > frames %d" % (ctx.B, F)
     latent = _uses_latent_pose(stage_cfgs)
@@ -435,20 +435,13 @@ def _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, fac
         _export(ctx, seq, chunk, lc, latent, result_folder, mesh_folder, faces, frames=seq["frames"][c0:c0 + n], rows=range(n))
 
 
-def _check_shared_shape(shared_shape, temporal_weight) -> None:
-    if isinstance(shared_shape, bool) or int(shared_shape) != shared_shape or shared_shape < 0:
-        raise ValueError("shared_shape: want a number of sweeps >= 0 (0: off), got %r" % (shared_shape,))
-    if shared_shape and temporal_weight is not None:
-        raise ValueError("shared_shape and temporal_weight do not combine: the shared shape's pose step fits frames "
-                         "independently, so the causal temporal term cannot be honoured")
-
-
-def _check_refine_cameras(refine_cameras, temporal_weight) -> None:
-    if isinstance(refine_cameras, bool) or int(refine_cameras) != refine_cameras or refine_cameras < 0:
-        raise ValueError("refine_cameras: want a number of sweeps >= 0 (0: off), got %r" % (refine_cameras,))
-    if refine_cameras and temporal_weight is not None:
-        raise ValueError("refine_cameras and temporal_weight do not combine: the camera refinement's body step fits frames "
-                         "independently, so the causal temporal term cannot be honoured")
+def _check_sweeps(option, sweeps, temporal_weight, step) -> None:
+    """option: shared_shape or refine_cameras, a number of sweeps; step: the part of it that fits frames independently"""
+    if isinstance(sweeps, bool) or int(sweeps) != sweeps or sweeps < 0:
+        raise ValueError("%s: want a number of sweeps >= 0 (0: off), got %r" % (option, sweeps))
+    if sweeps and temporal_weight is not None:
+        raise ValueError("%s and temporal_weight do not combine: %s fits frames independently, so the causal temporal term "
+                         "cannot be honoured" % (option, step))
 
 
 def refine_rigs(ctx, params, gt_uv, conf, jw, stage_cfgs, opt_cfg, sweeps, t3=None, rig=None, stats=None, result_folder=None):
@@ -533,8 +526,8 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
     refined rigs go into stats['refine_cameras'] and, with result_folder, into cameras_rig<r>.txt there.  The context keeps
     the refined cameras.  It does not combine with temporal_weight (ValueError).
     Returns a list (per sequence) of (params [T_s,86], loss [T_s]) and the summed stats."""
-    _check_shared_shape(shared_shape, temporal_weight)
-    _check_refine_cameras(refine_cameras, temporal_weight)
+    _check_sweeps("shared_shape", shared_shape, temporal_weight, "the shared shape's pose step")
+    _check_sweeps("refine_cameras", refine_cameras, temporal_weight, "the camera refinement's body step")
     S_ = len(seqs)
     tw = temporal_weight_vector(temporal_weight)
     latent = _uses_latent_pose(stage_cfgs)
