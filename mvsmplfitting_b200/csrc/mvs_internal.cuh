@@ -458,15 +458,15 @@ bool dense_supported(const mvs_ctx* ctx);      // the mesh fits frame_step's lis
 int launch_vposer_decode(mvs_ctx* ctx, const float* x_dev, float* body_pose_dev, cudaStream_t st);
 int launch_closure_resident(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev,
                             float* proj_dev, cudaStream_t st);
-int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
-                          const LossParams* lp_tab_host, int nstages, FrameScalars* frame_scalars_out, float* last_grad_dev,
-                          cudaStream_t st, const int2* stage_rng_dev, const FrameInputs* frames = nullptr);
+// The frame-resident optimiser over the nstages stages of the run's table (ctx->lbfgs->lp_tab, as begin_run filled it): one
+// CTA per frame of frames, rows params_dev [frames.n][86]; each frame's scalars to frame_scalars_out [frames.n]
+int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int nstages, const FrameInputs& frames,
+                          FrameScalars* frame_scalars_out, float* last_grad_dev, const int2* stage_rng_dev, cudaStream_t st);
 // the chaining run of mvs_fit_seq_stream in the frame-resident regime: one CTA per sequence of q.act.  temporal_w [F][86]
 // (mvs_fit_seq_stream_temporal; NULL: term off) are the anchor weights of the warm stages, whose anchor row is the
 // predecessor's fitted row of params_dev
-int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int history, const LossParams* lp_tab_dev,
-                              const LossParams* lp_tab_host, int nstages, const FrameInputs& frames, const SeqChain& q,
-                              cudaStream_t st, const float* temporal_w = nullptr);
+int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int nstages, const FrameInputs& frames,
+                              const SeqChain& q, cudaStream_t st, const float* temporal_w = nullptr);
 // the shape closure of mvs_fit_shared_shape: the part rows of chunk c's frames (loss, betas, scale); frames whose problem is
 // done are skipped
 int launch_shape_closure(mvs_ctx* ctx, const ShapeArgs& a, const ProblemChunk& c, const LossParams& lp, const LbfgsState& L,

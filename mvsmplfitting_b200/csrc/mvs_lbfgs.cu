@@ -43,19 +43,13 @@ __device__ __forceinline__ void init_frame_state(const LbfgsState& S, const floa
     VLOOP(i) S.x_eval[(size_t)b * kParams + i] = x[i];
     if (lane == 0) {
         FrameScalars s;
-        if (reset) {
-            memset(&s, 0, sizeof(s));
-            s.H_diag = 1.f;
+        if (reset) {                                        // this frame's slice of the stage table (mvs_fit_seq)
+            s = fresh_frame_scalars(stage_rng ? stage_rng[b] : make_int2(0, nstages));
         } else {
             s = S.sc[b];
             s.outer_n = 0; s.have_prev = 0; s.nan_flag = 0; s.iters = 0; s.evals = 0;
-        }
-        s.phase = PH_STEP_ENTRY;
-        s.final_loss = __int_as_float(0x7fc00000);
-        if (reset) {                                        // this frame's slice of the stage table (mvs_fit_seq)
-            s.stage = stage_rng ? stage_rng[b].x : 0;
-            s.stage_end = stage_rng ? stage_rng[b].y : nstages;
-            if (s.stage >= s.stage_end) s.phase = PH_DONE;  // no stage of this run is for this frame
+            s.phase = PH_STEP_ENTRY;
+            s.final_loss = __int_as_float(0x7fc00000);
         }
         S.sc[b] = s;
     }
@@ -126,11 +120,11 @@ __global__ void __launch_bounds__(1024) lbfgs_compact_kernel(LbfgsState S, int B
     if (tid == 0) *na = base;
 }
 
-__global__ void lbfgs_finalize_kernel(LbfgsState S, int B, float* __restrict__ final_loss, long long* __restrict__ totals,
-                                      int max_evals_as_rounds) {
+__global__ void lbfgs_finalize_kernel(const FrameScalars* __restrict__ sc, int B, float* __restrict__ final_loss,
+                                      long long* __restrict__ totals, int max_evals_as_rounds) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
-    const FrameScalars s = S.sc[b];
+    const FrameScalars s = sc[b];
     if (final_loss) final_loss[b] = s.final_loss;
     add_frame_totals(totals, s);
     if (max_evals_as_rounds) atomicMax((unsigned long long*)&totals[3], (unsigned long long)s.evals);
@@ -435,7 +429,7 @@ static int run_dense(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int n
     const int chunk = 8;
     // (a lane of a sequence stream may carry every frame of the call)
     const long long frames_per_lane = !la ? 1 : la->q.off ? la->F + 1 : (la->F + B - 1) / B + 1;
-    const long long max_rounds = ((long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8) * nst * frames_per_lane;
+    const long long max_rounds = stage_eval_cap(cfg) * nst * frames_per_lane;
     long long rounds = 0;
     int na_host = B;
     static const bool trace_na = getenv("MVS_TRACE_NA") != nullptr;       // debugging aid: active-list size per chunk
@@ -503,7 +497,7 @@ static int run_batched(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, boo
     Workspace& w = ctx->ws;
     const int B = w.B;
     const int chunk = 8;
-    const long long max_rounds = (long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8;
+    const long long max_rounds = stage_eval_cap(cfg);
     long long rounds = 0;
     int na_host = B;
     const bool resident = resident_closure_applies(ctx, false);     // (not the dense-round closure: it restarts the optimiser)
@@ -540,18 +534,26 @@ static int read_totals(mvs_ctx* ctx, const long long* rounds_dev, bool dense, mv
     return MVS_OK;
 }
 
-// End of a run: final losses and totals.  The frame-resident kernel wrote the last gradient itself and leaves the active
-// list alone; the round-based regimes copy the gradient and leave the context usable for plain closures (full active list).
-// The dense and frame-resident regimes report the largest per-frame evaluation count (the critical path) as rounds.
+// End of a run of regime rg over n frames whose scalars are sc: their final losses (final_loss_dev [n], or NULL), and the
+// run's totals added to stats.  The dense and frame-resident regimes report the largest per-frame evaluation count (the
+// critical path) as rounds.
+static int finish_run(mvs_ctx* ctx, Regime rg, const FrameScalars* sc, int n, float* final_loss_dev, mvs_lbfgs_stats* stats,
+                      cudaStream_t st) {
+    MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_finalize_kernel<<<(n + 255) / 256, 256, 0, st>>>(sc, n, final_loss_dev, ctx->lbfgs->totals,
+                                                                                         rg != kBatched));
+    return read_totals(ctx, nullptr, rg == kDense, stats, st);
+}
+
+// End of a round-based run (batched chain, dense rounds): the gradient at the last evaluated point, the context left usable
+// for plain closures (full active list), then finish_run over the slots
 static int end_run(mvs_ctx* ctx, Regime rg, float* final_loss_dev, float* last_grad_dev, mvs_lbfgs_stats* stats, cudaStream_t st) {
     LbfgsState& S = *ctx->lbfgs;
     Workspace& w = ctx->ws;
     const int B = w.B;
-    MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_finalize_kernel<<<(B + 255) / 256, 256, 0, st>>>(S, B, final_loss_dev, S.totals, rg != kBatched));
-    if (rg != kResident && last_grad_dev)
+    if (last_grad_dev)
         MVS_CUDA_OK(ctx, cudaMemcpyAsync(last_grad_dev, S.g_eval, (size_t)B * kParams * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    if (rg != kResident) MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
-    return read_totals(ctx, nullptr, rg == kDense, stats, st);
+    MVS_LAUNCH(ctx, KID_MISC, st, iota2_kernel<<<(B + 255) / 256, 256, 0, st>>>(w.fidx, B, w.na));
+    return finish_run(ctx, rg, S.sc, B, final_loss_dev, stats, st);
 }
 
 // Runs the stages o.lps[0 .. o.nst) (default: ctx->loss).  nst > 1 requires that all of them run in the same regime
@@ -568,9 +570,11 @@ static int run_stage(mvs_ctx* ctx, float* params_dev, float* final_loss_dev, con
     const int B = w.B;
     const Regime rg = stage_regime(ctx, ctx->loss, cfg.history, o.step);
     if (rg == kResident) {
-        // sparse regime: every frame runs its whole stage inside one CTA (mvs_resident.cu): one launch, no rounds
-        rc = launch_lbfgs_resident(ctx, params_dev, cfg, cfg.history, S.lp_tab, lps, nst, S.sc, o.last_grad, st, o.stage_rng);
-        return rc ? rc : end_run(ctx, kResident, final_loss_dev, nullptr, stats, st);
+        // sparse regime: every frame runs its whole stage inside one CTA (mvs_resident.cu): one launch, no rounds; the kernel
+        // writes the last gradient itself and leaves the active list alone
+        const FrameInputs in{B, w.gt_uv, w.conf, w.joint_w, w.j3d_xyz, w.j3d_conf, ctx->slot_rigs};
+        rc = launch_lbfgs_resident(ctx, params_dev, cfg, nst, in, S.sc, o.last_grad, o.stage_rng, st);
+        return rc ? rc : finish_run(ctx, kResident, S.sc, B, final_loss_dev, stats, st);
     }
     // use_vposer = 2 (VPoser decode on the device) exists in the frame-resident closure and in the dense-regime kernels, not in
     // the SIMT reference chain.  mvs_lbfgs_step therefore runs its one step() per call through the dense rounds when the SDF
@@ -832,15 +836,10 @@ static int run_stream_group(mvs_ctx* ctx, const mvs_frame_stream* s, const int* 
     const int F = s->n_frames;
     if (rg == kResident) {
         // one launch over all F frames, one CTA each: the block scheduler refills the SMs as frames finish
-        LbfgsState& S = *ctx->lbfgs;
         FrameScalars* sc = ctx->fstream->sc.p;
         const FrameInputs in{F, s->gt_uv, s->conf, s->joint_weights, s->gt_xyz, s->conf3d, rig};
-        if ((rc = launch_lbfgs_resident(ctx, s->params, cfg, cfg.history, S.lp_tab, lps, nst, sc, nullptr, st, nullptr, &in)))
-            return rc;
-        LbfgsState Sf = S;
-        Sf.sc = sc;
-        MVS_LAUNCH(ctx, KID_MISC, st, lbfgs_finalize_kernel<<<(F + 255) / 256, 256, 0, st>>>(Sf, F, s->final_loss, S.totals, 1));
-        return read_totals(ctx, nullptr, false, stats, st);
+        rc = launch_lbfgs_resident(ctx, s->params, cfg, nst, in, sc, nullptr, nullptr, st);
+        return rc ? rc : finish_run(ctx, kResident, sc, F, s->final_loss, stats, st);
     }
     LaneArgs a{};
     a.F = F; a.n_queue = F;
@@ -999,8 +998,7 @@ static int run_seq_chain(mvs_ctx* ctx, const mvs_sequence_stream* s, const Frame
     q.totals = S.totals;
     if (rg == kResident) {
         // one launch, one CTA per sequence; rounds: the largest number of evaluations one CTA ran (its frames' sum)
-        if ((rc = launch_lbfgs_resident_seq(ctx, s->params, cfg, cfg.history, S.lp_tab, tab.data(), nst, in, q, st,
-                                            temporal ? ctx->sstream->tw.p : nullptr)))
+        if ((rc = launch_lbfgs_resident_seq(ctx, s->params, cfg, nst, in, q, st, temporal ? ctx->sstream->tw.p : nullptr)))
             return rc;
         return read_totals(ctx, nullptr, false, stats, st);
     }

@@ -25,11 +25,12 @@ struct FrameScalars {
     long long iters, evals;
 };
 
-// A frame starting on its slice rng = [first, end) of the stage table, with a fresh optimiser
+// A frame starting on its slice rng = [first, end) of the stage table, with a fresh optimiser; an empty slice: the frame has
+// no stage in this run and is done at once (its parameters stay)
 __device__ __forceinline__ FrameScalars fresh_frame_scalars(int2 rng) {
     FrameScalars s;
     memset(&s, 0, sizeof(s));
-    s.phase = PH_STEP_ENTRY;
+    s.phase = rng.x < rng.y ? PH_STEP_ENTRY : PH_DONE;
     s.H_diag = 1.f;
     s.final_loss = __int_as_float(0x7fc00000);
     s.stage = rng.x; s.stage_end = rng.y;
@@ -40,14 +41,9 @@ __device__ __forceinline__ FrameScalars fresh_frame_scalars(int2 rng) {
 // builds one optimiser per stage, fitting.py / fit_single_frame) and the parameters it has: frames are independent
 // problems, so nothing makes a fast frame wait for the slowest one at a stage boundary.
 __device__ __forceinline__ void next_stage_scalars(FrameScalars& s) {
-    const long long it = s.iters, ev = s.evals;
-    const int st = s.stage + 1, nacc = s.nan_acc + s.nan_flag, end = s.stage_end;
-    memset(&s, 0, sizeof(s));
-    s.stage_end = end;
-    s.H_diag = 1.f;
-    s.phase = PH_STEP_ENTRY;
-    s.final_loss = __int_as_float(0x7fc00000);
-    s.iters = it; s.evals = ev; s.stage = st; s.nan_acc = nacc;
+    FrameScalars n = fresh_frame_scalars(make_int2(s.stage + 1, s.stage_end));
+    n.iters = s.iters; n.evals = s.evals; n.nan_acc = s.nan_acc + s.nan_flag;
+    s = n;
 }
 
 // A retiring frame's iterations, evaluations and NaN / Inf stops, added to totals[0 .. 2]
@@ -102,6 +98,22 @@ __device__ __forceinline__ float vabsmax(const float* a, int lane) {
     float p = 0.f;
     VLOOP(i) p = fmaxf(p, fabsf(a[i]));
     return warp_max(p);
+}
+
+// Hard bound on one frame's closure evaluations in one stage (never reached by a terminating line search; a guard against
+// hanging the GPU): every outer step costs at most 1 + max_eval + max_iter evaluations
+__host__ __device__ __forceinline__ long long stage_eval_cap(const LbfgsCfg& cfg) {
+    return (long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8;
+}
+
+// After an optimiser step of one warp: a frame that is done and has another stage in its slice moves on to it, its next
+// evaluation at the parameters it has (x_eval <- x)
+__device__ __forceinline__ void advance_stage_if_done(FrameScalars& s, float* x_eval, const float* x, int lane) {
+    if (s.phase == PH_DONE && s.stage + 1 < s.stage_end) {
+        next_stage_scalars(s);
+        VLOOP(i) x_eval[i] = x[i];
+        __syncwarp();
+    }
 }
 
 // lbfgs_ls.py:11-36.  Python's min(max(pos, lo), hi) keeps `pos` when a comparison with NaN fails.

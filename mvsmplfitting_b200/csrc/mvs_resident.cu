@@ -149,13 +149,7 @@ lbfgs_resident_kernel(ResidentModel m, RigSet rigs, const LossParams* __restrict
     // this frame's slice of the stage table (all of it unless the run mixes cold and warm-started frames, mvs_fit_seq)
     const int st_begin = stage_rng ? stage_rng[b].x : 0, st_end = stage_rng ? stage_rng[b].y : nstages;
     if (st_begin >= st_end) {                                            // nothing to do in this run: parameters stay
-        if (t == 0) {
-            FrameScalars s;
-            memset(&s, 0, sizeof(s));
-            s.phase = PH_DONE;
-            s.final_loss = __int_as_float(0x7fc00000);
-            sc_out[b] = s;
-        }
+        if (t == 0) sc_out[b] = fresh_frame_scalars(make_int2(st_begin, st_end));
         return;
     }
     const FrameRig rig = frame_rig(rigs, b);
@@ -166,9 +160,7 @@ lbfgs_resident_kernel(ResidentModel m, RigSet rigs, const LossParams* __restrict
     __syncthreads();
     LbfgsPtrs P{S.lx, S.lg, S.ld, S.lprev_g, S.lx_init, S.lg_prev, S.lbg0, S.lbg1, hy, hs, S.ro, S.al, S.lx_eval, S.lg_new, H,
                 S.gram, S.tl_scratch};
-    // hard bound on closure evaluations per frame and stage (never reached by a terminating line search; a guard
-    // against hanging the GPU): every outer step costs at most 1 + max_eval + max_iter evaluations
-    const long long eval_cap = (long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8;
+    const long long eval_cap = stage_eval_cap(cfg);
     long long stage_ev0 = 0;
     int cur_stage = st_begin;
     while (true) {
@@ -182,10 +174,7 @@ lbfgs_resident_kernel(ResidentModel m, RigSet rigs, const LossParams* __restrict
             FrameScalars s = S.fs;
             lbfgs_advance_core(s, P, S.sc[2], cfg, lane, S.lp.use_vposer == 2 ? 32 : kOffTransl - kOffPose);
             if (s.evals - stage_ev0 >= eval_cap && s.phase != PH_DONE) { s.phase = PH_DONE; s.nan_flag = 1; }
-            if (s.phase == PH_DONE && s.stage + 1 < s.stage_end) {      // this frame moves on to its next stage
-                next_stage_scalars(s);
-                VLOOP(i) S.lx_eval[i] = S.lx[i];
-            }
+            advance_stage_if_done(s, S.lx_eval, S.lx, lane);
             if (lane == 0) S.fs = s;
         }
         __syncthreads();
@@ -210,7 +199,8 @@ lbfgs_resident_kernel(ResidentModel m, RigSet rigs, const LossParams* __restrict
 // per-frame optimisation for each of its frames in turn, from its pending frame q.cur[seq] (cold) on.  After a frame it
 // writes the frame's parameters, final loss and counts, then starts the successor with a fresh optimiser: warm from the
 // fitted row in shared memory, cold from the successor's own row -- or, with q.park, leaves a cold successor to the next
-// pass.  B = F: the inputs' row stride.  Kept apart from lbfgs_resident_kernel so that kernel's code stays as it is.
+// pass.  B = F: the inputs' row stride.  A kernel of its own so that the sequence walk stays out of lbfgs_resident_kernel's
+// registers.  Its stage loop repeats lbfgs_resident_kernel's: shared as one inlined function, it cost that kernel 20 B of spills.
 __global__ void __launch_bounds__(kResThreads, 2)
 lbfgs_resident_seq_kernel(ResidentModel m, RigSet rigs, const LossParams* __restrict__ lp_tab, LbfgsCfg cfg,
                           float* __restrict__ params, const float* __restrict__ gt_uv, const float* __restrict__ conf,
@@ -230,7 +220,7 @@ lbfgs_resident_seq_kernel(ResidentModel m, RigSet rigs, const LossParams* __rest
     for (int i = t; i < kParams; i += kResThreads) { const float v = params[(size_t)b * kParams + i]; S.lx[i] = v; S.lx_eval[i] = v; }
     LbfgsPtrs P{S.lx, S.lg, S.ld, S.lprev_g, S.lx_init, S.lg_prev, S.lbg0, S.lbg1, hy, hs, S.ro, S.al, S.lx_eval, S.lg_new, H,
                 S.gram, S.tl_scratch};
-    const long long eval_cap = (long long)cfg.max_outer * (cfg.max_eval + cfg.max_iter + 2) + 8;
+    const long long eval_cap = stage_eval_cap(cfg);
     while (true) {                                                       // frames of the sequence
         const FrameRig rig = frame_rig(rigs, b);                         // a sequence's frames may change rig
         if (t == 0) S.fs = fresh_frame_scalars(rng);
@@ -246,10 +236,7 @@ lbfgs_resident_seq_kernel(ResidentModel m, RigSet rigs, const LossParams* __rest
                 FrameScalars s = S.fs;
                 lbfgs_advance_core(s, P, S.sc[2], cfg, lane, S.lp.use_vposer == 2 ? 32 : kOffTransl - kOffPose);
                 if (s.evals - stage_ev0 >= eval_cap && s.phase != PH_DONE) { s.phase = PH_DONE; s.nan_flag = 1; }
-                if (s.phase == PH_DONE && s.stage + 1 < s.stage_end) {
-                    next_stage_scalars(s);
-                    VLOOP(i) S.lx_eval[i] = S.lx[i];
-                }
+                advance_stage_if_done(s, S.lx_eval, S.lx, lane);
                 if (lane == 0) S.fs = s;
             }
             __syncthreads();
@@ -405,43 +392,51 @@ int launch_vposer_decode(mvs_ctx* ctx, const float* x_dev, float* body_pose_dev,
     return MVS_OK;
 }
 
-int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int H, const LossParams* lp_tab_dev,
-                          const LossParams* lph, int nstages, FrameScalars* sc_out, float* last_grad_dev, cudaStream_t st,
-                          const int2* stage_rng_dev, const FrameInputs* frames) {
-    const Workspace& w = ctx->ws;
-    int with_vposer = 0;
-    for (int i = 0; i < nstages; ++i) with_vposer |= (lph[i].use_vposer == 2);
-    const size_t smem = frame_smem(H, with_vposer != 0);
-    const FrameInputs in = frames ? *frames : FrameInputs{w.B, w.gt_uv, w.conf, w.joint_w, w.j3d_xyz, w.j3d_conf, ctx->slot_rigs};
-    ResidentModel rm = make_resident_model(ctx);
-    rm.j3d_xyz = in.j3d_xyz; rm.j3d_conf = in.j3d_conf;
+static int stages_with_vposer(const LbfgsState& L, int nstages) {
+    int v = 0;
+    for (int i = 0; i < nstages; ++i) v |= (L.lp_tab_host[i].use_vposer == 2);
+    return v;
+}
+
+// The launch set-up of the frame-resident optimiser kernels over the frames `in`: the model with in's 3-D target rows (row
+// stride in.n, as gt_uv / conf), in's rigs, and the shared memory of one frame with the run's history (and the VPoser decoder
+// when a stage of the run's table, as begin_run stored it, decodes one)
+struct ResidentLaunch { ResidentModel m; RigSet rigs; int with_vposer; size_t smem; };
+static ResidentLaunch resident_launch(const mvs_ctx* ctx, const FrameInputs& in, int H, int nstages) {
+    ResidentLaunch r;
+    r.m = make_resident_model(ctx);
+    r.m.j3d_xyz = in.j3d_xyz; r.m.j3d_conf = in.j3d_conf;
+    r.rigs = RigSet{ctx->rigs_dev.p, in.rig};
+    r.with_vposer = stages_with_vposer(*ctx->lbfgs, nstages);
+    r.smem = frame_smem(H, r.with_vposer != 0);
+    return r;
+}
+
+int launch_lbfgs_resident(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int nstages, const FrameInputs& in,
+                          FrameScalars* sc_out, float* last_grad_dev, const int2* stage_rng_dev, cudaStream_t st) {
+    const ResidentLaunch r = resident_launch(ctx, in, cfg.history, nstages);
     MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
-               lbfgs_resident_kernel<<<in.n, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev.p, in.rig}, lp_tab_dev, nstages, cfg, params_dev,
-                                                                      in.gt_uv, in.conf, in.joint_w, in.n, H, sc_out,
-                                                                      last_grad_dev, with_vposer, stage_rng_dev));
+               lbfgs_resident_kernel<<<in.n, kResThreads, r.smem, st>>>(r.m, r.rigs, ctx->lbfgs->lp_tab, nstages, cfg, params_dev,
+                                                                        in.gt_uv, in.conf, in.joint_w, in.n, cfg.history, sc_out,
+                                                                        last_grad_dev, r.with_vposer, stage_rng_dev));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }
 
-int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int H, const LossParams* lp_tab_dev,
-                              const LossParams* lph, int nstages, const FrameInputs& in, const SeqChain& q, cudaStream_t st,
-                              const float* temporal_w) {
-    int with_vposer = 0;
-    for (int i = 0; i < nstages; ++i) with_vposer |= (lph[i].use_vposer == 2);
-    const size_t smem = frame_smem(H, with_vposer != 0);
-    ResidentModel rm = make_resident_model(ctx);
-    rm.j3d_xyz = in.j3d_xyz; rm.j3d_conf = in.j3d_conf;              // row stride in.n, as gt_uv / conf
+int launch_lbfgs_resident_seq(mvs_ctx* ctx, float* params_dev, const LbfgsCfg& cfg, int nstages, const FrameInputs& in,
+                              const SeqChain& q, cudaStream_t st, const float* temporal_w) {
+    ResidentLaunch r = resident_launch(ctx, in, cfg.history, nstages);
     if (temporal_w) {
         // the closure reads frame b's anchor row at anchor + 86 b: here the row of frame b - 1 in params, which the CTA wrote
         // (the frame's fitted row) before the barrier that starts warm frame b.  Cold frames run no anchored stage, so the
         // row before params is never read.
-        rm.anchor = params_dev - kParams;
-        rm.anchor_w = temporal_w;
+        r.m.anchor = params_dev - kParams;
+        r.m.anchor_w = temporal_w;
     }
     MVS_LAUNCH(ctx, KID_RESIDENT_LBFGS, st,
-               lbfgs_resident_seq_kernel<<<q.n_act, kResThreads, smem, st>>>(rm, RigSet{ctx->rigs_dev.p, in.rig}, lp_tab_dev, cfg,
-                                                                             params_dev, in.gt_uv, in.conf, in.joint_w, in.n, H,
-                                                                             with_vposer, q));
+               lbfgs_resident_seq_kernel<<<q.n_act, kResThreads, r.smem, st>>>(r.m, r.rigs, ctx->lbfgs->lp_tab, cfg, params_dev,
+                                                                              in.gt_uv, in.conf, in.joint_w, in.n, cfg.history,
+                                                                              r.with_vposer, q));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }
@@ -456,12 +451,6 @@ int frame_step_begin_run(mvs_ctx* ctx, cudaStream_t st) {
     }
     MVS_CUDA_OK(ctx, cudaMemsetAsync(w.pose_valid, 0, (size_t)w.B * sizeof(int), st));
     return MVS_OK;
-}
-
-static int stages_with_vposer(const LbfgsState& L, int nstages) {
-    int v = 0;
-    for (int i = 0; i < nstages; ++i) v |= (L.lp_tab_host[i].use_vposer == 2);
-    return v;
 }
 
 static FrameStepArgs make_frame_step_args(mvs_ctx* ctx, float* params_dev, const LbfgsState& L, const LbfgsCfg& cfg, int nstages) {

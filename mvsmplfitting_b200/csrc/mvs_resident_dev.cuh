@@ -1050,11 +1050,7 @@ frame_step_kernel(FrameStepArgs a, const int* __restrict__ fidx, const int* __re
                     S.lg_new, L.H, S.gram, S.tl_scratch};
         lbfgs_advance_core(s, P, S.sc[2], cfg, lane, S.lp.use_vposer == 2 ? 32 : kOffTransl - kOffPose);
         __syncwarp();
-        if (s.phase == PH_DONE && s.stage + 1 < s.stage_end) {  // this frame moves on to its next stage
-            next_stage_scalars(s);
-            VLOOP(i) S.lx_eval[i] = S.lx[i];
-            __syncwarp();
-        }
+        advance_stage_if_done(s, S.lx_eval, S.lx, lane);
         VLOOP(i) S.x[i] = S.lx_eval[i];                // the next trial point: input of next_pose_forward
         if (lane == 0) { L.sc[b] = s; S.fs = s; }
     }
