@@ -2,9 +2,11 @@
 // host-side pre-contractions, workspace allocation, and the thin entry points that enqueue the
 // kernels of mvs_closure.cu / mvs_lbfgs.cu / mvs_sdf.cu on the caller's stream.
 #include <algorithm>
+#include <mutex>
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include "mvs_internal.cuh"
@@ -37,12 +39,6 @@ void dev_free(mvs_ctx* ctx, void* p) {
     ctx->allocs.erase(std::find(ctx->allocs.begin(), ctx->allocs.end(), p));
     cudaFree(p);
 }
-template <class T> int dev_upload(mvs_ctx* ctx, T** p, const T* host, size_t count) {
-    int rc = dev_alloc(ctx, p, count);
-    if (rc) return rc;
-    if (count) MVS_CUDA_OK(ctx, cudaMemcpy(*p, host, count * sizeof(T), cudaMemcpyHostToDevice));
-    return MVS_OK;
-}
 template int dev_alloc<unsigned short>(mvs_ctx*, unsigned short**, size_t);
 template int dev_alloc<float>(mvs_ctx*, float**, size_t);
 template int dev_alloc<int>(mvs_ctx*, int**, size_t);
@@ -57,8 +53,99 @@ template int dev_alloc<CamRefine>(mvs_ctx*, CamRefine**, size_t);
 template int dev_alloc<CameraProblem>(mvs_ctx*, CameraProblem**, size_t);
 template int dev_alloc<LossParams>(mvs_ctx*, LossParams**, size_t);
 template int dev_alloc<FrameScalars>(mvs_ctx*, FrameScalars**, size_t);
-template int dev_upload<float>(mvs_ctx*, float**, const float*, size_t);
-template int dev_upload<int>(mvs_ctx*, int**, const int*, size_t);
+
+// ----------------------------------------------------------------------------- model constants shared between contexts
+// Every context of the process that uploads the same constants to the same device (mvs_set_model, mvs_set_gmm_prior,
+// mvs_set_vposer) reads ONE device copy of them.  Several batches in flight, each on its own context, then stream one posedirs
+// table through L2 instead of one each (DESIGN.md section 5), and a context costs ~20 MB less device memory.  An entry is
+// keyed by its device and the exact bytes of its arrays, kept on the host and compared in full, so two different models never
+// alias.  It counts the contexts that hold it; the last one out frees it (mvs_destroy).  Sharing is sound because nothing
+// writes into these arrays after the upload (the const pointers of DevModel).  MVS_SHARE_MODEL=0 in the environment gives
+// every context its own copy (A/B measurements of one build).
+struct ConstArray {
+    const void** dev;                 // where the device pointer goes
+    const void* host;
+    size_t bytes;
+};
+template <class T> static ConstArray const_array(const T*& dev, const T* host, size_t count) {
+    return ConstArray{reinterpret_cast<const void**>(&dev), host, count * sizeof(T)};
+}
+
+struct SharedConsts {
+    int device = 0;
+    int refs = 0;
+    std::vector<size_t> sizes;        // bytes of each array
+    std::vector<char> bytes;          // their contents back to back (shared entries only: the key)
+    std::vector<void*> dev;
+};
+
+static std::mutex g_consts_mu;
+static std::vector<SharedConsts*> g_consts;   // the shared entries of every device
+
+static bool same_consts(const SharedConsts* e, int device, const std::vector<ConstArray>& a) {
+    if (e->device != device || e->sizes.size() != a.size()) return false;
+    for (size_t i = 0; i < a.size(); ++i)
+        if (e->sizes[i] != a[i].bytes) return false;
+    size_t off = 0;
+    for (const ConstArray& x : a) {
+        if (x.bytes && memcmp(e->bytes.data() + off, x.host, x.bytes) != 0) return false;
+        off += x.bytes;
+    }
+    return true;
+}
+
+static void free_consts(SharedConsts* e) {
+    for (void* p : e->dev) cudaFree(p);
+    delete e;
+}
+
+// Points *a[i].dev at a device copy of a[i].host for every i: the shared copy of an entry with the same bytes on ctx's device,
+// else a new upload (inserted into the store unless MVS_SHARE_MODEL=0).  The context holds the entry until mvs_destroy.
+static int upload_consts(mvs_ctx* ctx, const std::vector<ConstArray>& a) {
+    static const bool share = !(getenv("MVS_SHARE_MODEL") && strcmp(getenv("MVS_SHARE_MODEL"), "0") == 0);
+    std::lock_guard<std::mutex> lock(g_consts_mu);
+    SharedConsts* e = nullptr;
+    if (share)
+        for (SharedConsts* s : g_consts)
+            if (same_consts(s, ctx->device, a)) { e = s; break; }
+    if (!e) {
+        e = new SharedConsts();
+        e->device = ctx->device;
+        for (const ConstArray& x : a) {
+            void* d = nullptr;
+            cudaError_t err = cudaMalloc(&d, std::max<size_t>(x.bytes, 1));
+            if (err == cudaSuccess) {
+                e->dev.push_back(d);
+                if (x.bytes) err = cudaMemcpy(d, x.host, x.bytes, cudaMemcpyHostToDevice);
+            }
+            if (err != cudaSuccess) {
+                free_consts(e);
+                return set_error(ctx, MVS_ERR_CUDA, "uploading the model constants failed: %s", cudaGetErrorString(err));
+            }
+            e->sizes.push_back(x.bytes);
+        }
+        if (share) {
+            for (const ConstArray& x : a)
+                e->bytes.insert(e->bytes.end(), (const char*)x.host, (const char*)x.host + x.bytes);
+            g_consts.push_back(e);
+        }
+    }
+    ++e->refs;
+    ctx->consts.push_back(e);
+    for (size_t i = 0; i < a.size(); ++i) *a[i].dev = e->dev[i];
+    return MVS_OK;
+}
+
+// mvs_destroy: drops the context's entries; the last holder of an entry frees its arrays
+static void release_consts(mvs_ctx* ctx) {
+    std::lock_guard<std::mutex> lock(g_consts_mu);
+    for (SharedConsts* e : ctx->consts) {
+        if (--e->refs) continue;
+        g_consts.erase(std::remove(g_consts.begin(), g_consts.end(), e), g_consts.end());
+        free_consts(e);
+    }
+    ctx->consts.clear();
+}
 
 void prof_mark(mvs_ctx* ctx, int kid, cudaStream_t st) {
     Profiler& P = ctx->prof;
@@ -235,6 +322,7 @@ void mvs_destroy(mvs_ctx* ctx) {
     release_fit_state(ctx);
     release_tc_state(ctx);
     for (void* p : ctx->allocs) cudaFree(p);
+    release_consts(ctx);
     delete ctx;
 }
 
@@ -275,149 +363,125 @@ int mvs_set_model(mvs_ctx* ctx, const mvs_model_desc* d) {
     }
 
     // Qk rows: [posedirs column | shapedirs row | v_template | pad]
-    {
-        std::vector<float> Q((size_t)3 * N * kFeatPad, 0.f);
-        for (int col = 0; col < 3 * N; ++col) {
-            float* row = &Q[(size_t)col * kFeatPad];
-            for (int k = 0; k < kPoseBasis; ++k) row[k] = d->posedirs[(size_t)k * 3 * N + col];
-            for (int l = 0; l < kBetas; ++l) row[kPoseBasis + l] = d->shapedirs[(size_t)col * kBetas + l];
-            row[kFeat - 1] = d->v_template[col];
-        }
-        int rc = dev_upload(ctx, &m.Qk, Q.data(), Q.size());
-        if (rc) return rc;
-        if ((rc = tc_upload_model(ctx))) return rc;
-        std::vector<float> stv((size_t)N * 33);
-        for (int n = 0; n < N; ++n)
-            for (int c = 0; c < 3; ++c) {
-                for (int l = 0; l < kBetas; ++l) stv[(size_t)n * 33 + 11 * c + l] = d->shapedirs[((size_t)3 * n + c) * kBetas + l];
-                stv[(size_t)n * 33 + 11 * c + kBetas] = d->v_template[3 * n + c];
-            }
-        if ((rc = dev_upload(ctx, &m.ST, stv.data(), stv.size()))) return rc;
+    std::vector<float> Q((size_t)3 * N * kFeatPad, 0.f);
+    for (int col = 0; col < 3 * N; ++col) {
+        float* row = &Q[(size_t)col * kFeatPad];
+        for (int k = 0; k < kPoseBasis; ++k) row[k] = d->posedirs[(size_t)k * 3 * N + col];
+        for (int l = 0; l < kBetas; ++l) row[kPoseBasis + l] = d->shapedirs[(size_t)col * kBetas + l];
+        row[kFeat - 1] = d->v_template[col];
     }
+    std::vector<float> stv((size_t)N * 33);
+    for (int n = 0; n < N; ++n)
+        for (int c = 0; c < 3; ++c) {
+            for (int l = 0; l < kBetas; ++l) stv[(size_t)n * 33 + 11 * c + l] = d->shapedirs[((size_t)3 * n + c) * kBetas + l];
+            stv[(size_t)n * 33 + 11 * c + kBetas] = d->v_template[3 * n + c];
+        }
     // rest joints pre-contracted through the shape blend shapes (fp64)
-    {
-        std::vector<float> Jt(kJoints * 3), JS(kJoints * 3 * kBetas);
-        for (int j = 0; j < kJoints; ++j)
-            for (int c = 0; c < 3; ++c) {
-                double a = 0.0;
-                double al[kBetas] = {0};
-                for (int n = 0; n < N; ++n) {
-                    const double w = d->J_regressor[(size_t)j * N + n];
-                    if (w == 0.0) continue;
-                    a += w * (double)d->v_template[3 * n + c];
-                    for (int l = 0; l < kBetas; ++l) al[l] += w * (double)d->shapedirs[((size_t)3 * n + c) * kBetas + l];
-                }
-                Jt[3 * j + c] = (float)a;
-                for (int l = 0; l < kBetas; ++l) JS[(3 * j + c) * kBetas + l] = (float)al[l];
+    std::vector<float> Jt(kJoints * 3), JS(kJoints * 3 * kBetas);
+    for (int j = 0; j < kJoints; ++j)
+        for (int c = 0; c < 3; ++c) {
+            double a = 0.0;
+            double al[kBetas] = {0};
+            for (int n = 0; n < N; ++n) {
+                const double w = d->J_regressor[(size_t)j * N + n];
+                if (w == 0.0) continue;
+                a += w * (double)d->v_template[3 * n + c];
+                for (int l = 0; l < kBetas; ++l) al[l] += w * (double)d->shapedirs[((size_t)3 * n + c) * kBetas + l];
             }
-        int rc = dev_upload(ctx, &m.Jt, Jt.data(), Jt.size());
-        if (rc) return rc;
-        rc = dev_upload(ctx, &m.JS, JS.data(), JS.size());
-        if (rc) return rc;
-    }
+            Jt[3 * j + c] = (float)a;
+            for (int l = 0; l < kBetas; ++l) JS[(3 * j + c) * kBetas + l] = (float)al[l];
+        }
     // skinning weights: ELL + dense
-    {
-        int KW = 1;
-        for (int n = 0; n < N; ++n) {
-            int c = 0;
-            for (int j = 0; j < kJoints; ++j) c += d->lbs_weights[(size_t)n * kJoints + j] != 0.f;
-            KW = std::max(KW, c);
-        }
-        m.KW = KW;
-        std::vector<int> ej((size_t)N * KW, 0);
-        std::vector<float> ew((size_t)N * KW, 0.f);
-        for (int n = 0; n < N; ++n) {
-            int c = 0;
-            for (int j = 0; j < kJoints; ++j) {
-                const float w = d->lbs_weights[(size_t)n * kJoints + j];
-                if (w != 0.f) { ej[(size_t)n * KW + c] = j; ew[(size_t)n * KW + c] = w; ++c; }
-            }
-        }
-        int rc = dev_upload(ctx, &m.ell_j, ej.data(), ej.size());
-        if (rc) return rc;
-        rc = dev_upload(ctx, &m.ell_w, ew.data(), ew.size());
-        if (rc) return rc;
-        rc = dev_upload(ctx, &m.Wd, d->lbs_weights, (size_t)N * kJoints);
-        if (rc) return rc;
+    int KW = 1;
+    for (int n = 0; n < N; ++n) {
+        int c = 0;
+        for (int j = 0; j < kJoints; ++j) c += d->lbs_weights[(size_t)n * kJoints + j] != 0.f;
+        KW = std::max(KW, c);
     }
-    if (d->faces && d->n_faces > 0) {
+    m.KW = KW;
+    std::vector<int> ej((size_t)N * KW, 0);
+    std::vector<float> ew((size_t)N * KW, 0.f);
+    for (int n = 0; n < N; ++n) {
+        int c = 0;
+        for (int j = 0; j < kJoints; ++j) {
+            const float w = d->lbs_weights[(size_t)n * kJoints + j];
+            if (w != 0.f) { ej[(size_t)n * KW + c] = j; ew[(size_t)n * KW + c] = w; ++c; }
+        }
+    }
+    if (d->faces && d->n_faces > 0)
         for (int c = 0; c < 3; ++c) m.tri0[c] = d->faces[c];
-        int rc = dev_upload(ctx, &m.faces, d->faces, (size_t)d->n_faces * 3);
-        if (rc) return rc;
-    }
     // keypoint definition
-    {
-        const int K = d->n_keypoints;
-        const int n_src = (d->n_reg > 0 ? d->n_reg : kJoints) + d->n_extra;
-        MVS_REQUIRE(ctx, d->joint_map, "mvs_set_model: joint_map is NULL");
-        MVS_REQUIRE(ctx, d->n_reg == 0 || d->joint_regressor, "mvs_set_model: joint_regressor is NULL");
-        std::vector<int> ptr(K + 1, 0), vidx, chain(K, -1);
-        std::vector<float> wts;
-        for (int k = 0; k < K; ++k) {
-            const int src = d->joint_map[k];
-            MVS_REQUIRE(ctx, src >= 0 && src < n_src, "mvs_set_model: joint_map[%d]=%d out of range", k, src);
-            const int n_first = d->n_reg > 0 ? d->n_reg : kJoints;
-            if (src < n_first) {
-                if (d->n_reg > 0) {
-                    for (int n = 0; n < N; ++n) {
-                        const float w = d->joint_regressor[(size_t)src * N + n];
-                        if (w != 0.f) { vidx.push_back(n); wts.push_back(w); }
-                    }
-                } else {
-                    chain[k] = src;
+    const int K = d->n_keypoints;
+    const int n_src = (d->n_reg > 0 ? d->n_reg : kJoints) + d->n_extra;
+    MVS_REQUIRE(ctx, d->joint_map, "mvs_set_model: joint_map is NULL");
+    MVS_REQUIRE(ctx, d->n_reg == 0 || d->joint_regressor, "mvs_set_model: joint_regressor is NULL");
+    std::vector<int> ptr(K + 1, 0), vidx, chain(K, -1);
+    std::vector<float> wts;
+    for (int k = 0; k < K; ++k) {
+        const int src = d->joint_map[k];
+        MVS_REQUIRE(ctx, src >= 0 && src < n_src, "mvs_set_model: joint_map[%d]=%d out of range", k, src);
+        const int n_first = d->n_reg > 0 ? d->n_reg : kJoints;
+        if (src < n_first) {
+            if (d->n_reg > 0) {
+                for (int n = 0; n < N; ++n) {
+                    const float w = d->joint_regressor[(size_t)src * N + n];
+                    if (w != 0.f) { vidx.push_back(n); wts.push_back(w); }
                 }
             } else {
-                const int v = d->extra_vertex_ids[src - n_first];
-                MVS_REQUIRE(ctx, v >= 0 && v < N, "mvs_set_model: extra vertex id out of range");
-                vidx.push_back(v);
-                wts.push_back(1.f);
+                chain[k] = src;
             }
-            ptr[k + 1] = (int)vidx.size();
+        } else {
+            const int v = d->extra_vertex_ids[src - n_first];
+            MVS_REQUIRE(ctx, v >= 0 && v < N, "mvs_set_model: extra vertex id out of range");
+            vidx.push_back(v);
+            wts.push_back(1.f);
         }
-        std::vector<int> sup(vidx);
-        std::sort(sup.begin(), sup.end());
-        sup.erase(std::unique(sup.begin(), sup.end()), sup.end());
-        const int nsup = (int)sup.size();
-        std::vector<int> spos(vidx.size());
-        for (size_t e = 0; e < vidx.size(); ++e) spos[e] = (int)(std::lower_bound(sup.begin(), sup.end(), vidx[e]) - sup.begin());
-        std::vector<int> sptr(nsup + 1, 0), sk;
-        std::vector<float> swt;
-        for (int i = 0; i < nsup; ++i) {
-            for (int k = 0; k < K; ++k)
-                for (int e = ptr[k]; e < ptr[k + 1]; ++e)
-                    if (vidx[e] == sup[i]) { sk.push_back(k); swt.push_back(wts[e]); }
-            sptr[i + 1] = (int)sk.size();
-        }
-        m.K = K; m.nsup = nsup; m.n_kp_entries = (int)vidx.size();
-        int rc;
-        if ((rc = dev_upload(ctx, &m.kp_ptr, ptr.data(), ptr.size()))) return rc;
-        if ((rc = dev_upload(ctx, &m.kp_vidx, vidx.data(), vidx.size()))) return rc;
-        if ((rc = dev_upload(ctx, &m.kp_spos, spos.data(), spos.size()))) return rc;
-        if ((rc = dev_upload(ctx, &m.kp_w, wts.data(), wts.size()))) return rc;
-        if ((rc = dev_upload(ctx, &m.kp_chain, chain.data(), chain.size()))) return rc;
-        if ((rc = dev_upload(ctx, &m.sup, sup.data(), sup.size()))) return rc;
-        // per joint: which support vertices it skins (adjoint dA_j without atomics in the frame-resident kernel)
-        {
-            std::vector<int> jp(kJoints + 1, 0), ji;
-            std::vector<float> jw;
-            for (int j = 0; j < kJoints; ++j) {
-                for (int i = 0; i < nsup; ++i) {
-                    const float w = d->lbs_weights[(size_t)sup[i] * kJoints + j];
-                    if (w != 0.f) { ji.push_back(i); jw.push_back(w); }
-                }
-                jp[j + 1] = (int)ji.size();
-            }
-            if ((rc = dev_upload(ctx, &m.supj_ptr, jp.data(), jp.size()))) return rc;
-            if ((rc = dev_upload(ctx, &m.supj_i, ji.data(), ji.size()))) return rc;
-            if ((rc = dev_upload(ctx, &m.supj_w, jw.data(), jw.size()))) return rc;
-        }
-        std::vector<int> comb(sup);
-        for (int n = 0; n < N; ++n) comb.push_back(n);
-        if ((rc = dev_upload(ctx, &m.sup_then_all, comb.data(), comb.size()))) return rc;
-        if ((rc = dev_upload(ctx, &m.sup_ptr, sptr.data(), sptr.size()))) return rc;
-        if ((rc = dev_upload(ctx, &m.sup_k, sk.data(), sk.size()))) return rc;
-        if ((rc = dev_upload(ctx, &m.sup_w, swt.data(), swt.size()))) return rc;
+        ptr[k + 1] = (int)vidx.size();
     }
+    std::vector<int> sup(vidx);
+    std::sort(sup.begin(), sup.end());
+    sup.erase(std::unique(sup.begin(), sup.end()), sup.end());
+    const int nsup = (int)sup.size();
+    std::vector<int> spos(vidx.size());
+    for (size_t e = 0; e < vidx.size(); ++e) spos[e] = (int)(std::lower_bound(sup.begin(), sup.end(), vidx[e]) - sup.begin());
+    std::vector<int> sptr(nsup + 1, 0), sk;
+    std::vector<float> swt;
+    for (int i = 0; i < nsup; ++i) {
+        for (int k = 0; k < K; ++k)
+            for (int e = ptr[k]; e < ptr[k + 1]; ++e)
+                if (vidx[e] == sup[i]) { sk.push_back(k); swt.push_back(wts[e]); }
+        sptr[i + 1] = (int)sk.size();
+    }
+    m.K = K; m.nsup = nsup; m.n_kp_entries = (int)vidx.size();
+    // per joint: which support vertices it skins (adjoint dA_j without atomics in the frame-resident kernel)
+    std::vector<int> jp(kJoints + 1, 0), ji;
+    std::vector<float> jw;
+    for (int j = 0; j < kJoints; ++j) {
+        for (int i = 0; i < nsup; ++i) {
+            const float w = d->lbs_weights[(size_t)sup[i] * kJoints + j];
+            if (w != 0.f) { ji.push_back(i); jw.push_back(w); }
+        }
+        jp[j + 1] = (int)ji.size();
+    }
+    std::vector<int> comb(sup);
+    for (int n = 0; n < N; ++n) comb.push_back(n);
+    // the scalars above (N, F, KW, K, nsup, n_kp_entries, tri0) follow from these arrays' sizes and contents, so a context
+    // that finds them in the store has the same scalars as the one that uploaded them
+    std::vector<ConstArray> arrays = {
+        const_array(m.Qk, Q.data(), Q.size()), const_array(m.ST, stv.data(), stv.size()),
+        const_array(m.Jt, Jt.data(), Jt.size()), const_array(m.JS, JS.data(), JS.size()),
+        const_array(m.ell_j, ej.data(), ej.size()), const_array(m.ell_w, ew.data(), ew.size()),
+        const_array(m.Wd, d->lbs_weights, (size_t)N * kJoints),
+        const_array(m.kp_ptr, ptr.data(), ptr.size()), const_array(m.kp_vidx, vidx.data(), vidx.size()),
+        const_array(m.kp_spos, spos.data(), spos.size()), const_array(m.kp_w, wts.data(), wts.size()),
+        const_array(m.kp_chain, chain.data(), chain.size()), const_array(m.sup, sup.data(), sup.size()),
+        const_array(m.supj_ptr, jp.data(), jp.size()), const_array(m.supj_i, ji.data(), ji.size()),
+        const_array(m.supj_w, jw.data(), jw.size()), const_array(m.sup_then_all, comb.data(), comb.size()),
+        const_array(m.sup_ptr, sptr.data(), sptr.size()), const_array(m.sup_k, sk.data(), sk.size()),
+        const_array(m.sup_w, swt.data(), swt.size())};
+    if (d->faces && d->n_faces > 0) arrays.push_back(const_array(m.faces, d->faces, (size_t)d->n_faces * 3));
+    int rc;
+    if ((rc = upload_consts(ctx, arrays)) || (rc = tc_upload_model(ctx))) return rc;
     ctx->have_model = true;
     return MVS_OK;
 }
@@ -438,11 +502,8 @@ int mvs_set_gmm_prior(mvs_ctx* ctx, int M, const float* means, const float* prec
     }
     DevModel& dm = ctx->m;
     dm.M = M;
-    int rc;
-    if ((rc = dev_upload(ctx, &dm.gmm_means, means, (size_t)M * D))) return rc;
-    if ((rc = dev_upload(ctx, &dm.gmm_prec, P.data(), P.size()))) return rc;
-    if ((rc = dev_upload(ctx, &dm.gmm_lognllw, lw.data(), lw.size()))) return rc;
-    return MVS_OK;
+    return upload_consts(ctx, {const_array(dm.gmm_means, means, (size_t)M * D), const_array(dm.gmm_prec, P.data(), P.size()),
+                               const_array(dm.gmm_lognllw, lw.data(), lw.size())});
 }
 
 int mvs_set_vposer(mvs_ctx* ctx, const float* fc1_w, const float* fc1_b, const float* fc2_w, const float* fc2_b,
@@ -452,22 +513,17 @@ int mvs_set_vposer(mvs_ctx* ctx, const float* fc1_w, const float* fc1_b, const f
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     DevModel& m = ctx->m;
     constexpr int H = 512, Z = 32, O = 138;
-    auto up = [&](float** plain, float** transposed, const float* w, int no, int ni) -> int {
+    auto transpose = [](const float* w, int no, int ni) {
         std::vector<float> t((size_t)no * ni);
         for (int o = 0; o < no; ++o)
             for (int i = 0; i < ni; ++i) t[(size_t)i * no + o] = w[(size_t)o * ni + i];
-        int rc = dev_upload(ctx, plain, w, (size_t)no * ni);
-        if (rc) return rc;
-        return dev_upload(ctx, transposed, t.data(), t.size());
+        return t;
     };
-    int rc;
-    if ((rc = up(&m.vp_w1, &m.vp_w1t, fc1_w, H, Z))) return rc;
-    if ((rc = up(&m.vp_w2, &m.vp_w2t, fc2_w, H, H))) return rc;
-    if ((rc = up(&m.vp_w3, &m.vp_w3t, out_w, O, H))) return rc;
-    if ((rc = dev_upload(ctx, &m.vp_b1, fc1_b, H))) return rc;
-    if ((rc = dev_upload(ctx, &m.vp_b2, fc2_b, H))) return rc;
-    if ((rc = dev_upload(ctx, &m.vp_b3, out_b, O))) return rc;
-    return MVS_OK;
+    const std::vector<float> w1t = transpose(fc1_w, H, Z), w2t = transpose(fc2_w, H, H), w3t = transpose(out_w, O, H);
+    return upload_consts(ctx, {const_array(m.vp_w1, fc1_w, (size_t)H * Z), const_array(m.vp_w1t, w1t.data(), w1t.size()),
+                               const_array(m.vp_w2, fc2_w, (size_t)H * H), const_array(m.vp_w2t, w2t.data(), w2t.size()),
+                               const_array(m.vp_w3, out_w, (size_t)O * H), const_array(m.vp_w3t, w3t.data(), w3t.size()),
+                               const_array(m.vp_b1, fc1_b, H), const_array(m.vp_b2, fc2_b, H), const_array(m.vp_b3, out_b, O)});
 }
 
 int mvs_set_camera_rigs(mvs_ctx* ctx, int n_rigs, const int* num_views, const float* R, const float* t, const float* f,

@@ -95,41 +95,44 @@ enum Regime { kResident, kDense, kBatched };
 //                   through lbs.py:179; computed in fp64 at upload)
 //   ell_j/ell_w [N][KW]  skinning weights in ELL form (KW = max non-zeros per vertex, 4 for SMPL)
 //   Wd  [N][24]     dense skinning weights (vertex backward)
+// Read-only after upload: every array here may be shared with other contexts that uploaded the same bytes (upload_consts in
+// mvs_api.cu), so no kernel or host path writes through these pointers; they are const so that the compiler holds to it.
+// The per-call pointers that ride along with them (ResidentModel's anchor / 3-D targets) are swapped, never written through.
 struct DevModel {
     int N = 0, F = 0, KW = 0;
-    float* Qk = nullptr;
-    float* Jt = nullptr;
-    float* JS = nullptr;
-    int* parents = nullptr;
-    int* ell_j = nullptr;
-    float* ell_w = nullptr;
-    float* Wd = nullptr;
-    float* ST = nullptr;      // [N][3][11] shapedirs row | template, fp32 (skinning kernel of the tensor-core path)
-    int* faces = nullptr;
+    const float* Qk = nullptr;
+    const float* Jt = nullptr;
+    const float* JS = nullptr;
+    const int* parents = nullptr;
+    const int* ell_j = nullptr;
+    const float* ell_w = nullptr;
+    const float* Wd = nullptr;
+    const float* ST = nullptr;  // [N][3][11] shapedirs row | template, fp32 (skinning kernel of the tensor-core path)
+    const int* faces = nullptr;
     int tri0[3] = {0, 0, 0};          // vertex ids of face 0 (the triangle the as-written SDF term sees)
     // keypoints: k-th keypoint = sum_e kp_w[e] * v[kp_vidx[e]]  (+ posed chain joint kp_chain[k] if >= 0) + transl
     int K = 0, n_kp_entries = 0, nsup = 0;
-    int* kp_ptr = nullptr;    // [K+1]
-    int* kp_vidx = nullptr;   // vertex id
-    int* kp_spos = nullptr;   // position of that vertex in the support list
-    float* kp_w = nullptr;
-    int* kp_chain = nullptr;  // [K]
-    int* sup = nullptr;       // [nsup] sorted unique vertex ids touched by any keypoint
-    int* sup_then_all = nullptr;  // [nsup + N] the support list followed by 0..N-1 (backward list with the SDF term)
-    int* sup_ptr = nullptr;   // [nsup+1] transposed structure: support vertex -> (keypoint, weight)
-    int* sup_k = nullptr;
-    float* sup_w = nullptr;
-    int* supj_ptr = nullptr;  // [25] per joint: support vertices it skins (frame-resident adjoint)
-    int* supj_i = nullptr;
-    float* supj_w = nullptr;
+    const int* kp_ptr = nullptr;    // [K+1]
+    const int* kp_vidx = nullptr;   // vertex id
+    const int* kp_spos = nullptr;   // position of that vertex in the support list
+    const float* kp_w = nullptr;
+    const int* kp_chain = nullptr;  // [K]
+    const int* sup = nullptr;       // [nsup] sorted unique vertex ids touched by any keypoint
+    const int* sup_then_all = nullptr;  // [nsup + N] the support list followed by 0..N-1 (backward list with the SDF term)
+    const int* sup_ptr = nullptr;   // [nsup+1] transposed structure: support vertex -> (keypoint, weight)
+    const int* sup_k = nullptr;
+    const float* sup_w = nullptr;
+    const int* supj_ptr = nullptr;  // [25] per joint: support vertices it skins (frame-resident adjoint)
+    const int* supj_i = nullptr;
+    const float* supj_w = nullptr;
     // GMM prior
     int M = 0;
-    float* gmm_means = nullptr;     // [M][69]
-    float* gmm_prec = nullptr;      // [M][69][69] symmetrised
-    float* gmm_lognllw = nullptr;   // [M]  log(nll_weights)
+    const float* gmm_means = nullptr;     // [M][69]
+    const float* gmm_prec = nullptr;      // [M][69][69] symmetrised
+    const float* gmm_lognllw = nullptr;   // [M]  log(nll_weights)
     // VPoser decoder (mvs_set_vposer): [out][in] as uploaded and the transposes [in][out] (coalesced mat-vec both ways)
-    float *vp_w1 = nullptr, *vp_w2 = nullptr, *vp_w3 = nullptr, *vp_w1t = nullptr, *vp_w2t = nullptr, *vp_w3t = nullptr;
-    float *vp_b1 = nullptr, *vp_b2 = nullptr, *vp_b3 = nullptr;
+    const float *vp_w1 = nullptr, *vp_w2 = nullptr, *vp_w3 = nullptr, *vp_w1t = nullptr, *vp_w2t = nullptr, *vp_w3t = nullptr;
+    const float *vp_b1 = nullptr, *vp_b2 = nullptr, *vp_b3 = nullptr;
 };
 
 struct FrameBox;
@@ -141,6 +144,7 @@ struct FrameScalars;
 struct TcState;
 struct StreamState;                   // mvs_fit_stream scratch (mvs_lbfgs.cu)
 struct SeqState;                      // mvs_fit_seq_stream, mvs_fit_shared_shape and mvs_refine_cameras scratch (mvs_lbfgs.cu)
+struct SharedConsts;                  // model constants shared by the contexts that uploaded the same bytes (mvs_api.cu)
 
 // A device array of the context that only grows (dev_grow): cap elements at p
 template <class T> struct DevBuf {
@@ -341,6 +345,7 @@ struct mvs_ctx {
     int exec_mode = 0;               // mvs_set_exec_mode: 0 auto, 1 batched chain only, 2 stage barriers, 3 dense-round closures
     bool have_model = false, have_cams = false, have_kp = false, have_loss = false;
     std::vector<void*> allocs;       // everything cudaMalloc'ed, freed in mvs_destroy (dev_alloc / dev_free)
+    std::vector<mvs::SharedConsts*> consts;   // the entries holding ctx->m's arrays, dropped by mvs_destroy (upload_consts)
     // The state objects below are set only once complete, and released by mvs_destroy (release_fit_state, release_tc_state)
     mvs::LbfgsState* lbfgs = nullptr;    // optimiser state (mvs_lbfgs.cu)
     mvs::Profiler prof;
@@ -438,7 +443,6 @@ template <class T> int dev_grow(mvs_ctx* ctx, DevBuf<T>& b, size_t n) {
     b.cap = n;
     return MVS_OK;
 }
-template <class T> int dev_upload(mvs_ctx* ctx, T** p, const T* host, size_t count);
 
 // mvs_lbfgs.cu: mvs_closure through the frame-resident closure, a dense round or the batched chain
 int evaluate_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev, float* proj_dev,
