@@ -176,6 +176,24 @@ int mvs_closure(mvs_ctx* ctx, const float* params_dev, float* loss_dev, float* g
  *      says: decode latent codes first (mvs_vposer_decode). */
 int mvs_forward(mvs_ctx* ctx, const float* params_dev, float* joints_dev, float* verts_dev, void* stream);
 
+/* ---- vector-Jacobian product of mvs_forward (the autograd backward of SMPL.forward, body_models_scale.py:327-412 +
+ *      lbs.py:135-222, outside the closure): given params_dev [B,86] and cotangents of its outputs -- djoints_dev [B,K,3]
+ *      and / or dverts_dev [B,n_verts,3] (device, either may be NULL, not both) -- writes dparams_dev [B,86] =
+ *      d<dj,joints> + d<dv,verts> with respect to every entry (betas, global_orient, body_pose as axis-angle, transl, scale).
+ *      Needs only the model and the batch size, like mvs_forward; recomputes what it needs from params_dev (nothing is kept
+ *      from an earlier mvs_forward).  It is the model's Jacobian and nothing else: the frozen mask, the loss configuration,
+ *      the anchor, keypoints, 3-D targets, cameras and rigs are neither read nor changed, and neither is the optimiser state
+ *      mvs_lbfgs_step keeps between calls.  Workspace it borrows, which every entry point writes before it reads: the forward
+ *      arrays of the batch (pose features, skinning transforms, chain joints, v_posed, vertices; what mvs_forward writes)
+ *      and the closure's backward scratch (per-vertex cotangents, per-strip partials, translation and chain-joint
+ *      cotangents); with dverts_dev, the d v_posed operand of the tensor-core contraction, grow-only and its own.
+ *      With dverts_dev the adjoint runs over all vertices (the blend-shape contraction on the tensor cores; exec mode 1:
+ *      SIMT); joints only, over the <= 86 vertices the keypoints read.  Deterministic: the same call gives the same bits.
+ *      Asynchronous on `stream`.  MVS_ERR_INVALID: ctx, params_dev or dparams_dev NULL, both cotangents NULL, no model or
+ *      batch. */
+int mvs_forward_vjp(mvs_ctx* ctx, const float* params_dev, const float* djoints_dev, const float* dverts_dev,
+                    float* dparams_dev, void* stream);
+
 /* ---- optimiser: replaces LBFGS.step + _strong_Wolfe (code/optimizers/lbfgs_ls.py:39-445) driven by
  *      FittingMonitor.run_fitting (code/utils/fitting.py:71-142), one independent problem per frame,
  *      entirely on the device. */

@@ -247,6 +247,26 @@ class FittingContext:
                                                 self._stream()), "mvs_forward")
         return out
 
+    def forward_vjp(self, params: torch.Tensor, djoints: torch.Tensor | None = None,
+                    dverts: torch.Tensor | None = None) -> torch.Tensor:
+        """Vector-Jacobian product of forward_only (mvs_forward_vjp): dparams [B,86] = d<djoints, joints> + d<dverts, verts>
+        with respect to params [B,86] (body_pose as axis-angle).  djoints [B,K,3] and dverts [B,N,3] may each be None, not
+        both; every tensor is float32 on this context's device."""
+        def check(name, t, shape):
+            if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.device != self.device or tuple(t.shape) != shape:
+                raise ValueError("forward_vjp: want %s as a float32 tensor of shape %s on %s, got %s" % (
+                    name, shape, self.device, (t.dtype, tuple(t.shape), t.device) if isinstance(t, torch.Tensor) else type(t)))
+            return t.contiguous()
+        if djoints is None and dverts is None:
+            raise ValueError("forward_vjp: give djoints, dverts or both")
+        params = check("params", params, (self.B, S.NUM_PARAMS))
+        djoints = None if djoints is None else check("djoints", djoints, (self.B, self.K, 3))
+        dverts = None if dverts is None else check("dverts", dverts, (self.B, self.N, 3))
+        out = torch.empty(self.B, S.NUM_PARAMS, dtype=torch.float32, device=self.device)
+        _lib.check(self.h, self.lib.mvs_forward_vjp(self.h, _ptr(params), _ptr(djoints), _ptr(dverts), _ptr(out),
+                                                    self._stream()), "mvs_forward_vjp")
+        return out
+
     @staticmethod
     def make_lbfgs_config(max_outer=30, max_iter=30, max_eval=None, history_size=100, lr=1.0, tolerance_grad=1e-5,
                           tolerance_change=1e-9, ftol=1e-9, gtol=1e-9) -> _lib.LbfgsConfig:

@@ -725,6 +725,16 @@ int mvs_forward(mvs_ctx* ctx, const float* params_dev, float* joints_dev, float*
     return launch_closure(ctx, params_dev, nullptr, nullptr, joints_dev, nullptr, verts_dev, (cudaStream_t)stream, true);
 }
 
+int mvs_forward_vjp(mvs_ctx* ctx, const float* params_dev, const float* djoints_dev, const float* dverts_dev,
+                    float* dparams_dev, void* stream) {
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    MVS_REQUIRE(ctx, ctx->have_model && ctx->ws.B > 0, "mvs_forward_vjp: model and batch must be set first");
+    MVS_REQUIRE(ctx, params_dev && dparams_dev, "mvs_forward_vjp: params_dev and dparams_dev are required");
+    MVS_REQUIRE(ctx, djoints_dev || dverts_dev, "mvs_forward_vjp: give djoints_dev, dverts_dev or both");
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    return launch_forward_vjp(ctx, params_dev, djoints_dev, dverts_dev, dparams_dev, (cudaStream_t)stream);
+}
+
 int mvs_vposer_decode(mvs_ctx* ctx, const float* params_dev, float* body_pose_dev, void* stream) {
     if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
     MVS_REQUIRE(ctx, ctx->have_model && ctx->ws.B > 0 && ctx->m.vp_w1, "mvs_vposer_decode: model, batch and mvs_set_vposer first");

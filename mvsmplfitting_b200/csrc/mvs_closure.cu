@@ -218,6 +218,40 @@ struct KeypointModel {
     const int* sup; const int* sup_ptr; const int* sup_k; const float* sup_w;
 };
 
+// The adjoint of the keypoint map and of the output translation for one frame (slot): dq [K][3] (shared memory, complete)
+// holds the cotangent of every keypoint.  Writes dtransl[slot] = tr_extra (or 0) + sum_k dq, dgchain[slot] (the posed chain
+// joints the keypoints name, model type 'smpl') and, through put(i, d0, d1, d2), the cotangent of support vertex i (the
+// regressor rows and extra vertices that feed the keypoints).  Called by every thread of a block of >= 88 threads.
+template <class PutFn>
+__device__ __forceinline__ void route_keypoint_cotangent(const KeypointModel& km, const float* dq, int slot,
+                                                         const float* tr_extra, float* __restrict__ dtransl,
+                                                         float* __restrict__ dgchain, PutFn put) {
+    const int t = threadIdx.x, K = km.K;
+    if (t >= 32 && t < 35) {
+        const int c = t - 32;
+        float a = tr_extra ? tr_extra[c] : 0.f;
+        for (int k = 0; k < K; ++k) a += dq[3 * k + c];
+        dtransl[(size_t)slot * 3 + c] = a;
+    }
+    if (t >= 64 && t < 64 + kJoints) {
+        const int j = t - 64;
+        float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+        for (int k = 0; k < K; ++k)
+            if (km.kp_chain[k] == j) { a0 += dq[3 * k]; a1 += dq[3 * k + 1]; a2 += dq[3 * k + 2]; }
+        dgchain[((size_t)slot * kJoints + j) * 3] = a0; dgchain[((size_t)slot * kJoints + j) * 3 + 1] = a1;
+        dgchain[((size_t)slot * kJoints + j) * 3 + 2] = a2;
+    }
+    for (int i = t; i < km.nsup; i += blockDim.x) {
+        float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+        for (int e = km.sup_ptr[i]; e < km.sup_ptr[i + 1]; ++e) {
+            const int k = km.sup_k[e];
+            const float w = km.sup_w[e];
+            a0 = fmaf(w, dq[3 * k], a0); a1 = fmaf(w, dq[3 * k + 1], a1); a2 = fmaf(w, dq[3 * k + 2], a2);
+        }
+        put(i, a0, a1, a2);
+    }
+}
+
 __global__ void __launch_bounds__(kFrameThreads)
 keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, const int* __restrict__ na_ptr,
                      KeypointModel km, const float* __restrict__ verts, int nv, int dense,
@@ -317,32 +351,56 @@ keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, 
         }
         data_loss[slot] = a;
     }
-    if (t >= 32 && t < 35) {
-        const int c = t - 32;
-        float a = 0.f;
-        for (int k = 0; k < K; ++k) a += dq[3 * k + c];
-        dtransl[(size_t)slot * 3 + c] = a;
-    }
-    if (t >= 64 && t < 64 + kJoints) {
-        const int j = t - 64;
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-        for (int k = 0; k < K; ++k)
-            if (km.kp_chain[k] == j) { a0 += dq[3 * k]; a1 += dq[3 * k + 1]; a2 += dq[3 * k + 2]; }
-        dgchain[((size_t)slot * kJoints + j) * 3] = a0; dgchain[((size_t)slot * kJoints + j) * 3 + 1] = a1;
-        dgchain[((size_t)slot * kJoints + j) * 3 + 2] = a2;
-    }
-    for (int i = t; i < km.nsup; i += blockDim.x) {
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-        for (int e = km.sup_ptr[i]; e < km.sup_ptr[i + 1]; ++e) {
-            const int k = km.sup_k[e];
-            const float w = km.sup_w[e];
-            a0 = fmaf(w, dq[3 * k], a0); a1 = fmaf(w, dq[3 * k + 1], a1); a2 = fmaf(w, dq[3 * k + 2], a2);
-        }
-        // keypoint gradients occupy the first nsup entries of the frame's backward list (the SDF term, when on,
-        // appends one entry per vertex after them)
+    // keypoint gradients occupy the first nsup entries of the frame's backward list (the SDF term, when on, appends one
+    // entry per vertex after them)
+    route_keypoint_cotangent(km, dq, slot, nullptr, dtransl, dgchain, [&](int i, float a0, float a1, float a2) {
         float* d = dv + ((size_t)slot * dv_stride + i) * 3;
         d[0] = a0; d[1] = a1; d[2] = a2;
+    });
+}
+
+// mvs_forward_vjp: the cotangents of slot b's outputs.  djoints [B][K][3] goes through the keypoint map as above; dverts
+// [B][N][3] (may be NULL) is copied into the dense backward list dv [B][N][3], whose support vertices then also carry the
+// keypoints' share.  dtransl = sum of dverts + sum of djoints (the output translation, body_models_scale.py:401-403).
+__global__ void __launch_bounds__(kFrameThreads)
+vjp_cotangent_kernel(const int* __restrict__ fidx, const int* __restrict__ na_ptr, KeypointModel km,
+                     const float* __restrict__ djoints, const float* __restrict__ dverts, float* __restrict__ dtransl,
+                     float* __restrict__ dgchain, float* __restrict__ dv) {
+    const int slot = blockIdx.x;
+    if (slot >= *na_ptr) return;
+    const int b = fidx[slot];
+    const int t = threadIdx.x, N = km.N;
+    __shared__ float dq[kMaxKeypoints * 3];
+    __shared__ float red[3][kFrameThreads];
+    __shared__ float vsum[3];
+    for (int i = t; i < 3 * km.K; i += blockDim.x) dq[i] = djoints ? djoints[(size_t)b * km.K * 3 + i] : 0.f;
+    const float* src = dverts ? dverts + (size_t)b * N * 3 : nullptr;
+    float* dst = dv + (size_t)slot * N * 3;
+    if (src) {
+        float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+        for (int n = t; n < N; n += blockDim.x) {
+            const float d0 = src[3 * n], d1 = src[3 * n + 1], d2 = src[3 * n + 2];
+            dst[3 * n] = d0; dst[3 * n + 1] = d1; dst[3 * n + 2] = d2;
+            a0 += d0; a1 += d1; a2 += d2;
+        }
+        red[0][t] = a0; red[1][t] = a1; red[2][t] = a2;
     }
+    __syncthreads();
+    if (src && t < 3) {                    // fixed order: the same bits on every call
+        float a = 0.f;
+        for (int i = 0; i < (int)blockDim.x; ++i) a += red[t][i];
+        vsum[t] = a;
+    }
+    __syncthreads();
+    route_keypoint_cotangent(km, dq, slot, src ? vsum : nullptr, dtransl, dgchain, [&](int i, float a0, float a1, float a2) {
+        if (src) {                         // dense list: vertex sup[i] = its dverts row + the keypoints' share
+            const int n = km.sup[i];
+            dst[3 * n] = src[3 * n] + a0; dst[3 * n + 1] = src[3 * n + 1] + a1; dst[3 * n + 2] = src[3 * n + 2] + a2;
+        } else {                           // keypoint support list, as the closure's
+            float* d = dv + ((size_t)slot * km.nsup + i) * 3;
+            d[0] = a0; d[1] = a1; d[2] = a2;
+        }
+    });
 }
 
 // ------------------------------------------------------------------------------------------ K4
@@ -353,12 +411,16 @@ constexpr int kQbLd = kFeatPad + 4;      // 228
 constexpr size_t kVertBwdSmem =
     (size_t)(2 * kTileC * kDvLd + kTileC * kDvpLd + kTileV * kJoints + kBwdCols * kQbLd + kSkinFloats * kTileF) * sizeof(float);
 
+// kDvpOut (mvs_forward_vjp, tensor-core path): d v_posed is not contracted here but written out, split into TF32 hi | lo,
+// to dvp [2][ldA][ldR] (row = frame slot, column 3 n + c, hi rows then lo rows) for vertex_bwd_tc_kernel (mvs_tc.cu); the
+// per-strip partials then hold the skinning adjoint only.  Tiles without upstream gradient are written too (as zeros).
+template <bool kDvpOut>
 __global__ void __launch_bounds__(kVertThreads, 1)
 vertex_bwd_kernel(const float* __restrict__ Qk, const float* __restrict__ At, int ldA,
                   const int* __restrict__ ell_j, const float* __restrict__ ell_w, int KW,
                   const float* __restrict__ Wd, const int* __restrict__ blist_n, const int* __restrict__ blist_pos,
                   int nvb, int nv_fwd, const float* __restrict__ vposed, const float* __restrict__ dv,
-                  const int* __restrict__ na_ptr, int ntiles, float* __restrict__ part) {
+                  const int* __restrict__ na_ptr, int ntiles, float* __restrict__ part, float* __restrict__ dvp, int ldR) {
     extern __shared__ __align__(16) float smem[];
     float* DV = smem;                          // [96][65]   upstream d loss / d vertex, column-major
     float* VP = DV + kTileC * kDvLd;           // [96][65]   v_posed
@@ -415,7 +477,7 @@ vertex_bwd_kernel(const float* __restrict__ Qk, const float* __restrict__ At, in
             const int n = s_n[idx / kJoints];
             Ws[idx] = n >= 0 ? Wd[(size_t)n * kJoints + idx % kJoints] : 0.f;
         }
-        if (!__syncthreads_or(any)) continue;          // no upstream gradient anywhere in this tile
+        if (!__syncthreads_or(any) && !kDvpOut) continue;   // no upstream gradient anywhere in this tile
         if (!ats_loaded) {
             for (int e = tid; e < kSkinFloats * kTileF; e += kVertThreads)
                 Ats[e] = At[(size_t)(e >> 6) * ldA + min(f0 + (e & 63), na - 1)];
@@ -475,6 +537,21 @@ vertex_bwd_kernel(const float* __restrict__ Qk, const float* __restrict__ At, in
                 }
             }
         }
+        if constexpr (kDvpOut) {
+            __syncthreads();
+            for (int idx = tid; idx < kTileF * kTileC; idx += kVertThreads) {
+                const int bb = idx / kTileC, col = idx % kTileC;
+                const int slot = f0 + bb, n = s_n[col / 3];
+                if (slot < na && n >= 0) {
+                    float hi, lo;
+                    tf32_split(dVp[col * kDvpLd + bb], hi, lo);
+                    const size_t o = (size_t)slot * ldR + 3 * (size_t)n + col % 3;
+                    dvp[o] = hi;
+                    dvp[(size_t)ldA * ldR + o] = lo;
+                }
+            }
+            continue;
+        }
         // d Phi[b][k] += sum_col dVp[b][col] * Qk[col][k]; the next 16 Qk rows are fetched into registers while
         // the current ones are consumed from shared memory
         constexpr int kQv = (kBwdCols * (kFeatPad / 4) + kVertThreads - 1) / kVertThreads;      // float4 per thread (4)
@@ -520,7 +597,7 @@ vertex_bwd_kernel(const float* __restrict__ Qk, const float* __restrict__ At, in
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const int slot = f0 + 4 * ty + i;
-        if (slot < na) {
+        if (slot < na && !kDvpOut) {
             float* o = part + ((size_t)strip * ldA + slot) * kPartFloats + kSkinFloats + 14 * tx;
 #pragma unroll
             for (int k = 0; k < 14; ++k) o[k] = accP[i][k];
@@ -548,7 +625,7 @@ frame_bwd_kernel(const float* __restrict__ x, const int* __restrict__ fidx, cons
                  const float* __restrict__ data_loss, const float* __restrict__ pen_loss /* NULL: term off */,
                  const float* __restrict__ dtransl, const float* __restrict__ dgchain, PriorModel pm, LossParams lp,
                  const float* __restrict__ anchor, const float* __restrict__ anchor_w,
-                 float* __restrict__ loss_out, float* __restrict__ grad_out) {
+                 float* __restrict__ loss_out, float* __restrict__ grad_out, int model_only) {
     const int slot = blockIdx.x;
     if (slot >= *na_ptr) return;
     const int b = fidx[slot];
@@ -622,6 +699,10 @@ frame_bwd_kernel(const float* __restrict__ x, const int* __restrict__ fidx, cons
             grad[kOffTransl + t - 64] = dtransl[(size_t)slot * 3 + t - 64];
         }
         __syncthreads();
+    }
+    if (model_only) {          // mvs_forward_vjp: the model's Jacobian alone (no loss, priors, anchor or frozen mask)
+        for (int i = t; i < kParams; i += blockDim.x) grad_out[(size_t)b * kParams + i] = grad[i];
+        return;
     }
 
     // ---------------- priors (fitting.py:327-350); value + gradient, data-dependent guards on device
@@ -752,8 +833,19 @@ __global__ void fill_kernel(float* p, float v, size_t n) {
 
 int closure_set_attributes(mvs_ctx* ctx) {
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertFwdSmem));
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertBwdSmem));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertBwdSmem));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVertBwdSmem));
     return MVS_OK;
+}
+
+// strips of the vertex backward over ntiles vertex tiles: about one CTA per SM over the 64-frame tiles, at most nstrips_max
+static int bwd_strips(const mvs_ctx* ctx, int ntiles) {
+    const int ftiles = ctx->ws.ldA / kTileF;
+    int want = (ctx->sm_count + ftiles - 1) / ftiles;
+    if (want < 1) want = 1;
+    if (want > ctx->ws.nstrips_max) want = ctx->ws.nstrips_max;
+    const int tps = (ntiles + want - 1) / want;
+    return (ntiles + tps - 1) / tps;
 }
 
 int launch_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev,
@@ -814,27 +906,83 @@ int launch_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* gra
         const int* blist_n = sdf_on ? m.sup_then_all : m.sup;
         const int* blist_pos = sdf_on ? m.sup_then_all : (dense ? m.sup : nullptr);
         const int ntiles = (nvb + kTileV - 1) / kTileV;
-        int want = (ctx->sm_count + ftiles - 1) / ftiles;
-        if (want < 1) want = 1;
-        if (want > w.nstrips_max) want = w.nstrips_max;
-        int tps = (ntiles + want - 1) / want;
-        nstrips = (ntiles + tps - 1) / tps;
+        nstrips = bwd_strips(ctx, ntiles);
         dim3 g4(nstrips, ftiles);
         MVS_LAUNCH(ctx, KID_VERTEX_BWD, st,
-                   vertex_bwd_kernel<<<g4, kVertThreads, kVertBwdSmem, st>>>(m.Qk, w.At, w.ldA, m.ell_j, m.ell_w, m.KW, m.Wd,
-                                                                             blist_n, blist_pos, nvb, nv, w.vposed, w.dv,
-                                                                             w.na, ntiles, w.part));
+                   vertex_bwd_kernel<false><<<g4, kVertThreads, kVertBwdSmem, st>>>(m.Qk, w.At, w.ldA, m.ell_j, m.ell_w, m.KW, m.Wd,
+                                                                                    blist_n, blist_pos, nvb, nv, w.vposed, w.dv,
+                                                                                    w.na, ntiles, w.part, nullptr, 0));
     }
     PriorModel pm{m.M, m.gmm_means, m.gmm_prec, m.gmm_lognllw};
     MVS_LAUNCH(ctx, KID_FRAME_BWD, st,
                frame_bwd_kernel<<<B, kFrameThreads, 0, st>>>(x_dev, w.fidx, w.na, par, m.Jt, m.JS, w.part, nstrips, w.ldA,
                                                              have_grad ? 1 : 0, w.data_loss, sdf_on ? w.pen_loss : nullptr, w.dtransl,
                                                              w.dgchain, pm, lp, w.anchor, w.anchor_w,
-                                                             loss_dev ? loss_dev : w.loss_scratch, grad_dev));
+                                                             loss_dev ? loss_dev : w.loss_scratch, grad_dev, 0));
     if (verts_dev) {
         dim3 g6((m.N * 3 + 255) / 256, B);
         MVS_LAUNCH(ctx, KID_MISC, st, verts_out_kernel<<<g6, 256, 0, st>>>(w.verts, x_dev, w.fidx, w.na, m.N, verts_dev));
     }
+    MVS_CUDA_OK(ctx, cudaGetLastError());
+    return MVS_OK;
+}
+
+// mvs_forward_vjp.  The forward is recomputed as mvs_forward computes it (exec mode 0: the tensor-core vertex forward, which
+// stores v_posed; joints-only calls and exec mode 1: vertex_fwd_kernel), then
+//   vjp_cotangent -> [dense, mode 0]  vertex_bwd<dvp out> (skinning adjoint, d v_posed) -> vertex_bwd_tc (d Phi, tensor cores)
+//                    [otherwise]      vertex_bwd (skinning adjoint and d Phi, SIMT)
+//                 -> frame_bwd (model only).
+// Joints-only calls run on the keypoint support list, as the closure does.
+int launch_forward_vjp(mvs_ctx* ctx, const float* x_dev, const float* djoints, const float* dverts, float* dparams,
+                       cudaStream_t st) {
+    const DevModel& m = ctx->m;
+    Workspace& w = ctx->ws;
+    const int B = w.B;
+    const bool dense = dverts != nullptr;
+    const bool tc = dense && ctx->exec_mode != 1;
+    const int nv = dense ? m.N : m.nsup;
+    const Parents par = ctx->parents;
+    const int ftiles = w.ldA / kTileF;
+    MVS_LAUNCH(ctx, KID_FRAME_FWD, st,
+               frame_fwd_kernel<<<B, kFrameThreads, 0, st>>>(x_dev, w.fidx, w.na, par, m.Jt, m.JS, w.Phi, w.PhiTc, w.At, w.ldA,
+                                                             w.gchain, w.slot_tr));
+    if (tc) {
+        if (int rc = launch_vertex_fwd_tc(ctx, st, true, false)) return rc;
+    } else {
+        dim3 g2((nv + kTileV - 1) / kTileV, ftiles);
+        MVS_LAUNCH(ctx, KID_VERTEX_FWD, st,
+                   vertex_fwd_kernel<<<g2, kVertThreads, kVertFwdSmem, st>>>(m.Qk, w.Phi, w.At, w.ldA, m.ell_j, m.ell_w, m.KW,
+                                                                             dense ? nullptr : m.sup, nv, w.na, w.vposed, w.verts));
+    }
+    const KeypointModel km{m.K, m.nsup, m.N, m.kp_ptr, m.kp_vidx, m.kp_spos, m.kp_w, m.kp_chain, m.sup, m.sup_ptr, m.sup_k, m.sup_w};
+    MVS_LAUNCH(ctx, KID_KEYPOINT, st,
+               vjp_cotangent_kernel<<<B, kFrameThreads, 0, st>>>(w.fidx, w.na, km, djoints, dverts, w.dtransl, w.dgchain, w.dv));
+    // backward list: every vertex (dense) or the keypoint support
+    const int* blist_n = dense ? nullptr : m.sup;
+    const int ntiles = (nv + kTileV - 1) / kTileV;
+    const int nstrips = bwd_strips(ctx, ntiles);
+    const dim3 g4(nstrips, ftiles);
+    if (tc) {
+        float* dvp = nullptr;
+        int ldR = 0;
+        if (int rc = tc_vjp_buffer(ctx, &dvp, &ldR)) return rc;
+        MVS_LAUNCH(ctx, KID_VERTEX_BWD, st,
+                   vertex_bwd_kernel<true><<<g4, kVertThreads, kVertBwdSmem, st>>>(m.Qk, w.At, w.ldA, m.ell_j, m.ell_w, m.KW, m.Wd,
+                                                                                   blist_n, nullptr, nv, nv, w.vposed, w.dv, w.na,
+                                                                                   ntiles, w.part, dvp, ldR));
+        if (int rc = launch_vertex_bwd_tc(ctx, nstrips, st)) return rc;
+    } else {
+        MVS_LAUNCH(ctx, KID_VERTEX_BWD, st,
+                   vertex_bwd_kernel<false><<<g4, kVertThreads, kVertBwdSmem, st>>>(m.Qk, w.At, w.ldA, m.ell_j, m.ell_w, m.KW, m.Wd,
+                                                                                    blist_n, nullptr, nv, nv, w.vposed, w.dv, w.na,
+                                                                                    ntiles, w.part, nullptr, 0));
+    }
+    const PriorModel pm{0, nullptr, nullptr, nullptr};
+    const LossParams lp{};
+    MVS_LAUNCH(ctx, KID_FRAME_BWD, st,
+               frame_bwd_kernel<<<B, kFrameThreads, 0, st>>>(x_dev, w.fidx, w.na, par, m.Jt, m.JS, w.part, nstrips, w.ldA, 1,
+                                                             nullptr, nullptr, w.dtransl, w.dgchain, pm, lp, nullptr, nullptr,
+                                                             nullptr, dparams, 1));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }

@@ -456,6 +456,9 @@ int sdf_set_attributes(mvs_ctx* ctx);
 int launch_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev,
                    float* proj_dev, float* verts_dev, cudaStream_t st, bool geometry_only = false);
 int launch_sdf_terms(mvs_ctx* ctx, const float* x_dev, cudaStream_t st);   // mvs_sdf.cu
+// mvs_forward_vjp (mvs_closure.cu): dparams [B][86] from params x_dev and the cotangents djoints [B][K][3] / dverts [B][N][3]
+int launch_forward_vjp(mvs_ctx* ctx, const float* x_dev, const float* djoints, const float* dverts, float* dparams,
+                       cudaStream_t st);
 // mvs_resident.cu: frame-resident (one CTA per frame) closure and whole-stage optimiser for the sparse regime
 bool resident_supported(const mvs_ctx* ctx);   // the model fits the frame-resident kernels
 bool dense_supported(const mvs_ctx* ctx);      // the mesh fits frame_step's list of 256-vertex blocks
@@ -497,6 +500,11 @@ SdfSetupArgs make_sdf_setup_args(mvs_ctx* ctx);          // mvs_sdf.cu
 int tc_upload_model(mvs_ctx* ctx);                 // after m.Qk is on the device
 int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool sdf_setup);
 int tc_check_error(mvs_ctx* ctx);
+// the d v_posed operand of vertex_bwd_tc_kernel, [2][ldA][ldR] (TF32 hi rows, then lo rows), allocated on first use
+int tc_vjp_buffer(mvs_ctx* ctx, float** dvp, int* ldR);
+// d Phi of mvs_forward_vjp on the tensor cores: the feature columns of the nstrips per-strip partials (w.part) from the
+// d v_posed rows vertex_bwd_kernel<true> wrote
+int launch_vertex_bwd_tc(mvs_ctx* ctx, int nstrips, cudaStream_t st);
 float* tc_poffT(mvs_ctx* ctx);                 // [3N][ldA] pose offsets of the tensor-core contraction (written by launch_vertex_fwd_tc)
 int launch_frame_step(mvs_ctx* ctx, float* params_dev, const LbfgsState& L, const LbfgsCfg& cfg, int nstages, cudaStream_t st);
 int frame_step_begin_run(mvs_ctx* ctx, cudaStream_t st);                 // mvs_resident.cu

@@ -169,6 +169,120 @@ posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_
     if (threadIdx.x == 0) TC_MARK(20);
 }
 
+// The blend-shape adjoint of mvs_forward_vjp on the tensor cores:
+//
+//   dPhi[b][k] = sum_r dVp[b][r] Qk[r][k]        r over the 3N posedirs rows (K = 20670), k over the 224 feature columns
+//
+// run as dPhi^T = Qk^T . dVp^T: the features are the wgmma M side (four consumer warpgroups of 64 features, 256 >= 224), the
+// frames the N side (8 .. 64 per column tile), the posedirs rows the reduction.  Split-K: CTA (s, c) sums the rows of strip s
+// (a contiguous range of 32-row chunks) for column tile c and writes its partial into the feature columns of
+// part[s][slot][288 ..] -- the per-strip layout frame_bwd_kernel reduces, in strip order, next to the skinning partials
+// vertex_bwd_kernel<true> wrote.  No atomics: the sum has a fixed order, so a call gives the same bits every time.
+//   warp 16              TMA producer (one thread): per 32-row chunk the seven 32 x 32 boxes of Qk (fp32, straight from the
+//                        model's rows) and the frames' dVp hi and lo boxes (written split by vertex_bwd_kernel<true>), through
+//                        a 4-stage mbarrier ring.
+//   warpgroups 0 .. 3    the A fragment (Qk^T: feature x row) gathered from the swizzled boxes and split into TF32 hi and lo in
+//                        registers; B (dVp) from shared memory; the 3xTF32 products of posedirs_gemm_tc_kernel.
+constexpr int kTbRows = 32;                                 // posedirs rows per ring stage (the reduction chunk)
+constexpr int kTbBoxes = kFeatPad / 32;                     // 7 boxes of 32 features per row chunk
+constexpr int kTbQBytes = kTbBoxes * kTbRows * 128;         // 28 KB of Qk per stage
+constexpr int kTbWg = 4;                                    // consumer warpgroups
+constexpr int kTbThreads = 128 * kTbWg + 32;                // + the producer warp
+constexpr int kTbStages = 4;
+constexpr int kTbCols = 64;                                 // largest frame column tile (wgmma N)
+__host__ __device__ constexpr int tb_stage_bytes(int nf) { return kTbQBytes + 2 * tc_fbytes(nf); }
+__host__ __device__ constexpr size_t tb_smem(int nf) { return 1024 + (size_t)kTbStages * tb_stage_bytes(nf) + 256; }
+__host__ __device__ constexpr int tb_dvp_ld(int N) { return (3 * N + 3) / 4 * 4; }       // 16-byte rows for the tensor map
+
+template <int NF>
+__global__ void __launch_bounds__(kTbThreads, 1)
+vertex_bwd_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_d, int ldA,
+                     const int* __restrict__ na_ptr, int nchunks, float* __restrict__ part, int* __restrict__ err_flag) {
+    constexpr uint32_t kFBytes = tc_fbytes(NF), kStageBytes = tb_stage_bytes(NF);
+    extern __shared__ unsigned char smem_raw[];
+    unsigned char* sR = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint64_t* full = reinterpret_cast<uint64_t*>(sR + (size_t)kTbStages * kStageBytes);
+    uint64_t* empty = full + kTbStages;
+    const int na = *na_ptr;
+    const int f0 = blockIdx.y * NF;
+    if (f0 >= na) return;
+    const int strip = blockIdx.x;
+    const int per = (nchunks + gridDim.x - 1) / gridDim.x;
+    const int c_begin = min(strip * per, nchunks), c_end = min(c_begin + per, nchunks);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (int st = 0; st < kTbStages; ++st) { mbar_init(&full[st], 1); mbar_init(&empty[st], kTbWg); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (warp == 4 * kTbWg) {
+        if (lane == 0) {               // TMA producer; rows past 3N (last chunk) are zero-filled by both tensor maps
+            int stage = 0; uint32_t phase = 0;
+            for (int kc = c_begin; kc < c_end; ++kc) {
+                if (!mbar_wait(&empty[stage], phase ^ 1, err_flag)) return;
+                unsigned char* sP = sR + (size_t)stage * kStageBytes;
+                mbar_expect_tx(&full[stage], kStageBytes);
+                for (int bx = 0; bx < kTbBoxes; ++bx) tma_load_2d(sP + bx * kTbRows * 128, &map_q, 32 * bx, kc * kTbRows, &full[stage]);
+                tma_load_2d(sP + kTbQBytes, &map_d, kc * kTbRows, f0, &full[stage]);
+                tma_load_2d(sP + kTbQBytes + kFBytes, &map_d, kc * kTbRows, ldA + f0, &full[stage]);
+                if (++stage == kTbStages) { stage = 0; phase ^= 1; }
+            }
+        }
+        return;
+    }
+    // consumer warpgroup g: features 64 g + 16 w + lr (+ 8), w = warp of the warpgroup, lr = lane / 4; rows q, q + 4 of each k8
+    const int g = warp >> 2, wt = threadIdx.x & 127, w = wt >> 5, q = lane & 3, lr = lane >> 2;
+    const int fa = 64 * g + 16 * w + lr;                      // feature of a[0], a[2]; a[1], a[3] have fa + 8 (same box)
+    const bool fvalid = fa < kFeatPad;                        // warpgroup 3's upper half is past the 224 columns
+    const int box = min(fa >> 5, kTbBoxes - 1), ca = fa & 31;
+    float acc[NF / 2];
+#pragma unroll
+    for (int i = 0; i < NF / 2; ++i) acc[i] = 0.f;
+    int stage = 0, held = -1; uint32_t phase = 0;
+    for (int kc = c_begin; kc < c_end; ++kc) {
+        mbar_wait(&full[stage], phase, err_flag);            // on a timeout the flag is raised and the warpgroup carries on
+        const unsigned char* sQ = sR + (size_t)stage * kStageBytes + box * kTbRows * 128;
+        const uint32_t bh = smem_u32(sR + (size_t)stage * kStageBytes + kTbQBytes), bl = bh + kFBytes;
+#pragma unroll
+        for (int k = 0; k < kTbRows / 8; ++k) {
+            uint32_t ahi[4], alo[4];
+#pragma unroll
+            for (int v = 0; v < 4; ++v) {
+                const int r = 8 * k + q + 4 * (v >> 1), c = ca + 8 * (v & 1);     // row of the chunk, column of the box
+                float x = *reinterpret_cast<const float*>(sQ + r * 128 + ((((c >> 2) ^ (r & 7))) << 4) + 4 * (c & 3));
+                if (!fvalid) x = 0.f;
+                float hi, lo;
+                tf32_split(x, hi, lo);
+                ahi[v] = __float_as_uint(hi);
+                alo[v] = __float_as_uint(lo);
+            }
+            wgmma_fence();
+            WgmmaTf32Rs<NF>::mma(acc, ahi, wgmma_desc_k_sw128(bh + k * 32), 1u);
+            WgmmaTf32Rs<NF>::mma(acc, ahi, wgmma_desc_k_sw128(bl + k * 32), 1u);
+            WgmmaTf32Rs<NF>::mma(acc, alo, wgmma_desc_k_sw128(bh + k * 32), 1u);
+            wgmma_commit();
+            wgmma_wait1();                                    // the previous chunk's groups have retired: its stage is free
+            if (k == 0 && held >= 0) mbar_arrive_if(&empty[held], wt == 0);
+        }
+        held = stage;
+        if (++stage == kTbStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait0();
+    // d[4 i + 2 h + j] = dPhi^T[feature fa + 8 h][frame f0 + 8 i + 2 q + j]
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int f = fa + 8 * h;
+        if (f >= kFeatPad) continue;
+#pragma unroll
+        for (int i = 0; i < NF / 8; ++i)
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                const int slot = f0 + 8 * i + 2 * q + j;
+                if (slot < na) part[((size_t)strip * ldA + slot) * kPartFloats + kSkinFloats + f] = acc[4 * i + 2 * h + j];
+            }
+    }
+}
+
 // grid (nchunks, frame groups of 32); kSkinSmem bytes of dynamic shared memory
 __global__ void __launch_bounds__(kSkinThreads)
 skin_kernel(SkinArgs ar, const int* __restrict__ na_ptr, int cta_slots) {
@@ -412,14 +526,22 @@ sdf_setup_kernel(const SdfSetupArgs sa, const float* bboxp, const float* verts, 
 constexpr int kTcInstances[] = {8, 16, 32, 64, 128};       // wgmma N instances of posedirs_gemm_tc_kernel
 constexpr int kTcNumInst = 5;
 
+constexpr int kTbNumInst = 4;                               // wgmma N instances of vertex_bwd_tc_kernel: 8, 16, 32, 64
+
 struct TcState {
     CUtensorMap map_p;              // fp32 posedirs: the model's Qk rows [3N][224], box 128 rows x 32
     CUtensorMap map_f[kTcNumInst];  // PhiTc [2][ldA][224] (hi rows, then lo rows), box kTcInstances[i] rows x 32
     float* poffT = nullptr;         // [3N][ldA] pose offsets, frame fastest (output of the tensor-core contraction)
     int* err = nullptr;
+    // mvs_forward_vjp (vertex_bwd_tc_kernel), set up on first use
+    CUtensorMap map_q;              // the model's Qk rows [3N][224], box 32 rows x 32
+    CUtensorMap map_d[kTbNumInst];  // dvp [2][ldA][3N] (row stride ldR), box kTcInstances[i] rows x 32
+    float* dvp = nullptr;           // [2][ldA][ldR] d v_posed split into TF32 hi | lo (vertex_bwd_kernel<true>)
 };
 
-static int encode_map(mvs_ctx* ctx, CUtensorMap* map, const float* ptr, uint64_t rows, uint32_t box_rows) {
+// 2-D fp32 tensor map [rows][cols] (row stride ld floats), box box_rows x 32 floats, 128-byte swizzle
+static int encode_map(mvs_ctx* ctx, CUtensorMap* map, const float* ptr, uint64_t rows, uint32_t box_rows,
+                      uint64_t cols = kFeatPad, uint64_t ld = kFeatPad) {
     static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
     if (!fn) {
         cudaDriverEntryPointQueryResult q;
@@ -428,8 +550,8 @@ static int encode_map(mvs_ctx* ctx, CUtensorMap* map, const float* ptr, uint64_t
             return set_error(ctx, MVS_ERR_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
         fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(p);
     }
-    cuuint64_t dims[2] = {(cuuint64_t)kFeatPad, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)kFeatPad * sizeof(float)};
+    cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+    cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
     cuuint32_t box[2] = {(cuuint32_t)kTcBK, box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), dims, strides, box, estr,
@@ -468,6 +590,44 @@ int tc_set_attributes(mvs_ctx* ctx) {
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(64)));
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(128)));
     MVS_CUDA_OK(ctx, cudaFuncSetAttribute(skin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSkinSmem));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_tc_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tb_smem(8)));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tb_smem(16)));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tb_smem(32)));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tb_smem(64)));
+    return MVS_OK;
+}
+
+int tc_vjp_buffer(mvs_ctx* ctx, float** dvp, int* ldR) {
+    TcState* T = ctx->tc;
+    const Workspace& w = ctx->ws;
+    const int N = ctx->m.N, ld = tb_dvp_ld(N);
+    if (!T->dvp) {                                      // allocated on first use: only mvs_forward_vjp needs it
+        float* p = nullptr;
+        if (int rc = dev_alloc(ctx, &p, (size_t)2 * w.ldA * ld)) return rc;
+        int rc;
+        if ((rc = encode_map(ctx, &T->map_q, ctx->m.Qk, (uint64_t)3 * N, kTbRows))) return rc;
+        for (int i = 0; i < kTbNumInst; ++i)
+            if ((rc = encode_map(ctx, &T->map_d[i], p, (uint64_t)2 * w.ldA, kTcInstances[i], (uint64_t)3 * N, ld))) return rc;
+        T->dvp = p;
+    }
+    *dvp = T->dvp;
+    *ldR = ld;
+    return MVS_OK;
+}
+
+int launch_vertex_bwd_tc(mvs_ctx* ctx, int nstrips, cudaStream_t st) {
+    const TcState* T = ctx->tc;
+    const Workspace& w = ctx->ws;
+    const int nchunks = (3 * ctx->m.N + kTbRows - 1) / kTbRows;
+    const int nf = std::min(tc_cols_for(w.B), kTbCols);
+    const dim3 grid(nstrips, (w.B + nf - 1) / nf);
+    const int inst = nf == 8 ? 0 : nf == 16 ? 1 : nf == 32 ? 2 : 3;
+#define MVS_TB_LAUNCH(NF) vertex_bwd_tc_kernel<NF><<<grid, kTbThreads, tb_smem(NF), st>>>(T->map_q, T->map_d[inst], w.ldA, w.na, nchunks, w.part, T->err)
+    MVS_LAUNCH(ctx, KID_VERTEX_BWD, st,
+               if (nf == 8) MVS_TB_LAUNCH(8); else if (nf == 16) MVS_TB_LAUNCH(16); else if (nf == 32) MVS_TB_LAUNCH(32);
+               else MVS_TB_LAUNCH(64));
+#undef MVS_TB_LAUNCH
+    MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }
 

@@ -7,8 +7,10 @@ Mirrors the public surface of reference code/smplx/body_models_scale.py for the 
 reset_params(), and forward() -> ModelOutput.  SMPLH / SMPLX are out of scope (unreachable from
 cfg_files/fit_smpl.yaml).
 
-forward() returns DETACHED tensors: inside the fitting loop gradients come from the fused closure
-(FittingMonitor.create_fitting_closure), which never builds an autograd graph.
+By default forward() returns DETACHED tensors: inside the fitting loop gradients come from the fused closure
+(FittingMonitor.create_fitting_closure), which never builds an autograd graph.  With differentiable=True, forward() keeps
+the module's parameters and the tensors passed to it in the graph and back-propagates through mvs_forward_vjp, like the
+reference's autograd module (first derivatives only).
 """
 from __future__ import annotations
 
@@ -40,7 +42,8 @@ def _np(a, dtype=np.float32):
 
 
 def create_scale(model_path, model_type="smpl", **kwargs):
-    """Same dispatch as the reference factory (body_models_scale.py:39-89)."""
+    """Same dispatch as the reference factory (body_models_scale.py:39-89).  differentiable=True (passed on to SMPL) gives a
+    module whose forward() back-propagates into its parameters and inputs."""
     if os.path.isdir(model_path):
         model_path = os.path.join(model_path, "smpl")
     mt = model_type.lower()
@@ -70,8 +73,9 @@ class SMPL(nn.Module):
                  global_orient=None, create_body_pose=True, body_pose=None, create_transl=True, transl=None,
                  create_scale=True, scale=None, dtype=torch.float32, batch_size=1, joint_mapper=None,
                  model_type="smpl", gender="neutral", vertex_ids=None, lsp_regressor_path="data/J_regressor_lsp.npz",
-                 **kwargs):
+                 differentiable=False, **kwargs):
         self.model_type = model_type
+        self.differentiable = bool(differentiable)
         self.gender = gender
         if data_struct is None:
             fn = os.path.join(model_path, "SMPL_{}.pkl".format(gender.upper())) if os.path.isdir(model_path) else model_path
@@ -171,12 +175,34 @@ class SMPL(nn.Module):
         return torch.cat([get("betas", 10, 0.0), get("global_orient", 3, 0.0), get("body_pose", 69, 0.0),
                           get("transl", 3, 0.0), get("scale", 1, 1.0)], dim=1).contiguous()
 
+    def graph_params(self, betas=None, body_pose=None, global_orient=None, transl=None, scale=None) -> torch.Tensor:
+        """[B,86] in the library's order from the tensors passed in, else the module's parameters, NOT detached
+        (differentiable=True); a tensor missing from both is filled with its default (0, scale 1)"""
+        B = self.batch_size
+        dev = self.v_template.device
+
+        def get(name, given, n, default):
+            t = given if given is not None else getattr(self, name, None)
+            if t is None:
+                return torch.full((B, n), default, dtype=torch.float32, device=dev)
+            return t.reshape(B, n).to(torch.float32)
+        return torch.cat([get("betas", betas, 10, 0.0), get("global_orient", global_orient, 3, 0.0),
+                          get("body_pose", body_pose, 69, 0.0), get("transl", transl, 3, 0.0),
+                          get("scale", scale, 1, 1.0)], dim=1)
+
     def forward(self, betas=None, body_pose=None, global_orient=None, transl=None, scale=None, return_verts=True,
                 return_full_pose=False, **kwargs):
         from ..fitting import model_context
         if not self.v_template.is_cuda:
             raise RuntimeError("mvsmplfitting_b200.SMPL.forward needs the model on a CUDA device (no CPU fallback)")
         ctx = model_context(self)
+        if self.differentiable:
+            from ..autograd import smpl_apply
+            x = self.graph_params(betas=betas, body_pose=body_pose, global_orient=global_orient, transl=transl, scale=scale)
+            joints, verts = smpl_apply(ctx, x, want_verts=return_verts)
+            go, bp = x[:, 10:13], x[:, 13:82]
+            return ModelOutput(vertices=verts, joints=joints, global_orient=go, body_pose=bp, betas=x[:, :10],
+                               full_pose=torch.cat([go, bp], dim=1) if return_full_pose else None)
         x = self.flat_params(body_pose=body_pose)
         over = dict(betas=(betas, 0, 10), global_orient=(global_orient, 10, 13), transl=(transl, 82, 85), scale=(scale, 85, 86))
         for t, a, e in over.values():
