@@ -12,12 +12,10 @@
 //                        active count; batches above 128 run column tiles of 128 frames as a second grid dimension).  The
 //                        accumulator fragment is [coordinate][frame], the layout of poffT, and is stored straight from
 //                        registers.
-//   warp 8               TMA producer (one thread): per (row tile, k chunk) the fp32 posedirs box 128 x 32 (straight from
-//                        the model's Qk rows) and the frames' feature hi and lo boxes, through a 4-stage mbarrier ring.
-//   warpgroups 0, 1      64 posedirs rows each: load the fp32 A fragment from shared memory, split it into TF32 hi and lo
-//                        in registers, issue wgmma.m64nNk8 with A from registers and B (features) from shared memory; one
-//                        wgmma group stays in flight while the next chunk is split, and a ring stage is released once the
-//                        group that read it has retired.  CTAs are persistent over a contiguous range of row tiles.
+//   ring                 the TMA / wgmma ring of mvs_tc_dev.cuh.  Warp 8 is its producer: per (row tile, k chunk) the fp32
+//                        posedirs box 128 x 32 (straight from the model's Qk rows) and the frames' feature hi and lo boxes.
+//   warpgroups 0, 1      its consumers, 64 posedirs rows each: A (posedirs) gathered from the swizzled box, B (features) from
+//                        shared memory.  CTAs are persistent over a contiguous range of row tiles.
 //
 // The rest of the vertex forward (template + shape blend shapes in fp32, linear blend skinning, box partials) is
 // skin_kernel / skin_small_kernel below.
@@ -34,6 +32,7 @@
 #include <cudaTypedefs.h>
 
 #include <algorithm>
+#include <type_traits>
 #include "mvs_internal.cuh"
 #include "mvs_tc_dev.cuh"
 
@@ -54,11 +53,6 @@ posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_
     constexpr uint32_t kFBytes = tc_fbytes(NF), kStageBytes = tc_stage_bytes(NF);
     pdl_wait();
     extern __shared__ unsigned char smem_raw[];
-    unsigned char* sR = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    // ring: kTcStages x (posedirs fp32 [128 rows][128 B] | features hi [NF rows][128 B] | features lo), all 1024-aligned
-    uint64_t* full = reinterpret_cast<uint64_t*>(sR + (size_t)kTcStages * kStageBytes);      // [stages]
-    uint64_t* empty = full + kTcStages;                                                      // [stages]
-
     const int na = *na_ptr;
     const int f0 = blockIdx.y * kTcCols;                              // this CTA's column tile of frames
     if (f0 >= na) return;
@@ -74,31 +68,19 @@ posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) TC_MARK(0);
 
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kTcStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
+    const Ring<kStageBytes> ring = ring_setup<kStageBytes>(smem_raw, kTcRows / kTcWgRows);
     if (threadIdx.x == 0) TC_MARK(1);
 
     if (warp == 8) {
-        if (lane == 0) {
-            // ---------------- TMA producer.  Rows past 3N (last row tile) are zero-filled by the tensor map; feature rows
-            // past the active frames hold stale slots, which only feed accumulator columns that are never stored.
-            // lo parts of the features: rows ldA.. of PhiTc (same tensor map, row offset)
-            int stage = 0; uint32_t phase = 0;
-            for (int tile = tile_begin; tile < tile_end; ++tile) {
-                for (int kc = 0; kc < kTcKCh; ++kc) {
-                    if (!mbar_wait(&empty[stage], phase ^ 1, err_flag)) return;
-                    unsigned char* sP = sR + (size_t)stage * kStageBytes;
-                    mbar_expect_tx(&full[stage], kStageBytes);
-                    tma_load_2d(sP, &map_p, kc * kTcBK, tile * kTcRows, &full[stage]);
-                    tma_load_2d(sP + kTcPBytes, &map_f, kc * kTcBK, f0, &full[stage]);
-                    tma_load_2d(sP + kTcPBytes + kFBytes, &map_f, kc * kTcBK, ldA + f0, &full[stage]);
-                    if (++stage == kTcStages) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
+        // ---------------- TMA producer.  Rows past 3N (last row tile) are zero-filled by the tensor map; feature rows past
+        // the active frames hold stale slots, which only feed accumulator columns that are never stored.  lo parts of the
+        // features: rows ldA.. of PhiTc (same tensor map, row offset)
+        if (lane == 0)
+            ring_produce<kTcKCh>(ring, tile_begin, tile_end, err_flag, [&](int tile, int kc, unsigned char* sP, uint64_t* bar) {
+                tma_load_2d(sP, &map_p, kc * kTcBK, tile * kTcRows, bar);
+                tma_load_2d(sP + kTcPBytes, &map_f, kc * kTcBK, f0, bar);
+                tma_load_2d(sP + kTcPBytes + kFBytes, &map_f, kc * kTcBK, ldA + f0, bar);
+            });
         return;
     }
 
@@ -111,22 +93,19 @@ posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_
     float acc[NF / 2];
 #pragma unroll
     for (int i = 0; i < NF / 2; ++i) acc[i] = 0.f;
-    int stage = 0; uint32_t phase = 0;
+    RingPos pos;
     for (int tile = tile_begin; tile < tile_end; ++tile) {
         int held = 0;                                                 // ring stage read by the wgmma group in flight
 #pragma unroll
         for (int kc = 0; kc < kTcKCh; ++kc) {
-            // a timeout raises the error flag (the host reports it) and the warpgroup carries on: leaving the loop here
-            // would be a divergent exit with a wgmma group in flight, which makes ptxas serialise every group
-            mbar_wait(&full[stage], phase, err_flag);
+            ring.wait_full(pos, err_flag);
             if (kc == 0 && tile == tile_begin && wt == 0) TC_MARK(2);
-            const unsigned char* sP = sR + (size_t)stage * kStageBytes;
+            // (spelled out: through Ring::stage, ptxas allocates the unrolled k8 steps' registers differently)
+            const unsigned char* sP = ring.base + (size_t)pos.stage * kStageBytes;
             const uint32_t bh = smem_u32(sP + kTcPBytes), bl = bh + kFBytes;
 #pragma unroll
             for (int k = 0; k < kTcBK / 8; ++k) {
-                // A fragment of the k8 step, split x = hi + lo (tf32_split: round to nearest, ties away, as the host-side
-                // split of the earlier pre-split copy did); columns k >= 207 hold shape blend shapes and the template in
-                // Qk and enter as zero
+                // A fragment of the k8 step; columns k >= 207 hold shape blend shapes and the template in Qk and enter as zero
                 uint32_t ahi[4], alo[4];
 #pragma unroll
                 for (int v = 0; v < 4; ++v) {
@@ -143,16 +122,13 @@ posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_
                 WgmmaTf32Rs<NF>::mma(acc, ahi, wgmma_desc_k_sw128(bl + k * 32), 1u);
                 WgmmaTf32Rs<NF>::mma(acc, alo, wgmma_desc_k_sw128(bh + k * 32), 1u);
                 wgmma_commit();
-                // one group in flight while the next fragment is split; once the first group of this chunk is issued,
-                // every group of the previous chunk has retired and its ring stage goes back to the producer
                 wgmma_wait1();
-                if (k == 0 && kc > 0) mbar_arrive_if(&empty[held], wt == 0);
+                if (k == 0 && kc > 0) mbar_arrive_if(&ring.empty[held], wt == 0);
             }
-            held = stage;
-            if (++stage == kTcStages) { stage = 0; phase ^= 1; }
+            held = pos.next();
         }
         wgmma_wait0();
-        mbar_arrive_if(&empty[held], wt == 0);
+        mbar_arrive_if(&ring.empty[held], wt == 0);
         if (wt == 0) TC_MARK(3 + (tile - tile_begin));
         // d[4 i + 2 h + j] = poffT[row tile + frow + 8 h][f0 + 8 i + 2 q + j]: 32-byte row segments per quad.  Slots past
         // the active count are not stored (ldA is a multiple of 64, so a pair that starts below na stays inside the row).
@@ -178,20 +154,16 @@ posedirs_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_
 // (a contiguous range of 32-row chunks) for column tile c and writes its partial into the feature columns of
 // part[s][slot][288 ..] -- the per-strip layout frame_bwd_kernel reduces, in strip order, next to the skinning partials
 // vertex_bwd_kernel<true> wrote.  No atomics: the sum has a fixed order, so a call gives the same bits every time.
-//   warp 16              TMA producer (one thread): per 32-row chunk the seven 32 x 32 boxes of Qk (fp32, straight from the
-//                        model's rows) and the frames' dVp hi and lo boxes (written split by vertex_bwd_kernel<true>), through
-//                        a 4-stage mbarrier ring.
-//   warpgroups 0 .. 3    the A fragment (Qk^T: feature x row) gathered from the swizzled boxes and split into TF32 hi and lo in
-//                        registers; B (dVp) from shared memory; the 3xTF32 products of posedirs_gemm_tc_kernel.
+//   ring                 the TMA / wgmma ring of mvs_tc_dev.cuh.  Warp 16 is its producer: per 32-row chunk the seven 32 x 32
+//                        boxes of Qk (fp32, the model's rows) and the frames' dVp hi and lo boxes (vertex_bwd_kernel<true>).
+//   warpgroups 0 .. 3    its consumers: A (Qk^T: feature x row) gathered from the swizzled boxes, B (dVp) from shared memory.
 constexpr int kTbRows = 32;                                 // posedirs rows per ring stage (the reduction chunk)
 constexpr int kTbBoxes = kFeatPad / 32;                     // 7 boxes of 32 features per row chunk
 constexpr int kTbQBytes = kTbBoxes * kTbRows * 128;         // 28 KB of Qk per stage
 constexpr int kTbWg = 4;                                    // consumer warpgroups
 constexpr int kTbThreads = 128 * kTbWg + 32;                // + the producer warp
-constexpr int kTbStages = 4;
 constexpr int kTbCols = 64;                                 // largest frame column tile (wgmma N)
-__host__ __device__ constexpr int tb_stage_bytes(int nf) { return kTbQBytes + 2 * tc_fbytes(nf); }
-__host__ __device__ constexpr size_t tb_smem(int nf) { return 1024 + (size_t)kTbStages * tb_stage_bytes(nf) + 256; }
+__host__ __device__ constexpr int tb_stage_bytes(int nf) { return kTbQBytes + 2 * tc_fbytes(nf); }   // Qk boxes | dVp hi | lo
 __host__ __device__ constexpr int tb_dvp_ld(int N) { return (3 * N + 3) / 4 * 4; }       // 16-byte rows for the tensor map
 
 template <int NF>
@@ -200,9 +172,6 @@ vertex_bwd_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
                      const int* __restrict__ na_ptr, int nchunks, float* __restrict__ part, int* __restrict__ err_flag) {
     constexpr uint32_t kFBytes = tc_fbytes(NF), kStageBytes = tb_stage_bytes(NF);
     extern __shared__ unsigned char smem_raw[];
-    unsigned char* sR = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = reinterpret_cast<uint64_t*>(sR + (size_t)kTbStages * kStageBytes);
-    uint64_t* empty = full + kTbStages;
     const int na = *na_ptr;
     const int f0 = blockIdx.y * NF;
     if (f0 >= na) return;
@@ -210,24 +179,14 @@ vertex_bwd_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
     const int per = (nchunks + gridDim.x - 1) / gridDim.x;
     const int c_begin = min(strip * per, nchunks), c_end = min(c_begin + per, nchunks);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        for (int st = 0; st < kTbStages; ++st) { mbar_init(&full[st], 1); mbar_init(&empty[st], kTbWg); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
+    const Ring<kStageBytes> ring = ring_setup<kStageBytes>(smem_raw, kTbWg);
     if (warp == 4 * kTbWg) {
-        if (lane == 0) {               // TMA producer; rows past 3N (last chunk) are zero-filled by both tensor maps
-            int stage = 0; uint32_t phase = 0;
-            for (int kc = c_begin; kc < c_end; ++kc) {
-                if (!mbar_wait(&empty[stage], phase ^ 1, err_flag)) return;
-                unsigned char* sP = sR + (size_t)stage * kStageBytes;
-                mbar_expect_tx(&full[stage], kStageBytes);
-                for (int bx = 0; bx < kTbBoxes; ++bx) tma_load_2d(sP + bx * kTbRows * 128, &map_q, 32 * bx, kc * kTbRows, &full[stage]);
-                tma_load_2d(sP + kTbQBytes, &map_d, kc * kTbRows, f0, &full[stage]);
-                tma_load_2d(sP + kTbQBytes + kFBytes, &map_d, kc * kTbRows, ldA + f0, &full[stage]);
-                if (++stage == kTbStages) { stage = 0; phase ^= 1; }
-            }
-        }
+        if (lane == 0)                 // TMA producer; rows past 3N (last chunk) are zero-filled by both tensor maps
+            ring_produce<1>(ring, c_begin, c_end, err_flag, [&](int kc, int, unsigned char* sP, uint64_t* bar) {
+                for (int bx = 0; bx < kTbBoxes; ++bx) tma_load_2d(sP + bx * kTbRows * 128, &map_q, 32 * bx, kc * kTbRows, bar);
+                tma_load_2d(sP + kTbQBytes, &map_d, kc * kTbRows, f0, bar);
+                tma_load_2d(sP + kTbQBytes + kFBytes, &map_d, kc * kTbRows, ldA + f0, bar);
+            });
         return;
     }
     // consumer warpgroup g: features 64 g + 16 w + lr (+ 8), w = warp of the warpgroup, lr = lane / 4; rows q, q + 4 of each k8
@@ -238,11 +197,13 @@ vertex_bwd_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
     float acc[NF / 2];
 #pragma unroll
     for (int i = 0; i < NF / 2; ++i) acc[i] = 0.f;
-    int stage = 0, held = -1; uint32_t phase = 0;
+    RingPos pos;
+    int held = -1;                                            // ring stage read by the wgmma group in flight
     for (int kc = c_begin; kc < c_end; ++kc) {
-        mbar_wait(&full[stage], phase, err_flag);            // on a timeout the flag is raised and the warpgroup carries on
-        const unsigned char* sQ = sR + (size_t)stage * kStageBytes + box * kTbRows * 128;
-        const uint32_t bh = smem_u32(sR + (size_t)stage * kStageBytes + kTbQBytes), bl = bh + kFBytes;
+        ring.wait_full(pos, err_flag);
+        const unsigned char* sS = ring.stage(pos.stage);
+        const unsigned char* sQ = sS + box * kTbRows * 128;
+        const uint32_t bh = smem_u32(sS + kTbQBytes), bl = bh + kFBytes;
 #pragma unroll
         for (int k = 0; k < kTbRows / 8; ++k) {
             uint32_t ahi[4], alo[4];
@@ -262,10 +223,9 @@ vertex_bwd_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
             WgmmaTf32Rs<NF>::mma(acc, alo, wgmma_desc_k_sw128(bh + k * 32), 1u);
             wgmma_commit();
             wgmma_wait1();                                    // the previous chunk's groups have retired: its stage is free
-            if (k == 0 && held >= 0) mbar_arrive_if(&empty[held], wt == 0);
+            if (k == 0 && held >= 0) mbar_arrive_if(&ring.empty[held], wt == 0);
         }
-        held = stage;
-        if (++stage == kTbStages) { stage = 0; phase ^= 1; }
+        held = pos.next();
     }
     wgmma_wait0();
     // d[4 i + 2 h + j] = dPhi^T[feature fa + 8 h][frame f0 + 8 i + 2 q + j]
@@ -523,10 +483,17 @@ sdf_setup_kernel(const SdfSetupArgs sa, const float* bboxp, const float* verts, 
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-constexpr int kTcInstances[] = {8, 16, 32, 64, 128};       // wgmma N instances of posedirs_gemm_tc_kernel
-constexpr int kTcNumInst = 5;
+constexpr int kTcInstances[] = {8, 16, 32, 64, 128};       // wgmma N instances (frames per column tile); the VJP has the first 4
+constexpr int kTcNumInst = 5, kTbNumInst = 4;
+static_assert(kTcInstances[kTcNumInst - 1] == kTcCols && kTcInstances[kTbNumInst - 1] == kTbCols, "instances up to the column tiles");
 
-constexpr int kTbNumInst = 4;                               // wgmma N instances of vertex_bwd_tc_kernel: 8, 16, 32, 64
+// f(std::integral_constant<int, kTcInstances[I]>(), I) for the instance equal to nf; the kernel templates are instantiated
+// for the instances up to kMax only.  Returns f's error, cudaErrorInvalidValue if no instance matches.
+template <int kMax, int I = 0, class F>
+static cudaError_t with_instance(int nf, F f) {
+    if constexpr (I == kTcNumInst || kTcInstances[I] > kMax) return cudaErrorInvalidValue;
+    else return nf == kTcInstances[I] ? f(std::integral_constant<int, kTcInstances[I]>(), I) : with_instance<kMax, I + 1>(nf, f);
+}
 
 struct TcState {
     CUtensorMap map_p;              // fp32 posedirs: the model's Qk rows [3N][224], box 128 rows x 32
@@ -584,16 +551,15 @@ int tc_set_attributes(mvs_ctx* ctx) {
     if ((rc = encode_map(ctx, &T->map_p, ctx->m.Qk, (uint64_t)3 * ctx->m.N, kTcRows))) return rc;
     for (int i = 0; i < kTcNumInst; ++i)                                                           // hi rows, then lo rows
         if ((rc = encode_map(ctx, &T->map_f[i], w.PhiTc, (uint64_t)2 * w.ldA, kTcInstances[i]))) return rc;
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(8)));
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(16)));
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(32)));
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(64)));
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(posedirs_gemm_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem(128)));
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(skin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSkinSmem));
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_tc_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tb_smem(8)));
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tb_smem(16)));
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tb_smem(32)));
-    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(vertex_bwd_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tb_smem(64)));
+    constexpr cudaFuncAttribute kSmem = cudaFuncAttributeMaxDynamicSharedMemorySize;
+    for (int nf : kTcInstances)
+        MVS_CUDA_OK(ctx, with_instance<kTcCols>(nf, [&](auto n, int) {
+                        cudaError_t e = cudaFuncSetAttribute(posedirs_gemm_tc_kernel<n>, kSmem, (int)ring_smem(tc_stage_bytes(n)));
+                        if constexpr (n <= kTbCols)
+                            if (e == cudaSuccess) e = cudaFuncSetAttribute(vertex_bwd_tc_kernel<n>, kSmem, (int)ring_smem(tb_stage_bytes(n)));
+                        return e;
+                    }));
+    MVS_CUDA_OK(ctx, cudaFuncSetAttribute(skin_kernel, kSmem, (int)kSkinSmem));
     return MVS_OK;
 }
 
@@ -621,24 +587,16 @@ int launch_vertex_bwd_tc(mvs_ctx* ctx, int nstrips, cudaStream_t st) {
     const int nchunks = (3 * ctx->m.N + kTbRows - 1) / kTbRows;
     const int nf = std::min(tc_cols_for(w.B), kTbCols);
     const dim3 grid(nstrips, (w.B + nf - 1) / nf);
-    const int inst = nf == 8 ? 0 : nf == 16 ? 1 : nf == 32 ? 2 : 3;
-#define MVS_TB_LAUNCH(NF) vertex_bwd_tc_kernel<NF><<<grid, kTbThreads, tb_smem(NF), st>>>(T->map_q, T->map_d[inst], w.ldA, w.na, nchunks, w.part, T->err)
-    MVS_LAUNCH(ctx, KID_VERTEX_BWD, st,
-               if (nf == 8) MVS_TB_LAUNCH(8); else if (nf == 16) MVS_TB_LAUNCH(16); else if (nf == 32) MVS_TB_LAUNCH(32);
-               else MVS_TB_LAUNCH(64));
-#undef MVS_TB_LAUNCH
+    MVS_LAUNCH(ctx, KID_VERTEX_BWD, st, MVS_CUDA_OK(ctx, with_instance<kTbCols>(nf, [&](auto n, int i) {
+                   vertex_bwd_tc_kernel<n><<<grid, kTbThreads, ring_smem(tb_stage_bytes(n)), st>>>(T->map_q, T->map_d[i], w.ldA, w.na,
+                                                                                              nchunks, w.part, T->err);
+                   return cudaSuccess;
+               })));
     MVS_CUDA_OK(ctx, cudaGetLastError());
     return MVS_OK;
 }
 
 float* tc_poffT(mvs_ctx* ctx) { return ctx->tc->poffT; }
-
-template <int NF>
-static cudaError_t launch_gemm(mvs_ctx* ctx, const TcState* T, int inst, dim3 grid, cudaStream_t st, int ntiles) {
-    const Workspace& w = ctx->ws;
-    return launch_pdl(posedirs_gemm_tc_kernel<NF>, grid, dim3(kTcThreads), tc_smem(NF), st, T->map_p, T->map_f[inst], w.ldA,
-                      3 * ctx->m.N, (const int*)w.na, ctx->sm_count, ntiles, T->poffT, T->err);
-}
 
 int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool sdf_setup) {
     TcState* T = ctx->tc;
@@ -660,12 +618,10 @@ int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool s
     const int ntiles = (3 * m.N + kTcRows - 1) / kTcRows;
     const int nf = tc_cols_for(nb);
     dim3 grid(std::min(ctx->sm_count, ntiles), (nb + kTcCols - 1) / kTcCols);   // surplus CTAs exit: the kernel splits the tiles from *na
-    MVS_LAUNCH(ctx, KID_VERTEX_FWD_TC, st,
-               MVS_CUDA_OK(ctx, nf == 8    ? launch_gemm<8>(ctx, T, 0, grid, st, ntiles)
-                                : nf == 16 ? launch_gemm<16>(ctx, T, 1, grid, st, ntiles)
-                                : nf == 32 ? launch_gemm<32>(ctx, T, 2, grid, st, ntiles)
-                                : nf == 64 ? launch_gemm<64>(ctx, T, 3, grid, st, ntiles)
-                                           : launch_gemm<128>(ctx, T, 4, grid, st, ntiles)));
+    MVS_LAUNCH(ctx, KID_VERTEX_FWD_TC, st, MVS_CUDA_OK(ctx, with_instance<kTcCols>(nf, [&](auto n, int i) {
+                   return launch_pdl(posedirs_gemm_tc_kernel<n>, grid, dim3(kTcThreads), ring_smem(tc_stage_bytes(n)), st, T->map_p,
+                                     T->map_f[i], w.ldA, 3 * m.N, (const int*)w.na, ctx->sm_count, ntiles, T->poffT, T->err);
+               })));
     const int nchunks = (m.N + kSkinV - 1) / kSkinV, fgroups = (nb + 31) / 32;
     const SkinArgs sa{T->poffT, m.ST, w.Phi, w.At, w.ldA, m.ell_j, m.ell_w, m.KW, m.N, need_vposed ? w.vposed : nullptr, w.verts, w.bboxp,
                       setup_in_skin ? sd : SdfSetupArgs{}};
@@ -688,10 +644,10 @@ int launch_vertex_fwd_tc(mvs_ctx* ctx, cudaStream_t st, bool need_vposed, bool s
 
 int tc_check_error(mvs_ctx* ctx) {          // host-side check after a synchronisation point
     TcState* T = ctx->tc;
-    if (!T->poffT) return MVS_OK;                  // the kernel has never run
+    if (!T->poffT) return MVS_OK;                  // no tensor-core kernel has run
     int e = 0;
     MVS_CUDA_OK(ctx, cudaMemcpy(&e, T->err, sizeof(int), cudaMemcpyDeviceToHost));
-    if (e) return set_error(ctx, MVS_ERR_CUDA, "vertex_fwd_tc_kernel: mbarrier wait timed out (pipeline protocol error)");
+    if (e) return set_error(ctx, MVS_ERR_CUDA, "tensor-core pipeline: an mbarrier wait of the TMA / wgmma ring timed out (protocol error)");
     return MVS_OK;
 }
 

@@ -1,6 +1,6 @@
-// Device-side building blocks of the tensor-core vertex forward (mvs_tc.cu): mbarrier / TMA / wgmma wrappers, tile
-// constants, and the one vertex routine every skinning variant calls (so that a frame gets the same bits whichever
-// kernel evaluated it).
+// Device-side building blocks of the tensor-core kernels (mvs_tc.cu): mbarrier / TMA / wgmma wrappers, tile constants, the
+// TMA / wgmma ring both contractions share, and the one vertex routine every skinning variant calls (so that a frame gets
+// the same bits whichever kernel evaluated it).
 #pragma once
 #include <cuda.h>
 #include "mvs_internal.cuh"
@@ -15,14 +15,13 @@ constexpr int kTcWgRows = 64;         // posedirs rows per consumer warpgroup
 constexpr int kTcCols = 128;          // frames per column tile (largest wgmma N instance used); larger batches run several
 constexpr int kTcBK = 32;             // floats per 128-byte swizzle row
 constexpr int kTcKCh = kFeatPad / kTcBK;   // 7 K chunks
-constexpr int kTcStages = 4;          // ring stages of (posedirs chunk | feature hi chunk | feature lo chunk)
 constexpr int kTcPBytes = kTcRows * kTcBK * 4;     // 16 KB fp32 posedirs per stage (split into TF32 hi | lo on chip)
 constexpr int kTcThreads = 288;       // warpgroups 0, 1: convert + wgmma + store, 64 rows each; warp 8: TMA producer
 // frame columns of one launch (wgmma N): the active-frame bound rounded up to 8, 16, 32, 64 or 128
 __host__ __device__ constexpr int tc_cols_for(int nb) { return nb <= 8 ? 8 : nb <= 16 ? 16 : nb <= 32 ? 32 : nb <= 64 ? 64 : 128; }
 __host__ __device__ constexpr int tc_fbytes(int nf) { return nf * kTcBK * 4; }            // one feature chunk (hi or lo): nf rows of 128 B
+// ring stage: posedirs chunk | feature hi chunk | feature lo chunk
 __host__ __device__ constexpr int tc_stage_bytes(int nf) { return kTcPBytes + 2 * tc_fbytes(nf); }
-__host__ __device__ constexpr size_t tc_smem(int nf) { return 1024 /*align slack*/ + (size_t)kTcStages * tc_stage_bytes(nf) + 256 /*barriers*/; }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -31,9 +30,6 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 // arrive if `pred`, as a predicated instruction rather than a branch (no divergent path between in-flight wgmma groups)
 __device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
@@ -59,12 +55,6 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
-}
-// shared -> global tile store (bulk async group of the issuing thread); the tensor map clips the box at the tensor's bounds
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                 ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
 // wgmma shared-memory matrix descriptor: K-major, 128-byte swizzle, rows of 128 B packed 8 per 1024 B
 // (start >> 4, LBO = 1 (unused for swizzled K-major), SBO = 1024 B, layout type 1 = SWIZZLE_128B)
@@ -166,6 +156,61 @@ template <> struct WgmmaTf32Rs<128> {
     }
 };
 
+// ------------------------------------------------------------------------------------------------ the TMA / wgmma ring
+// Both tensor-core kernels stream their operands through kRingStages stages of kStageBytes, 1024-byte aligned (the period
+// of the 128-byte swizzle), with a `full` and an `empty` mbarrier per stage.  One producer thread waits until a stage is
+// empty, arms `full` with the stage's byte count and issues its TMA boxes (ring_produce).  Each consumer warpgroup waits
+// until the stage is full (Ring::wait_full), runs its k8 steps on it (A split into TF32 hi + lo, hi.Bhi, hi.Blo, lo.Bhi as
+// one wgmma group, one group kept in flight by wait_group 1) and hands it back with one predicated arrival on `empty` once
+// every group that read it has retired: after the next stage's first group, or after wait_group 0 at the end.
+constexpr int kRingStages = 4;
+__host__ __device__ constexpr size_t ring_smem(int stage_bytes) { return 1024 /*align slack*/ + (size_t)kRingStages * stage_bytes + 256 /*barriers*/; }
+
+struct RingPos {                      // a thread's stage and the parity of its pass; next() moves on, returns the stage left
+    int stage = 0;
+    uint32_t phase = 0;
+    __device__ __forceinline__ int next() { const int s = stage; if (++stage == kRingStages) { stage = 0; phase ^= 1; } return s; }
+};
+
+template <uint32_t kStageBytes>
+struct Ring {
+    unsigned char* base;              // stage s at base + s * kStageBytes
+    uint64_t* full;                   // [kRingStages] completed by the producer's expect_tx and the TMA bytes
+    uint64_t* empty;                  // [kRingStages] one arrival per consumer warpgroup
+    __device__ __forceinline__ unsigned char* stage(int s) const { return base + (size_t)s * kStageBytes; }
+    // consumer: wait for stage p to be full.  A timeout raises the error flag (the host reports it) and the warpgroup carries
+    // on: leaving the loop would be a divergent exit with a wgmma group in flight, which makes ptxas serialise every group
+    __device__ __forceinline__ void wait_full(const RingPos& p, int* err_flag) const { mbar_wait(&full[p.stage], p.phase, err_flag); }
+};
+
+// By the whole CTA: the ring in the dynamic shared memory (ring_smem bytes), its barriers set for `consumers` warpgroups.
+template <uint32_t kStageBytes>
+__device__ __forceinline__ Ring<kStageBytes> ring_setup(unsigned char* smem_raw, uint32_t consumers) {
+    Ring<kStageBytes> r;
+    r.base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    r.full = reinterpret_cast<uint64_t*>(r.stage(kRingStages));
+    r.empty = r.full + kRingStages;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kRingStages; ++s) { mbar_init(&r.full[s], 1); mbar_init(&r.empty[s], consumers); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    return r;
+}
+
+// The producer (one thread): ring steps (item, chunk), item in [item_begin, item_end), chunk in [0, kChunks).  issue(item,
+// chunk, dst, bar) issues the step's TMA boxes into the stage at dst, completing on bar.  Returns once a wait timed out.
+template <int kChunks, uint32_t kStageBytes, class Issue>
+__device__ __forceinline__ void ring_produce(const Ring<kStageBytes>& r, int item_begin, int item_end, int* err_flag, Issue issue) {
+    RingPos p;
+    for (int item = item_begin; item < item_end; ++item)
+        for (int chunk = 0; chunk < kChunks; ++chunk) {
+            if (!mbar_wait(&r.empty[p.stage], p.phase ^ 1, err_flag)) return;
+            mbar_expect_tx(&r.full[p.stage], kStageBytes);
+            issue(item, chunk, r.stage(p.stage), &r.full[p.stage]);
+            p.next();
+        }
+}
 
 // One vertex of one frame: v_posed = template + shapedirs.betas + pose offset, then linear blend skinning
 // (lbs.py:179,203,207-220).  skin_kernel (lane = frame) and skin_small_kernel (lane = vertex) both call this with every
