@@ -461,7 +461,6 @@ int launch_forward_vjp(mvs_ctx* ctx, const float* x_dev, const float* djoints, c
                        cudaStream_t st);
 // mvs_resident.cu: frame-resident (one CTA per frame) closure and whole-stage optimiser for the sparse regime
 bool resident_supported(const mvs_ctx* ctx);   // the model fits the frame-resident kernels
-bool dense_supported(const mvs_ctx* ctx);      // the mesh fits frame_step's list of 256-vertex blocks
 int launch_vposer_decode(mvs_ctx* ctx, const float* x_dev, float* body_pose_dev, cudaStream_t st);
 int launch_closure_resident(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* grad_dev, float* joints_dev,
                             float* proj_dev, cudaStream_t st);

@@ -367,7 +367,7 @@ struct RunOpts {
 static Regime stage_regime(const mvs_ctx* ctx, const LossParams& lp, int history, bool step) {
     if (ctx->exec_mode == 1 || !resident_supported(ctx)) return kBatched;
     if (!sdf_term_on(lp)) return !step && history <= 100 ? kResident : kBatched;
-    return (!step || lp.use_vposer == 2) && dense_supported(ctx) ? kDense : kBatched;
+    return !step || lp.use_vposer == 2 ? kDense : kBatched;
 }
 
 static bool resident_closure_applies(const mvs_ctx* ctx, bool want_verts) {
@@ -623,8 +623,7 @@ int evaluate_closure(mvs_ctx* ctx, const float* x_dev, float* loss_dev, float* g
                      float* verts_dev, cudaStream_t st) {
     if (resident_closure_applies(ctx, verts_dev != nullptr))
         return launch_closure_resident(ctx, x_dev, loss_dev, grad_dev, joints_dev, proj_dev, st);
-    if (ctx->exec_mode == 3 && sdf_term_on(ctx->loss) && !joints_dev && !proj_dev && !verts_dev && resident_supported(ctx) &&
-        dense_supported(ctx))
+    if (ctx->exec_mode == 3 && sdf_term_on(ctx->loss) && !joints_dev && !proj_dev && !verts_dev && resident_supported(ctx))
         return dense_regime_closure(ctx, x_dev, loss_dev, grad_dev, st);
     if (ctx->loss.use_vposer == 2)
         return set_error(ctx, MVS_ERR_INVALID, "use_vposer = 2 (VPoser decode on the device) is implemented in the "

@@ -304,8 +304,6 @@ bool resident_supported(const mvs_ctx* ctx) {
            ctx->vmax * m.K <= kResMaxVK && m.M <= kResMaxM;
 }
 
-bool dense_supported(const mvs_ctx* ctx) { return (ctx->m.N + 255) / 256 <= 64; }     // frame_step's block list holds 64 entries
-
 // dynamic shared memory of lbfgs_resident_kernel and frame_step_kernel: one frame, history H (+ the VPoser decoder)
 static size_t frame_smem(int H, bool with_vposer) {
     return sizeof(ResidentSmem) + (size_t)2 * H * kParams * sizeof(float) + (with_vposer ? sizeof(VposerSmem) : 0);

@@ -19,6 +19,7 @@ constexpr int kResMaxSupJ = 512;          // (support vertex, joint) pairs with 
 constexpr int kResMaxVK = 272;            // views x keypoints (16 x 17)
 constexpr int kResMaxM = 8;               // GMM components
 constexpr int kResMaxKpE = 256;           // (keypoint, support vertex) entries staged in shared memory
+constexpr int kFlagList = 64;             // penetration-flagged 256-vertex blocks listed in shared memory (16384 vertices)
 // resident_closure splits the CTA from P4 to P10: warps 0-5 run the data term and its adjoint, warps 6-7 the part of the
 // priors that only needs the pose (GMM mat-vec and log-likelihoods, |theta|^2).  Each group syncs on its own named barrier;
 // warp 6 then joins the data warps for P8.
@@ -111,7 +112,7 @@ struct ResidentSmem {
     int ext_n[8];
     float ext_d[24];
     float sdf_sc[4];                       // [0] cg / scale, [1] pen loss, [2] number of extreme entries
-    int fl[64], nfl;                       // 256-vertex blocks with a penetration adjoint partial
+    int fl[kFlagList], nfl;                // 256-vertex blocks with a penetration adjoint partial (the first kFlagList), count
     LossParams lp;                         // this frame's CURRENT stage (multi-stage kernels)
     FrameScalars fs;
 };
@@ -134,8 +135,8 @@ struct DenseIn {
     float pen_loss;
     const float* Wd;          // [N][24] dense skinning weights (adjoint of the extra vertices)
     const float* part;        // [nblocks][512] this frame's unit-factor partial adjoints, or NULL (no penetration)
-    const int* fl;            // [nfl] blocks that wrote partials, ascending
-    int nfl;
+    const int* fl;            // nfl <= kFlagList: [nfl] blocks that wrote partials, ascending; else [nblocks] flag per block
+    int nfl;                  // number of blocks that wrote partials
     float factor;             // cg / scale: d pen / d (sum of samples) over the box scale
     bool pose_ready;          // R, J, Gam, g, A of this trial point are already in shared memory (frame_step's pose cache)
 };
@@ -343,6 +344,18 @@ static __device__ void vposer_decode_bwd(const ResidentModel& m, VposerSmem& W) 
     __syncthreads();
 }
 
+// sum over the flagged blocks, ascending, of entry e of their unit-factor partials.  A frame with more flagged blocks than
+// the list holds walks the blocks' flags up to the last flagged one: the same terms added in the same order.
+__device__ __forceinline__ float pen_partial_sum(const DenseIn& din, int e) {
+    if (din.nfl <= kFlagList)
+        return serial_sum8(din.nfl, [&](int q) { return din.part[(size_t)din.fl[q] * kPartFloats + e]; });
+    float a = 0.f;
+#pragma unroll 1
+    for (int p = 0, q = 0; q < din.nfl; ++p)
+        if (din.fl[p] != 0) { a += din.part[(size_t)p * kPartFloats + e]; ++q; }
+    return a;
+}
+
 // P8 of the closure for feature column k: dPhi[k] = sum_col dvp[col] Qk[row(col)][k] in ascending col, then the
 // penetration partials.  32 independent L2 loads in flight: the phase is as long as its round trips to L2 (258 rows: 8
 // instead of 21).
@@ -365,8 +378,7 @@ __device__ __forceinline__ void dphi_col(ResidentSmem& S, const ResidentModel& m
     }
     for (; col < ncol_all; ++col) a = fmaf(S.dvp[col], __ldg(m.Qk + (size_t)S.rowbase[col] * kFeatPad + k), a);
     if (din.part) {
-        const float pa = serial_sum8(din.nfl, [&](int q) { return din.part[(size_t)din.fl[q] * kPartFloats + kSkinFloats + k]; });
-        a = fmaf(pa, din.factor, a);
+        a = fmaf(pen_partial_sum(din, kSkinFloats + k), din.factor, a);
     }
     S.dPhi[k] = a;
 }
@@ -677,8 +689,7 @@ static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m,
                     }
                 }
                 if (din.part) {                                    // penetration gradient: unit-factor block partials
-                    const float pa = serial_sum8(din.nfl, [&](int q) { return din.part[(size_t)din.fl[q] * kPartFloats + e]; });
-                    a = fmaf(pa, din.factor, a);
+                    a = fmaf(pen_partial_sum(din, e), din.factor, a);
                 }
                 S.dA[e] = a;
             }
@@ -1014,10 +1025,10 @@ frame_step_kernel(FrameStepArgs a, const int* __restrict__ fidx, const int* __re
             const int p = p0 + lane;
             const bool f = p < nparts && pflag[(size_t)slot * nparts + p] != 0;
             const unsigned mk = __ballot_sync(0xffffffffu, f);
-            if (f) { const int pos = nfl + __popc(mk & ((1u << lane) - 1u)); if (pos < 64) S.fl[pos] = p; }
+            if (f) { const int pos = nfl + __popc(mk & ((1u << lane) - 1u)); if (pos < kFlagList) S.fl[pos] = p; }
             nfl += __popc(mk);
         }
-        if (lane == 0) S.nfl = nfl < 64 ? nfl : 64;
+        if (lane == 0) S.nfl = nfl;
     }
     cp_async_wait_group<1>();                          // group 0: the frame state the closure starts from
     __syncthreads();
@@ -1032,7 +1043,7 @@ frame_step_kernel(FrameStepArgs a, const int* __restrict__ fidx, const int* __re
     din.Wd = Wd;
     din.factor = S.sdf_sc[0];
     din.part = (din.factor != 0.f && S.nfl > 0) ? part + (size_t)slot * nparts * kPartFloats : nullptr;
-    din.fl = S.fl;
+    din.fl = S.nfl <= kFlagList ? S.fl : pflag + (size_t)slot * nparts;
     din.nfl = S.nfl;
     din.pose_ready = pose_ready;
     resident_closure(S, m, rig, S.lp, gt_uv, conf, joint_w, B, b, true, nullptr, nullptr, din, W);

@@ -169,6 +169,17 @@ def rotmat_to_aa(R):
     return aa
 
 
+def sdf_bin_entries(tri):
+    """the entry counts of mvs_sdf_bins.cuh's candidate lists for tri [F,3,3] float32 box coordinates, and which capacity they
+    exceed: (cell_entries, ray_entries, rc) with rc 0 (both fit), 1 (kBinCapD) or 2 (kBinCapR)"""
+    lib = _build()
+    tri = np.ascontiguousarray(tri, dtype=np.float32).reshape(-1, 9)
+    ev = np.zeros(4, np.int64)
+    lib.hostsim_sdf_bins.restype = ctypes.c_int
+    rc = lib.hostsim_sdf_bins(ctypes.c_int(tri.shape[0]), _P(tri), ctypes.c_int(16), ctypes.c_long(0), None, None, None, _P(ev))
+    return int(ev[2]), int(ev[3]), int(rc)
+
+
 def sdf_bins(tri, G, voxel_ids, brute=True):
     """mvs_sdf_bins.cuh on the host: tri [F,3,3] float32 box coordinates -> (phi over candidate lists, phi by brute force or None,
     dict(ray_evals, dist_evals, cell_entries, ray_entries))"""

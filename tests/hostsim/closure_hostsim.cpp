@@ -363,6 +363,7 @@ int hostsim_sdf_bins(int F, const float* tri, int G, long n, const long* vox, fl
     }
     for (int i = 0; i < kBinCells; ++i) cell_cnt[i + 1] += cell_cnt[i];
     for (int i = 0; i < kBinRays; ++i) ray_cnt[i + 1] += ray_cnt[i];
+    evals[0] = evals[1] = 0; evals[2] = cell_cnt[kBinCells]; evals[3] = ray_cnt[kBinRays];
     if (cell_cnt[kBinCells] > kBinCapD) return 1;
     if (ray_cnt[kBinRays] > kBinCapR) return 2;
     std::vector<unsigned short> cell_idx(cell_cnt[kBinCells] + 1), ray_idx(ray_cnt[kBinRays] + 1);
@@ -379,7 +380,6 @@ int hostsim_sdf_bins(int F, const float* tri, int G, long n, const long* vox, fl
         for (int x = rl[0]; x <= rh[0]; ++x) for (int y = rl[1]; y <= rh[1]; ++y) ray_idx[rc[x * kBinR + y]++] = (unsigned short)f;
     }
     v.tri = tri; v.cell_ptr = cell_cnt.data(); v.cell_idx = cell_idx.data(); v.ray_ptr = ray_cnt.data(); v.ray_idx = ray_idx.data();
-    evals[0] = evals[1] = 0; evals[2] = cell_cnt[kBinCells]; evals[3] = ray_cnt[kBinRays];
     for (long q = 0; q < n; ++q) {
         const long id = vox[q];
         float c[3];

@@ -28,15 +28,43 @@ LSP_ROWS = sorted({int(s) for s in S.JOINT_MAP_LSP14 if s < 14})        # the 12
 
 
 def limits() -> dict:
-    """the kernels' envelope constants, read from the CUDA headers"""
+    """the kernels' envelope and tiling constants, read from the CUDA sources (`= 64;` and `= 1 << 17;` forms)"""
     out = {}
-    for f in ("mvs_resident_dev.cuh", "mvs_tc_dev.cuh", "mvs_math.cuh"):
+    for f in ("mvs_resident_dev.cuh", "mvs_tc_dev.cuh", "mvs_math.cuh", "mvs_tc.cu", "mvs_sdf_dev.cuh", "mvs_internal.cuh",
+              "mvs_sdf_bins.cuh"):
         src = open(os.path.join(CSRC, f)).read()
-        for k, v in re.findall(r"constexpr\s+int\s+(k\w+)\s*=\s*(\d+)\s*;", src):
-            out[k] = int(v)
+        for k, a, s in re.findall(r"constexpr\s+int\s+(k\w+)\s*=\s*(\d+)\s*(?:<<\s*(\d+)\s*)?;", src):
+            out[k] = int(a) << int(s or 0)
     m = re.search(r"m\.nsup\s*\+\s*(\d+)\s*<=\s*kResMaxSup", open(os.path.join(CSRC, "mvs_resident.cu")).read())
     out["kResExtraSup"] = int(m.group(1))          # resident_supported(): room for the box-extreme vertices
     return out
+
+
+def tails(N: int, lim: dict | None = None) -> dict:
+    """host mirror of the vertex-count-dependent tiling of the dense kernels at N vertices"""
+    lim = lim or limits()
+    rows = 3 * N
+    last = rows % lim["kTcRows"] or lim["kTcRows"]          # rows of the last posedirs tile
+    nbox = -(-N // lim["kSkinV"])                           # 64-vertex skinning chunks = chunk boxes
+    return dict(
+        tc_tiles=-(-rows // lim["kTcRows"]),                # posedirs_gemm_tc 128-row tiles
+        tc_last_rows=last,
+        tc_last_wg1_rows=max(0, last - lim["kTcRows"] // 2),   # rows of warpgroup 1 in the last tile (0: idle)
+        nbox=nbox,
+        chunk_tail=N % lim["kSkinV"],                       # vertices of a partial last chunk (0: none)
+        setup_groups=-(-nbox // (32 * lim["kSetupCh"])),    # sdf_frame_setup fold-loop trips
+        cull=nbox <= 32 * lim["kSdfSkipWords"],             # chunk-cull bits cover every chunk
+        sdf_blocks=-(-N // lim["kSdfFThreads"]),            # 256-vertex blocks of sdf_fused = partials frame_step sums
+        block_tail=N % lim["kSdfFThreads"],
+        tb_chunks=-(-rows // lim["kTbRows"]),               # vertex_bwd_tc 32-row reduction chunks
+        tb_pad=(rows + 3) // 4 * 4 - rows,                  # tb_dvp_ld(N) - 3N
+        simt_tail=N % lim["kTileV"],                        # vertices of the SIMT kernels' partial last tile
+    )
+
+
+def sdf_passes_for(na: int, nblocks: int, cta_slots: int) -> int:
+    """csrc/mvs_internal.cuh sdf_passes_for: 256-vertex blocks per sdf_fused CTA (cta_slots = 3 x SM count)"""
+    return 2 if na * nblocks > 2 * cta_slots else 1
 
 
 def bookkeeping(model, model_type="smpllsp", joint_map=None, extra_vertex_ids=None) -> dict:
@@ -146,6 +174,71 @@ def _skin_rows(model, verts, counts):
         W[n] = 0.0
         W[n, js] = (w / w.sum()).astype(np.float32)
     return W
+
+
+# ------------------------------------------------------------------------------------------------- meshes of other sizes
+# N -> what the size reaches in the dense kernels (tests/test_model_sizes.py asserts each from tails() and limits())
+SIZES = (431, 1723, 6890, 6912, 6913, 6944, 10475, 27554)
+
+
+def make_sized_model(n_verts: int, seed: int = 0):
+    """(model, extra_vertex_ids): a body model of n_verts vertices built the way synthetic.make_model builds its own (a
+    Fibonacci sphere in height bands, its convex hull with F = 2N - 4 outward faces, J_regressor, <= 4 skinning weights per
+    vertex, shapedirs and posedirs from the same draws; at 6890 and seed 0 all of these are make_model(0)'s).  Keypoints: every
+    non-zero LSP regressor row of make_model(0) is rebuilt on the vertices nearest the point it regresses in the rest pose
+    (as many as it has non-zeros, Gaussian weights, non-negative, sums to 1), and the 5 face keypoints become the vertices
+    nearest make_model(0)'s face vertices."""
+    from scipy.spatial import ConvexHull
+    N, J = n_verts, S.NUM_JOINTS
+    rng = np.random.RandomState(seed)
+    pts = S._fibonacci_sphere(N)
+    pts = pts + rng.normal(0.0, 2e-3, size=pts.shape)
+    pts /= np.linalg.norm(pts, axis=1, keepdims=True)
+    band = np.floor((pts[:, 1] + 1.0) * 20.0)
+    pts = pts[np.lexsort((np.arctan2(pts[:, 2], pts[:, 0]), band))]
+    vt = pts * np.array([0.25, 0.85, 0.15])
+    faces = ConvexHull(pts).simplices.astype(np.int64)
+    a, b, c = pts[faces[:, 0]], pts[faces[:, 1]], pts[faces[:, 2]]
+    flip = np.einsum("ij,ij->i", np.cross(b - a, c - a), a + b + c) < 0
+    faces[flip] = faces[flip][:, [0, 2, 1]]
+    faces = faces[np.lexsort((faces[:, 2], faces[:, 1], faces[:, 0]))]
+    assert faces.shape == (2 * N - 4, 3)
+    d2 = ((vt[None, :, :] - S._skeleton_rest()[:, None, :]) ** 2).sum(-1)          # [24, N]
+    Jreg = np.zeros((J, N))
+    for j in range(J):
+        idx = np.argsort(d2[j])[:64]
+        w = np.exp(-(d2[j, idx] - d2[j, idx].min()) / (2 * 0.05 ** 2)) * rng.uniform(0.5, 1.0, size=64)
+        Jreg[j, idx] = w / w.sum()
+    weights = np.zeros((N, J))
+    near = np.argsort(d2.T, axis=1)[:, :4]
+    dn = np.take_along_axis(d2.T, near, axis=1)
+    w = np.exp(-(dn - dn[:, :1]) / (2 * 0.06 ** 2))
+    w[w < 1e-3] = 0.0
+    w /= w.sum(1, keepdims=True)
+    np.put_along_axis(weights, near, w, axis=1)
+    shapedirs = rng.normal(0.0, 0.01, size=(N, 3, S.NUM_BETAS))
+    posedirs = rng.normal(0.0, 0.001, size=(N, 3, S.NUM_POSE_BASIS)).astype(np.float32)
+    kintree = np.zeros((2, J), dtype=np.uint32)
+    kintree[0] = S.SMPL_PARENTS.astype(np.int64) % (2 ** 32)
+    kintree[1] = np.arange(J)
+    # keypoints where make_model(0)'s regress them in the rest pose
+    base_vt = S.make_model(0, with_faces=False)["v_template"].astype(np.float64)
+    base_reg = S.load_lsp_regressor().astype(np.float64)
+    lsp = np.zeros((base_reg.shape[0], N), dtype=np.float64)
+    for r in range(base_reg.shape[0]):
+        own = np.flatnonzero(base_reg[r])
+        if len(own) == 0:
+            continue
+        centre = base_reg[r, own] @ base_vt[own]
+        dd = ((vt - centre) ** 2).sum(1)
+        idx = np.argsort(dd, kind="stable")[:len(own)]
+        w = np.exp(-(dd[idx] - dd[idx].min()) / (2 * 0.03 ** 2)) + 1e-3
+        lsp[r, idx] = w / w.sum()
+    extra = tuple(int(np.argmin(((vt - base_vt[v]) ** 2).sum(1))) for v in S.FACE_VERTEX_IDS)
+    model = dict(v_template=vt.astype(np.float32), f=faces.astype(np.int32), shapedirs=shapedirs.astype(np.float32),
+                 posedirs=posedirs, J_regressor=Jreg.astype(np.float32), kintree_table=kintree,
+                 weights=weights.astype(np.float32), lsp_regressor=lsp.astype(np.float32))
+    return model, extra
 
 
 FACE18 = tuple(int(v) for v in S.FACE_VERTEX_IDS)
