@@ -104,6 +104,20 @@ int mvs_set_cameras(mvs_ctx* ctx, int num_views, const float* R, const float* t,
 int mvs_set_camera_rigs(mvs_ctx* ctx, int n_rigs, const int* num_views, const float* R, const float* t, const float* f,
                         const float* c, const float* data_weight_scale);
 
+/* ---- mvs_set_camera_rigs with lens distortion: dist [n_rigs,Vmax,5] (host) holds each view's OpenCV projectPoints coefficients
+ *      (k1, k2, p1, p2, k3); rows v >= num_views[r] are not read.  With x' = x/z, y' = y/z, r2 = x'^2 + y'^2 and
+ *      a = 1 + k1 r2 + k2 r2^2 + k3 r2^3 every projection is
+ *          u = fx (x' a + 2 p1 x'y' + p2 (r2 + 2 x'^2)) + cx,   v = fy (y' a + p1 (r2 + 2 y'^2) + 2 p2 x'y') + cy
+ *      with no clamp: fits are only meaningful inside the calibrated field of view, where this map is monotone.  It serves the
+ *      2-D term of every closure and fitting driver, mvs_init_guess (which undistorts each detection with non-zero confidence
+ *      before it triangulates or takes the one-view depth guess) and mvs_refine_cameras (the coefficients are held, like f and
+ *      c, and the refined table keeps them).  A rig whose coefficients are all zero is evaluated exactly as without them.
+ *      Otherwise the same as mvs_set_camera_rigs (same validation, waits for the device, keypoints and per-slot rigs must be
+ *      set again); MVS_ERR_INVALID naming the rig and view if a coefficient is not finite.  mvs_set_camera_rigs is this call
+ *      with dist = NULL. */
+int mvs_set_camera_rigs_dist(mvs_ctx* ctx, int n_rigs, const int* num_views, const float* R, const float* t, const float* f,
+                             const float* c, const float* dist, const float* data_weight_scale);
+
 /* The rig of every slot of the batch: rig_host [B] (HOST ints in [0, n_rigs)), validated and copied before return (waits for
  *      the device first).  Read by mvs_closure, mvs_lbfgs_run, mvs_lbfgs_step, mvs_fit, mvs_fit_seq, mvs_fit_host and
  *      mvs_init_guess.  With more than one rig, those entry points return MVS_ERR_INVALID unless per-slot rigs were given

@@ -74,7 +74,7 @@ class SequenceStream(ctypes.Structure):
 
 EXPORTS = (
     "mvs_version", "mvs_build_id", "mvs_create", "mvs_destroy", "mvs_last_error", "mvs_launch_count", "mvs_set_model",
-    "mvs_set_gmm_prior", "mvs_set_vposer", "mvs_vposer_decode", "mvs_set_cameras", "mvs_set_camera_rigs", "mvs_set_frame_rigs", "mvs_set_batch", "mvs_set_keypoints", "mvs_set_loss_config",
+    "mvs_set_gmm_prior", "mvs_set_vposer", "mvs_vposer_decode", "mvs_set_cameras", "mvs_set_camera_rigs", "mvs_set_camera_rigs_dist", "mvs_set_frame_rigs", "mvs_set_batch", "mvs_set_keypoints", "mvs_set_loss_config",
     "mvs_closure", "mvs_forward", "mvs_forward_vjp", "mvs_lbfgs_run", "mvs_lbfgs_step", "mvs_fit", "mvs_fit_seq", "mvs_fit_stream", "mvs_fit_seq_stream", "mvs_fit_seq_stream3d",
     "mvs_fit_stream_rigs", "mvs_fit_seq_stream_rigs", "mvs_fit_host", "mvs_sdf_grid", "mvs_profile", "mvs_profile_read",
     "mvs_kernel_name", "mvs_set_exec_mode", "mvs_set_anchor", "mvs_set_joints3d", "mvs_init_guess", "mvs_fit_seq_temporal",
@@ -108,6 +108,7 @@ def load() -> ctypes.CDLL:
     lib.mvs_set_gmm_prior.argtypes = [vp, ci, vp, vp, vp]
     lib.mvs_set_cameras.argtypes = [vp, ci, vp, vp, vp, vp]
     lib.mvs_set_camera_rigs.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp]
+    lib.mvs_set_camera_rigs_dist.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp]
     lib.mvs_set_frame_rigs.argtypes = [vp, vp]
     lib.mvs_set_batch.argtypes = [vp, ci]
     lib.mvs_set_keypoints.argtypes = [vp, vp, vp, vp, ci, vp]

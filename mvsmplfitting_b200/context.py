@@ -140,7 +140,10 @@ class FittingContext:
         _lib.check(self.h, self.lib.mvs_vposer_decode(self.h, _ptr(params), _ptr(out), self._stream()), "mvs_vposer_decode")
         return out
 
-    def set_cameras(self, R, t, f, c):
+    def set_cameras(self, R, t, f, c, dist=None):
+        """One rig of V views (mvs_set_cameras); dist [V,5] OpenCV coefficients (k1, k2, p1, p2, k3) per view or None (none)"""
+        if dist is not None:
+            return self.set_camera_rigs([dict(R=R, t=t, f=f, c=c, dist=dist)])
         R, t, f, c = _f32(R), _f32(t), _f32(f), _f32(c)
         self.V = R.shape[0]
         _lib.check(self.h, self.lib.mvs_set_cameras(self.h, self.V, _ptr(R), _ptr(t), _ptr(f), _ptr(c)), "mvs_set_cameras")
@@ -151,7 +154,9 @@ class FittingContext:
         """A table of camera rigs (mvs_set_camera_rigs): rigs is a list of dict(R [V_r,3,3], t [V_r,3], f [V_r,2], c [V_r,2])
         such as seqio.camera_arrays returns; data_weight_scale [n_rigs] multiplies every stage's data_weight for the frames
         of each rig (None: all 1).  Detection arrays then have V = max V_r view rows; rows v >= V_r of a frame with rig r are
-        not read.  Name each slot's rig with set_frame_rigs, or each frame's with fit_stream / fit_seq_stream(rig=...)."""
+        not read.  Name each slot's rig with set_frame_rigs, or each frame's with fit_stream / fit_seq_stream(rig=...).
+        A rig dict may carry "dist" [V_r,5]: its views' lens distortion, OpenCV's (k1, k2, p1, p2, k3)
+        (mvs_set_camera_rigs_dist); a rig without it has none."""
         if not rigs:
             raise ValueError("set_camera_rigs: want at least one rig")
         nv = [int(np.asarray(r["R"]).shape[0]) for r in rigs]
@@ -165,10 +170,23 @@ class FittingContext:
         if scale is not None and scale.shape[0] != len(rigs):
             raise ValueError("set_camera_rigs: %d rigs, %d data-weight scales" % (len(rigs), scale.shape[0]))
         nva = _i32(nv)
-        _lib.check(self.h, self.lib.mvs_set_camera_rigs(self.h, len(rigs), _ptr(nva), _ptr(R), _ptr(t), _ptr(f), _ptr(c),
-                                                        _ptr(scale)), "mvs_set_camera_rigs")
+        has_dist = [r.get("dist") is not None for r in rigs]
+        if any(has_dist):
+            for i, (r, n) in enumerate(zip(rigs, nv)):
+                if r.get("dist") is not None and np.shape(r["dist"]) != (n, 5):
+                    raise ValueError("set_camera_rigs: rig %d has %d views, dist of shape %s (want [%d,5])"
+                                     % (i, n, np.shape(r["dist"]), n))
+            dist = _f32(np.stack([pad(r["dist"] if h else np.zeros((n, 5)), n, (5,)) for r, n, h in zip(rigs, nv, has_dist)]))
+            _lib.check(self.h, self.lib.mvs_set_camera_rigs_dist(self.h, len(rigs), _ptr(nva), _ptr(R), _ptr(t), _ptr(f), _ptr(c),
+                                                                 _ptr(dist), _ptr(scale)), "mvs_set_camera_rigs_dist")
+        else:
+            _lib.check(self.h, self.lib.mvs_set_camera_rigs(self.h, len(rigs), _ptr(nva), _ptr(R), _ptr(t), _ptr(f), _ptr(c),
+                                                            _ptr(scale)), "mvs_set_camera_rigs")
         self.V, self.rig_views = V, nv
         self._rigs = [dict(R=R[r, :n].copy(), t=t[r, :n].copy(), f=f[r, :n].copy(), c=c[r, :n].copy()) for r, n in enumerate(nv)]
+        for r, h in enumerate(has_dist):
+            if h:
+                self._rigs[r]["dist"] = dist[r, :nv[r]].copy()
 
     def set_frame_rigs(self, rig):
         """the rig of every slot of the batch (mvs_set_frame_rigs): rig [B] ints in [0, n_rigs)"""
@@ -450,7 +468,7 @@ class FittingContext:
         rows in, result out; gt_uv [V,F,K,2], conf [V,F,K], joint_weights [K], joints3d / conf3d and rig as in fit_stream.  The
         context keeps the refined cameras; afterwards it holds no keypoints, no 3-D targets and no per-slot rigs.  Returns
         (final_loss [F], rigs, camera_stats, pose_stats), rigs: the refined table as the list of dict(R, t, f, c) that
-        set_camera_rigs takes (same views per rig, f and c unchanged)."""
+        set_camera_rigs takes (same views per rig, f, c and any "dist" unchanged)."""
         assert params.is_cuda and params.dtype == torch.float32 and params.is_contiguous() and params.dim() == 2
         F = params.shape[0]
         if isinstance(sweeps, bool) or int(sweeps) != sweeps or sweeps < 1:

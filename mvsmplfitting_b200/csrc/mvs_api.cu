@@ -526,8 +526,8 @@ int mvs_set_vposer(mvs_ctx* ctx, const float* fc1_w, const float* fc1_b, const f
                                const_array(m.vp_b1, fc1_b, H), const_array(m.vp_b2, fc2_b, H), const_array(m.vp_b3, out_b, O)});
 }
 
-int mvs_set_camera_rigs(mvs_ctx* ctx, int n_rigs, const int* num_views, const float* R, const float* t, const float* f,
-                        const float* c, const float* data_weight_scale) {
+int mvs_set_camera_rigs_dist(mvs_ctx* ctx, int n_rigs, const int* num_views, const float* R, const float* t, const float* f,
+                             const float* c, const float* dist, const float* data_weight_scale) {
     if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
     MVS_REQUIRE(ctx, n_rigs > 0 && num_views && R && t && f && c, "mvs_set_camera_rigs: need n_rigs >= 1 and the camera arrays");
     int vmax = 0;
@@ -539,6 +539,13 @@ int mvs_set_camera_rigs(mvs_ctx* ctx, int n_rigs, const int* num_views, const fl
                     data_weight_scale ? data_weight_scale[r] : 1.f);
         vmax = std::max(vmax, num_views[r]);
     }
+    if (dist)
+        for (int r = 0; r < n_rigs; ++r)
+            for (int v = 0; v < num_views[r]; ++v)
+                for (int k = 0; k < 5; ++k)
+                    MVS_REQUIRE(ctx, isfinite(dist[((size_t)r * vmax + v) * 5 + k]),
+                                "mvs_set_camera_rigs_dist: rig %d view %d has distortion coefficient %d = %g (want finite)", r, v, k,
+                                dist[((size_t)r * vmax + v) * 5 + k]);
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     std::vector<Rig> rigs((size_t)n_rigs);
     for (int r = 0; r < n_rigs; ++r) {
@@ -552,6 +559,10 @@ int mvs_set_camera_rigs(mvs_ctx* ctx, int n_rigs, const int* num_views, const fl
             memcpy(g.cam[v].t, t + 3 * i, 3 * sizeof(float));
             memcpy(g.cam[v].f, f + 2 * i, 2 * sizeof(float));
             memcpy(g.cam[v].c, c + 2 * i, 2 * sizeof(float));
+            if (!dist) continue;
+            const float* d = dist + 5 * i;
+            g.dist[v] = Dist{d[0], d[1], d[2], d[3], d[4], {0.f, 0.f, 0.f}};
+            for (int k = 0; k < 5; ++k) g.distorted |= d[k] != 0.f;  // all zero: the pinhole instructions, bit for bit
         }
     }
     // no kernel may still read the table it replaces
@@ -564,6 +575,11 @@ int mvs_set_camera_rigs(mvs_ctx* ctx, int n_rigs, const int* num_views, const fl
     ctx->have_kp = false;                                   // keypoints are per view: must be set again
     ctx->slot_rigs = nullptr;                               // so are the slots' rigs
     return MVS_OK;
+}
+
+int mvs_set_camera_rigs(mvs_ctx* ctx, int n_rigs, const int* num_views, const float* R, const float* t, const float* f,
+                        const float* c, const float* data_weight_scale) {
+    return mvs_set_camera_rigs_dist(ctx, n_rigs, num_views, R, t, f, c, nullptr, data_weight_scale);
 }
 
 int mvs_set_cameras(mvs_ctx* ctx, int V, const float* R, const float* t, const float* f, const float* c) {

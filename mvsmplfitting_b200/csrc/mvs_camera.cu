@@ -14,9 +14,11 @@ __device__ __noinline__ void build_camera(const CamRefine& cr, const float* w, c
 }
 
 // One warp per work item (problem slot, frame of its rig), lane = keypoint.  The frame's view term is resident_closure P6's for
-// that view: the same projection, weights, GMoF and dw^2, the keypoints' terms added in keypoint order.  Its gradient with
-// respect to the camera (R, t) is summed over the keypoints, then taken back to the problem's variables.
-__global__ void __launch_bounds__(128)
+// that view: the same projection (with the view's distortion, held like f and c), weights, GMoF and dw^2, the keypoints' terms
+// added in keypoint order.  Its gradient with respect to the camera (R, t) is summed over the keypoints, then taken back to the
+// problem's variables.  At most 64 registers, so that eight 128-thread CTAs stay resident per SM: the out-of-line distorted
+// projection would otherwise take the kernel to 68 (allocated as 72: seven CTAs); at 64 it does not spill.
+__global__ void __launch_bounds__(128, 8)
 camera_closure_kernel(LossParams lp, LbfgsState L, CameraArgs a, ProblemChunk ch) {
     const int lane = threadIdx.x & 31;
     const int item = ch.i0 + blockIdx.x * 4 + (threadIdx.x >> 5);
@@ -35,6 +37,7 @@ camera_closure_kernel(LossParams lp, LbfgsState L, CameraArgs a, ProblemChunk ch
     const Rig& rig = a.rigs[P.rig];
     cam.f[0] = rig.cam[P.view].f[0]; cam.f[1] = rig.cam[P.view].f[1];
     cam.c[0] = rig.cam[P.view].c[0]; cam.c[1] = rig.cam[P.view].c[1];
+    const Dist* dp = rig.distorted ? rig.dist + P.view : nullptr;    // the view's distortion (NULL: none), held like f and c
     const float dw = lp.data_weight * rig.dw_scale;
     const float rho2 = lp.rho * lp.rho, dw2 = dw * dw;
     float lterm = 0.f, g[12];
@@ -44,7 +47,7 @@ camera_closure_kernel(LossParams lp, LbfgsState L, CameraArgs a, ProblemChunk ch
         const float* q = a.q + ((size_t)f * K + lane) * 3;
         const float qk[3] = {q[0], q[1], q[2]};
         float xc[3], uv[2];
-        project_fwd(cam, qk, xc, uv);
+        project_fwd(cam, qk, xc, uv, dp);
         const size_t o = ((size_t)P.view * F + f) * K + lane;
         float wk = a.in.joint_w[lane];
         if (lp.use_joints_conf) wk *= a.in.conf[o];
@@ -55,7 +58,7 @@ camera_closure_kernel(LossParams lp, LbfgsState L, CameraArgs a, ProblemChunk ch
         lterm = w2 * g0 + w2 * g1;
         const float duv[2] = {-(w2 * d0) * dw2, -(w2 * d1) * dw2};
         float dx[3];
-        project_bwd_x(cam, xc, duv, dx);
+        project_bwd_x(cam, xc, duv, dx, dp);
 #pragma unroll
         for (int r = 0; r < 3; ++r) {
 #pragma unroll

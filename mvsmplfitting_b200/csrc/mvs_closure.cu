@@ -266,7 +266,7 @@ keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, 
     const int b = fidx[slot];
     const int t = threadIdx.x;
     // with_views == 0 (joints / vertices only): no rig, no detections read
-    const FrameRig rig = with_views ? frame_rig(rigs, b) : FrameRig{nullptr, 0, 1.f};
+    const FrameRig rig = with_views ? frame_rig(rigs, b) : FrameRig{nullptr, 0, 1.f, nullptr};
     const int K = km.K, V = rig.num_views;                         // V: the views of this frame's rig
     __shared__ float q[kMaxKeypoints * 3];
     __shared__ float dq[kMaxKeypoints * 3];
@@ -302,7 +302,8 @@ keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, 
         const int v = idx / K, k = idx % K;
         float xc[3], uv[2];
         const CamF cam = rig_camera(rig, v);
-        project_fwd(cam, &q[3 * k], xc, uv);
+        const Dist* dp = rig.dist ? rig.dist + v : nullptr;          // this view's distortion (NULL: none)
+        project_fwd(cam, &q[3 * k], xc, uv, dp);
         const size_t o = ((size_t)v * B + b) * K + k;
         if (proj_out) { proj_out[2 * o] = uv[0]; proj_out[2 * o + 1] = uv[1]; }
         float w = joint_w[k];
@@ -314,7 +315,7 @@ keypoint_loss_kernel(const float* __restrict__ x, const int* __restrict__ fidx, 
         lterm[idx] = w2 * g0 + w2 * g1;
         const float duv[2] = {-(w2 * d0) * dw2, -(w2 * d1) * dw2};
         float dqv[3] = {0.f, 0.f, 0.f};
-        project_bwd(cam, xc, duv, dqv);
+        project_bwd(cam, xc, duv, dqv, dp);
         contrib[3 * idx] = dqv[0]; contrib[3 * idx + 1] = dqv[1]; contrib[3 * idx + 2] = dqv[2];
     }
     __syncthreads();

@@ -4,6 +4,7 @@
 //   1. rest joints: the model's keypoints at zero pose, zero shape, scale = fixed_scale  (init_guess.py:29-52)
 //      -- the library's own forward pass on a seeded parameter block;
 //   2. triangulation of the K keypoints from the V views                                 (recompute3D.py:24-61)
+//      (a rig with lens distortion: every detection with non-zero confidence undistorted first, mvs_init.cuh undistort_px)
 //   3. similarity alignment rest joints -> triangulated joints, torso joints only by default (init_guess.py:80-85),
 //      rotation -> axis-angle (:86), and the parameter block fix_params leaves behind (:190-212).
 //
@@ -47,11 +48,12 @@ __global__ void __launch_bounds__(128) init_guess_kernel(float* __restrict__ par
         } else if (cams.num_views == 1) {                 // init_guess.py:54-78: depth guess along the optical axis
             double rj[kMaxKeypoints * 3];
             for (int i = 0; i < K * 3; ++i) rj[i] = (double)rest[i];
-            const double d = single_view_depth<double>(cams.cam[0], rj, gt_uv + (size_t)b * K * 2, conf + (size_t)b * K);
+            const double d = single_view_depth<double>(cams.cam[0], rj, gt_uv + (size_t)b * K * 2, conf + (size_t)b * K,
+                                                       cams.dist);
             for (int c = 0; c < 3; ++c) X[c] = rj[3 * lane + c] + d * (double)cams.cam[0].R[6 + c];
         } else {
             triangulate_point<double>(cams, gt_uv + ((size_t)b * K + lane) * 2, conf + (size_t)b * K + lane, (long)B * K * 2,
-                                      (long)B * K, X);
+                                      (long)B * K, X, cams.dist);
         }
         dst[3 * lane] = X[0]; dst[3 * lane + 1] = X[1]; dst[3 * lane + 2] = X[2];
         if (joints3d) {

@@ -50,6 +50,27 @@ template <class T, class C> MVS_HD void ray_normal_eq(const C& cam, T u, T v, T 
     }
 }
 
+// A detection (u, v) of a view with lens distortion d, taken to the ideal (pinhole) pixel that project_fwd without distortion
+// would give: invert (x', y') -> (x'', y'') (mvs_math.cuh distort_norm) by kUndistortSteps Newton steps from (x'', y'') with the
+// 2x2 Jacobian.  A fixed count, no convergence test: every thread runs the same steps (deterministic).  Converges inside the
+// monotone region of the map (the calibrated field of view).
+constexpr int kUndistortSteps = 10;
+template <class T, class C> MVS_HD void undistort_px(const C& cam, const Dist& d, T u, T v, T* uu, T* vu) {
+    const T fx = T(cam.f[0]), fy = T(cam.f[1]), cx = T(cam.c[0]), cy = T(cam.c[1]);
+    const T xd = (u - cx) / fx, yd = (v - cy) / fy;
+    T xn = xd, yn = yd;
+    for (int it = 0; it < kUndistortSteps; ++it) {
+        T ex, ey, J[4];
+        distort_norm(d, xn, yn, &ex, &ey, J);
+        ex -= xd; ey -= yd;
+        const T det = J[0] * J[3] - J[1] * J[2];
+        xn -= (J[3] * ex - J[1] * ey) / det;
+        yn -= (J[0] * ey - J[2] * ex) / det;
+    }
+    *uu = xn * fx + cx;
+    *vu = yn * fy + cy;
+}
+
 // x = M^-1 b for a 3x3 system, Gaussian elimination with partial pivoting (what np.linalg.solve / LAPACK gesv does)
 template <class T> MVS_HD void solve3(const T* M, const T* b, T* x) {
     T a[3][4] = {{M[0], M[1], M[2], b[0]}, {M[3], M[4], M[5], b[1]}, {M[6], M[7], M[8], b[2]}};
@@ -77,11 +98,17 @@ template <class T> MVS_HD void solve3(const T* M, const T* b, T* x) {
 
 // recompute3D.py:24-61 for ONE keypoint: (u, v) of view w at uv[w * stride_uv + {0, 1}], its confidence at
 // conf[w * stride_conf].  CS: anything with .num_views and .cam[w] (R, t, f, c).  X[3] = world point.
+// dist [num_views] or NULL (no distortion): a detection with non-zero confidence is undistorted first (undistort_px); one with
+// confidence 0 is used as it stands (its weight is 1e-6, and a zero row far outside the field may have no preimage).
 template <class T, class CS> MVS_HD void triangulate_point(const CS& cams, const float* uv, const float* conf,
-                                                           long stride_uv, long stride_conf, T* X) {
+                                                           long stride_uv, long stride_conf, T* X, const Dist* dist = nullptr) {
     T M[9] = {T(0), T(0), T(0), T(0), T(0), T(0), T(0), T(0), T(0)}, b[3] = {T(0), T(0), T(0)};
-    for (int w = 0; w < cams.num_views; ++w)
-        ray_normal_eq<T>(cams.cam[w], T(uv[w * stride_uv]), T(uv[w * stride_uv + 1]), T(conf[w * stride_conf]), M, b);
+    for (int w = 0; w < cams.num_views; ++w) {
+        T u = T(uv[w * stride_uv]), v = T(uv[w * stride_uv + 1]);
+        const float cf = conf[w * stride_conf];
+        if (dist && cf != 0.f) undistort_px<T>(cams.cam[w], dist[w], u, v, &u, &v);
+        ray_normal_eq<T>(cams.cam[w], u, v, T(cf), M, b);
+    }
 #pragma unroll
     for (int k = 0; k < 9; ++k) M[k] = T(float(M[k]));        // AtA.astype(np.float32), recompute3D.py:52
     solve3<T>(M, b, X);
@@ -268,12 +295,17 @@ template <class T> MVS_HD bool umeyama_fit(const T* src, const T* dst, int n, bo
 // torso heights: |j5 - j11| and |j6 - j12| in 3-D (rest joints; camera rotation leaves the norms alone), and in 2-D the
 // L-shoulder -- L-hip difference taken TWICE (:66 repeats torso2d[0] - torso2d[2]) over the detection rows (u, v, conf),
 // i.e. the confidence difference is part of the norm.  joints3d = E^-1 (E j + est_d e_z) = j + est_d * R^T e_z.
-template <class T, class C> MVS_HD T single_view_depth(const C& cam, const T* rest, const float* uv, const float* conf) {
+// dist != NULL: the view's distortion; the two detections with non-zero confidence are undistorted first (undistort_px).
+template <class T, class C> MVS_HD T single_view_depth(const C& cam, const T* rest, const float* uv, const float* conf,
+                                                       const Dist* dist = nullptr) {
+    T p5[2] = {T(uv[10]), T(uv[11])}, p11[2] = {T(uv[22]), T(uv[23])};
+    if (dist && conf[5] != 0.f) undistort_px<T>(cam, *dist, p5[0], p5[1], &p5[0], &p5[1]);
+    if (dist && conf[11] != 0.f) undistort_px<T>(cam, *dist, p11[0], p11[1], &p11[0], &p11[1]);
     const T h3 = (mvs_sqrt((rest[15] - rest[33]) * (rest[15] - rest[33]) + (rest[16] - rest[34]) * (rest[16] - rest[34]) +
                            (rest[17] - rest[35]) * (rest[17] - rest[35])) +
                   mvs_sqrt((rest[18] - rest[36]) * (rest[18] - rest[36]) + (rest[19] - rest[37]) * (rest[19] - rest[37]) +
                            (rest[20] - rest[38]) * (rest[20] - rest[38]))) * T(0.5);
-    const T du = T(uv[10]) - T(uv[22]), dv = T(uv[11]) - T(uv[23]), dc = T(conf[5]) - T(conf[11]);
+    const T du = p5[0] - p11[0], dv = p5[1] - p11[1], dc = T(conf[5]) - T(conf[11]);
     const T h2 = mvs_sqrt(du * du + dv * dv + dc * dc);
     return T(cam.f[0]) * (h3 / h2);
 }

@@ -34,14 +34,19 @@ struct ChainSched {
 };
 
 // One camera rig of the context's table (mvs_set_camera_rigs): its views, their number and the scale of every stage's
-// data_weight for the frames that name it.  Lives in device memory; kernels reach it through frame_rig() only.
+// data_weight for the frames that name it, and its views' lens distortion (mvs_set_camera_rigs_dist).  Lives in device memory;
+// kernels reach it through frame_rig() only.  distorted = 1 iff some coefficient of some view is non-zero: only then do kernels
+// see the coefficients, so a rig without distortion runs the pinhole instructions.
 struct __align__(16) Rig {
     CamF cam[kMaxViews];
     int num_views;
     float dw_scale;
-    int pad[2];
+    int distorted;
+    int pad;
+    Dist dist[kMaxViews];
 };
-static_assert(sizeof(CamF) == 64 && sizeof(Rig) % 16 == 0, "rig layout (float4 loads of a camera)");
+static_assert(sizeof(CamF) == 64 && sizeof(Dist) == 32 && sizeof(Rig) % 16 == 0,
+              "rig layout (float4 loads of a camera and of its distortion)");
 
 // Where a kernel finds each frame's rig: the context's table and the rig index of every row it indexes frames by (frame of
 // a stream, slot of a batch or lane of a dense run); of == NULL: every row has rig 0 (a table of one rig).
@@ -50,16 +55,18 @@ struct RigSet {
     const int* of;
 };
 
-// What a kernel reads of a frame's rig: the rig's cameras (device memory), view count and data-weight scale
+// What a kernel reads of a frame's rig: the rig's cameras (device memory), view count, data-weight scale and the views'
+// distortion (NULL: the rig has none)
 struct FrameRig {
     const CamF* cam;
     int num_views;
     float dw_scale;
+    const Dist* dist;
 };
 #ifdef __CUDACC__
 __device__ __forceinline__ FrameRig frame_rig(const RigSet& rs, int row) {
     const Rig* r = rs.rig + (rs.of ? __ldg(rs.of + row) : 0);
-    return FrameRig{r->cam, __ldg(&r->num_views), __ldg(&r->dw_scale)};
+    return FrameRig{r->cam, __ldg(&r->num_views), __ldg(&r->dw_scale), __ldg(&r->distorted) ? r->dist : nullptr};
 }
 // camera v of a frame's rig, into registers (four 16-byte loads)
 __device__ __forceinline__ CamF rig_camera(const FrameRig& fr, int v) {

@@ -12,8 +12,10 @@
 
 #if defined(__CUDACC__)
 #define MVS_HD __host__ __device__ __forceinline__
+#define MVS_DIST_FN __host__ __device__ __noinline__
 #else
 #define MVS_HD inline
+#define MVS_DIST_FN inline
 #endif
 
 namespace mvs {
@@ -286,31 +288,84 @@ template <class T> MVS_HD void chain_step_bwd(const T* dGam, const T* dg, const 
 // ---------------------------------------------------------------- camera + robust residual
 struct CamF { float R[9]; float t[3]; float f[2]; float c[2]; };
 
-// camera.py:93-117 : x = R q + t ; uv = f * x.xy / x.z + c        (no distortion, no clamp)
-template <class T, class C> MVS_HD void project_fwd(const C& cam, const T* q, T* x, T* uv) {
+// A view's lens distortion (mvs_set_camera_rigs_dist): OpenCV's projectPoints coefficients (k1, k2, p1, p2, k3), two float4
+// per view.  Applied to the normalised coordinates (x', y') = (x/z, y/z):
+//   r2 = x'^2 + y'^2,  a = 1 + k1 r2 + k2 r2^2 + k3 r2^3
+//   x'' = x' a + 2 p1 x'y' + p2 (r2 + 2 x'^2),   y'' = y' a + p1 (r2 + 2 y'^2) + 2 p2 x'y',   uv = f (x'', y'') + c
+// No clamp (as OpenCV): the map is only monotone, and a fit only meaningful, inside the calibrated field of view.
+struct alignas(16) Dist { float k1, k2, p1, p2, k3, pad[3]; };
+
+// (x', y') -> (x'', y'') and, with J != NULL, the Jacobian J = d(x'', y'')/d(x', y') row-major (it is symmetric: J[1] = J[2])
+template <class T> MVS_HD void distort_norm(const Dist& d, T xn, T yn, T* xd, T* yd, T* J = nullptr) {
+    const T k1 = T(d.k1), k2 = T(d.k2), k3 = T(d.k3), p1 = T(d.p1), p2 = T(d.p2);
+    const T r2 = xn * xn + yn * yn, xy = xn * yn;
+    const T a = T(1) + r2 * (k1 + r2 * (k2 + r2 * k3));
+    *xd = xn * a + T(2) * p1 * xy + p2 * (r2 + T(2) * xn * xn);
+    *yd = yn * a + p1 * (r2 + T(2) * yn * yn) + T(2) * p2 * xy;
+    if (J) {
+        const T da = k1 + r2 * (T(2) * k2 + T(3) * k3 * r2);        // d a / d r2
+        J[0] = a + T(2) * xn * xn * da + T(2) * p1 * yn + T(6) * p2 * xn;
+        J[1] = T(2) * xy * da + T(2) * p1 * xn + T(2) * p2 * yn;
+        J[2] = J[1];
+        J[3] = a + T(2) * yn * yn * da + T(6) * p1 * yn + T(2) * p2 * xn;
+    }
+}
+
+// The distorted halves of project_fwd / project_bwd_x, kept out of line on the device: the pinhole path of the kernels that
+// call them keeps its own register allocation, and the distorted path pays a call.
+template <class T> struct Pair { T a, b; };
+template <class T> MVS_DIST_FN Pair<T> distort_px(const Dist* d, T x0, T x1, T x2) {
+    Pair<T> o;
+    distort_norm(*d, x0 / x2, x1 / x2, &o.a, &o.b);
+    return o;
+}
+// (J^T g) / z: the adjoint of (x0, x1) through the divide's numerators, g = d loss / d(x'', y'')
+template <class T> MVS_DIST_FN Pair<T> distort_px_adjoint(const Dist* d, T x0, T x1, T x2, T g0, T g1) {
+    T xd, yd, J[4];
+    distort_norm(*d, x0 / x2, x1 / x2, &xd, &yd, J);
+    const T iz = T(1) / x2;
+    return Pair<T>{(J[0] * g0 + J[2] * g1) * iz, (J[1] * g0 + J[3] * g1) * iz};
+}
+
+// camera.py:93-117 : x = R q + t ; uv = f * x.xy / x.z + c        (no clamp)
+// dist != NULL: uv = f * distort(x.xy / x.z) + c.  dist == NULL evaluates exactly the pinhole expressions.
+template <class T, class C> MVS_HD void project_fwd(const C& cam, const T* q, T* x, T* uv, const Dist* dist = nullptr) {
     const T R0 = cam.R[0], R1 = cam.R[1], R2 = cam.R[2], R3 = cam.R[3], R4 = cam.R[4], R5 = cam.R[5],
             R6 = cam.R[6], R7 = cam.R[7], R8 = cam.R[8];
     x[0] = R0 * q[0] + R1 * q[1] + R2 * q[2] + T(cam.t[0]);
     x[1] = R3 * q[0] + R4 * q[1] + R5 * q[2] + T(cam.t[1]);
     x[2] = R6 * q[0] + R7 * q[1] + R8 * q[2] + T(cam.t[2]);
+    if (dist) {
+        const Pair<T> d = distort_px(dist, x[0], x[1], x[2]);
+        uv[0] = d.a * T(cam.f[0]) + T(cam.c[0]);
+        uv[1] = d.b * T(cam.f[1]) + T(cam.c[1]);
+        return;
+    }
     uv[0] = (x[0] / x[2]) * T(cam.f[0]) + T(cam.c[0]);
     uv[1] = (x[1] / x[2]) * T(cam.f[1]) + T(cam.c[1]);
 }
-// dq += R^T dx, with dx the adjoint of the perspective divide
-template <class T, class C> MVS_HD void project_bwd(const C& cam, const T* x, const T* duv, T* dq) {
+// dx = the camera-space adjoint of the projection: duv through f, the distortion's Jacobian (transposed) when dist != NULL,
+// and the perspective divide
+template <class T, class C> MVS_HD void project_bwd_x(const C& cam, const T* x, const T* duv, T* dx, const Dist* dist = nullptr) {
     const T iz = T(1) / x[2];
-    const T dx0 = duv[0] * T(cam.f[0]) * iz, dx1 = duv[1] * T(cam.f[1]) * iz;
-    const T dx2 = -(dx0 * x[0] + dx1 * x[1]) * iz;
+    if (dist) {
+        const Pair<T> d = distort_px_adjoint(dist, x[0], x[1], x[2], duv[0] * T(cam.f[0]), duv[1] * T(cam.f[1]));
+        dx[0] = d.a;
+        dx[1] = d.b;
+    } else {
+        dx[0] = duv[0] * T(cam.f[0]) * iz;
+        dx[1] = duv[1] * T(cam.f[1]) * iz;
+    }
+    dx[2] = -(dx[0] * x[0] + dx[1] * x[1]) * iz;
+}
+// dq += R^T dx, with dx the adjoint of the projection (project_bwd_x)
+template <class T, class C> MVS_HD void project_bwd(const C& cam, const T* x, const T* duv, T* dq, const Dist* dist = nullptr) {
+    T dx[3];
+    project_bwd_x(cam, x, duv, dx, dist);
+    const T dx0 = dx[0], dx1 = dx[1], dx2 = dx[2];
     dq[0] += T(cam.R[0]) * dx0 + T(cam.R[3]) * dx1 + T(cam.R[6]) * dx2;
     dq[1] += T(cam.R[1]) * dx0 + T(cam.R[4]) * dx1 + T(cam.R[7]) * dx2;
     dq[2] += T(cam.R[2]) * dx0 + T(cam.R[5]) * dx1 + T(cam.R[8]) * dx2;
-}
-// dx = the camera-space adjoint of the perspective divide (the first half of project_bwd)
-template <class T, class C> MVS_HD void project_bwd_x(const C& cam, const T* x, const T* duv, T* dx) {
-    const T iz = T(1) / x[2];
-    dx[0] = duv[0] * T(cam.f[0]) * iz;
-    dx[1] = duv[1] * T(cam.f[1]) * iz;
-    dx[2] = -(dx[0] * x[0] + dx[1] * x[1]) * iz;
 }
 
 // ---------------------------------------------------------------- camera refinement (mvs_refine_cameras, DESIGN.md section 4)

@@ -562,7 +562,8 @@ static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m,
                 const int v = idx / K, k = idx % K;
                 float xc[3], uv[2];
                 const CamF cam = rig_camera(rig, v);
-                project_fwd(cam, &S.q[3 * k], xc, uv);
+                const Dist* dp = rig.dist ? rig.dist + v : nullptr;          // this view's distortion (NULL: none)
+                project_fwd(cam, &S.q[3 * k], xc, uv, dp);
                 const size_t o = ((size_t)v * B + b) * K + k;
                 if (proj_out) { proj_out[2 * o] = uv[0]; proj_out[2 * o + 1] = uv[1]; }
                 float w = joint_w[k];
@@ -574,7 +575,7 @@ static __device__ void resident_closure(ResidentSmem& S, const ResidentModel& m,
                 S.lterm[idx] = w2 * g0 + w2 * g1;
                 const float duv[2] = {-(w2 * d0) * dw2, -(w2 * d1) * dw2};
                 float dqv[3] = {0.f, 0.f, 0.f};
-                project_bwd(cam, xc, duv, dqv);
+                project_bwd(cam, xc, duv, dqv, dp);
                 S.contrib[3 * idx] = dqv[0]; S.contrib[3 * idx + 1] = dqv[1]; S.contrib[3 * idx + 2] = dqv[2];
             }
             data_sync();

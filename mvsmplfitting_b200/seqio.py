@@ -5,6 +5,7 @@ frames of a sequence go through `mvs_init_guess` + `mvs_fit` as one batch instea
 
 Reference interfaces mirrored (file:line of /root/reference/code):
   load_camera_para     utils/utils.py:352-394      camera file -> extrinsics [V,4,4], intrinsics [V,3,3]
+                                                   (load_camera_distortion reads the distortion lines it skips)
   read_keypoints       utils/data_parser.py:42-90  OpenPose-style JSON -> [17,3] (u, v, confidence), body part only
                                                    (use_hands = use_face = False is the only configuration of the path)
   FittingData          utils/data_parser.py:257-433  folder layout <keypoints>/<serial>/<camera>/<frame>_keypoints.json,
@@ -41,15 +42,39 @@ def load_camera_para(path: str):
     return np.array(extris), np.array(intris)
 
 
-def camera_arrays(extris, intris, views=None) -> dict:
+def load_camera_distortion(path: str) -> np.ndarray:
+    """The lens distortion of every view of a camera file, [V,5] float64 (k1, k2, p1, p2, k3) in OpenCV's order: the line
+    between a view's three intrinsic rows and its [R | t] rows, which load_camera_para skips.  A line of 2 numbers is
+    (k1, k2); a line of 5 numbers is OpenCV's (k1, k2, p1, p2, k3); a view without such a line has zeros."""
+    n_intr, dist = 0, {}
+    with open(path) as f:
+        for line in f:
+            words = line.split()
+            if len(words) == 3:
+                n_intr += 1
+            elif len(words) in (2, 5) and n_intr > 0 and n_intr % 3 == 0:
+                d = [float(w) for w in words]
+                dist[n_intr // 3 - 1] = d + [0.0] * (5 - len(d))
+    out = np.zeros((n_intr // 3, 5))
+    for v, d in dist.items():
+        out[v] = d
+    return out
+
+
+def camera_arrays(extris, intris, views=None, dist=None) -> dict:
     """(extrinsics, intrinsics) -> the R [V,3,3], t [V,3], f [V,2], c [V,2] float32 arrays FittingContext.set_cameras
-    takes (what create_camera receives per view at init.py:108-131)."""
+    takes (what create_camera receives per view at init.py:108-131).  dist [V,5] (load_camera_distortion) adds the key
+    "dist" (float32), the views' lens distortion; without it the dict has no such key."""
     extris, intris = np.asarray(extris, np.float64), np.asarray(intris, np.float64)
     if views is not None:
         extris, intris = extris[list(views)], intris[list(views)]
     f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
-    return dict(R=f32(extris[:, :3, :3]), t=f32(extris[:, :3, 3]), f=f32(np.stack([intris[:, 0, 0], intris[:, 1, 1]], 1)),
-                c=f32(np.stack([intris[:, 0, 2], intris[:, 1, 2]], 1)))
+    out = dict(R=f32(extris[:, :3, :3]), t=f32(extris[:, :3, 3]), f=f32(np.stack([intris[:, 0, 0], intris[:, 1, 1]], 1)),
+               c=f32(np.stack([intris[:, 0, 2], intris[:, 1, 2]], 1)))
+    if dist is not None:
+        dist = np.asarray(dist, np.float64).reshape(-1, 5)
+        out["dist"] = f32(dist[list(views)] if views is not None else dist)
+    return out
 
 
 def camera_matrices(cams: dict):
@@ -65,10 +90,12 @@ def camera_matrices(cams: dict):
     return extris, intris
 
 
-def write_camera_para(path: str, extris, intris) -> None:
+def write_camera_para(path: str, extris, intris, dist=None) -> None:
     """A camera file in the reference's layout (what load_camera_para reads): per view its index line, the three intrinsic
-    rows, '0 0' (no distortion), the three [R | t] rows and a blank line.  Numbers are written with repr, so float32 inputs
-    read back as the same float32 values."""
+    rows, the distortion line, the three [R | t] rows and a blank line.  The distortion line is '0 0' when dist is None;
+    with dist [V,5] (k1, k2, p1, p2, k3) it is 'k1 k2', or all five numbers when p1, p2 or k3 is non-zero
+    (load_camera_distortion reads both).  Numbers are written with repr, so float32 inputs read back as the same float32
+    values."""
     extris, intris = np.asarray(extris), np.asarray(intris)
     row = lambda r: " ".join(repr(float(x)) for x in r) + " \n"
     with open(path, "w") as fh:
@@ -76,7 +103,11 @@ def write_camera_para(path: str, extris, intris) -> None:
             fh.write("%d\n" % v)
             for r in intris[v]:
                 fh.write(row(r))
-            fh.write("0 0\n")
+            if dist is None:
+                fh.write("0 0\n")
+            else:
+                d = np.asarray(dist)[v]
+                fh.write(row(d if np.any(d[2:] != 0) else d[:2]))
             for r in extris[v][:3]:
                 fh.write(row(r))
             fh.write("\n")
@@ -449,7 +480,7 @@ def refine_rigs(ctx, params, gt_uv, conf, jw, stage_cfgs, opt_cfg, sweeps, t3=No
     (device, updated in place) of all frames, under the last stage configuration; t3 (_targets_3d of the frames) adds the
     3-D term, rig [F] each frame's rig.  Returns the frames' final losses [F]; stats (a dict) gets 'refine_cameras': the
     refined rigs (camera dicts, as set_camera_rigs takes them) and the camera and body steps' counts.  With result_folder,
-    rig r's refined calibration is written to <result_folder>/cameras_rig<r>.txt (write_camera_para)."""
+    rig r's refined calibration, with its lens distortion, is written to <result_folder>/cameras_rig<r>.txt (write_camera_para)."""
     kw = {} if rig is None else dict(rig=rig)
     if t3 is not None:
         kw.update(joints3d=t3[0], conf3d=t3[1])
@@ -459,7 +490,7 @@ def refine_rigs(ctx, params, gt_uv, conf, jw, stage_cfgs, opt_cfg, sweeps, t3=No
     if result_folder is not None:
         os.makedirs(result_folder, exist_ok=True)
         for r, cams in enumerate(rigs):
-            write_camera_para(os.path.join(result_folder, "cameras_rig%d.txt" % r), *camera_matrices(cams))
+            write_camera_para(os.path.join(result_folder, "cameras_rig%d.txt" % r), *camera_matrices(cams), dist=cams.get("dist"))
     return final
 
 

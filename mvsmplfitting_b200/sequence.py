@@ -110,7 +110,7 @@ class SequenceFitter:
         self.ctx.set_model(model, model_type=model_type)
         if gmm is not None:
             self.ctx.set_gmm_from_dict(gmm)
-        self.ctx.set_cameras(cams["R"], cams["t"], cams["f"], cams["c"])
+        self.ctx.set_cameras(cams["R"], cams["t"], cams["f"], cams["c"], dist=cams.get("dist"))   # lens distortion, if any
         self.ctx.set_batch(self.stop - self.start)
         self.B = self.stop - self.start
 

@@ -301,12 +301,60 @@ def model_keypoints_np(model: dict, betas, global_orient, body_pose, transl, sca
 
 
 def project_np(cams: dict, joints: np.ndarray) -> np.ndarray:
-    """[B,K,3] -> [V,B,K,2] (reference camera.py:102-116)."""
+    """[B,K,3] -> [V,B,K,2] (reference camera.py:102-116); with cams["dist"] [V,5] through each view's lens distortion
+    (OpenCV's k1, k2, p1, p2, k3, as mvs_set_camera_rigs_dist)."""
     x = np.einsum("vab,nkb->vnka", cams["R"].astype(np.float64), joints) + \
         cams["t"].astype(np.float64)[:, None, None, :]
     uv = x[..., :2] / x[..., 2:3]
+    if cams.get("dist") is not None:
+        d = np.asarray(cams["dist"], np.float64)[:, None, None, :]
+        k1, k2, p1, p2, k3 = (d[..., i] for i in range(5))
+        xn, yn = uv[..., 0], uv[..., 1]
+        r2 = xn * xn + yn * yn
+        a = 1 + k1 * r2 + k2 * r2 * r2 + k3 * r2 * r2 * r2
+        uv = np.stack([xn * a + 2 * p1 * xn * yn + p2 * (r2 + 2 * xn * xn),
+                       yn * a + p1 * (r2 + 2 * yn * yn) + 2 * p2 * xn * yn], -1)
     return uv * cams["f"].astype(np.float64)[:, None, None, :] + \
         cams["c"].astype(np.float64)[:, None, None, :]
+
+
+WIDE_OFFSET = (0.6, 0.0, 0.3)            # where make_frames_wide puts the bodies: off the wide rig's common optical centre
+
+
+def make_wide_cameras(num_views: int, radius: float = 2.5, focal: float = 1000.0, distorted: bool = True) -> dict:
+    """A wide-angle test rig: make_cameras' ring, close (radius 2.5 m) and short (f = 1000 px on a 2048 x 1536 image), so that
+    a body make_frames_wide places off-centre reaches normalised image radius >= 0.4, where lens distortion moves detections by
+    tens of pixels.  distorted: "dist" [V,5] (float32) holds each view's coefficients, mid-range barrel lenses
+    (k1 -0.18 .. -0.26) with small tangential terms."""
+    cams = make_cameras(num_views, radius=radius, focal=focal)
+    if distorted:
+        v = np.arange(num_views)
+        cams["dist"] = np.ascontiguousarray(np.stack([-0.18 - 0.08 * (v % 3) / 2, 0.04 + 0.02 * (v % 2), 6e-4 * np.cos(v),
+                                                      -4e-4 * np.sin(v), -0.004 * (v % 2)], 1), dtype=np.float32)
+    return cams
+
+
+def make_frames_wide(model: dict, cams: dict, num_frames: int, seed: int = 1, noise: float = 2.0,
+                     model_type: str = "smpllsp") -> dict:
+    """make_frames for make_wide_cameras: bodies off-centre by WIDE_OFFSET, detections projected through cams (with its "dist",
+    if any) plus `noise` px of Gaussian noise.  Same keys as make_frames."""
+    rng = np.random.RandomState(seed)
+    B = num_frames
+    body_pose = rng.normal(0, 0.15, size=(B, 69))
+    global_orient = rng.normal(0, 0.2, size=(B, 3))
+    transl = np.asarray(WIDE_OFFSET)[None, :] + rng.normal(0, 0.1, size=(B, 3))
+    betas = rng.normal(0, 1.0, size=(B, 10))
+    scale = np.ones((B, 1))
+    joints = model_keypoints_np(model, betas, global_orient, body_pose, transl, scale, model_type)
+    V = cams["R"].shape[0]
+    gt_uv = project_np(cams, joints) + rng.normal(0, noise, size=(V, B, NUM_KEYPOINTS, 2))
+    conf = rng.uniform(0.6, 0.95, size=(V, B, NUM_KEYPOINTS))
+    init = dict(betas=np.zeros((B, 10)), global_orient=0.5 * global_orient, body_pose=0.5 * body_pose,
+                transl=transl + rng.normal(0, 0.05, size=(B, 3)), scale=np.ones((B, 1)))
+    f32 = lambda d: {k: np.ascontiguousarray(v, dtype=np.float32) for k, v in d.items()}
+    return dict(gt=f32(dict(betas=betas, global_orient=global_orient, body_pose=body_pose, transl=transl, scale=scale)),
+                init=f32(init), gt_uv=gt_uv.astype(np.float32), conf=conf.astype(np.float32),
+                joint_weights=np.ones(NUM_KEYPOINTS, dtype=np.float32), gt_joints3d=joints.astype(np.float32))
 
 
 def make_frames(model: dict, cams: dict, num_frames: int, seed: int = 1,
