@@ -292,7 +292,10 @@ struct __align__(16) SdfFrameSetup {
     float cn[3][3], cm[3];
     float pn[3], pd, pm;
     float vpad[3], vpadp;
-    float unused[2];
+    // bit (b & 31) of word b / 32: 256-vertex block b (chunks 4b..4b+3) has a chunk that is not culled.  All ones when the
+    // cull is off (all faces, or more than 32 * kSdfSkipWords chunks, i.e. more than 64 blocks).  sdf_fused retires the CTAs
+    // none of whose blocks is set before they touch a vertex.
+    unsigned live_blocks[2];
     unsigned skip[kSdfSkipWords];     // bit (c & 31) of word c / 32: no vertex of chunk c can see phi != 0
 };
 static_assert(sizeof(SdfFrameSetup) == 208, "SdfFrameSetup layout");

@@ -522,6 +522,10 @@ SdfFusedArgs make_sdf_fused_args(mvs_ctx* ctx) {
     const bool binned = lp.sdf_all_faces == 1 && w.bins_tri != nullptr;
     a.bins.tri = binned ? w.bins_tri : nullptr; a.bins.cell_ptr = w.bins_cell_ptr; a.bins.cell_idx = w.bins_cell_idx;
     a.bins.ray_ptr = w.bins_ray_ptr; a.bins.ray_idx = w.bins_ray_idx; a.bins.meta = w.bins_meta; a.bins.F = m.F;
+    {   // A/B knob (experiments only): MVS_SDF_BLOCK_SKIP=0 runs every CTA as if each of its blocks had a live chunk
+        static const int block_skip = getenv("MVS_SDF_BLOCK_SKIP") ? atoi(getenv("MVS_SDF_BLOCK_SKIP")) : 1;
+        a.block_skip = block_skip != 0;
+    }
     return a;
 }
 
@@ -615,6 +619,18 @@ extern "C" int mvs_debug_sdf_setup(mvs_ctx* ctx, void* rec) {
     if (cudaDeviceSynchronize() != cudaSuccess) return -1;
     if (!w.sdf_setup) return -2;
     return cudaMemcpy(rec, w.sdf_setup, (size_t)w.B * sizeof(mvs::SdfFrameSetup), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
+}
+
+// Testing aid, not part of the ABI (tests/test_gpu_sdf_block_mask.py): copies sdf_fused's per-block adjoint partials
+// [B][nblocks][kPartFloats] as the last dense round left them (only the rows of flagged blocks are written each round).
+// part == nullptr: returns kPartFloats.  Synchronises the device first.
+extern "C" int mvs_debug_sdf_part(mvs_ctx* ctx, float* part) {
+    const mvs::Workspace& w = ctx->ws;
+    if (!part) return mvs::kPartFloats;
+    const size_t B = (size_t)w.B, nblocks = ((size_t)ctx->m.N + mvs::kSdfFThreads - 1) / mvs::kSdfFThreads;
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+    if (!w.sdf_part) return -2;
+    return cudaMemcpy(part, w.sdf_part, B * nblocks * mvs::kPartFloats * sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
 }
 
 #ifdef MVS_PHASE_DBG

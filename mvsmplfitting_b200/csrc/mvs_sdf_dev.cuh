@@ -83,6 +83,7 @@ struct SdfFusedArgs {
     const float* At; int ldA; const int* ell_j; const float* ell_w; int KW; const float* Wd; const float* Qk;
     float* parts5; float* part; int* pflag; float* gcoord;
     SdfBinsDev bins;
+    int block_skip;                        // 0: ignore the record's live-block mask (MVS_SDF_BLOCK_SKIP=0, experiments only)
 };
 
 // kAll = false: the reference call as written (the kernel sees triangle 0), the default and the benchmark's mode; kAll = true: the
@@ -109,8 +110,8 @@ sdf_fused_kernel(SdfFusedArgs ar, const int* __restrict__ na_ptr, int passes) {
     if (slot >= na) return;
     if (pidx * passes * kSdfFThreads >= N) return;
     // ---- prologue: the frame's set-up (box, triangle 0, cone / plane, chunk-cull verdicts; computed once per frame before
-    //      this launch, sdf_frame_setup), its translation and this CTA's first vertices, all addressed by the slot alone:
-    //      one round trip
+    //      this launch, sdf_frame_setup) with its live-block mask, and its translation, all addressed by the slot alone:
+    //      one round trip; then the first vertices of the chunks the cull leaves
     const SdfFrameSetup* rec = ar.setup + slot;
     const float* vf = verts + (size_t)slot * N * 3;
     const float4 tr4 = *reinterpret_cast<const float4*>(slot_tr + 4 * slot);
@@ -123,18 +124,39 @@ sdf_fused_kernel(SdfFusedArgs ar, const int* __restrict__ na_ptr, int passes) {
     }
     const float pd = rec->pd, pm = rec->pm, vpadp = rec->vpadp;
     const float* tri = rec->tri;                       // triangle 0 in box coordinates: read only by the (rare) exact voxel tests
-    // Chunk-level cull (sdf_frame_setup): lane p of a warp reads the verdict of the warp's 64-vertex chunk in pass p; the
-    // pass loop takes it with a shuffle.  A culled chunk's value and gradient are exactly zero: its warps skip loads,
-    // divisions, corners.
-    bool my_skip = false;
-    if (lane < passes) {
+    const uint2 lb = *reinterpret_cast<const uint2*>(rec->live_blocks);
+    // Chunk-level cull (sdf_frame_setup): lane p of a warp reads the verdict of the warp's 64-vertex chunk in pass p; a
+    // ballot gives every lane all of them (bit p: pass p).  A culled chunk's value and gradient are exactly zero: its warps
+    // skip loads, divisions, corners.
+    unsigned skipm;
+    {
         const int chunk = ((pidx * passes + lane) * kSdfFThreads + warp * 32) / 64;
-        if (chunk < nbox && chunk < 32 * kSdfSkipWords) my_skip = (rec->skip[chunk >> 5] >> (chunk & 31)) & 1u;
+        const unsigned word = rec->skip[min(chunk >> 5, kSdfSkipWords - 1)];
+        const bool my_skip = lane < passes && chunk < nbox && chunk < 32 * kSdfSkipWords && ((word >> (chunk & 31)) & 1u);
+        skipm = __ballot_sync(0xffffffffu, my_skip);
+    }
+    const int nblocks = (N + kSdfFThreads - 1) / kSdfFThreads;
+    if (!kAll && ar.block_skip) {
+        // Block-level cull: a CTA none of whose blocks has a chunk that is not culled writes what the sampling below would
+        // (five +0 sums and flag 0 per block) and retires before its first vertex load and its first barrier.
+        const int b0 = pidx * passes;
+        const unsigned long long live = ((unsigned long long)lb.y << 32) | lb.x;
+        if (b0 < 64 && ((live >> b0) & ((1ull << passes) - 1ull)) == 0ull) {
+            if (t < 5 * passes) {
+                const int blk = b0 + t / 5;
+                if (blk < nblocks) parts5[((size_t)slot * nblocks + blk) * 5 + t % 5] = 0.f;
+            } else if (t >= 128 && t < 128 + passes) {
+                const int blk = b0 + t - 128;
+                if (blk < nblocks) pflag[(size_t)slot * nblocks + blk] = 0;
+            }
+            return;
+        }
     }
     float vcur[3] = {0.f, 0.f, 0.f};                   // this pass' vertex; the next one is fetched a pass ahead
     {
         const int n0 = pidx * passes * kSdfFThreads + t;
-        if (n0 < N) { vcur[0] = vf[3 * n0]; vcur[1] = vf[3 * n0 + 1]; vcur[2] = vf[3 * n0 + 2]; }
+        // a culled chunk's vertices are never read
+        if (n0 < N && !(skipm & 1u)) { vcur[0] = vf[3 * n0]; vcur[1] = vf[3 * n0 + 1]; vcur[2] = vf[3 * n0 + 2]; }
     }
     if (t < G && t < 256) ctab[t] = (float)(-1 + (t + 0.5) * (double)(float)(2. / (G - 1)));   // voxel_centre, tabulated
     const float tr[3] = {tr4.x, tr4.y, tr4.z};
@@ -163,19 +185,18 @@ sdf_fused_kernel(SdfFusedArgs ar, const int* __restrict__ na_ptr, int passes) {
     }
     const bool cull = (num_faces == 1);
     const bool tab = (G <= 256);
-    const int nblocks = (N + kSdfFThreads - 1) / kSdfFThreads;
 #pragma unroll 1
     for (int pass = 0; pass < passes; ++pass) {
         const int blk = pidx * passes + pass;
         if (blk >= nblocks) { if (lane == 0) s_wcnt[pass][warp] = 0; continue; }
         const int n = blk * kSdfFThreads + t;
         const float vme[3] = {vcur[0], vcur[1], vcur[2]};
-        if (pass + 1 < passes && n + kSdfFThreads < N) {
+        if (pass + 1 < passes && n + kSdfFThreads < N && !((skipm >> (pass + 1)) & 1u)) {
             vcur[0] = vf[3 * (n + kSdfFThreads)]; vcur[1] = vf[3 * (n + kSdfFThreads) + 1]; vcur[2] = vf[3 * (n + kSdfFThreads) + 2];
         }
         float acc[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
         float gcv[3] = {0.f, 0.f, 0.f};
-        const bool skip = __shfl_sync(0xffffffffu, (int)my_skip, pass) != 0;
+        const bool skip = (skipm >> pass) & 1u;
         // all faces over candidate lists: the warp evaluates its 32 vertices' voxels ONE AT A TIME, the lanes sharing out the
         // candidates (phi_binned_warp); every lane then goes on with its own eight values exactly as in the other modes
         float pc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};

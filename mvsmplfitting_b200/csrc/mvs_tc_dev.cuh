@@ -386,6 +386,7 @@ static __device__ __noinline__ void sdf_frame_setup(const SdfSetupArgs sa, const
     // shifted); if the whole box of a 64-vertex chunk is on the negative side of one cone plane and on the positive side
     // of another, no vertex of the chunk can see a voxel with phi != 0: value and gradient are exactly zero.
     const bool cull = sa.cull && nbox <= 32 * kSdfSkipWords;
+    unsigned live_lo = 0u, live_hi = 0u;               // bit b of the pair: block b has a chunk that is not culled
 #pragma unroll 1
     for (int k = 0; k < kSdfSkipWords; ++k) {
         const int chunk = 32 * k + lane;
@@ -429,6 +430,15 @@ static __device__ __noinline__ void sdf_frame_setup(const SdfSetupArgs sa, const
         }
         const unsigned bits = __ballot_sync(0xffffffffu, skip);
         if (lane == 0) rec->skip[k] = bits;
+        // the word's 32 chunks are blocks 8k..8k+7: a block is live when one of its chunks below nbox is not culled
+        unsigned live = __ballot_sync(0xffffffffu, chunk < nbox && !skip);
+        live |= live >> 1;
+        live |= live >> 2;
+        unsigned b8 = 0u;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) b8 |= ((live >> (4 * j)) & 1u) << j;
+        if (k < 4) live_lo |= b8 << (8 * k);
+        else live_hi |= b8 << (8 * (k - 4));
     }
     if (lane == 0) {
         rec->fb = fb;
@@ -440,7 +450,8 @@ static __device__ __noinline__ void sdf_frame_setup(const SdfSetupArgs sa, const
             rec->cm[q] = cm[q]; rec->pn[q] = pn[q]; rec->vpad[q] = vpad[q];
         }
         rec->pd = pd; rec->pm = pm; rec->vpadp = vpadp;
-        rec->unused[0] = 0.f; rec->unused[1] = 0.f;
+        rec->live_blocks[0] = cull ? live_lo : ~0u;
+        rec->live_blocks[1] = cull ? live_hi : ~0u;
         sa.boxout[slot] = fb;
         sa.arrive[slot] = 0;
     }
