@@ -497,6 +497,34 @@ int mvs_init_guess(mvs_ctx* ctx, float* params_dev, float* joints3d_dev, const m
 int mvs_sdf_grid(mvs_ctx* ctx, float* phi_dev, const int* faces_dev, int num_faces, const float* verts_dev,
                  int batch, int n_verts, int grid_size, void* stream);
 
+/* ---- render fitted meshes into every view's image (what the reference's save_images option draws with pyrender and cv2,
+ *      code/utils/utils.py:574-712, 866-882), see DESIGN.md section 4d.  For every frame f < n_frames with rig r and every view
+ *      v < V_r: the mesh verts_dev [n,N,3] (e.g. what mvs_forward writes) projected through view v (with its lens distortion),
+ *      rasterised with a depth buffer (pixel (x, y) sampled at (u, v) = (x, y); watertight edges, top-left fill rule, both
+ *      windings; a triangle with a vertex at camera depth <= 1e-3 is not drawn), shaded by a headlight plus ambient light and
+ *      drawn opaque over the background, with a filled disc of marker_radius px in marker_color around every keypoint of
+ *      keypoints_dev [n,K,3] (NULL: no markers) in front of the camera.
+ *      rig_dev [n] (device ints) names each frame's rig; NULL: rig 0, allowed only with a table of one rig.
+ *      background_dev [n,Vmax,H,W,3] uint8 (NULL: black).  Outputs, each [n,Vmax,H,W(,3)] and each may be NULL but not all:
+ *      image_dev (uint8), face_dev (int32, -1 = background), depth_dev (float, +inf = background).  Rows v >= V_r are not
+ *      written.  A shaded channel is min(255, floor(255 base_color[c] I + 1/2)), I = ambient + (1 - ambient) max(0, n.l) with
+ *      the interpolated camera-space normal n and l the unit vector from the surface point to the camera.  Deterministic: a
+ *      frame gets the same bits alone and in a call of any size.  Needs mvs_set_model with faces and cameras; uses no batch,
+ *      keypoints, loss configuration or optimiser state and changes none.  Refused (MVS_ERR_INVALID, nothing written): no
+ *      faces or cameras, n_frames < 1, verts_dev NULL, all outputs NULL, a size or config value out of range or not finite,
+ *      several rigs without rig_dev, a rig index out of range (naming the frame).  Enqueued on `stream`; synchronises it once
+ *      per chunk of frames to size the screen tiles' triangle lists (and once for the rig check when rig_dev is given). */
+typedef struct {
+    int width, height;               /* every view's image size, 1 .. 8192 */
+    float base_color[3];             /* in the images' channel order, [0, 1] */
+    float ambient;                   /* [0, 1] */
+    float marker_radius;             /* px, >= 0; 0 = no markers */
+    unsigned char marker_color[3];
+} mvs_render_config;
+int mvs_render(mvs_ctx* ctx, int n_frames, const float* verts_dev, const float* keypoints_dev, const int* rig_dev,
+               const unsigned char* background_dev, unsigned char* image_dev, int* face_dev, float* depth_dev,
+               const mvs_render_config* cfg, void* stream);
+
 /* Execution mode: 0 (default) = frame-resident kernels wherever they apply (sparse regime: no vertices requested,
  * no SDF term): one CTA per frame runs the closure -- and in mvs_lbfgs_run / mvs_fit_host the frame's whole
  * L-BFGS stage -- out of shared memory;  1 = always the batched multi-kernel path (used by tests to cross-check);

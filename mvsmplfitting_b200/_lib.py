@@ -52,6 +52,12 @@ class LbfgsStats(ctypes.Structure):
                 ("dense_rounds", ctypes.c_int), ("reserved", ctypes.c_int)]
 
 
+class RenderConfig(ctypes.Structure):
+    """mvs_render_config (include/mvsmpl.h)"""
+    _fields_ = [("width", ctypes.c_int), ("height", ctypes.c_int), ("base_color", ctypes.c_float * 3), ("ambient", ctypes.c_float),
+                ("marker_radius", ctypes.c_float), ("marker_color", ctypes.c_ubyte * 3)]
+
+
 class InitConfig(ctypes.Structure):
     """mvs_init_config (include/mvsmpl.h)"""
     _fields_ = [("estimate_scale", ctypes.c_int), ("fixed_scale", ctypes.c_float), ("use_torso", ctypes.c_int),
@@ -78,7 +84,7 @@ EXPORTS = (
     "mvs_closure", "mvs_forward", "mvs_forward_vjp", "mvs_lbfgs_run", "mvs_lbfgs_step", "mvs_fit", "mvs_fit_seq", "mvs_fit_stream", "mvs_fit_seq_stream", "mvs_fit_seq_stream3d",
     "mvs_fit_stream_rigs", "mvs_fit_seq_stream_rigs", "mvs_fit_host", "mvs_sdf_grid", "mvs_profile", "mvs_profile_read",
     "mvs_kernel_name", "mvs_set_exec_mode", "mvs_set_anchor", "mvs_set_joints3d", "mvs_init_guess", "mvs_fit_seq_temporal",
-    "mvs_fit_seq_stream_temporal", "mvs_fit_shared_shape", "mvs_refine_cameras",
+    "mvs_fit_seq_stream_temporal", "mvs_fit_shared_shape", "mvs_refine_cameras", "mvs_render",
 )
 NUM_KERNEL_IDS = 19
 
@@ -148,6 +154,7 @@ def load() -> ctypes.CDLL:
     lib.mvs_fit_host.argtypes = [vp, vp, vp, vp, vp, ci, ctypes.POINTER(LossConfig), ctypes.POINTER(LbfgsConfig), vp,
                                  ctypes.POINTER(LbfgsStats), vp]
     lib.mvs_sdf_grid.argtypes = [vp, vp, vp, ci, vp, ci, ci, ci, vp]
+    lib.mvs_render.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, ctypes.POINTER(RenderConfig), vp]
     lib.mvs_set_exec_mode.argtypes = [vp, ci]
     lib.mvs_set_anchor.argtypes = [vp, vp, vp, ci, vp]
     lib.mvs_set_joints3d.argtypes = [vp, vp, vp, ci, ci, vp]

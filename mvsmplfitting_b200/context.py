@@ -517,6 +517,55 @@ class FittingContext:
                                                  self._stream()), "mvs_sdf_grid")
         return phi
 
+    def render(self, verts: torch.Tensor, keypoints: torch.Tensor | None = None, rig=None, background: torch.Tensor | None = None,
+               width: int | None = None, height: int | None = None, outputs=("image",), base_color=(0.5, 0.5, 0.5),
+               ambient: float = 0.3, marker_radius: float = 8.0, marker_color=(0, 0, 255)) -> dict:
+        """The fitted meshes verts [n,N,3] (CUDA float32, e.g. forward_only's) drawn into every view of each frame's rig
+        (mvs_render, DESIGN.md section 4d): shaded by a headlight plus ambient light over background [n,V,H,W,3] (CUDA uint8;
+        None: black), with a disc of marker_radius px in marker_color around every keypoint of keypoints [n,K,3] (None: no
+        markers).  rig [n] names each frame's camera rig (None: rig 0, one rig only).  width and height default to the
+        background's.  outputs: any of "image" (uint8 [n,V,H,W,3]), "face" (int32 [n,V,H,W], -1 = background) and "depth"
+        (float32 [n,V,H,W], +inf = background); rows v >= V_r of a frame with rig r hold what background holds: zeros (image), -1
+        (face), +inf (depth).
+        The defaults are the reference's renderer's numbers: base colour 0.5, ambient 0.3, markers red in cv2's BGR order.
+        Returns a dict of the requested outputs."""
+        def check(name, t, dtype, shape):
+            if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.device != self.device or tuple(t.shape) != shape:
+                raise ValueError("render: want %s as a %s tensor of shape %s on %s, got %s" % (
+                    name, dtype, shape, self.device, (t.dtype, tuple(t.shape), t.device) if isinstance(t, torch.Tensor) else type(t)))
+            return t.contiguous()
+        outputs = tuple(outputs)
+        if not outputs or any(o not in ("image", "face", "depth") for o in outputs):
+            raise ValueError("render: outputs must be a non-empty subset of ('image', 'face', 'depth'), got %r" % (outputs,))
+        if verts.dim() != 3:
+            raise ValueError("render: want verts [n,%d,3], got %s" % (self.N, tuple(verts.shape)))
+        n = verts.shape[0]
+        verts = check("verts", verts, torch.float32, (n, self.N, 3))
+        if background is not None and background.dim() == 5:
+            height = background.shape[2] if height is None else height
+            width = background.shape[3] if width is None else width
+        if width is None or height is None:
+            raise ValueError("render: give width and height, or a background")
+        W, H = int(width), int(height)
+        if background is not None:
+            background = check("background", background, torch.uint8, (n, self.V, H, W, 3))
+        if keypoints is not None:
+            keypoints = check("keypoints", keypoints, torch.float32, (n, self.K, 3))
+        rg = self._stream_rigs("render", n, rig)
+        out = {}
+        if "image" in outputs:
+            out["image"] = torch.zeros(n, self.V, H, W, 3, dtype=torch.uint8, device=self.device)
+        if "face" in outputs:
+            out["face"] = torch.full((n, self.V, H, W), -1, dtype=torch.int32, device=self.device)
+        if "depth" in outputs:
+            out["depth"] = torch.full((n, self.V, H, W), float("inf"), dtype=torch.float32, device=self.device)
+        cfg = _lib.RenderConfig(W, H, (ctypes.c_float * 3)(*[float(c) for c in base_color]), float(ambient), float(marker_radius),
+                                (ctypes.c_ubyte * 3)(*[int(c) for c in marker_color]))
+        _lib.check(self.h, self.lib.mvs_render(self.h, n, _ptr(verts), _ptr(keypoints), _ptr(rg), _ptr(background), _ptr(out.get("image")),
+                                               _ptr(out.get("face")), _ptr(out.get("depth")), ctypes.byref(cfg), self._stream()),
+                   "mvs_render")
+        return out
+
     def set_anchor(self, anchor: torch.Tensor | None, weight: torch.Tensor | None = None):
         """per-frame quadratic anchor sum_i w_i (x_i - a_i)^2 (sequence mode); anchor=None switches it off.
         Takes effect with the next set_loss()."""

@@ -45,6 +45,7 @@ template int dev_alloc<int>(mvs_ctx*, int**, size_t);
 template int dev_alloc<double>(mvs_ctx*, double**, size_t);
 template int dev_alloc<unsigned char>(mvs_ctx*, unsigned char**, size_t);
 template int dev_alloc<int2>(mvs_ctx*, int2**, size_t);
+template int dev_alloc<float4>(mvs_ctx*, float4**, size_t);
 template int dev_alloc<FrameBox>(mvs_ctx*, FrameBox**, size_t);
 template int dev_alloc<SdfFrameSetup>(mvs_ctx*, SdfFrameSetup**, size_t);
 template int dev_alloc<long long>(mvs_ctx*, long long**, size_t);
@@ -479,7 +480,21 @@ int mvs_set_model(mvs_ctx* ctx, const mvs_model_desc* d) {
         const_array(m.supj_w, jw.data(), jw.size()), const_array(m.sup_then_all, comb.data(), comb.size()),
         const_array(m.sup_ptr, sptr.data(), sptr.size()), const_array(m.sup_k, sk.data(), sk.size()),
         const_array(m.sup_w, swt.data(), swt.size())};
+    // vertex -> face CSR (faces in ascending order) for the renderer's vertex normals (mvs_render); only for faces whose vertex
+    // ids are all in range, without which mvs_render refuses the model
+    std::vector<int> vfp(N + 1, 0), vfi;
+    bool faces_ok = d->faces && d->n_faces > 0;
+    for (int e = 0; faces_ok && e < 3 * d->n_faces; ++e) faces_ok = d->faces[e] >= 0 && d->faces[e] < N;
     if (d->faces && d->n_faces > 0) arrays.push_back(const_array(m.faces, d->faces, (size_t)d->n_faces * 3));
+    if (faces_ok) {
+        for (int e = 0; e < 3 * d->n_faces; ++e) ++vfp[d->faces[e] + 1];
+        for (int n = 0; n < N; ++n) vfp[n + 1] += vfp[n];
+        vfi.resize(vfp[N]);
+        std::vector<int> cur(vfp.begin(), vfp.end() - 1);
+        for (int e = 0; e < 3 * d->n_faces; ++e) vfi[cur[d->faces[e]]++] = e / 3;
+        arrays.push_back(const_array(m.vf_ptr, vfp.data(), vfp.size()));
+        arrays.push_back(const_array(m.vf_idx, vfi.data(), vfi.size()));
+    }
     int rc;
     if ((rc = upload_consts(ctx, arrays)) || (rc = tc_upload_model(ctx))) return rc;
     ctx->have_model = true;
@@ -757,6 +772,35 @@ int mvs_vposer_decode(mvs_ctx* ctx, const float* params_dev, float* body_pose_de
     MVS_REQUIRE(ctx, params_dev && body_pose_dev, "mvs_vposer_decode: NULL argument");
     MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
     return launch_vposer_decode(ctx, params_dev, body_pose_dev, (cudaStream_t)stream);
+}
+
+int mvs_render(mvs_ctx* ctx, int n_frames, const float* verts_dev, const float* keypoints_dev, const int* rig_dev,
+               const unsigned char* background_dev, unsigned char* image_dev, int* face_dev, float* depth_dev,
+               const mvs_render_config* cfg, void* stream) {
+    if (!ctx) return set_error(nullptr, MVS_ERR_INVALID, "ctx is NULL");
+    MVS_REQUIRE(ctx, ctx->have_model && ctx->m.F > 0 && ctx->m.faces, "mvs_render: needs a model with faces (mvs_set_model)");
+    MVS_REQUIRE(ctx, ctx->m.vf_ptr, "mvs_render: the model's faces name vertices out of range");
+    MVS_REQUIRE(ctx, ctx->have_cams, "mvs_render: set the cameras first");
+    MVS_REQUIRE(ctx, n_frames >= 1, "mvs_render: n_frames = %d (want >= 1)", n_frames);
+    MVS_REQUIRE(ctx, verts_dev, "mvs_render: verts_dev is NULL");
+    MVS_REQUIRE(ctx, image_dev || face_dev || depth_dev, "mvs_render: every output is NULL");
+    MVS_REQUIRE(ctx, cfg, "mvs_render: NULL config");
+    MVS_REQUIRE(ctx, cfg->width >= 1 && cfg->width <= 8192 && cfg->height >= 1 && cfg->height <= 8192,
+                "mvs_render: image size %d x %d (want 1 .. 8192 each)", cfg->width, cfg->height);
+    for (int c = 0; c < 3; ++c)
+        MVS_REQUIRE(ctx, isfinite(cfg->base_color[c]) && cfg->base_color[c] >= 0.f && cfg->base_color[c] <= 1.f,
+                    "mvs_render: base_color[%d] = %g (want [0, 1])", c, cfg->base_color[c]);
+    MVS_REQUIRE(ctx, isfinite(cfg->ambient) && cfg->ambient >= 0.f && cfg->ambient <= 1.f, "mvs_render: ambient = %g (want [0, 1])",
+                cfg->ambient);
+    MVS_REQUIRE(ctx, isfinite(cfg->marker_radius) && cfg->marker_radius >= 0.f, "mvs_render: marker_radius = %g (want finite, >= 0)",
+                cfg->marker_radius);
+    MVS_REQUIRE(ctx, rig_dev || ctx->rigs.size() == 1,
+                "mvs_render: the context has %d camera rigs and no per-frame rigs were given", (int)ctx->rigs.size());
+    MVS_CUDA_OK(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (rig_dev)
+        if (int rc = check_frame_rigs(ctx, "mvs_render", rig_dev, n_frames, st)) return rc;
+    return render_launch(ctx, n_frames, verts_dev, keypoints_dev, rig_dev, background_dev, image_dev, face_dev, depth_dev, *cfg, st);
 }
 
 int mvs_sdf_grid(mvs_ctx* ctx, float* phi_dev, const int* faces_dev, int num_faces, const float* verts_dev, int batch,

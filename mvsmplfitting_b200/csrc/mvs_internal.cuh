@@ -116,6 +116,8 @@ struct DevModel {
     const float* Wd = nullptr;
     const float* ST = nullptr;  // [N][3][11] shapedirs row | template, fp32 (skinning kernel of the tensor-core path)
     const int* faces = nullptr;
+    const int* vf_ptr = nullptr;      // [N+1] vertex -> face CSR (faces around each vertex, ascending): the renderer's normals
+    const int* vf_idx = nullptr;      // [3F]
     int tri0[3] = {0, 0, 0};          // vertex ids of face 0 (the triangle the as-written SDF term sees)
     // keypoints: k-th keypoint = sum_e kp_w[e] * v[kp_vidx[e]]  (+ posed chain joint kp_chain[k] if >= 0) + transl
     int K = 0, n_kp_entries = 0, nsup = 0;
@@ -273,6 +275,15 @@ struct Workspace {
     int* bins_ray_ptr = nullptr; unsigned short* bins_ray_idx = nullptr; float* bins_meta = nullptr;
 };
 
+// mvs_render's grow-only scratch (mvs_render.cu), for one chunk of frames: vertex normal sums [frames][N], screen vertices
+// [items][N] and keypoints [items][K] (item = frame x view), per-tile triangle counts [items][tiles] and their exclusive scan
+// [items x tiles + 1], the scan's block sums, and the tiles' triangle lists
+struct RenderScratch {
+    DevBuf<float4> nrm, sv, sk;
+    DevBuf<int> cnt, list;
+    DevBuf<long long> off, part;
+};
+
 struct FrameBox {                     // bounding box of one frame's mesh (fitting.py:352-359)
     float centre[3];
     float scale;
@@ -365,6 +376,7 @@ struct mvs_ctx {
     int2* stage_rng = nullptr;       // [B] per-frame slice of the stage table (mvs_fit_seq), device
     mvs::StreamState* fstream = nullptr;  // frame-stream scratch (mvs_fit_stream), created on first use
     mvs::SeqState* sstream = nullptr;     // sequence-stream, shared-shape and camera-refinement scratch, created on first use
+    mvs::RenderScratch render;            // mvs_render
 };
 
 namespace mvs {
@@ -529,6 +541,9 @@ inline RigSet slot_rig_set(const mvs_ctx* ctx) { return RigSet{ctx->rigs_dev.p, 
 int check_frame_rigs(mvs_ctx* ctx, const char* who, const int* rig_dev, int n, cudaStream_t st);
 void release_fit_state(mvs_ctx* ctx);          // mvs_lbfgs.cu: the optimiser state and the stream scratch (mvs_destroy)
 void release_tc_state(mvs_ctx* ctx);           // mvs_tc.cu (mvs_destroy)
+// mvs_render.cu: mvs_render's kernels for frames [0, n) (arguments checked by the entry point)
+int render_launch(mvs_ctx* ctx, int n, const float* verts, const float* keypoints, const int* rig, const unsigned char* background,
+                  unsigned char* image, int* face, float* depth, const mvs_render_config& cfg, cudaStream_t st);
 int sdf_grid_launch(mvs_ctx* ctx, float* phi, const int* faces, int num_faces, const float* verts, int batch,
                     int n_verts, int G, cudaStream_t st);
 }  // namespace mvs

@@ -330,21 +330,27 @@ def _pad_views(seq: dict, V: int) -> dict:
     return dict(seq, gt_uv=pad(seq["gt_uv"]), conf=pad(seq["conf"]), present=pad(seq["present"]))
 
 
-def _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces, frames=None, rows=None):
-    """per-frame result pickles (+ meshes) of `rows` of the batch (default: all), named by `frames`"""
+def _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces, frames=None, rows=None, plan=None, rig=None):
+    """per-frame result pickles (+ meshes) of `rows` of the batch (default: all), named by `frames`; with plan (_render_plan)
+    also the frames' overlays, rig: the sequence's camera rig (None: the context's only one)"""
     x = params.cpu().numpy()
     B = x.shape[0]
     rows = list(range(B)) if rows is None else list(rows)
     frames = seq["frames"] if frames is None else frames
     decoded = ctx.vposer_decode(params).cpu().numpy() if latent else None      # utils.py:741-743
     verts = None
-    if mesh_folder is not None:          # the mesh is rebuilt from the SAVED pose (extremities zeroed), utils.py:865-871
+    if mesh_folder is not None or plan is not None:   # the mesh is rebuilt from the SAVED pose (extremities zeroed), utils.py:865-871
         saved = params.clone()
         if latent:
             saved[:, 13:82] = torch.as_tensor(decoded, device=saved.device)
         for a, b in ((18, 24), (27, 33), (57, 69)):
             saved[:, 13 + a:13 + b] = 0.0
-        verts = ctx.forward_only(saved, want_verts=True)["verts"].cpu().numpy()
+        fwd = ctx.forward_only(saved, want_verts=True)
+        if plan is not None:
+            _render_rows(ctx, plan, fwd["verts"], fwd["joints"], rows, frames, rig)
+        verts = fwd["verts"].cpu().numpy() if mesh_folder is not None else None
+    if result_folder is None:
+        return
     for b, fr in zip(rows, frames):
         res = result_from_params(x[b], loss[b], pose_embedding=x[b, 13:45] if latent else None,
                                  body_pose=decoded[b] if latent else None)
@@ -352,10 +358,82 @@ def _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces, f
                      mesh_folder=mesh_folder)
 
 
+RENDER_CHUNK_BYTES = 1 << 30             # image buffers (background + overlay) of one render call
+
+
+def _render_plan(seq: dict, image_folder, render_folder):
+    """What the save_images option (utils.py:866-882) draws for a sequence: every (view, frame) with detections (present) and an
+    image at <image_folder>/<serial>/<camera>/<frame>.jpg or .png (data_parser.py:296-323), whose overlay goes to
+    <render_folder>/<serial>/<frame>/<camera>.jpg.  None when neither folder is given; ValueError when only one is.  Checked
+    before any fitting: that cv2 imports and that the sequence's first image reads (its size is the sequence's image size)."""
+    if image_folder is None and render_folder is None:
+        return None
+    if image_folder is None or render_folder is None:
+        raise ValueError("image_folder and render_folder go together (got %r, %r)" % (image_folder, render_folder))
+    import cv2                                            # the reference reads and writes its images with cv2
+    images = {}
+    for v, cam in enumerate(seq["cameras"]):
+        for b, fr in enumerate(seq["frames"]):
+            if not seq["present"][v, b]:
+                continue
+            for ext in (".jpg", ".png"):
+                path = os.path.join(image_folder, seq["serial"], cam, fr + ext)
+                if os.path.exists(path):
+                    images[v, fr] = path
+                    break
+    plan = dict(serial=seq["serial"], cameras=list(seq["cameras"]), images=images, render_folder=render_folder, size=None)
+    if images:
+        _read_image(cv2, plan, next(iter(images.values())))
+    return plan
+
+
+def _read_image(cv2, plan: dict, path: str):
+    """one image of a sequence (BGR uint8 [H,W,3]); ValueError when it does not read or its size is not the sequence's"""
+    im = cv2.imread(path, cv2.IMREAD_COLOR)
+    if im is None:
+        raise ValueError("cannot read image %s" % path)
+    if plan["size"] is None:
+        plan["size"] = im.shape[:2]
+    if im.shape[:2] != plan["size"]:
+        raise ValueError("sequence %s: image %s is %dx%d, other views are %dx%d (one image size per sequence)"
+                         % (plan["serial"], path, im.shape[1], im.shape[0], plan["size"][1], plan["size"][0]))
+    return im
+
+
+def _render_rows(ctx, plan: dict, verts, joints, rows, frames, rig=None):
+    """Overlays of the batch rows `rows` (named `frames`) of verts [B,N,3] / joints [B,K,3]: FittingContext.render over each
+    frame's images (markers on the keypoints), written as JPEG with cv2.  Frames go in chunks whose image buffers (the
+    backgrounds and the overlays, on the host and on the device) stay under RENDER_CHUNK_BYTES each; a chunk's images are read
+    when it is rendered."""
+    import cv2
+    todo = [(b, fr, [v for v in range(len(plan["cameras"])) if (v, fr) in plan["images"]]) for b, fr in zip(rows, frames)]
+    todo = [t for t in todo if t[2]]
+    if not todo:
+        return
+    H, W = plan["size"]
+    chunk = max(1, RENDER_CHUNK_BYTES // (2 * ctx.V * H * W * 3))
+    for c0 in range(0, len(todo), chunk):
+        part = todo[c0:c0 + chunk]
+        bg = np.zeros((len(part), ctx.V, H, W, 3), np.uint8)
+        for i, (b, fr, views) in enumerate(part):
+            for v in views:
+                bg[i, v] = _read_image(cv2, plan, plan["images"][v, fr])
+        idx = torch.as_tensor([b for b, _, _ in part], device=verts.device)
+        out = ctx.render(verts[idx].contiguous(), keypoints=joints[idx].contiguous(),
+                         rig=None if rig is None else np.full(len(part), rig, np.int32),
+                         background=torch.as_tensor(bg, device=verts.device))["image"].cpu().numpy()
+        del bg
+        for i, (b, fr, views) in enumerate(part):
+            d = os.path.join(plan["render_folder"], plan["serial"], fr)
+            os.makedirs(d, exist_ok=True)
+            for v in views:
+                cv2.imwrite(os.path.join(d, plan["cameras"][v] + ".jpg"), out[i, v])
+
+
 def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool = False, fixed_scale: float = 1.0,
                  use_hip: bool = True, pose_format: str = "coco17", result_folder: str | None = None,
                  mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, use_3d: bool = False,
-                 shared_shape: int = 0, refine_cameras: int = 0):
+                 shared_shape: int = 0, refine_cameras: int = 0, image_folder: str | None = None, render_folder: str | None = None):
     """The frame loop of main.py:32-89 for one sequence as ONE batch (every frame from its own initial guess, is_seq = False):
     upload the detections, initial guess on the device (init_guess + fix_params), all stages (`mvs_fit`), results per
     frame.  `ctx` is a FittingContext whose model, priors (GMM / VPoser decoder), cameras and batch (= number of frames) are
@@ -372,9 +450,13 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
     refine_cameras (sweeps, 0: off): after the fit, one FittingContext.refine_cameras call over all frames refines the context's
     camera extrinsics from them (before shared_shape when both are given), see refine_rigs; the refined rigs go into stats and,
     with result_folder, into cameras_rig<r>.txt there.
+    image_folder with render_folder (the reference's save_images): every (view, frame) with detections and an image
+    <image_folder>/<serial>/<camera>/<frame>.jpg|.png gets the fitted mesh (the saved pose, as the .obj) and keypoint markers
+    drawn over it by FittingContext.render, written to <render_folder>/<serial>/<frame>/<camera>.jpg (cv2).
     Returns (params [F,86] numpy -- pose slot = latent code under VPoser --, final_loss [F], stats)."""
     _check_sweeps("shared_shape", shared_shape, None, "the shared shape's pose step")
     _check_sweeps("refine_cameras", refine_cameras, None, "the camera refinement's body step")
+    plan = _render_plan(seq, image_folder, render_folder)
     F = len(seq["frames"])
     assert ctx.B <= F, "context batch %d > frames %d" % (ctx.B, F)
     latent = _uses_latent_pose(stage_cfgs)
@@ -400,8 +482,8 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
         if shared_shape:
             final = share_shape(ctx, params, seq["gt_uv"], seq["conf"], jw, [F], stage_cfgs, opt_cfg, shared_shape, t3, stats=stats)
         loss = final.cpu().numpy()
-        if result_folder is not None:
-            _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces)
+        if result_folder is not None or plan is not None:
+            _export(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces, plan=plan)
         return params.cpu().numpy(), loss, stats
     params = _cold_guesses(ctx, seq["gt_uv"], seq["conf"], jw, stage_cfgs, guess, t3)
     if t3 is None:
@@ -415,8 +497,8 @@ def fit_sequence(ctx, seq: dict, stage_cfgs, opt_cfg=None, estimate_scale: bool 
     if shared_shape:
         final = share_shape(ctx, params, seq["gt_uv"], seq["conf"], jw, [F], stage_cfgs, opt_cfg, shared_shape, t3, stats=stats)
     loss = final.cpu().numpy()
-    if result_folder is not None:
-        _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces)
+    if result_folder is not None or plan is not None:
+        _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces, plan)
     return params.cpu().numpy(), loss, stats
 
 
@@ -453,7 +535,7 @@ def _cold_guesses(ctx, gt_uv, conf, jw, stage_cfgs, guess: dict, t3=None, rig=No
     return params
 
 
-def _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces):
+def _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, faces, plan=None, rig=None):
     """_export of one sequence's F rows (params [F,86] on the device, loss [F]) in chunks of ctx.B rows, as the export takes
     whole batches; the last chunk is padded"""
     F, B = params.shape[0], ctx.B
@@ -463,7 +545,8 @@ def _export_rows(ctx, seq, params, loss, latent, result_folder, mesh_folder, fac
         chunk[:n] = params[c0:c0 + n]
         lc = np.zeros(B, np.float32)
         lc[:n] = loss[c0:c0 + n]
-        _export(ctx, seq, chunk, lc, latent, result_folder, mesh_folder, faces, frames=seq["frames"][c0:c0 + n], rows=range(n))
+        _export(ctx, seq, chunk, lc, latent, result_folder, mesh_folder, faces, frames=seq["frames"][c0:c0 + n], rows=range(n),
+                plan=plan, rig=rig)
 
 
 def _check_sweeps(option, sweeps, temporal_weight, step) -> None:
@@ -526,7 +609,7 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
                   use_hip: bool = True, pose_format: str = "coco17", result_folder: str | None = None,
                   mesh_folder: str | None = None, faces=None, umeyama_as_written: bool = False, reinit_loss: float = 5000.0,
                   use_3d: bool = False, rigs=None, rig_data_weight_scale=None, temporal_weight=None, shared_shape: int = 0,
-                  refine_cameras: int = 0):
+                  refine_cameras: int = 0, image_folder: str | None = None, render_folder: str | None = None):
     """main.py:32-89 with is_seq = True for S sequences in lock-step: the batch of step t is frame t of every sequence
     (context batch = S).  A sequence's first frame gets the initial guess and every stage; a later frame
     starts from the previous frame's result as load_init + fix_params leave it (init_guess.py:137-166,190-212: betas,
@@ -556,9 +639,11 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
     refine_cameras call over all frames with each frame's rig (see refine_rigs), before shared_shape when both are given; the
     refined rigs go into stats['refine_cameras'] and, with result_folder, into cameras_rig<r>.txt there.  The context keeps
     the refined cameras.  It does not combine with temporal_weight (ValueError).
+    image_folder with render_folder: every sequence's overlays, as fit_sequence writes them (each in its rig's cameras).
     Returns a list (per sequence) of (params [T_s,86], loss [T_s]) and the summed stats."""
     _check_sweeps("shared_shape", shared_shape, temporal_weight, "the shared shape's pose step")
     _check_sweeps("refine_cameras", refine_cameras, temporal_weight, "the camera refinement's body step")
+    plans = [_render_plan(q, image_folder, render_folder) for q in seqs]
     S_ = len(seqs)
     tw = temporal_weight_vector(temporal_weight)
     latent = _uses_latent_pose(stage_cfgs)
@@ -583,7 +668,7 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
                                      pose_format, use_hip, dict(estimate_scale=estimate_scale, fixed_scale=fixed_scale,
                                                                 use_torso=True, hip_seed=1.0, want_joints3d=False,
                                                                 umeyama_as_written=umeyama_as_written), t3, seq_rig, rig_views, tw,
-                                     shared_shape, refine_cameras)
+                                     shared_shape, refine_cameras, plans)
     T = max(len(q["frames"]) for q in seqs)
     V = seqs[0]["gt_uv"].shape[0]
     off = np.concatenate([[0], np.cumsum([len(q["frames"]) for q in seqs])])
@@ -634,10 +719,11 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
         for s_, q in enumerate(seqs):
             if live[s_]:
                 out_x[s_][t], out_l[s_][t] = x[s_], prev_loss[s_]
-        if result_folder is not None and not (shared_shape or refine_cameras):
+        if (result_folder is not None or plans[0] is not None) and not (shared_shape or refine_cameras):
             for s_, q in enumerate(seqs):
                 if live[s_]:
-                    _export(ctx, q, params, prev_loss, latent, result_folder, mesh_folder, faces, frames=[q["frames"][t]], rows=[s_])
+                    _export(ctx, q, params, prev_loss, latent, result_folder, mesh_folder, faces, frames=[q["frames"][t]], rows=[s_],
+                            plan=plans[s_], rig=None if seq_rig is None else seq_rig[s_])
     if t3 is not None:
         ctx.set_joints3d(None)
     if shared_shape or refine_cameras:
@@ -654,18 +740,20 @@ def fit_sequences(ctx, seqs, stage_cfgs, opt_cfg=None, estimate_scale: bool = Fa
         xs = x.cpu().numpy()
         out_x = [xs[off[s_]:off[s_ + 1]] for s_ in range(S_)]
         out_l = [final[off[s_]:off[s_ + 1]] for s_ in range(S_)]
-        if result_folder is not None:
+        if result_folder is not None or plans[0] is not None:
             for s_, q in enumerate(seqs):
-                _export_rows(ctx, q, x[off[s_]:off[s_ + 1]], out_l[s_], latent, result_folder, mesh_folder, faces)
+                _export_rows(ctx, q, x[off[s_]:off[s_ + 1]], out_l[s_], latent, result_folder, mesh_folder, faces, plans[s_],
+                             None if seq_rig is None else seq_rig[s_])
     return list(zip(out_x, out_l)), tot
 
 
 def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, result_folder, mesh_folder, faces, pose_format,
-                          use_hip, guess, t3=None, seq_rig=None, rig_views=None, tw=None, shared_shape=0, refine_cameras=0):
+                          use_hip, guess, t3=None, seq_rig=None, rig_views=None, tw=None, shared_shape=0, refine_cameras=0, plans=None):
     """fit_sequences through mvs_fit_seq_stream: the sequences' frames back to back, every frame's cold start point from
     _cold_guesses; t3: _targets_3d of those frames (mvs_fit_seq_stream3d); seq_rig [S]: each sequence's rig, which every
     one of its frames takes (mvs_fit_seq_stream_rigs); tw [86]: the temporal weight (mvs_fit_seq_stream_temporal);
-    shared_shape: sweeps of share_shape after the fit (0: off); refine_cameras: sweeps of refine_rigs before it (0: off)"""
+    shared_shape: sweeps of share_shape after the fit (0: off); refine_cameras: sweeps of refine_rigs before it (0: off); plans:
+    each sequence's _render_plan"""
     lengths = [len(q["frames"]) for q in seqs]
     off = np.concatenate([[0], np.cumsum(lengths)])
     gt_uv = np.concatenate([q["gt_uv"] for q in seqs], axis=1)
@@ -686,7 +774,8 @@ def _fit_sequences_stream(ctx, seqs, stage_cfgs, opt_cfg, latent, reinit_loss, r
     if shared_shape:
         final = share_shape(ctx, params, gt_uv, conf, jw, lengths, stage_cfgs, opt_cfg, shared_shape, t3, rig, stats)
     x, loss = params.cpu().numpy(), final.cpu().numpy()
-    if result_folder is not None:
+    if result_folder is not None or (plans and plans[0] is not None):
         for s_, q in enumerate(seqs):
-            _export_rows(ctx, q, params[off[s_]:off[s_ + 1]], loss[off[s_]:off[s_ + 1]], latent, result_folder, mesh_folder, faces)
+            _export_rows(ctx, q, params[off[s_]:off[s_ + 1]], loss[off[s_]:off[s_ + 1]], latent, result_folder, mesh_folder, faces,
+                         None if plans is None else plans[s_], None if seq_rig is None else seq_rig[s_])
     return [(x[off[s_]:off[s_ + 1]], loss[off[s_]:off[s_ + 1]]) for s_ in range(len(seqs))], stats
